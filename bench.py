@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- the WORLD analysis hot path on N B200s (driver contract, see DESIGN.md "Measurement").
+"""bench.py -- the WORLD analysis hot path on N GPUs (driver contract, see DESIGN.md "Measurement").
 
 One "step" = one pass of {Harvest -> CheapTrick -> D4C} over one batch of synthetic 16 kHz speech
 (default: BASELINE.json configs[2], 1024 utterances x 10 s per GPU; weak scaling over ranks with
 one NCCL all-gather per output array to reassemble the batch, north_star).  Prints ONE JSON line.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
-                  [--f0 harvest|dio] [--utts U] [--seconds S] [--fs FS]
+                  [--f0 harvest|dio] [--utts U] [--seconds S] [--fs FS] [--dump-outputs DIR]
 
 value      frames/s with inputs and outputs resident in HBM (CUDA events, max over ranks)
 e2e        the same through world_b200_analyze_host(): pinned HOST buffers in, HOST buffers out
@@ -14,6 +14,10 @@ roofline   dominant kernel (largest share of the step, timed live with CUDA even
            library): algorithmic HBM bytes / kernel time vs the measured copy peak
 cpu_baseline   the compiled reference (oracle/_ref) on this box's host, one thread, bounded sample
 --impl reference   the reference's own CPU implementation on all host cores (rank 0 only)
+--dump-outputs DIR   after the timed steps, rank 0 writes what the last timed step returned (time_axis, f0,
+           spectrogram, aperiodicity; gathered over ranks where the step gathers them; float64) as
+           DIR/<name>.npy: whole arrays when they fit DUMP_BYTES, else the rows at a seeded sample of
+           (utterance, frame) positions
 """
 import argparse
 import json
@@ -49,7 +53,8 @@ def parse():
                     help="test hook: hold this much extra device memory (emulates the gathered arrays of a larger world)")
     ap.add_argument("--config", type=int, default=0, choices=[0, 2, 3, 4, 5],
                     help="BASELINE.json configs[N-1]: 2 = 1024x10s Dio+StoneMask chain, 3 = 1024x10s Harvest chain (default), "
-                         "4 = 256x30s @48 kHz CheapTrick+D4C on a precomputed f0, 5 = 8192x5s Harvest chain sharded over --gpus")
+                         "4 = 256x30s @48 kHz CheapTrick+D4C on a precomputed f0, 5 = 8192x5s Harvest chain sharded over --gpus "
+                         "(at most 4096 utterances per GPU)")
     ap.add_argument("--stages", default="full", choices=["full", "spectral"],
                     help="spectral: time CheapTrick+D4C only, on an f0 computed (untimed) by Dio+StoneMask")
     ap.add_argument("--parity-utts", type=int, default=3, help="extra utterances (middle / last rows of the batch) checked against the reference")
@@ -57,7 +62,11 @@ def parse():
                     help="device-resident leg through the separate stage calls on one stream instead of world_b200_analyze_batch")
     ap.add_argument("--slices", type=int, default=1,
                     help="utterance slices per step: F0 of slice s+1 overlaps CheapTrick/D4C of slice s on a second stream")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (see the module docstring)")
     a = ap.parse_args()
+    if a.steps < 1 or a.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     if a.config == 2:
         a.f0, a.utts, a.seconds, a.fs = "dio", 1024, 10.0, 16000
     elif a.config == 3:
@@ -65,7 +74,12 @@ def parse():
     elif a.config == 4:
         a.f0, a.utts, a.seconds, a.fs, a.stages = "dio", 256, 30.0, 48000, "spectral"
     elif a.config == 5:
-        a.f0, a.utts, a.seconds, a.fs = "harvest", max(1, 8192 // max(1, a.gpus)), 5.0, 16000
+        # the spectrogram + aperiodicity of 4096 five-second utterances (34 GB) is what an 80 GB GPU holds next to
+        # the waveforms and the scratch arenas; one GPU runs half the batch
+        a.f0, a.utts, a.seconds, a.fs = "harvest", min(4096, max(1, 8192 // max(1, a.gpus))), 5.0, 16000
+        if a.utts * a.gpus < 8192:
+            print(f"bench.py: config 5 on {a.gpus} GPU(s) runs {a.utts * a.gpus} of its 8192 utterances "
+                  "(at most 4096 per GPU)", file=sys.stderr)
     return a
 
 
@@ -77,6 +91,8 @@ def chain_name(a):
 
 def workload_name(a):
     tail = " (f0 from Dio+StoneMask, not timed)" if a.stages == "spectral" else ""
+    if a.config == 5 and a.utts * a.gpus < 8192:
+        tail += f" -- {a.utts * a.gpus} of the 8192 utterances BASELINE config 5 names"
     return f"{a.utts}x{a.seconds:g}s synthetic {a.fs // 1000} kHz batch per GPU, {chain_name(a)}{tail}"
 
 
@@ -133,7 +149,7 @@ def parity_summary(entries, rows, what):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -193,7 +209,30 @@ def measured_peak_hbm():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s), not measured"
+
+
+DUMP_BYTES = 60 * 1000 * 1000   # --dump-outputs stays under 64 MB
+
+
+def dump_outputs(d, arrays):
+    """arrays: name -> contiguous device tensor [utterances, frames, ...].  Writes DIR/<name>.npy (float64): whole
+    arrays when they all fit DUMP_BYTES, else the rows at a seeded sample of (utterance, frame) positions, sorted;
+    arrays of the same shape[:2] share one sample, each array keeps the same fraction of its positions."""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    nbytes = sum(8 * v.numel() for v in arrays.values())
+    frac = min(1.0, DUMP_BYTES / nbytes)
+    samples = {}
+    for name, v in arrays.items():
+        total = v.shape[0] * v.shape[1]
+        if frac < 1.0:
+            if v.shape[:2] not in samples:
+                keep = int(total * frac)
+                samples[v.shape[:2]] = torch.from_numpy(np.sort(np.random.default_rng(0).choice(total, size=keep, replace=False)))
+            v = v.reshape((total,) + tuple(v.shape[2:]))[samples[v.shape[:2]].to(v.device)]
+        np.save(os.path.join(d, name + ".npy"), v.to(torch.float64).cpu().numpy())
 
 
 def algorithmic_bytes_per_step(kernel, a, n_utts):
@@ -500,6 +539,13 @@ def main():
     prof = w.profile_report()
     clocks = sampler.stop() if rank == 0 else None
     w.synchronize()
+    if a.dump_outputs and rank == 0:
+        # what the last timed step handed its caller: the gathered arrays where the step all-gathers them (f0 / time
+        # axis always, spectrogram / aperiodicity when they fit every rank), else this rank's rows; f0 / time axis
+        # are inputs in spectral mode
+        outs = {} if spectral else {"time_axis": t_all if gather else t_loc, "f0": f0_all if gather else f0_loc}
+        outs.update(spectrogram=sp_all if gather_full else sp, aperiodicity=ap_all if gather_full else ap)
+        dump_outputs(a.dump_outputs, outs)
     if world > 1:
         tms = torch.tensor([ms], dtype=torch.float64, device=dev)
         dist.all_reduce(tms, op=dist.ReduceOp.MAX)
@@ -670,14 +716,8 @@ def main():
         nbytes = algorithmic_bytes_per_step(dom, a, U)
         kms = kernels[dom]["ms_per_step"]
         achieved = (nbytes / 1e9) / (kms / 1e3) if nbytes else None
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-        if os.path.exists(tp):
-            per_utt = json.load(open(tp)).get(dom, {}).get("dram_bytes_per_utt")
-            if per_utt:
-                traffic = per_utt * U / max(1.0, kernels[dom]["launches_per_step"])
         roof = {"kernel": dom, "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak if achieved else None, "traffic": traffic, "peak_source": peak_src,
+                "frac": achieved / peak if achieved else None, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": nbytes / max(1.0, kernels[dom]["launches_per_step"]) if nbytes else None,
                 "kernel_ms_per_step": kms, "share_of_step": kms / (ms / a.steps),
                 "note": "FP64-ALU/shared-memory bound path (SURVEY.md 8d): HBM fraction is reported as BASELINE.json asks"}
@@ -745,7 +785,7 @@ def main():
            "ms_per_step": ms / a.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
            "dtype": "f64", "data": "synthetic",
            "config": {"workload": workload_name(a), "baseline_config": a.config or None, "fs": fs, "frame_period_ms": 5.0, "frames_per_step": frames_step,
-                      "l2_policy": "inputs+outputs per step (>= 18 GB) exceed the 126 MB L2; no flush needed",
+                      "l2_policy": "inputs+outputs per step (>= 18 GB) exceed the 50 MB L2; no flush needed",
                       "multi_gpu": ("utterances sharded over ranks; the library's own NCCL communicator (C ABI) reassembles f0/time_axis" +
                                     ("/spectrogram/aperiodicity, slice by slice under the compute (peer-to-peer copies over CUDA IPC mappings; NCCL broadcasts with WB_NO_P2P=1)" if gather_full else "")) if world > 1 else "single GPU",
                       "gathered_equals_local_recompute": gather_check},

@@ -1,4 +1,4 @@
-/* world_b200.h -- batched C ABI of the B200-native WORLD analysis engine.
+/* world_b200.h -- batched C ABI of the GPU-native (H100, sm_90a) WORLD analysis engine.
  *
  * The reference (mmorise/World) has no plugin registry; its boundary is the public C API of
  * the src/world headers (SURVEY.md 8b).  That API is kept source-compatible in include/world/

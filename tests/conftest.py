@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 def _have_gpu():
@@ -21,8 +21,8 @@ def _have_gpu():
         return False
 
 
-# GPU tests that exercise code changed after the last run on a B200 (DIO's ripple path, event rings, drop-in
-# programs) run after the ones that were measured there: with `pytest -x` an early surprise must not hide the rest.
+# GPU tests of the newest code (DIO's ripple path, event rings, drop-in programs) run after the others: with
+# `pytest -x` an early surprise must not hide the rest.
 _RUN_LAST = ("golden_dio", "dio_path", "dio_decimated", "edge_cases", "long_48k", "legacy_api_and_analyze_host",
              "analyze_coded_host", "host_pipeline_chunking", "event_dense", "zero_tail_f0", "mirroring_ripple",
              "reference_examples", "cpp_batched")
@@ -40,13 +40,10 @@ def pytest_collection_modifyitems(config, items):
 
 @pytest.fixture(scope="session")
 def ref():
-    """The unmodified reference compiled into oracle/_ref (prebuilt file travels to the GPU box)."""
+    """The unmodified reference, compiled into oracle/_ref by build() where its sources are present."""
     from refworld import RefWorld, REF_LIB
     if not os.path.exists(REF_LIB):
-        if os.path.isdir("/root/reference/src"):
-            subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "ref"])
-        else:
-            pytest.skip("oracle/_ref/libworld_ref.so missing and /root/reference absent")
+        pytest.skip("oracle/_ref/libworld_ref.so missing: build() found no reference sources")
     return RefWorld(REF_LIB)
 
 

@@ -1,5 +1,5 @@
 """Parity tests proper: the CUDA library (through the C ABI) against the golden vectors and the
-compiled reference, on a real B200.  Tolerance 1e-6 relative (north_star); integers bit exact."""
+compiled reference, on a real GPU.  Tolerance 1e-6 relative (north_star); integers bit exact."""
 import numpy as np
 import pytest
 

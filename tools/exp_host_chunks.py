@@ -1,5 +1,5 @@
 """GPU experiment: host pipeline (world_b200_analyze_host / _coded_host) versus its outer / sub chunk sizes.
-Usage on the GPU box:  python tools/exp_host_chunks.py [n_utts] > gpurun_out/host_chunks.txt"""
+Usage (on a GPU machine):  python tools/exp_host_chunks.py [n_utts] > host_chunks.txt"""
 import os
 import sys
 import time

@@ -16,7 +16,7 @@ def line_table(kernel):
     tmp = tempfile.mkdtemp()
     subprocess.run(["cuobjdump", "-xelf", "all", os.path.join(ROOT, "world_b200", "lib", "libworld_b200.so")],
                    cwd=tmp, capture_output=True)
-    for cub in glob.glob(os.path.join(tmp, "*sm_100a.cubin")):
+    for cub in glob.glob(os.path.join(tmp, "*sm_90a.cubin")):
         txt = subprocess.run(["nvdisasm", "--print-line-info", cub], capture_output=True, text=True).stdout
         m = re.search(r"\.text\.(\S*%s\S*):" % re.escape(kernel), txt)
         if not m:

@@ -1,7 +1,7 @@
 """ctypes mirror of the batched C ABI (include/world_b200.h) and of the reference's operator
 names (Dio / Harvest / StoneMask / CheapTrick / D4C, src/world/*.h).
 
-This module is plumbing: it loads ``world_b200/lib/libworld_b200.so`` (hand-written sm_100a CUDA
+This module is plumbing: it loads ``world_b200/lib/libworld_b200.so`` (hand-written sm_90a CUDA
 behind an extern "C" ABI), hands it raw pointers and returns arrays.  There is no Python or CPU
 implementation of any stage behind it -- if the library or a CUDA device is missing, loading
 or ``World()`` raises.
@@ -153,7 +153,7 @@ def load_library(path: str | None = None) -> C.CDLL:
     path = path or os.environ.get("WORLD_B200_LIB") or DEFAULT_LIB
     if not os.path.exists(path):
         raise WorldError(f"{path} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                         "(nvcc, sm_100a).  There is no CPU fallback.")
+                         "(nvcc, sm_90a).  There is no CPU fallback.")
     lib = C.CDLL(path)
     for name, (res, args) in ABI.items():
         fn = getattr(lib, name)  # AttributeError if the ABI is incomplete

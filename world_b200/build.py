@@ -1,4 +1,4 @@
-"""Builds world_b200/lib/libworld_b200.so with nvcc for sm_100a (in-tree, no torch involved)."""
+"""Builds world_b200/lib/libworld_b200.so with nvcc for sm_90a (in-tree, no torch involved)."""
 import os
 import subprocess
 import sys
@@ -13,7 +13,7 @@ SOURCES = ["wb_api.cu", "wb_host.cu", "wb_rng.cu", "wb_cheaptrick.cu", "wb_d4c.c
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 # -fmad=false: values that feed int casts / comparisons must round like the reference's x86-64 -O1
 # build (SURVEY.md App. B2); hot loops use explicit fma() where contraction is harmless.
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "-fmad=false",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-fmad=false",
          "-Xcompiler", "-fPIC", "-Xptxas", "-v", "-I", os.path.join(HERE, "..", "include")]
 
 
@@ -34,6 +34,10 @@ def build(verbose=False, force=False, defines=(), tag=""):
     os.makedirs(objdir, exist_ok=True)
     out = os.path.join(LIBDIR, "libworld_b200%s.so" % ("_" + tag if tag else ""))
     flags = FLAGS + ["-D" + d for d in defines]
+    # objects compiled with other flags (another architecture, say) are stale whatever their mtime
+    stamp = os.path.join(objdir, "flags.txt")
+    if not os.path.exists(stamp) or open(stamp).read() != " ".join(flags):
+        force = True
     jobs = []
     for s in SOURCES:
         src = os.path.join(CSRC, s)
@@ -61,6 +65,8 @@ def build(verbose=False, force=False, defines=(), tag=""):
         r = subprocess.run([NVCC, "-shared", "-o", out] + objs + ["-lcudart", "-ldl"], capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n" + r.stdout + r.stderr)
+    with open(stamp, "w") as f:
+        f.write(" ".join(flags))
     return out
 
 

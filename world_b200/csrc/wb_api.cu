@@ -316,7 +316,7 @@ int world_b200_create(int device, WorldB200 **out) {
   if (cudaSetDevice(device) != cudaSuccess) { delete h; return WORLD_B200_ECUDA; }
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) h->c.sm_count = prop.multiProcessorCount;
-  // default scratch budget: a third of what is free now, between 4 and 64 GiB (a B200 has 180 GB; the
+  // default scratch budget: a third of what is free now, between 4 and 64 GiB (an H100 has 80 GB; the
   // larger the passes, the fewer launches of the latency-bound per-utterance kernels)
   size_t free_b = 0, total_b = 0;
   if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess) {
@@ -574,7 +574,7 @@ static int analyze_batch_impl(WorldB200 *h, const double *x, int n, int x_stride
   }
   const int bins = opt->cheaptrick.fft_size / 2 + 1;
   const double frame_period = opt->f0_method == WORLD_B200_F0_HARVEST ? opt->harvest.frame_period : opt->dio.frame_period;
-  // two slices (one per lane) overlap best on one GPU (profiles/r2d: 861 / 869 / 872 ms for 2 / 4 / 8 slices); with the
+  // two slices (one per lane) overlap best on one GPU (more slices only add launches); with the
   // gather the exposed tail is the LAST slice's transfer, so more, smaller slices win there
   int n_slices = gather ? 10 : 2;
   if (const char *e = getenv("WB_LANE_SLICES")) n_slices = atoi(e);
@@ -600,8 +600,8 @@ static int analyze_batch_impl(WorldB200 *h, const double *x, int n, int x_stride
         if (rc) { h->c.last_error = "analyze_batch: cannot create a lane context"; return rc; }
         cudaStream_t st;
         cudaEvent_t ev;
-        // equal (lowest) priority for both lanes: giving one lane the highest priority was measured slower
-        // (profiles/r2l: 804 vs 794 ms); only the communication stream outranks them (wb_multi.cu)
+        // equal (lowest) priority for both lanes: giving one lane the highest priority was measured slower;
+        // only the communication stream outranks them (wb_multi.cu)
         if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess ||
             cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) {
           h->c.last_error = "analyze_batch: cannot create a lane stream";

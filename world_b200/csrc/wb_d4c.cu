@@ -247,7 +247,7 @@ WB_DEV double select_kth_largest(const double *a, int n, int kth, double *red) {
 }
 
 // The same order statistic through a short candidate list (GPU only; round 1's bisection -- 32 rounds over all n
-// values with a barrier each -- was a quarter of the body kernel's instructions, profiles/r2c_ncu_d4c_body_kernel.txt):
+// values with a barrier each -- was a large share of the body kernel's instructions):
 //   1. every thread takes the maximum of the values it owns (a[tid], a[tid + nth], ...);
 //   2. L = the kth largest of those maxima (of 32 maxima over four threads each when kth <= 32) is a lower bound of
 //      the answer (the kth largest maxima are kth distinct elements >= L), and for spectra -- no long runs of equal
@@ -338,8 +338,7 @@ WB_DEV bool select_kth_largest_fast(const double *a, int n, int kth, unsigned lo
 // frame when d_fft > 4096 (this kernel's thread count would not fit a CTA).
 // Doubles of the power row.  It also holds the windowed signal of the centroid transforms, whose longest window (f0
 // at the 47 Hz floor, ratio 4) is up to twice d_fft / 2 + 1; shared memory per CTA decides how many CTAs an SM holds
-// and the kernel is latency bound (profiles/r2e: sizing the row for the longest window cost a CTA per SM at 48 kHz
-// and 13 % of the kernel), so the row grows only as far as the CTA count of the minimal layout allows.  Frames with
+// and the kernel is latency bound (sizing the row for the longest window costs a CTA per SM at 48 kHz), so the row grows only as far as the CTA count of the minimal layout allows.  Frames with
 // a longer window (f0 below ~54 Hz at 16 kHz, ~75 Hz at 48 kHz) go to slow_list / d4c_body_slow_kernel.
 WB_HD inline size_t d4c_body_smem_bytes_for(int d_fft, int pw_doubles, int n_ap, int threads) {
   return (size_t)WB_FPAD_SLOTS(d_fft / 2) * sizeof(double2) +

@@ -459,7 +459,7 @@ WB_KERNEL(WB_SWEEP_THREADS, 3) band_sweep_list_kernel(SweepParams p) {
 //
 // band_sweep_kernel does everything for one (utterance, band) in one streaming pass: FIR tile, event detection,
 // compaction, interval rings, frame finalisation -- fourteen block barriers per tile and a round trip of the fine
-// edges through global memory; the FIR ran at 45 % of the FP64 pipe (profiles/r2c_ncu_band_sweep_kernel.txt).
+// edges through global memory, which leaves the FIR's FP64 pipe idle for much of the tile.
 // Split:
 //   band_fir_events_kernel  FIR (the same register tile, the same FMA order: bit-identical filtered samples) +
 //                           the four event trains of every tile, fine edges appended to COMPLETE per-train lists
@@ -500,7 +500,7 @@ WB_DEV void mbar_wait(unsigned long long *bar, unsigned parity) {
 
 // Warp-specialised: warps 0-3 (128 threads) only filter -- tile t+1 while warps 4-7 pick the events of tile t out of
 // the other half of the double-buffered output tile.  The first version ran the two phases one after the other in
-// all eight warps: the FP64 pipe idled through every event phase (57 % busy, profiles/r2f_ncu_band_fir_events_kernel.txt).
+// all eight warps: the FP64 pipe idled through every event phase.
 // Hand-over by named barriers (bar.arrive on one side, bar.sync on the other): full[2] filter -> events,
 // empty[2] events -> filter; the input segments arrive by TMA on two mbarriers.
 #define WB_FE_GROUP 128                      // threads per role
@@ -513,8 +513,8 @@ WB_DEV void bar_arrive_named(int id, int count) { asm volatile("bar.arrive %0, %
 // acc[r] += h * w[r], r = 0..8, as ONE block of nine DFMAs in this order.  A DFMA reads three 64-bit operands; the
 // register file delivers two per issue slot of the half-rate FP64 pipe, the third has to come from the operand-reuse
 // cache, i.e. from the previous instruction's same slot.  Left to the scheduler, the nine FMAs of a tap were
-// interleaved with those of other taps (13 % of the kernel's DFMAs carried a reuse flag, FP64 pipe stuck at 58 %,
-// profiles/r2m); written as one block `h` stays in its slot for all nine.
+// interleaved with those of other taps (few DFMAs carried a reuse flag); written as one block `h` stays in its slot
+// for all nine.
 WB_DEV void fe_fma9(double (&acc)[9], double h, double w0, double w1, double w2, double w3, double w4, double w5,
                     double w6, double w7, double w8) {
 #ifdef WB_EMU
@@ -879,8 +879,8 @@ WB_KERNEL(256, 4) band_interp_kernel(SweepParams p) {
     WB_SYNC();
     bool more = true;
     // One pass over the (train, interval) pairs of all four windows: the four trains' loads and divisions run side by
-    // side instead of one latency chain after the other (profiles/r2p: a quarter of the kernel's samples waited at the
-    // barrier behind the 20-60 loading threads of a low band).  The thread that loads a window's last interval tells
+    // side instead of one latency chain after the other (otherwise the kernel waits at the barrier
+    // behind the 20-60 loading threads of a low band).  The thread that loads a window's last interval tells
     // the CTA through more_flag[] whether that interval still starts inside the round; the flag of the next iteration
     // is cleared while this one's is read.
     for (int itn = 0; more; ++itn) {

@@ -167,8 +167,8 @@ WB_DEV void split_pair(const double2 *z, int n, int k, double2 &A, double2 &B) {
 
 // =============================================================================================
 // Stockham (self-sorting) FFT, round 2.  The in-place DIT above needs a bit-reversal pass and its first
-// passes walk shared memory with power-of-two strides of double2: 38-50 % of the shared wavefronts of the
-// frame kernels were bank conflicts (profiles/r1l_ncu_*).  The transform below goes natural order in ->
+// passes walk shared memory with power-of-two strides of double2: a large share of the shared wavefronts of
+// the frame kernels were bank conflicts.  The transform below goes natural order in ->
 // natural order out with NO permutation pass, ping-ponging between two buffers (one barrier per pass, any
 // block size, also one emulated thread), and every access is conflict free:
 //   * layout: element i of a buffer lives at fpad(i) = i + (i >> 3) (one spare double2 per 8);

@@ -210,7 +210,7 @@ WB_DEV void hv_refine_one(const double *__restrict__ y, int y_len, double afs, d
       // twiddles exp(-j 2 pi bin j / nfft) by rotation: four interleaved chains (one per unrolled
       // slot) start from exact table values and advance by exp(-j 2 pi bin 4 cstep / nfft); a
       // chain is <= nwin / (4 cstep) steps long, so the accumulated rounding stays ~1e-15.
-      // (A table gather per sample made this kernel L1-LSU bound: profiles/r1c.)
+      // (A table gather per sample made this kernel L1-LSU bound.)
       const double2 rot = hv_tw(tw, ((bin * 4 * cstep) & (nfft - 1)) << shift);
       double2 wq[4];
 #pragma unroll
@@ -326,8 +326,8 @@ WB_KERNEL(32 * WB_HV_WARPS, 6) harvest_refine_kernel(HvRefineParams p) {
 // it builds the template once (w e^{-j theta}, dw e^{-j theta}) and feeds 7 x 4 accumulators from the seven
 // S-shifted samples.  Outputs go to slot j of frame k, slot j + nc g of frame k + g and slot j + nc (g + 3) of
 // frame k - g (the inverse of hv_slot_candidate); every other slot keeps the zero the driver memset.
-// Default since round 2 wherever S is integral (profiles/r2b: 379.5 -> 152.1 ms per 1024 x 10 s, f0 within 2e-14 of
-// the reference with no V/UV flip on the GPU); WB_NO_REFINE_CHAIN=1 selects the per-frame kernel for A/B runs.
+// Default wherever S is integral (the per-frame kernel recomputes each template seven times; f0 stays within the
+// parity bound with no V/UV flip); WB_NO_REFINE_CHAIN=1 selects the per-frame kernel for A/B runs.
 //
 // Lane-generic source: WB_FOR_LANES runs the lane body for lane = threadIdx.x & 31 on the GPU and for all 32
 // lanes in turn in the host emulation, so the lane layout and the shuffles are checked on the CPU too.
@@ -452,7 +452,7 @@ WB_DEV void refine_chain_body(const HvChainParams &cp) {
           for (int g = 0; g < 7; ++g) {
             const double xv = xs[i + S * g];
             // (pinning these four DFMAs in one asm block for operand reuse, as fe_fma9 does for the FIR, was measured
-            // slower here: 164 vs 152 ms, profiles/r2n -- the scheduler needs the freedom to hide the smem loads)
+            // slower here -- the scheduler needs the freedom to hide the smem loads)
             a[4 * g + 0] = fma(xv, P, a[4 * g + 0]);
             a[4 * g + 1] = fma(xv, Q, a[4 * g + 1]);
             a[4 * g + 2] = fma(xv, R, a[4 * g + 2]);

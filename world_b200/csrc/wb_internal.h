@@ -45,7 +45,7 @@ struct Ctx {
   Staging staging;
   std::vector<PoolBuf> pool;
   size_t scratch_budget = (size_t)24 << 30;  // bytes of scratch a stage may use per chunk
-  int sm_count = 148;
+  int sm_count = 132;
   int *status_dev = nullptr;         // sticky device-side error word
   std::string last_error;
 };

@@ -107,7 +107,7 @@ int comm_create(int n_ranks, int rank, const unsigned char *id128, Comm **out, s
   if (r != ncclSuccess) { *err = std::string("ncclCommInitRank: ") + g_nccl.GetErrorString(r); delete c; return 1; }
   // highest stream priority: when a compute kernel's CTA retires, the waiting blocks of the collective are placed
   // first -- at equal priority the blocks of the (earlier launched, 10^5-block) compute kernels keep filling the SMs
-  // and the transfer only runs in their tails (profiles/r2j: 8 ranks at 0.84 with the transfer enqueued "under" the compute)
+  // and the transfer only runs in their tails
   int prio_least = 0, prio_greatest = 0;
   cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest);
   if (cudaStreamCreateWithPriority(&c->stream, cudaStreamNonBlocking, prio_greatest) != cudaSuccess ||
@@ -192,9 +192,8 @@ int comm_gather_rows_multi(Comm *c, int n_arrays, double *const *full, const siz
 
 // ---------------------------------------------------------------------------------------------------------------
 // Peer-to-peer push (one process per GPU, all on one NVLink / NVSwitch node).  With NCCL the transfer of an output
-// slice is a kernel on every rank: 16-32 CTAs that occupy SMs for as long as the bytes flow -- eight ranks gathering
-// 118 GB per step each cost the compute ~100 ms (profiles/r2o: 0.89 of the single-GPU rate; fewer channels only make
-// the transfer the bottleneck, r2q).  Here every rank maps the other ranks' output arrays (CUDA IPC handles, exchanged
+// slice is a kernel on every rank: 16-32 CTAs that occupy SMs for as long as the bytes flow, taken from the compute
+// (fewer channels only make the transfer the bottleneck).  Here every rank maps the other ranks' output arrays (CUDA IPC handles, exchanged
 // ONCE per set of arrays through the communicator itself) and, as soon as a slice of its own rows is final, copies
 // them into every peer's array with cudaMemcpyAsync on a copy stream: the copy engines move the bytes over NVLink,
 // no SM is involved.  A rank only ever writes rows of its own block, so pushes never collide; one 4-byte all-reduce

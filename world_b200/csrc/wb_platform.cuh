@@ -1,5 +1,5 @@
 // wb_platform.cuh -- one place that knows whether the kernel sources are being compiled by
-// nvcc for sm_100a (the product) or by g++ as a single-thread host emulation (tests only).
+// nvcc for sm_90a (the product) or by g++ as a single-thread host emulation (tests only).
 //
 // The emulation exists because the development container has no GPU: every kernel in this
 // tree is written block-size-agnostic (strided `for (i = tid; i < n; i += nthreads)` phases

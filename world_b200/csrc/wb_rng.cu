@@ -5,7 +5,7 @@
 // CheapTrick()/D4C() call (cheaptrick.cpp:205-206, d4c.cpp:345-346) and consumed frame after
 // frame, so frame i's noise depends on how many draws frames 0..i-1 took.
 //
-// B200 restatement: the draw counts per frame are a pure function of f0 (counted by the
+// GPU restatement: the draw counts per frame are a pure function of f0 (counted by the
 // stage's own kernel), an exclusive scan gives every frame its offset into the utterance's
 // stream, and the stream itself is materialised by `rng_fill_kernel`: thread g produces draws
 // [128 g, 128 g + 128) after jumping there with popcount(g) GF(2) matrix-vector products
