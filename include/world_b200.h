@@ -74,6 +74,10 @@ int world_b200_profile_report(WorldB200 *ctx, char *buf, unsigned long long cap)
  * events): the roofline the analysis path is bound by (no FP64 figure exists in MEASURED_PEAKS). */
 int world_b200_fp64_peak(WorldB200 *ctx, double *tflops);
 
+/* Measured FP64 tensor-core peak of the device in TFLOP/s: the same harness with 8 independent
+ * mma.m16n8k4.f64 chains per warp (Harvest's band-pass filter bank runs on this pipe). */
+int world_b200_fp64_tensor_peak(WorldB200 *ctx, double *tflops);
+
 /* Test hook: forward real FFT of n = 2^k doubles (4 <= n <= 8192) with the library's shared-memory
  * FFT; out_dev receives n/2+1 interleaved complex values (n + 2 doubles).  DEVICE pointers. */
 int world_b200_rfft_test(WorldB200 *ctx, const double *x_dev, int n, double *out_dev);

@@ -63,6 +63,7 @@ ABI = {
     "world_b200_rfft_test": (C.c_int, [_P, _P, C.c_int, _P]),
     "world_b200_sfft_test": (C.c_int, [_P, _P, C.c_int, _P]),
     "world_b200_fp64_peak": (C.c_int, [_P, C.POINTER(C.c_double)]),
+    "world_b200_fp64_tensor_peak": (C.c_int, [_P, C.POINTER(C.c_double)]),
     "world_b200_profile": (C.c_int, [_P, C.c_int]),
     "world_b200_profile_report": (C.c_int, [_P, C.c_char_p, C.c_ulonglong]),
     "world_b200_dio_batch": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(DioOption), _P, _P, C.c_int]),
@@ -255,6 +256,11 @@ class World:
     def fp64_peak(self) -> float:
         v = C.c_double(0.0)
         self._check(self.lib.world_b200_fp64_peak(self._h, C.byref(v)))
+        return v.value
+
+    def fp64_tensor_peak(self) -> float:
+        v = C.c_double(0.0)
+        self._check(self.lib.world_b200_fp64_tensor_peak(self._h, C.byref(v)))
         return v.value
 
     def profile(self, enable=True):

@@ -837,6 +837,58 @@ int world_b200_fp64_peak(WorldB200 *h, double *tflops) {
 #endif
 }
 
+// FP64 tensor-core (DMMA) peak: the same harness with 8 independent mma.m16n8k4.f64 chains per warp
+// (16 x 8 x 4 MACs per instruction) instead of DFMA chains.
+#ifndef WB_EMU
+__global__ void fp64_tensor_peak_kernel(double *out, int iters) {
+  double c[8][4];
+  const double a = 1e-3 * (threadIdx.x & 7), b = 1e-3;
+#pragma unroll
+  for (int k = 0; k < 8; ++k)
+    for (int r = 0; r < 4; ++r) c[k][r] = k + r;
+  for (int i = 0; i < iters; ++i) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+      asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+                   : "+d"(c[k][0]), "+d"(c[k][1]), "+d"(c[k][2]), "+d"(c[k][3]) : "d"(a), "d"(a), "d"(b));
+  }
+  double s = 0.0;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) s += c[k][0] + c[k][1] + c[k][2] + c[k][3];
+  out[blockIdx.x * blockDim.x + threadIdx.x] = s;
+}
+#endif
+
+int world_b200_fp64_tensor_peak(WorldB200 *h, double *tflops) {
+  if (!h || !tflops) return WORLD_B200_EINVAL;
+  DeviceGuard guard_(&h->c);
+  *tflops = 0.0;
+#ifndef WB_EMU
+  Ctx *ctx = &h->c;
+  const int blocks = ctx->sm_count * 8, threads = 256, iters = 1 << 12;
+  unsigned char *blk = arena_block(ctx, (size_t)blocks * threads * 8);
+  if (!blk) return WORLD_B200_ENOMEM;
+  cudaEvent_t a, b;
+  cudaEventCreate(&a); cudaEventCreate(&b);
+  float best = 1e30f;
+  for (int rep = 0; rep < 4; ++rep) {
+    cudaEventRecord(a, ctx->stream);
+    fp64_tensor_peak_kernel<<<blocks, threads, 0, ctx->stream>>>((double *)blk, iters);
+    cudaEventRecord(b, ctx->stream);
+    cudaEventSynchronize(b);
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, a, b);
+    if (rep > 0 && ms < best) best = ms;
+  }
+  cudaEventDestroy(a); cudaEventDestroy(b);
+  // per warp and iteration: 8 MMAs of 16 x 8 x 4 multiply-adds
+  *tflops = (double)blocks * (threads / 32) * iters * 8 * (16 * 8 * 4) * 2 / (best * 1e-3) / 1e12;
+  return dev_check(ctx, "fp64_tensor_peak");
+#else
+  return 0;
+#endif
+}
+
 // Known-answer hook for the shared-memory FFT: r2c of n = 2^lg reals (n/2+1 complex out), one CTA.
 namespace wb {
 WB_KERNEL(128, 1) rfft_test_kernel(const double *x, int n, int lg, double *out, const double2 *tw) {

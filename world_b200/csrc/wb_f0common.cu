@@ -461,12 +461,12 @@ WB_KERNEL(WB_SWEEP_THREADS, 3) band_sweep_list_kernel(SweepParams p) {
 // compaction, interval rings, frame finalisation -- fourteen block barriers per tile and a round trip of the fine
 // edges through global memory, which leaves the FIR's FP64 pipe idle for much of the tile.
 // Split:
-//   band_fir_events_kernel  FIR (the same register tile, the same FMA order: bit-identical filtered samples) +
-//                           the four event trains of every tile, fine edges appended to COMPLETE per-train lists
-//                           in global memory (written once, never read back here).  Three block barriers per tile.
-//                           The input segment of the next tile arrives by TMA (cp.async.bulk + mbarrier) while the
-//                           current one is filtered: nine outputs per thread make consecutive threads 9 doubles
-//                           apart -- conflict free without padding, so the segment is one contiguous bulk copy.
+//   band_fir_events_kernel  FIR on the FP64 tensor cores (polyphase DMMA, fe_fir_warp: the same sums as the
+//                           streaming kernel's DFMA tile in another order, so the filtered samples agree to rounding,
+//                           not bit for bit) + the four event trains of every tile, fine edges appended to COMPLETE
+//                           per-train lists in global memory (written once, never read back here).  Three block
+//                           barriers per tile.  The input segment of the next tile arrives by TMA (cp.async.bulk +
+//                           mbarrier) while the current one is filtered.
 //   band_interp_kernel      edge lists -> intervals -> interp1 onto the frame grid, 256 frames per round; interval
 //                           counts per frame by a fill (every interval owns the frames between its first frame and
 //                           the next interval's), no search, no scan.
@@ -504,68 +504,76 @@ WB_DEV void mbar_wait(unsigned long long *bar, unsigned parity) {
 // Hand-over by named barriers (bar.arrive on one side, bar.sync on the other): full[2] filter -> events,
 // empty[2] events -> filter; the input segments arrive by TMA on two mbarriers.
 #define WB_FE_GROUP 128                      // threads per role
-#define WB_FE_TILE (WB_FE_R * WB_FE_GROUP)   // outputs per tile
 #ifndef WB_EMU
 WB_DEV void bar_sync_named(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 WB_DEV void bar_arrive_named(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 #endif
 
-// acc[r] += h * w[r], r = 0..8, as ONE block of nine DFMAs in this order.  A DFMA reads three 64-bit operands; the
-// register file delivers two per issue slot of the half-rate FP64 pipe, the third has to come from the operand-reuse
-// cache, i.e. from the previous instruction's same slot.  Left to the scheduler, the nine FMAs of a tap were
-// interleaved with those of other taps (few DFMAs carried a reuse flag); written as one block `h` stays in its slot
-// for all nine.
-WB_DEV void fe_fma9(double (&acc)[9], double h, double w0, double w1, double w2, double w3, double w4, double w5,
-                    double w6, double w7, double w8) {
-#ifdef WB_EMU
-  acc[0] = fma(h, w0, acc[0]); acc[1] = fma(h, w1, acc[1]); acc[2] = fma(h, w2, acc[2]);
-  acc[3] = fma(h, w3, acc[3]); acc[4] = fma(h, w4, acc[4]); acc[5] = fma(h, w5, acc[5]);
-  acc[6] = fma(h, w6, acc[6]); acc[7] = fma(h, w7, acc[7]); acc[8] = fma(h, w8, acc[8]);
-#else
-  asm("fma.rn.f64 %0, %9, %10, %0;\n\t"
-      "fma.rn.f64 %1, %9, %11, %1;\n\t"
-      "fma.rn.f64 %2, %9, %12, %2;\n\t"
-      "fma.rn.f64 %3, %9, %13, %3;\n\t"
-      "fma.rn.f64 %4, %9, %14, %4;\n\t"
-      "fma.rn.f64 %5, %9, %15, %5;\n\t"
-      "fma.rn.f64 %6, %9, %16, %6;\n\t"
-      "fma.rn.f64 %7, %9, %17, %7;\n\t"
-      "fma.rn.f64 %8, %9, %18, %8;"
-      : "+d"(acc[0]), "+d"(acc[1]), "+d"(acc[2]), "+d"(acc[3]), "+d"(acc[4]), "+d"(acc[5]), "+d"(acc[6]), "+d"(acc[7]),
-        "+d"(acc[8])
-      : "d"(h), "d"(w0), "d"(w1), "d"(w2), "d"(w3), "d"(w4), "d"(w5), "d"(w6), "d"(w7), "d"(w8));
-#endif
+#ifndef WB_EMU
+// D = A B + D, one m16n8k8 FP64 tensor-core MMA (DMMA).  Fragments of lane (g, t) = (lane / 4, lane % 4): a0 / a1 =
+// A[g][t] / A[g + 8][t], a2 / a3 = A[g][t + 4] / A[g + 8][t + 4]; b0 / b1 = B[t][g] / B[t + 4][g]; d0, d1 = D[g][2t],
+// D[g][2t + 1]; d2, d3 = D[g + 8][2t], D[g + 8][2t + 1].
+WB_DEV void mma_f64_16x8x8(double (&d)[4], double a0, double a1, double a2, double a3, double b0, double b1) {
+  asm("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
+      : "d"(a0), "d"(a1), "d"(a2), "d"(a3), "d"(b0), "d"(b1));
 }
+#endif
 
-// FIR of register group g (outputs 9 g .. 9 g + 8 of the tile): the same FMA order as band_sweep_kernel
-WB_DEV void fe_fir_group(const double *seg, const double *hrev, int ntaps, int g, double *st) {
-  const int R = WB_FE_R, base = R * g;
-  double acc[WB_FE_R], win[WB_FE_R];
-  const double *sp = seg + base + R;
-  const double *hp = hrev;
-#pragma unroll
-  for (int r = 0; r < R; ++r) { acc[r] = 0.0; win[r] = seg[base + r]; }
-  for (int j0 = 0; j0 < ntaps; j0 += R, sp += R, hp += R) {
-#pragma unroll
-    for (int jj = 0; jj < R; ++jj) {
-      const double hj = hp[jj];
-      fe_fma9(acc, hj, win[jj % 9], win[(jj + 1) % 9], win[(jj + 2) % 9], win[(jj + 3) % 9], win[(jj + 4) % 9],
-              win[(jj + 5) % 9], win[(jj + 6) % 9], win[(jj + 7) % 9], win[(jj + 8) % 9]);
-      win[jj] = sp[jj];
+// Polyphase FIR of filter warp w on the FP64 tensor cores: outputs y[m] = sum_j h[j] s[m + par + j] of the tile.
+// With rows of 8 outputs, Y[i][p] = y[8 i + p], this is the product Y = A B with A[i][k] = s[8 i + k] and
+// B[k][p] = h[k - p - par] (zero outside the taps), k < 8 nq.  One m16n8k8 MMA covers 16 rows and 8 k; warp w owns
+// rows 32 w .. 32 w + 31, two row tiles that share every B fragment.
+//  * The order of k inside an MMA is free as long as A and B agree: slot t carries k = 2t and slot t + 4 carries
+//    k = 2t + 1, so a lane's two A elements of a row are adjacent -- one 128-bit load, conflict free (8 lanes read
+//    128 contiguous bytes).  That needs s 16-byte aligned; an odd start is moved into the taps (`par`).
+//  * A of k-step q + 8 is A of step q moved down by 8 rows, one register octet.  So the k-steps run as 8 chains
+//    q = r, r + 8, ... and each step loads one new octet for both row tiles: per MMA a quarter of an A fragment and
+//    half a B fragment come from shared memory, half of what it delivers at the DMMA rate.
+// hb: the taps with 8 zeros before hb[0] and zeros after them up to hb[8 nq - 1]; st: pad8 layout.
+WB_DEV void fe_fir_warp(const double *s, const double *hb, int par, int nq, int w, int lane, double *st) {
+#ifdef WB_EMU
+  (void)lane;   // the same sums, fma in k order (= tap order: the products with the padding zeros are exact zeros)
+  for (int m = 256 * w; m < 256 * w + 256; ++m) {
+    const int p = m & 7;
+    double acc = 0.0;
+    for (int k = 0; k < 8 * nq; ++k) acc = fma(s[m - p + k], hb[k - p - par], acc);
+    st[pad8(m)] = acc;
+  }
+#else
+  const int g = lane >> 2, t = lane & 3;
+  const double *sa = s + 8 * (32 * w + g) + 2 * t;   // octet o of step q (rows 32 w + 8 o + g + q): sa + 8 (q + 8 o)
+  const double *hp = hb + 2 * t - g - par;           // B of step q: hp[8 q], hp[8 q + 1]
+  double c[2][4] = {{0.0, 0.0, 0.0, 0.0}, {0.0, 0.0, 0.0, 0.0}};
+  for (int r = 0; r < 8 && r < nq; ++r) {
+    double2 o0 = *reinterpret_cast<const double2 *>(sa + 8 * r);
+    double2 o1 = *reinterpret_cast<const double2 *>(sa + 8 * (r + 8));
+    double2 o2 = *reinterpret_cast<const double2 *>(sa + 8 * (r + 16));
+    for (int q = r; q < nq; q += 8) {
+      const double2 o3 = *reinterpret_cast<const double2 *>(sa + 8 * (q + 24));
+      const double b0 = hp[8 * q], b1 = hp[8 * q + 1];
+      mma_f64_16x8x8(c[0], o0.x, o1.x, o0.y, o1.y, b0, b1);
+      mma_f64_16x8x8(c[1], o2.x, o3.x, o2.y, o3.y, b0, b1);
+      o0 = o1; o1 = o2; o2 = o3;
     }
   }
 #pragma unroll
-  for (int r = 0; r < R; ++r) st[base + r] = acc[r];
+  for (int m = 0; m < 2; ++m) {   // rows g and g + 8 of row tile m, outputs 2t and 2t + 1 of each
+    const int row = 32 * w + 16 * m + g;
+    st[9 * row + 2 * t] = c[m][0]; st[9 * row + 2 * t + 1] = c[m][1];
+    st[9 * (row + 8) + 2 * t] = c[m][2]; st[9 * (row + 8) + 2 * t + 1] = c[m][3];
+  }
+#endif
 }
 
-// the 11 filtered samples group g looks at: positions pos = 9 g + r (relative to n0 - 2) need s[pos .. pos + 2];
-// sample p of that axis is carry[p] for p < 2 (the last two outputs of the previous tile), st[p - 2] otherwise
+// the 10 filtered samples group g looks at: positions pos = 8 g + r (relative to n0 - 2) need s[pos .. pos + 2];
+// sample p of that axis is carry[p] for p < 2 (the last two outputs of the previous tile), st[pad8(p - 2)] otherwise
 WB_DEV void fe_load_group(const double *st, double c0, double c1, int g, double (&v)[WB_FE_R + 2]) {
   const int base = WB_FE_R * g;
 #pragma unroll
   for (int k = 0; k < WB_FE_R + 2; ++k) {
     const int pp = base + k;
-    v[k] = pp >= 2 ? st[pp - 2] : (pp == 0 ? c0 : c1);
+    v[k] = pp >= 2 ? st[pad8(pp - 2)] : (pp == 0 ? c0 : c1);
   }
 }
 
@@ -645,20 +653,22 @@ WB_DEV void fe_emit_group(const double (&v)[WB_FE_R + 2], unsigned long long mas
 // so a CTA with one band is either waiting for its filter warps or for its event warps; the pair sums are within
 // 2x of each other and sit on the filter side.  Both bands read the same input segment (the long band's).
 struct FeBand {
-  int ntaps, seg_off, cap, band;   // seg_off: where this band's segment starts inside the pair's (long) segment
+  int ntaps, cap, band;
+  int s_off, par, nq;   // the band's FIR input starts at seg[s_off + par], s_off even; k-steps of fe_fir_warp
   double *edges;
 };
 
+// Three CTAs per SM (80 registers, about 51 KB of shared memory each): on H100 the isolated kernel took 169 ms per
+// 1024 x 10 s step; two CTAs per SM with 102 registers and no spills took 179 ms.
 WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
   WB_DYN_SMEM(double, smem);
   const int pr = blockIdx.x, u = blockIdx.y;
   const int T = WB_FE_TILE, R = WB_FE_R, G = WB_FE_GROUP;
-  const int segd = fe_seg_doubles(p.max_taps);
+  const int segd = fe_seg_doubles(p.max_taps), hcap = fe_hrev_doubles(p.max_taps);
   double *segbuf[2] = {smem, smem + segd};
-  const int hcap = ((p.max_taps + R - 1) / R) * R + R;
   double *hrev[2] = {smem + 2 * segd, smem + 2 * segd + hcap};
-  double *stbuf[2] = {hrev[1] + hcap, hrev[1] + hcap + (T + 2)};
-  unsigned long long *wtot = reinterpret_cast<unsigned long long *>(stbuf[1] + (T + 2));   // [2][4] warp totals
+  double *stbuf[2] = {hrev[1] + hcap, hrev[1] + hcap + fe_st_doubles()};
+  unsigned long long *wtot = reinterpret_cast<unsigned long long *>(stbuf[1] + fe_st_doubles());   // [2][4] warp totals
   unsigned long long *bars = wtot + 8;           // two mbarriers
   const int ylen = p.y_len[u];
   const size_t abs0 = (size_t)u * p.sig_stride + p.sig_origin;   // index of s(0) in p.sig
@@ -667,25 +677,28 @@ WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
   const int nslot = b_short > b_long ? 2 : 1;    // the middle band of an odd count is alone
   FeBand fb[2];
   const int lead = p.shift[b_long] - p.ntaps[b_long] + 1;     // segment of tile t starts at s(t T + lead)
+  // seg[i] = s(n0 + lead - odd + i), odd = (abs0 + lead) & 1: the bulk copy starts at an even index of p.sig (T is
+  // even, so the same for every tile).  A band reads seg[s_off .. s_off + T + 8 nq): the short filter starts later and
+  // ends earlier than the long one, so that lies inside segd = T + fe_kpad(max_taps) + 16.  Beyond a filter's span its
+  // taps are zero; the signal buffer is zero padded, so whatever lies there is finite.
+  const int odd = (int)((abs0 + (size_t)lead) & 1);
+  int seg_count = 0;
   for (int s = 0; s < nslot; ++s) {
     const int b = s == 0 ? b_long : b_short;
     fb[s].band = b; fb[s].ntaps = p.ntaps[b];
-    fb[s].seg_off = (p.shift[b] - p.ntaps[b] + 1) - lead;     // >= 0: the short filter starts later and ends earlier
+    const int start = odd + (p.shift[b] - p.ntaps[b] + 1) - lead;   // >= 0
+    fb[s].par = start & 1; fb[s].s_off = start - fb[s].par;
+    fb[s].nq = (fb[s].ntaps + fb[s].par + 14) / 8;                  // 8 nq >= K + 7 + par: every tap of every phase
     fb[s].cap = p.edge_cap[b];
     fb[s].edges = p.edges + (size_t)u * p.edge_stride + (size_t)p.edge_off[b];
+    seg_count = imax(seg_count, fb[s].s_off + T + 8 * fb[s].nq);   // even
   }
-  // seg[i] = s(n0 + lead + i), i < T + nt9 of the long band (beyond a filter's span its taps are zero; the signal
-  // buffer is zero padded, so whatever lies there is finite)
-  const int nt9_long = ((p.ntaps[b_long] + R - 1) / R) * R;
-  const int seg_count = (T + nt9_long + 2) & ~1;
   int tot[2][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}};   // events so far per band and train
 #ifndef WB_EMU
   const int tid = threadIdx.x;
-  for (int s = 0; s < nslot; ++s) {
-    const int nt9 = ((fb[s].ntaps + R - 1) / R) * R;
-    for (int j = tid; j < nt9 + R; j += blockDim.x)
-      hrev[s][j] = j < fb[s].ntaps ? __ldg(&p.taps_rev[p.tap_off[fb[s].band] + j]) : 0.0;
-  }
+  for (int s = 0; s < nslot; ++s)   // 8 leading zeros, the taps, zeros
+    for (int j = tid; j < hcap; j += blockDim.x)
+      hrev[s][j] = j >= 8 && j - 8 < fb[s].ntaps ? __ldg(&p.taps_rev[p.tap_off[fb[s].band] + j - 8]) : 0.0;
   if (tid == 0) {
     mbar_init(&bars[0], 1);
     mbar_init(&bars[1], 1);
@@ -711,7 +724,10 @@ WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
       mbar_wait(&bars[t & 1], (unsigned)((t >> 1) & 1));
       for (int s = 0; s < nslot; ++s, ++item) {
         if (item >= 2) bar_sync_named(3 + (item & 1), 2 * G);    // the event warps are done with this half (item - 2)
-        fe_fir_group(segbuf[t & 1] + (a0 & 1) + fb[s].seg_off, hrev[s], fb[s].ntaps, tid, stbuf[item & 1]);
+        // pointers formed from `smem` itself, not read from the arrays above: so the compiler knows they are shared
+        // and issues LDS, not generic loads
+        fe_fir_warp(smem + (t & 1) * segd + fb[s].s_off, smem + 2 * segd + s * hcap + 8, fb[s].par, fb[s].nq, tid >> 5,
+                    tid & 31, smem + 2 * segd + 2 * hcap + (item & 1) * fe_st_doubles());
         __threadfence_block();
         bar_arrive_named(1 + (item & 1), 2 * G);                 // the item is ready
       }
@@ -750,7 +766,7 @@ WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
         fe_emit_group(v, mask, i0, basew + inc - c, tot[s], fb[s].edges, fb[s].cap);
         tot[s][0] += (int)(all & 0xffffull); tot[s][1] += (int)((all >> 16) & 0xffffull);
         tot[s][2] += (int)((all >> 32) & 0xffffull); tot[s][3] += (int)((all >> 48) & 0xffffull);
-        if (ct == 0) { c0[s] = st[T - 2]; c1[s] = st[T - 1]; }
+        if (ct == 0) { c0[s] = st[pad8(T - 2)]; c1[s] = st[pad8(T - 1)]; }
         __threadfence_block();
         bar_arrive_named(3 + (item & 1), 2 * G);                 // this half may be overwritten (item + 2)
         ++item;
@@ -770,18 +786,17 @@ WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
   }
 #else
   // one emulated thread: both roles, tile after tile, band after band
-  for (int s = 0; s < nslot; ++s) {
-    const int nt9 = ((fb[s].ntaps + R - 1) / R) * R;
-    for (int j = 0; j < nt9 + R; ++j) hrev[s][j] = j < fb[s].ntaps ? p.taps_rev[p.tap_off[fb[s].band] + j] : 0.0;
-  }
+  for (int s = 0; s < nslot; ++s)
+    for (int j = 0; j < hcap; ++j)
+      hrev[s][j] = j >= 8 && j - 8 < fb[s].ntaps ? p.taps_rev[p.tap_off[fb[s].band] + j - 8] : 0.0;
   double c0[2] = {0.0, 0.0}, c1[2] = {0.0, 0.0};
   for (int t = 0; t < n_tiles; ++t) {
     const int n0 = t * T;
     const size_t a0 = abs0 + (size_t)(n0 + lead);
-    for (int i = 0; i < seg_count; ++i) segbuf[0][i] = p.sig[a0 + i];
+    for (int i = 0; i < seg_count; ++i) segbuf[0][i] = p.sig[(a0 & ~(size_t)1) + i];
     for (int s = 0; s < nslot; ++s) {
       double *st = stbuf[s];
-      for (int g = 0; g < G; ++g) fe_fir_group(segbuf[0] + fb[s].seg_off, hrev[s], fb[s].ntaps, g, st);
+      for (int w = 0; w < G / 32; ++w) fe_fir_warp(segbuf[0] + fb[s].s_off, hrev[s] + 8, fb[s].par, fb[s].nq, w, 0, st);
       unsigned long long run = 0ull;
       for (int g = 0; g < G; ++g) {
         double v[WB_FE_R + 2];
@@ -794,7 +809,7 @@ WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
       }
       tot[s][0] += (int)(run & 0xffffull); tot[s][1] += (int)((run >> 16) & 0xffffull);
       tot[s][2] += (int)((run >> 32) & 0xffffull); tot[s][3] += (int)((run >> 48) & 0xffffull);
-      c0[s] = st[T - 2]; c1[s] = st[T - 1];
+      c0[s] = st[pad8(T - 2)]; c1[s] = st[pad8(T - 1)];
     }
   }
   for (int s = 0; s < nslot; ++s) {

@@ -9,8 +9,9 @@
 // memory.  Its filters are short FIRs (<= ~1000 taps), its FFT size is chosen so that the
 // circular convolution never wraps (dio.cpp:592-594, harvest.cpp:1164-1165), and the spectral
 // mirroring quirk is inert for Harvest's long band-pass filters (SURVEY.md App. B5), so
-// the filtered signal IS the linear convolution; it is evaluated directly, register-tiled, FP64
-// FMA bound.  Filter taps are computed on the host with the same libm expressions as the
+// the filtered signal IS the linear convolution; it is evaluated directly: register-tiled FP64 FMA
+// in the streaming sweep, FP64 tensor-core MMA (polyphase, band_fir_events_kernel) for Harvest on
+// decimated input.  Filter taps are computed on the host with the same libm expressions as the
 // reference and uploaded.  Where it matters the ripple the mirroring loop leaves behind IS added
 // (nyquist_bins_kernel, band_sweep_ripple_kernel): DIO always -- it decides what the reference sees in digital
 // silence and under heavy decimation -- and Harvest when its input is not decimated.
@@ -99,17 +100,19 @@ struct SweepParams {
   int *redo_list; int *redo_count;   // (utterance * n_bands + band) pairs for the streaming kernel (history rings)
 };
 
-// band_fir_events_kernel: 9 outputs per thread, so that consecutive threads walk shared memory with a stride of 9
-// doubles -- conflict free WITHOUT padding, which lets the input segment arrive as one TMA bulk copy.  128 filter
-// threads -> tiles of 1152 outputs; two input segments (TMA double buffer) and two output tiles (filter / event warps).
-#define WB_FE_R 9
-WB_HD inline int fe_seg_doubles(int max_taps) {   // one input segment: tile + filter span + slack, even
-  return (WB_FE_R * 128 + ((max_taps + WB_FE_R - 1) / WB_FE_R) * WB_FE_R + WB_FE_R + 8) & ~1;
-}
+// band_fir_events_kernel: tiles of 1024 outputs = 8 outputs per event thread x 128 = 64 FIR rows of 16 outputs
+// (m16n8k8 row tiles), two per filter warp.  Two input segments (TMA double buffer), the taps of two bands with 8
+// leading zeros and zero padding to K + 16 (the polyphase B operand reads h[k - p] for k - p in [-8, K + 8)), two
+// filtered tiles in the pad8 layout (the event threads read 8 outputs each: stride 9 doubles, conflict free).
+#define WB_FE_R 8
+#define WB_FE_TILE (WB_FE_R * 128)
+WB_HD inline int fe_kpad(int ntaps) { return (ntaps + 8 + 7) / 8 * 8; }   // >= 8 ceil((K + 1 + 7) / 8), see fe_fir_warp
+WB_HD inline int fe_seg_doubles(int max_taps) { return WB_FE_TILE + fe_kpad(max_taps) + 16; }    // even
+WB_HD inline int fe_hrev_doubles(int max_taps) { return fe_kpad(max_taps) + 16; }
+WB_HD inline int fe_st_doubles() { return WB_FE_TILE + (WB_FE_TILE >> 3) + 8; }
 WB_HD inline size_t fe_smem_bytes(int max_taps) {
   // two segments, the taps of two bands, two filtered tiles, 2 x 4 warp totals, two mbarriers
-  return (size_t)(2 * fe_seg_doubles(max_taps) + 2 * (((max_taps + WB_FE_R - 1) / WB_FE_R) * WB_FE_R + WB_FE_R) +
-                  2 * (WB_FE_R * 128 + 2) + 8 + 2 + 6) * 8;
+  return (size_t)(2 * fe_seg_doubles(max_taps) + 2 * fe_hrev_doubles(max_taps) + 2 * fe_st_doubles() + 8 + 2 + 6) * 8;
 }
 
 WB_HD inline size_t sweep_smem_bytes(int max_taps) {
