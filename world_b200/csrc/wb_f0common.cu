@@ -1,6 +1,7 @@
 // wb_f0common.cu -- kernels shared by DIO and Harvest (see wb_f0common.cuh for the design notes).
 #include "wb_internal.h"
 #include "wb_f0common.cuh"
+#include "wb_mma.cuh"
 #include <stdlib.h>
 
 namespace wb {
@@ -507,17 +508,6 @@ WB_DEV void mbar_wait(unsigned long long *bar, unsigned parity) {
 #ifndef WB_EMU
 WB_DEV void bar_sync_named(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 WB_DEV void bar_arrive_named(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-#endif
-
-#ifndef WB_EMU
-// D = A B + D, one m16n8k8 FP64 tensor-core MMA (DMMA).  Fragments of lane (g, t) = (lane / 4, lane % 4): a0 / a1 =
-// A[g][t] / A[g + 8][t], a2 / a3 = A[g][t + 4] / A[g + 8][t + 4]; b0 / b1 = B[t][g] / B[t + 4][g]; d0, d1 = D[g][2t],
-// D[g][2t + 1]; d2, d3 = D[g + 8][2t], D[g + 8][2t + 1].
-WB_DEV void mma_f64_16x8x8(double (&d)[4], double a0, double a1, double a2, double a3, double b0, double b1) {
-  asm("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
-      : "d"(a0), "d"(a1), "d"(a2), "d"(a3), "d"(b0), "d"(b1));
-}
 #endif
 
 // Polyphase FIR of filter warp w on the FP64 tensor cores: outputs y[m] = sum_j h[j] s[m + par + j] of the tile.
