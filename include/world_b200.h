@@ -100,6 +100,13 @@ int world_b200_dio_batch(WorldB200 *ctx, const double *x, int n_utts, int x_stri
 int world_b200_harvest_batch(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
                              const int *x_lengths, int fs, const HarvestOption *option,
                              double *time_axis, double *f0, int f0_stride);
+/* The same with one option per utterance: harvest_options is a HOST array of n_utts.  f0_floor / f0_ceil may differ
+ * between utterances (a speaker's or singer's own range); frame_period must be the same for all (else EINVAL).  Each
+ * row equals what world_b200_harvest_batch gives that utterance with its own option.  A range the on-chip kernels
+ * cannot serve is EINVAL, and world_b200_last_error() names the first such utterance. */
+int world_b200_harvest_batch_options(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
+                                     const int *x_lengths, int fs, const HarvestOption *harvest_options,
+                                     double *time_axis, double *f0, int f0_stride);
 /* StoneMask() over a batch (stonemask.h:27). refined_f0 may alias f0. */
 int world_b200_stonemask_batch(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
                                const int *x_lengths, int fs, const double *time_axis,
@@ -189,6 +196,14 @@ int world_b200_analyze_batch(WorldB200 *ctx, const double *x, int n_utts, int x_
                              const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
                              double *time_axis, double *f0, int f0_stride, double *spectrogram,
                              double *aperiodicity);
+/* The same chain with one Harvest option per utterance (harvest_options: HOST array of n_utts, see
+ * world_b200_harvest_batch_options; the slices split it with the utterances).  option->f0_method must be
+ * WORLD_B200_F0_HARVEST and every harvest_options[u].frame_period must equal option->harvest.frame_period (else
+ * EINVAL); option->harvest's floor and ceiling are not used.  The *_options variants below follow the same rules. */
+int world_b200_analyze_batch_options(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
+                                     const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                     const HarvestOption *harvest_options, double *time_axis, double *f0,
+                                     int f0_stride, double *spectrogram, double *aperiodicity);
 
 /* ---- multi-GPU: one context per GPU (one process or thread each), utterances sharded over ranks --------------
  * There is no exchange inside the analysis; the one collective reassembles the output arrays on every rank
@@ -215,6 +230,14 @@ int world_b200_analyze_batch_allgather(WorldB200 *ctx, const double *x, int n_ut
                                        const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
                                        double *time_axis_full, double *f0_full, int f0_stride,
                                        double *spectrogram_full, double *aperiodicity_full);
+/* ... with one Harvest option per utterance of THIS rank's shard (harvest_options: HOST array of n_utts).  The ranges
+ * may differ between ranks; n_utts, strides, fs and option must still be the same on every rank. */
+int world_b200_analyze_batch_allgather_options(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
+                                               const int *x_lengths, int fs,
+                                               const WorldB200AnalysisOption *option,
+                                               const HarvestOption *harvest_options, double *time_axis_full,
+                                               double *f0_full, int f0_stride, double *spectrogram_full,
+                                               double *aperiodicity_full);
 
 /* {Dio+StoneMask | Harvest} -> CheapTrick -> D4C for n_utts host waveforms; outputs are host
  * arrays laid out as described above.  Input upload, compute and result download are pipelined
@@ -224,6 +247,11 @@ int world_b200_analyze_host(WorldB200 *ctx, const double *x, int n_utts, int x_s
                             const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
                             double *time_axis, double *f0, int f0_stride, double *spectrogram,
                             double *aperiodicity);
+/* ... with one Harvest option per utterance (HOST array of n_utts; the chunks split it). */
+int world_b200_analyze_host_options(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
+                                    const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                    const HarvestOption *harvest_options, double *time_axis, double *f0,
+                                    int f0_stride, double *spectrogram, double *aperiodicity);
 
 /* The same chain with the ingest and the codec fused in on the device: x holds samples of `nbit`
  * bits (0 = doubles as above; 8/16/24/32 = little-endian PCM as in a WAV data chunk), and the

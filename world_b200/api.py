@@ -68,6 +68,8 @@ ABI = {
     "world_b200_profile_report": (C.c_int, [_P, C.c_char_p, C.c_ulonglong]),
     "world_b200_dio_batch": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(DioOption), _P, _P, C.c_int]),
     "world_b200_harvest_batch": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(HarvestOption), _P, _P, C.c_int]),
+    "world_b200_harvest_batch_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(HarvestOption), _P,
+                                                   _P, C.c_int]),
     "world_b200_stonemask_batch": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, _P, _P, _IP, C.c_int, _P]),
     "world_b200_cheaptrick_batch": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, _P, _P, _IP, C.c_int,
                                               C.POINTER(CheapTrickOption), _P]),
@@ -86,6 +88,13 @@ ABI = {
                                            _P, _P, C.c_int, _P, _P]),
     "world_b200_analyze_batch_allgather": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(AnalysisOption),
                                                      _P, _P, C.c_int, _P, _P]),
+    "world_b200_analyze_host_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(AnalysisOption),
+                                                  C.POINTER(HarvestOption), _P, _P, C.c_int, _P, _P]),
+    "world_b200_analyze_batch_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(AnalysisOption),
+                                                   C.POINTER(HarvestOption), _P, _P, C.c_int, _P, _P]),
+    "world_b200_analyze_batch_allgather_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int,
+                                                             C.POINTER(AnalysisOption), C.POINTER(HarvestOption), _P,
+                                                             _P, C.c_int, _P, _P]),
     "world_b200_comm_unique_id": (C.c_int, [_P, C.c_int]),
     "world_b200_comm_init": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int]),
     "world_b200_comm_destroy": (C.c_int, [_P]),
@@ -169,6 +178,19 @@ def _ptr(a):
     if hasattr(a, "data_ptr"):
         return a.data_ptr()
     return a.ctypes.data
+
+
+def _harvest_options(options, n):
+    """A list of n HarvestOption (one per utterance) as a ctypes array; None for a single option or None."""
+    if options is None or isinstance(options, HarvestOption):
+        return None
+    options = list(options)
+    if len(options) != n:
+        raise ValueError(f"{len(options)} Harvest options for {n} utterances")
+    arr = (HarvestOption * n)()
+    for i, o in enumerate(options):
+        arr[i].f0_floor, arr[i].f0_ceil, arr[i].frame_period = o.f0_floor, o.f0_ceil, o.frame_period
+    return arr
 
 
 def _int_array(v, n):
@@ -321,16 +343,24 @@ class World:
                                                   _ptr(t), _ptr(f0), f_stride))
         return t, f0, fl
 
-    def harvest(self, x, fs, option: HarvestOption | None = None, x_lengths=None):
-        option = option or self.harvest_option()
+    def harvest(self, x, fs, option=None, x_lengths=None):
+        """option: one HarvestOption for the batch, or a list of one per utterance (f0_floor / f0_ceil may differ,
+        frame_period may not)."""
         n, stride = x.shape
-        f_stride, fl = self._f0_stride(fs, x, x_lengths, option.frame_period)
+        per_utt = _harvest_options(option, n)
+        option = option or self.harvest_option()
+        frame_period = per_utt[0].frame_period if per_utt is not None and n else getattr(option, "frame_period", 5.0)
+        f_stride, fl = self._f0_stride(fs, x, x_lengths, frame_period)
         t = self._zeros(x, (n, f_stride))
         f0 = self._zeros(x, (n, f_stride))
         xl, keep = _int_array(x_lengths, n)
         self._use_current_stream()
-        self._check(self.lib.world_b200_harvest_batch(self._h, _ptr(x), n, stride, xl, fs, C.byref(option),
-                                                      _ptr(t), _ptr(f0), f_stride))
+        if per_utt is not None:
+            self._check(self.lib.world_b200_harvest_batch_options(self._h, _ptr(x), n, stride, xl, fs, per_utt,
+                                                                  _ptr(t), _ptr(f0), f_stride))
+        else:
+            self._check(self.lib.world_b200_harvest_batch(self._h, _ptr(x), n, stride, xl, fs, C.byref(option),
+                                                          _ptr(t), _ptr(f0), f_stride))
         return t, f0, fl
 
     def stonemask(self, x, fs, time_axis, f0, x_lengths=None, f0_lengths=None):
@@ -417,8 +447,9 @@ class World:
         return o
 
     def analyze_batch(self, x, fs, option: AnalysisOption, x_lengths=None, time_axis=None, f0=None,
-                      spectrogram=None, aperiodicity=None):
-        """Whole chain on DEVICE arrays in one call (two internal streams); returns (t, f0, sp, ap, frame counts)."""
+                      spectrogram=None, aperiodicity=None, harvest_options=None):
+        """Whole chain on DEVICE arrays in one call (two internal streams); returns (t, f0, sp, ap, frame counts).
+        harvest_options: a list of one HarvestOption per utterance (Harvest with a per-utterance F0 range)."""
         n, stride = x.shape
         frame_period = option.dio.frame_period if option.f0_method == F0_DIO_STONEMASK else option.harvest.frame_period
         f_stride, fl = self._f0_stride(fs, x, x_lengths, frame_period)
@@ -432,10 +463,17 @@ class World:
         if aperiodicity is None:
             aperiodicity = self._zeros(x, (n, f_stride, bins))
         xl, keep = _int_array(x_lengths, n)
+        per_utt = _harvest_options(harvest_options, n)
         self._use_current_stream()
-        self._check(self.lib.world_b200_analyze_batch(self._h, _ptr(x), n, stride, xl, fs, C.byref(option),
-                                                      _ptr(time_axis), _ptr(f0), time_axis.shape[1],
-                                                      _ptr(spectrogram), _ptr(aperiodicity)))
+        if per_utt is not None:
+            self._check(self.lib.world_b200_analyze_batch_options(self._h, _ptr(x), n, stride, xl, fs, C.byref(option),
+                                                                  per_utt, _ptr(time_axis), _ptr(f0),
+                                                                  time_axis.shape[1], _ptr(spectrogram),
+                                                                  _ptr(aperiodicity)))
+        else:
+            self._check(self.lib.world_b200_analyze_batch(self._h, _ptr(x), n, stride, xl, fs, C.byref(option),
+                                                          _ptr(time_axis), _ptr(f0), time_axis.shape[1],
+                                                          _ptr(spectrogram), _ptr(aperiodicity)))
         return time_axis, f0, spectrogram, aperiodicity, fl
 
     # -- multi-GPU: one World per GPU / process; the NCCL id travels by the caller's own means -------------------
@@ -463,20 +501,28 @@ class World:
         return full
 
     def analyze_batch_allgather(self, x, fs, option: AnalysisOption, time_axis_full, f0_full, spectrogram_full,
-                                aperiodicity_full, x_lengths=None):
-        """analyze_batch on this rank's shard with every finished slice broadcast into the FULL arrays of all ranks."""
+                                aperiodicity_full, x_lengths=None, harvest_options=None):
+        """analyze_batch on this rank's shard with every finished slice broadcast into the FULL arrays of all ranks.
+        harvest_options: a list of one HarvestOption per utterance of THIS rank's shard."""
         n, stride = x.shape
         xl, keep = _int_array(x_lengths, n)
+        per_utt = _harvest_options(harvest_options, n)
+        outs = (_ptr(time_axis_full), _ptr(f0_full), time_axis_full.shape[1],
+                _ptr(spectrogram_full) if spectrogram_full is not None else None,
+                _ptr(aperiodicity_full) if aperiodicity_full is not None else None)
         self._use_current_stream()
-        self._check(self.lib.world_b200_analyze_batch_allgather(
-            self._h, _ptr(x), n, stride, xl, fs, C.byref(option), _ptr(time_axis_full), _ptr(f0_full),
-            time_axis_full.shape[1], _ptr(spectrogram_full) if spectrogram_full is not None else None,
-            _ptr(aperiodicity_full) if aperiodicity_full is not None else None))
+        if per_utt is not None:
+            self._check(self.lib.world_b200_analyze_batch_allgather_options(
+                self._h, _ptr(x), n, stride, xl, fs, C.byref(option), per_utt, *outs))
+        else:
+            self._check(self.lib.world_b200_analyze_batch_allgather(
+                self._h, _ptr(x), n, stride, xl, fs, C.byref(option), *outs))
 
     def analyze_host(self, x_host, fs, option: AnalysisOption, x_lengths=None, time_axis=None, f0=None,
-                     spectrogram=None, aperiodicity=None, f0_stride=None):
+                     spectrogram=None, aperiodicity=None, f0_stride=None, harvest_options=None):
         """Whole chain on HOST arrays (numpy or pinned torch CPU tensors); outputs are written
-        into the given host arrays (allocated with numpy when None)."""
+        into the given host arrays (allocated with numpy when None).  harvest_options: a list of one
+        HarvestOption per utterance."""
         import numpy as np
         n, stride = x_host.shape
         frame_period = option.dio.frame_period if option.f0_method == F0_DIO_STONEMASK else option.harvest.frame_period
@@ -493,9 +539,15 @@ class World:
         if aperiodicity is None:
             aperiodicity = np.zeros((n, f0_stride, bins))
         xl, keep = _int_array(x_lengths, n)
-        self._check(self.lib.world_b200_analyze_host(self._h, _ptr(x_host), n, stride, xl, fs, C.byref(option),
-                                                     _ptr(time_axis), _ptr(f0), f0_stride, _ptr(spectrogram),
-                                                     _ptr(aperiodicity)))
+        per_utt = _harvest_options(harvest_options, n)
+        if per_utt is not None:
+            self._check(self.lib.world_b200_analyze_host_options(self._h, _ptr(x_host), n, stride, xl, fs,
+                                                                 C.byref(option), per_utt, _ptr(time_axis), _ptr(f0),
+                                                                 f0_stride, _ptr(spectrogram), _ptr(aperiodicity)))
+        else:
+            self._check(self.lib.world_b200_analyze_host(self._h, _ptr(x_host), n, stride, xl, fs, C.byref(option),
+                                                         _ptr(time_axis), _ptr(f0), f0_stride, _ptr(spectrogram),
+                                                         _ptr(aperiodicity)))
         return time_axis, f0, spectrogram, aperiodicity, fl
 
     # -- codec (codec.h) and ingest ----------------------------------------------------------

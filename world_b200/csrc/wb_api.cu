@@ -293,6 +293,24 @@ static int frames_for(int fs, int x_length, double frame_period) {
   return static_cast<int>(1000.0 * x_length / fs / frame_period) + 1;
 }
 
+namespace wb {
+
+// Per-utterance options: one frame_period for the whole batch; with ranges (fs > 0) also every utterance's F0 range
+// against the on-chip limits, up front, so that a chain cut into slices or chunks names the batch's first bad utterance.
+int check_harvest_options(Ctx *c, const HarvestOption *opts, int n, double frame_period, int fs) {
+  for (int u = 0; u < n; ++u)
+    if (!(opts[u].frame_period == frame_period)) {
+      c->last_error = "harvest options: frame_period differs from the batch's (utterance " + std::to_string(u) + ")";
+      return WORLD_B200_EINVAL;
+    }
+  if (fs <= 0 || n <= 0) return 0;
+  std::vector<HarvestParams> p(n);
+  for (int u = 0; u < n; ++u) p[u] = {opts[u].f0_floor, opts[u].f0_ceil, opts[u].frame_period};
+  return harvest_check_options(c, fs, p.data(), n);
+}
+
+}  // namespace wb
+
 extern "C" {
 
 int world_b200_frames(int fs, int x_length, double frame_period) {
@@ -530,10 +548,15 @@ int world_b200_dio_batch(WorldB200 *h, const double *x, int n, int x_stride, con
   return dio_run(&h->c, b, p, time_axis, f0);
 }
 
-int world_b200_harvest_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
-                             int fs, const HarvestOption *opt, double *time_axis, double *f0, int f0_stride) {
+// opt: one option for every utterance, or (per_utt) an array of n
+static int harvest_batch_impl(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
+                              const HarvestOption *opt, bool per_utt, double *time_axis, double *f0, int f0_stride) {
   if (!h || !x || !time_axis || !f0 || !opt || n < 0 || fs <= 0) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
+  if (per_utt && n > 0) {
+    const int rc = check_harvest_options(&h->c, opt, n, opt[0].frame_period, 0);   // harvest_run checks the ranges
+    if (rc) return rc;
+  }
   std::vector<int> fl;
   int rc = f0_lengths_from_x(n, x_stride, x_lengths, fs, opt->frame_period, f0_stride, &fl, &h->c.last_error);
   if (rc) return rc;
@@ -545,8 +568,20 @@ int world_b200_harvest_batch(WorldB200 *h, const double *x, int n, int x_stride,
   for (int i = 0; i < n; ++i) l1[i] = frames_for(fs, x_lengths ? x_lengths[i] : x_stride, 1.0);
   b.l1_host = l1.data();
   b.x_len_host = x_lengths;
-  HarvestParams p = {opt->f0_floor, opt->f0_ceil, opt->frame_period};
-  return harvest_run(&h->c, b, p, time_axis, f0);
+  std::vector<HarvestParams> p(per_utt ? (n > 0 ? n : 1) : 1);
+  for (size_t u = 0; u < p.size(); ++u) p[u] = {opt[u].f0_floor, opt[u].f0_ceil, opt[u].frame_period};
+  return harvest_run(&h->c, b, p.data(), per_utt, time_axis, f0);
+}
+
+int world_b200_harvest_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
+                             int fs, const HarvestOption *opt, double *time_axis, double *f0, int f0_stride) {
+  return harvest_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, false, time_axis, f0, f0_stride);
+}
+
+int world_b200_harvest_batch_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
+                                     const HarvestOption *harvest_options, double *time_axis, double *f0,
+                                     int f0_stride) {
+  return harvest_batch_impl(h, x, n, x_stride, x_lengths, fs, harvest_options, true, time_axis, f0, f0_stride);
 }
 
 // The whole chain on device arrays, cut into utterance slices that alternate between two lanes (sibling contexts
@@ -557,12 +592,22 @@ int world_b200_harvest_batch(WorldB200 *h, const double *x, int n, int x_stride,
 // gather = false: time_axis / f0 / spectrogram / aperiodicity hold this call's n utterances.
 // gather = true (multi-GPU): they are the FULL arrays of n_ranks * n utterances; this rank computes into block `rank`
 // and every finished slice is broadcast to the other ranks on the communication stream while the next one is computed.
+// harvest_options: nullptr, or one HarvestOption per utterance (f0_method HARVEST, frame_period = opt->harvest's)
 static int analyze_batch_impl(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
-                              const WorldB200AnalysisOption *opt, double *time_axis, double *f0, int f0_stride,
+                              const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
+                              double *time_axis, double *f0, int f0_stride,
                               double *spectrogram, double *aperiodicity, bool gather) {
   if (!h || !x || !opt || !time_axis || !f0 || n < 0 || fs <= 0 || x_stride <= 0 || f0_stride <= 0) return WORLD_B200_EINVAL;
   if ((spectrogram || aperiodicity) && opt->cheaptrick.fft_size < 16) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
+  if (harvest_options) {
+    if (opt->f0_method != WORLD_B200_F0_HARVEST) {
+      h->c.last_error = "analyze_batch: per-utterance Harvest options need f0_method == WORLD_B200_F0_HARVEST";
+      return WORLD_B200_EINVAL;
+    }
+    const int rc = check_harvest_options(&h->c, harvest_options, n, opt->harvest.frame_period, fs);
+    if (rc) return rc;
+  }
   if (n == 0) return 0;
   size_t my_block = 0;
   if (gather) {
@@ -650,7 +695,8 @@ static int analyze_batch_impl(WorldB200 *h, const double *x, int n, int x_stride
     const int *xl = x_lengths ? x_lengths + u0 : nullptr;
     double *ts = time_axis + (size_t)u0 * f0_stride, *fs_ = f0 + (size_t)u0 * f0_stride;
     if (opt->f0_method == WORLD_B200_F0_HARVEST) {
-      rc = world_b200_harvest_batch(L, xs, m, x_stride, xl, fs, &opt->harvest, ts, fs_, f0_stride);
+      rc = harvest_options ? world_b200_harvest_batch_options(L, xs, m, x_stride, xl, fs, harvest_options + u0, ts, fs_, f0_stride)
+                           : world_b200_harvest_batch(L, xs, m, x_stride, xl, fs, &opt->harvest, ts, fs_, f0_stride);
     } else {
       rc = world_b200_dio_batch(L, xs, m, x_stride, xl, fs, &opt->dio, ts, fs_, f0_stride);
       if (!rc) rc = world_b200_stonemask_batch(L, xs, m, x_stride, xl, fs, ts, fs_, fl.data() + u0, f0_stride, fs_);
@@ -697,7 +743,17 @@ static int analyze_batch_impl(WorldB200 *h, const double *x, int n, int x_stride
 int world_b200_analyze_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
                              const WorldB200AnalysisOption *opt, double *time_axis, double *f0, int f0_stride,
                              double *spectrogram, double *aperiodicity) {
-  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, time_axis, f0, f0_stride, spectrogram, aperiodicity, false);
+  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, nullptr, time_axis, f0, f0_stride, spectrogram,
+                            aperiodicity, false);
+}
+
+int world_b200_analyze_batch_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
+                                     const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
+                                     double *time_axis, double *f0, int f0_stride, double *spectrogram,
+                                     double *aperiodicity) {
+  if (!harvest_options) return WORLD_B200_EINVAL;
+  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, harvest_options, time_axis, f0, f0_stride,
+                            spectrogram, aperiodicity, false);
 }
 
 // ---- multi-GPU (SURVEY.md 8e): utterances sharded over ranks, outputs reassembled on every rank by NCCL
@@ -751,8 +807,18 @@ int world_b200_allgather_rows(WorldB200 *h, double *full, unsigned long long row
 int world_b200_analyze_batch_allgather(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
                                        const WorldB200AnalysisOption *opt, double *time_axis_full, double *f0_full,
                                        int f0_stride, double *spectrogram_full, double *aperiodicity_full) {
-  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, time_axis_full, f0_full, f0_stride, spectrogram_full,
-                            aperiodicity_full, true);
+  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, nullptr, time_axis_full, f0_full, f0_stride,
+                            spectrogram_full, aperiodicity_full, true);
+}
+
+int world_b200_analyze_batch_allgather_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
+                                               int fs, const WorldB200AnalysisOption *opt,
+                                               const HarvestOption *harvest_options, double *time_axis_full,
+                                               double *f0_full, int f0_stride, double *spectrogram_full,
+                                               double *aperiodicity_full) {
+  if (!harvest_options) return WORLD_B200_EINVAL;
+  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, harvest_options, time_axis_full, f0_full, f0_stride,
+                            spectrogram_full, aperiodicity_full, true);
 }
 
 // Per-kernel timing: enable, run, then fetch a JSON object {"kernel": {"launches": n, "ms": t}, ...}

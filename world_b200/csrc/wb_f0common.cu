@@ -130,14 +130,15 @@ WB_DEV unsigned long long scan_packed(unsigned long long *c, int G, unsigned lon
 }
 
 // One frame of one band from the four interpolated values (dio.cpp:441-465, 562-566 / harvest.cpp:240-254)
-WB_DEV void sweep_store_candidate(const SweepParams &p, double v0, double v1, double v2, double v3, int i, double bf,
-                                  double *cand, double *score) {
+WB_DEV void sweep_store_candidate(const SweepParams &p, int grp, double v0, double v1, double v2, double v3, int i,
+                                  double bf, double *cand, double *score) {
   double c = (v0 + v1 + v2 + v3) / 4.0, sc = 0.0;
+  const double f0_floor = grp < 0 ? p.f0_floor : p.grp_floor[grp], f0_ceil = grp < 0 ? p.f0_ceil : p.grp_ceil[grp];
   if (p.mode == 0) {
     sc = sqrt(((v0 - c) * (v0 - c) + (v1 - c) * (v1 - c) + (v2 - c) * (v2 - c) + (v3 - c) * (v3 - c)) / 3.0);
-    if (c > bf || c < bf / 2.0 || c > p.f0_ceil || c < p.f0_floor) { c = 0.0; sc = 100000.0; }
+    if (c > bf || c < bf / 2.0 || c > f0_ceil || c < f0_floor) { c = 0.0; sc = 100000.0; }
   } else {
-    if (c > bf * 1.1 || c < bf * 0.9 || c > p.f0_ceil || c < p.f0_floor) c = 0.0;
+    if (c > bf * 1.1 || c < bf * 0.9 || c > f0_ceil || c < f0_floor) c = 0.0;
   }
   cand[i] = c;
   if (score) score[i] = sc / (c + kTiny);  // dio.cpp:562-566
@@ -147,7 +148,7 @@ WB_DEV void sweep_store_candidate(const SweepParams &p, double v0, double v1, do
 // (indices lo_j .. ni-1) are binned by the first frame they precede-or-equal; a packed block scan
 // turns the bins into per-frame interval counts, i.e. interp1's segment index, without any search.
 // lo_j advances past the intervals consumed.  Block-cooperative; ends with a barrier.
-WB_DEV void finalize_frames(const SweepParams &p, const Trains &T, int *lo_j, const int *ni, int f_begin, int f_end,
+WB_DEV void finalize_frames(const SweepParams &p, int grp, const Trains &T, int *lo_j, const int *ni, int f_begin, int f_end,
                             unsigned long long *marks, unsigned long long *orig, unsigned long long *scan_tmp,
                             double bf, double *cand, double *score) {
   const int tid = WB_TID, nth = WB_NTH;
@@ -172,7 +173,7 @@ WB_DEV void finalize_frames(const SweepParams &p, const Trains &T, int *lo_j, co
       const double v1 = train_value(T, 1, lo_j[1] + (int)((inc >> 16) & 0xffffull), ni[1], t);
       const double v2 = train_value(T, 2, lo_j[2] + (int)((inc >> 32) & 0xffffull), ni[2], t);
       const double v3 = train_value(T, 3, lo_j[3] + (int)((inc >> 48) & 0xffffull), ni[3], t);
-      sweep_store_candidate(p, v0, v1, v2, v3, c0 + i, bf, cand, score);
+      sweep_store_candidate(p, grp, v0, v1, v2, v3, c0 + i, bf, cand, score);
     }
     lo_j[0] += (int)(all & 0xffffull); lo_j[1] += (int)((all >> 16) & 0xffffull);
     lo_j[2] += (int)((all >> 32) & 0xffffull); lo_j[3] += (int)((all >> 48) & 0xffffull);
@@ -221,7 +222,9 @@ WB_DEV void sweep_body(const SweepParams &p, const int b, const int u) {
   WB_DYN_SMEM(double, smem);
   const int tid = WB_TID, nth = WB_NTH;
   const int T = WB_SWEEP_T, R = WB_SWEEP_R, G = T / R;
-  const int ntaps = p.ntaps[b], shift = p.shift[b];
+  const UttBands ub = utt_bands(p, u);
+  const int bt = ub.band0 + b;   // the band's row of the tables
+  const int ntaps = p.ntaps[bt], shift = p.shift[bt];
   const int seg_len = T + ntaps - 1;
   const int seg_cap = T + p.max_taps + 16;
   double *seg = smem;                                   // padded: pad8(seg_cap)
@@ -234,9 +237,9 @@ WB_DEV void sweep_body(const SweepParams &p, const int b, const int u) {
 
   const int ylen = p.y_len[u];
   const double *sig = p.sig + (size_t)u * p.sig_stride + p.sig_origin;
-  double *edges = p.edges + (size_t)u * p.edge_stride + (size_t)p.edge_off[b];
-  const int cap = p.edge_cap[b];
-  for (int j = tid; j < ntaps; j += nth) hrev[j] = __ldg(&p.taps_rev[p.tap_off[b] + j]);
+  double *edges = p.edges + (size_t)u * p.edge_stride + (size_t)p.edge_off[bt];
+  const int cap = p.edge_cap[bt];
+  for (int j = tid; j < ntaps; j += nth) hrev[j] = __ldg(&p.taps_rev[p.tap_off[bt] + j]);
   for (int j = ntaps + tid; j < ntaps + 8; j += nth) hrev[j] = 0.0;
   if (tid == 0) { st[0] = 0.0; st[1] = 0.0; }
   Trains tr;
@@ -249,7 +252,7 @@ WB_DEV void sweep_body(const SweepParams &p, const int b, const int u) {
   const int nf = p.n_frames[u];
   double *cand = p.cand + ((size_t)u * p.n_bands + b) * p.frame_stride;
   double *score = p.score ? p.score + ((size_t)u * p.n_bands + b) * p.frame_stride : nullptr;
-  const double bf = p.boundary[b];
+  const double bf = p.boundary[bt];
   WB_SYNC();
   // DIO: this band's window at bins N/2 - 1 and N/2, combined with the utterance's spectrum there into the
   // amplitudes of the ripple  (-1)^m (2 Re(dq e^{-j 2 pi m / N}) + dn) / N  at filtered-signal index m - shift
@@ -420,7 +423,7 @@ WB_DEV void sweep_body(const SweepParams &p, const int b, const int u) {
       int i_safe = first_frame_at_or_after(t_safe, p.frame_period);  // frames below have t_i < t_safe
       if (i_safe > nf) i_safe = nf;
       if (i_safe > next_frame) {
-        finalize_frames(p, tr, lo_j, ni, next_frame, i_safe, marks, orig, cnt + G + 4, bf, cand, score);
+        finalize_frames(p, ub.grp, tr, lo_j, ni, next_frame, i_safe, marks, orig, cnt + G + 4, bf, cand, score);
         next_frame = i_safe;
       }
     }
@@ -433,7 +436,7 @@ WB_DEV void sweep_body(const SweepParams &p, const int b, const int u) {
     if (n_int - 2 <= 0) ok = false;                 // CheckEvent(n - 2), dio.cpp:475-484
   }
   if (ok) {
-    finalize_frames(p, tr, lo_j, ni, next_frame, nf, marks, orig, cnt + G + 4, bf, cand, score);
+    finalize_frames(p, ub.grp, tr, lo_j, ni, next_frame, nf, marks, orig, cnt + G + 4, bf, cand, score);
   } else {
     for (int i = tid; i < nf; i += nth) {
       cand[i] = 0.0;
@@ -442,8 +445,19 @@ WB_DEV void sweep_body(const SweepParams &p, const int b, const int u) {
   }
 }
 
-WB_KERNEL(WB_SWEEP_THREADS, 3) band_sweep_kernel(SweepParams p) { sweep_body<0>(p, blockIdx.x, blockIdx.y); }          // Harvest on decimated input
-WB_KERNEL(WB_SWEEP_THREADS, 3) band_sweep_ripple_kernel(SweepParams p) { sweep_body<1>(p, blockIdx.x, blockIdx.y); }   // DIO; Harvest at ratio 1
+// (band, utterance) of this block: grid (band, utterance), or flat over the utterances' own bands (SweepParams::ugrp)
+WB_DEV int sweep_block(const SweepParams &p, int *u) {
+  if (!p.ugrp) { *u = blockIdx.y; return blockIdx.x; }
+  return flat_block(p.blk0_band, p.n_utts, blockIdx.x, u);
+}
+template <int kRipple>
+WB_DEV void sweep_grid_body(const SweepParams &p) {
+  int u;
+  const int b = sweep_block(p, &u);
+  sweep_body<kRipple>(p, b, u);
+}
+WB_KERNEL(WB_SWEEP_THREADS, 3) band_sweep_kernel(SweepParams p) { sweep_grid_body<0>(p); }          // Harvest on decimated input
+WB_KERNEL(WB_SWEEP_THREADS, 3) band_sweep_ripple_kernel(SweepParams p) { sweep_grid_body<1>(p); }   // DIO; Harvest at ratio 1
 // the same streaming sweep over a device list of (utterance, band) pairs: bands whose complete edge lists did not fit
 // (band_fir_events_kernel), i.e. far more zero crossings than the band frequency allows for -- usually none
 WB_KERNEL(WB_SWEEP_THREADS, 3) band_sweep_list_kernel(SweepParams p) {
@@ -643,7 +657,7 @@ WB_DEV void fe_emit_group(const double (&v)[WB_FE_R + 2], unsigned long long mas
 // so a CTA with one band is either waiting for its filter warps or for its event warps; the pair sums are within
 // 2x of each other and sit on the filter side.  Both bands read the same input segment (the long band's).
 struct FeBand {
-  int ntaps, cap, band;
+  int ntaps, cap, band;   // band: the utterance's own index (its row of the band tables: + UttBands::band0)
   int s_off, par, nq;   // the band's FIR input starts at seg[s_off + par], s_off even; k-steps of fe_fir_warp
   double *edges;
 };
@@ -652,7 +666,9 @@ struct FeBand {
 // 1024 x 10 s step; two CTAs per SM with 102 registers and no spills took 179 ms.
 WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
   WB_DYN_SMEM(double, smem);
-  const int pr = blockIdx.x, u = blockIdx.y;
+  int u = blockIdx.y, pr = blockIdx.x;
+  if (p.ugrp) pr = flat_block(p.blk0_pair, p.n_utts, blockIdx.x, &u);
+  const UttBands ub = utt_bands(p, u);
   const int T = WB_FE_TILE, R = WB_FE_R, G = WB_FE_GROUP;
   const int segd = fe_seg_doubles(p.max_taps), hcap = fe_hrev_doubles(p.max_taps);
   double *segbuf[2] = {smem, smem + segd};
@@ -663,10 +679,10 @@ WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
   const int ylen = p.y_len[u];
   const size_t abs0 = (size_t)u * p.sig_stride + p.sig_origin;   // index of s(0) in p.sig
   const int n_tiles = (ylen + 2 + T - 1) / T;
-  const int b_long = pr, b_short = p.n_bands - 1 - pr;
+  const int b_long = pr, b_short = ub.nb - 1 - pr;   // the utterance's own band list, tables at ub.band0 + b
   const int nslot = b_short > b_long ? 2 : 1;    // the middle band of an odd count is alone
   FeBand fb[2];
-  const int lead = p.shift[b_long] - p.ntaps[b_long] + 1;     // segment of tile t starts at s(t T + lead)
+  const int lead = p.shift[ub.band0 + b_long] - p.ntaps[ub.band0 + b_long] + 1;     // segment of tile t starts at s(t T + lead)
   // seg[i] = s(n0 + lead - odd + i), odd = (abs0 + lead) & 1: the bulk copy starts at an even index of p.sig (T is
   // even, so the same for every tile).  A band reads seg[s_off .. s_off + T + 8 nq): the short filter starts later and
   // ends earlier than the long one, so that lies inside segd = T + fe_kpad(max_taps) + 16.  Beyond a filter's span its
@@ -675,12 +691,13 @@ WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
   int seg_count = 0;
   for (int s = 0; s < nslot; ++s) {
     const int b = s == 0 ? b_long : b_short;
-    fb[s].band = b; fb[s].ntaps = p.ntaps[b];
-    const int start = odd + (p.shift[b] - p.ntaps[b] + 1) - lead;   // >= 0
+    const int bt = ub.band0 + b;
+    fb[s].band = b; fb[s].ntaps = p.ntaps[bt];
+    const int start = odd + (p.shift[bt] - p.ntaps[bt] + 1) - lead;   // >= 0
     fb[s].par = start & 1; fb[s].s_off = start - fb[s].par;
     fb[s].nq = (fb[s].ntaps + fb[s].par + 14) / 8;                  // 8 nq >= K + 7 + par: every tap of every phase
-    fb[s].cap = p.edge_cap[b];
-    fb[s].edges = p.edges + (size_t)u * p.edge_stride + (size_t)p.edge_off[b];
+    fb[s].cap = p.edge_cap[bt];
+    fb[s].edges = p.edges + (size_t)u * p.edge_stride + (size_t)p.edge_off[bt];
     seg_count = imax(seg_count, fb[s].s_off + T + 8 * fb[s].nq);   // even
   }
   int tot[2][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}};   // events so far per band and train
@@ -688,7 +705,7 @@ WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
   const int tid = threadIdx.x;
   for (int s = 0; s < nslot; ++s)   // 8 leading zeros, the taps, zeros
     for (int j = tid; j < hcap; j += blockDim.x)
-      hrev[s][j] = j >= 8 && j - 8 < fb[s].ntaps ? __ldg(&p.taps_rev[p.tap_off[fb[s].band] + j - 8]) : 0.0;
+      hrev[s][j] = j >= 8 && j - 8 < fb[s].ntaps ? __ldg(&p.taps_rev[p.tap_off[ub.band0 + fb[s].band] + j - 8]) : 0.0;
   if (tid == 0) {
     mbar_init(&bars[0], 1);
     mbar_init(&bars[1], 1);
@@ -778,7 +795,7 @@ WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
   // one emulated thread: both roles, tile after tile, band after band
   for (int s = 0; s < nslot; ++s)
     for (int j = 0; j < hcap; ++j)
-      hrev[s][j] = j >= 8 && j - 8 < fb[s].ntaps ? p.taps_rev[p.tap_off[fb[s].band] + j - 8] : 0.0;
+      hrev[s][j] = j >= 8 && j - 8 < fb[s].ntaps ? p.taps_rev[p.tap_off[ub.band0 + fb[s].band] + j - 8] : 0.0;
   double c0[2] = {0.0, 0.0}, c1[2] = {0.0, 0.0};
   for (int t = 0; t < n_tiles; ++t) {
     const int n0 = t * T;
@@ -847,15 +864,17 @@ WB_KERNEL(256, 4) band_interp_kernel(SweepParams p) {
   WB_SHARED unsigned long long orig[WB_IP_F];
   WB_SHARED int more_flag[2];   // "the last interval of a window still starts inside the round", per iteration parity
   const int tid = WB_TID, nth = WB_NTH;
-  const int b = blockIdx.x, u = blockIdx.y;
+  int u;
+  const int b = sweep_block(p, &u);
+  const UttBands ub = utt_bands(p, u);
   const int *ec = p.ev_count + ((size_t)u * p.n_bands + b) * 4;
   if (ec[0] < 0) return;   // lists overflowed: the streaming kernel redoes this band
   const int nf = p.n_frames[u];
   double *cand = p.cand + ((size_t)u * p.n_bands + b) * p.frame_stride;
   double *score = p.score ? p.score + ((size_t)u * p.n_bands + b) * p.frame_stride : nullptr;
-  const double bf = p.boundary[b];
-  const int cap = p.edge_cap[b];
-  const double *edges = p.edges + (size_t)u * p.edge_stride + (size_t)p.edge_off[b];
+  const double bf = p.boundary[ub.band0 + b];
+  const int cap = p.edge_cap[ub.band0 + b];
+  const double *edges = p.edges + (size_t)u * p.edge_stride + (size_t)p.edge_off[ub.band0 + b];
   IpTrain tr[4];
   bool ok = true;
   for (int q = 0; q < 4; ++q) {
@@ -942,7 +961,7 @@ WB_KERNEL(256, 4) band_interp_kernel(SweepParams p) {
         const double s = (t - x0) / (x1 - x0);
         v[q] = y0 + s * (y1 - y0);
       }
-      sweep_store_candidate(p, v[0], v[1], v[2], v[3], i, bf, cand, score);
+      sweep_store_candidate(p, ub.grp, v[0], v[1], v[2], v[3], i, bf, cand, score);
     }
     cursor[0] += (int)(all & 0xffffull); cursor[1] += (int)((all >> 16) & 0xffffull);
     cursor[2] += (int)((all >> 32) & 0xffffull); cursor[3] += (int)((all >> 48) & 0xffffull);
@@ -1023,6 +1042,10 @@ void launch_nyquist_bins(Ctx *ctx, const NyquistParams &p, unsigned n_utts) {
   WB_LAUNCH_COOP(nyquist_bins_kernel, dim3(n_utts), 256, 0, ctx->stream, p);
 }
 
+static dim3 sweep_grid(const SweepParams &p, unsigned n_utts) {
+  return p.ugrp ? dim3((unsigned)p.n_blk_band) : dim3((unsigned)p.n_bands, n_utts);
+}
+
 void launch_band_sweep(Ctx *ctx, const SweepParams &p_in, unsigned n_utts) {
   SweepParams p = p_in;
   p.debug_skip = 0;
@@ -1032,12 +1055,12 @@ void launch_band_sweep(Ctx *ctx, const SweepParams &p_in, unsigned n_utts) {
 #ifndef WB_EMU
     cudaFuncSetAttribute(band_sweep_ripple_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 #endif
-    WB_LAUNCH_COOP(band_sweep_ripple_kernel, dim3((unsigned)p.n_bands, n_utts), WB_SWEEP_THREADS, smem, ctx->stream, p);
+    WB_LAUNCH_COOP(band_sweep_ripple_kernel, sweep_grid(p, n_utts), WB_SWEEP_THREADS, smem, ctx->stream, p);
   } else {
 #ifndef WB_EMU
     cudaFuncSetAttribute(band_sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 #endif
-    WB_LAUNCH_COOP(band_sweep_kernel, dim3((unsigned)p.n_bands, n_utts), WB_SWEEP_THREADS, smem, ctx->stream, p);
+    WB_LAUNCH_COOP(band_sweep_kernel, sweep_grid(p, n_utts), WB_SWEEP_THREADS, smem, ctx->stream, p);
   }
 }
 
@@ -1049,8 +1072,9 @@ void launch_band_sweep_split(Ctx *ctx, const SweepParams &p_in, unsigned n_utts)
   cudaFuncSetAttribute(band_fir_events_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_fe);
   cudaFuncSetAttribute(band_sweep_list_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sw);
 #endif
-  WB_LAUNCH_COOP(band_fir_events_kernel, dim3((unsigned)((p.n_bands + 1) / 2), n_utts), WB_SWEEP_THREADS, smem_fe, ctx->stream, p);
-  WB_LAUNCH_COOP(band_interp_kernel, dim3((unsigned)p.n_bands, n_utts), 256, 0, ctx->stream, p);
+  const dim3 pair_grid = p.ugrp ? dim3((unsigned)p.n_blk_pair) : dim3((unsigned)((p.n_bands + 1) / 2), n_utts);
+  WB_LAUNCH_COOP(band_fir_events_kernel, pair_grid, WB_SWEEP_THREADS, smem_fe, ctx->stream, p);
+  WB_LAUNCH_COOP(band_interp_kernel, sweep_grid(p, n_utts), 256, 0, ctx->stream, p);
   // bands whose edge lists overflowed (usually none): the streaming kernel with its history rings, over the list
   WB_LAUNCH_COOP(band_sweep_list_kernel, dim3((unsigned)(3 * ctx->sm_count)), WB_SWEEP_THREADS, smem_sw, ctx->stream, p);
 }

@@ -98,7 +98,40 @@ struct SweepParams {
   // complete edge lists to global memory) and band_interp_kernel (edge lists -> candidates on the frame grid).
   int *ev_count;          // [n][n_bands][4] events per train; ev_count[..][0] = -1 marks a band whose lists overflowed
   int *redo_list; int *redo_count;   // (utterance * n_bands + band) pairs for the streaming kernel (history rings)
+  // Harvest, one F0 range per utterance.  The per-band tables above (taps, tap_off, ntaps, shift, boundary, edge_cap,
+  // edge_off) hold the band lists of every range group of the batch one after the other; utterance u uses group
+  // g = ugrp[u]: bands grp_band0[g] .. grp_band0[g] + grp_nb[g] - 1 of the tables, floor / ceiling grp_floor[g] /
+  // grp_ceil[g].  Band indices b elsewhere (cand rows, ev_count, redo_list) are the utterance's own 0 .. grp_nb - 1,
+  // strided by n_bands = the batch maximum.  The grids are flat over the utterances' own bands (band pairs for
+  // band_fir_events_kernel): blk0_band[u] / blk0_pair[u] is the first block of utterance u ([n_utts + 1] prefix sums,
+  // totals n_blk_band / n_blk_pair), so the work follows the sum of the channel counts, not n x the largest.
+  // ugrp == nullptr (DIO): bands 0 .. n_bands - 1 and f0_floor / f0_ceil for every utterance, grid (band, utterance).
+  const int *ugrp = nullptr; const int *grp_band0 = nullptr, *grp_nb = nullptr;
+  const double *grp_floor = nullptr, *grp_ceil = nullptr;
+  const int *blk0_band = nullptr, *blk0_pair = nullptr; int n_blk_band = 0, n_blk_pair = 0, n_utts = 0;
 };
+
+// the band list of utterance u (see SweepParams::ugrp); grp = -1 without range groups.  The thresholds are read where
+// they are used (sweep_store_candidate): a kernel keeps one int live, not two doubles.
+struct UttBands { int band0, nb, grp; };
+WB_DEV UttBands utt_bands(const SweepParams &p, int u) {
+  UttBands r;
+  if (!p.ugrp) { r.band0 = 0; r.nb = p.n_bands; r.grp = -1; return r; }
+  r.grp = p.ugrp[u];
+  r.band0 = p.grp_band0[r.grp]; r.nb = p.grp_nb[r.grp];
+  return r;
+}
+
+// flat grid: the utterance u with first[u] <= blk < first[u + 1] (first[0] = 0, nondecreasing) and blk's index in it
+WB_DEV int flat_block(const int *first, int n_utts, int blk, int *u) {
+  int lo = 0, hi = n_utts - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (first[mid] <= blk) lo = mid; else hi = mid - 1;
+  }
+  *u = lo;
+  return blk - first[lo];
+}
 
 // band_fir_events_kernel: tiles of 1024 outputs = 8 outputs per event thread x 128 = 64 FIR rows of 16 outputs
 // (m16n8k8 row tiles), two per filter warp.  Two input segments (TMA double buffer), the taps of two bands with 8

@@ -16,6 +16,11 @@
 
 using namespace wb;
 
+namespace wb {
+// wb_api.cu: frame_period and F0 range checks of per-utterance Harvest options
+int check_harvest_options(Ctx *c, const HarvestOption *opts, int n, double frame_period, int fs);
+}  // namespace wb
+
 namespace {
 
 struct DevBuf {
@@ -48,9 +53,10 @@ namespace {
 // un-overlapped tail is one sub-chunk.  Result buffers form a ring two outer chunks deep, so downloads
 // may lag behind the frame kernels and catch up under the next outer chunk's F0 stage.  Streams: s_in
 // (uploads), the context's stream (all kernels), s_out (downloads); events order buffer reuse.
+// harvest_options: nullptr, or one HarvestOption per utterance (checked by the caller); the chunks split the array.
 int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride, const int *x_lengths, int fs,
-                     const WorldB200AnalysisOption *opt, int dims, double *time_axis, double *f0, int f0_stride,
-                     double *out_sp, double *out_ap) {
+                     const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options, int dims,
+                     double *time_axis, double *f0, int f0_stride, double *out_sp, double *out_ap) {
   Ctx *ctx = ctx_of(h);
   const int bins = opt->cheaptrick.fft_size / 2 + 1;
   const int n_ap = GetNumberOfAperiodicities(fs);
@@ -190,7 +196,8 @@ int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_st
     const double *xd = (const double *)(nbit ? dx[s].p : din[s].p);
     double *td = (double *)dt[s].p, *fd = (double *)df[s].p;
     if (opt->f0_method == WORLD_B200_F0_HARVEST) {
-      rc = world_b200_harvest_batch(h, xd, n, x_stride, xl, fs, &opt->harvest, td, fd, f0_stride);
+      rc = harvest_options ? world_b200_harvest_batch_options(h, xd, n, x_stride, xl, fs, harvest_options + u0, td, fd, f0_stride)
+                           : world_b200_harvest_batch(h, xd, n, x_stride, xl, fs, &opt->harvest, td, fd, f0_stride);
     } else {
       rc = world_b200_dio_batch(h, xd, n, x_stride, xl, fs, &opt->dio, td, fd, f0_stride);
       if (!rc) rc = world_b200_stonemask_batch(h, xd, n, x_stride, xl, fs, td, fd, fl, f0_stride, fd);
@@ -324,8 +331,25 @@ extern "C" int world_b200_analyze_host(WorldB200 *h, const double *x, int n_utts
                                        double *aperiodicity) {
   if (!h || !x || !opt || n_utts < 0 || fs <= 0 || x_stride <= 0 || f0_stride <= 0) return WORLD_B200_EINVAL;
   DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  return analyze_pipeline(h, x, 0, n_utts, x_stride, x_lengths, fs, opt, 0, time_axis, f0, f0_stride, spectrogram,
+  return analyze_pipeline(h, x, 0, n_utts, x_stride, x_lengths, fs, opt, nullptr, 0, time_axis, f0, f0_stride, spectrogram,
                           aperiodicity);
+}
+
+extern "C" int world_b200_analyze_host_options(WorldB200 *h, const double *x, int n_utts, int x_stride,
+                                               const int *x_lengths, int fs, const WorldB200AnalysisOption *opt,
+                                               const HarvestOption *harvest_options, double *time_axis, double *f0,
+                                               int f0_stride, double *spectrogram, double *aperiodicity) {
+  if (!h || !x || !opt || !harvest_options || n_utts < 0 || fs <= 0 || x_stride <= 0 || f0_stride <= 0)
+    return WORLD_B200_EINVAL;
+  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
+  if (opt->f0_method != WORLD_B200_F0_HARVEST) {
+    ctx_of(h)->last_error = "analyze_host: per-utterance Harvest options need f0_method == WORLD_B200_F0_HARVEST";
+    return WORLD_B200_EINVAL;
+  }
+  const int rc = check_harvest_options(ctx_of(h), harvest_options, n_utts, opt->harvest.frame_period, fs);
+  if (rc) return rc;
+  return analyze_pipeline(h, x, 0, n_utts, x_stride, x_lengths, fs, opt, harvest_options, 0, time_axis, f0, f0_stride,
+                          spectrogram, aperiodicity);
 }
 
 extern "C" int world_b200_analyze_coded_host(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride,
@@ -339,7 +363,7 @@ extern "C" int world_b200_analyze_coded_host(WorldB200 *h, const void *x, int nb
     ctx_of(h)->last_error = "analyze_coded_host: number_of_dimensions must be in [1, fft_size/4 + 1]";
     return WORLD_B200_EINVAL;
   }
-  return analyze_pipeline(h, x, nbit, n_utts, x_stride, x_lengths, fs, opt, number_of_dimensions, time_axis, f0,
+  return analyze_pipeline(h, x, nbit, n_utts, x_stride, x_lengths, fs, opt, nullptr, number_of_dimensions, time_axis, f0,
                           f0_stride, coded_spectral_envelope, coded_aperiodicity);
 }
 

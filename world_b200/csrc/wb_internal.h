@@ -155,6 +155,9 @@ int stonemask_run(Ctx *ctx, const Batch &b, double *refined_f0);
 struct DioParams { double f0_floor, f0_ceil, channels_in_octave, frame_period, allowed_range; int speed; };
 int dio_run(Ctx *ctx, const Batch &b, const DioParams &p, double *time_axis_out, double *f0_out);
 struct HarvestParams { double f0_floor, f0_ceil, frame_period; };
-int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams &p, double *time_axis_out, double *f0_out);
+// per_utt: opts[u] is utterance u's option (f0_floor / f0_ceil may differ, frame_period may not); else opts[0] for all
+int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_utt, double *time_axis_out, double *f0_out);
+// the range checks of harvest_run for n per-utterance options; 3 (EINVAL) + last_error naming the first bad utterance
+int harvest_check_options(Ctx *ctx, int fs, const HarvestParams *opts, int n);
 
 }  // namespace wb
