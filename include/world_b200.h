@@ -13,7 +13,10 @@
  *     (x_stride samples / f0_stride frames).  Padding is never read; padded frames are never
  *     written.
  *   - The *_batch functions take DEVICE pointers for the big arrays and enqueue their work on
- *     the context's stream (world_b200_set_stream); they do not synchronise.  The *_host
+ *     the context's stream (world_b200_set_stream); they do not synchronise.  One exception:
+ *     world_b200_synthesis_batch reads its pulse counts back once per chunk of utterances, which
+ *     synchronises the context's stream (all work queued on it before the call included) before
+ *     the chunk's remaining kernels are enqueued.  The *_host
  *     functions take host pointers, stage through device memory and return when the results are
  *     in the caller's buffers.
  *   - Every function returns 0 on success or a WORLD_B200_E* code; world_b200_last_error()

@@ -261,6 +261,10 @@ def test_gpu_unsupported_configurations_fail_cleanly(gpu_world):
     f = torch.full((1, 21), 150.0, dtype=torch.float64, device=dev)
     cases.append(("StoneMask fs=192k", lambda: w.stonemask(x, 192000, t, f)))
     cases.append(("D4C fs=192k", lambda: w.d4c(x, 192000, t, f, 8192)))
+    # StoneMask, and with it the DIO chain, above 48 kHz (Harvest, CheapTrick and D4C run there)
+    from test_stage_paths import high_rate_rejections
+    for fs_hi in (88200, 96000):
+        cases += high_rate_rejections(w, fs_hi)
     # Harvest with a floor whose refinement window / band filters do not fit on chip
     o = w.harvest_option(); o.f0_floor = 8.0
     cases.append(("Harvest floor 8 Hz", lambda: w.harvest(x[:, :16000], 16000, o)))

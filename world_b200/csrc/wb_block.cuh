@@ -11,10 +11,12 @@ namespace wb {
 
 #define WB_RED_DOUBLES 72
 
+// The host emulation runs one thread per block; its reductions still store the partial sums where warp 0 of a CTA
+// stores them (red[0], red[33], ...), so a kernel that keeps live data in `red` across a reduction fails there too.
 WB_DEV double block_sum(double v, double *red) {
 #ifdef WB_EMU
-  (void)red;
-  return v;
+  red[0] = v;
+  return red[0];
 #else
   for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
@@ -30,7 +32,8 @@ WB_DEV double block_sum(double v, double *red) {
 // two sums with one pair of barriers
 WB_DEV void block_sum2(double &a, double &b, double *red) {
 #ifdef WB_EMU
-  (void)red;
+  red[0] = a; red[33] = b;
+  a = red[0]; b = red[33];
 #else
   for (int o = 16; o; o >>= 1) {
     a += __shfl_xor_sync(0xffffffffu, a, o);
@@ -48,8 +51,9 @@ WB_DEV void block_sum2(double &a, double &b, double *red) {
 
 WB_DEV int block_sum_int(int v, double *red) {
 #ifdef WB_EMU
-  (void)red;
-  return v;
+  int *ired = reinterpret_cast<int *>(red);
+  ired[0] = v;
+  return ired[0];
 #else
   int *ired = reinterpret_cast<int *>(red);
   v = __reduce_add_sync(0xffffffffu, v);
@@ -101,7 +105,7 @@ namespace wb {
 template <int K>
 WB_DEV void block_sum_n(double (&v)[K], double *red) {
 #ifdef WB_EMU
-  (void)v; (void)red;
+  for (int k = 0; k < K; ++k) { red[33 * k] = v[k]; v[k] = red[33 * k]; }
 #else
 #pragma unroll
   for (int k = 0; k < K; ++k)

@@ -31,6 +31,7 @@ struct SynParams {
   double *vuv;              // [n][y_stride] interpolated vuv (0/1)
   int *flag_cnt;            // [n][258]
   int *pulse_idx; double *pulse_shift; int *n_pulses; int pulse_cap;   // [n][pulse_cap]
+  int *pulse_count;         // [n] pulses found, also those beyond pulse_cap (the host sizes the arrays from it)
   unsigned *draw_cnt; unsigned *draw_off; unsigned *draw_tot;
   const unsigned *draws; size_t draw_stride;
   double *resp;             // [n][pulse_cap][fft_size]
@@ -98,7 +99,8 @@ WB_KERNEL(256, 2) syn_timebase_kernel(SynParams p) {
     for (int t = 0; t < nth; ++t) { const int v = cnt[t]; cnt[t] = run; run += v; }
     cnt[nth] = run;
     p.n_pulses[u] = imin(run, p.pulse_cap);
-    if (run > p.pulse_cap) atomicOr_status(p.status, 4);
+    p.pulse_count[u] = run;   // run > pulse_cap: the host lays the chunk out again before anything reads the list
+    if (run > p.pulse_cap) atomicOr_status(p.status, 4);   // status is null unless the counts sized this layout
   }
   WB_SYNC();
   int k = cnt[tid];
@@ -326,24 +328,31 @@ extern "C" int world_b200_synthesis_batch(WorldB200 *h, const double *f0, const 
     }
     for (int i = 0; i < fft_size / 2; ++i) { dcr[i] /= dc; dcr[fft_size - i - 1] = dcr[i]; }
   }
-  // at most one pulse per two samples is impossible below fs/2; 1200 pulses/s covers f0 <= 1.2 kHz
-  const int pulse_cap = (int)((double)max_y / fs * 1200.0) + 64;
+  // Pulse arrays and responses are sized for 1200 pulses per second (f0 <= 1.2 kHz; the +64 covers the ends).
+  // The caller's f0 may be anything up to fs/2 (a pitch-shifted contour), so syn_timebase_kernel also counts the
+  // pulses it could not store; a chunk where that count exceeds the cap is laid out again with room for its largest
+  // count, in as many passes as the scratch budget needs.  The common case pays one read-back of n counts per chunk.
+  const int nominal_cap = (int)((double)max_y / fs * 1200.0) + 64;
   const size_t draw_stride = (size_t)max_y + 8;
-  const size_t per_utt = (size_t)y_stride * 16 + (size_t)pulse_cap * (4 + 8 + 8) + (size_t)pulse_cap * fft_size * 8 +
-                         draw_stride * 4 + 4096;
-  int chunk = balanced_chunk(imin(n_utts, 65535), (int)dmin(65535.0, (double)ctx->scratch_budget / (double)per_utt));
+  auto per_utt = [&](int cap) {
+    return (size_t)y_stride * 16 + (size_t)cap * (4 + 8 + 8) + (size_t)cap * fft_size * 8 + draw_stride * 4 + 4096;
+  };
+  auto fit = [&](int cap) { return (int)dmin(65535.0, (double)ctx->scratch_budget / (double)per_utt(cap)); };
+  const int chunk = balanced_chunk(imin(n_utts, 65535), fit(nominal_cap));
   const int half = fft_size / 2;
   const size_t smem = (size_t)(2 * fft_size + 2 * (half + 2) + (fft_size + 2) + 2 * (half + 1) + fft_size + WB_RED_DOUBLES) * 8;
 #ifndef WB_EMU
   cudaFuncSetAttribute(syn_pulse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 #endif
-  for (int u0 = 0; u0 < n_utts; u0 += chunk) {
-    const int n = imin(chunk, n_utts - u0);
+  std::vector<int> counts;
+  int u0 = 0, n = imin(chunk, n_utts), pulse_cap = nominal_cap;
+  bool relaid = false;
+  while (u0 < n_utts) {
     ArenaPlan plan;
     const size_t o_len = plan.add((size_t)2 * n * 4);
     const size_t o_phase = plan.add((size_t)n * y_stride * 8), o_vuv = plan.add((size_t)n * y_stride * 8);
     const size_t o_pidx = plan.add((size_t)n * pulse_cap * 4), o_psh = plan.add((size_t)n * pulse_cap * 8);
-    const size_t o_np = plan.add((size_t)n * 4);
+    const size_t o_np = plan.add((size_t)n * 4), o_cnt = plan.add((size_t)n * 4);
     const size_t o_dc = plan.add((size_t)n * pulse_cap * 4), o_do = plan.add((size_t)n * pulse_cap * 4);
     const size_t o_dt = plan.add((size_t)n * 4), o_pl = plan.add((size_t)n * 4);
     const size_t o_draws = plan.add((size_t)n * draw_stride * 4);
@@ -364,18 +373,39 @@ extern "C" int world_b200_synthesis_batch(WorldB200 *h, const double *f0, const 
     p.y_len = (const int *)(blk + o_len) + n; p.y_stride = y_stride;
     p.phase = (double *)(blk + o_phase); p.vuv = (double *)(blk + o_vuv); p.flag_cnt = nullptr;
     p.pulse_idx = (int *)(blk + o_pidx); p.pulse_shift = (double *)(blk + o_psh); p.n_pulses = (int *)(blk + o_np);
-    p.pulse_cap = pulse_cap;
+    p.pulse_cap = pulse_cap; p.pulse_count = (int *)(blk + o_cnt);
     p.draw_cnt = (unsigned *)(blk + o_dc); p.draw_off = (unsigned *)(blk + o_do); p.draw_tot = (unsigned *)(blk + o_dt);
     p.draws = (const unsigned *)(blk + o_draws); p.draw_stride = draw_stride;
     p.resp = (double *)(blk + o_resp); p.dc_remover = (const double *)(blk + o_dcr);
-    p.y = y + (size_t)u0 * y_stride; p.tw = ctx->twiddle; p.status = ctx->status_dev;
+    p.y = y + (size_t)u0 * y_stride; p.tw = ctx->twiddle;
+    // a pass laid out from the counts reports a pulse beyond its arrays as a scratch overflow (status bit 4)
+    p.status = relaid ? ctx->status_dev : nullptr;
     WB_LAUNCH_COOP(syn_timebase_kernel, dim3((unsigned)n), 256, 0, ctx->stream, p);
+    if (!relaid) {
+      counts.resize(n);
+      rc = dev_memcpy_d2h(ctx, counts.data(), p.pulse_count, (size_t)n * 4);
+      if (!rc) rc = dev_sync(ctx);
+      if (rc) return rc;
+      int most = 0;
+      for (int i = 0; i < n; ++i) most = imax(most, counts[i]);
+      if (most > pulse_cap) {
+        // the time base is deterministic: run again over the first n' of these utterances, it finds the same pulses
+        pulse_cap = most;
+        n = imin(n, imax(1, fit(pulse_cap)));
+        relaid = true;
+        continue;
+      }
+    }
     scan_counts(ctx, p.draw_cnt, (const int *)(blk + o_pl), pulse_cap, nullptr, p.draw_off, p.draw_tot, n);
     rng_fill(ctx, p.draw_tot, (unsigned *)(blk + o_draws), draw_stride, draw_stride, n);
     WB_LAUNCH_COOP(syn_pulse_kernel, dim3((unsigned)pulse_cap, (unsigned)n), 128, smem, ctx->stream, p);
     WB_LAUNCH_FLAT(syn_overlap_kernel, dim3((unsigned)((max_y + 255) / 256), (unsigned)n), 256, 0, ctx->stream, p);
     rc = dev_check(ctx, "synthesis");
     if (rc) return rc;
+    u0 += n;
+    n = imin(chunk, n_utts - u0);
+    pulse_cap = nominal_cap;
+    relaid = false;
   }
   return 0;
 }
