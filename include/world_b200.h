@@ -99,6 +99,14 @@ int world_b200_frames(int fs, int x_length, double frame_period);
 int world_b200_dio_batch(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
                          const int *x_lengths, int fs, const DioOption *option,
                          double *time_axis, double *f0, int f0_stride);
+/* The same with one option per utterance: dio_options is a HOST array of n_utts.  f0_floor, f0_ceil,
+ * channels_in_octave and allowed_range may differ between utterances; frame_period and speed must be the same for all
+ * (they fix the decimation, the low-cut filter and the frame grid; else EINVAL).  Each row equals what
+ * world_b200_dio_batch gives that utterance with its own option.  A band list the on-chip kernels cannot serve is
+ * EINVAL, and world_b200_last_error() names the first such utterance. */
+int world_b200_dio_batch_options(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
+                                 const int *x_lengths, int fs, const DioOption *dio_options,
+                                 double *time_axis, double *f0, int f0_stride);
 /* Harvest() over a batch (harvest.h:35). */
 int world_b200_harvest_batch(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
                              const int *x_lengths, int fs, const HarvestOption *option,
@@ -207,6 +215,14 @@ int world_b200_analyze_batch_options(WorldB200 *ctx, const double *x, int n_utts
                                      const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
                                      const HarvestOption *harvest_options, double *time_axis, double *f0,
                                      int f0_stride, double *spectrogram, double *aperiodicity);
+/* ... with one DIO option per utterance (dio_options: HOST array of n_utts, see world_b200_dio_batch_options).
+ * option->f0_method must be WORLD_B200_F0_DIO_STONEMASK, and every dio_options[u].frame_period and .speed must equal
+ * option->dio's (else EINVAL); option->dio's floor, ceiling, channels_in_octave and allowed_range are not used.  The
+ * *_dio_options variants below follow the same rules.  Options of the other F0 method are EINVAL. */
+int world_b200_analyze_batch_dio_options(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
+                                         const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                         const DioOption *dio_options, double *time_axis, double *f0,
+                                         int f0_stride, double *spectrogram, double *aperiodicity);
 
 /* ---- multi-GPU: one context per GPU (one process or thread each), utterances sharded over ranks --------------
  * There is no exchange inside the analysis; the one collective reassembles the output arrays on every rank
@@ -241,6 +257,13 @@ int world_b200_analyze_batch_allgather_options(WorldB200 *ctx, const double *x, 
                                                const HarvestOption *harvest_options, double *time_axis_full,
                                                double *f0_full, int f0_stride, double *spectrogram_full,
                                                double *aperiodicity_full);
+/* ... with one DIO option per utterance of THIS rank's shard (dio_options: HOST array of n_utts). */
+int world_b200_analyze_batch_allgather_dio_options(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
+                                                   const int *x_lengths, int fs,
+                                                   const WorldB200AnalysisOption *option,
+                                                   const DioOption *dio_options, double *time_axis_full,
+                                                   double *f0_full, int f0_stride, double *spectrogram_full,
+                                                   double *aperiodicity_full);
 
 /* {Dio+StoneMask | Harvest} -> CheapTrick -> D4C for n_utts host waveforms; outputs are host
  * arrays laid out as described above.  Input upload, compute and result download are pipelined
@@ -255,6 +278,11 @@ int world_b200_analyze_host_options(WorldB200 *ctx, const double *x, int n_utts,
                                     const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
                                     const HarvestOption *harvest_options, double *time_axis, double *f0,
                                     int f0_stride, double *spectrogram, double *aperiodicity);
+/* ... with one DIO option per utterance (HOST array of n_utts; the chunks split it). */
+int world_b200_analyze_host_dio_options(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
+                                        const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                        const DioOption *dio_options, double *time_axis, double *f0,
+                                        int f0_stride, double *spectrogram, double *aperiodicity);
 
 /* The same chain with the ingest and the codec fused in on the device: x holds samples of `nbit`
  * bits (0 = doubles as above; 8/16/24/32 = little-endian PCM as in a WAV data chunk), and the
@@ -265,6 +293,18 @@ int world_b200_analyze_coded_host(WorldB200 *ctx, const void *x, int nbit, int n
                                   const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
                                   int number_of_dimensions, double *time_axis, double *f0, int f0_stride,
                                   double *coded_spectral_envelope, double *coded_aperiodicity);
+/* ... with one option per utterance of the chain's F0 method (HOST array of n_utts; the chunks split it): Harvest
+ * options as for world_b200_analyze_host_options, DIO options as for world_b200_analyze_host_dio_options. */
+int world_b200_analyze_coded_host_options(WorldB200 *ctx, const void *x, int nbit, int n_utts, int x_stride,
+                                          const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                          const HarvestOption *harvest_options, int number_of_dimensions,
+                                          double *time_axis, double *f0, int f0_stride,
+                                          double *coded_spectral_envelope, double *coded_aperiodicity);
+int world_b200_analyze_coded_host_dio_options(WorldB200 *ctx, const void *x, int nbit, int n_utts, int x_stride,
+                                              const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                              const DioOption *dio_options, int number_of_dimensions,
+                                              double *time_axis, double *f0, int f0_stride,
+                                              double *coded_spectral_envelope, double *coded_aperiodicity);
 
 #ifdef __cplusplus
 }

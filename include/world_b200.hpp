@@ -139,6 +139,27 @@ inline int Harvest(const double *const *xs, const int *x_lengths, int n_utts, in
   return rc;
 }
 
+// One DIO option per utterance (options.size() == n_utts): f0_floor / f0_ceil / channels_in_octave / allowed_range may
+// differ, frame_period and speed may not (world_b200_dio_batch_options).  A vector, as for Harvest above.
+inline int Dio(const double *const *xs, const int *x_lengths, int n_utts, int fs, const std::vector<DioOption> &options,
+               double *const *temporal_positions, double *const *f0s) {
+  using namespace world_b200;
+  if (n_utts < 0 || options.size() != static_cast<size_t>(n_utts)) return WORLD_B200_EINVAL;
+  if (n_utts == 0) return 0;
+  WorldB200 *w = shared_context();
+  if (!w) return WORLD_B200_ECUDA;
+  const int xs_stride = max_of(x_lengths, n_utts);
+  const std::vector<int> fl = frame_counts(x_lengths, n_utts, fs, options[0].frame_period);
+  const int f_stride = max_of(fl.data(), n_utts);
+  DeviceArray dx(static_cast<size_t>(n_utts) * xs_stride), dt(static_cast<size_t>(n_utts) * f_stride), df(static_cast<size_t>(n_utts) * f_stride);
+  int rc = upload(dx, pack(xs, x_lengths, n_utts, xs_stride));
+  if (!rc) rc = world_b200_dio_batch_options(w, dx.p, n_utts, xs_stride, x_lengths, fs, options.data(), dt.p, df.p, f_stride);
+  if (!rc) rc = world_b200_synchronize(w);
+  if (!rc) rc = download_rows(dt, n_utts, f_stride, fl.data(), temporal_positions);
+  if (!rc) rc = download_rows(df, n_utts, f_stride, fl.data(), f0s);
+  return rc;
+}
+
 inline int StoneMask(const double *const *xs, const int *x_lengths, int n_utts, int fs,
                      const double *const *temporal_positions, const double *const *f0s, const int *f0_lengths,
                      double *const *refined_f0s) {

@@ -67,6 +67,8 @@ ABI = {
     "world_b200_profile": (C.c_int, [_P, C.c_int]),
     "world_b200_profile_report": (C.c_int, [_P, C.c_char_p, C.c_ulonglong]),
     "world_b200_dio_batch": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(DioOption), _P, _P, C.c_int]),
+    "world_b200_dio_batch_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(DioOption), _P, _P,
+                                               C.c_int]),
     "world_b200_harvest_batch": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(HarvestOption), _P, _P, C.c_int]),
     "world_b200_harvest_batch_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(HarvestOption), _P,
                                                    _P, C.c_int]),
@@ -95,6 +97,14 @@ ABI = {
     "world_b200_analyze_batch_allgather_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int,
                                                              C.POINTER(AnalysisOption), C.POINTER(HarvestOption), _P,
                                                              _P, C.c_int, _P, _P]),
+    "world_b200_analyze_host_dio_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(AnalysisOption),
+                                                      C.POINTER(DioOption), _P, _P, C.c_int, _P, _P]),
+    "world_b200_analyze_batch_dio_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int,
+                                                       C.POINTER(AnalysisOption), C.POINTER(DioOption), _P, _P, C.c_int,
+                                                       _P, _P]),
+    "world_b200_analyze_batch_allgather_dio_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int,
+                                                                 C.POINTER(AnalysisOption), C.POINTER(DioOption), _P,
+                                                                 _P, C.c_int, _P, _P]),
     "world_b200_comm_unique_id": (C.c_int, [_P, C.c_int]),
     "world_b200_comm_init": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int]),
     "world_b200_comm_destroy": (C.c_int, [_P]),
@@ -123,6 +133,12 @@ ABI = {
     "world_b200_pcm_to_double_batch": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, _P]),
     "world_b200_analyze_coded_host": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int,
                                                 C.POINTER(AnalysisOption), C.c_int, _P, _P, C.c_int, _P, _P]),
+    "world_b200_analyze_coded_host_options": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int,
+                                                        C.POINTER(AnalysisOption), C.POINTER(HarvestOption), C.c_int,
+                                                        _P, _P, C.c_int, _P, _P]),
+    "world_b200_analyze_coded_host_dio_options": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int,
+                                                            C.POINTER(AnalysisOption), C.POINTER(DioOption), C.c_int,
+                                                            _P, _P, C.c_int, _P, _P]),
     # host-only file glue (tools/audioio.h, tools/parameterio.h)
     "wavwrite": (None, [_P, C.c_int, C.c_int, C.c_int, C.c_char_p]),
     "GetAudioLength": (C.c_int, [C.c_char_p]),
@@ -191,6 +207,32 @@ def _harvest_options(options, n):
     for i, o in enumerate(options):
         arr[i].f0_floor, arr[i].f0_ceil, arr[i].frame_period = o.f0_floor, o.f0_ceil, o.frame_period
     return arr
+
+
+def _dio_options(options, n):
+    """A list of n DioOption (one per utterance) as a ctypes array; None for a single option or None."""
+    if options is None or isinstance(options, DioOption):
+        return None
+    options = list(options)
+    if len(options) != n:
+        raise ValueError(f"{len(options)} DIO options for {n} utterances")
+    arr = (DioOption * n)()
+    for i, o in enumerate(options):
+        for name, _ in DioOption._fields_:
+            setattr(arr[i], name, getattr(o, name))
+    return arr
+
+
+def _chain_options(harvest_options, dio_options, n):
+    """The per-utterance options of a chain as (harvest array or None, DIO array or None).  A chain takes the options
+    of one F0 method only, as a list of one option per utterance: a single option is refused rather than ignored
+    (the chain's own option in the AnalysisOption is the way to give one option for the batch)."""
+    if harvest_options is not None and dio_options is not None:
+        raise ValueError("harvest_options and dio_options: pass the options of one F0 method")
+    if isinstance(harvest_options, HarvestOption) or isinstance(dio_options, DioOption):
+        raise TypeError("harvest_options / dio_options: a list of one option per utterance (one option for the batch "
+                        "goes into the AnalysisOption)")
+    return _harvest_options(harvest_options, n), _dio_options(dio_options, n)
 
 
 def _int_array(v, n):
@@ -331,16 +373,24 @@ class World:
         fl = [self.frames(fs, v, frame_period) for v in lens]
         return max(fl), fl
 
-    def dio(self, x, fs, option: DioOption | None = None, x_lengths=None):
-        option = option or self.dio_option()
+    def dio(self, x, fs, option=None, x_lengths=None):
+        """option: one DioOption for the batch, or a list of one per utterance (f0_floor / f0_ceil /
+        channels_in_octave / allowed_range may differ, frame_period and speed may not)."""
         n, stride = x.shape
-        f_stride, fl = self._f0_stride(fs, x, x_lengths, option.frame_period)
+        per_utt = _dio_options(option, n)
+        option = option or self.dio_option()
+        frame_period = per_utt[0].frame_period if per_utt is not None and n else getattr(option, "frame_period", 5.0)
+        f_stride, fl = self._f0_stride(fs, x, x_lengths, frame_period)
         t = self._zeros(x, (n, f_stride))
         f0 = self._zeros(x, (n, f_stride))
         xl, keep = _int_array(x_lengths, n)
         self._use_current_stream()
-        self._check(self.lib.world_b200_dio_batch(self._h, _ptr(x), n, stride, xl, fs, C.byref(option),
-                                                  _ptr(t), _ptr(f0), f_stride))
+        if per_utt is not None:
+            self._check(self.lib.world_b200_dio_batch_options(self._h, _ptr(x), n, stride, xl, fs, per_utt,
+                                                              _ptr(t), _ptr(f0), f_stride))
+        else:
+            self._check(self.lib.world_b200_dio_batch(self._h, _ptr(x), n, stride, xl, fs, C.byref(option),
+                                                      _ptr(t), _ptr(f0), f_stride))
         return t, f0, fl
 
     def harvest(self, x, fs, option=None, x_lengths=None):
@@ -447,9 +497,10 @@ class World:
         return o
 
     def analyze_batch(self, x, fs, option: AnalysisOption, x_lengths=None, time_axis=None, f0=None,
-                      spectrogram=None, aperiodicity=None, harvest_options=None):
+                      spectrogram=None, aperiodicity=None, harvest_options=None, dio_options=None):
         """Whole chain on DEVICE arrays in one call (two internal streams); returns (t, f0, sp, ap, frame counts).
-        harvest_options: a list of one HarvestOption per utterance (Harvest with a per-utterance F0 range)."""
+        harvest_options: a list of one HarvestOption per utterance (Harvest with a per-utterance F0 range);
+        dio_options: a list of one DioOption per utterance (DIO + StoneMask with a per-utterance F0 range)."""
         n, stride = x.shape
         frame_period = option.dio.frame_period if option.f0_method == F0_DIO_STONEMASK else option.harvest.frame_period
         f_stride, fl = self._f0_stride(fs, x, x_lengths, frame_period)
@@ -463,13 +514,18 @@ class World:
         if aperiodicity is None:
             aperiodicity = self._zeros(x, (n, f_stride, bins))
         xl, keep = _int_array(x_lengths, n)
-        per_utt = _harvest_options(harvest_options, n)
+        per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
         self._use_current_stream()
         if per_utt is not None:
             self._check(self.lib.world_b200_analyze_batch_options(self._h, _ptr(x), n, stride, xl, fs, C.byref(option),
                                                                   per_utt, _ptr(time_axis), _ptr(f0),
                                                                   time_axis.shape[1], _ptr(spectrogram),
                                                                   _ptr(aperiodicity)))
+        elif per_dio is not None:
+            self._check(self.lib.world_b200_analyze_batch_dio_options(self._h, _ptr(x), n, stride, xl, fs,
+                                                                      C.byref(option), per_dio, _ptr(time_axis),
+                                                                      _ptr(f0), time_axis.shape[1], _ptr(spectrogram),
+                                                                      _ptr(aperiodicity)))
         else:
             self._check(self.lib.world_b200_analyze_batch(self._h, _ptr(x), n, stride, xl, fs, C.byref(option),
                                                           _ptr(time_axis), _ptr(f0), time_axis.shape[1],
@@ -501,12 +557,12 @@ class World:
         return full
 
     def analyze_batch_allgather(self, x, fs, option: AnalysisOption, time_axis_full, f0_full, spectrogram_full,
-                                aperiodicity_full, x_lengths=None, harvest_options=None):
+                                aperiodicity_full, x_lengths=None, harvest_options=None, dio_options=None):
         """analyze_batch on this rank's shard with every finished slice broadcast into the FULL arrays of all ranks.
-        harvest_options: a list of one HarvestOption per utterance of THIS rank's shard."""
+        harvest_options / dio_options: a list of one option per utterance of THIS rank's shard."""
         n, stride = x.shape
         xl, keep = _int_array(x_lengths, n)
-        per_utt = _harvest_options(harvest_options, n)
+        per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
         outs = (_ptr(time_axis_full), _ptr(f0_full), time_axis_full.shape[1],
                 _ptr(spectrogram_full) if spectrogram_full is not None else None,
                 _ptr(aperiodicity_full) if aperiodicity_full is not None else None)
@@ -514,15 +570,18 @@ class World:
         if per_utt is not None:
             self._check(self.lib.world_b200_analyze_batch_allgather_options(
                 self._h, _ptr(x), n, stride, xl, fs, C.byref(option), per_utt, *outs))
+        elif per_dio is not None:
+            self._check(self.lib.world_b200_analyze_batch_allgather_dio_options(
+                self._h, _ptr(x), n, stride, xl, fs, C.byref(option), per_dio, *outs))
         else:
             self._check(self.lib.world_b200_analyze_batch_allgather(
                 self._h, _ptr(x), n, stride, xl, fs, C.byref(option), *outs))
 
     def analyze_host(self, x_host, fs, option: AnalysisOption, x_lengths=None, time_axis=None, f0=None,
-                     spectrogram=None, aperiodicity=None, f0_stride=None, harvest_options=None):
+                     spectrogram=None, aperiodicity=None, f0_stride=None, harvest_options=None, dio_options=None):
         """Whole chain on HOST arrays (numpy or pinned torch CPU tensors); outputs are written
-        into the given host arrays (allocated with numpy when None).  harvest_options: a list of one
-        HarvestOption per utterance."""
+        into the given host arrays (allocated with numpy when None).  harvest_options / dio_options: a list of
+        one option per utterance of the chain's F0 method."""
         import numpy as np
         n, stride = x_host.shape
         frame_period = option.dio.frame_period if option.f0_method == F0_DIO_STONEMASK else option.harvest.frame_period
@@ -539,11 +598,16 @@ class World:
         if aperiodicity is None:
             aperiodicity = np.zeros((n, f0_stride, bins))
         xl, keep = _int_array(x_lengths, n)
-        per_utt = _harvest_options(harvest_options, n)
+        per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
         if per_utt is not None:
             self._check(self.lib.world_b200_analyze_host_options(self._h, _ptr(x_host), n, stride, xl, fs,
                                                                  C.byref(option), per_utt, _ptr(time_axis), _ptr(f0),
                                                                  f0_stride, _ptr(spectrogram), _ptr(aperiodicity)))
+        elif per_dio is not None:
+            self._check(self.lib.world_b200_analyze_host_dio_options(self._h, _ptr(x_host), n, stride, xl, fs,
+                                                                     C.byref(option), per_dio, _ptr(time_axis),
+                                                                     _ptr(f0), f0_stride, _ptr(spectrogram),
+                                                                     _ptr(aperiodicity)))
         else:
             self._check(self.lib.world_b200_analyze_host(self._h, _ptr(x_host), n, stride, xl, fs, C.byref(option),
                                                          _ptr(time_axis), _ptr(f0), f0_stride, _ptr(spectrogram),
@@ -606,9 +670,11 @@ class World:
         return x
 
     def analyze_coded_host(self, x_host, nbit, fs, option: AnalysisOption, number_of_dimensions, x_lengths=None,
-                           time_axis=None, f0=None, coded_sp=None, coded_ap=None, f0_stride=None):
+                           time_axis=None, f0=None, coded_sp=None, coded_ap=None, f0_stride=None, harvest_options=None,
+                           dio_options=None):
         """Whole chain with device-side ingest (nbit 0 = float64 rows, 16 = int16 rows, ...) and codec;
-        only the coded rows are downloaded."""
+        only the coded rows are downloaded.  harvest_options / dio_options: a list of one option per utterance of
+        the chain's F0 method (not both)."""
         import numpy as np
         n = x_host.shape[0]
         item = x_host.element_size() if hasattr(x_host, "element_size") else x_host.itemsize
@@ -627,7 +693,15 @@ class World:
         if coded_ap is None:
             coded_ap = np.zeros((n, f0_stride, max(1, n_ap)))
         xl, keep = _int_array(x_lengths, n)
-        self._check(self.lib.world_b200_analyze_coded_host(self._h, _ptr(x_host), nbit, n, stride, xl, fs,
-                                                           C.byref(option), number_of_dimensions, _ptr(time_axis),
-                                                           _ptr(f0), f0_stride, _ptr(coded_sp), _ptr(coded_ap)))
+        per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
+        outs = (number_of_dimensions, _ptr(time_axis), _ptr(f0), f0_stride, _ptr(coded_sp), _ptr(coded_ap))
+        if per_utt is not None:
+            self._check(self.lib.world_b200_analyze_coded_host_options(self._h, _ptr(x_host), nbit, n, stride, xl, fs,
+                                                                       C.byref(option), per_utt, *outs))
+        elif per_dio is not None:
+            self._check(self.lib.world_b200_analyze_coded_host_dio_options(self._h, _ptr(x_host), nbit, n, stride, xl,
+                                                                           fs, C.byref(option), per_dio, *outs))
+        else:
+            self._check(self.lib.world_b200_analyze_coded_host(self._h, _ptr(x_host), nbit, n, stride, xl, fs,
+                                                               C.byref(option), *outs))
         return time_axis, f0, coded_sp, coded_ap, fl

@@ -309,6 +309,65 @@ int check_harvest_options(Ctx *c, const HarvestOption *opts, int n, double frame
   return harvest_check_options(c, fs, p.data(), n);
 }
 
+// The same for DIO: one frame_period and one speed for the whole batch (they fix the decimation ratio, the low-cut
+// filter and the frame grid); with fs > 0 also every utterance's band list against the on-chip limits.
+int check_dio_options(Ctx *c, const DioOption *opts, int n, double frame_period, int speed, int fs) {
+  for (int u = 0; u < n; ++u) {
+    const char *what = !(opts[u].frame_period == frame_period) ? "frame_period" : (opts[u].speed != speed ? "speed" : nullptr);
+    if (what) {
+      c->last_error = std::string("dio options: ") + what + " differs from the batch's (utterance " + std::to_string(u) + ")";
+      return WORLD_B200_EINVAL;
+    }
+  }
+  if (fs <= 0 || n <= 0) return 0;
+  std::vector<DioParams> p(n);
+  for (int u = 0; u < n; ++u)
+    p[u] = {opts[u].f0_floor, opts[u].f0_ceil, opts[u].channels_in_octave, opts[u].frame_period, opts[u].allowed_range,
+            opts[u].speed};
+  return dio_check_options(c, fs, p.data(), n);
+}
+
+// Per-utterance F0 options of a chain (harvest_options or dio_options, at most one): they must belong to the chain's
+// f0_method and pass check_*_options for the whole batch before a slice or chunk is queued.  `who` prefixes the error.
+int check_chain_f0_options(Ctx *c, const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
+                           const DioOption *dio_options, int n, int fs, const char *who) {
+  if (harvest_options && dio_options) {
+    c->last_error = std::string(who) + ": per-utterance options of both F0 methods";
+    return WORLD_B200_EINVAL;
+  }
+  if (harvest_options) {
+    if (opt->f0_method != WORLD_B200_F0_HARVEST) {
+      c->last_error = std::string(who) + ": per-utterance Harvest options need f0_method == WORLD_B200_F0_HARVEST";
+      return WORLD_B200_EINVAL;
+    }
+    return check_harvest_options(c, harvest_options, n, opt->harvest.frame_period, fs);
+  }
+  if (dio_options) {
+    if (opt->f0_method != WORLD_B200_F0_DIO_STONEMASK) {
+      c->last_error = std::string(who) + ": per-utterance DIO options need f0_method == WORLD_B200_F0_DIO_STONEMASK";
+      return WORLD_B200_EINVAL;
+    }
+    return check_dio_options(c, dio_options, n, opt->dio.frame_period, opt->dio.speed, fs);
+  }
+  return 0;
+}
+
+// The F0 stage of a chain on m utterances: Harvest, or DIO + StoneMask.  harvest_options / dio_options: nullptr (the
+// chain's own option) or the options of these m utterances, checked by check_chain_f0_options.
+int run_f0_stage(WorldB200 *h, const double *x, int m, int x_stride, const int *x_lengths, int fs,
+                 const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options, const DioOption *dio_options,
+                 const int *f0_lengths, double *time_axis, double *f0, int f0_stride) {
+  if (opt->f0_method == WORLD_B200_F0_HARVEST)
+    return harvest_options
+               ? world_b200_harvest_batch_options(h, x, m, x_stride, x_lengths, fs, harvest_options, time_axis, f0, f0_stride)
+               : world_b200_harvest_batch(h, x, m, x_stride, x_lengths, fs, &opt->harvest, time_axis, f0, f0_stride);
+  int rc = dio_options
+               ? world_b200_dio_batch_options(h, x, m, x_stride, x_lengths, fs, dio_options, time_axis, f0, f0_stride)
+               : world_b200_dio_batch(h, x, m, x_stride, x_lengths, fs, &opt->dio, time_axis, f0, f0_stride);
+  if (!rc) rc = world_b200_stonemask_batch(h, x, m, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, f0);
+  return rc;
+}
+
 }  // namespace wb
 
 extern "C" {
@@ -531,10 +590,16 @@ static int f0_lengths_from_x(int n, int x_stride, const int *x_lengths, int fs, 
   return 0;
 }
 
-int world_b200_dio_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
-                         const DioOption *opt, double *time_axis, double *f0, int f0_stride) {
+// opt: one option for every utterance, or (per_utt) an array of n
+static int dio_batch_impl(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
+                          const DioOption *opt, bool per_utt, double *time_axis, double *f0, int f0_stride) {
   if (!h || !x || !time_axis || !f0 || !opt || n < 0 || fs <= 0) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
+  if (per_utt && n > 0) {
+    // every band list too, before the lengths are uploaded: a bad option queues nothing on the device
+    const int rc = check_dio_options(&h->c, opt, n, opt[0].frame_period, opt[0].speed, fs);
+    if (rc) return rc;
+  }
   std::vector<int> fl;
   int rc = f0_lengths_from_x(n, x_stride, x_lengths, fs, opt->frame_period, f0_stride, &fl, &h->c.last_error);
   if (rc) return rc;
@@ -543,9 +608,21 @@ int world_b200_dio_batch(WorldB200 *h, const double *x, int n, int x_stride, con
   rc = upload_lengths(h, n, x_stride, x_lengths, f0_stride, fl.data(), &b);
   if (rc) return rc;
   b.x_len_host = x_lengths;
-  DioParams p = {opt->f0_floor, opt->f0_ceil, opt->channels_in_octave, opt->frame_period,
-                 opt->allowed_range, opt->speed};
-  return dio_run(&h->c, b, p, time_axis, f0);
+  std::vector<DioParams> p(per_utt ? (n > 0 ? n : 1) : 1);
+  for (size_t u = 0; u < p.size(); ++u)
+    p[u] = {opt[u].f0_floor, opt[u].f0_ceil, opt[u].channels_in_octave, opt[u].frame_period, opt[u].allowed_range,
+            opt[u].speed};
+  return dio_run(&h->c, b, p.data(), per_utt, time_axis, f0);
+}
+
+int world_b200_dio_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
+                         const DioOption *opt, double *time_axis, double *f0, int f0_stride) {
+  return dio_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, false, time_axis, f0, f0_stride);
+}
+
+int world_b200_dio_batch_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
+                                 const DioOption *dio_options, double *time_axis, double *f0, int f0_stride) {
+  return dio_batch_impl(h, x, n, x_stride, x_lengths, fs, dio_options, true, time_axis, f0, f0_stride);
 }
 
 // opt: one option for every utterance, or (per_utt) an array of n
@@ -554,7 +631,8 @@ static int harvest_batch_impl(WorldB200 *h, const double *x, int n, int x_stride
   if (!h || !x || !time_axis || !f0 || !opt || n < 0 || fs <= 0) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
   if (per_utt && n > 0) {
-    const int rc = check_harvest_options(&h->c, opt, n, opt[0].frame_period, 0);   // harvest_run checks the ranges
+    // every range too, before the lengths are uploaded: a bad option queues nothing on the device
+    const int rc = check_harvest_options(&h->c, opt, n, opt[0].frame_period, fs);
     if (rc) return rc;
   }
   std::vector<int> fl;
@@ -592,20 +670,17 @@ int world_b200_harvest_batch_options(WorldB200 *h, const double *x, int n, int x
 // gather = false: time_axis / f0 / spectrogram / aperiodicity hold this call's n utterances.
 // gather = true (multi-GPU): they are the FULL arrays of n_ranks * n utterances; this rank computes into block `rank`
 // and every finished slice is broadcast to the other ranks on the communication stream while the next one is computed.
-// harvest_options: nullptr, or one HarvestOption per utterance (f0_method HARVEST, frame_period = opt->harvest's)
+// harvest_options / dio_options: nullptr, or one option per utterance of the chain's F0 method (at most one of the two;
+// check_chain_f0_options); the slices split the array with the utterances.
 static int analyze_batch_impl(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
                               const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
-                              double *time_axis, double *f0, int f0_stride,
+                              const DioOption *dio_options, double *time_axis, double *f0, int f0_stride,
                               double *spectrogram, double *aperiodicity, bool gather) {
   if (!h || !x || !opt || !time_axis || !f0 || n < 0 || fs <= 0 || x_stride <= 0 || f0_stride <= 0) return WORLD_B200_EINVAL;
   if ((spectrogram || aperiodicity) && opt->cheaptrick.fft_size < 16) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
-  if (harvest_options) {
-    if (opt->f0_method != WORLD_B200_F0_HARVEST) {
-      h->c.last_error = "analyze_batch: per-utterance Harvest options need f0_method == WORLD_B200_F0_HARVEST";
-      return WORLD_B200_EINVAL;
-    }
-    const int rc = check_harvest_options(&h->c, harvest_options, n, opt->harvest.frame_period, fs);
+  {
+    const int rc = check_chain_f0_options(&h->c, opt, harvest_options, dio_options, n, fs, "analyze_batch");
     if (rc) return rc;
   }
   if (n == 0) return 0;
@@ -694,13 +769,8 @@ static int analyze_batch_impl(WorldB200 *h, const double *x, int n, int x_stride
     const double *xs = x + (size_t)u0 * x_stride;
     const int *xl = x_lengths ? x_lengths + u0 : nullptr;
     double *ts = time_axis + (size_t)u0 * f0_stride, *fs_ = f0 + (size_t)u0 * f0_stride;
-    if (opt->f0_method == WORLD_B200_F0_HARVEST) {
-      rc = harvest_options ? world_b200_harvest_batch_options(L, xs, m, x_stride, xl, fs, harvest_options + u0, ts, fs_, f0_stride)
-                           : world_b200_harvest_batch(L, xs, m, x_stride, xl, fs, &opt->harvest, ts, fs_, f0_stride);
-    } else {
-      rc = world_b200_dio_batch(L, xs, m, x_stride, xl, fs, &opt->dio, ts, fs_, f0_stride);
-      if (!rc) rc = world_b200_stonemask_batch(L, xs, m, x_stride, xl, fs, ts, fs_, fl.data() + u0, f0_stride, fs_);
-    }
+    rc = run_f0_stage(L, xs, m, x_stride, xl, fs, opt, harvest_options ? harvest_options + u0 : nullptr,
+                      dio_options ? dio_options + u0 : nullptr, fl.data() + u0, ts, fs_, f0_stride);
     if (!rc && spectrogram)
       rc = world_b200_cheaptrick_batch(L, xs, m, x_stride, xl, fs, ts, fs_, fl.data() + u0, f0_stride, &opt->cheaptrick,
                                        spectrogram + (size_t)u0 * f0_stride * bins);
@@ -743,8 +813,8 @@ static int analyze_batch_impl(WorldB200 *h, const double *x, int n, int x_stride
 int world_b200_analyze_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
                              const WorldB200AnalysisOption *opt, double *time_axis, double *f0, int f0_stride,
                              double *spectrogram, double *aperiodicity) {
-  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, nullptr, time_axis, f0, f0_stride, spectrogram,
-                            aperiodicity, false);
+  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, nullptr, nullptr, time_axis, f0, f0_stride,
+                            spectrogram, aperiodicity, false);
 }
 
 int world_b200_analyze_batch_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
@@ -752,7 +822,16 @@ int world_b200_analyze_batch_options(WorldB200 *h, const double *x, int n, int x
                                      double *time_axis, double *f0, int f0_stride, double *spectrogram,
                                      double *aperiodicity) {
   if (!harvest_options) return WORLD_B200_EINVAL;
-  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, harvest_options, time_axis, f0, f0_stride,
+  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, harvest_options, nullptr, time_axis, f0, f0_stride,
+                            spectrogram, aperiodicity, false);
+}
+
+int world_b200_analyze_batch_dio_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
+                                         int fs, const WorldB200AnalysisOption *opt, const DioOption *dio_options,
+                                         double *time_axis, double *f0, int f0_stride, double *spectrogram,
+                                         double *aperiodicity) {
+  if (!dio_options) return WORLD_B200_EINVAL;
+  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, nullptr, dio_options, time_axis, f0, f0_stride,
                             spectrogram, aperiodicity, false);
 }
 
@@ -807,7 +886,7 @@ int world_b200_allgather_rows(WorldB200 *h, double *full, unsigned long long row
 int world_b200_analyze_batch_allgather(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
                                        const WorldB200AnalysisOption *opt, double *time_axis_full, double *f0_full,
                                        int f0_stride, double *spectrogram_full, double *aperiodicity_full) {
-  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, nullptr, time_axis_full, f0_full, f0_stride,
+  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, nullptr, nullptr, time_axis_full, f0_full, f0_stride,
                             spectrogram_full, aperiodicity_full, true);
 }
 
@@ -817,8 +896,18 @@ int world_b200_analyze_batch_allgather_options(WorldB200 *h, const double *x, in
                                                double *f0_full, int f0_stride, double *spectrogram_full,
                                                double *aperiodicity_full) {
   if (!harvest_options) return WORLD_B200_EINVAL;
-  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, harvest_options, time_axis_full, f0_full, f0_stride,
-                            spectrogram_full, aperiodicity_full, true);
+  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, harvest_options, nullptr, time_axis_full, f0_full,
+                            f0_stride, spectrogram_full, aperiodicity_full, true);
+}
+
+int world_b200_analyze_batch_allgather_dio_options(WorldB200 *h, const double *x, int n, int x_stride,
+                                                   const int *x_lengths, int fs, const WorldB200AnalysisOption *opt,
+                                                   const DioOption *dio_options, double *time_axis_full,
+                                                   double *f0_full, int f0_stride, double *spectrogram_full,
+                                                   double *aperiodicity_full) {
+  if (!dio_options) return WORLD_B200_EINVAL;
+  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, nullptr, dio_options, time_axis_full, f0_full,
+                            f0_stride, spectrogram_full, aperiodicity_full, true);
 }
 
 // Per-kernel timing: enable, run, then fetch a JSON object {"kernel": {"launches": n, "ms": t}, ...}

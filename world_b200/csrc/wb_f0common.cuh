@@ -98,14 +98,15 @@ struct SweepParams {
   // complete edge lists to global memory) and band_interp_kernel (edge lists -> candidates on the frame grid).
   int *ev_count;          // [n][n_bands][4] events per train; ev_count[..][0] = -1 marks a band whose lists overflowed
   int *redo_list; int *redo_count;   // (utterance * n_bands + band) pairs for the streaming kernel (history rings)
-  // Harvest, one F0 range per utterance.  The per-band tables above (taps, tap_off, ntaps, shift, boundary, edge_cap,
+  // One F0 range per utterance (Harvest and DIO).  The per-band tables above (taps, tap_off, ntaps, shift, boundary, edge_cap,
   // edge_off) hold the band lists of every range group of the batch one after the other; utterance u uses group
   // g = ugrp[u]: bands grp_band0[g] .. grp_band0[g] + grp_nb[g] - 1 of the tables, floor / ceiling grp_floor[g] /
   // grp_ceil[g].  Band indices b elsewhere (cand rows, ev_count, redo_list) are the utterance's own 0 .. grp_nb - 1,
   // strided by n_bands = the batch maximum.  The grids are flat over the utterances' own bands (band pairs for
   // band_fir_events_kernel): blk0_band[u] / blk0_pair[u] is the first block of utterance u ([n_utts + 1] prefix sums,
   // totals n_blk_band / n_blk_pair), so the work follows the sum of the channel counts, not n x the largest.
-  // ugrp == nullptr (DIO): bands 0 .. n_bands - 1 and f0_floor / f0_ceil for every utterance, grid (band, utterance).
+  // ugrp == nullptr (one range for the batch): bands 0 .. n_bands - 1 and f0_floor / f0_ceil for every utterance, grid
+  // (band, utterance).
   const int *ugrp = nullptr; const int *grp_band0 = nullptr, *grp_nb = nullptr;
   const double *grp_floor = nullptr, *grp_ceil = nullptr;
   const int *blk0_band = nullptr, *blk0_pair = nullptr; int n_blk_band = 0, n_blk_pair = 0, n_utts = 0;

@@ -17,8 +17,12 @@
 using namespace wb;
 
 namespace wb {
-// wb_api.cu: frame_period and F0 range checks of per-utterance Harvest options
-int check_harvest_options(Ctx *c, const HarvestOption *opts, int n, double frame_period, int fs);
+// wb_api.cu: checks of per-utterance F0 options for a chain, and the chain's F0 stage
+int check_chain_f0_options(Ctx *c, const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
+                           const DioOption *dio_options, int n, int fs, const char *who);
+int run_f0_stage(WorldB200 *h, const double *x, int m, int x_stride, const int *x_lengths, int fs,
+                 const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options, const DioOption *dio_options,
+                 const int *f0_lengths, double *time_axis, double *f0, int f0_stride);
 }  // namespace wb
 
 namespace {
@@ -53,10 +57,12 @@ namespace {
 // un-overlapped tail is one sub-chunk.  Result buffers form a ring two outer chunks deep, so downloads
 // may lag behind the frame kernels and catch up under the next outer chunk's F0 stage.  Streams: s_in
 // (uploads), the context's stream (all kernels), s_out (downloads); events order buffer reuse.
-// harvest_options: nullptr, or one HarvestOption per utterance (checked by the caller); the chunks split the array.
+// harvest_options / dio_options: nullptr, or one option per utterance (checked by the caller, at most one of the two);
+// the outer chunks split the array.
 int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride, const int *x_lengths, int fs,
-                     const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options, int dims,
-                     double *time_axis, double *f0, int f0_stride, double *out_sp, double *out_ap) {
+                     const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
+                     const DioOption *dio_options, int dims, double *time_axis, double *f0, int f0_stride,
+                     double *out_sp, double *out_ap) {
   Ctx *ctx = ctx_of(h);
   const int bins = opt->cheaptrick.fft_size / 2 + 1;
   const int n_ap = GetNumberOfAperiodicities(fs);
@@ -195,13 +201,8 @@ int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_st
     dev_memset(ctx, df[s].p, 0, fsz * 8);
     const double *xd = (const double *)(nbit ? dx[s].p : din[s].p);
     double *td = (double *)dt[s].p, *fd = (double *)df[s].p;
-    if (opt->f0_method == WORLD_B200_F0_HARVEST) {
-      rc = harvest_options ? world_b200_harvest_batch_options(h, xd, n, x_stride, xl, fs, harvest_options + u0, td, fd, f0_stride)
-                           : world_b200_harvest_batch(h, xd, n, x_stride, xl, fs, &opt->harvest, td, fd, f0_stride);
-    } else {
-      rc = world_b200_dio_batch(h, xd, n, x_stride, xl, fs, &opt->dio, td, fd, f0_stride);
-      if (!rc) rc = world_b200_stonemask_batch(h, xd, n, x_stride, xl, fs, td, fd, fl, f0_stride, fd);
-    }
+    rc = run_f0_stage(h, xd, n, x_stride, xl, fs, opt, harvest_options ? harvest_options + u0 : nullptr,
+                      dio_options ? dio_options + u0 : nullptr, fl, td, fd, f0_stride);
     if (rc) break;
 #ifndef WB_EMU
     cudaEventRecord(ev_f0[s], s_compute);
@@ -331,31 +332,47 @@ extern "C" int world_b200_analyze_host(WorldB200 *h, const double *x, int n_utts
                                        double *aperiodicity) {
   if (!h || !x || !opt || n_utts < 0 || fs <= 0 || x_stride <= 0 || f0_stride <= 0) return WORLD_B200_EINVAL;
   DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  return analyze_pipeline(h, x, 0, n_utts, x_stride, x_lengths, fs, opt, nullptr, 0, time_axis, f0, f0_stride, spectrogram,
-                          aperiodicity);
+  return analyze_pipeline(h, x, 0, n_utts, x_stride, x_lengths, fs, opt, nullptr, nullptr, 0, time_axis, f0, f0_stride,
+                          spectrogram, aperiodicity);
+}
+
+// analyze_host with per-utterance options of one F0 method (harvest_options or dio_options)
+static int analyze_host_per_utt(WorldB200 *h, const double *x, int n_utts, int x_stride, const int *x_lengths, int fs,
+                                const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
+                                const DioOption *dio_options, double *time_axis, double *f0, int f0_stride,
+                                double *spectrogram, double *aperiodicity) {
+  if (!h || !x || !opt || n_utts < 0 || fs <= 0 || x_stride <= 0 || f0_stride <= 0) return WORLD_B200_EINVAL;
+  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
+  const int rc = check_chain_f0_options(ctx_of(h), opt, harvest_options, dio_options, n_utts, fs, "analyze_host");
+  if (rc) return rc;
+  return analyze_pipeline(h, x, 0, n_utts, x_stride, x_lengths, fs, opt, harvest_options, dio_options, 0, time_axis, f0,
+                          f0_stride, spectrogram, aperiodicity);
 }
 
 extern "C" int world_b200_analyze_host_options(WorldB200 *h, const double *x, int n_utts, int x_stride,
                                                const int *x_lengths, int fs, const WorldB200AnalysisOption *opt,
                                                const HarvestOption *harvest_options, double *time_axis, double *f0,
                                                int f0_stride, double *spectrogram, double *aperiodicity) {
-  if (!h || !x || !opt || !harvest_options || n_utts < 0 || fs <= 0 || x_stride <= 0 || f0_stride <= 0)
-    return WORLD_B200_EINVAL;
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  if (opt->f0_method != WORLD_B200_F0_HARVEST) {
-    ctx_of(h)->last_error = "analyze_host: per-utterance Harvest options need f0_method == WORLD_B200_F0_HARVEST";
-    return WORLD_B200_EINVAL;
-  }
-  const int rc = check_harvest_options(ctx_of(h), harvest_options, n_utts, opt->harvest.frame_period, fs);
-  if (rc) return rc;
-  return analyze_pipeline(h, x, 0, n_utts, x_stride, x_lengths, fs, opt, harvest_options, 0, time_axis, f0, f0_stride,
-                          spectrogram, aperiodicity);
+  if (!harvest_options) return WORLD_B200_EINVAL;
+  return analyze_host_per_utt(h, x, n_utts, x_stride, x_lengths, fs, opt, harvest_options, nullptr, time_axis, f0,
+                              f0_stride, spectrogram, aperiodicity);
 }
 
-extern "C" int world_b200_analyze_coded_host(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride,
-                                             const int *x_lengths, int fs, const WorldB200AnalysisOption *opt,
-                                             int number_of_dimensions, double *time_axis, double *f0, int f0_stride,
-                                             double *coded_spectral_envelope, double *coded_aperiodicity) {
+extern "C" int world_b200_analyze_host_dio_options(WorldB200 *h, const double *x, int n_utts, int x_stride,
+                                                   const int *x_lengths, int fs, const WorldB200AnalysisOption *opt,
+                                                   const DioOption *dio_options, double *time_axis, double *f0,
+                                                   int f0_stride, double *spectrogram, double *aperiodicity) {
+  if (!dio_options) return WORLD_B200_EINVAL;
+  return analyze_host_per_utt(h, x, n_utts, x_stride, x_lengths, fs, opt, nullptr, dio_options, time_axis, f0,
+                              f0_stride, spectrogram, aperiodicity);
+}
+
+// analyze_coded_host with per-utterance options of one F0 method, or none (both nullptr)
+static int analyze_coded_host_impl(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride, const int *x_lengths,
+                                   int fs, const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
+                                   const DioOption *dio_options, int number_of_dimensions, double *time_axis,
+                                   double *f0, int f0_stride, double *coded_spectral_envelope,
+                                   double *coded_aperiodicity) {
   if (!h || !x || !opt || n_utts < 0 || fs <= 0 || x_stride <= 0 || f0_stride <= 0) return WORLD_B200_EINVAL;
   DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
   if (nbit != 0 && nbit != 8 && nbit != 16 && nbit != 24 && nbit != 32) return WORLD_B200_EINVAL;
@@ -363,8 +380,42 @@ extern "C" int world_b200_analyze_coded_host(WorldB200 *h, const void *x, int nb
     ctx_of(h)->last_error = "analyze_coded_host: number_of_dimensions must be in [1, fft_size/4 + 1]";
     return WORLD_B200_EINVAL;
   }
-  return analyze_pipeline(h, x, nbit, n_utts, x_stride, x_lengths, fs, opt, nullptr, number_of_dimensions, time_axis, f0,
-                          f0_stride, coded_spectral_envelope, coded_aperiodicity);
+  const int rc = check_chain_f0_options(ctx_of(h), opt, harvest_options, dio_options, n_utts, fs, "analyze_coded_host");
+  if (rc) return rc;
+  return analyze_pipeline(h, x, nbit, n_utts, x_stride, x_lengths, fs, opt, harvest_options, dio_options,
+                          number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope, coded_aperiodicity);
+}
+
+extern "C" int world_b200_analyze_coded_host(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride,
+                                             const int *x_lengths, int fs, const WorldB200AnalysisOption *opt,
+                                             int number_of_dimensions, double *time_axis, double *f0, int f0_stride,
+                                             double *coded_spectral_envelope, double *coded_aperiodicity) {
+  return analyze_coded_host_impl(h, x, nbit, n_utts, x_stride, x_lengths, fs, opt, nullptr, nullptr,
+                                 number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope,
+                                 coded_aperiodicity);
+}
+
+extern "C" int world_b200_analyze_coded_host_options(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride,
+                                                     const int *x_lengths, int fs, const WorldB200AnalysisOption *opt,
+                                                     const HarvestOption *harvest_options, int number_of_dimensions,
+                                                     double *time_axis, double *f0, int f0_stride,
+                                                     double *coded_spectral_envelope, double *coded_aperiodicity) {
+  if (!harvest_options) return WORLD_B200_EINVAL;
+  return analyze_coded_host_impl(h, x, nbit, n_utts, x_stride, x_lengths, fs, opt, harvest_options, nullptr,
+                                 number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope,
+                                 coded_aperiodicity);
+}
+
+extern "C" int world_b200_analyze_coded_host_dio_options(WorldB200 *h, const void *x, int nbit, int n_utts,
+                                                         int x_stride, const int *x_lengths, int fs,
+                                                         const WorldB200AnalysisOption *opt,
+                                                         const DioOption *dio_options, int number_of_dimensions,
+                                                         double *time_axis, double *f0, int f0_stride,
+                                                         double *coded_spectral_envelope, double *coded_aperiodicity) {
+  if (!dio_options) return WORLD_B200_EINVAL;
+  return analyze_coded_host_impl(h, x, nbit, n_utts, x_stride, x_lengths, fs, opt, nullptr, dio_options,
+                                 number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope,
+                                 coded_aperiodicity);
 }
 
 // ------------------------------------------------------------------ legacy single-utterance API

@@ -153,7 +153,11 @@ int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *ap
             const CodecTables *coded = nullptr, double *coded_out = nullptr);
 int stonemask_run(Ctx *ctx, const Batch &b, double *refined_f0);
 struct DioParams { double f0_floor, f0_ceil, channels_in_octave, frame_period, allowed_range; int speed; };
-int dio_run(Ctx *ctx, const Batch &b, const DioParams &p, double *time_axis_out, double *f0_out);
+// per_utt: opts[u] is utterance u's option (f0_floor / f0_ceil / channels_in_octave / allowed_range may differ,
+// frame_period and speed may not); else opts[0] for all
+int dio_run(Ctx *ctx, const Batch &b, const DioParams *opts, bool per_utt, double *time_axis_out, double *f0_out);
+// the range checks of dio_run for n per-utterance options; 3 (EINVAL) + last_error naming the first bad utterance
+int dio_check_options(Ctx *ctx, int fs, const DioParams *opts, int n);
 struct HarvestParams { double f0_floor, f0_ceil, frame_period; };
 // per_utt: opts[u] is utterance u's option (f0_floor / f0_ceil may differ, frame_period may not); else opts[0] for all
 int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_utt, double *time_axis_out, double *f0_out);
