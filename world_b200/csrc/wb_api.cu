@@ -236,14 +236,19 @@ int ctx_init_tables(Ctx *ctx) {
     tw[k].x = (double)cosl(a);
     tw[k].y = (double)(-sinl(a));
   }
+  std::vector<double2> tw_sized(WB_TW_SIZED_ENTRIES);
+  for (int lg = 1; lg <= WB_TW_LOG2; ++lg)
+    for (int n = 0; n < (1 << (lg - 1)); ++n) tw_sized[tw_sized_offset(lg) + n] = tw[n << (WB_TW_LOG2 - lg)];
   ctx->twiddle = (double2 *)dev_malloc(ctx, tw.size() * sizeof(double2));
-  if (!ctx->twiddle) return WORLD_B200_ENOMEM;
+  ctx->twiddle_sized = (double2 *)dev_malloc(ctx, tw_sized.size() * sizeof(double2));
+  if (!ctx->twiddle || !ctx->twiddle_sized) return WORLD_B200_ENOMEM;
   std::vector<uint32_t> jump((size_t)WB_RNG_NJ * 32 * 16 * 4);
   rng_build_jump_tables(jump.data());
   ctx->rng_jump = (uint32_t *)dev_malloc(ctx, jump.size() * 4);
   ctx->status_dev = (int *)dev_malloc(ctx, sizeof(int));
   if (!ctx->rng_jump || !ctx->status_dev) return WORLD_B200_ENOMEM;
   int rc = dev_memcpy_h2d(ctx, ctx->twiddle, tw.data(), tw.size() * sizeof(double2));
+  if (!rc) rc = dev_memcpy_h2d(ctx, ctx->twiddle_sized, tw_sized.data(), tw_sized.size() * sizeof(double2));
   if (!rc) rc = dev_memcpy_h2d(ctx, ctx->rng_jump, jump.data(), jump.size() * 4);
   if (!rc) rc = dev_memset(ctx, ctx->status_dev, 0, sizeof(int));
   if (!rc) rc = dev_sync(ctx);
@@ -430,6 +435,7 @@ void world_b200_destroy(WorldB200 *h) {
 #endif
   if (h->comm) comm_destroy(h->comm);
   dev_free(h->c.twiddle);
+  dev_free(h->c.twiddle_sized);
   dev_free(h->c.rng_jump);
   dev_free(h->c.status_dev);
   dev_free(h->c.arena.base);

@@ -34,6 +34,7 @@ struct D4cParams {
   int pw_doubles;                    // doubles of the fast body kernel's power row (d4c_body_pw_doubles)
   double *out;
   const double2 *tw;
+  const double2 *tw_body;   // compact twiddles of size d_fft (tw_sized_offset): the fast body kernel's
   int *status;
   // coded output (CodeAperiodicity, codec.cpp:228-238): with c_out set the kernels write the dB value at the c_n
   // band centres instead of the ct_fft_size/2+1 bins
@@ -335,7 +336,7 @@ WB_DEV bool select_kth_largest_fast(const double *a, int n, int kth, unsigned lo
 //     split of the two real spectra pairs up, have the same parity).  The windowed signal waits in the power row.
 // Frames whose window is longer than the power row (d4c_body_pw_doubles: f0 near the 47 Hz floor) go to slow_list
 // and are done by d4c_body_slow_kernel (the round-1 body on the in-place DIT FFT, any window length), as is every
-// frame when d_fft > 4096 (this kernel's thread count would not fit a CTA).
+// frame when d_fft is above 4096 or below 512 (this kernel's thread count would not fit a CTA, or fill a warp).
 // Doubles of the power row.  It also holds the windowed signal of the centroid transforms, whose longest window (f0
 // at the 47 Hz floor, ratio 4) is up to twice d_fft / 2 + 1; shared memory per CTA decides how many CTAs an SM holds
 // and the kernel is latency bound (sizing the row for the longest window costs a CTA per SM at 48 kHz), so the row grows only as far as the CTA count of the minimal layout allows.  Frames with
@@ -356,7 +357,10 @@ WB_HD inline int d4c_body_pw_doubles(int d_fft, int fs, int n_ap, int threads) {
   return imax(half1, imin(nwin_max + 1, grown));
 }
 
-template <int kOcc>   // CTAs of 128 threads per SM the register budget is cut for (A/B: WB_D4C_OCC)
+// kLg = log2(d_fft), 9..12: the transforms are sfft_forward_fixed at compile-time size on d_fft / 16 threads, with the
+// compact twiddle table p.tw_body of size d_fft (every twiddle the frame reads: the passes, the real-FFT unpack and the
+// centroid's DIF split)
+template <int kLg>
 WB_DEV void d4c_body_frame(const D4cParams &p) {
   WB_DYN_SMEM(double2, smem2);
   const int tid = WB_TID, nth = WB_NTH;
@@ -364,7 +368,9 @@ WB_DEV void d4c_body_frame(const D4cParams &p) {
   if (i >= p.f_len[u]) return;
   const size_t fidx = (size_t)u * p.f_stride + i;
   if (!p.selected[fidx]) return;
-  const int N = p.d_fft, half = N / 2, fs = p.fs;
+  constexpr int N = 1 << kLg, half = N / 2;
+  const int fs = p.fs;
+  const double2 *__restrict__ twc = p.tw_body;
   const int slots = WB_FPAD_SLOTS(half);
   double2 *P = smem2;
   double *pd = reinterpret_cast<double *>(P);            // the same buffer as 2 * slots plain doubles
@@ -395,8 +401,6 @@ WB_DEV void d4c_body_frame(const D4cParams &p) {
   const double *x = p.x + (size_t)u * p.x_stride;
   const int x_len = p.x_len[u];
   const unsigned *draw = p.draws + (size_t)u * p.draw_stride + p.off_b[fidx];
-  const int lgh = p.d_lg - 1;              // log2(half)
-  const int tw_shift = WB_TW_LOG2 - p.d_lg;
 
   // ---- static centroid = centroid(t - 1/4f) + centroid(t + 1/4f)   (d4c.cpp:90-140)
   for (int pass = 0; pass < 2; ++pass) {
@@ -413,10 +417,10 @@ WB_DEV void d4c_body_frame(const D4cParams &p) {
         double2 z0 = make_double2(0.0, 0.0), z1 = make_double2(0.0, 0.0);
         if (n < nwin) { const double v = pw[n] / rt; z0 = make_double2(v, v * (n + 1.0)); }
         if (n + half < nwin) { const double v = pw[n + half] / rt; z1 = make_double2(v, v * (n + half + 1.0)); }
-        P[fpad(n)] = part == 0 ? cadd(z0, z1) : cmul(__ldg(&p.tw[n << tw_shift]), csub(z0, z1));
+        P[fpad(n)] = part == 0 ? cadd(z0, z1) : cmul(__ldg(&twc[n]), csub(z0, z1));
       }
       WB_SYNC();
-      sfft_forward_inplace(P, lgh, p.tw);
+      sfft_forward_fixed<kLg - 1>(P, twc);
       // bins k = 2 m + part; partner N - k = 2 (half - m - part) + part.  A = spectrum of v, B = of (n+1) v
       for (int m = tid; 2 * m + part <= half; m += nth) {
         const double2 zp = P[fpad(m)], zq = P[fpad((half - m - part) & (half - 1))];
@@ -437,8 +441,8 @@ WB_DEV void d4c_body_frame(const D4cParams &p) {
                                   [&](int j) { return pw + j; }, red);
     for (int j = nwin + tid; j < N; j += nth) pd[rpad(j)] = 0.0;
     WB_SYNC();
-    sfft_forward_inplace(P, lgh, p.tw);
-    rfft_unpack(P, p.d_lg, p.tw, [&](int k, double2 c) { pw[k] = c.x * c.x + c.y * c.y; });
+    sfft_forward_fixed<kLg - 1>(P, twc);
+    rfft_unpack(P, kLg, twc, [&](int k, double2 c) { pw[k] = c.x * c.x + c.y * c.y; }, kLg);
     WB_SYNC();
     dc_correction(pw, f, fs, N, pd);
     if (!linear_smoothing<false>(pw, f, fs, N, pw, pd, red_big)) {
@@ -465,26 +469,24 @@ WB_DEV void d4c_body_frame(const D4cParams &p) {
     for (int j = tid; j < N; j += nth)
       pd[rpad(j)] = (j <= half_w * 2) ? pw[center - half_w + j] * __ldg(&p.nuttall[j]) : 0.0;
     WB_SYNC();
-    sfft_forward_inplace(P, lgh, p.tw);
+    sfft_forward_fixed<kLg - 1>(P, twc);
     double tot = 0.0;
-    rfft_unpack(P, p.d_lg, p.tw, [&](int k, double2 c) {
+    rfft_unpack(P, kLg, twc, [&](int k, double2 c) {
       const double v = c.x * c.x + c.y * c.y;
       cent[k] = v;
       tot += v;
-    });
+    }, kLg);
     tot = block_sum(tot, red);  // contains the barrier that publishes cent[]
     const int n_small = half - p.bd;  // entries in the sorted prefix, index half-bd-1 inclusive
     double kth;
     // the FFT buffer is idle: candidate scratch (nth + WB_SEL_CAP + 4 words <= 2 * slots)
     if (!select_kth_largest_fast(cent, half + 1, p.bd + 1, reinterpret_cast<unsigned long long *>(pd), &kth))
       kth = select_kth_largest(cent, half + 1, p.bd + 1, red);
-    double below = 0.0;
-    int n_below = 0;
+    double below = 0.0, n_below = 0.0;   // the count is exact in a double: one reduction for both
     for (int k = tid; k <= half; k += nth)
-      if (cent[k] < kth) { below += cent[k]; ++n_below; }
-    below = block_sum(below, red);
-    n_below = block_sum_int(n_below, red);
-    const double small = below + (double)(n_small - n_below) * kth;
+      if (cent[k] < kth) { below += cent[k]; n_below += 1.0; }
+    block_sum2(below, n_below, red);
+    const double small = below + (double)(n_small - (int)n_below) * kth;
     if (tid == 0) {
       const double c = 10.0 * log10(small / tot);
       coarse[b + 1] = dmin(0.0, c + (f - 100.0) / 50.0);  // d4c.cpp:314-316
@@ -498,12 +500,22 @@ WB_DEV void d4c_body_frame(const D4cParams &p) {
   d4c_write_frame<true>(p, fidx, coarse);
 }
 
-#ifndef WB_EMU
-__global__ void __launch_bounds__(256, 3) d4c_body_kernel(D4cParams p) { d4c_body_frame<6>(p); }      // 80 registers
-__global__ void __launch_bounds__(256, 2) d4c_body_kernel_r128(D4cParams p) { d4c_body_frame<4>(p); } // 128 registers
-#else
-void d4c_body_kernel(D4cParams p) { d4c_body_frame<6>(p); }
-#endif
+// d_fft / 16 threads; the register budget (80) of 768 threads per SM -- six CTAs at 16 kHz, as many as the shared
+// memory holds
+template <int kLg>
+WB_KERNEL(1 << (kLg - 4), 768 >> (kLg - 4)) d4c_body_kernel_lg(D4cParams p) { d4c_body_frame<kLg>(p); }
+
+typedef void (*D4cBodyKernel)(D4cParams);
+// nullptr: no fast body kernel at this size (d_fft below 512 or above 4096)
+static D4cBodyKernel d4c_body_kernel_for(int d_lg) {
+  switch (d_lg) {
+    case 9: return d4c_body_kernel_lg<9>;
+    case 10: return d4c_body_kernel_lg<10>;
+    case 11: return d4c_body_kernel_lg<11>;
+    case 12: return d4c_body_kernel_lg<12>;
+    default: return nullptr;
+  }
+}
 
 // ------------------------------------------------------------------ pass B, any window length (round-1 body, in-place DIT FFT)
 // Persistent kernel over slow_list (frames the fast kernel handed over); with d_fft > 4096 (fs above 48.1 kHz: the
@@ -631,7 +643,7 @@ WB_KERNEL(256, 2) d4c_body_slow_kernel(D4cParams p) {
   }
 }
 
-// d_fft > 4096: every selected frame goes through the list
+// no fast body kernel at this d_fft: every selected frame goes through the list
 WB_KERNEL_PLAIN d4c_list_all_kernel(D4cParams p, int n_utts) {
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= (long long)n_utts * p.f_stride) return;
@@ -686,9 +698,11 @@ int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *ap
   const size_t draw_stride_full = (max_a + max_b) * (size_t)b.max_f_len;
   const size_t per_utt_bytes = draw_stride_full * 4 + (size_t)b.f_stride * 28 + 64;
   int chunk = balanced_chunk(imin(b.n, 65535), (int)dmin(65535.0, (double)ctx->scratch_budget / (double)per_utt_bytes));
-  // fast body kernel: one radix-8 butterfly per thread in the passes of the d_fft / 2 complex transforms
-  const bool all_slow = p.d_fft > 4096;   // d_fft / 16 threads would exceed the kernel's launch bounds
-  int body_threads = imax(32, p.d_fft / 16), lt_threads = 128, slow_threads = 128;
+  // fast body kernel: one radix-8 butterfly per thread in the passes of the d_fft / 2 complex transforms; at d_fft
+  // above 4096 its thread count would exceed a CTA, below 512 a warp
+  const D4cBodyKernel d4c_body_kernel = d4c_body_kernel_for(p.d_lg);
+  const bool all_slow = d4c_body_kernel == nullptr;
+  int body_threads = p.d_fft / 16, lt_threads = 128, slow_threads = 128;
   if (const char *e = getenv("WB_LT_THREADS")) lt_threads = atoi(e);
   const size_t smem_lt = (size_t)2 * WB_FPAD_SLOTS(p.lt_fft / 2) * sizeof(double2) + WB_RED_DOUBLES * sizeof(double);
   p.pw_doubles = d4c_body_pw_doubles(p.d_fft, fs, p.n_ap, body_threads);
@@ -697,9 +711,7 @@ int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *ap
                                     (slow_threads + 1) + (p.n_ap + 2) + 2) * sizeof(double);
 #ifndef WB_EMU
   cudaFuncSetAttribute(d4c_lovetrain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_lt);
-  cudaFuncSetAttribute(d4c_body_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_body);
-  cudaFuncSetAttribute(d4c_body_kernel_r128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_body);
-  const bool fat_regs = getenv("WB_D4C_FAT") != nullptr;
+  if (!all_slow) cudaFuncSetAttribute(d4c_body_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_body);
   cudaFuncSetAttribute(d4c_body_slow_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_slow);
 #endif
   int rc = 0;
@@ -733,6 +745,7 @@ int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *ap
     p.off_a = off_a; p.count_b = count_b; p.off_b = off_b; p.selected = selected;
     p.out = aperiodicity ? aperiodicity + (size_t)u0 * b.f_stride * bins : nullptr;
     p.tw = ctx->twiddle; p.status = ctx->status_dev;
+    p.tw_body = ctx->twiddle_sized + tw_sized_offset(p.d_lg);
     if (coded) {
       rc = dev_memcpy_h2d(ctx, blk + o_cidx, coded->idx.data(), n_tab * 4);
       if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_cfrac, coded->frac.data(), n_tab * 8);
@@ -755,16 +768,8 @@ int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *ap
     if (all_slow)
       WB_LAUNCH_FLAT(d4c_list_all_kernel, dim3((unsigned)((slots + 255) / 256)), 256, 0, ctx->stream, p, n);
     else
-    {
-#ifndef WB_EMU
-      if (fat_regs)
-        WB_LAUNCH_COOP(d4c_body_kernel_r128, dim3((unsigned)b.max_f_len, (unsigned)n), body_threads, smem_body,
-                       ctx->stream, p);
-      else
-#endif
       WB_LAUNCH_COOP(d4c_body_kernel, dim3((unsigned)b.max_f_len, (unsigned)n), body_threads, smem_body,
                      ctx->stream, p);
-    }
     // long windows (f0 near the floor): persistent CTAs over the list the fast kernel filled, usually empty
     WB_LAUNCH_COOP(d4c_body_slow_kernel, dim3((unsigned)(2 * ctx->sm_count)), slow_threads, smem_slow, ctx->stream, p);
     rc = dev_check(ctx, "d4c");

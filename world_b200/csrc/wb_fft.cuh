@@ -293,99 +293,104 @@ WB_DEV double2 *sfft_forward(double2 *a, double2 *b, int lg, const double2 *__re
   return src;
 }
 
-// Same transform in ONE padded buffer: every thread keeps the (at most) eight values it owns in a pass in
-// registers -- load, barrier, butterflies + store, barrier.  Two barriers per pass instead of one, half the shared
-// memory (more CTAs per SM for the barrier-heavy frame kernels).  Needs 2^lg <= 8 * blockDim.x.  Natural order in,
-// natural order out, result in `a`; the caller must have made `a` visible; ends with a barrier.
-WB_DEV_NOINLINE void sfft_forward_inplace(double2 *a, int lg, const double2 *__restrict__ tw) {
+// Compact twiddle tables (Ctx::twiddle_sized): for every transform size N = 2^L, 1 <= L <= WB_TW_LOG2, the N/2
+// entries W_N^n = tw[n << (WB_TW_LOG2 - L)], n < N/2, stored contiguously from tw_sized_offset(L) on.  The values are
+// those of the full table; a kernel that works at one size reads N/2 * 16 contiguous bytes instead of every
+// 2^(WB_TW_LOG2 - L)-th entry of the full table, which spreads the same entries over that many times the cache lines.
+#define WB_TW_SIZED_ENTRIES (WB_TW_N - 1)
+WB_HD inline int tw_sized_offset(int lg) { return (1 << (lg - 1)) - 1; }
+
+// sfft_forward in ONE padded buffer, at a compile-time size: 2^kLgH complex values, run by exactly 2^kLgH / 8 threads
+// (one radix-8 butterfly per thread and pass).  Every thread keeps the values it owns in a pass in registers -- load,
+// barrier, butterflies + store, barrier: two barriers per pass instead of one, half the shared memory (more CTAs per SM
+// for the barrier-heavy frame kernels).  The pass structure is fixed at compile time and nothing is called (a
+// __noinline__ transform made its callers save and restore their live registers through local memory).
+// tw: the compact table of size 2^(kLgH + 1) (tw_sized_offset(kLgH + 1)).  Natural order in and out, result in `a`;
+// the caller must have made `a` visible; ends with a barrier.  Same butterflies and twiddle values as sfft_forward,
+// so the same result bit for bit; the emulation runs the same butterflies with the loads of a
+// pass taken from a copy of the buffer (what the barrier between loads and stores gives the GPU).
+template <int kR>
+WB_DEV void sfft_fixed_load(const double2 *src, int i, int T, double2 (&x)[kR]) {
+  if constexpr (kR == 8) {   // bit-reversed slot order (radix8_butterfly)
+    x[0] = src[fpad(i)];         x[4] = src[fpad(i + T)];     x[2] = src[fpad(i + 2 * T)]; x[6] = src[fpad(i + 3 * T)];
+    x[1] = src[fpad(i + 4 * T)]; x[5] = src[fpad(i + 5 * T)]; x[3] = src[fpad(i + 6 * T)]; x[7] = src[fpad(i + 7 * T)];
+  } else {
+#pragma unroll
+    for (int r = 0; r < kR; ++r) x[r] = src[fpad(i + r * T)];
+  }
+}
+
+template <int kLgH, int kLgp, int kR>
+WB_DEV void sfft_fixed_store(double2 *dst, int i, double2 (&x)[kR], const double2 *__restrict__ tw) {
+  constexpr int p = 1 << kLgp;
+  constexpr int lgr = kR == 8 ? 3 : (kR == 4 ? 2 : 1);
+  constexpr int tws = kLgH + 1 - kLgp - lgr;   // W_{R p}^k = W_{2^(kLgH + 1)}^(k << tws)
+  const int k = i & (p - 1), j = ((i - k) << lgr) + k;
+  if constexpr (kR == 8) {
+    if constexpr (kLgp == 0) radix8_butterfly<false>(x, make_double2(1.0, 0.0));
+    else radix8_butterfly<true>(x, __ldg(&tw[k << tws]));
+#pragma unroll
+    for (int m = 0; m < kR; ++m) dst[fpad(j + m * p)] = x[m];
+  } else if constexpr (kR == 4) {
+    const double2 b = __ldg(&tw[k << tws]);
+    const double2 aa = cmul(b, b);
+    const double2 t2 = cmul(aa, x[2]), t3 = cmul(aa, x[3]);
+    const double2 y0 = cadd(x[0], t2), y1 = csub(x[0], t2), y2 = cadd(x[1], t3), y3 = csub(x[1], t3);
+    const double2 v2 = cmul(b, y2), v3 = mul_mj(cmul(b, y3));
+    dst[fpad(j)] = cadd(y0, v2);     dst[fpad(j + 2 * p)] = csub(y0, v2);
+    dst[fpad(j + p)] = cadd(y1, v3); dst[fpad(j + 3 * p)] = csub(y1, v3);
+  } else {
+    const double2 v = cmul(__ldg(&tw[k << tws]), x[1]);
+    dst[fpad(j)] = cadd(x[0], v);
+    dst[fpad(j + p)] = csub(x[0], v);
+  }
+}
+
+template <int kLgH, int kLgp, int kR>
+WB_DEV void sfft_fixed_pass(double2 *a, const double2 *__restrict__ tw) {
+  constexpr int n = 1 << kLgH, T = n / kR;
 #ifdef WB_EMU
-  // one emulated thread: run the ping-pong passes against a scratch buffer (same arithmetic), copy back
-  static double2 tmp[WB_FPAD_SLOTS(WB_TW_N)];
-  double2 *r = sfft_forward(a, tmp, lg, tw);
-  if (r != a) for (int i = 0; i < WB_FPAD_SLOTS(1 << lg); ++i) a[i] = r[i];
+  static double2 src[WB_FPAD_SLOTS(n)];
+  for (int s = 0; s < WB_FPAD_SLOTS(n); ++s) src[s] = a[s];
+  for (int i = 0; i < T; ++i) {
+    double2 x[kR];
+    sfft_fixed_load<kR>(src, i, T, x);
+    sfft_fixed_store<kLgH, kLgp, kR>(a, i, x, tw);
+  }
 #else
-  const int tid = threadIdx.x, nth = blockDim.x;
-  const int n = 1 << lg;
-  int lgp = 0;
-  if (lg >= 3) {
-    const int T = n >> 3;
-    for (; lg - lgp >= 3; lgp += 3) {
-      const int p = 1 << lgp, i = tid;
-      double2 x[8];
-      if (i < T) {
-        x[0] = a[fpad(i)];         x[4] = a[fpad(i + T)];     x[2] = a[fpad(i + 2 * T)]; x[6] = a[fpad(i + 3 * T)];
-        x[1] = a[fpad(i + 4 * T)]; x[5] = a[fpad(i + 5 * T)]; x[3] = a[fpad(i + 6 * T)]; x[7] = a[fpad(i + 7 * T)];
-      }
-      __syncthreads();
-      if (i < T) {
-        const int k = i & (p - 1), j = ((i - k) << 3) + k;
-        if (lgp == 0) {
-          radix8_butterfly<false>(x, make_double2(1.0, 0.0));
-        } else {
-          radix8_butterfly<true>(x, __ldg(&tw[k << (WB_TW_LOG2 - lgp - 3)]));
-        }
+  constexpr int kPer = 8 / kR;   // butterflies per thread: n / 8 threads
+  double2 x[kPer][kR];
 #pragma unroll
-        for (int m = 0; m < 8; ++m) a[fpad(j + m * p)] = x[m];
-      }
-      __syncthreads();
-    }
-  }
-  if (lg - lgp == 2) {
-    const int T = n >> 2, p = 1 << lgp;
-    double2 u[2][4];
+  for (int q = 0; q < kPer; ++q) sfft_fixed_load<kR>(a, threadIdx.x + q * (n >> 3), T, x[q]);
+  __syncthreads();
 #pragma unroll
-    for (int q = 0; q < 2; ++q) {
-      const int i = tid + q * nth;
-      if (i < T) { u[q][0] = a[fpad(i)]; u[q][1] = a[fpad(i + T)]; u[q][2] = a[fpad(i + 2 * T)]; u[q][3] = a[fpad(i + 3 * T)]; }
-    }
-    __syncthreads();
-#pragma unroll
-    for (int q = 0; q < 2; ++q) {
-      const int i = tid + q * nth;
-      if (i < T) {
-        const int k = i & (p - 1), j = ((i - k) << 2) + k;
-        const double2 b = __ldg(&tw[k << (WB_TW_LOG2 - lgp - 2)]);
-        const double2 aa = cmul(b, b);
-        const double2 t2 = cmul(aa, u[q][2]), t3 = cmul(aa, u[q][3]);
-        const double2 y0 = cadd(u[q][0], t2), y1 = csub(u[q][0], t2), y2 = cadd(u[q][1], t3), y3 = csub(u[q][1], t3);
-        const double2 v2 = cmul(b, y2), v3 = mul_mj(cmul(b, y3));
-        a[fpad(j)] = cadd(y0, v2);     a[fpad(j + 2 * p)] = csub(y0, v2);
-        a[fpad(j + p)] = cadd(y1, v3); a[fpad(j + 3 * p)] = csub(y1, v3);
-      }
-    }
-    __syncthreads();
-  } else if (lg - lgp == 1) {
-    const int T = n >> 1, p = 1 << lgp;
-    double2 u[4][2];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const int i = tid + q * nth;
-      if (i < T) { u[q][0] = a[fpad(i)]; u[q][1] = a[fpad(i + T)]; }
-    }
-    __syncthreads();
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const int i = tid + q * nth;
-      if (i < T) {
-        const int k = i & (p - 1), j = ((i - k) << 1) + k;
-        const double2 v = cmul(__ldg(&tw[k << (WB_TW_LOG2 - lgp - 1)]), u[q][1]);
-        a[fpad(j)] = cadd(u[q][0], v);
-        a[fpad(j + p)] = csub(u[q][0], v);
-      }
-    }
-    __syncthreads();
-  }
+  for (int q = 0; q < kPer; ++q) sfft_fixed_store<kLgH, kLgp, kR>(a, threadIdx.x + q * (n >> 3), x[q], tw);
+  __syncthreads();
 #endif
+}
+
+template <int kLgH, int kLgp = 0>
+WB_DEV void sfft_forward_fixed(double2 *a, const double2 *__restrict__ tw) {
+  static_assert(kLgH >= 3, "one radix-8 butterfly per thread needs at least 8 values");
+  if constexpr (kLgH - kLgp >= 3) {
+    sfft_fixed_pass<kLgH, kLgp, 8>(a, tw);
+    sfft_forward_fixed<kLgH, kLgp + 3>(a, tw);
+  } else if constexpr (kLgH - kLgp == 2) {
+    sfft_fixed_pass<kLgH, kLgp, 4>(a, tw);
+  } else if constexpr (kLgH - kLgp == 1) {
+    sfft_fixed_pass<kLgH, kLgp, 2>(a, tw);
+  }
 }
 
 // Real FFT on top: the N = 2^lg real samples were packed two per slot (sample e at rpad(e)) and transformed as
 // N/2 complex values by sfft_forward -> z.  Calls f(k, X[k]) once for every k in 0..N/2 (thread t handles k = t
-// and N/2 - t), X = r2c of the real sequence.  No barrier; reads z only.
+// and N/2 - t), X = r2c of the real sequence.  No barrier; reads z only.  tw_lg: log2 of the size whose twiddles tw
+// holds (WB_TW_LOG2 for the full table, lg for the compact table of this size).
 template <class F>
-WB_DEV void rfft_unpack(const double2 *z, int lg, const double2 *__restrict__ tw, F f) {
+WB_DEV void rfft_unpack(const double2 *z, int lg, const double2 *__restrict__ tw, F f, int tw_lg = WB_TW_LOG2) {
   const int tid = WB_TID, nth = WB_NTH;
   const int m = 1 << (lg - 1);
-  const int tws = WB_TW_LOG2 - lg;
+  const int tws = tw_lg - lg;
   for (int k = tid; k <= (m >> 1); k += nth) {
     if (k == 0) {
       const double2 z0 = z[0];

@@ -40,6 +40,7 @@ struct Ctx {
   int device = 0;
   wb_stream_t stream = 0;
   double2 *twiddle = nullptr;        // [WB_TW_N/2] exp(-j 2 pi k / WB_TW_N)
+  double2 *twiddle_sized = nullptr;  // [WB_TW_SIZED_ENTRIES] the same values, one contiguous table per size (wb_fft.cuh)
   uint32_t *rng_jump = nullptr;      // [WB_RNG_NJ][32][16] uint4
   Arena arena;
   Staging staging;
