@@ -570,19 +570,19 @@ WB_DEV void fe_fir_warp(const double *s, const double *hb, int par, int nq, int 
 #endif
 }
 
-// the 10 filtered samples group g looks at: positions pos = 8 g + r (relative to n0 - 2) need s[pos .. pos + 2];
-// sample p of that axis is carry[p] for p < 2 (the last two outputs of the previous tile), st[pad8(p - 2)] otherwise
-WB_DEV void fe_load_group(const double *st, double c0, double c1, int g, double (&v)[WB_FE_R + 2]) {
-  const int base = WB_FE_R * g;
+// Positions pos = 8 g + r of group g (r < 8; relative to n0 - 2: position pos is i = n0 - 2 + pos) need samples
+// pos .. pos + 2 of an axis whose sample p is st[pad8(p - 2)]: p < 2 are the last two outputs of the band's previous
+// tile (the carry), kept at st[-3], st[-2] ahead of the tile.  With R = 8, pad8(8 g + k - 2) = 9 g + k - 2 for
+// k >= 2 and 9 g + k - 3 below: 10 loads at fixed offsets.
+WB_DEV void fe_load_group(const double *st, int g, double (&v)[WB_FE_R + 2]) {
+  const double *b = st + 9 * g;
 #pragma unroll
-  for (int k = 0; k < WB_FE_R + 2; ++k) {
-    const int pp = base + k;
-    v[k] = pp >= 2 ? st[pad8(pp - 2)] : (pp == 0 ? c0 : c1);
-  }
+  for (int k = 0; k < WB_FE_R + 2; ++k) v[k] = b[k < 2 ? k - 3 : k - 2];
 }
 
-// sign tests on the bit pattern (integer pipe; DSETP would queue behind the filter's DFMAs on the FP64 pipe):
-// v > 0 <=> pattern > 0 as a signed integer; v < 0 <=> sign bit set and not -0.0.  (NaN never occurs here.)
+// sign tests on the bit pattern (integer pipe; DSETP would queue on the FP64 pipe), one 64-bit compare each:
+// v > 0 <=> pattern > 0 as a signed integer; v < 0, not -0.0 <=> pattern > 0x8000...0 as unsigned.  (NaN never
+// occurs here.)
 WB_DEV long long fe_bits(double v) {
 #ifdef WB_EMU
   long long b; memcpy(&b, &v, 8); return b;
@@ -590,64 +590,81 @@ WB_DEV long long fe_bits(double v) {
   return __double_as_longlong(v);
 #endif
 }
-WB_DEV bool fe_pos(long long b) { return b > 0; }
-WB_DEV bool fe_neg(long long b) { return b < 0 && b != (long long)0x8000000000000000ull; }
+WB_DEV unsigned fe_pos(long long b) { return b > 0 ? 1u : 0u; }
+WB_DEV unsigned fe_neg(long long b) { return (unsigned long long)b > 0x8000000000000000ull ? 1u : 0u; }
 
-// Events of group g: 4 flag bits per position (bit q = train q, position r at bits 4 r .. 4 r + 3) and the packed
-// per-train counts.  `edge` = the tile touches the ends of the signal (positions before sample 0 / after the last
-// pair are not events); interior tiles skip those tests.
-WB_DEV unsigned long long fe_mask_group(const double (&v)[WB_FE_R + 2], int i0, int ylen, bool edge, unsigned long long *counts) {
-  long long sb[WB_FE_R + 2], db[WB_FE_R + 1];
-#pragma unroll
-  for (int k = 0; k < WB_FE_R + 2; ++k) sb[k] = fe_bits(v[k]);
-#pragma unroll
-  for (int k = 0; k < WB_FE_R + 1; ++k) db[k] = fe_bits(v[k + 1] - v[k]);
-  unsigned long long mask = 0ull, c = 0ull;
-#pragma unroll
-  for (int r = 0; r < WB_FE_R; ++r) {
-    unsigned m = 0u;
-    if (fe_pos(sb[r]) && !fe_pos(sb[r + 1])) m |= 1u;   // s[i] > 0 >= s[i+1]
-    if (fe_neg(sb[r]) && !fe_neg(sb[r + 1])) m |= 2u;   // s[i] < 0 <= s[i+1]
-    if (fe_pos(db[r]) && !fe_pos(db[r + 1])) m |= 4u;   // d[i] > 0 >= d[i+1]
-    if (fe_neg(db[r]) && !fe_neg(db[r + 1])) m |= 8u;   // d[i] < 0 <= d[i+1]
-    if (edge) {
-      const int i = i0 + r;
-      if (!(i >= 0 && i + 1 <= ylen - 1)) m &= ~3u;
-      if (!(i >= 0 && i + 1 <= ylen - 2)) m &= ~12u;
-    }
-    mask |= (unsigned long long)m << (4 * r);
-    c += (unsigned long long)(m & 1u) + ((unsigned long long)((m >> 1) & 1u) << 16) +
-         ((unsigned long long)((m >> 2) & 1u) << 32) + ((unsigned long long)((m >> 3) & 1u) << 48);
-  }
-  *counts = c;
-  return mask;
+// bits lo .. hi of 0 .. 7
+WB_DEV unsigned fe_span(int lo, int hi) {
+  lo = imax(lo, 0); hi = imin(hi, 7);
+  return hi < lo ? 0u : (0xffu >> (7 - hi)) & (0xffu << lo);
 }
 
-// fine edges of group g's events (one division per event), appended in position order at tot[q] + (offsets in o)
-WB_DEV void fe_emit_group(const double (&v)[WB_FE_R + 2], unsigned long long mask, int i0, unsigned long long o,
-                          const int (&tot)[4], double *edges, int cap) {
-  int off[4] = {(int)(o & 0xffffull), (int)((o >> 16) & 0xffffull), (int)((o >> 32) & 0xffffull), (int)((o >> 48) & 0xffffull)};
-  while (mask) {
-#ifdef WB_EMU
-    const int bit = __builtin_ctzll(mask);
-#else
-    const int bit = __ffsll((long long)mask) - 1;
-#endif
-    mask &= mask - 1ull;
-    const int r = bit >> 2, q = bit & 3;
-    double a = v[0], bb = v[1], cc = v[2];
+// Events of group g as one mask, bit 8 q + r = train q fires at position r:
+//   q = 0: s[i] > 0 >= s[i+1]   q = 1: s[i] < 0 <= s[i+1]   q = 2: d[i] > 0 >= d[i+1]   q = 3: d[i] < 0 <= d[i+1]
+// with d[i] = s[i+1] - s[i]: per train a predicate mask P over the 9 samples (differences) the group reads, and the
+// train's events are P & ~(P >> 1).  A train fires where its predicate falls, so at most at every other position:
+// 4 events per train and group.  `edge` = the tile touches the ends of the signal (positions before sample 0 / after
+// the last pair are not events); interior tiles skip that mask.
+WB_DEV unsigned fe_mask_group(const double (&v)[WB_FE_R + 2], int i0, int ylen, bool edge) {
+  unsigned sp = 0u, sn = 0u, dp = 0u, dn = 0u;
 #pragma unroll
-    for (int k = 1; k < WB_FE_R; ++k)            // register array: select by comparison, not by a runtime index
-      if (k == r) { a = v[k]; bb = v[k + 1]; cc = v[k + 2]; }
-    double e;
-    if (q < 2) {
-      e = (double)(i0 + r + 1) - a / (bb - a);
-    } else {
-      const double d0 = bb - a, d1 = cc - bb;
-      e = (double)(i0 + r + 1) - d0 / (d1 - d0);
-    }
-    const int at = tot[q] + off[q];
-    ++off[q];
+  for (int k = 0; k <= WB_FE_R; ++k) {
+    const long long sb = fe_bits(v[k]), db = fe_bits(v[k + 1] - v[k]);
+    sp |= fe_pos(sb) << k; sn |= fe_neg(sb) << k;
+    dp |= fe_pos(db) << k; dn |= fe_neg(db) << k;
+  }
+  unsigned m = (sp & ~(sp >> 1) & 0xffu) | (sn & ~(sn >> 1) & 0xffu) << 8 | (dp & ~(dp >> 1) & 0xffu) << 16 |
+               (dn & ~(dn >> 1) & 0xffu) << 24;
+  if (edge)   // trains 0, 1 need 0 <= i <= ylen - 2, trains 2, 3 0 <= i <= ylen - 3
+    m &= fe_span(-i0, ylen - 2 - i0) * 0x0101u | fe_span(-i0, ylen - 3 - i0) * 0x01010000u;
+  return m;
+}
+
+// events per train of a mask, one byte each (<= 4 per group, so a warp's sums stay below 256)
+WB_DEV unsigned fe_counts(unsigned m) {
+  m = m - ((m >> 1) & 0x55555555u);
+  m = (m & 0x33333333u) + ((m >> 2) & 0x33333333u);
+  return (m + (m >> 4)) & 0x0f0f0f0fu;
+}
+WB_DEV int fe_byte(unsigned x, int q) { return (int)((x >> (8 * q)) & 0xffu); }
+WB_DEV int fe_ctz(unsigned m) {
+#ifdef WB_EMU
+  return __builtin_ctz(m);
+#else
+  return __ffs((int)m) - 1;
+#endif
+}
+
+// A warp's events of an item go through a list in shared memory, train after train, each train in position order:
+// train q starts at s_q = the warp's events of trains < q (wsum: the warp's counts), and the events of group g at
+// s_q + (the counts of the warp's groups before g, ex).  Entries are positions; every entry then costs one lane the
+// same work, wherever its group is, and a train's consecutive entries are consecutive slots of its edge list.
+WB_DEV void fe_stage(unsigned m, unsigned c, unsigned ex, unsigned wsum, int pos0, unsigned short *lst) {
+  // the j-th event of the group (train after train) goes to lst[b_q + j]
+  const int s1 = fe_byte(wsum, 0), s2 = s1 + fe_byte(wsum, 1), s3 = s2 + fe_byte(wsum, 2);
+  const int c0 = fe_byte(c, 0), c01 = c0 + fe_byte(c, 1), c012 = c01 + fe_byte(c, 2);
+  const int b0 = fe_byte(ex, 0), b1 = s1 + fe_byte(ex, 1) - c0, b2 = s2 + fe_byte(ex, 2) - c01,
+            b3 = s3 + fe_byte(ex, 3) - c012;
+  int j = 0;
+  for (; m; m &= m - 1u, ++j) {
+    const int bit = fe_ctz(m), q = bit >> 3;
+    lst[(q == 0 ? b0 : q == 1 ? b1 : q == 2 ? b2 : b3) + j] = (unsigned short)(pos0 + (bit & 7));
+  }
+}
+
+// fine edges of list entries j0, j0 + dj, ... (one division each): entry j of train q is slot d_q + j of the train's
+// list; slots beyond `cap` are counted, not written
+WB_DEV void fe_emit_list(const double *st, const unsigned short *lst, int j0, int dj, unsigned wsum, const int (&d)[4],
+                         int n0, double *edges, int cap) {
+  const int s1 = fe_byte(wsum, 0), s2 = s1 + fe_byte(wsum, 1), s3 = s2 + fe_byte(wsum, 2), n = s3 + fe_byte(wsum, 3);
+  for (int j = j0; j < n; j += dj) {
+    const int pos = lst[j];
+    const int q = (j >= s1) + (j >= s2) + (j >= s3);
+    const int at = (q == 0 ? d[0] : q == 1 ? d[1] : q == 2 ? d[2] : d[3]) + j;
+    const double a = st[pad8(pos - 2)], bb = st[pad8(pos - 1)], cc = st[pad8(pos)];
+    const double d0 = bb - a;
+    const double num = q < 2 ? a : d0, den = q < 2 ? d0 : (cc - bb) - d0;
+    const double e = (double)(n0 - 1 + pos) - num / den;
     if (at < cap) edges[(size_t)q * cap + at] = e;
   }
 }
@@ -662,8 +679,11 @@ struct FeBand {
   double *edges;
 };
 
-// Three CTAs per SM (80 registers, about 51 KB of shared memory each): on H100 the isolated kernel took 169 ms per
-// 1024 x 10 s step; two CTAs per SM with 102 registers and no spills took 179 ms.
+// Three CTAs per SM (80 registers, about 59 KB of shared memory each at 16 kHz): on H100 the isolated kernel took 169 ms
+// per 1024 x 10 s step when the events were picked lane by lane; two CTAs per SM with 102 registers and no spills took
+// 179 ms.  Per item an event thread tests its 8 positions as bit masks, stages its events in its warp's list and then
+// takes its share of the list's entries (fe_stage, fe_emit_list): the event side alone went from 82 to 49 ms, below
+// the filter warps' 135-139 ms alone, which now bound the kernel (DESIGN.md section 4).
 WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
   WB_DYN_SMEM(double, smem);
   int u = blockIdx.y, pr = blockIdx.x;
@@ -673,9 +693,11 @@ WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
   const int segd = fe_seg_doubles(p.max_taps), hcap = fe_hrev_doubles(p.max_taps);
   double *segbuf[2] = {smem, smem + segd};
   double *hrev[2] = {smem + 2 * segd, smem + 2 * segd + hcap};
-  double *stbuf[2] = {hrev[1] + hcap, hrev[1] + hcap + fe_st_doubles()};
-  unsigned long long *wtot = reinterpret_cast<unsigned long long *>(stbuf[1] + fe_st_doubles());   // [2][4] warp totals
-  unsigned long long *bars = wtot + 8;           // two mbarriers
+  double *stbuf[2] = {hrev[1] + hcap + 8, hrev[1] + hcap + fe_st_doubles() + 8};   // the carry ahead of each tile
+  unsigned long long *tail = reinterpret_cast<unsigned long long *>(stbuf[1] + fe_st_doubles() - 8);
+  unsigned *wtot = reinterpret_cast<unsigned *>(tail);   // [2][4] warp event counts, a byte per train
+  unsigned long long *bars = tail + 8;           // two mbarriers
+  unsigned short *evl = reinterpret_cast<unsigned short *>(tail + 16);   // [2][4 warps][32 WB_FE_EVMAX] event lists
   const int ylen = p.y_len[u];
   const size_t abs0 = (size_t)u * p.sig_stride + p.sig_origin;   // index of s(0) in p.sig
   const int n_tiles = (ylen + 2 + T - 1) / T;
@@ -734,7 +756,7 @@ WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
         // pointers formed from `smem` itself, not read from the arrays above: so the compiler knows they are shared
         // and issues LDS, not generic loads
         fe_fir_warp(smem + (t & 1) * segd + fb[s].s_off, smem + 2 * segd + s * hcap + 8, fb[s].par, fb[s].nq, tid >> 5,
-                    tid & 31, smem + 2 * segd + 2 * hcap + (item & 1) * fe_st_doubles());
+                    tid & 31, smem + 2 * segd + 2 * hcap + (item & 1) * fe_st_doubles() + 8);
         __threadfence_block();
         bar_arrive_named(1 + (item & 1), 2 * G);                 // the item is ready
       }
@@ -743,7 +765,8 @@ WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
   } else {
     // ---------------------------------------------------------------- event warps
     const int ct = tid - G, lane = ct & 31, w = ct >> 5;
-    // carry (the last two outputs of the band's previous tile): only group 0 reads it, and group 0 is this role's thread 0
+    // carry (the last two outputs of the band's previous tile): group 0, this role's thread 0, keeps it and puts it
+    // ahead of the tile, where its own loads and the list entries of warp 0 read it
     double c0[2] = {0.0, 0.0}, c1[2] = {0.0, 0.0};
     int item = 0;
     for (int t = 0; t < n_tiles; ++t) {
@@ -753,26 +776,38 @@ WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
       for (int s = 0; s < 2; ++s) {
         if (s >= nslot) break;
         bar_sync_named(1 + (item & 1), 2 * G);
-        const double *st = stbuf[item & 1];
+        // formed from `smem` itself (LDS, not generic loads; see the filter warps)
+        double *st = smem + 2 * segd + 2 * hcap + (item & 1) * fe_st_doubles() + 8;
+        if (ct == 0) { st[-3] = c0[s]; st[-2] = c1[s]; }
         double v[WB_FE_R + 2];
-        fe_load_group(st, c0[s], c1[s], ct, v);
-        const int i0 = n0 - 2 + R * ct;
-        unsigned long long c;
-        const unsigned long long mask = fe_mask_group(v, i0, ylen, edge, &c);
-        unsigned long long inc = c;
+        fe_load_group(st, ct, v);
+        const unsigned m = fe_mask_group(v, n0 - 2 + R * ct, ylen, edge);
+        const unsigned c = fe_counts(m);
+        unsigned inc = c;                          // inclusive warp scan of the byte counts (each sum <= 128)
         for (int o = 1; o < 32; o <<= 1) {
-          const unsigned long long up = __shfl_up_sync(0xffffffffu, inc, o);
+          const unsigned up = __shfl_up_sync(0xffffffffu, inc, o);
           if (lane >= o) inc += up;
         }
-        unsigned long long *wt = wtot + 4 * (item & 1);
+        const unsigned wsum = __shfl_sync(0xffffffffu, inc, 31);
+        unsigned short *lst = evl + ((item & 1) * 4 + w) * (32 * WB_FE_EVMAX);
+        fe_stage(m, c, inc - c, wsum, R * ct, lst);
+        unsigned *wt = wtot + 4 * (item & 1);
         if (lane == 31) wt[w] = inc;
         bar_sync_named(6, G);
-        unsigned long long basew = 0ull, all = 0ull;
+        // the item's events before this warp's (two trains per word, 16-bit fields) and in all
+        unsigned lo = 0u, hi = 0u, alo = 0u, ahi = 0u;
 #pragma unroll
-        for (int k = 0; k < 4; ++k) { const unsigned long long x = wt[k]; if (k < w) basew += x; all += x; }
-        fe_emit_group(v, mask, i0, basew + inc - c, tot[s], fb[s].edges, fb[s].cap);
-        tot[s][0] += (int)(all & 0xffffull); tot[s][1] += (int)((all >> 16) & 0xffffull);
-        tot[s][2] += (int)((all >> 32) & 0xffffull); tot[s][3] += (int)((all >> 48) & 0xffffull);
+        for (int k = 0; k < 4; ++k) {
+          const unsigned x = wt[k], xl = x & 0x00ff00ffu, xh = (x >> 8) & 0x00ff00ffu;
+          if (k < w) { lo += xl; hi += xh; }
+          alo += xl; ahi += xh;
+        }
+        const int s1 = fe_byte(wsum, 0), s2 = s1 + fe_byte(wsum, 1), s3 = s2 + fe_byte(wsum, 2);
+        const int d[4] = {tot[s][0] + (int)(lo & 0xffffu), tot[s][1] + (int)(hi & 0xffffu) - s1,
+                          tot[s][2] + (int)(lo >> 16) - s2, tot[s][3] + (int)(hi >> 16) - s3};
+        fe_emit_list(st, lst, lane, 32, wsum, d, n0, fb[s].edges, fb[s].cap);
+        tot[s][0] += (int)(alo & 0xffffu); tot[s][1] += (int)(ahi & 0xffffu);
+        tot[s][2] += (int)(alo >> 16); tot[s][3] += (int)(ahi >> 16);
         if (ct == 0) { c0[s] = st[pad8(T - 2)]; c1[s] = st[pad8(T - 1)]; }
         __threadfence_block();
         bar_arrive_named(3 + (item & 1), 2 * G);                 // this half may be overwritten (item + 2)
@@ -804,18 +839,26 @@ WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
     for (int s = 0; s < nslot; ++s) {
       double *st = stbuf[s];
       for (int w = 0; w < G / 32; ++w) fe_fir_warp(segbuf[0] + fb[s].s_off, hrev[s] + 8, fb[s].par, fb[s].nq, w, 0, st);
-      unsigned long long run = 0ull;
-      for (int g = 0; g < G; ++g) {
-        double v[WB_FE_R + 2];
-        fe_load_group(st, c0[s], c1[s], g, v);
-        const int i0 = n0 - 2 + R * g;
-        unsigned long long c;
-        const unsigned long long mask = fe_mask_group(v, i0, ylen, true, &c);
-        fe_emit_group(v, mask, i0, run, tot[s], fb[s].edges, fb[s].cap);
-        run += c;
+      st[-3] = c0[s]; st[-2] = c1[s];
+      int done[4] = {0, 0, 0, 0};   // events of the tile's earlier warps
+      for (int w = 0; w < G / 32; ++w) {   // the warps' lists one after the other, the scan as a running sum
+        unsigned m[32], c[32], wsum = 0u;
+        for (int l = 0; l < 32; ++l) {
+          const int g = 32 * w + l;
+          double v[WB_FE_R + 2];
+          fe_load_group(st, g, v);
+          m[l] = fe_mask_group(v, n0 - 2 + R * g, ylen, true);
+          c[l] = fe_counts(m[l]);
+          wsum += c[l];
+        }
+        unsigned ex = 0u;
+        for (int l = 0; l < 32; ++l) { fe_stage(m[l], c[l], ex, wsum, R * (32 * w + l), evl); ex += c[l]; }
+        const int s1 = fe_byte(wsum, 0), s2 = s1 + fe_byte(wsum, 1), s3 = s2 + fe_byte(wsum, 2);
+        const int d[4] = {tot[s][0] + done[0], tot[s][1] + done[1] - s1, tot[s][2] + done[2] - s2, tot[s][3] + done[3] - s3};
+        fe_emit_list(st, evl, 0, 1, wsum, d, n0, fb[s].edges, fb[s].cap);
+        for (int q = 0; q < 4; ++q) done[q] += fe_byte(wsum, q);
       }
-      tot[s][0] += (int)(run & 0xffffull); tot[s][1] += (int)((run >> 16) & 0xffffull);
-      tot[s][2] += (int)((run >> 32) & 0xffffull); tot[s][3] += (int)((run >> 48) & 0xffffull);
+      for (int q = 0; q < 4; ++q) tot[s][q] += done[q];
       c0[s] = st[pad8(T - 2)]; c1[s] = st[pad8(T - 1)];
     }
   }

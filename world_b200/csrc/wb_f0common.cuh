@@ -137,16 +137,20 @@ WB_DEV int flat_block(const int *first, int n_utts, int blk, int *u) {
 // band_fir_events_kernel: tiles of 1024 outputs = 8 outputs per event thread x 128 = 64 FIR rows of 16 outputs
 // (m16n8k8 row tiles), two per filter warp.  Two input segments (TMA double buffer), the taps of two bands with 8
 // leading zeros and zero padding to K + 16 (the polyphase B operand reads h[k - p] for k - p in [-8, K + 8)), two
-// filtered tiles in the pad8 layout (the event threads read 8 outputs each: stride 9 doubles, conflict free).
+// filtered tiles in the pad8 layout (the event threads read 8 outputs each: stride 9 doubles, conflict free; 8
+// doubles ahead of each tile hold the carry), two sets of per-warp event lists.
 #define WB_FE_R 8
 #define WB_FE_TILE (WB_FE_R * 128)
+#define WB_FE_EVMAX 16   // events of one group (8 positions, four trains) at most: 4 per train
 WB_HD inline int fe_kpad(int ntaps) { return (ntaps + 8 + 7) / 8 * 8; }   // >= 8 ceil((K + 1 + 7) / 8), see fe_fir_warp
 WB_HD inline int fe_seg_doubles(int max_taps) { return WB_FE_TILE + fe_kpad(max_taps) + 16; }    // even
 WB_HD inline int fe_hrev_doubles(int max_taps) { return fe_kpad(max_taps) + 16; }
 WB_HD inline int fe_st_doubles() { return WB_FE_TILE + (WB_FE_TILE >> 3) + 8; }
 WB_HD inline size_t fe_smem_bytes(int max_taps) {
-  // two segments, the taps of two bands, two filtered tiles, 2 x 4 warp totals, two mbarriers
-  return (size_t)(2 * fe_seg_doubles(max_taps) + 2 * fe_hrev_doubles(max_taps) + 2 * fe_st_doubles() + 8 + 2 + 6) * 8;
+  // two segments, the taps of two bands, two filtered tiles, 2 x 4 warp counts, two mbarriers, 2 x 4 event lists of
+  // 32 WB_FE_EVMAX 16-bit entries
+  return (size_t)(2 * fe_seg_doubles(max_taps) + 2 * fe_hrev_doubles(max_taps) + 2 * fe_st_doubles() + 8 + 2 + 6) * 8 +
+         (size_t)2 * 128 * WB_FE_EVMAX * 2;
 }
 
 WB_HD inline size_t sweep_smem_bytes(int max_taps) {
