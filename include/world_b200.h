@@ -45,7 +45,9 @@ extern "C" {
 #define WORLD_B200_ENOMEM 2    /* device scratch could not be allocated                       */
 #define WORLD_B200_EINVAL 3    /* argument outside what the on-chip kernels support           */
 #define WORLD_B200_EDOMAIN 4   /* a frame hit a case that is undefined in the reference
-                                  (e.g. f0 below the floor implied by fft_size); see message  */
+                                  (e.g. f0 below the floor implied by fft_size), or an
+                                  utterance needs more than the 2^31 randn() draws the library
+                                  reproduces; see message                                      */
 
 typedef struct WorldB200 WorldB200;
 
@@ -90,6 +92,11 @@ int world_b200_sfft_test(WorldB200 *ctx, const double *x_dev, int n, double *out
 /* Test hook: first n_draws values of the reference's randn() stream (matlabfunctions.cpp:237-264)
  * as raw 32-bit sums (value = sum / 2^28 - 6) into a DEVICE buffer of n_draws uint32. */
 int world_b200_randn_stream(WorldB200 *ctx, unsigned n_draws, unsigned *out_dev);
+/* Test hook: draws [first, first + n) of the same stream, in the same form, into a DEVICE buffer of n
+ * uint32.  The library reproduces the stream up to draw 2^31 of each utterance (first + n <= 2^31, else
+ * EINVAL); a CheapTrick, D4C or Synthesis call whose utterance would draw more reports WORLD_B200_EDOMAIN
+ * at world_b200_synchronize() rather than reuse the stream. */
+int world_b200_randn_window(WorldB200 *ctx, unsigned long long first, unsigned n, unsigned *out_dev);
 
 /* int(1000.0 * x_length / fs / frame_period) + 1 */
 int world_b200_frames(int fs, int x_length, double frame_period);

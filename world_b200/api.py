@@ -60,6 +60,7 @@ ABI = {
     "world_b200_launch_count": (C.c_ulonglong, [_P]),
     "world_b200_frames": (C.c_int, [C.c_int, C.c_int, C.c_double]),
     "world_b200_randn_stream": (C.c_int, [_P, C.c_uint, _P]),
+    "world_b200_randn_window": (C.c_int, [_P, C.c_ulonglong, C.c_uint, _P]),
     "world_b200_rfft_test": (C.c_int, [_P, _P, C.c_int, _P]),
     "world_b200_sfft_test": (C.c_int, [_P, _P, C.c_int, _P]),
     "world_b200_fp64_peak": (C.c_int, [_P, C.POINTER(C.c_double)]),
@@ -340,6 +341,12 @@ class World:
         """test hook: raw draw sums into a uint32 array/tensor of n_draws elements"""
         self._use_current_stream()
         self._check(self.lib.world_b200_randn_stream(self._h, n_draws, _ptr(out_u32)))
+        return out_u32
+
+    def randn_window(self, first, n, out_u32):
+        """test hook: raw draw sums of draws [first, first + n) into a uint32 array/tensor of n elements"""
+        self._use_current_stream()
+        self._check(self.lib.world_b200_randn_window(self._h, first, n, _ptr(out_u32)))
         return out_u32
 
     def frames(self, fs, x_length, frame_period=5.0) -> int:

@@ -496,12 +496,13 @@ int world_b200_synchronize(WorldB200 *h) {
   if (!rc) rc = dev_sync(&h->c);
   if (rc) return rc;
   if (status) {
-    char msg[160];
+    char msg[256];
     snprintf(msg, sizeof msg,
-             "device status 0x%x: %s%s%s", status,
+             "device status 0x%x: %s%s%s%s", status,
              (status & 1) ? "[analysis window longer than fft_size: f0 below the fft_size floor] " : "",
              (status & 2) ? "[smoothing width exceeds the spectrum] " : "",
-             (status & 4) ? "[scratch overflow] " : "");
+             (status & 4) ? "[scratch overflow] " : "",
+             (status & 8) ? "[randn stream past the 2^31 draws per utterance it reproduces] " : "");
     h->c.last_error = msg;
     dev_memset(&h->c, h->c.status_dev, 0, sizeof(int));
     return WORLD_B200_EDOMAIN;
@@ -1104,15 +1105,26 @@ int world_b200_rfft_test(WorldB200 *h, const double *x_dev, int n, double *out_d
 // Known-answer hook: the first n_draws randn() draws after randn_reseed(), as the raw 32-bit
 // sums (value = sum / 2^28 - 6), written to a device buffer of n_draws uint32.
 int world_b200_randn_stream(WorldB200 *h, unsigned n_draws, unsigned *out_dev) {
+  return world_b200_randn_window(h, 0, n_draws, out_dev);
+}
+
+// Known-answer hook: draws [first, first + n) of the same stream, through the kernel the stages use.
+int world_b200_randn_window(WorldB200 *h, unsigned long long first, unsigned n, unsigned *out_dev) {
   if (!h || !out_dev) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
   Ctx *ctx = &h->c;
+  if (first > WB_RNG_REACH || n > WB_RNG_REACH - first) {
+    ctx->last_error = "randn_window: the stream is reproduced up to draw 2^31";
+    return WORLD_B200_EINVAL;
+  }
+  if (n == 0) return 0;
   unsigned char *blk = arena_block(ctx, 256);
   if (!blk) return WORLD_B200_ENOMEM;
-  int rc = dev_memcpy_h2d(ctx, blk, &n_draws, sizeof(unsigned));
+  const unsigned end = (unsigned)(first + n);
+  int rc = dev_memcpy_h2d(ctx, blk, &end, sizeof(unsigned));
   if (rc) return rc;
-  rng_fill(ctx, reinterpret_cast<unsigned *>(blk), out_dev, 0, n_draws, 1);
-  return dev_check(ctx, "randn_stream");
+  rng_fill(ctx, reinterpret_cast<unsigned *>(blk), out_dev, 0, end, 1, (unsigned)first);
+  return dev_check(ctx, "randn_window");
 }
 
 // ---- option helpers: pure host arithmetic, the reference's expressions verbatim in meaning

@@ -7,7 +7,9 @@
 #include <vector>
 
 #define WB_RNG_CHUNK 128   // draws produced by one rng_fill thread
-#define WB_RNG_NJ 24       // jump tables J_k = T^(12*128*2^k): reach 2^31 draws per utterance
+#define WB_RNG_NJ 24       // jump tables J_k = T^(12*128*2^k), one per bit of the chunk index
+// draws per utterance the tables reach (2^31): a stage whose draws would go further reports WORLD_B200_EDOMAIN
+#define WB_RNG_REACH ((unsigned long long)WB_RNG_CHUNK << WB_RNG_NJ)
 #define WB_RNG_WARPS 4
 
 namespace wb {
@@ -98,8 +100,9 @@ int dev_check(Ctx *ctx, const char *what);      // cudaGetLastError -> last_erro
 
 // wb_rng.cu
 void rng_build_jump_tables(uint32_t *tables);
+// draws [first, totals[u]) of utterance u's stream into out + u * utt_stride (first = 0 in the stages)
 void rng_fill(const Ctx *ctx, const unsigned *totals_dev, unsigned *out, size_t utt_stride,
-              size_t max_draws_per_utt, int n_utts);
+              size_t max_draws_per_utt, int n_utts, unsigned first = 0);
 void scan_counts(const Ctx *ctx, const unsigned *counts, const int *lens_dev, int stride,
                  const unsigned *base, unsigned *offsets, unsigned *totals, int n_utts);
 

@@ -89,28 +89,38 @@ WB_DEV unsigned rng_draw(uint4 &s) {
   return acc;
 }
 
-// grid: (ceil(max_chunks / 32) , n_utts); block: 32*WB_RNG_WARPS threads; each warp produces
+// grid: (ceil(chunks / 32) , n_utts); block: 32*WB_RNG_WARPS threads; each warp produces
 // 32 chunks of WB_RNG_CHUNK draws = 4096 consecutive draws, stored coalesced via a smem tile.
+// Draws [first, totals[u]) of the stream, draw d at out[u * utt_stride + d - first]; the stages
+// pass first = 0, the window hook any first.  Every total is at most WB_RNG_REACH (scan_counts
+// clamps and flags larger ones), so chunk g < 2^WB_RNG_NJ and no draw index wraps.
 WB_KERNEL_PLAIN rng_fill_kernel(const uint4 *__restrict__ jump, const unsigned *__restrict__ totals,
-                                unsigned *__restrict__ out, size_t utt_stride) {
+                                unsigned *__restrict__ out, size_t utt_stride, unsigned first) {
   const int utt = blockIdx.y;
   const unsigned total = totals[utt];
   unsigned *dst = out + (size_t)utt * utt_stride;
+  const unsigned chunk0 = first / WB_RNG_CHUNK;
+  // draw d goes to dst[d - first] if d - first < span: one unsigned compare (d < first wraps past span)
+  const unsigned span = total > first ? total - first : 0u;
 #ifdef WB_EMU
   // flat emulation: one "thread" = one chunk
-  const unsigned g = blockIdx.x * blockDim.x + threadIdx.x;
-  const unsigned first = g * WB_RNG_CHUNK;
-  if (first >= total) return;
+  const unsigned g = chunk0 + blockIdx.x * blockDim.x + threadIdx.x;
+  const unsigned start = g * WB_RNG_CHUNK;
+  if (start >= total) return;
   uint4 s = make_uint4(123456789u, 362436069u, 521288629u, 88675123u);
   for (int k = 0; k < WB_RNG_NJ; ++k)
     if ((g >> k) & 1u) s = rng_apply(jump + (size_t)k * 512, s);
-  for (unsigned i = 0; i < WB_RNG_CHUNK && first + i < total; ++i) dst[first + i] = rng_draw(s);
+  for (unsigned i = 0; i < WB_RNG_CHUNK && start + i < total; ++i) {
+    const unsigned v = rng_draw(s), rel = start + i - first;
+    if (rel < span) dst[rel] = v;
+  }
 #else
   __shared__ unsigned tile[WB_RNG_WARPS][32][33];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const unsigned g = (blockIdx.x * WB_RNG_WARPS + warp) * 32 + lane;
-  const unsigned warp_first = (blockIdx.x * WB_RNG_WARPS + warp) * 32 * WB_RNG_CHUNK;
+  const unsigned g = chunk0 + (blockIdx.x * WB_RNG_WARPS + warp) * 32 + lane;
+  const unsigned warp_first = (chunk0 + (blockIdx.x * WB_RNG_WARPS + warp) * 32) * WB_RNG_CHUNK;
   if (warp_first >= total) return;  // whole warp leaves together
+  const unsigned warp_rel = warp_first - first;
   uint4 s = make_uint4(123456789u, 362436069u, 521288629u, 88675123u);
   if (g * WB_RNG_CHUNK < total)
     for (int k = 0; k < WB_RNG_NJ; ++k)
@@ -120,8 +130,8 @@ WB_KERNEL_PLAIN rng_fill_kernel(const uint4 *__restrict__ jump, const unsigned *
     for (int i = 0; i < 32; ++i) tile[warp][lane][i] = rng_draw(s);
     __syncwarp();
     for (int row = 0; row < 32; ++row) {
-      const unsigned idx = warp_first + row * WB_RNG_CHUNK + c * 32 + lane;
-      if (idx < total) dst[idx] = tile[warp][row][lane];
+      const unsigned rel = warp_rel + row * WB_RNG_CHUNK + c * 32 + lane;
+      if (rel < span) dst[rel] = tile[warp][row][lane];
     }
     __syncwarp();
   }
@@ -129,47 +139,56 @@ WB_KERNEL_PLAIN rng_fill_kernel(const uint4 *__restrict__ jump, const unsigned *
 }
 
 void rng_fill(const Ctx *ctx, const unsigned *totals_dev, unsigned *out, size_t utt_stride,
-              size_t max_draws_per_utt, int n_utts) {
-  if (n_utts <= 0 || max_draws_per_utt == 0) return;
-  const size_t chunks = (max_draws_per_utt + WB_RNG_CHUNK - 1) / WB_RNG_CHUNK;
+              size_t max_draws_per_utt, int n_utts, unsigned first) {
+  if (max_draws_per_utt > WB_RNG_REACH) max_draws_per_utt = WB_RNG_REACH;   // totals never exceed the reach
+  if (n_utts <= 0 || max_draws_per_utt <= first) return;
+  const size_t chunk0 = first / WB_RNG_CHUNK;
+  const size_t chunks = (max_draws_per_utt + WB_RNG_CHUNK - 1) / WB_RNG_CHUNK - chunk0;
   const unsigned per_block = 32 * WB_RNG_WARPS;
   dim3 grid((unsigned)((chunks + per_block - 1) / per_block), (unsigned)n_utts);
   WB_LAUNCH_FLAT(rng_fill_kernel, grid, per_block, 0, ctx->stream,
-                 reinterpret_cast<const uint4 *>(ctx->rng_jump), totals_dev, out, utt_stride);
+                 reinterpret_cast<const uint4 *>(ctx->rng_jump), totals_dev, out, utt_stride, first);
 }
 
 // ------------------------------------------------------------------ per-utterance scans
 // counts[u][0..len_u) -> exclusive offsets (same layout) + totals[u] (+ base[u] added to every
-// offset, used by D4C's second pass which continues the stream after the first pass).
+// offset, used by D4C's second pass which continues the stream after the first pass).  The sums
+// run in 64 bits: a total beyond WB_RNG_REACH sets status bit 8 (world_b200_synchronize reports
+// WORLD_B200_EDOMAIN) and is stored clamped to the reach, so rng_fill never repeats the stream.
 WB_KERNEL_PLAIN scan_counts_kernel(const unsigned *__restrict__ counts, const int *__restrict__ lens,
                                    int stride, const unsigned *__restrict__ base,
-                                   unsigned *__restrict__ offsets, unsigned *__restrict__ totals) {
-  WB_SHARED unsigned part[1025];
+                                   unsigned *__restrict__ offsets, unsigned *__restrict__ totals,
+                                   int *__restrict__ status) {
+  WB_SHARED unsigned long long part[1025];
   const int utt = blockIdx.x, tid = WB_TID, nth = WB_NTH;
   const int len = lens[utt];
   const unsigned *c = counts + (size_t)utt * stride;
   unsigned *o = offsets + (size_t)utt * stride;
   const int chunk = (len + nth - 1) / nth;
   const int lo = imin(len, tid * chunk), hi = imin(len, lo + chunk);
-  unsigned s = 0;
+  unsigned long long s = 0;
   for (int i = lo; i < hi; ++i) s += c[i];
   part[tid] = s;
   WB_SYNC();
   if (tid == 0) {
-    unsigned run = base ? base[utt] : 0u;
-    for (int t = 0; t < nth; ++t) { const unsigned v = part[t]; part[t] = run; run += v; }
-    totals[utt] = run;
+    unsigned long long run = base ? base[utt] : 0u;
+    for (int t = 0; t < nth; ++t) { const unsigned long long v = part[t]; part[t] = run; run += v; }
+    if (run > WB_RNG_REACH) {
+      atomicOr_status(status, 8);
+      run = WB_RNG_REACH;
+    }
+    totals[utt] = (unsigned)run;
   }
   WB_SYNC();
-  unsigned run = part[tid];
-  for (int i = lo; i < hi; ++i) { const unsigned v = c[i]; o[i] = run; run += v; }
+  unsigned long long run = part[tid];
+  for (int i = lo; i < hi; ++i) { const unsigned v = c[i]; o[i] = (unsigned)run; run += v; }
 }
 
 void scan_counts(const Ctx *ctx, const unsigned *counts, const int *lens_dev, int stride,
                  const unsigned *base, unsigned *offsets, unsigned *totals, int n_utts) {
   if (n_utts <= 0) return;
   WB_LAUNCH_COOP(scan_counts_kernel, dim3((unsigned)n_utts), 256, 0, ctx->stream, counts, lens_dev,
-                 stride, base, offsets, totals);
+                 stride, base, offsets, totals, ctx->status_dev);
 }
 
 }  // namespace wb
