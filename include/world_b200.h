@@ -313,6 +313,62 @@ int world_b200_analyze_coded_host_dio_options(WorldB200 *ctx, const void *x, int
                                               double *time_axis, double *f0, int f0_stride,
                                               double *coded_spectral_envelope, double *coded_aperiodicity);
 
+/* The coded chain on DEVICE arrays: world_b200_analyze_batch with the input and output formats of
+ * world_b200_analyze_coded_host.  x (DEVICE) holds rows of x_stride samples of `nbit` bits (0 = doubles; 8/16/24/32 =
+ * little-endian PCM, converted exactly as world_b200_pcm_to_double_batch does; a row is x_stride * nbit/8 bytes);
+ * x_lengths is HOST or NULL.  time_axis / f0 are [n_utts][f0_stride], coded_spectral_envelope is
+ * [n_utts][f0_stride][number_of_dimensions] and coded_aperiodicity [n_utts][f0_stride][GetNumberOfAperiodicities(fs)],
+ * all DEVICE; frames beyond an utterance's own count are not written.  Only the coded rows reach device memory (the
+ * frame kernels code them), so the outputs are number_of_dimensions and GetNumberOfAperiodicities(fs) doubles per frame
+ * instead of 2 * (fft_size/2 + 1).  coded_spectral_envelope NULL skips CheapTrick, coded_aperiodicity NULL skips D4C;
+ * below 12 kHz there are no aperiodicity bands and D4C is skipped (coded_aperiodicity may be NULL).  Every row equals
+ * world_b200_analyze_coded_host's for the same utterance and options, bit for bit.  Bad nbit, number_of_dimensions
+ * outside [1, fft_size/4 + 1], per-utterance options that break the rules of world_b200_analyze_batch_options /
+ * _dio_options, or lengths outside their rows are EINVAL before any work is queued.  Stream behaviour and the two
+ * internal streams as for world_b200_analyze_batch; with PCM input each internal stream also holds one float64 buffer
+ * of its largest slice, taken from its half of the scratch budget. */
+int world_b200_analyze_coded_batch(WorldB200 *ctx, const void *x, int nbit, int n_utts, int x_stride,
+                                   const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                   int number_of_dimensions, double *time_axis, double *f0, int f0_stride,
+                                   double *coded_spectral_envelope, double *coded_aperiodicity);
+/* ... with one Harvest option per utterance (HOST array of n_utts), as world_b200_analyze_batch_options. */
+int world_b200_analyze_coded_batch_options(WorldB200 *ctx, const void *x, int nbit, int n_utts, int x_stride,
+                                           const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                           const HarvestOption *harvest_options, int number_of_dimensions,
+                                           double *time_axis, double *f0, int f0_stride,
+                                           double *coded_spectral_envelope, double *coded_aperiodicity);
+/* ... with one DIO option per utterance (HOST array of n_utts), as world_b200_analyze_batch_dio_options. */
+int world_b200_analyze_coded_batch_dio_options(WorldB200 *ctx, const void *x, int nbit, int n_utts, int x_stride,
+                                               const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                               const DioOption *dio_options, int number_of_dimensions,
+                                               double *time_axis, double *f0, int f0_stride,
+                                               double *coded_spectral_envelope, double *coded_aperiodicity);
+/* world_b200_analyze_coded_batch on this rank's n_utts utterances with the outputs given as the FULL arrays of
+ * n_ranks * n_utts utterances, gathered on every rank as world_b200_analyze_batch_allgather gathers the full rows:
+ * the exchanged rows are the coded ones (f0_stride * number_of_dimensions and f0_stride * GetNumberOfAperiodicities(fs)
+ * doubles per utterance), and an array that is NULL or has no bands is not exchanged.  Collective. */
+int world_b200_analyze_coded_batch_allgather(WorldB200 *ctx, const void *x, int nbit, int n_utts, int x_stride,
+                                             const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                             int number_of_dimensions, double *time_axis_full, double *f0_full,
+                                             int f0_stride, double *coded_spectral_envelope_full,
+                                             double *coded_aperiodicity_full);
+/* ... with one Harvest option per utterance of THIS rank's shard (HOST array of n_utts). */
+int world_b200_analyze_coded_batch_allgather_options(WorldB200 *ctx, const void *x, int nbit, int n_utts, int x_stride,
+                                                     const int *x_lengths, int fs,
+                                                     const WorldB200AnalysisOption *option,
+                                                     const HarvestOption *harvest_options, int number_of_dimensions,
+                                                     double *time_axis_full, double *f0_full, int f0_stride,
+                                                     double *coded_spectral_envelope_full,
+                                                     double *coded_aperiodicity_full);
+/* ... with one DIO option per utterance of THIS rank's shard (HOST array of n_utts). */
+int world_b200_analyze_coded_batch_allgather_dio_options(WorldB200 *ctx, const void *x, int nbit, int n_utts,
+                                                         int x_stride, const int *x_lengths, int fs,
+                                                         const WorldB200AnalysisOption *option,
+                                                         const DioOption *dio_options, int number_of_dimensions,
+                                                         double *time_axis_full, double *f0_full, int f0_stride,
+                                                         double *coded_spectral_envelope_full,
+                                                         double *coded_aperiodicity_full);
+
 #ifdef __cplusplus
 }
 #endif

@@ -140,6 +140,24 @@ ABI = {
     "world_b200_analyze_coded_host_dio_options": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int,
                                                             C.POINTER(AnalysisOption), C.POINTER(DioOption), C.c_int,
                                                             _P, _P, C.c_int, _P, _P]),
+    "world_b200_analyze_coded_batch": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int,
+                                                 C.POINTER(AnalysisOption), C.c_int, _P, _P, C.c_int, _P, _P]),
+    "world_b200_analyze_coded_batch_options": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int,
+                                                         C.POINTER(AnalysisOption), C.POINTER(HarvestOption), C.c_int,
+                                                         _P, _P, C.c_int, _P, _P]),
+    "world_b200_analyze_coded_batch_dio_options": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int,
+                                                             C.POINTER(AnalysisOption), C.POINTER(DioOption), C.c_int,
+                                                             _P, _P, C.c_int, _P, _P]),
+    "world_b200_analyze_coded_batch_allgather": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int,
+                                                           C.POINTER(AnalysisOption), C.c_int, _P, _P, C.c_int, _P,
+                                                           _P]),
+    "world_b200_analyze_coded_batch_allgather_options": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int,
+                                                                   C.POINTER(AnalysisOption), C.POINTER(HarvestOption),
+                                                                   C.c_int, _P, _P, C.c_int, _P, _P]),
+    "world_b200_analyze_coded_batch_allgather_dio_options": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP,
+                                                                       C.c_int, C.POINTER(AnalysisOption),
+                                                                       C.POINTER(DioOption), C.c_int, _P, _P, C.c_int,
+                                                                       _P, _P]),
     # host-only file glue (tools/audioio.h, tools/parameterio.h)
     "wavwrite": (None, [_P, C.c_int, C.c_int, C.c_int, C.c_char_p]),
     "GetAudioLength": (C.c_int, [C.c_char_p]),
@@ -712,3 +730,73 @@ class World:
             self._check(self.lib.world_b200_analyze_coded_host(self._h, _ptr(x_host), nbit, n, stride, xl, fs,
                                                                C.byref(option), *outs))
         return time_axis, f0, coded_sp, coded_ap, fl
+
+    def _coded_rows(self, x, nbit, option):
+        """(n, row stride in samples, frame_period) of a coded chain's input: float64 rows for nbit 0, else PCM rows
+        of nbit/8 bytes per sample held in any integer dtype (int16 for 16-bit, uint8 rows for 8/24/32-bit)."""
+        if nbit not in (0, 8, 16, 24, 32):
+            raise ValueError(f"nbit must be 0, 8, 16, 24 or 32, not {nbit}")
+        item = x.element_size() if hasattr(x, "element_size") else x.itemsize
+        width = nbit // 8 if nbit else 8
+        if (x.shape[1] * item) % width:
+            raise ValueError(f"rows of {x.shape[1] * item} bytes do not hold whole {width}-byte samples")
+        frame_period = option.dio.frame_period if option.f0_method == F0_DIO_STONEMASK else option.harvest.frame_period
+        return x.shape[0], x.shape[1] * item // width, frame_period
+
+    def analyze_coded_batch(self, x, nbit, fs, option: AnalysisOption, number_of_dimensions, x_lengths=None,
+                            time_axis=None, f0=None, coded_sp=None, coded_ap=None, harvest_options=None,
+                            dio_options=None):
+        """Whole chain on DEVICE arrays with coded rows out: analyze_batch's two internal streams, analyze_coded_host's
+        formats.  x: float64 rows (nbit 0) or PCM rows (nbit 16: int16; 8/24/32: uint8 rows of nbit/8 bytes per
+        sample); the PCM is converted slice by slice on the device.  Outputs are allocated on x's device when None
+        and the work is enqueued on torch's current stream.  Returns (t, f0, coded_sp, coded_ap, frame counts) with
+        coded_sp [n, L, number_of_dimensions] and coded_ap [n, L, max(1, GetNumberOfAperiodicities(fs))] (left zero
+        below 12 kHz).  harvest_options / dio_options: a list of one option per utterance of the chain's F0 method."""
+        n, stride, frame_period = self._coded_rows(x, nbit, option)
+        lens = [stride] * n if x_lengths is None else [int(v) for v in x_lengths]
+        fl = [self.frames(fs, v, frame_period) for v in lens]
+        f_stride = max(fl) if fl else 1
+        if time_axis is None:
+            time_axis = self._zeros(x, (n, f_stride))
+        if f0 is None:
+            f0 = self._zeros(x, (n, f_stride))
+        if coded_sp is None:
+            coded_sp = self._zeros(x, (n, f_stride, number_of_dimensions))
+        if coded_ap is None:
+            coded_ap = self._zeros(x, (n, f_stride, max(1, self.number_of_aperiodicities(fs))))
+        xl, keep = _int_array(x_lengths, n)
+        per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
+        outs = (number_of_dimensions, _ptr(time_axis), _ptr(f0), time_axis.shape[1], _ptr(coded_sp), _ptr(coded_ap))
+        self._use_current_stream()
+        if per_utt is not None:
+            self._check(self.lib.world_b200_analyze_coded_batch_options(self._h, _ptr(x), nbit, n, stride, xl, fs,
+                                                                        C.byref(option), per_utt, *outs))
+        elif per_dio is not None:
+            self._check(self.lib.world_b200_analyze_coded_batch_dio_options(self._h, _ptr(x), nbit, n, stride, xl, fs,
+                                                                            C.byref(option), per_dio, *outs))
+        else:
+            self._check(self.lib.world_b200_analyze_coded_batch(self._h, _ptr(x), nbit, n, stride, xl, fs,
+                                                                C.byref(option), *outs))
+        return time_axis, f0, coded_sp, coded_ap, fl
+
+    def analyze_coded_batch_allgather(self, x, nbit, fs, option: AnalysisOption, number_of_dimensions, time_axis_full,
+                                      f0_full, coded_sp_full, coded_ap_full, x_lengths=None, harvest_options=None,
+                                      dio_options=None):
+        """analyze_coded_batch on this rank's shard with every finished slice sent into the FULL arrays of all ranks
+        (the coded rows are what crosses between GPUs).  coded_sp_full / coded_ap_full may be None to skip CheapTrick /
+        D4C.  harvest_options / dio_options: a list of one option per utterance of THIS rank's shard."""
+        n, stride, _ = self._coded_rows(x, nbit, option)
+        xl, keep = _int_array(x_lengths, n)
+        per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
+        outs = (number_of_dimensions, _ptr(time_axis_full), _ptr(f0_full), time_axis_full.shape[1],
+                _ptr(coded_sp_full), _ptr(coded_ap_full))
+        self._use_current_stream()
+        if per_utt is not None:
+            self._check(self.lib.world_b200_analyze_coded_batch_allgather_options(
+                self._h, _ptr(x), nbit, n, stride, xl, fs, C.byref(option), per_utt, *outs))
+        elif per_dio is not None:
+            self._check(self.lib.world_b200_analyze_coded_batch_allgather_dio_options(
+                self._h, _ptr(x), nbit, n, stride, xl, fs, C.byref(option), per_dio, *outs))
+        else:
+            self._check(self.lib.world_b200_analyze_coded_batch_allgather(
+                self._h, _ptr(x), nbit, n, stride, xl, fs, C.byref(option), *outs))

@@ -679,28 +679,54 @@ int world_b200_harvest_batch_options(WorldB200 *h, const double *x, int n, int x
 // and every finished slice is broadcast to the other ranks on the communication stream while the next one is computed.
 // harvest_options / dio_options: nullptr, or one option per utterance of the chain's F0 method (at most one of the two;
 // check_chain_f0_options); the slices split the array with the utterances.
-static int analyze_batch_impl(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
+// nbit: 0 = x holds doubles; 8/16/24/32 = little-endian PCM, converted slice by slice on the lane that analyses it.
+// dims: 0 = spectrogram / aperiodicity receive the fft_size/2+1-bin rows; > 0 = they receive the coded rows
+// (number_of_dimensions / GetNumberOfAperiodicities(fs) values per frame) straight from the fused frame kernels.
+static int analyze_batch_impl(WorldB200 *h, const void *x, int nbit, int n, int x_stride, const int *x_lengths, int fs,
                               const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
-                              const DioOption *dio_options, double *time_axis, double *f0, int f0_stride,
+                              const DioOption *dio_options, int dims, double *time_axis, double *f0, int f0_stride,
                               double *spectrogram, double *aperiodicity, bool gather) {
   if (!h || !x || !opt || !time_axis || !f0 || n < 0 || fs <= 0 || x_stride <= 0 || f0_stride <= 0) return WORLD_B200_EINVAL;
   if ((spectrogram || aperiodicity) && opt->cheaptrick.fft_size < 16) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
+  const char *who = dims ? "analyze_coded_batch" : "analyze_batch";
+  if (nbit != 0 && nbit != 8 && nbit != 16 && nbit != 24 && nbit != 32) {
+    h->c.last_error = std::string(who) + ": nbit must be 0, 8, 16, 24 or 32";
+    return WORLD_B200_EINVAL;
+  }
   {
-    const int rc = check_chain_f0_options(&h->c, opt, harvest_options, dio_options, n, fs, "analyze_batch");
+    const int rc = check_chain_f0_options(&h->c, opt, harvest_options, dio_options, n, fs, who);
     if (rc) return rc;
   }
+  const int bins = opt->cheaptrick.fft_size / 2 + 1;
+  const int n_ap = dims ? GetNumberOfAperiodicities(fs) : 0;
+  if (dims) {
+    // the codec tables of every slice, built once here so that a bad dimension count or fft_size queues nothing
+    CodecTables t;
+    int rc = spectrogram ? codec_sp_tables(&h->c, fs, opt->cheaptrick.fft_size, dims, &t) : 0;
+    if (!rc && aperiodicity) rc = codec_ap_tables(&h->c, fs, opt->cheaptrick.fft_size, &t);
+    if (rc) return rc;
+    if (n_ap == 0) aperiodicity = nullptr;   // no bands below 12 kHz: nothing to write, D4C is skipped
+  }
+  const size_t sp_row = dims ? (size_t)dims : (size_t)bins, ap_row = dims ? (size_t)n_ap : (size_t)bins;
   if (n == 0) return 0;
+  const double frame_period = opt->f0_method == WORLD_B200_F0_HARVEST ? opt->harvest.frame_period : opt->dio.frame_period;
+  // every utterance's length and frame count up front: a bad one queues no slice
+  std::vector<int> fl(n);
+  for (int i = 0; i < n; ++i) {
+    const int xl = x_lengths ? x_lengths[i] : x_stride;
+    if (xl < 1 || xl > x_stride) { h->c.last_error = "utterance length outside its padded row"; return WORLD_B200_EINVAL; }
+    fl[i] = frames_for(fs, xl, frame_period);
+    if (fl[i] > f0_stride) { h->c.last_error = "f0_stride smaller than the frame count of an utterance"; return WORLD_B200_EINVAL; }
+  }
   size_t my_block = 0;
   if (gather) {
-    if (!h->comm) { h->c.last_error = "analyze_batch_allgather: no communicator (world_b200_comm_init)"; return WORLD_B200_EINVAL; }
+    if (!h->comm) { h->c.last_error = std::string(who) + "_allgather: no communicator (world_b200_comm_init)"; return WORLD_B200_EINVAL; }
     my_block = (size_t)comm_rank(h->comm) * (size_t)n;
     time_axis += my_block * f0_stride; f0 += my_block * f0_stride;
-    if (spectrogram) spectrogram += my_block * f0_stride * (opt->cheaptrick.fft_size / 2 + 1);
-    if (aperiodicity) aperiodicity += my_block * f0_stride * (opt->cheaptrick.fft_size / 2 + 1);
+    if (spectrogram) spectrogram += my_block * f0_stride * sp_row;
+    if (aperiodicity) aperiodicity += my_block * f0_stride * ap_row;
   }
-  const int bins = opt->cheaptrick.fft_size / 2 + 1;
-  const double frame_period = opt->f0_method == WORLD_B200_F0_HARVEST ? opt->harvest.frame_period : opt->dio.frame_period;
   // two slices (one per lane) overlap best on one GPU (more slices only add launches); with the
   // gather the exposed tail is the LAST slice's transfer, so more, smaller slices win there
   int n_slices = gather ? 10 : 2;
@@ -750,21 +776,44 @@ static int analyze_batch_impl(WorldB200 *h, const double *x, int n, int x_stride
   }
 #endif
   int rc = 0;
-  std::vector<int> fl(n);
-  for (int i = 0; i < n; ++i) fl[i] = frames_for(fs, x_lengths ? x_lengths[i] : x_stride, frame_period);
+  // nbit != 0: each lane converts its slice into a float64 buffer, which the slice's three stages then read.  A lane
+  // runs its slices in stream order, so one buffer per lane, sized for its largest slice, serves all of them.  It comes
+  // from the lane's pool, not its arena (the stage drivers reset the arena when they return), and its bytes come out
+  // of the lane's scratch budget; the stages keep at least half of that budget (less would only mean more passes).
+  double *xbuf[2] = {nullptr, nullptr};
+  const size_t own_budget = h->c.scratch_budget;   // restored on return when the context is its own (only) lane
+  if (nbit) {
+    const bool one_lane = lanes[0] == lanes[1];
+    int most[2] = {0, 0};
+    for (int s = 0; s < n_slices; ++s) {
+      const int l = one_lane ? 0 : (s & 1);
+      most[l] = imax(most[l], bounds[s + 1] - bounds[s]);
+    }
+    for (int l = 0; l < 2 && !rc; ++l) {
+      if (most[l] == 0) continue;
+      Ctx *c = &lanes[l]->c;
+      const size_t bytes = (size_t)most[l] * x_stride * sizeof(double);
+      xbuf[l] = (double *)pool_acquire(c, bytes);
+      if (!xbuf[l]) { h->c.last_error = c->last_error; rc = WORLD_B200_ENOMEM; }
+      c->scratch_budget -= bytes < c->scratch_budget / 2 ? bytes : c->scratch_budget / 2;
+    }
+    if (one_lane) xbuf[1] = xbuf[0];
+  }
 #ifndef WB_EMU
   // multi-GPU: the full arrays and how a finished slice reaches the other ranks -- pushed into their (IPC-mapped)
-  // arrays by the copy engines where that is possible, grouped NCCL broadcasts otherwise (wb_multi.cu)
+  // arrays by the copy engines where that is possible, grouped NCCL broadcasts otherwise (wb_multi.cu).  An array
+  // that is not computed is NULL here, so it is neither exported nor sent.
   double *fulls[4] = {time_axis - my_block * f0_stride, f0 - my_block * f0_stride,
-                      spectrogram ? spectrogram - my_block * f0_stride * bins : nullptr,
-                      aperiodicity ? aperiodicity - my_block * f0_stride * bins : nullptr};
-  const size_t full_elems[4] = {(size_t)f0_stride, (size_t)f0_stride, (size_t)f0_stride * bins, (size_t)f0_stride * bins};
+                      spectrogram ? spectrogram - my_block * f0_stride * sp_row : nullptr,
+                      aperiodicity ? aperiodicity - my_block * f0_stride * ap_row : nullptr};
+  const size_t full_elems[4] = {(size_t)f0_stride, (size_t)f0_stride, spectrogram ? (size_t)f0_stride * sp_row : 0,
+                                aperiodicity ? (size_t)f0_stride * ap_row : 0};
   const bool exchange = gather && comm_ranks(h->comm) > 1;
   bool push = false;
-  if (exchange && !getenv("WB_NO_P2P")) {
+  if (!rc && exchange && !getenv("WB_NO_P2P")) {
     std::string err;
     const int pr = comm_p2p_prepare(h->comm, 4, fulls, &err);
-    if (pr == 2) { h->c.last_error = err; return WORLD_B200_ECUDA; }
+    if (pr == 2) { h->c.last_error = err; rc = WORLD_B200_ECUDA; }
     push = pr == 0;
   }
 #endif
@@ -773,17 +822,29 @@ static int analyze_batch_impl(WorldB200 *h, const double *x, int n, int x_stride
     const int m = u1 - u0;
     if (m <= 0) continue;
     WorldB200 *L = lanes[s & 1];
-    const double *xs = x + (size_t)u0 * x_stride;
     const int *xl = x_lengths ? x_lengths + u0 : nullptr;
+    const double *xs = xbuf[s & 1];
+    if (nbit)
+      rc = world_b200_pcm_to_double_batch(L, (const unsigned char *)x + (size_t)u0 * x_stride * (nbit / 8), nbit, m,
+                                          x_stride, xl, xbuf[s & 1]);
+    else
+      xs = (const double *)x + (size_t)u0 * x_stride;
     double *ts = time_axis + (size_t)u0 * f0_stride, *fs_ = f0 + (size_t)u0 * f0_stride;
-    rc = run_f0_stage(L, xs, m, x_stride, xl, fs, opt, harvest_options ? harvest_options + u0 : nullptr,
-                      dio_options ? dio_options + u0 : nullptr, fl.data() + u0, ts, fs_, f0_stride);
-    if (!rc && spectrogram)
-      rc = world_b200_cheaptrick_batch(L, xs, m, x_stride, xl, fs, ts, fs_, fl.data() + u0, f0_stride, &opt->cheaptrick,
-                                       spectrogram + (size_t)u0 * f0_stride * bins);
-    if (!rc && aperiodicity)
-      rc = world_b200_d4c_batch(L, xs, m, x_stride, xl, fs, ts, fs_, fl.data() + u0, f0_stride, opt->cheaptrick.fft_size,
-                                &opt->d4c, aperiodicity + (size_t)u0 * f0_stride * bins);
+    const int *fls = fl.data() + u0;
+    if (!rc)
+      rc = run_f0_stage(L, xs, m, x_stride, xl, fs, opt, harvest_options ? harvest_options + u0 : nullptr,
+                        dio_options ? dio_options + u0 : nullptr, fls, ts, fs_, f0_stride);
+    double *sps = spectrogram ? spectrogram + (size_t)u0 * f0_stride * sp_row : nullptr;
+    double *aps = aperiodicity ? aperiodicity + (size_t)u0 * f0_stride * ap_row : nullptr;
+    if (!rc && sps)
+      rc = dims ? world_b200_cheaptrick_coded_batch(L, xs, m, x_stride, xl, fs, ts, fs_, fls, f0_stride, &opt->cheaptrick,
+                                                    dims, sps)
+                : world_b200_cheaptrick_batch(L, xs, m, x_stride, xl, fs, ts, fs_, fls, f0_stride, &opt->cheaptrick, sps);
+    if (!rc && aps)
+      rc = dims ? world_b200_d4c_coded_batch(L, xs, m, x_stride, xl, fs, ts, fs_, fls, f0_stride,
+                                             opt->cheaptrick.fft_size, &opt->d4c, aps)
+                : world_b200_d4c_batch(L, xs, m, x_stride, xl, fs, ts, fs_, fls, f0_stride, opt->cheaptrick.fft_size,
+                                       &opt->d4c, aps);
     if (rc && L != h) h->c.last_error = L->c.last_error;
 #ifndef WB_EMU
     if (!rc && exchange) {
@@ -814,13 +875,18 @@ static int analyze_batch_impl(WorldB200 *h, const double *x, int n, int x_stride
       cudaStreamWaitEvent(h->c.stream, (cudaEvent_t)h->ev_join[l], 0);
     }
 #endif
+  // back to the pool while the lanes may still read them: a pooled buffer is only handed out again to work that is
+  // ordered after this call's (the lane's next slices, or the host pipelines, whose uploads wait for the stream)
+  pool_release(&lanes[0]->c, xbuf[0]);
+  if (xbuf[1] != xbuf[0]) pool_release(&lanes[1]->c, xbuf[1]);
+  h->c.scratch_budget = own_budget;
   return rc;
 }
 
 int world_b200_analyze_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
                              const WorldB200AnalysisOption *opt, double *time_axis, double *f0, int f0_stride,
                              double *spectrogram, double *aperiodicity) {
-  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, nullptr, nullptr, time_axis, f0, f0_stride,
+  return analyze_batch_impl(h, x, 0, n, x_stride, x_lengths, fs, opt, nullptr, nullptr, 0, time_axis, f0, f0_stride,
                             spectrogram, aperiodicity, false);
 }
 
@@ -829,7 +895,7 @@ int world_b200_analyze_batch_options(WorldB200 *h, const double *x, int n, int x
                                      double *time_axis, double *f0, int f0_stride, double *spectrogram,
                                      double *aperiodicity) {
   if (!harvest_options) return WORLD_B200_EINVAL;
-  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, harvest_options, nullptr, time_axis, f0, f0_stride,
+  return analyze_batch_impl(h, x, 0, n, x_stride, x_lengths, fs, opt, harvest_options, nullptr, 0, time_axis, f0, f0_stride,
                             spectrogram, aperiodicity, false);
 }
 
@@ -838,7 +904,7 @@ int world_b200_analyze_batch_dio_options(WorldB200 *h, const double *x, int n, i
                                          double *time_axis, double *f0, int f0_stride, double *spectrogram,
                                          double *aperiodicity) {
   if (!dio_options) return WORLD_B200_EINVAL;
-  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, nullptr, dio_options, time_axis, f0, f0_stride,
+  return analyze_batch_impl(h, x, 0, n, x_stride, x_lengths, fs, opt, nullptr, dio_options, 0, time_axis, f0, f0_stride,
                             spectrogram, aperiodicity, false);
 }
 
@@ -893,7 +959,7 @@ int world_b200_allgather_rows(WorldB200 *h, double *full, unsigned long long row
 int world_b200_analyze_batch_allgather(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
                                        const WorldB200AnalysisOption *opt, double *time_axis_full, double *f0_full,
                                        int f0_stride, double *spectrogram_full, double *aperiodicity_full) {
-  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, nullptr, nullptr, time_axis_full, f0_full, f0_stride,
+  return analyze_batch_impl(h, x, 0, n, x_stride, x_lengths, fs, opt, nullptr, nullptr, 0, time_axis_full, f0_full, f0_stride,
                             spectrogram_full, aperiodicity_full, true);
 }
 
@@ -903,7 +969,7 @@ int world_b200_analyze_batch_allgather_options(WorldB200 *h, const double *x, in
                                                double *f0_full, int f0_stride, double *spectrogram_full,
                                                double *aperiodicity_full) {
   if (!harvest_options) return WORLD_B200_EINVAL;
-  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, harvest_options, nullptr, time_axis_full, f0_full,
+  return analyze_batch_impl(h, x, 0, n, x_stride, x_lengths, fs, opt, harvest_options, nullptr, 0, time_axis_full, f0_full,
                             f0_stride, spectrogram_full, aperiodicity_full, true);
 }
 
@@ -913,8 +979,90 @@ int world_b200_analyze_batch_allgather_dio_options(WorldB200 *h, const double *x
                                                    double *f0_full, int f0_stride, double *spectrogram_full,
                                                    double *aperiodicity_full) {
   if (!dio_options) return WORLD_B200_EINVAL;
-  return analyze_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, nullptr, dio_options, time_axis_full, f0_full,
+  return analyze_batch_impl(h, x, 0, n, x_stride, x_lengths, fs, opt, nullptr, dio_options, 0, time_axis_full, f0_full,
                             f0_stride, spectrogram_full, aperiodicity_full, true);
+}
+
+// The device chain with coded rows out (and PCM or doubles in): the checks of analyze_coded_host, then the slices of
+// analyze_batch_impl with the fused coded frame kernels.
+static int analyze_coded_batch_impl(WorldB200 *h, const void *x, int nbit, int n, int x_stride, const int *x_lengths,
+                                    int fs, const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
+                                    const DioOption *dio_options, int number_of_dimensions, double *time_axis,
+                                    double *f0, int f0_stride, double *coded_spectral_envelope,
+                                    double *coded_aperiodicity, bool gather) {
+  if (!h || !opt) return WORLD_B200_EINVAL;
+  if (number_of_dimensions < 1 || number_of_dimensions > opt->cheaptrick.fft_size / 4 + 1) {
+    h->c.last_error = "analyze_coded_batch: number_of_dimensions must be in [1, fft_size/4 + 1]";
+    return WORLD_B200_EINVAL;
+  }
+  return analyze_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, harvest_options, dio_options,
+                            number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope, coded_aperiodicity,
+                            gather);
+}
+
+int world_b200_analyze_coded_batch(WorldB200 *h, const void *x, int nbit, int n, int x_stride, const int *x_lengths,
+                                   int fs, const WorldB200AnalysisOption *opt, int number_of_dimensions,
+                                   double *time_axis, double *f0, int f0_stride, double *coded_spectral_envelope,
+                                   double *coded_aperiodicity) {
+  return analyze_coded_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, nullptr, nullptr, number_of_dimensions,
+                                  time_axis, f0, f0_stride, coded_spectral_envelope, coded_aperiodicity, false);
+}
+
+int world_b200_analyze_coded_batch_options(WorldB200 *h, const void *x, int nbit, int n, int x_stride,
+                                           const int *x_lengths, int fs, const WorldB200AnalysisOption *opt,
+                                           const HarvestOption *harvest_options, int number_of_dimensions,
+                                           double *time_axis, double *f0, int f0_stride,
+                                           double *coded_spectral_envelope, double *coded_aperiodicity) {
+  if (!harvest_options) return WORLD_B200_EINVAL;
+  return analyze_coded_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, harvest_options, nullptr,
+                                  number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope,
+                                  coded_aperiodicity, false);
+}
+
+int world_b200_analyze_coded_batch_dio_options(WorldB200 *h, const void *x, int nbit, int n, int x_stride,
+                                               const int *x_lengths, int fs, const WorldB200AnalysisOption *opt,
+                                               const DioOption *dio_options, int number_of_dimensions,
+                                               double *time_axis, double *f0, int f0_stride,
+                                               double *coded_spectral_envelope, double *coded_aperiodicity) {
+  if (!dio_options) return WORLD_B200_EINVAL;
+  return analyze_coded_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, nullptr, dio_options,
+                                  number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope,
+                                  coded_aperiodicity, false);
+}
+
+int world_b200_analyze_coded_batch_allgather(WorldB200 *h, const void *x, int nbit, int n, int x_stride,
+                                             const int *x_lengths, int fs, const WorldB200AnalysisOption *opt,
+                                             int number_of_dimensions, double *time_axis_full, double *f0_full,
+                                             int f0_stride, double *coded_spectral_envelope_full,
+                                             double *coded_aperiodicity_full) {
+  return analyze_coded_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, nullptr, nullptr, number_of_dimensions,
+                                  time_axis_full, f0_full, f0_stride, coded_spectral_envelope_full,
+                                  coded_aperiodicity_full, true);
+}
+
+int world_b200_analyze_coded_batch_allgather_options(WorldB200 *h, const void *x, int nbit, int n, int x_stride,
+                                                     const int *x_lengths, int fs, const WorldB200AnalysisOption *opt,
+                                                     const HarvestOption *harvest_options, int number_of_dimensions,
+                                                     double *time_axis_full, double *f0_full, int f0_stride,
+                                                     double *coded_spectral_envelope_full,
+                                                     double *coded_aperiodicity_full) {
+  if (!harvest_options) return WORLD_B200_EINVAL;
+  return analyze_coded_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, harvest_options, nullptr,
+                                  number_of_dimensions, time_axis_full, f0_full, f0_stride,
+                                  coded_spectral_envelope_full, coded_aperiodicity_full, true);
+}
+
+int world_b200_analyze_coded_batch_allgather_dio_options(WorldB200 *h, const void *x, int nbit, int n, int x_stride,
+                                                         const int *x_lengths, int fs,
+                                                         const WorldB200AnalysisOption *opt,
+                                                         const DioOption *dio_options, int number_of_dimensions,
+                                                         double *time_axis_full, double *f0_full, int f0_stride,
+                                                         double *coded_spectral_envelope_full,
+                                                         double *coded_aperiodicity_full) {
+  if (!dio_options) return WORLD_B200_EINVAL;
+  return analyze_coded_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, nullptr, dio_options,
+                                  number_of_dimensions, time_axis_full, f0_full, f0_stride,
+                                  coded_spectral_envelope_full, coded_aperiodicity_full, true);
 }
 
 // Per-kernel timing: enable, run, then fetch a JSON object {"kernel": {"launches": n, "ms": t}, ...}

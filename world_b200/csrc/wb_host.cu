@@ -110,8 +110,8 @@ int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_st
     cudaStreamDestroy(s_in);
     return WORLD_B200_ECUDA;
   }
-  cudaEvent_t ev_in[2], ev_cdone[2], ev_f0[2], ev_tf[2];
-  bool ev_ok = true;
+  cudaEvent_t ev_in[2], ev_cdone[2], ev_f0[2], ev_tf[2], ev_start;
+  bool ev_ok = cudaEventCreateWithFlags(&ev_start, cudaEventDisableTiming) == cudaSuccess;
   for (int i = 0; i < 2; ++i) {
     ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_in[i], cudaEventDisableTiming) == cudaSuccess;
     ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_cdone[i], cudaEventDisableTiming) == cudaSuccess;
@@ -151,6 +151,10 @@ int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_st
   };
 #ifndef WB_EMU
   mark("start", 0, s_compute);
+  // the uploads start after the work already on the context's stream: a pooled buffer released by a stream-ordered
+  // call (the PCM buffer of world_b200_analyze_coded_batch) may still be read there
+  cudaEventRecord(ev_start, s_compute);
+  cudaStreamWaitEvent(s_in, ev_start, 0);
 #endif
   DevBuf din[2], dx[2], dt[2], df[2];
   const int raw_slots = dims ? (unfused ? 1 : 0) : ring;   // unfused coded mode: the full rows are consumed on the same stream
@@ -308,6 +312,7 @@ int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_st
     cudaEventDestroy(ev_in[i]); cudaEventDestroy(ev_cdone[i]); cudaEventDestroy(ev_f0[i]); cudaEventDestroy(ev_tf[i]);
   }
   for (int i = 0; i < ring; ++i) { cudaEventDestroy(ev_sub_done[i]); cudaEventDestroy(ev_sub_out[i]); }
+  cudaEventDestroy(ev_start);
   cudaStreamDestroy(s_in);
   cudaStreamDestroy(s_out);
   if (!rc) {
