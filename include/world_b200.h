@@ -14,7 +14,8 @@
  *     written.
  *   - The *_batch functions take DEVICE pointers for the big arrays and enqueue their work on
  *     the context's stream (world_b200_set_stream); they do not synchronise.  One exception:
- *     world_b200_synthesis_batch reads its pulse counts back once per chunk of utterances, which
+ *     world_b200_synthesis_batch and world_b200_synthesis_coded_batch read their pulse counts back once per chunk of
+ *     utterances, which
  *     synchronises the context's stream (all work queued on it before the call included) before
  *     the chunk's remaining kernels are enqueued.  The *_host
  *     functions take host pointers, stage through device memory and return when the results are
@@ -148,6 +149,28 @@ int world_b200_synthesis_batch(WorldB200 *ctx, const double *f0, const int *f0_l
                                int f0_stride, const double *spectrogram, const double *aperiodicity,
                                int fft_size, double frame_period, int fs, const int *y_lengths,
                                int y_stride, double *y);
+
+/* Synthesis() from coded rows: DecodeSpectralEnvelope() (codec.h:86) + DecodeAperiodicity() (codec.h:53) + Synthesis()
+ * (synthesis.h:30) over a batch, without full-row arrays.  f0 [n][f0_stride], coded_spectral_envelope
+ * [n][f0_stride][number_of_dimensions], coded_aperiodicity [n][f0_stride][GetNumberOfAperiodicities(fs)],
+ * y [n][y_stride], all DEVICE; f0_lengths / y_lengths HOST or NULL (full rows).  frame_period in ms.
+ *   - Output: every row equals, bit for bit, what world_b200_decode_spectral_envelope_batch +
+ *     world_b200_decode_aperiodicity_batch + world_b200_synthesis_batch give for the same utterance (the same kernels
+ *     run on the same values).  The rows are decoded chunk by chunk into the call's scratch, so the decoded rows of
+ *     one chunk of utterances (16 * (fft_size/2+1) bytes per frame) are held at a time, never those of the batch.
+ *   - Validation, before any work is queued (WORLD_B200_EINVAL): fft_size a power of two in [16, 4096];
+ *     number_of_dimensions in [1, fft_size/2]; f0 and y lengths >= 2 and within their rows; coded_aperiodicity
+ *     non-NULL whenever GetNumberOfAperiodicities(fs) > 0.
+ *   - Below 12 kHz there are no aperiodicity bands: coded_aperiodicity may be NULL and is not read, and the
+ *     aperiodicity decodes as world_b200_decode_aperiodicity_batch decodes zero bands (the reference's CheckVUV mean
+ *     is 0/0, which takes the voiced branch, over the nodes {0 Hz: -60 dB, fs/2: -1e-12 dB}).
+ *   - Stream behaviour is world_b200_synthesis_batch's, with its one exception: one read-back of the pulse counts per
+ *     chunk of utterances, which synchronises the context's stream. */
+int world_b200_synthesis_coded_batch(WorldB200 *ctx, const double *f0, const int *f0_lengths, int n_utts,
+                                     int f0_stride, const double *coded_spectral_envelope,
+                                     int number_of_dimensions, const double *coded_aperiodicity,
+                                     int fft_size, double frame_period, int fs, const int *y_lengths,
+                                     int y_stride, double *y);
 
 /* ---- codec over a batch (codec.h:20-92) -- SURVEY.md 8 row f2; all DEVICE pointers ------ */
 /* aperiodicity [n][f0_stride][fft_size/2+1] -> coded [n][f0_stride][GetNumberOfAperiodicities(fs)]. */

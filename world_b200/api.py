@@ -84,6 +84,8 @@ ABI = {
                                              C.POINTER(D4COption), _P]),
     "world_b200_synthesis_batch": (C.c_int, [_P, _P, _IP, C.c_int, C.c_int, _P, _P, C.c_int, C.c_double, C.c_int, _IP,
                                              C.c_int, _P]),
+    "world_b200_synthesis_coded_batch": (C.c_int, [_P, _P, _IP, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, C.c_double,
+                                                   C.c_int, _IP, C.c_int, _P]),
     "world_b200_default_analysis_option": (None, [C.c_int, C.c_int, C.POINTER(AnalysisOption)]),
     "world_b200_analyze_host": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(AnalysisOption),
                                           _P, _P, C.c_int, _P, _P]),
@@ -514,6 +516,24 @@ class World:
         self._check(self.lib.world_b200_synthesis_batch(self._h, _ptr(f0), fl, n, f0.shape[1], _ptr(spectrogram),
                                                         _ptr(aperiodicity), fft_size, frame_period, fs, yl, y_length,
                                                         _ptr(y)))
+        return y
+
+    def synthesis_coded(self, f0, coded_spectral_envelope, coded_aperiodicity, fft_size, frame_period, fs, y_length,
+                        f0_lengths=None, y_lengths=None):
+        """Batched Synthesis() from coded rows: f0 [n, L], coded_spectral_envelope [n, L, number_of_dimensions],
+        coded_aperiodicity [n, L, GetNumberOfAperiodicities(fs)] -> y [n, y_length].  The rows are decoded chunk by
+        chunk inside the call; the output equals decode_spectral_envelope + decode_aperiodicity + synthesis bit for
+        bit.  coded_aperiodicity may be None below 12 kHz (no bands)."""
+        n = f0.shape[0]
+        y = self._zeros(f0, (n, y_length))
+        fl, k1 = _int_array(f0_lengths, n)
+        yl, k2 = _int_array(y_lengths, n)
+        self._use_current_stream()
+        self._check(self.lib.world_b200_synthesis_coded_batch(self._h, _ptr(f0), fl, n, f0.shape[1],
+                                                              _ptr(coded_spectral_envelope),
+                                                              int(coded_spectral_envelope.shape[-1]),
+                                                              _ptr(coded_aperiodicity), fft_size, frame_period, fs,
+                                                              yl, y_length, _ptr(y)))
         return y
 
     def analysis_option(self, fs, f0_method=F0_HARVEST) -> AnalysisOption:

@@ -151,6 +151,15 @@ struct CodecTables {
 };
 int codec_sp_tables(Ctx *ctx, int fs, int fft_size, int number_of_dimensions, CodecTables *t);
 int codec_ap_tables(Ctx *ctx, int fs, int fft_size, CodecTables *t);   // t->dims = 0 below 12 kHz
+// The decode half of the codec for a driver that lays out its own scratch (Synthesis from coded rows decodes chunk
+// by chunk into its own block): the tables world_b200_decode_*_batch build, and the launch of their kernels over
+// tables, lengths (f_len, n_utts entries, largest max_f) and rows already on the device.
+int codec_decode_sp_tables(Ctx *ctx, int fs, int fft_size, int number_of_dimensions, CodecTables *t);
+void codec_decode_ap_tables(int fs, int fft_size, CodecTables *t);    // t->dims = GetNumberOfAperiodicities(fs)
+struct CodecDeviceTables { const int *idx; const double *frac; const double2 *weight; };
+void codec_decode_launch(Ctx *ctx, bool spectral_envelope, const CodecTables &t, const CodecDeviceTables &d,
+                         int fft_size, const int *f_len, int n_utts, int f_stride, int max_f, const double *in,
+                         double *out);
 int cheaptrick_run(Ctx *ctx, const Batch &b, double q1, int fft_size, double *spectrogram,
                    const CodecTables *coded = nullptr, double *coded_out = nullptr);
 int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *aperiodicity,

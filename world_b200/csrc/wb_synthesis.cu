@@ -287,24 +287,31 @@ WB_KERNEL_PLAIN syn_overlap_kernel(SynParams p) {
   p.y[(size_t)u * p.y_stride + s] = acc;
 }
 
-}  // namespace wb
+namespace {
 
-using namespace wb;
+// Synthesis from coded rows: the decode tables, made once per call; every chunk decodes its own utterances into its
+// own block before the pulse kernel reads them.
+struct CodedRows {
+  const double *sp, *ap;      // [n][f0_stride][tsp.dims], [n][f0_stride][tap.dims] (ap null when tap.dims == 0)
+  CodecTables tsp, tap;
+};
 
-extern "C" int world_b200_synthesis_batch(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts,
-                                          int f0_stride, const double *spectrogram, const double *aperiodicity,
-                                          int fft_size, double frame_period, int fs, const int *y_lengths,
-                                          int y_stride, double *y) {
-  if (!h || !f0 || !spectrogram || !aperiodicity || !y || n_utts < 0 || fs <= 0 || frame_period <= 0)
-    return WORLD_B200_EINVAL;
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  Ctx *ctx = reinterpret_cast<Ctx *>(h);
+int synthesis_fft(Ctx *ctx, int fft_size, int *lg_out) {
   int lg = 0;
   while ((1 << lg) < fft_size) ++lg;
   if ((1 << lg) != fft_size || fft_size < 16 || fft_size > WB_TW_N / 2) {
     ctx->last_error = "Synthesis: fft_size must be a power of two in [16, 4096]";
     return WORLD_B200_EINVAL;
   }
+  *lg_out = lg;
+  return 0;
+}
+
+// The chunk driver of both entry points: full rows (spectrogram / aperiodicity) or, with `coded`, rows decoded per
+// chunk into the chunk's block.
+int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts, int f0_stride,
+                  const double *spectrogram, const double *aperiodicity, const CodedRows *coded, int fft_size, int lg,
+                  double frame_period, int fs, const int *y_lengths, int y_stride, double *y) {
   if (n_utts == 0) return 0;
   std::vector<int> lens((size_t)2 * n_utts);
   int max_y = 0;
@@ -328,6 +335,18 @@ extern "C" int world_b200_synthesis_batch(WorldB200 *h, const double *f0, const 
     }
     for (int i = 0; i < fft_size / 2; ++i) { dcr[i] /= dc; dcr[fft_size - i - 1] = dcr[i]; }
   }
+  const int half = fft_size / 2;
+  const size_t bins = (size_t)half + 1;
+  // The coded call holds one chunk's decoded envelope and aperiodicity (16 B per bin and frame) and the decode tables.
+  size_t tables = 0;
+  if (coded) {
+    ArenaPlan tp;
+    tp.add(coded->tsp.idx.size() * 4); tp.add(coded->tsp.frac.size() * 8); tp.add(coded->tsp.weight.size() * 16);
+    tp.add(coded->tap.idx.size() * 4); tp.add(coded->tap.frac.size() * 8);
+    tables = tp.total;
+  }
+  const size_t decoded_per_utt = coded ? (size_t)f0_stride * bins * 16 : 0;
+  const double budget = (double)ctx->scratch_budget - (double)tables;
   // Pulse arrays and responses are sized for 1200 pulses per second (f0 <= 1.2 kHz; the +64 covers the ends).
   // The caller's f0 may be anything up to fs/2 (a pitch-shifted contour), so syn_timebase_kernel also counts the
   // pulses it could not store; a chunk where that count exceeds the cap is laid out again with room for its largest
@@ -335,11 +354,11 @@ extern "C" int world_b200_synthesis_batch(WorldB200 *h, const double *f0, const 
   const int nominal_cap = (int)((double)max_y / fs * 1200.0) + 64;
   const size_t draw_stride = (size_t)max_y + 8;
   auto per_utt = [&](int cap) {
-    return (size_t)y_stride * 16 + (size_t)cap * (4 + 8 + 8) + (size_t)cap * fft_size * 8 + draw_stride * 4 + 4096;
+    return (size_t)y_stride * 16 + (size_t)cap * (4 + 8 + 8) + (size_t)cap * fft_size * 8 + draw_stride * 4 + 4096 +
+           decoded_per_utt;
   };
-  auto fit = [&](int cap) { return (int)dmin(65535.0, (double)ctx->scratch_budget / (double)per_utt(cap)); };
+  auto fit = [&](int cap) { return (int)dmin(65535.0, budget / (double)per_utt(cap)); };
   const int chunk = balanced_chunk(imin(n_utts, 65535), fit(nominal_cap));
-  const int half = fft_size / 2;
   const size_t smem = (size_t)(2 * fft_size + 2 * (half + 2) + (fft_size + 2) + 2 * (half + 1) + fft_size + WB_RED_DOUBLES) * 8;
 #ifndef WB_EMU
   cudaFuncSetAttribute(syn_pulse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -358,6 +377,13 @@ extern "C" int world_b200_synthesis_batch(WorldB200 *h, const double *f0, const 
     const size_t o_draws = plan.add((size_t)n * draw_stride * 4);
     const size_t o_resp = plan.add((size_t)n * pulse_cap * fft_size * 8);
     const size_t o_dcr = plan.add((size_t)fft_size * 8);
+    size_t o_dsp = 0, o_dap = 0, o_sidx = 0, o_sfrac = 0, o_sw = 0, o_aidx = 0, o_afrac = 0;
+    if (coded) {
+      o_dsp = plan.add((size_t)n * f0_stride * bins * 8); o_dap = plan.add((size_t)n * f0_stride * bins * 8);
+      o_sidx = plan.add(coded->tsp.idx.size() * 4); o_sfrac = plan.add(coded->tsp.frac.size() * 8);
+      o_sw = plan.add(coded->tsp.weight.size() * 16);
+      o_aidx = plan.add(coded->tap.idx.size() * 4); o_afrac = plan.add(coded->tap.frac.size() * 8);
+    }
     unsigned char *blk = arena_block(ctx, plan.total);
     if (!blk) return WORLD_B200_ENOMEM;
     std::vector<int> l2((size_t)2 * n), pl(n, pulse_cap);
@@ -365,10 +391,22 @@ extern "C" int world_b200_synthesis_batch(WorldB200 *h, const double *f0, const 
     int rc = dev_memcpy_h2d(ctx, blk + o_len, l2.data(), l2.size() * 4);
     if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_dcr, dcr.data(), dcr.size() * 8);
     if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_pl, pl.data(), (size_t)n * 4);
+    if (coded) {
+      const CodecTables &s = coded->tsp, &a = coded->tap;
+      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_sidx, s.idx.data(), s.idx.size() * 4);
+      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_sfrac, s.frac.data(), s.frac.size() * 8);
+      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_sw, s.weight.data(), s.weight.size() * 16);
+      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_aidx, a.idx.data(), a.idx.size() * 4);
+      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_afrac, a.frac.data(), a.frac.size() * 8);
+    }
     if (rc) return rc;
     SynParams p;
     p.f0 = f0 + (size_t)u0 * f0_stride; p.f_len = (const int *)(blk + o_len); p.f_stride = f0_stride;
-    p.sp = spectrogram + (size_t)u0 * f0_stride * (half + 1); p.ap = aperiodicity + (size_t)u0 * f0_stride * (half + 1);
+    if (coded) {
+      p.sp = (const double *)(blk + o_dsp); p.ap = (const double *)(blk + o_dap);
+    } else {
+      p.sp = spectrogram + (size_t)u0 * f0_stride * bins; p.ap = aperiodicity + (size_t)u0 * f0_stride * bins;
+    }
     p.fft_size = fft_size; p.lg_fft = lg; p.frame_period = frame_period / 1000.0; p.fs = fs;
     p.y_len = (const int *)(blk + o_len) + n; p.y_stride = y_stride;
     p.phase = (double *)(blk + o_phase); p.vuv = (double *)(blk + o_vuv); p.flag_cnt = nullptr;
@@ -396,6 +434,20 @@ extern "C" int world_b200_synthesis_batch(WorldB200 *h, const double *f0, const 
         continue;
       }
     }
+    if (coded) {
+      // DecodeSpectralEnvelope / DecodeAperiodicity of this pass's utterances, frames [0, f0_length)
+      int max_f = 0;
+      for (int i = 0; i < n; ++i) max_f = imax(max_f, l2[i]);
+      const CodecDeviceTables ts = {(const int *)(blk + o_sidx), (const double *)(blk + o_sfrac),
+                                    (const double2 *)(blk + o_sw)};
+      const CodecDeviceTables ta = {(const int *)(blk + o_aidx), (const double *)(blk + o_afrac), nullptr};
+      double *dsp = (double *)(blk + o_dsp), *dap = (double *)(blk + o_dap);
+      codec_decode_launch(ctx, true, coded->tsp, ts, fft_size, p.f_len, n, f0_stride, max_f,
+                          coded->sp + (size_t)u0 * f0_stride * coded->tsp.dims, dsp);
+      // below 12 kHz there are no bands: the kernel reads no coded value (its input pointer only has to be valid)
+      codec_decode_launch(ctx, false, coded->tap, ta, fft_size, p.f_len, n, f0_stride, max_f,
+                          coded->ap ? coded->ap + (size_t)u0 * f0_stride * coded->tap.dims : dap, dap);
+    }
     scan_counts(ctx, p.draw_cnt, (const int *)(blk + o_pl), pulse_cap, nullptr, p.draw_off, p.draw_tot, n);
     rng_fill(ctx, p.draw_tot, (unsigned *)(blk + o_draws), draw_stride, draw_stride, n);
     WB_LAUNCH_COOP(syn_pulse_kernel, dim3((unsigned)pulse_cap, (unsigned)n), 128, smem, ctx->stream, p);
@@ -408,4 +460,51 @@ extern "C" int world_b200_synthesis_batch(WorldB200 *h, const double *f0, const 
     relaid = false;
   }
   return 0;
+}
+
+}  // namespace
+
+}  // namespace wb
+
+using namespace wb;
+
+extern "C" int world_b200_synthesis_batch(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts,
+                                          int f0_stride, const double *spectrogram, const double *aperiodicity,
+                                          int fft_size, double frame_period, int fs, const int *y_lengths,
+                                          int y_stride, double *y) {
+  if (!h || !f0 || !spectrogram || !aperiodicity || !y || n_utts < 0 || fs <= 0 || frame_period <= 0)
+    return WORLD_B200_EINVAL;
+  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
+  Ctx *ctx = reinterpret_cast<Ctx *>(h);
+  int lg = 0;
+  const int rc = synthesis_fft(ctx, fft_size, &lg);
+  if (rc) return rc;
+  return synthesis_run(ctx, f0, f0_lengths, n_utts, f0_stride, spectrogram, aperiodicity, nullptr, fft_size, lg,
+                       frame_period, fs, y_lengths, y_stride, y);
+}
+
+extern "C" int world_b200_synthesis_coded_batch(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts,
+                                                int f0_stride, const double *coded_spectral_envelope,
+                                                int number_of_dimensions, const double *coded_aperiodicity,
+                                                int fft_size, double frame_period, int fs, const int *y_lengths,
+                                                int y_stride, double *y) {
+  if (!h || !f0 || !coded_spectral_envelope || !y || n_utts < 0 || fs <= 0 || frame_period <= 0)
+    return WORLD_B200_EINVAL;
+  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
+  Ctx *ctx = reinterpret_cast<Ctx *>(h);
+  int lg = 0;
+  int rc = synthesis_fft(ctx, fft_size, &lg);
+  if (rc) return rc;
+  CodedRows coded;
+  rc = codec_decode_sp_tables(ctx, fs, fft_size, number_of_dimensions, &coded.tsp);
+  if (rc) return rc;
+  codec_decode_ap_tables(fs, fft_size, &coded.tap);
+  if (coded.tap.dims > 0 && !coded_aperiodicity) {
+    ctx->last_error = "Synthesis: coded_aperiodicity is NULL, but fs has GetNumberOfAperiodicities(fs) > 0 bands";
+    return WORLD_B200_EINVAL;
+  }
+  coded.sp = coded_spectral_envelope;
+  coded.ap = coded.tap.dims > 0 ? coded_aperiodicity : nullptr;
+  return synthesis_run(ctx, f0, f0_lengths, n_utts, f0_stride, nullptr, nullptr, &coded, fft_size, lg, frame_period,
+                       fs, y_lengths, y_stride, y);
 }
