@@ -14,8 +14,8 @@
  *     written.
  *   - The *_batch functions take DEVICE pointers for the big arrays and enqueue their work on
  *     the context's stream (world_b200_set_stream); they do not synchronise.  One exception:
- *     world_b200_synthesis_batch and world_b200_synthesis_coded_batch read their pulse counts back once per chunk of
- *     utterances, which
+ *     world_b200_synthesis_batch, world_b200_synthesis_coded_batch and world_b200_synthesis_coded_batch_pcm16 read
+ *     their pulse counts back once per chunk of utterances, which
  *     synchronises the context's stream (all work queued on it before the call included) before
  *     the chunk's remaining kernels are enqueued.  The *_host
  *     functions take host pointers, stage through device memory and return when the results are
@@ -171,6 +171,38 @@ int world_b200_synthesis_coded_batch(WorldB200 *ctx, const double *f0, const int
                                      int number_of_dimensions, const double *coded_aperiodicity,
                                      int fft_size, double frame_period, int fs, const int *y_lengths,
                                      int y_stride, double *y);
+
+/* world_b200_synthesis_coded_batch with 16-bit PCM out: the same arguments, checks and stream behaviour, but y is
+ * [n][y_stride] int16 (DEVICE).  The overlap-add kernel stores wavwrite's quantisation (tools/audioio.cpp) of each
+ * sample it sums, so the float64 waveform never reaches device memory (2 bytes per sample instead of 8):
+ *     v = (int)(sample * 32767)   (truncation toward zero),   v = clamp(v, -32768, 32767).
+ * Where |sample * 32767| < 2^31 every value equals the library's own wavwrite() of what
+ * world_b200_synthesis_coded_batch writes for that sample, bit for bit.  Beyond that range the reference's int cast
+ * is undefined behaviour; here such a sample saturates by its sign (-32768 or 32767), and NaN gives 0.  Padded
+ * samples (beyond an utterance's y_length) are not written. */
+int world_b200_synthesis_coded_batch_pcm16(WorldB200 *ctx, const double *f0, const int *f0_lengths, int n_utts,
+                                           int f0_stride, const double *coded_spectral_envelope,
+                                           int number_of_dimensions, const double *coded_aperiodicity,
+                                           int fft_size, double frame_period, int fs, const int *y_lengths,
+                                           int y_stride, short *y);
+
+/* Synthesis from coded rows for HOST arrays, the counterpart of world_b200_analyze_coded_host: f0 [n][f0_stride],
+ * coded_spectral_envelope [n][f0_stride][number_of_dimensions], coded_aperiodicity
+ * [n][f0_stride][GetNumberOfAperiodicities(fs)] (may be NULL below 12 kHz), f0_lengths / y_lengths (or NULL) and y,
+ * all HOST.  y is [n][y_stride] float64 for nbit 0 or int16 for nbit 16 (any other nbit is WORLD_B200_EINVAL).
+ *   - Output: equal bit for bit to world_b200_synthesis_coded_batch (nbit 0) or
+ *     world_b200_synthesis_coded_batch_pcm16 (nbit 16) for the same utterance.  Whole rows are written back: samples
+ *     beyond an utterance's y_length read as 0.
+ *   - Validation is that of world_b200_synthesis_coded_batch plus nbit, all before any work is queued; after an error
+ *     y is unchanged.
+ *   - Upload, synthesis and download are pipelined over utterance chunks on three streams (uploads, the context's
+ *     stream, downloads); the call returns when the results are in y.  Pinned host buffers (cudaHostAlloc /
+ *     cudaHostRegister) let the copies run under the kernels; pageable ones give the same results, with the copies
+ *     serialised against the host. */
+int world_b200_synthesis_coded_host(WorldB200 *ctx, const double *f0, const int *f0_lengths, int n_utts,
+                                    int f0_stride, const double *coded_spectral_envelope, int number_of_dimensions,
+                                    const double *coded_aperiodicity, int fft_size, double frame_period, int fs,
+                                    const int *y_lengths, int y_stride, int nbit, void *y);
 
 /* ---- codec over a batch (codec.h:20-92) -- SURVEY.md 8 row f2; all DEVICE pointers ------ */
 /* aperiodicity [n][f0_stride][fft_size/2+1] -> coded [n][f0_stride][GetNumberOfAperiodicities(fs)]. */

@@ -86,6 +86,10 @@ ABI = {
                                              C.c_int, _P]),
     "world_b200_synthesis_coded_batch": (C.c_int, [_P, _P, _IP, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, C.c_double,
                                                    C.c_int, _IP, C.c_int, _P]),
+    "world_b200_synthesis_coded_batch_pcm16": (C.c_int, [_P, _P, _IP, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int,
+                                                         C.c_double, C.c_int, _IP, C.c_int, _P]),
+    "world_b200_synthesis_coded_host": (C.c_int, [_P, _P, _IP, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, C.c_double,
+                                                  C.c_int, _IP, C.c_int, C.c_int, _P]),
     "world_b200_default_analysis_option": (None, [C.c_int, C.c_int, C.POINTER(AnalysisOption)]),
     "world_b200_analyze_host": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(AnalysisOption),
                                           _P, _P, C.c_int, _P, _P]),
@@ -254,6 +258,16 @@ def _chain_options(harvest_options, dio_options, n):
         raise TypeError("harvest_options / dio_options: a list of one option per utterance (one option for the batch "
                         "goes into the AnalysisOption)")
     return _harvest_options(harvest_options, n), _dio_options(dio_options, n)
+
+
+def _pcm16(dtype):
+    """True for an int16 dtype (torch.int16, numpy.int16 or "int16"), False for None / float64."""
+    name = str(getattr(dtype, "__name__", dtype)).replace("torch.", "")
+    if dtype is None or name == "float64":
+        return False
+    if name == "int16":
+        return True
+    raise ValueError(f"dtype must be float64 or int16, not {dtype}")
 
 
 def _int_array(v, n):
@@ -519,21 +533,59 @@ class World:
         return y
 
     def synthesis_coded(self, f0, coded_spectral_envelope, coded_aperiodicity, fft_size, frame_period, fs, y_length,
-                        f0_lengths=None, y_lengths=None):
+                        f0_lengths=None, y_lengths=None, dtype=None):
         """Batched Synthesis() from coded rows: f0 [n, L], coded_spectral_envelope [n, L, number_of_dimensions],
         coded_aperiodicity [n, L, GetNumberOfAperiodicities(fs)] -> y [n, y_length].  The rows are decoded chunk by
         chunk inside the call; the output equals decode_spectral_envelope + decode_aperiodicity + synthesis bit for
-        bit.  coded_aperiodicity may be None below 12 kHz (no bands)."""
+        bit.  coded_aperiodicity may be None below 12 kHz (no bands).  dtype: float64 (default) for the waveform, or
+        int16 for its 16-bit PCM, quantised as wavwrite does by the overlap-add kernel itself."""
+        pcm16 = _pcm16(dtype)
         n = f0.shape[0]
-        y = self._zeros(f0, (n, y_length))
+        if pcm16 and self.xp == "torch":
+            y = self.torch.zeros((n, y_length), dtype=self.torch.int16, device=f0.device)
+        elif pcm16:
+            import numpy as np
+            y = np.zeros((n, y_length), dtype=np.int16)
+        else:
+            y = self._zeros(f0, (n, y_length))
         fl, k1 = _int_array(f0_lengths, n)
         yl, k2 = _int_array(y_lengths, n)
+        fn = self.lib.world_b200_synthesis_coded_batch_pcm16 if pcm16 else self.lib.world_b200_synthesis_coded_batch
         self._use_current_stream()
-        self._check(self.lib.world_b200_synthesis_coded_batch(self._h, _ptr(f0), fl, n, f0.shape[1],
-                                                              _ptr(coded_spectral_envelope),
-                                                              int(coded_spectral_envelope.shape[-1]),
-                                                              _ptr(coded_aperiodicity), fft_size, frame_period, fs,
-                                                              yl, y_length, _ptr(y)))
+        self._check(fn(self._h, _ptr(f0), fl, n, f0.shape[1], _ptr(coded_spectral_envelope),
+                       int(coded_spectral_envelope.shape[-1]), _ptr(coded_aperiodicity), fft_size, frame_period, fs,
+                       yl, y_length, _ptr(y)))
+        return y
+
+    def synthesis_coded_host(self, f0, coded_sp, coded_ap, fft_size, frame_period, fs, y_length, nbit=16,
+                             f0_lengths=None, y_lengths=None, out=None):
+        """synthesis_coded for HOST arrays (numpy arrays or CPU tensors, float64): upload, synthesis and download are
+        pipelined over utterance chunks (world_b200_synthesis_coded_host).  Returns y [n, y_length] as a numpy array,
+        int16 for nbit 16 or float64 for nbit 0, whole rows (samples beyond an utterance's y_length are 0).  out: a
+        host array of that shape and dtype to write into (a pinned one lets the downloads overlap the kernels).
+        coded_ap may be None below 12 kHz (no bands)."""
+        import numpy as np
+
+        def host(a):
+            if a is None:
+                return None
+            if hasattr(a, "numpy"):
+                a = a.detach().numpy()
+            return np.ascontiguousarray(a, dtype=np.float64)
+
+        f0, coded_sp, coded_ap = host(f0), host(coded_sp), host(coded_ap)
+        n = f0.shape[0]
+        if out is None:
+            out = np.empty((n, y_length), dtype=np.int16 if nbit == 16 else np.float64)
+        y = out.numpy() if hasattr(out, "numpy") else out
+        if nbit in (0, 16) and (y.shape != (n, y_length) or y.dtype != (np.int16 if nbit == 16 else np.float64)
+                                or not y.flags.c_contiguous):
+            raise ValueError(f"out: a contiguous [{n}, {y_length}] {'int16' if nbit == 16 else 'float64'} host array")
+        fl, k1 = _int_array(f0_lengths, n)
+        yl, k2 = _int_array(y_lengths, n)
+        self._check(self.lib.world_b200_synthesis_coded_host(self._h, _ptr(f0), fl, n, f0.shape[1], _ptr(coded_sp),
+                                                             int(coded_sp.shape[-1]), _ptr(coded_ap), fft_size,
+                                                             frame_period, fs, yl, y_length, nbit, _ptr(y)))
         return y
 
     def analysis_option(self, fs, f0_method=F0_HARVEST) -> AnalysisOption:

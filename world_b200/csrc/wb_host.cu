@@ -1,6 +1,8 @@
 // wb_host.cu -- host-pointer entry points built on the device-pointer ABI:
 //   * world_b200_analyze_host(): {Dio+StoneMask | Harvest} -> CheapTrick -> D4C for N host
 //     waveforms, upload / compute / download pipelined over utterance chunks on three streams;
+//   * world_b200_synthesis_coded_host(): the way back, f0 + coded rows -> waveforms or 16-bit PCM,
+//     pipelined the same way;
 //   * the reference's own single-utterance functions (Dio, Harvest, StoneMask, CheapTrick, D4C;
 //     src/world/*.h) as n_utts = 1 batches on a lazily created process-wide context, so existing
 //     callers relink unchanged.  They keep the reference's `void` signature; failures are
@@ -330,6 +332,225 @@ int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_st
 }
 
 }  // namespace
+
+namespace {
+
+// Synthesis from coded rows for host arrays: utterance chunks, uploads on s_in, synthesis_run on the context's stream,
+// downloads on s_out.  Inputs (f0 + coded rows) are double-buffered, outputs go through a ring of `ring` chunk slots;
+// events order the reuse of both.  synthesis_run synchronises the context's stream once per pass (its pulse counts),
+// so the upload of chunk k+1 is enqueued before synthesis_run is called for chunk k: it then runs under chunk k's
+// kernels instead of after the host has waited for them.  A chunk is one pass of synthesis_run: a longer chunk would
+// hold its download until all its passes were done, and a shorter one would pay the pass's fixed cost more often
+// (syn_timebase_kernel's sequential phase sum over each utterance takes about as long for a few utterances as for a
+// pass of hundreds; at 1024 x 10 s, 16 kHz, chunks of 128 utterances made the call slower than the serial path).  Two
+// input sets and the output ring stay within a third of the scratch budget.  `lens` holds the checked lengths
+// (synthesis_lengths).
+int synthesis_pipeline(WorldB200 *h, CodedRows *coded, int lg, const double *f0, const int *f0_lengths, int n_utts,
+                       int f0_stride, int fft_size, double frame_period, int fs, const int *y_lengths, int y_stride,
+                       const int *lens, int nbit, void *y) {
+  Ctx *ctx = ctx_of(h);
+  const int dims = coded->tsp.dims, n_ap = coded->tap.dims;
+  const double *h_sp = coded->sp, *h_ap = coded->ap;
+  const size_t out_bytes = nbit ? 2 : 8;
+  const size_t per_in = (size_t)f0_stride * (1 + dims + n_ap) * 8, per_out = (size_t)y_stride * out_bytes;
+  int max_y = 0;
+  for (int i = 0; i < n_utts; ++i) max_y = imax(max_y, lens[n_utts + i]);
+  const SynthesisSizing sz(ctx, coded, fft_size, f0_stride, y_stride, max_y, fs);
+  int ring = 3;
+  const size_t third = ctx->scratch_budget / 3;
+  int chunk = imax(1, sz.fit(sz.nominal_cap));
+  chunk = imin(chunk, (int)dmax(1.0, (double)third / (double)(2 * per_in + ring * per_out)));
+  chunk = balanced_chunk(n_utts, chunk);
+  const int n_chunks = (n_utts + chunk - 1) / chunk;
+  ring = imin(ring, n_chunks);
+  ArenaPlan in_plan;
+  const size_t o_f0 = in_plan.add((size_t)chunk * f0_stride * 8);
+  const size_t o_sp = in_plan.add((size_t)chunk * f0_stride * dims * 8);
+  const size_t o_ap = in_plan.add((size_t)chunk * f0_stride * n_ap * 8);
+
+#ifndef WB_EMU
+  cudaStream_t s_compute = ctx->stream, s_in = nullptr, s_out = nullptr;
+  if (cudaStreamCreateWithFlags(&s_in, cudaStreamNonBlocking) != cudaSuccess) {
+    ctx->last_error = "cudaStreamCreate failed";
+    cudaGetLastError();
+    return WORLD_B200_ECUDA;
+  }
+  if (cudaStreamCreateWithFlags(&s_out, cudaStreamNonBlocking) != cudaSuccess) {
+    ctx->last_error = "cudaStreamCreate failed";
+    cudaGetLastError();
+    cudaStreamDestroy(s_in);
+    return WORLD_B200_ECUDA;
+  }
+  cudaEvent_t ev_in[2], ev_cdone[2], ev_start;
+  std::vector<cudaEvent_t> ev_out(ring);
+  bool ev_ok = cudaEventCreateWithFlags(&ev_start, cudaEventDisableTiming) == cudaSuccess;
+  for (int i = 0; i < 2; ++i) {
+    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_in[i], cudaEventDisableTiming) == cudaSuccess;
+    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_cdone[i], cudaEventDisableTiming) == cudaSuccess;
+  }
+  for (int i = 0; i < ring; ++i)
+    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_out[i], cudaEventDisableTiming) == cudaSuccess;
+  if (!ev_ok) {   // (as in analyze_pipeline: events created so far are released with the process)
+    ctx->last_error = "cudaEventCreate failed";
+    cudaGetLastError();
+    cudaStreamDestroy(s_in);
+    cudaStreamDestroy(s_out);
+    return WORLD_B200_ECUDA;
+  }
+#endif
+  // WB_HOST_TRACE=1: timeline of this call on stderr (timing events on the three streams + host clock)
+  const bool trace = getenv("WB_HOST_TRACE") != nullptr;
+  struct Mark { const char *what; int idx; double host_ms; void *ev; };
+  std::vector<Mark> marks;
+  const auto t_host0 = std::chrono::steady_clock::now();
+  auto mark = [&](const char *what, int idx, void *stream) {
+    if (!trace) return;
+    Mark m{what, idx, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_host0).count(), nullptr};
+#ifndef WB_EMU
+    cudaEvent_t e;
+    cudaEventCreate(&e);
+    cudaEventRecord(e, (cudaStream_t)stream);
+    m.ev = e;
+#else
+    (void)stream;
+#endif
+    marks.push_back(m);
+  };
+#ifndef WB_EMU
+  mark("start", 0, s_compute);
+  // the uploads start after the work already on the context's stream: a pooled buffer released by a stream-ordered
+  // call may still be read there
+  cudaEventRecord(ev_start, s_compute);
+  cudaStreamWaitEvent(s_in, ev_start, 0);
+#endif
+  DevBuf din[2];
+  std::vector<DevBuf> dout(ring);
+  int rc = 0;
+  for (int i = 0; i < (n_chunks > 1 ? 2 : 1) && !rc; ++i) rc = ensure(ctx, &din[i], in_plan.total);
+  for (int i = 0; i < ring && !rc; ++i) rc = ensure(ctx, &dout[i], (size_t)chunk * per_out);
+
+  // chunk k's f0 and coded rows into din[k & 1]
+  auto upload = [&](int k) {
+    const int u0 = k * chunk, m = imin(chunk, n_utts - u0);
+    const size_t frames = (size_t)m * f0_stride, row0 = (size_t)u0 * f0_stride;
+    unsigned char *d = (unsigned char *)din[k & 1].p;
+#ifndef WB_EMU
+    if (k >= 2) cudaStreamWaitEvent(s_in, ev_cdone[k & 1], 0);   // the kernels of chunk k-2 have read din[k & 1]
+    cudaMemcpyAsync(d + o_f0, f0 + row0, frames * 8, cudaMemcpyHostToDevice, s_in);
+    cudaMemcpyAsync(d + o_sp, h_sp + row0 * dims, frames * dims * 8, cudaMemcpyHostToDevice, s_in);
+    if (n_ap) cudaMemcpyAsync(d + o_ap, h_ap + row0 * n_ap, frames * n_ap * 8, cudaMemcpyHostToDevice, s_in);
+    cudaEventRecord(ev_in[k & 1], s_in);
+    mark("h2d_done", k, s_in);
+#else
+    memcpy(d + o_f0, f0 + row0, frames * 8);
+    memcpy(d + o_sp, h_sp + row0 * dims, frames * dims * 8);
+    if (n_ap) memcpy(d + o_ap, h_ap + row0 * n_ap, frames * n_ap * 8);
+#endif
+  };
+  if (!rc) upload(0);
+  for (int k = 0; k < n_chunks && !rc; ++k) {
+    const int u0 = k * chunk, m = imin(chunk, n_utts - u0), s = k & 1, slot = k % ring;
+    if (k + 1 < n_chunks) upload(k + 1);
+    unsigned char *d = (unsigned char *)din[s].p;
+#ifndef WB_EMU
+    cudaStreamWaitEvent(s_compute, ev_in[s], 0);
+    if (k >= ring) cudaStreamWaitEvent(s_compute, ev_out[slot], 0);   // the slot's previous chunk is on the host
+    mark("syn_begin", k, s_compute);
+#endif
+    // whole padded rows are downloaded: samples beyond an utterance's length read as zero on the host
+    bool ragged = false;
+    for (int i = 0; i < m; ++i) ragged = ragged || lens[n_utts + u0 + i] != y_stride;
+    if (ragged) rc = dev_memset(ctx, dout[slot].p, 0, (size_t)m * per_out);
+    coded->sp = (const double *)(d + o_sp);
+    coded->ap = n_ap ? (const double *)(d + o_ap) : nullptr;
+    if (!rc)
+      rc = synthesis_run(ctx, (const double *)(d + o_f0), f0_lengths ? f0_lengths + u0 : nullptr, m, f0_stride, nullptr,
+                         nullptr, coded, fft_size, lg, frame_period, fs, y_lengths ? y_lengths + u0 : nullptr, y_stride,
+                         dout[slot].p, nbit);
+    if (rc) break;
+    unsigned char *dst = (unsigned char *)y + (size_t)u0 * per_out;
+#ifndef WB_EMU
+    cudaEventRecord(ev_cdone[s], s_compute);   // behind chunk k's overlap kernel
+    mark("syn_end", k, s_compute);
+    cudaStreamWaitEvent(s_out, ev_cdone[s], 0);
+    cudaMemcpyAsync(dst, dout[slot].p, (size_t)m * per_out, cudaMemcpyDeviceToHost, s_out);
+    cudaEventRecord(ev_out[slot], s_out);
+    mark("d2h_end", k, s_out);
+#else
+    memcpy(dst, dout[slot].p, (size_t)m * per_out);
+#endif
+  }
+  coded->sp = h_sp;
+  coded->ap = h_ap;
+  const double issued_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_host0).count();
+#ifndef WB_EMU
+  // copies and memsets above are not checked one by one: a failure is sticky and surfaces here
+  cudaError_t e_sync = cudaStreamSynchronize(s_in);
+  if (e_sync == cudaSuccess) e_sync = cudaStreamSynchronize(s_compute);
+  if (e_sync == cudaSuccess) e_sync = cudaStreamSynchronize(s_out);
+  if (e_sync != cudaSuccess && !rc) { ctx->last_error = std::string("synthesis pipeline: ") + cudaGetErrorString(e_sync); rc = WORLD_B200_ECUDA; }
+#endif
+  if (trace) {
+    const double done_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_host0).count();
+    fprintf(stderr, "[wb trace] synthesis chunk %d chunks %d ring %d n %d nbit %d: all work issued at %.1f ms, "
+            "finished at %.1f ms (host clock)\n", chunk, n_chunks, ring, n_utts, nbit, issued_ms, done_ms);
+#ifndef WB_EMU
+    for (size_t i = 1; i < marks.size(); ++i) {
+      float gpu_ms = 0.f;
+      cudaEventElapsedTime(&gpu_ms, (cudaEvent_t)marks[0].ev, (cudaEvent_t)marks[i].ev);
+      fprintf(stderr, "[wb trace] %-9s %3d  issued %8.1f  gpu %8.1f\n", marks[i].what, marks[i].idx, marks[i].host_ms, gpu_ms);
+    }
+    for (auto &m : marks) cudaEventDestroy((cudaEvent_t)m.ev);
+#endif
+  }
+#ifndef WB_EMU
+  for (int i = 0; i < 2; ++i) { cudaEventDestroy(ev_in[i]); cudaEventDestroy(ev_cdone[i]); }
+  for (int i = 0; i < ring; ++i) cudaEventDestroy(ev_out[i]);
+  cudaEventDestroy(ev_start);
+  cudaStreamDestroy(s_in);
+  cudaStreamDestroy(s_out);
+  if (!rc) {
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { ctx->last_error = cudaGetErrorString(e); rc = WORLD_B200_ECUDA; }
+  }
+#endif
+  for (int i = 0; i < 2; ++i) pool_release(ctx, din[i].p);
+  for (auto &b : dout) pool_release(ctx, b.p);
+  if (!rc) rc = world_b200_synchronize(h);
+  return rc;
+}
+
+}  // namespace
+
+extern "C" int world_b200_synthesis_coded_host(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts,
+                                               int f0_stride, const double *coded_spectral_envelope,
+                                               int number_of_dimensions, const double *coded_aperiodicity,
+                                               int fft_size, double frame_period, int fs, const int *y_lengths,
+                                               int y_stride, int nbit, void *y) {
+  if (!h || !f0 || !coded_spectral_envelope || !y || n_utts < 0 || fs <= 0 || frame_period <= 0)
+    return WORLD_B200_EINVAL;
+  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
+  Ctx *ctx = ctx_of(h);
+  if (nbit != 0 && nbit != 16) {
+    ctx->last_error = "synthesis_coded_host: nbit must be 0 (double) or 16 (int16)";
+    return WORLD_B200_EINVAL;
+  }
+  int lg = 0;
+  int rc = synthesis_fft(ctx, fft_size, &lg);
+  if (rc) return rc;
+  CodedRows coded;
+  rc = synthesis_coded_tables(ctx, fs, fft_size, number_of_dimensions, coded_aperiodicity != nullptr, &coded);
+  if (rc) return rc;
+  if (n_utts == 0) return 0;
+  // every length is checked before the first chunk is queued
+  std::vector<int> lens((size_t)2 * n_utts);
+  rc = synthesis_lengths(ctx, f0_lengths, n_utts, f0_stride, y_lengths, y_stride, lens.data());
+  if (rc) return rc;
+  coded.sp = coded_spectral_envelope;
+  coded.ap = coded.tap.dims > 0 ? coded_aperiodicity : nullptr;
+  return synthesis_pipeline(h, &coded, lg, f0, f0_lengths, n_utts, f0_stride, fft_size, frame_period, fs, y_lengths,
+                            y_stride, lens.data(), nbit, y);
+}
 
 extern "C" int world_b200_analyze_host(WorldB200 *h, const double *x, int n_utts, int x_stride,
                                        const int *x_lengths, int fs, const WorldB200AnalysisOption *opt,

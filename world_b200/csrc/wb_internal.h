@@ -160,6 +160,33 @@ struct CodecDeviceTables { const int *idx; const double *frac; const double2 *we
 void codec_decode_launch(Ctx *ctx, bool spectral_envelope, const CodecTables &t, const CodecDeviceTables &d,
                          int fft_size, const int *f_len, int n_utts, int f_stride, int max_f, const double *in,
                          double *out);
+// wb_synthesis.cu: the Synthesis driver, shared by the device entry points and the host pipeline (wb_host.cu)
+struct CodedRows {            // Synthesis from coded rows: the decode tables, made once per call
+  const double *sp, *ap;      // [n][f0_stride][tsp.dims], [n][f0_stride][tap.dims] (ap null when tap.dims == 0)
+  CodecTables tsp, tap;
+};
+int synthesis_fft(Ctx *ctx, int fft_size, int *lg_out);   // EINVAL unless a power of two in [16, 4096]
+// the decode tables of a coded call; EINVAL for number_of_dimensions, or no aperiodicity rows where fs has bands
+int synthesis_coded_tables(Ctx *ctx, int fs, int fft_size, int number_of_dimensions, bool have_aperiodicity,
+                           CodedRows *coded);
+// lens[0, n) = f0 lengths, lens[n, 2n) = y lengths (NULL: full rows); EINVAL when one is < 2 or beyond its row
+int synthesis_lengths(Ctx *ctx, const int *f0_lengths, int n_utts, int f0_stride, const int *y_lengths, int y_stride,
+                      int *lens);
+// Per-utterance scratch of synthesis_run for a batch whose longest y_length is max_y; fit(nominal_cap) utterances
+// make one pass when no utterance has more than 1,200 pulses per second.
+struct SynthesisSizing {
+  SynthesisSizing(const Ctx *ctx, const CodedRows *coded, int fft_size, int f0_stride, int y_stride, int max_y, int fs);
+  size_t per_utt(int cap) const;
+  int fit(int cap) const;
+  int fft_size, y_stride, nominal_cap;
+  size_t decoded_per_utt, draw_stride;
+  double budget;
+};
+// Enqueues Synthesis of n_utts utterances (device rows; host lengths) on ctx->stream, in passes that fit the scratch
+// budget, each with one read-back of its pulse counts.  coded null: full rows; y: double (nbit 0) or int16 (nbit 16).
+int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts, int f0_stride,
+                  const double *spectrogram, const double *aperiodicity, const CodedRows *coded, int fft_size, int lg,
+                  double frame_period, int fs, const int *y_lengths, int y_stride, void *y, int nbit);
 int cheaptrick_run(Ctx *ctx, const Batch &b, double q1, int fft_size, double *spectrogram,
                    const CodecTables *coded = nullptr, double *coded_out = nullptr);
 int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *aperiodicity,

@@ -16,6 +16,7 @@
 #include "wb_internal.h"
 #include "wb_spectral.cuh"
 #include "../../include/world_b200.h"
+#include <type_traits>
 #include <vector>
 
 namespace wb {
@@ -39,6 +40,7 @@ struct SynParams {
   double *y;
   const double2 *tw;
   int *status;
+  short *y16;               // [n][y_stride] 16-bit PCM output (syn_overlap_kernel<short>), else null
 };
 
 WB_KERNEL(256, 2) syn_timebase_kernel(SynParams p) {
@@ -269,6 +271,19 @@ WB_KERNEL(128, 3) syn_pulse_kernel(SynParams p) {
   }
 }
 
+// wavwrite's quantisation (tools/audioio.cpp:163-165, wb_fileio.cu wavwrite): (int)(v * 32767) truncated toward zero,
+// then clamped to [-32768, 32767].  Where the product does not fit an int the reference's cast is undefined; here it
+// saturates by sign, and NaN gives 0.
+WB_HD inline short pcm16_of(double v) {
+  const double s = v * 32767;
+  if (!(s == s)) return 0;
+  if (s >= 32767.0) return 32767;
+  if (s <= -32768.0) return -32768;
+  return static_cast<short>(static_cast<int>(s));
+}
+
+// Out = double: the waveform (p.y); Out = short: its 16-bit PCM (p.y16), the sum never reaching memory
+template <typename Out>
 WB_KERNEL_PLAIN syn_overlap_kernel(SynParams p) {
   const int u = blockIdx.y;
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
@@ -284,17 +299,9 @@ WB_KERNEL_PLAIN syn_overlap_kernel(SynParams p) {
     const int j = s - (pidx[i] - half + 1);
     acc += p.resp[((size_t)u * p.pulse_cap + i) * N + j];
   }
-  p.y[(size_t)u * p.y_stride + s] = acc;
+  if constexpr (std::is_same<Out, short>::value) p.y16[(size_t)u * p.y_stride + s] = pcm16_of(acc);
+  else p.y[(size_t)u * p.y_stride + s] = acc;
 }
-
-namespace {
-
-// Synthesis from coded rows: the decode tables, made once per call; every chunk decodes its own utterances into its
-// own block before the pulse kernel reads them.
-struct CodedRows {
-  const double *sp, *ap;      // [n][f0_stride][tsp.dims], [n][f0_stride][tap.dims] (ap null when tap.dims == 0)
-  CodecTables tsp, tap;
-};
 
 int synthesis_fft(Ctx *ctx, int fft_size, int *lg_out) {
   int lg = 0;
@@ -307,14 +314,20 @@ int synthesis_fft(Ctx *ctx, int fft_size, int *lg_out) {
   return 0;
 }
 
-// The chunk driver of both entry points: full rows (spectrogram / aperiodicity) or, with `coded`, rows decoded per
-// chunk into the chunk's block.
-int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts, int f0_stride,
-                  const double *spectrogram, const double *aperiodicity, const CodedRows *coded, int fft_size, int lg,
-                  double frame_period, int fs, const int *y_lengths, int y_stride, double *y) {
-  if (n_utts == 0) return 0;
-  std::vector<int> lens((size_t)2 * n_utts);
-  int max_y = 0;
+int synthesis_coded_tables(Ctx *ctx, int fs, int fft_size, int number_of_dimensions, bool have_aperiodicity,
+                           CodedRows *coded) {
+  const int rc = codec_decode_sp_tables(ctx, fs, fft_size, number_of_dimensions, &coded->tsp);
+  if (rc) return rc;
+  codec_decode_ap_tables(fs, fft_size, &coded->tap);
+  if (coded->tap.dims > 0 && !have_aperiodicity) {
+    ctx->last_error = "Synthesis: coded_aperiodicity is NULL, but fs has GetNumberOfAperiodicities(fs) > 0 bands";
+    return WORLD_B200_EINVAL;
+  }
+  return 0;
+}
+
+int synthesis_lengths(Ctx *ctx, const int *f0_lengths, int n_utts, int f0_stride, const int *y_lengths, int y_stride,
+                      int *lens) {
   for (int i = 0; i < n_utts; ++i) {
     lens[i] = f0_lengths ? f0_lengths[i] : f0_stride;
     lens[n_utts + i] = y_lengths ? y_lengths[i] : y_stride;
@@ -322,8 +335,47 @@ int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts,
       ctx->last_error = "Synthesis: lengths outside the padded rows (need f0_length >= 2, y_length >= 2)";
       return WORLD_B200_EINVAL;
     }
-    if (lens[n_utts + i] > max_y) max_y = lens[n_utts + i];
   }
+  return 0;
+}
+
+SynthesisSizing::SynthesisSizing(const Ctx *ctx, const CodedRows *coded, int fft_size, int f0_stride, int y_stride,
+                                 int max_y, int fs)
+    : fft_size(fft_size), y_stride(y_stride) {
+  const size_t bins = (size_t)fft_size / 2 + 1;
+  // The coded call holds one chunk's decoded envelope and aperiodicity (16 B per bin and frame) and the decode tables.
+  size_t tables = 0;
+  if (coded) {
+    ArenaPlan tp;
+    tp.add(coded->tsp.idx.size() * 4); tp.add(coded->tsp.frac.size() * 8); tp.add(coded->tsp.weight.size() * 16);
+    tp.add(coded->tap.idx.size() * 4); tp.add(coded->tap.frac.size() * 8);
+    tables = tp.total;
+  }
+  decoded_per_utt = coded ? (size_t)f0_stride * bins * 16 : 0;
+  budget = (double)ctx->scratch_budget - (double)tables;
+  // Pulse arrays and responses are sized for 1200 pulses per second (f0 <= 1.2 kHz; the +64 covers the ends).
+  nominal_cap = (int)((double)max_y / fs * 1200.0) + 64;
+  draw_stride = (size_t)max_y + 8;
+}
+
+size_t SynthesisSizing::per_utt(int cap) const {
+  return (size_t)y_stride * 16 + (size_t)cap * (4 + 8 + 8) + (size_t)cap * fft_size * 8 + draw_stride * 4 + 4096 +
+         decoded_per_utt;
+}
+
+int SynthesisSizing::fit(int cap) const { return (int)dmin(65535.0, budget / (double)per_utt(cap)); }
+
+// The chunk driver of both entry points: full rows (spectrogram / aperiodicity) or, with `coded`, rows decoded per
+// chunk into the chunk's block.  nbit 0 writes the waveform (double), nbit 16 its 16-bit PCM (short).
+int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts, int f0_stride,
+                  const double *spectrogram, const double *aperiodicity, const CodedRows *coded, int fft_size, int lg,
+                  double frame_period, int fs, const int *y_lengths, int y_stride, void *y, int nbit) {
+  if (n_utts == 0) return 0;
+  std::vector<int> lens((size_t)2 * n_utts);
+  int rc = synthesis_lengths(ctx, f0_lengths, n_utts, f0_stride, y_lengths, y_stride, lens.data());
+  if (rc) return rc;
+  int max_y = 0;
+  for (int i = 0; i < n_utts; ++i) max_y = imax(max_y, lens[n_utts + i]);
   // DC remover (GetDCRemover, synthesis.cpp:319-333), host libm like the reference
   std::vector<double> dcr(fft_size);
   {
@@ -337,27 +389,13 @@ int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts,
   }
   const int half = fft_size / 2;
   const size_t bins = (size_t)half + 1;
-  // The coded call holds one chunk's decoded envelope and aperiodicity (16 B per bin and frame) and the decode tables.
-  size_t tables = 0;
-  if (coded) {
-    ArenaPlan tp;
-    tp.add(coded->tsp.idx.size() * 4); tp.add(coded->tsp.frac.size() * 8); tp.add(coded->tsp.weight.size() * 16);
-    tp.add(coded->tap.idx.size() * 4); tp.add(coded->tap.frac.size() * 8);
-    tables = tp.total;
-  }
-  const size_t decoded_per_utt = coded ? (size_t)f0_stride * bins * 16 : 0;
-  const double budget = (double)ctx->scratch_budget - (double)tables;
-  // Pulse arrays and responses are sized for 1200 pulses per second (f0 <= 1.2 kHz; the +64 covers the ends).
   // The caller's f0 may be anything up to fs/2 (a pitch-shifted contour), so syn_timebase_kernel also counts the
   // pulses it could not store; a chunk where that count exceeds the cap is laid out again with room for its largest
   // count, in as many passes as the scratch budget needs.  The common case pays one read-back of n counts per chunk.
-  const int nominal_cap = (int)((double)max_y / fs * 1200.0) + 64;
-  const size_t draw_stride = (size_t)max_y + 8;
-  auto per_utt = [&](int cap) {
-    return (size_t)y_stride * 16 + (size_t)cap * (4 + 8 + 8) + (size_t)cap * fft_size * 8 + draw_stride * 4 + 4096 +
-           decoded_per_utt;
-  };
-  auto fit = [&](int cap) { return (int)dmin(65535.0, budget / (double)per_utt(cap)); };
+  const SynthesisSizing sz(ctx, coded, fft_size, f0_stride, y_stride, max_y, fs);
+  const int nominal_cap = sz.nominal_cap;
+  const size_t draw_stride = sz.draw_stride;
+  auto fit = [&](int cap) { return sz.fit(cap); };
   const int chunk = balanced_chunk(imin(n_utts, 65535), fit(nominal_cap));
   const size_t smem = (size_t)(2 * fft_size + 2 * (half + 2) + (fft_size + 2) + 2 * (half + 1) + fft_size + WB_RED_DOUBLES) * 8;
 #ifndef WB_EMU
@@ -388,7 +426,7 @@ int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts,
     if (!blk) return WORLD_B200_ENOMEM;
     std::vector<int> l2((size_t)2 * n), pl(n, pulse_cap);
     for (int i = 0; i < n; ++i) { l2[i] = lens[u0 + i]; l2[n + i] = lens[n_utts + u0 + i]; }
-    int rc = dev_memcpy_h2d(ctx, blk + o_len, l2.data(), l2.size() * 4);
+    rc = dev_memcpy_h2d(ctx, blk + o_len, l2.data(), l2.size() * 4);
     if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_dcr, dcr.data(), dcr.size() * 8);
     if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_pl, pl.data(), (size_t)n * 4);
     if (coded) {
@@ -415,7 +453,9 @@ int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts,
     p.draw_cnt = (unsigned *)(blk + o_dc); p.draw_off = (unsigned *)(blk + o_do); p.draw_tot = (unsigned *)(blk + o_dt);
     p.draws = (const unsigned *)(blk + o_draws); p.draw_stride = draw_stride;
     p.resp = (double *)(blk + o_resp); p.dc_remover = (const double *)(blk + o_dcr);
-    p.y = y + (size_t)u0 * y_stride; p.tw = ctx->twiddle;
+    p.y = nbit ? nullptr : (double *)y + (size_t)u0 * y_stride;
+    p.y16 = nbit ? (short *)y + (size_t)u0 * y_stride : nullptr;
+    p.tw = ctx->twiddle;
     // a pass laid out from the counts reports a pulse beyond its arrays as a scratch overflow (status bit 4)
     p.status = relaid ? ctx->status_dev : nullptr;
     WB_LAUNCH_COOP(syn_timebase_kernel, dim3((unsigned)n), 256, 0, ctx->stream, p);
@@ -451,7 +491,10 @@ int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts,
     scan_counts(ctx, p.draw_cnt, (const int *)(blk + o_pl), pulse_cap, nullptr, p.draw_off, p.draw_tot, n);
     rng_fill(ctx, p.draw_tot, (unsigned *)(blk + o_draws), draw_stride, draw_stride, n);
     WB_LAUNCH_COOP(syn_pulse_kernel, dim3((unsigned)pulse_cap, (unsigned)n), 128, smem, ctx->stream, p);
-    WB_LAUNCH_FLAT(syn_overlap_kernel, dim3((unsigned)((max_y + 255) / 256), (unsigned)n), 256, 0, ctx->stream, p);
+    if (nbit)
+      WB_LAUNCH_FLAT(syn_overlap_kernel<short>, dim3((unsigned)((max_y + 255) / 256), (unsigned)n), 256, 0, ctx->stream, p);
+    else
+      WB_LAUNCH_FLAT(syn_overlap_kernel<double>, dim3((unsigned)((max_y + 255) / 256), (unsigned)n), 256, 0, ctx->stream, p);
     rc = dev_check(ctx, "synthesis");
     if (rc) return rc;
     u0 += n;
@@ -461,8 +504,6 @@ int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts,
   }
   return 0;
 }
-
-}  // namespace
 
 }  // namespace wb
 
@@ -480,14 +521,14 @@ extern "C" int world_b200_synthesis_batch(WorldB200 *h, const double *f0, const 
   const int rc = synthesis_fft(ctx, fft_size, &lg);
   if (rc) return rc;
   return synthesis_run(ctx, f0, f0_lengths, n_utts, f0_stride, spectrogram, aperiodicity, nullptr, fft_size, lg,
-                       frame_period, fs, y_lengths, y_stride, y);
+                       frame_period, fs, y_lengths, y_stride, y, 0);
 }
 
-extern "C" int world_b200_synthesis_coded_batch(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts,
-                                                int f0_stride, const double *coded_spectral_envelope,
-                                                int number_of_dimensions, const double *coded_aperiodicity,
-                                                int fft_size, double frame_period, int fs, const int *y_lengths,
-                                                int y_stride, double *y) {
+// world_b200_synthesis_coded_batch (nbit 0, y double) and world_b200_synthesis_coded_batch_pcm16 (nbit 16, y short)
+static int synthesis_coded_batch(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts, int f0_stride,
+                                 const double *coded_spectral_envelope, int number_of_dimensions,
+                                 const double *coded_aperiodicity, int fft_size, double frame_period, int fs,
+                                 const int *y_lengths, int y_stride, void *y, int nbit) {
   if (!h || !f0 || !coded_spectral_envelope || !y || n_utts < 0 || fs <= 0 || frame_period <= 0)
     return WORLD_B200_EINVAL;
   DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
@@ -496,15 +537,28 @@ extern "C" int world_b200_synthesis_coded_batch(WorldB200 *h, const double *f0, 
   int rc = synthesis_fft(ctx, fft_size, &lg);
   if (rc) return rc;
   CodedRows coded;
-  rc = codec_decode_sp_tables(ctx, fs, fft_size, number_of_dimensions, &coded.tsp);
+  rc = synthesis_coded_tables(ctx, fs, fft_size, number_of_dimensions, coded_aperiodicity != nullptr, &coded);
   if (rc) return rc;
-  codec_decode_ap_tables(fs, fft_size, &coded.tap);
-  if (coded.tap.dims > 0 && !coded_aperiodicity) {
-    ctx->last_error = "Synthesis: coded_aperiodicity is NULL, but fs has GetNumberOfAperiodicities(fs) > 0 bands";
-    return WORLD_B200_EINVAL;
-  }
   coded.sp = coded_spectral_envelope;
   coded.ap = coded.tap.dims > 0 ? coded_aperiodicity : nullptr;
   return synthesis_run(ctx, f0, f0_lengths, n_utts, f0_stride, nullptr, nullptr, &coded, fft_size, lg, frame_period,
-                       fs, y_lengths, y_stride, y);
+                       fs, y_lengths, y_stride, y, nbit);
+}
+
+extern "C" int world_b200_synthesis_coded_batch(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts,
+                                                int f0_stride, const double *coded_spectral_envelope,
+                                                int number_of_dimensions, const double *coded_aperiodicity,
+                                                int fft_size, double frame_period, int fs, const int *y_lengths,
+                                                int y_stride, double *y) {
+  return synthesis_coded_batch(h, f0, f0_lengths, n_utts, f0_stride, coded_spectral_envelope, number_of_dimensions,
+                               coded_aperiodicity, fft_size, frame_period, fs, y_lengths, y_stride, y, 0);
+}
+
+extern "C" int world_b200_synthesis_coded_batch_pcm16(WorldB200 *h, const double *f0, const int *f0_lengths,
+                                                      int n_utts, int f0_stride, const double *coded_spectral_envelope,
+                                                      int number_of_dimensions, const double *coded_aperiodicity,
+                                                      int fft_size, double frame_period, int fs, const int *y_lengths,
+                                                      int y_stride, short *y) {
+  return synthesis_coded_batch(h, f0, f0_lengths, n_utts, f0_stride, coded_spectral_envelope, number_of_dimensions,
+                               coded_aperiodicity, fft_size, frame_period, fs, y_lengths, y_stride, y, 16);
 }
