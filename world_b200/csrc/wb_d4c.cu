@@ -672,7 +672,11 @@ int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *ap
   p.lt_fft = static_cast<int>(pow(2.0, 1.0 + static_cast<int>(log(3.0 * fs / 40.0 + 1) / kLog2)));
   for (p.d_lg = 0; (1 << p.d_lg) < p.d_fft; ++p.d_lg) {}
   for (p.lt_lg = 0; (1 << p.lt_lg) < p.lt_fft; ++p.lt_lg) {}
-  if (p.d_fft > WB_TW_N || p.lt_fft > WB_TW_N || fft_size < 4) {
+  if (fft_size < 4) {
+    ctx->last_error = "D4C: fft_size must be at least 4";
+    return 3;
+  }
+  if (p.d_fft > WB_TW_N || p.lt_fft > WB_TW_N) {
     ctx->last_error = "D4C: sampling rate too high for the on-chip FFT (fft > 8192)";
     return 3;
   }
