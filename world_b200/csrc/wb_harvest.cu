@@ -974,6 +974,51 @@ static int hv_make_groups(Ctx *ctx, const HarvestParams *opts, bool per_utt, int
 
 static int hv_ratio(int fs) { return imax(imin(round_half_away(fs / 8000.0), 12), 1); }   // harvest.cpp:1226, :1158
 
+// Stage capture (test hooks, README): WB_DUMP_DECIMATED / _RAW / _BASE / _REFINED=<prefix> writes <prefix>.<chunk>
+// after that stage of every chunk.  The file is "WBHVDUMP", int64 {version 1, stage 0..3, chunk, first utterance u0,
+// n, ratio, nb, l1_stride, max_cand, n_groups}, double afs, int32 ugrp[n], y_len[n], l1[n], nc[n], per group
+// {int32 nb, double f0_floor, double f0_ceil}, then the payload: stage 0 each utterance's y_len decimated samples,
+// stage 1 raw[n][nb][l1_stride], stage 2 base[n][l1_stride][32] + int32 count[n][l1_stride], stage 3
+// cand[n][l1_stride][max_cand] + score[n][l1_stride][max_cand] (before RemoveUnreliableCandidates).
+enum { HV_DUMP_DECIMATED, HV_DUMP_RAW, HV_DUMP_BASE, HV_DUMP_REFINED, HV_DUMP_STAGES };
+struct HvDumpPart { const void *dev; size_t bytes; };
+
+static int hv_dump(Ctx *ctx, const char *prefix, int stage, int chunk, int u0, int n, int ratio, double afs, int nb,
+                   int l1_stride, int max_cand, const std::vector<int> &ugrp, const std::vector<HvRange> &groups,
+                   const int *ylen_dev, const int *l1_dev, const int *nc_dev, std::vector<HvDumpPart> parts,
+                   const double *y_rows = nullptr, size_t y_stride = 0) {
+  std::vector<int> ylen(n), l1(n), nc(n);
+  int rc = dev_sync(ctx);
+  if (!rc) rc = dev_memcpy_d2h(ctx, ylen.data(), ylen_dev, (size_t)n * 4);
+  if (!rc) rc = dev_memcpy_d2h(ctx, l1.data(), l1_dev, (size_t)n * 4);
+  if (!rc) rc = dev_memcpy_d2h(ctx, nc.data(), nc_dev, (size_t)n * 4);
+  if (!rc) rc = dev_sync(ctx);
+  if (rc) return rc;
+  if (y_rows)   // the decimated rows: y_rows points at utterance 0's first sample
+    for (int u = 0; u < n; ++u) parts.push_back({y_rows + (size_t)u * y_stride, (size_t)ylen[u] * 8});
+  std::vector<std::vector<unsigned char>> host(parts.size());
+  for (size_t i = 0; i < parts.size(); ++i) {
+    host[i].resize(parts[i].bytes);
+    rc = dev_memcpy_d2h(ctx, host[i].data(), parts[i].dev, parts[i].bytes);
+    if (rc) return rc;
+  }
+  rc = dev_sync(ctx);
+  if (rc) return rc;
+  const std::string path = std::string(prefix) + "." + std::to_string(chunk);
+  FILE *f = fopen(path.c_str(), "wb");
+  if (!f) { ctx->last_error = "Harvest: cannot write " + path; return 3; }
+  const long long head[10] = {1, stage, chunk, u0, n, ratio, nb, l1_stride, max_cand, (long long)groups.size()};
+  fwrite("WBHVDUMP", 1, 8, f);
+  fwrite(head, 8, 10, f);
+  fwrite(&afs, 8, 1, f);
+  fwrite(ugrp.data() + u0, 4, n, f);
+  fwrite(ylen.data(), 4, n, f); fwrite(l1.data(), 4, n, f); fwrite(nc.data(), 4, n, f);
+  for (const HvRange &r : groups) { fwrite(&r.nb, 4, 1, f); fwrite(&r.f0_floor, 8, 1, f); fwrite(&r.f0_ceil, 8, 1, f); }
+  for (const auto &h : host) fwrite(h.data(), 1, h.size(), f);
+  fclose(f);
+  return 0;
+}
+
 int harvest_check_options(Ctx *ctx, int fs, const HarvestParams *opts, int n) {
   std::vector<HvRange> groups;
   std::vector<int> ugrp;
@@ -1039,6 +1084,8 @@ int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_ut
 #endif
   for (int u0 = 0; u0 < b.n; u0 += chunk) {
     const int n = imin(chunk, b.n - u0);
+    const char *dump[HV_DUMP_STAGES] = {getenv("WB_DUMP_DECIMATED"), getenv("WB_DUMP_RAW"), getenv("WB_DUMP_BASE"),
+                                        getenv("WB_DUMP_REFINED")};
     ArenaPlan plan;
     const size_t o_y = plan.add((size_t)n * y_stride * 8), o_ylen = plan.add((size_t)n * 4);
     const size_t o_l1 = plan.add((size_t)n * 4), o_nc = plan.add((size_t)n * 4);
@@ -1066,6 +1113,10 @@ int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_ut
     if (!blk) return 2;
     double *y = (double *)(blk + o_y);
     int *ylen = (int *)(blk + o_ylen), *l1 = (int *)(blk + o_l1), *nc = (int *)(blk + o_nc);
+    auto dump_stage = [&](int stage, std::vector<HvDumpPart> parts, const double *y_rows = nullptr) {
+      return hv_dump(ctx, dump[stage], stage, u0 / chunk, u0, n, ratio, afs, nb, l1_stride, max_cand, ugrp, groups,
+                     ylen, l1, nc, parts, y_rows, y_stride);
+    };
     int rc = dev_memset(ctx, y, 0, (size_t)n * y_stride * 8);
     if (!rc) rc = dev_memset(ctx, nc, 0, (size_t)n * 4);
     if (!rc) rc = dev_memcpy_h2d(ctx, l1, b.l1_host + u0, (size_t)n * 4);
@@ -1107,6 +1158,7 @@ int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_ut
       launch_decimate(ctx, dp, b.max_x_len, (unsigned)n);
     }
     WB_LAUNCH_COOP(harvest_prep_kernel, dim3((unsigned)n), 256, 0, ctx->stream, pp);
+    if (dump[HV_DUMP_DECIMATED] && (rc = dump_stage(HV_DUMP_DECIMATED, {}, y + padl))) return rc;
 
     SweepParams sp;
     sp.sig = y; sp.sig_stride = y_stride; sp.sig_origin = padl; sp.y_len = ylen; sp.n_bands = nb;
@@ -1155,24 +1207,16 @@ int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_ut
       launch_band_sweep(ctx, sp, (unsigned)n);
     }
 
-#ifdef WB_EMU
-    if (const char *dump = getenv("WB_DUMP_RAW")) {   // host emulation only: the raw candidate map, for A/B of sweep variants
-      FILE *f = fopen(dump, "wb");
-      if (f) { fwrite(sp.cand, 8, (size_t)n * nb * l1_stride, f); fclose(f); }
-    }
-#endif
+    if (dump[HV_DUMP_RAW] && (rc = dump_stage(HV_DUMP_RAW, {{sp.cand, (size_t)n * nb * l1_stride * 8}}))) return rc;
     const long long slots = (long long)n * l1_stride;
     HvDetectParams dp;
     dp.raw = sp.cand; dp.n_bands = nb; dp.l1_stride = l1_stride; dp.l1 = l1; dp.gr = gr;
     dp.base = (double *)(blk + o_base); dp.base_count = (int *)(blk + o_bcnt); dp.nc = nc; dp.n_utts = n;
     WB_LAUNCH_FLAT(harvest_detect_kernel, dim3((unsigned)((slots + 127) / 128)), 128, 0, ctx->stream, dp);
 
-#ifdef WB_EMU
-    if (const char *dump = getenv("WB_DUMP_BASE")) {   // host emulation only: base candidates per 1 ms frame (experiments)
-      FILE *f = fopen(dump, "wb");
-      if (f) { fwrite(dp.base, 8, (size_t)n * l1_stride * WB_HV_BASE, f); fclose(f); }
-    }
-#endif
+    if (dump[HV_DUMP_BASE] && (rc = dump_stage(HV_DUMP_BASE, {{dp.base, (size_t)slots * WB_HV_BASE * 8},
+                                                              {dp.base_count, (size_t)slots * 4}})))
+      return rc;
     HvRefineParams rp;
     rp.y = y; rp.y_stride = y_stride; rp.y_origin = padl; rp.y_len = ylen; rp.afs = afs;
     rp.base = dp.base; rp.nc = nc; rp.l1_stride = l1_stride; rp.l1 = l1; rp.max_cand = max_cand;
@@ -1202,6 +1246,9 @@ int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_ut
     } else {
       WB_LAUNCH_COOP(harvest_refine_kernel, dim3(refine_blocks, (unsigned)n), 32 * WB_HV_WARPS, smem_refine, ctx->stream, rp);
     }
+    if (dump[HV_DUMP_REFINED] && (rc = dump_stage(HV_DUMP_REFINED, {{rp.cand, (size_t)slots * max_cand * 8},
+                                                                    {rp.score, (size_t)slots * max_cand * 8}})))
+      return rc;
 
     HvRemoveParams mp;
     mp.cand_in = rp.cand; mp.score_in = rp.score; mp.cand = (double *)(blk + o_c2); mp.score = (double *)(blk + o_s2);
