@@ -82,10 +82,15 @@ def read_dump(path):
         d.data.append(np.frombuffer(b, "<f8", n * l1s * WB_HV_BASE, o).reshape(n, l1s, WB_HV_BASE).copy())
         o += 8 * n * l1s * WB_HV_BASE
         d.data.append(np.frombuffer(b, "<i4", n * l1s, o).reshape(n, l1s).copy()); o += 4 * n * l1s
-    else:
+    elif stage in (3, 4):
         for _ in range(2):
             d.data.append(np.frombuffer(b, "<f8", n * l1s * maxc, o).reshape(n, l1s, maxc).copy())
             o += 8 * n * l1s * maxc
+        if stage == 4:    # WB_DUMP_CLEANED: the cleaned rows and SearchF0Base's contour
+            d.data.append(np.frombuffer(b, "<f8", n * l1s, o).reshape(n, l1s).copy()); o += 8 * n * l1s
+    else:                 # WB_DUMP_CONTOUR: FixStep1 .. FixStep4
+        assert stage == 5
+        d.data.append(np.frombuffer(b, "<f8", n * 4 * l1s, o).reshape(n, 4, l1s).copy()); o += 8 * n * 4 * l1s
     assert o == len(b), f"{path}: {len(b) - o} trailing bytes"
     return d
 

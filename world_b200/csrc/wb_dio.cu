@@ -12,6 +12,7 @@
 // utterance's band count, floor and allowed_range.  speed and frame_period are shared by the batch.
 #include "wb_internal.h"
 #include "wb_f0common.cuh"
+#include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 #include <array>
@@ -257,6 +258,36 @@ int dio_check_options(Ctx *ctx, int fs, const DioParams *opts, int n) {
   return dio_make_groups(ctx, opts, true, n, static_cast<double>(fs) / dio_ratio(opts[0].speed), 1, &groups, &ugrp);
 }
 
+// WB_LOAD_DIO_CAND=<prefix> (test hook, README): before dio_contour_kernel each chunk's candidate and score rows are
+// replaced by those of <prefix>.<chunk>: "WBDICAND", int64 {version 1, chunk, n, n_bands, frame_stride}, then
+// cand[n][n_bands][frame_stride] and score[n][n_bands][frame_stride].  n, n_bands and frame_stride must be the
+// chunk's own; anything else is an error return, never a fallback.
+static int dio_load_cand(Ctx *ctx, const char *prefix, int chunk, int n, int nb, int fstr, double *cand_dev,
+                         double *score_dev) {
+  const std::string path = std::string(prefix) + "." + std::to_string(chunk);
+  auto fail = [&](const char *why) { ctx->last_error = "Dio: WB_LOAD_DIO_CAND " + path + ": " + why; return 3; };
+  FILE *f = fopen(path.c_str(), "rb");
+  if (!f) return fail("cannot read");
+  char magic[8];
+  long long head[5];
+  const size_t rows = (size_t)n * nb * fstr;
+  std::vector<double> cs;
+  const char *why = nullptr;
+  if (fread(magic, 1, 8, f) != 8 || memcmp(magic, "WBDICAND", 8) != 0 || fread(head, 8, 5, f) != 5 || head[0] != 1)
+    why = "not a version 1 WBDICAND file";
+  else if (head[2] != n || head[3] != nb || head[4] != fstr) why = "n, n_bands or frame_stride differ from the chunk's";
+  if (!why) {
+    cs.resize(2 * rows);
+    if (fread(cs.data(), 8, cs.size(), f) != cs.size() || fgetc(f) != EOF) why = "payload size differs from the header's";
+  }
+  fclose(f);
+  if (why) return fail(why);
+  int rc = dev_memcpy_h2d(ctx, cand_dev, cs.data(), rows * 8);
+  if (!rc) rc = dev_memcpy_h2d(ctx, score_dev, cs.data() + rows, rows * 8);
+  if (!rc) rc = dev_sync(ctx);
+  return rc;
+}
+
 int dio_run(Ctx *ctx, const Batch &b, const DioParams *opts, bool per_utt, double *time_axis_out, double *f0_out) {
   if (b.n <= 0) return 0;
   const int fs = b.fs;
@@ -319,6 +350,7 @@ int dio_run(Ctx *ctx, const Batch &b, const DioParams *opts, bool per_utt, doubl
   const size_t per_utt_bytes = y_stride * 16 + edge_stride * 8 + (size_t)nb * fstr * 16 +
                                (size_t)fstr * (4 * 8 + 2 * 4) + tmp_stride * 16 + 256;
   int chunk = balanced_chunk(imin(b.n, 65535), (int)dmin(65535.0, (double)ctx->scratch_budget / (double)per_utt_bytes));
+  const char *load_cand = getenv("WB_LOAD_DIO_CAND");
   for (int u0 = 0; u0 < b.n; u0 += chunk) {
     const int n = imin(chunk, b.n - u0);
     ArenaPlan plan;
@@ -422,6 +454,7 @@ int dio_run(Ctx *ctx, const Batch &b, const DioParams *opts, bool per_utt, doubl
     sp.cand = (double *)(blk + o_cand); sp.score = (double *)(blk + o_score);
     sp.max_taps = max_taps; sp.status = ctx->status_dev;
     launch_band_sweep(ctx, sp, (unsigned)n);
+    if (load_cand && (rc = dio_load_cand(ctx, load_cand, u0 / chunk, n, nb, fstr, sp.cand, sp.score))) return rc;
 
     DioContourParams cp;
     cp.cand = sp.cand; cp.score = sp.score; cp.n_bands = nb; cp.frame_stride = fstr; cp.f_len = b.f_len + u0;

@@ -980,7 +980,15 @@ static int hv_ratio(int fs) { return imax(imin(round_half_away(fs / 8000.0), 12)
 // {int32 nb, double f0_floor, double f0_ceil}, then the payload: stage 0 each utterance's y_len decimated samples,
 // stage 1 raw[n][nb][l1_stride], stage 2 base[n][l1_stride][32] + int32 count[n][l1_stride], stage 3
 // cand[n][l1_stride][max_cand] + score[n][l1_stride][max_cand] (before RemoveUnreliableCandidates).
-enum { HV_DUMP_DECIMATED, HV_DUMP_RAW, HV_DUMP_BASE, HV_DUMP_REFINED, HV_DUMP_STAGES };
+// Two more capture the decision stages: WB_DUMP_CLEANED (stage 4, after harvest_remove_kernel) the cleaned cand and
+// score in the stage 3 layout + base[n][l1_stride] (SearchF0Base), WB_DUMP_CONTOUR (stage 5, after
+// harvest_contour_kernel) steps[n][4][l1_stride] = FixStep1 .. FixStep4 (work rows 1 .. 4; the last is what
+// harvest_smooth_kernel smooths).
+// WB_LOAD_REFINED=<prefix> is the way in for tests of those stages: where WB_DUMP_REFINED is written, each chunk's
+// cand, score and nc are replaced by those of the stage 3 file <prefix>.<chunk>, whose n, l1_stride, max_cand and l1[]
+// must be the chunk's own (anything else is an error return, never a fallback), so that harvest_remove_kernel,
+// harvest_contour_kernel and harvest_smooth_kernel run, as launched here, on candidate maps the test chose.
+enum { HV_DUMP_DECIMATED, HV_DUMP_RAW, HV_DUMP_BASE, HV_DUMP_REFINED, HV_DUMP_CLEANED, HV_DUMP_CONTOUR, HV_DUMP_STAGES };
 struct HvDumpPart { const void *dev; size_t bytes; };
 
 static int hv_dump(Ctx *ctx, const char *prefix, int stage, int chunk, int u0, int n, int ratio, double afs, int nb,
@@ -1017,6 +1025,44 @@ static int hv_dump(Ctx *ctx, const char *prefix, int stage, int chunk, int u0, i
   for (const auto &h : host) fwrite(h.data(), 1, h.size(), f);
   fclose(f);
   return 0;
+}
+
+static int hv_load_refined(Ctx *ctx, const char *prefix, int chunk, int n, int l1_stride, int max_cand,
+                           const int *l1_host, double *cand_dev, double *score_dev, int *nc_dev) {
+  const std::string path = std::string(prefix) + "." + std::to_string(chunk);
+  auto fail = [&](const char *why) { ctx->last_error = "Harvest: WB_LOAD_REFINED " + path + ": " + why; return 3; };
+  FILE *f = fopen(path.c_str(), "rb");
+  if (!f) return fail("cannot read");
+  char magic[8];
+  long long head[10];
+  double afs;
+  const size_t rows = (size_t)n * l1_stride * max_cand;
+  std::vector<int> ints;
+  std::vector<double> cs;
+  const char *why = nullptr;
+  if (fread(magic, 1, 8, f) != 8 || memcmp(magic, "WBHVDUMP", 8) != 0 || fread(head, 8, 10, f) != 10 ||
+      fread(&afs, 8, 1, f) != 1) why = "not a WBHVDUMP file";
+  else if (head[0] != 1 || head[1] != HV_DUMP_REFINED) why = "not a version 1 refined-candidates (stage 3) file";
+  else if (head[4] != n || head[7] != l1_stride || head[8] != max_cand || head[9] < 0 || head[9] > 65535)
+    why = "n, l1_stride or max_cand differ from the chunk's";
+  if (!why) {
+    ints.resize((size_t)4 * n);
+    cs.resize(2 * rows);
+    if (fread(ints.data(), 4, ints.size(), f) != ints.size() || fseek(f, (long)head[9] * 20, SEEK_CUR) != 0 ||
+        fread(cs.data(), 8, cs.size(), f) != cs.size() || fgetc(f) != EOF) why = "payload size differs from the header's";
+  }
+  fclose(f);
+  if (why) return fail(why);
+  const int *l1 = ints.data() + 2 * (size_t)n, *nc = l1 + n;
+  for (int i = 0; i < n; ++i) {
+    if (l1[i] != l1_host[i]) return fail("l1[] differs from the chunk's frame counts");
+    if (nc[i] < 0 || nc[i] * 7 > max_cand) return fail("nc[] out of range");
+  }
+  int rc = dev_memcpy_h2d(ctx, nc_dev, nc, (size_t)n * 4);
+  if (!rc) rc = dev_memcpy_h2d(ctx, cand_dev, cs.data(), rows * 8);
+  if (!rc) rc = dev_memcpy_h2d(ctx, score_dev, cs.data() + rows, rows * 8);
+  if (!rc) rc = dev_sync(ctx);
+  return rc;
 }
 
 int harvest_check_options(Ctx *ctx, int fs, const HarvestParams *opts, int n) {
@@ -1071,6 +1117,9 @@ int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_ut
   const int lag = static_cast<int>(ceil(140.0 / ratio) * ratio);
   const size_t tmp_stride = ratio != 1 ? (size_t)b.max_x_len + 2 * lag + 32 : 0;
   const size_t pad_stride = (size_t)l1_stride + 600 + 8;
+  // multi-channel storage of harvest_contour_kernel: a section takes its frames + 208.  FixStep2 keeps sections of at
+  // least 7 frames (ed - st >= 6) and they lie at least one frame apart, so n sections need at most L + 208 n with
+  // n <= L / 8: 27 doubles per frame.  The kernel's overflow exit is a guard, not a reachable state.
   const size_t mc_stride = (size_t)28 * l1_stride + 1024;
   const int sec_slots = 32;
   const int seg_cap = l1_stride + 600 + 8;  // a section span never exceeds the padded contour
@@ -1085,7 +1134,8 @@ int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_ut
   for (int u0 = 0; u0 < b.n; u0 += chunk) {
     const int n = imin(chunk, b.n - u0);
     const char *dump[HV_DUMP_STAGES] = {getenv("WB_DUMP_DECIMATED"), getenv("WB_DUMP_RAW"), getenv("WB_DUMP_BASE"),
-                                        getenv("WB_DUMP_REFINED")};
+                                        getenv("WB_DUMP_REFINED"), getenv("WB_DUMP_CLEANED"), getenv("WB_DUMP_CONTOUR")};
+    const char *load_refined = getenv("WB_LOAD_REFINED");
     ArenaPlan plan;
     const size_t o_y = plan.add((size_t)n * y_stride * 8), o_ylen = plan.add((size_t)n * 4);
     const size_t o_l1 = plan.add((size_t)n * 4), o_nc = plan.add((size_t)n * 4);
@@ -1249,6 +1299,9 @@ int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_ut
     if (dump[HV_DUMP_REFINED] && (rc = dump_stage(HV_DUMP_REFINED, {{rp.cand, (size_t)slots * max_cand * 8},
                                                                     {rp.score, (size_t)slots * max_cand * 8}})))
       return rc;
+    if (load_refined && (rc = hv_load_refined(ctx, load_refined, u0 / chunk, n, l1_stride, max_cand, b.l1_host + u0,
+                                              rp.cand, rp.score, nc)))
+      return rc;
 
     HvRemoveParams mp;
     mp.cand_in = rp.cand; mp.score_in = rp.score; mp.cand = (double *)(blk + o_c2); mp.score = (double *)(blk + o_s2);
@@ -1260,12 +1313,22 @@ int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_ut
     const unsigned remove_blocks = (unsigned)((slots + WB_RM_WARPS - 1) / WB_RM_WARPS);
 #endif
     WB_LAUNCH_COOP(harvest_remove_kernel, dim3(remove_blocks), 32 * WB_RM_WARPS, 0, ctx->stream, mp);
+    if (dump[HV_DUMP_CLEANED]) {
+      std::vector<HvDumpPart> parts = {{mp.cand, (size_t)slots * max_cand * 8}, {mp.score, (size_t)slots * max_cand * 8}};
+      for (int i = 0; i < n; ++i) parts.push_back({mp.f0_base + (size_t)i * 5 * l1_stride, (size_t)l1_stride * 8});
+      if ((rc = dump_stage(HV_DUMP_CLEANED, parts))) return rc;
+    }
 
     HvContourParams cp;
     cp.cand = mp.cand; cp.score = mp.score; cp.nc = nc; cp.l1 = l1; cp.l1_stride = l1_stride; cp.max_cand = max_cand;
     cp.work = (double *)(blk + o_work); cp.iwork = (int *)(blk + o_iwork); cp.mc = (double *)(blk + o_mc);
     cp.mc_stride = mc_stride; cp.status = ctx->status_dev;
     WB_LAUNCH_COOP(harvest_contour_kernel, dim3((unsigned)n), 128, 0, ctx->stream, cp);
+    if (dump[HV_DUMP_CONTOUR]) {
+      std::vector<HvDumpPart> parts;
+      for (int i = 0; i < n; ++i) parts.push_back({cp.work + ((size_t)i * 5 + 1) * l1_stride, (size_t)4 * l1_stride * 8});
+      if ((rc = dump_stage(HV_DUMP_CONTOUR, parts))) return rc;
+    }
 
     HvSmoothParams hp;
     hp.work = cp.work; hp.l1_stride = l1_stride; hp.l1 = l1; hp.padded = (double *)(blk + o_pad);
