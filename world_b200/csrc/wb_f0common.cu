@@ -97,8 +97,10 @@ WB_DEV int first_frame_at_or_after(double x, double frame_period) {
 
 #ifdef WB_EMU
 static inline void smem_add_u64(unsigned long long *p, unsigned long long v) { *p += v; }
+static inline void smem_add_u32(unsigned *p, unsigned v) { *p += v; }
 #else
 __device__ __forceinline__ void smem_add_u64(unsigned long long *p, unsigned long long v) { atomicAdd(p, v); }
+__device__ __forceinline__ void smem_add_u32(unsigned *p, unsigned v) { atomicAdd(p, v); }
 #endif
 
 // Exclusive scan of G packed counters (4 x 16 bit) held in shared memory, in place; adds the
@@ -482,9 +484,8 @@ WB_KERNEL(WB_SWEEP_THREADS, 3) band_sweep_list_kernel(SweepParams p) {
 //                           per-train lists in global memory (written once, never read back here).  Three block
 //                           barriers per tile.  The input segment of the next tile arrives by TMA (cp.async.bulk +
 //                           mbarrier) while the current one is filtered.
-//   band_interp_kernel      edge lists -> intervals -> interp1 onto the frame grid, 256 frames per round; interval
-//                           counts per frame by a fill (every interval owns the frames between its first frame and
-//                           the next interval's), no search, no scan.
+//   band_interp_kernel      edge lists -> intervals -> interp1 onto the frame grid, rounds of up to 1024 frames;
+//                           interval counts per frame by marks and a scan, no search.
 // A band whose lists overflow their capacity (far more crossings than its frequency allows for: a loud out-of-band
 // tone) is left to the streaming kernel, whose history rings wrap instead (band_sweep_list_kernel).
 #ifndef WB_EMU
@@ -875,14 +876,53 @@ WB_KERNEL(2 * WB_FE_GROUP, 3) band_fir_events_kernel(SweepParams p) {
 }
 
 // ---- edge lists -> candidates
-// One CTA per (utterance, band); rounds of WB_IP_F frames, one frame per thread.  Per round and train a window of
-// intervals starting two before the cursor (the intervals already behind the round) is loaded into shared memory --
-// location x_j, value y_j and m_j = the first frame at or after x_j; its length follows the band (a 64 Hz band has
-// ~16 intervals per 256 ms, an 880 Hz band ~225).  interp1's segment index for frame i is cursor + #{j : m_j <= i}:
-// a binary search over the window's m.  A window that ends inside the round (far more crossings than the band
-// frequency suggests) leaves its last frames to the next iteration of the same round.
-#define WB_IP_F 256     // frames per round
-#define WB_IP_W 256     // intervals per train and window (capacity)
+// One CTA per (utterance, band); rounds of up to WB_IP_F frames, thread t taking frames t, t + 256, ... of the round.
+// Per round and train a window of intervals starting two before the cursor (the intervals already behind the round)
+// is loaded into shared memory -- location x_j and value y_j -- and each interval j adds one to the packed count of
+// m_j = the first frame at or after x_j.  interp1's segment index for frame i is cursor + #{j : m_j <= i}, the
+// inclusive scan of those counts.  The window length follows the band (a 64 Hz band has ~16 intervals per 256 ms, an
+// 880 Hz band ~225), and the round length follows the window: the longest of 1024, 512 and 256 frames whose expected
+// intervals fit, so a low band needs a quarter of the rounds (and of the block barriers) a high one does.  A window
+// that ends inside the round (far more crossings than the band frequency suggests) leaves its last frames to the next
+// iteration of the same round.
+#define WB_IP_F 1024    // frames per round (at most)
+#define WB_IP_W 512     // intervals per train and window (capacity)
+
+// In-place inclusive scan of the packed counts c[0, F), F a multiple of 256 and at most WB_IP_F; returns the total to
+// every thread.  CUDA path: 256 threads, thread t scans the entries t, t + 256, ... (the frames it evaluates, so it
+// reads back only what it wrote itself); one block barrier.
+WB_DEV unsigned long long ip_scan_inclusive(unsigned long long *c, int F, unsigned long long *warp_tot /* >= 32 */) {
+#ifdef WB_EMU
+  (void)warp_tot;
+  unsigned long long run = 0ull;
+  for (int i = 0; i < F; ++i) { run += c[i]; c[i] = run; }
+  return run;
+#else
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5, R = F >> 8;
+  unsigned long long inc[WB_IP_F / 256];
+#pragma unroll
+  for (int r = 0; r < WB_IP_F / 256; ++r) {
+    if (r >= R) break;
+    inc[r] = c[256 * r + tid];
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned long long t = __shfl_up_sync(0xffffffffu, inc[r], o);
+      if (lane >= o) inc[r] += t;
+    }
+    if (lane == 31) warp_tot[8 * r + w] = inc[r];
+  }
+  __syncthreads();
+  unsigned long long run = 0ull;
+#pragma unroll
+  for (int r = 0; r < WB_IP_F / 256; ++r) {
+    if (r >= R) break;
+    unsigned long long base = run;
+    for (int i = 0; i < 8; ++i) { const unsigned long long t = warp_tot[8 * r + i]; if (i < w) base += t; run += t; }
+    c[256 * r + tid] = base + inc[r];
+  }
+  return run;
+#endif
+}
+
 struct IpTrain {        // one train of one band: complete edge list in global memory
   const double *e; int n_int; double afs;
 };
@@ -903,8 +943,8 @@ WB_DEV int first_frame_fast(double x, double frame_period, double frames_per_sec
 
 WB_KERNEL(256, 4) band_interp_kernel(SweepParams p) {
   WB_SHARED double xw[4][WB_IP_W + 4], yw[4][WB_IP_W + 4];
-  WB_SHARED unsigned long long marks[WB_IP_F + 40];   // per frame: intervals whose first frame it is, 4 x 16 bit; + scan scratch
-  WB_SHARED unsigned long long orig[WB_IP_F];
+  WB_SHARED unsigned long long marks[WB_IP_F];   // per frame: intervals whose first frame it is, 4 x 16 bit
+  WB_SHARED unsigned long long warp_tot[32];     // scan scratch
   WB_SHARED int more_flag[2];   // "the last interval of a window still starts inside the round", per iteration parity
   const int tid = WB_TID, nth = WB_NTH;
   int u;
@@ -932,18 +972,24 @@ WB_KERNEL(256, 4) band_interp_kernel(SweepParams p) {
     }
     return;
   }
-  // window length of this band: intervals expected per round (band frequency x round duration) + 65 %, at least 24
-  int w_band = (int)(bf * 1.1 * (WB_IP_F * p.frame_period / 1000.0) * 1.65) + 24;
+  // round and window length of this band: intervals expected per round (band frequency x round duration) + 65 %, at
+  // least 24; the round halves (down to 256 frames) until they fit the window
+  int F = WB_IP_F, w_band = 0;
+  for (;; F >>= 1) {
+    w_band = (int)(bf * 1.1 * (F * p.frame_period / 1000.0) * 1.65) + 24;
+    if (w_band <= WB_IP_W || F == 256) break;
+  }
   if (w_band > WB_IP_W) w_band = WB_IP_W;
   const double fps = 1000.0 / p.frame_period;
+  // the marks are cleared here once and then by the threads that read them; both flags are zero after every round
+  for (int i = tid; i < WB_IP_F; i += nth) marks[i] = 0ull;
+  for (int i = tid; i < 2; i += nth) more_flag[i] = 0;
+  WB_SYNC();
   int cursor[4] = {0, 0, 0, 0};   // intervals whose first frame lies before the current round (identical in every thread)
-  for (int c0 = 0; c0 < nf; c0 += WB_IP_F) {
-    const int c1 = imin(nf, c0 + WB_IP_F);
-    for (int i = tid; i < WB_IP_F; i += nth) marks[i] = 0ull;
-    for (int i = tid; i < 2; i += nth) more_flag[i] = 0;
+  for (int c0 = 0; c0 < nf; c0 += F) {
+    const int c1 = imin(nf, c0 + F);
     int at[4] = {cursor[0], cursor[1], cursor[2], cursor[3]};   // first interval not yet examined in this round
     int wbase[4] = {0, 0, 0, 0}, wlen[4] = {0, 0, 0, 0};
-    WB_SYNC();
     bool more = true;
     // One pass over the (train, interval) pairs of all four windows: the four trains' loads and divisions run side by
     // side instead of one latency chain after the other (otherwise the kernel waits at the barrier
@@ -970,7 +1016,9 @@ WB_KERNEL(256, 4) band_interp_kernel(SweepParams p) {
         if (k >= aq - wb) {   // interval (wbase + k) is counted by every frame from its first frame on
           const int m = first_frame_fast(x, p.frame_period, fps);
           if (m < c1) {
-            smem_add_u64(&marks[imax(m, c0) - c0], 1ull << (16 * q));
+            // += 1 << 16 q on the 32-bit half that holds train q's field (little endian; no field carries into the
+            // next): a native shared-memory atomic, where a 64-bit add compiles to a compare-and-swap loop
+            smem_add_u32(reinterpret_cast<unsigned *>(&marks[imax(m, c0) - c0]) + (q >> 1), 1u << (16 * (q & 1)));
             if (k == wl - 1 && wb + wl < ni) more_flag[itn & 1] = 1;   // may be followed by more of them
           }
         }
@@ -981,12 +1029,11 @@ WB_KERNEL(256, 4) band_interp_kernel(SweepParams p) {
       for (int q = 0; q < 4; ++q) at[q] = wbase[q] + wlen[q];
       if (more) WB_SYNC();   // the windows are rewritten
     }
-    // inclusive counts per frame: exclusive scan + the frame's own marks
-    for (int i = tid; i < WB_IP_F; i += nth) orig[i] = marks[i];
-    WB_SYNC();
-    const unsigned long long all = scan_packed(marks, WB_IP_F, 0ull, marks + WB_IP_F + 4);
+    // inclusive counts per frame
+    const unsigned long long all = ip_scan_inclusive(marks, F, warp_tot);
     for (int i = c0 + tid; i < c1; i += nth) {
-      const unsigned long long inc = marks[i - c0] + orig[i - c0];
+      const unsigned long long inc = marks[i - c0];
+      marks[i - c0] = 0ull;
       const double t = i * p.frame_period / 1000.0;
       double v[4];
 #pragma unroll

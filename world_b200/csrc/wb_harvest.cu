@@ -92,33 +92,63 @@ struct HvDetectParams {
   int n_utts;
 };
 
-WB_KERNEL_PLAIN harvest_detect_kernel(HvDetectParams p) {
-  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= (long long)p.n_utts * p.l1_stride) return;
-  const int u = (int)(g / p.l1_stride), i = (int)(g % p.l1_stride);
-  if (i >= p.l1[u]) return;
-  const double *raw = p.raw + (size_t)u * p.n_bands * p.l1_stride + i;
+// One thread per 1 ms frame; a warp reads 32 consecutive frames of a band row (256 contiguous bytes).  The bands are
+// loaded WB_HV_DETECT_BATCH at a time into registers before the state machine runs over them, so that many row
+// loads are in flight per thread instead of one load, then a compare, then the next.
+#define WB_HV_DETECT_BATCH 16
+WB_DEV int hv_detect_frame(const HvDetectParams &p, int u, int i, double *out) {
+  const double *__restrict__ raw = p.raw + (size_t)u * p.n_bands * p.l1_stride + i;
   const int nb = p.gr.grp_nb[p.gr.ugrp[u]];
-  double *out = p.base + (size_t)g * WB_HV_BASE;
   int count = 0, prev = 0, st = 0;
   double sum = 0.0;
   // vuv[0] = vuv[nb-1] = 0; a section [st, ed) is closed when vuv falls (harvest.cpp:348-385)
-  for (int j = 1; j < nb; ++j) {
-    const int v = (j == nb - 1) ? 0 : (raw[(size_t)j * p.l1_stride] > 0 ? 1 : 0);
-    if (v - prev == 1) { st = j; sum = 0.0; }
-    if (v) sum += raw[(size_t)j * p.l1_stride];
-    if (v - prev == -1) {
-      if (j - st >= 10 && count < WB_HV_BASE) out[count++] = sum / (j - st);
+  for (int j0 = 1; j0 < nb; j0 += WB_HV_DETECT_BATCH) {
+    double r[WB_HV_DETECT_BATCH];
+#pragma unroll
+    for (int k = 0; k < WB_HV_DETECT_BATCH; ++k) r[k] = j0 + k < nb - 1 ? raw[(size_t)(j0 + k) * p.l1_stride] : 0.0;
+#pragma unroll
+    for (int k = 0; k < WB_HV_DETECT_BATCH; ++k) {
+      const int j = j0 + k;
+      if (j >= nb) break;
+      const int v = r[k] > 0 ? 1 : 0;   // 0 for j = nb - 1
+      if (v - prev == 1) { st = j; sum = 0.0; }
+      if (v) sum += r[k];
+      if (v - prev == -1) {
+        if (j - st >= 10 && count < WB_HV_BASE) out[count++] = sum / (j - st);
+      }
+      prev = v;
     }
-    prev = v;
   }
   for (int c = count; c < WB_HV_BASE; ++c) out[c] = 0.0;
-  p.base_count[g] = count;
+  return count;
+}
+
+// A frame's 32 base slots are collected in shared memory, and the CTA's 128 frames (one contiguous 32 KB block of
+// `base`) are stored together, coalesced.  A thread storing its own 256-byte row made every store instruction of a
+// warp touch 32 sectors 256 bytes apart.
+#define WB_HV_DETECT_THREADS 128
+WB_KERNEL(WB_HV_DETECT_THREADS, 4) harvest_detect_kernel(HvDetectParams p) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long slots = (long long)p.n_utts * p.l1_stride;
+  const int u = g < slots ? (int)(g / p.l1_stride) : 0, i = g < slots ? (int)(g % p.l1_stride) : 0;
+  const bool active = g < slots && i < p.l1[u];
 #ifdef WB_EMU
+  if (!active) return;
+  const int count = hv_detect_frame(p, u, i, p.base + (size_t)g * WB_HV_BASE);
   if (count > p.nc[u]) p.nc[u] = count;
 #else
+  __shared__ double tile[WB_HV_DETECT_THREADS][WB_HV_BASE + 1];
+  __shared__ int tile_ok[WB_HV_DETECT_THREADS];
+  tile_ok[threadIdx.x] = active;
+  const int count = active ? hv_detect_frame(p, u, i, tile[threadIdx.x]) : 0;
+  __syncthreads();
+  double *dst = p.base + (size_t)blockIdx.x * blockDim.x * WB_HV_BASE;   // frames past l1 or the batch are not written
+  for (int e = threadIdx.x; e < WB_HV_DETECT_THREADS * WB_HV_BASE; e += blockDim.x)
+    if (tile_ok[e / WB_HV_BASE]) dst[e] = tile[e / WB_HV_BASE][e % WB_HV_BASE];
+  if (!active) return;
   if (count > 0) atomicMax(&p.nc[u], count);
 #endif
+  p.base_count[g] = count;
 }
 
 // ------------------------------------------------------------------ K-HVr
@@ -543,20 +573,45 @@ struct HvRemoveParams {
 
 // min(1, min_c |reference - row[c]| / reference): SelectBestF0's error with allowed_range 1.0
 // (harvest.cpp:657-661).  Division by the positive reference is monotone under rounding, so the
-// minimum of the quotients is the quotient of the minimum: one division per call.
-WB_DEV double hv_min_rel_error(double reference, const double *row, int n) {
-  double dmin_abs = fabs(reference - row[0]);
-  for (int c = 1; c < n; ++c) dmin_abs = dmin(dmin_abs, fabs(reference - row[c]));
+// minimum of the quotients is the quotient of the minimum: one division per call.  `nz` holds only the
+// row's non-zero slots: a zero slot contributes |reference - 0| = |reference|, i.e. an error of exactly 1, the
+// clamp value, so starting the minimum at |reference| instead of visiting the zeros gives the same result.
+WB_DEV double hv_min_rel_error(double reference, const double *nz, int n_nz) {
+  double dmin_abs = fabs(reference);
+  for (int c = 0; c < n_nz; ++c) dmin_abs = dmin(dmin_abs, fabs(reference - nz[c]));
   const double e = dmin_abs / reference;
   return e > 1.0 ? 1.0 : e;
 }
 
+// Copies the non-zero entries of row[0, n) to nz in slot order (warp-cooperative); returns their number.
+WB_DEV int hv_compact_nonzero(const double *row, int n, double *nz) {
+#ifdef WB_EMU
+  int k = 0;
+  for (int j = 0; j < n; ++j)
+    if (row[j] != 0) nz[k++] = row[j];
+  return k;
+#else
+  const unsigned lane = threadIdx.x & 31;
+  int k = 0;
+  for (int j0 = 0; j0 < n; j0 += 32) {
+    const double v = j0 + (int)lane < n ? row[j0 + lane] : 0.0;
+    const unsigned m = __ballot_sync(0xffffffffu, v != 0);
+    if (v != 0) nz[k + __popc(m & ((1u << lane) - 1u))] = v;
+    k += __popc(m);
+  }
+  __syncwarp();
+  return k;
+#endif
+}
+
 // One warp per 1 ms frame, lanes over the frame's candidate slots (round 1 ran one THREAD per frame: rows of 105
-// doubles read with an 840-byte stride between threads; 40 ms per 1024 x 10 s).  Neighbour rows are read by all
-// lanes at the same address (broadcast).  SearchF0Base keeps the FIRST slot with the highest score: the warp
-// arg-max breaks ties towards the lower slot index.
+// doubles read with an 840-byte stride between threads; 40 ms per 1024 x 10 s).  The two neighbour rows are
+// compacted to their non-zero slots in shared memory first (most slots are empty), and each candidate is compared
+// against those only.  SearchF0Base keeps the FIRST slot with the highest score: the warp arg-max breaks ties
+// towards the lower slot index.
 #define WB_RM_WARPS 8
 WB_KERNEL(32 * WB_RM_WARPS, 4) harvest_remove_kernel(HvRemoveParams p) {
+  WB_SHARED double nz[WB_RM_WARPS][2][7 * WB_HV_BASE];   // per warp: the non-zero slots of rows i + 1 and i - 1
 #ifdef WB_EMU
   const int warp = 0, nwarps = 1;
 #else
@@ -573,13 +628,18 @@ WB_KERNEL(32 * WB_RM_WARPS, 4) harvest_remove_kernel(HvRemoveParams p) {
   double *oc = p.cand + (size_t)g * p.max_cand, *os = p.score + (size_t)g * p.max_cand;
   const double *srow = p.score_in + (size_t)g * p.max_cand;
   const bool interior = i >= 1 && i < L1 - 1;
+  int n_next = 0, n_prev = 0;
+  if (interior) {
+    n_next = hv_compact_nonzero(row + p.max_cand, n, nz[warp][0]);
+    n_prev = hv_compact_nonzero(row - p.max_cand, n, nz[warp][1]);
+  }
   double best = 0.0, best_score = 0.0;  // SearchF0Base (harvest.cpp:693-705) on the cleaned candidates
   int best_j = 0x7fffffff;
   for (int j = lane; j < n; j += WB_LANES) {
     double c = row[j], s = srow[j];
     if (interior && c != 0) {
-      const double e1 = hv_min_rel_error(c, row + p.max_cand, n);
-      const double e2 = hv_min_rel_error(c, row - p.max_cand, n);
+      const double e1 = hv_min_rel_error(c, nz[warp][0], n_next);
+      const double e2 = hv_min_rel_error(c, nz[warp][1], n_prev);
       if (dmin(e1, e2) > 0.05) { c = 0.0; s = 0.0; }
     }
     oc[j] = c; os[j] = s;
@@ -1262,7 +1322,8 @@ int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_ut
     HvDetectParams dp;
     dp.raw = sp.cand; dp.n_bands = nb; dp.l1_stride = l1_stride; dp.l1 = l1; dp.gr = gr;
     dp.base = (double *)(blk + o_base); dp.base_count = (int *)(blk + o_bcnt); dp.nc = nc; dp.n_utts = n;
-    WB_LAUNCH_FLAT(harvest_detect_kernel, dim3((unsigned)((slots + 127) / 128)), 128, 0, ctx->stream, dp);
+    WB_LAUNCH_FLAT(harvest_detect_kernel, dim3((unsigned)((slots + WB_HV_DETECT_THREADS - 1) / WB_HV_DETECT_THREADS)),
+                   WB_HV_DETECT_THREADS, 0, ctx->stream, dp);
 
     if (dump[HV_DUMP_BASE] && (rc = dump_stage(HV_DUMP_BASE, {{dp.base, (size_t)slots * WB_HV_BASE * 8},
                                                               {dp.base_count, (size_t)slots * 4}})))
