@@ -204,6 +204,56 @@ int world_b200_synthesis_coded_host(WorldB200 *ctx, const double *f0, const int 
                                     const double *coded_aperiodicity, int fft_size, double frame_period, int fs,
                                     const int *y_lengths, int y_stride, int nbit, void *y);
 
+/* ---- voice modification: F0 scaling and formant shift (the reference demo's ParameterModification,
+ * test/test.cpp:221-258), one factor per utterance --------------------------------------------------------------
+ * For utterance u with shift = f0_scale[u], ratio = spectral_ratio[u] and bins = fft_size/2 + 1, every frame
+ * i < f0_length is changed as the reference changes it:
+ *     f0[i] *= shift                                   (unvoiced frames stay 0)
+ *     sp[i][j] = exp(interp1(x, log(sp[i]), xi)[j])     x[m] = ratio * m / fft_size * fs, xi[m] = (double)m / fft_size * fs
+ *     ratio < 1: sp[i][j] = sp[i][c - 1] for j >= c = (int)(fft_size / 2.0 * ratio)
+ * (interp1 extrapolates with its last segment; ratio 1.0 still takes the log / exp round trip.)  Aperiodicity is not
+ * changed, and nothing is analysed again: scale after all analysis, as the reference does.
+ *   - f0 [n_utts][f0_stride] and spectrogram [n_utts][f0_stride][fft_size/2+1] are DEVICE rows, changed in place;
+ *     f0_lengths is HOST or NULL (full rows); f0_scale and spectral_ratio are HOST arrays of n_utts.  Either may be
+ *     NULL, which skips that half; f0 or spectrogram may then be NULL too.  Padding frames are never written.
+ *   - The segment and weight of each bin are planned on the host once per distinct ratio (the reference's expressions
+ *     and its histc), and the kernel rounds y[k-1] + s * (y[k] - y[k-1]) step by step, without FMA.  So f0 equals the
+ *     reference bit for bit, and an envelope differs from it only through the device's log / exp (within 1e-12
+ *     relative of the host's libm).
+ *   - Validation, before any work is queued (WORLD_B200_EINVAL, world_b200_last_error() naming the first bad
+ *     utterance): f0_lengths within [0, f0_stride]; a factor that is not finite or not > 0; with spectral_ratio,
+ *     fft_size a power of two in [16, 4096], fs > 0, and no ratio with c == 0 (the reference would read sp[-1]).
+ *   - Like the other *_batch stages the call does not synchronise. */
+int world_b200_modify_batch(WorldB200 *ctx, double *f0, const int *f0_lengths, int n_utts, int f0_stride,
+                            double *spectrogram, int fft_size, int fs, const double *f0_scale,
+                            const double *spectral_ratio);
+/* world_b200_synthesis_coded_batch with the modification applied inside: the arguments of that call plus f0_scale and
+ * spectral_ratio (HOST arrays of n_utts, NULL = none) and nbit (0: y is float64, 16: y is int16 quantised as
+ * world_b200_synthesis_coded_batch_pcm16 quantises; anything else is EINVAL).  The caller's f0 and coded rows are not
+ * changed: each chunk of utterances synthesises from a scaled copy of its f0 rows (held in the call's scratch, so
+ * the time base, the pulse count and a relaid pass all see the scaled contour) and stretches its decoded envelope
+ * block right after the decode.
+ *   - Output: equal bit for bit to world_b200_decode_spectral_envelope_batch -> world_b200_modify_batch ->
+ *     world_b200_decode_aperiodicity_batch -> world_b200_synthesis_batch for the same utterance (nbit 0), or to the
+ *     pcm16 rule applied to that waveform (nbit 16).  With both arrays NULL it is world_b200_synthesis_coded_batch /
+ *     _pcm16, on exactly their path.
+ *   - Validation is that of world_b200_synthesis_coded_batch and of world_b200_modify_batch, all before any work is
+ *     queued.  Stream behaviour as world_b200_synthesis_coded_batch. */
+int world_b200_synthesis_coded_batch_modified(WorldB200 *ctx, const double *f0, const int *f0_lengths, int n_utts,
+                                              int f0_stride, const double *coded_spectral_envelope,
+                                              int number_of_dimensions, const double *coded_aperiodicity,
+                                              int fft_size, double frame_period, int fs, const int *y_lengths,
+                                              int y_stride, const double *f0_scale, const double *spectral_ratio,
+                                              int nbit, void *y);
+/* The same for HOST arrays through the pipeline of world_b200_synthesis_coded_host (which slices f0_scale and
+ * spectral_ratio with the utterance chunks): equal bit for bit to world_b200_synthesis_coded_batch_modified. */
+int world_b200_synthesis_coded_host_modified(WorldB200 *ctx, const double *f0, const int *f0_lengths, int n_utts,
+                                             int f0_stride, const double *coded_spectral_envelope,
+                                             int number_of_dimensions, const double *coded_aperiodicity,
+                                             int fft_size, double frame_period, int fs, const int *y_lengths,
+                                             int y_stride, const double *f0_scale, const double *spectral_ratio,
+                                             int nbit, void *y);
+
 /* ---- codec over a batch (codec.h:20-92) -- SURVEY.md 8 row f2; all DEVICE pointers ------ */
 /* aperiodicity [n][f0_stride][fft_size/2+1] -> coded [n][f0_stride][GetNumberOfAperiodicities(fs)]. */
 int world_b200_code_aperiodicity_batch(WorldB200 *ctx, const double *aperiodicity, int n_utts,

@@ -90,6 +90,11 @@ ABI = {
                                                          C.c_double, C.c_int, _IP, C.c_int, _P]),
     "world_b200_synthesis_coded_host": (C.c_int, [_P, _P, _IP, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, C.c_double,
                                                   C.c_int, _IP, C.c_int, C.c_int, _P]),
+    "world_b200_modify_batch": (C.c_int, [_P, _P, _IP, C.c_int, C.c_int, _P, C.c_int, C.c_int, _P, _P]),
+    "world_b200_synthesis_coded_batch_modified": (C.c_int, [_P, _P, _IP, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int,
+                                                            C.c_double, C.c_int, _IP, C.c_int, _P, _P, C.c_int, _P]),
+    "world_b200_synthesis_coded_host_modified": (C.c_int, [_P, _P, _IP, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int,
+                                                           C.c_double, C.c_int, _IP, C.c_int, _P, _P, C.c_int, _P]),
     "world_b200_default_analysis_option": (None, [C.c_int, C.c_int, C.POINTER(AnalysisOption)]),
     "world_b200_analyze_host": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(AnalysisOption),
                                           _P, _P, C.c_int, _P, _P]),
@@ -268,6 +273,20 @@ def _pcm16(dtype):
     if name == "int16":
         return True
     raise ValueError(f"dtype must be float64 or int16, not {dtype}")
+
+
+def _factors(v, n, what):
+    """None, one factor for every utterance, or a sequence of n factors -> a ctypes double array (or None)."""
+    if v is None:
+        return None
+    if hasattr(v, "tolist"):
+        v = v.tolist()
+    if isinstance(v, (int, float)):
+        v = [v] * n
+    v = [float(t) for t in v]
+    if len(v) != n:
+        raise ValueError(f"{what}: {len(v)} factors for {n} utterances")
+    return (C.c_double * n)(*v)
 
 
 def _int_array(v, n):
@@ -533,12 +552,15 @@ class World:
         return y
 
     def synthesis_coded(self, f0, coded_spectral_envelope, coded_aperiodicity, fft_size, frame_period, fs, y_length,
-                        f0_lengths=None, y_lengths=None, dtype=None):
+                        f0_lengths=None, y_lengths=None, dtype=None, f0_scale=None, spectral_ratio=None):
         """Batched Synthesis() from coded rows: f0 [n, L], coded_spectral_envelope [n, L, number_of_dimensions],
         coded_aperiodicity [n, L, GetNumberOfAperiodicities(fs)] -> y [n, y_length].  The rows are decoded chunk by
         chunk inside the call; the output equals decode_spectral_envelope + decode_aperiodicity + synthesis bit for
         bit.  coded_aperiodicity may be None below 12 kHz (no bands).  dtype: float64 (default) for the waveform, or
-        int16 for its 16-bit PCM, quantised as wavwrite does by the overlap-add kernel itself."""
+        int16 for its 16-bit PCM, quantised as wavwrite does by the overlap-add kernel itself.
+        f0_scale / spectral_ratio (one factor, or one per utterance): synthesise the voice changed as modify() changes
+        it, without touching the inputs (world_b200_synthesis_coded_batch_modified); the output equals decode +
+        modify + synthesis bit for bit."""
         pcm16 = _pcm16(dtype)
         n = f0.shape[0]
         if pcm16 and self.xp == "torch":
@@ -550,20 +572,42 @@ class World:
             y = self._zeros(f0, (n, y_length))
         fl, k1 = _int_array(f0_lengths, n)
         yl, k2 = _int_array(y_lengths, n)
-        fn = self.lib.world_b200_synthesis_coded_batch_pcm16 if pcm16 else self.lib.world_b200_synthesis_coded_batch
         self._use_current_stream()
+        if f0_scale is not None or spectral_ratio is not None:
+            self._check(self.lib.world_b200_synthesis_coded_batch_modified(
+                self._h, _ptr(f0), fl, n, f0.shape[1], _ptr(coded_spectral_envelope),
+                int(coded_spectral_envelope.shape[-1]), _ptr(coded_aperiodicity), fft_size, frame_period, fs, yl,
+                y_length, _factors(f0_scale, n, "f0_scale"), _factors(spectral_ratio, n, "spectral_ratio"),
+                16 if pcm16 else 0, _ptr(y)))
+            return y
+        fn = self.lib.world_b200_synthesis_coded_batch_pcm16 if pcm16 else self.lib.world_b200_synthesis_coded_batch
         self._check(fn(self._h, _ptr(f0), fl, n, f0.shape[1], _ptr(coded_spectral_envelope),
                        int(coded_spectral_envelope.shape[-1]), _ptr(coded_aperiodicity), fft_size, frame_period, fs,
                        yl, y_length, _ptr(y)))
         return y
 
+    def modify(self, f0, spectrogram, fs, fft_size, f0_scale=None, spectral_ratio=None, f0_lengths=None):
+        """F0 scaling and formant shift in place (world_b200_modify_batch, the reference demo's ParameterModification):
+        f0 [n, L] *= f0_scale, and each envelope row [n, L, fft_size/2+1] is stretched along frequency by
+        spectral_ratio.  Either factor may be one number for every utterance, a sequence of one per utterance, or None
+        to leave that array alone (it may then be None too).  Returns (f0, spectrogram)."""
+        rows = f0 if f0 is not None else spectrogram
+        n, L = int(rows.shape[0]), int(rows.shape[1])
+        fl, k1 = _int_array(f0_lengths, n)
+        self._use_current_stream()
+        self._check(self.lib.world_b200_modify_batch(self._h, _ptr(f0), fl, n, L, _ptr(spectrogram), fft_size, fs,
+                                                     _factors(f0_scale, n, "f0_scale"),
+                                                     _factors(spectral_ratio, n, "spectral_ratio")))
+        return f0, spectrogram
+
     def synthesis_coded_host(self, f0, coded_sp, coded_ap, fft_size, frame_period, fs, y_length, nbit=16,
-                             f0_lengths=None, y_lengths=None, out=None):
+                             f0_lengths=None, y_lengths=None, out=None, f0_scale=None, spectral_ratio=None):
         """synthesis_coded for HOST arrays (numpy arrays or CPU tensors, float64): upload, synthesis and download are
         pipelined over utterance chunks (world_b200_synthesis_coded_host).  Returns y [n, y_length] as a numpy array,
         int16 for nbit 16 or float64 for nbit 0, whole rows (samples beyond an utterance's y_length are 0).  out: a
         host array of that shape and dtype to write into (a pinned one lets the downloads overlap the kernels).
-        coded_ap may be None below 12 kHz (no bands)."""
+        coded_ap may be None below 12 kHz (no bands).  f0_scale / spectral_ratio as in synthesis_coded
+        (world_b200_synthesis_coded_host_modified)."""
         import numpy as np
 
         def host(a):
@@ -583,6 +627,12 @@ class World:
             raise ValueError(f"out: a contiguous [{n}, {y_length}] {'int16' if nbit == 16 else 'float64'} host array")
         fl, k1 = _int_array(f0_lengths, n)
         yl, k2 = _int_array(y_lengths, n)
+        if f0_scale is not None or spectral_ratio is not None:
+            self._check(self.lib.world_b200_synthesis_coded_host_modified(
+                self._h, _ptr(f0), fl, n, f0.shape[1], _ptr(coded_sp), int(coded_sp.shape[-1]), _ptr(coded_ap),
+                fft_size, frame_period, fs, yl, y_length, _factors(f0_scale, n, "f0_scale"),
+                _factors(spectral_ratio, n, "spectral_ratio"), nbit, _ptr(y)))
+            return y
         self._check(self.lib.world_b200_synthesis_coded_host(self._h, _ptr(f0), fl, n, f0.shape[1], _ptr(coded_sp),
                                                              int(coded_sp.shape[-1]), _ptr(coded_ap), fft_size,
                                                              frame_period, fs, yl, y_length, nbit, _ptr(y)))

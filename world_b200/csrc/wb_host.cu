@@ -347,7 +347,7 @@ namespace {
 // (synthesis_lengths).
 int synthesis_pipeline(WorldB200 *h, CodedRows *coded, int lg, const double *f0, const int *f0_lengths, int n_utts,
                        int f0_stride, int fft_size, double frame_period, int fs, const int *y_lengths, int y_stride,
-                       const int *lens, int nbit, void *y) {
+                       const int *lens, int nbit, void *y, const ModifyPlan *mod) {
   Ctx *ctx = ctx_of(h);
   const int dims = coded->tsp.dims, n_ap = coded->tap.dims;
   const double *h_sp = coded->sp, *h_ap = coded->ap;
@@ -355,7 +355,7 @@ int synthesis_pipeline(WorldB200 *h, CodedRows *coded, int lg, const double *f0,
   const size_t per_in = (size_t)f0_stride * (1 + dims + n_ap) * 8, per_out = (size_t)y_stride * out_bytes;
   int max_y = 0;
   for (int i = 0; i < n_utts; ++i) max_y = imax(max_y, lens[n_utts + i]);
-  const SynthesisSizing sz(ctx, coded, fft_size, f0_stride, y_stride, max_y, fs);
+  const SynthesisSizing sz(ctx, coded, fft_size, f0_stride, y_stride, max_y, fs, mod);
   int ring = 3;
   const size_t third = ctx->scratch_budget / 3;
   int chunk = imax(1, sz.fit(sz.nominal_cap));
@@ -466,7 +466,7 @@ int synthesis_pipeline(WorldB200 *h, CodedRows *coded, int lg, const double *f0,
     if (!rc)
       rc = synthesis_run(ctx, (const double *)(d + o_f0), f0_lengths ? f0_lengths + u0 : nullptr, m, f0_stride, nullptr,
                          nullptr, coded, fft_size, lg, frame_period, fs, y_lengths ? y_lengths + u0 : nullptr, y_stride,
-                         dout[slot].p, nbit);
+                         dout[slot].p, nbit, mod, u0);
     if (rc) break;
     unsigned char *dst = (unsigned char *)y + (size_t)u0 * per_out;
 #ifndef WB_EMU
@@ -520,13 +520,12 @@ int synthesis_pipeline(WorldB200 *h, CodedRows *coded, int lg, const double *f0,
   return rc;
 }
 
-}  // namespace
-
-extern "C" int world_b200_synthesis_coded_host(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts,
-                                               int f0_stride, const double *coded_spectral_envelope,
-                                               int number_of_dimensions, const double *coded_aperiodicity,
-                                               int fft_size, double frame_period, int fs, const int *y_lengths,
-                                               int y_stride, int nbit, void *y) {
+// world_b200_synthesis_coded_host and, with f0_scale / spectral_ratio, world_b200_synthesis_coded_host_modified
+int synthesis_coded_host(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts, int f0_stride,
+                         const double *coded_spectral_envelope, int number_of_dimensions,
+                         const double *coded_aperiodicity, int fft_size, double frame_period, int fs,
+                         const int *y_lengths, int y_stride, int nbit, void *y, const double *f0_scale,
+                         const double *spectral_ratio) {
   if (!h || !f0 || !coded_spectral_envelope || !y || n_utts < 0 || fs <= 0 || frame_period <= 0)
     return WORLD_B200_EINVAL;
   DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
@@ -541,6 +540,10 @@ extern "C" int world_b200_synthesis_coded_host(WorldB200 *h, const double *f0, c
   CodedRows coded;
   rc = synthesis_coded_tables(ctx, fs, fft_size, number_of_dimensions, coded_aperiodicity != nullptr, &coded);
   if (rc) return rc;
+  ModifyPlan mod;
+  const bool modified = f0_scale || spectral_ratio;
+  if (modified) rc = modify_plan(ctx, n_utts, fft_size, fs, f0_scale, spectral_ratio, &mod);
+  if (rc) return rc;
   if (n_utts == 0) return 0;
   // every length is checked before the first chunk is queued
   std::vector<int> lens((size_t)2 * n_utts);
@@ -549,7 +552,31 @@ extern "C" int world_b200_synthesis_coded_host(WorldB200 *h, const double *f0, c
   coded.sp = coded_spectral_envelope;
   coded.ap = coded.tap.dims > 0 ? coded_aperiodicity : nullptr;
   return synthesis_pipeline(h, &coded, lg, f0, f0_lengths, n_utts, f0_stride, fft_size, frame_period, fs, y_lengths,
-                            y_stride, lens.data(), nbit, y);
+                            y_stride, lens.data(), nbit, y, modified ? &mod : nullptr);
+}
+
+}  // namespace
+
+extern "C" int world_b200_synthesis_coded_host(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts,
+                                               int f0_stride, const double *coded_spectral_envelope,
+                                               int number_of_dimensions, const double *coded_aperiodicity,
+                                               int fft_size, double frame_period, int fs, const int *y_lengths,
+                                               int y_stride, int nbit, void *y) {
+  return synthesis_coded_host(h, f0, f0_lengths, n_utts, f0_stride, coded_spectral_envelope, number_of_dimensions,
+                              coded_aperiodicity, fft_size, frame_period, fs, y_lengths, y_stride, nbit, y, nullptr,
+                              nullptr);
+}
+
+extern "C" int world_b200_synthesis_coded_host_modified(WorldB200 *h, const double *f0, const int *f0_lengths,
+                                                        int n_utts, int f0_stride,
+                                                        const double *coded_spectral_envelope,
+                                                        int number_of_dimensions, const double *coded_aperiodicity,
+                                                        int fft_size, double frame_period, int fs,
+                                                        const int *y_lengths, int y_stride, const double *f0_scale,
+                                                        const double *spectral_ratio, int nbit, void *y) {
+  return synthesis_coded_host(h, f0, f0_lengths, n_utts, f0_stride, coded_spectral_envelope, number_of_dimensions,
+                              coded_aperiodicity, fft_size, frame_period, fs, y_lengths, y_stride, nbit, y, f0_scale,
+                              spectral_ratio);
 }
 
 extern "C" int world_b200_analyze_host(WorldB200 *h, const double *x, int n_utts, int x_stride,

@@ -165,6 +165,31 @@ struct CodedRows {            // Synthesis from coded rows: the decode tables, m
   const double *sp, *ap;      // [n][f0_stride][tsp.dims], [n][f0_stride][tap.dims] (ap null when tap.dims == 0)
   CodecTables tsp, tap;
 };
+// wb_synthesis.cu: F0 scaling and spectral stretch (the reference demo's ParameterModification, test.cpp:221-258).
+// The interp1 segment and weight of each output bin depend only on (ratio, fft_size, fs), so they are planned on the
+// host once per distinct ratio; the tail rule (bins >= c copy bin c-1 when ratio < 1) is folded into the table.
+struct ModifyPlan {
+  std::vector<double> scale;   // [n_utts] f0 factor of each utterance; empty: f0 is not scaled
+  std::vector<int> table;      // [n_utts] stretch table of each utterance; empty: the envelope is not stretched
+  std::vector<int> idx;        // [n_tables][bins] a = k - 1 of interp1's segment (the kernel reads L[a], L[a + 1])
+  std::vector<double> frac;    // [n_tables][bins] s = (xi - x[a]) / (x[a + 1] - x[a])
+  int n_tables = 0, bins = 0;
+  size_t device_bytes(int n) const;   // arena bytes of one pass of n utterances: tables, factors, table indices
+};
+// Checks every factor (finite, > 0; a ratio below 1 must keep c = (int)(fft_size / 2.0 * ratio) >= 1) and builds the
+// plan; EINVAL with last_error naming the first bad utterance.  Either array may be null.
+int modify_plan(Ctx *ctx, int n_utts, int fft_size, int fs, const double *f0_scale, const double *spectral_ratio,
+                ModifyPlan *plan);
+// Plan entries [u0, u0 + n) in device memory (layout of device_bytes); the copies are enqueued on ctx->stream.
+struct ModifyDevice { const double *scale; const int *table; const int *idx; const double *frac; };
+int modify_upload(Ctx *ctx, const ModifyPlan &plan, int u0, int n, unsigned char *blk, ModifyDevice *d);
+// f0_out[u][i] = f0_in[u][i] * scale[u] for i < f_len[u] (f0_out may alias f0_in)
+void modify_f0_launch(Ctx *ctx, const ModifyDevice &d, const int *f_len, int n_utts, int f_stride, int max_f,
+                      const double *f0_in, double *f0_out);
+// the envelope rows [n][f_stride][bins] stretched in place, frames < f_len[u]
+void modify_stretch_launch(Ctx *ctx, const ModifyDevice &d, int bins, const int *f_len, int n_utts, int f_stride,
+                           int max_f, double *spectrogram);
+
 int synthesis_fft(Ctx *ctx, int fft_size, int *lg_out);   // EINVAL unless a power of two in [16, 4096]
 // the decode tables of a coded call; EINVAL for number_of_dimensions, or no aperiodicity rows where fs has bands
 int synthesis_coded_tables(Ctx *ctx, int fs, int fft_size, int number_of_dimensions, bool have_aperiodicity,
@@ -175,7 +200,9 @@ int synthesis_lengths(Ctx *ctx, const int *f0_lengths, int n_utts, int f0_stride
 // Per-utterance scratch of synthesis_run for a batch whose longest y_length is max_y; fit(nominal_cap) utterances
 // make one pass when no utterance has more than 1,200 pulses per second.
 struct SynthesisSizing {
-  SynthesisSizing(const Ctx *ctx, const CodedRows *coded, int fft_size, int f0_stride, int y_stride, int max_y, int fs);
+  // mod: the scaled f0 copy (f0_stride * 8 bytes per utterance) and the stretch tables are counted too
+  SynthesisSizing(const Ctx *ctx, const CodedRows *coded, int fft_size, int f0_stride, int y_stride, int max_y, int fs,
+                  const ModifyPlan *mod = nullptr);
   size_t per_utt(int cap) const;
   int fit(int cap) const;
   int fft_size, y_stride, nominal_cap;
@@ -184,9 +211,12 @@ struct SynthesisSizing {
 };
 // Enqueues Synthesis of n_utts utterances (device rows; host lengths) on ctx->stream, in passes that fit the scratch
 // budget, each with one read-back of its pulse counts.  coded null: full rows; y: double (nbit 0) or int16 (nbit 16).
+// mod (coded rows only): utterance i of the call is the plan's utterance mod_u0 + i; each pass synthesises from a
+// scaled copy of its f0 rows and stretches its decoded envelope block right after the decode.
 int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts, int f0_stride,
                   const double *spectrogram, const double *aperiodicity, const CodedRows *coded, int fft_size, int lg,
-                  double frame_period, int fs, const int *y_lengths, int y_stride, void *y, int nbit);
+                  double frame_period, int fs, const int *y_lengths, int y_stride, void *y, int nbit,
+                  const ModifyPlan *mod = nullptr, int mod_u0 = 0);
 int cheaptrick_run(Ctx *ctx, const Batch &b, double q1, int fft_size, double *spectrogram,
                    const CodecTables *coded = nullptr, double *coded_out = nullptr);
 int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *aperiodicity,

@@ -11,13 +11,26 @@
 //                         inverse transforms, DC removal -> one response of fft_size samples
 //   syn_overlap_kernel    output sample -> thread: sums the responses covering it in pulse order
 //                         (the reference's accumulation order, so the sum is deterministic)
+// and, ahead of it, the voice modification of the reference demo (F0 scaling and formant shift, section below):
+//   modify_stretch_kernel, modify_f0_kernel
 // FFT conventions (SURVEY.md App. A0): c2c FORWARD of a == FFT(conj a); c2r of X == Re FFT(conj X~)
 // with X~ the Hermitian extension -- both are forward transforms of wb_fft.cuh.
 #include "wb_internal.h"
 #include "wb_spectral.cuh"
 #include "../../include/world_b200.h"
+#include "../../include/world/matlabfunctions.h"
+#include <map>
+#include <stdio.h>
 #include <type_traits>
 #include <vector>
+
+#ifdef WB_EMU
+// the CUDA intrinsics the stretch uses; the emulation is compiled with -ffp-contract=off, so plain operators round
+// each step on their own
+static inline double __dadd_rn(double a, double b) { return a + b; }
+static inline double __dsub_rn(double a, double b) { return a - b; }
+static inline double __dmul_rn(double a, double b) { return a * b; }
+#endif
 
 namespace wb {
 
@@ -303,6 +316,166 @@ WB_KERNEL_PLAIN syn_overlap_kernel(SynParams p) {
   else p.y[(size_t)u * p.y_stride + s] = acc;
 }
 
+// ---- voice modification --------------------------------------------------------------------------------------------
+// F0 scaling and formant shift over a batch: the reference demo's ParameterModification (test/test.cpp:221-258), the
+// step a vocoder sits between analysis and synthesis for.  world_b200_modify_batch runs it on full rows; synthesis_run
+// runs the same two kernels on each pass's f0 copy and decoded envelope block.
+//
+// Per utterance, with shift (f0 factor) and ratio (spectral stretch), half = fft_size / 2, bins = half + 1:
+//   f0[i] *= shift
+//   x[i] = ratio * i / fft_size * fs,  xi[j] = (double)j / fft_size * fs,  L[m] = log(sp[m])
+//   sp[j] = exp(interp1(x, L, xi)[j])        (histc, then y[k-1] + s * (y[k] - y[k-1]), extrapolating)
+//   ratio < 1: sp[j] = sp[c - 1] for j >= c = (int)(fft_size / 2.0 * ratio)
+// The segment k and the weight s of every bin depend on (ratio, fft_size, fs) only.  They are planned on the host
+// with the reference's expressions and the library's own histc (wb_matlab.cu), one table per distinct ratio, and the
+// tail rule is folded in (entry j := entry c - 1 gives the same value).  The kernel is then one gather per bin:
+//   modify_stretch_kernel  (frame, utterance) -> CTA: the row's logs into shared memory, barrier,
+//                          out[j] = exp(L[a] + s * (L[a + 1] - L[a])), rounded step by step as the reference's
+//                          unfused x86-64 build rounds it
+//   modify_f0_kernel       frame -> thread: f0 * shift
+
+#define WB_MODIFY_THREADS 128
+
+// Rows of frames >= f_len[u] (and utterances >= n_utts) are never touched.  The `continue` is uniform over the CTA.
+WB_KERNEL(WB_MODIFY_THREADS, 8) modify_stretch_kernel(double *sp, const int *__restrict__ f_len, int n_utts,
+                                                      int f_stride, int bins, const int *__restrict__ table,
+                                                      const int *__restrict__ idx, const double *__restrict__ frac) {
+  WB_DYN_SMEM(double, logs);   // bins
+  const int tid = WB_TID, nth = WB_NTH, f = blockIdx.x;
+  for (int u = blockIdx.y; u < n_utts; u += gridDim.y) {
+    if (f >= f_len[u]) continue;
+    double *row = sp + ((size_t)u * f_stride + f) * bins;
+    const size_t t0 = (size_t)__ldg(&table[u]) * bins;
+    for (int j = tid; j < bins; j += nth) logs[j] = log(row[j]);
+    WB_SYNC();
+    for (int j = tid; j < bins; j += nth) {
+      const int a = __ldg(&idx[t0 + j]);
+      const double s = __ldg(&frac[t0 + j]);
+      const double la = logs[a], lb = logs[a + 1];
+      // y[k-1] + s * (y[k] - y[k-1]) (matlabfunctions.cpp:171): three roundings, no FMA
+      row[j] = exp(__dadd_rn(la, __dmul_rn(s, __dsub_rn(lb, la))));
+    }
+    WB_SYNC();
+  }
+}
+
+WB_KERNEL_PLAIN modify_f0_kernel(const double *f0_in, double *f0_out, const double *__restrict__ scale,
+                                 const int *__restrict__ f_len, int n_utts, int f_stride) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  for (int u = blockIdx.y; u < n_utts; u += gridDim.y)
+    if (i < f_len[u]) f0_out[(size_t)u * f_stride + i] = __dmul_rn(f0_in[(size_t)u * f_stride + i], scale[u]);
+}
+
+namespace {
+struct ModifyLayout {
+  size_t o_idx, o_frac, o_scale, o_table, total;
+  ModifyLayout(const ModifyPlan &p, int n) {
+    ArenaPlan a;
+    const size_t cells = (size_t)p.n_tables * p.bins;
+    o_idx = a.add(cells * 4); o_frac = a.add(cells * 8);
+    o_scale = a.add(p.scale.empty() ? 0 : (size_t)n * 8); o_table = a.add(p.table.empty() ? 0 : (size_t)n * 4);
+    total = a.total;
+  }
+};
+
+int modify_fail(Ctx *ctx, const char *what, int u, double v, const char *why) {
+  char msg[256];
+  snprintf(msg, sizeof msg, "modify: %s[%d] = %.17g %s", what, u, v, why);
+  ctx->last_error = msg;
+  return WORLD_B200_EINVAL;
+}
+}  // namespace
+
+size_t ModifyPlan::device_bytes(int n) const { return ModifyLayout(*this, n).total; }
+
+int modify_plan(Ctx *ctx, int n_utts, int fft_size, int fs, const double *f0_scale, const double *spectral_ratio,
+                ModifyPlan *plan) {
+  *plan = ModifyPlan();
+  if (f0_scale) {
+    for (int u = 0; u < n_utts; ++u) {
+      const double v = f0_scale[u];
+      if (!(v > 0.0) || !isfinite(v)) return modify_fail(ctx, "f0_scale", u, v, "is not a finite factor > 0");
+    }
+    plan->scale.assign(f0_scale, f0_scale + n_utts);
+  }
+  if (!spectral_ratio) return 0;
+  if (fft_size < 16 || fft_size > 4096 || (fft_size & (fft_size - 1))) {
+    ctx->last_error = "modify: fft_size must be a power of two in [16, 4096]";
+    return WORLD_B200_EINVAL;
+  }
+  if (fs <= 0) {
+    ctx->last_error = "modify: fs must be > 0";
+    return WORLD_B200_EINVAL;
+  }
+  for (int u = 0; u < n_utts; ++u) {
+    const double r = spectral_ratio[u];
+    // histc needs an ascending axis; below 1 the tail copies bin c - 1, which must exist (c == 0 reads sp[-1])
+    if (!(r > 0.0) || !isfinite(r)) return modify_fail(ctx, "spectral_ratio", u, r, "is not a finite ratio > 0");
+    if (r < 1.0 && static_cast<int>(fft_size / 2.0 * r) < 1)
+      return modify_fail(ctx, "spectral_ratio", u, r, "leaves no bin below (int)(fft_size / 2.0 * ratio)");
+  }
+  const int half = fft_size / 2, bins = half + 1;
+  plan->bins = bins;
+  plan->table.resize(n_utts);
+  std::map<double, int> seen;
+  std::vector<double> x(bins), xi(bins);
+  std::vector<int> k(bins);
+  for (int u = 0; u < n_utts; ++u) {
+    const double ratio = spectral_ratio[u];
+    auto it = seen.find(ratio);
+    if (it != seen.end()) { plan->table[u] = it->second; continue; }
+    const int t = plan->n_tables++;
+    seen[ratio] = t;
+    plan->table[u] = t;
+    for (int i = 0; i <= half; ++i) {   // test.cpp:237-240, the same expressions in the same order
+      x[i] = ratio * i / fft_size * fs;
+      xi[i] = static_cast<double>(i) / fft_size * fs;
+    }
+    histc(x.data(), bins, xi.data(), bins, k.data());
+    plan->idx.resize((size_t)plan->n_tables * bins);
+    plan->frac.resize((size_t)plan->n_tables * bins);
+    int *ia = plan->idx.data() + (size_t)t * bins;
+    double *sa = plan->frac.data() + (size_t)t * bins;
+    for (int j = 0; j < bins; ++j) {   // matlabfunctions.cpp:162-171: h[k-1] = x[k] - x[k-1], s = (xi - x[k-1]) / h
+      const int a = k[j] - 1;
+      ia[j] = a;
+      sa[j] = (xi[j] - x[a]) / (x[a + 1] - x[a]);
+    }
+    if (ratio < 1.0) {                 // test.cpp:250-254
+      const int c = static_cast<int>(fft_size / 2.0 * ratio);
+      for (int j = c; j < bins; ++j) { ia[j] = ia[c - 1]; sa[j] = sa[c - 1]; }
+    }
+  }
+  return 0;
+}
+
+int modify_upload(Ctx *ctx, const ModifyPlan &plan, int u0, int n, unsigned char *blk, ModifyDevice *d) {
+  const ModifyLayout l(plan, n);
+  int rc = 0;
+  if (!plan.idx.empty()) rc = dev_memcpy_h2d(ctx, blk + l.o_idx, plan.idx.data(), plan.idx.size() * 4);
+  if (!rc && !plan.frac.empty()) rc = dev_memcpy_h2d(ctx, blk + l.o_frac, plan.frac.data(), plan.frac.size() * 8);
+  if (!rc && !plan.scale.empty()) rc = dev_memcpy_h2d(ctx, blk + l.o_scale, plan.scale.data() + u0, (size_t)n * 8);
+  if (!rc && !plan.table.empty()) rc = dev_memcpy_h2d(ctx, blk + l.o_table, plan.table.data() + u0, (size_t)n * 4);
+  d->idx = (const int *)(blk + l.o_idx); d->frac = (const double *)(blk + l.o_frac);
+  d->scale = (const double *)(blk + l.o_scale); d->table = (const int *)(blk + l.o_table);
+  return rc;
+}
+
+void modify_f0_launch(Ctx *ctx, const ModifyDevice &d, const int *f_len, int n_utts, int f_stride, int max_f,
+                      const double *f0_in, double *f0_out) {
+  if (n_utts <= 0 || max_f <= 0) return;
+  const dim3 grid((unsigned)((max_f + 255) / 256), (unsigned)imin(n_utts, 65535));
+  WB_LAUNCH_FLAT(modify_f0_kernel, grid, 256, 0, ctx->stream, f0_in, f0_out, d.scale, f_len, n_utts, f_stride);
+}
+
+void modify_stretch_launch(Ctx *ctx, const ModifyDevice &d, int bins, const int *f_len, int n_utts, int f_stride,
+                           int max_f, double *spectrogram) {
+  if (n_utts <= 0 || max_f <= 0) return;
+  const dim3 grid((unsigned)max_f, (unsigned)imin(n_utts, 65535));
+  WB_LAUNCH_COOP(modify_stretch_kernel, grid, WB_MODIFY_THREADS, (size_t)bins * 8, ctx->stream, spectrogram, f_len,
+                 n_utts, f_stride, bins, d.table, d.idx, d.frac);
+}
+
 int synthesis_fft(Ctx *ctx, int fft_size, int *lg_out) {
   int lg = 0;
   while ((1 << lg) < fft_size) ++lg;
@@ -340,7 +513,7 @@ int synthesis_lengths(Ctx *ctx, const int *f0_lengths, int n_utts, int f0_stride
 }
 
 SynthesisSizing::SynthesisSizing(const Ctx *ctx, const CodedRows *coded, int fft_size, int f0_stride, int y_stride,
-                                 int max_y, int fs)
+                                 int max_y, int fs, const ModifyPlan *mod)
     : fft_size(fft_size), y_stride(y_stride) {
   const size_t bins = (size_t)fft_size / 2 + 1;
   // The coded call holds one chunk's decoded envelope and aperiodicity (16 B per bin and frame) and the decode tables.
@@ -352,6 +525,12 @@ SynthesisSizing::SynthesisSizing(const Ctx *ctx, const CodedRows *coded, int fft
     tables = tp.total;
   }
   decoded_per_utt = coded ? (size_t)f0_stride * bins * 16 : 0;
+  // A modified call also holds the stretch tables, and per utterance its factor, table index and scaled f0 row (the
+  // 256-byte alignment of the two small arrays is in the 4096 below).
+  if (mod) {
+    tables += mod->device_bytes(0);
+    decoded_per_utt += (size_t)f0_stride * 8 + 12;
+  }
   budget = (double)ctx->scratch_budget - (double)tables;
   // Pulse arrays and responses are sized for 1200 pulses per second (f0 <= 1.2 kHz; the +64 covers the ends).
   nominal_cap = (int)((double)max_y / fs * 1200.0) + 64;
@@ -369,7 +548,8 @@ int SynthesisSizing::fit(int cap) const { return (int)dmin(65535.0, budget / (do
 // chunk into the chunk's block.  nbit 0 writes the waveform (double), nbit 16 its 16-bit PCM (short).
 int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts, int f0_stride,
                   const double *spectrogram, const double *aperiodicity, const CodedRows *coded, int fft_size, int lg,
-                  double frame_period, int fs, const int *y_lengths, int y_stride, void *y, int nbit) {
+                  double frame_period, int fs, const int *y_lengths, int y_stride, void *y, int nbit,
+                  const ModifyPlan *mod, int mod_u0) {
   if (n_utts == 0) return 0;
   std::vector<int> lens((size_t)2 * n_utts);
   int rc = synthesis_lengths(ctx, f0_lengths, n_utts, f0_stride, y_lengths, y_stride, lens.data());
@@ -392,7 +572,8 @@ int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts,
   // The caller's f0 may be anything up to fs/2 (a pitch-shifted contour), so syn_timebase_kernel also counts the
   // pulses it could not store; a chunk where that count exceeds the cap is laid out again with room for its largest
   // count, in as many passes as the scratch budget needs.  The common case pays one read-back of n counts per chunk.
-  const SynthesisSizing sz(ctx, coded, fft_size, f0_stride, y_stride, max_y, fs);
+  const SynthesisSizing sz(ctx, coded, fft_size, f0_stride, y_stride, max_y, fs, mod);
+  const bool scale_f0 = mod && !mod->scale.empty(), stretch = mod && !mod->table.empty();
   const int nominal_cap = sz.nominal_cap;
   const size_t draw_stride = sz.draw_stride;
   auto fit = [&](int cap) { return sz.fit(cap); };
@@ -422,10 +603,13 @@ int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts,
       o_sw = plan.add(coded->tsp.weight.size() * 16);
       o_aidx = plan.add(coded->tap.idx.size() * 4); o_afrac = plan.add(coded->tap.frac.size() * 8);
     }
+    const size_t o_mod = mod ? plan.add(mod->device_bytes(n)) : 0;
+    const size_t o_f0m = scale_f0 ? plan.add((size_t)n * f0_stride * 8) : 0;
     unsigned char *blk = arena_block(ctx, plan.total);
     if (!blk) return WORLD_B200_ENOMEM;
     std::vector<int> l2((size_t)2 * n), pl(n, pulse_cap);
-    for (int i = 0; i < n; ++i) { l2[i] = lens[u0 + i]; l2[n + i] = lens[n_utts + u0 + i]; }
+    int max_f = 0;
+    for (int i = 0; i < n; ++i) { l2[i] = lens[u0 + i]; l2[n + i] = lens[n_utts + u0 + i]; max_f = imax(max_f, l2[i]); }
     rc = dev_memcpy_h2d(ctx, blk + o_len, l2.data(), l2.size() * 4);
     if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_dcr, dcr.data(), dcr.size() * 8);
     if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_pl, pl.data(), (size_t)n * 4);
@@ -437,6 +621,8 @@ int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts,
       if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_aidx, a.idx.data(), a.idx.size() * 4);
       if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_afrac, a.frac.data(), a.frac.size() * 8);
     }
+    ModifyDevice md = {};
+    if (mod && !rc) rc = modify_upload(ctx, *mod, mod_u0 + u0, n, blk + o_mod, &md);
     if (rc) return rc;
     SynParams p;
     p.f0 = f0 + (size_t)u0 * f0_stride; p.f_len = (const int *)(blk + o_len); p.f_stride = f0_stride;
@@ -458,6 +644,12 @@ int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts,
     p.tw = ctx->twiddle;
     // a pass laid out from the counts reports a pulse beyond its arrays as a scratch overflow (status bit 4)
     p.status = relaid ? ctx->status_dev : nullptr;
+    if (scale_f0) {
+      // the time base, the pulse count (and the relaid pass it may call for) and the pulses all see the scaled contour
+      double *f0m = (double *)(blk + o_f0m);
+      modify_f0_launch(ctx, md, p.f_len, n, f0_stride, max_f, p.f0, f0m);
+      p.f0 = f0m;
+    }
     WB_LAUNCH_COOP(syn_timebase_kernel, dim3((unsigned)n), 256, 0, ctx->stream, p);
     if (!relaid) {
       counts.resize(n);
@@ -476,14 +668,13 @@ int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts,
     }
     if (coded) {
       // DecodeSpectralEnvelope / DecodeAperiodicity of this pass's utterances, frames [0, f0_length)
-      int max_f = 0;
-      for (int i = 0; i < n; ++i) max_f = imax(max_f, l2[i]);
       const CodecDeviceTables ts = {(const int *)(blk + o_sidx), (const double *)(blk + o_sfrac),
                                     (const double2 *)(blk + o_sw)};
       const CodecDeviceTables ta = {(const int *)(blk + o_aidx), (const double *)(blk + o_afrac), nullptr};
       double *dsp = (double *)(blk + o_dsp), *dap = (double *)(blk + o_dap);
       codec_decode_launch(ctx, true, coded->tsp, ts, fft_size, p.f_len, n, f0_stride, max_f,
                           coded->sp + (size_t)u0 * f0_stride * coded->tsp.dims, dsp);
+      if (stretch) modify_stretch_launch(ctx, md, (int)bins, p.f_len, n, f0_stride, max_f, dsp);
       // below 12 kHz there are no bands: the kernel reads no coded value (its input pointer only has to be valid)
       codec_decode_launch(ctx, false, coded->tap, ta, fft_size, p.f_len, n, f0_stride, max_f,
                           coded->ap ? coded->ap + (size_t)u0 * f0_stride * coded->tap.dims : dap, dap);
@@ -524,11 +715,13 @@ extern "C" int world_b200_synthesis_batch(WorldB200 *h, const double *f0, const 
                        frame_period, fs, y_lengths, y_stride, y, 0);
 }
 
-// world_b200_synthesis_coded_batch (nbit 0, y double) and world_b200_synthesis_coded_batch_pcm16 (nbit 16, y short)
+// world_b200_synthesis_coded_batch (nbit 0, y double), world_b200_synthesis_coded_batch_pcm16 (nbit 16, y short) and,
+// with f0_scale / spectral_ratio, world_b200_synthesis_coded_batch_modified
 static int synthesis_coded_batch(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts, int f0_stride,
                                  const double *coded_spectral_envelope, int number_of_dimensions,
                                  const double *coded_aperiodicity, int fft_size, double frame_period, int fs,
-                                 const int *y_lengths, int y_stride, void *y, int nbit) {
+                                 const int *y_lengths, int y_stride, void *y, int nbit,
+                                 const double *f0_scale = nullptr, const double *spectral_ratio = nullptr) {
   if (!h || !f0 || !coded_spectral_envelope || !y || n_utts < 0 || fs <= 0 || frame_period <= 0)
     return WORLD_B200_EINVAL;
   DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
@@ -539,10 +732,30 @@ static int synthesis_coded_batch(WorldB200 *h, const double *f0, const int *f0_l
   CodedRows coded;
   rc = synthesis_coded_tables(ctx, fs, fft_size, number_of_dimensions, coded_aperiodicity != nullptr, &coded);
   if (rc) return rc;
+  ModifyPlan mod;
+  const bool modified = f0_scale || spectral_ratio;
+  if (modified) rc = modify_plan(ctx, n_utts, fft_size, fs, f0_scale, spectral_ratio, &mod);
+  if (rc) return rc;
   coded.sp = coded_spectral_envelope;
   coded.ap = coded.tap.dims > 0 ? coded_aperiodicity : nullptr;
   return synthesis_run(ctx, f0, f0_lengths, n_utts, f0_stride, nullptr, nullptr, &coded, fft_size, lg, frame_period,
-                       fs, y_lengths, y_stride, y, nbit);
+                       fs, y_lengths, y_stride, y, nbit, modified ? &mod : nullptr);
+}
+
+extern "C" int world_b200_synthesis_coded_batch_modified(WorldB200 *h, const double *f0, const int *f0_lengths,
+                                                         int n_utts, int f0_stride,
+                                                         const double *coded_spectral_envelope,
+                                                         int number_of_dimensions, const double *coded_aperiodicity,
+                                                         int fft_size, double frame_period, int fs,
+                                                         const int *y_lengths, int y_stride, const double *f0_scale,
+                                                         const double *spectral_ratio, int nbit, void *y) {
+  if (h && nbit != 0 && nbit != 16) {
+    reinterpret_cast<Ctx *>(h)->last_error = "synthesis_coded_batch_modified: nbit must be 0 (double) or 16 (int16)";
+    return WORLD_B200_EINVAL;
+  }
+  return synthesis_coded_batch(h, f0, f0_lengths, n_utts, f0_stride, coded_spectral_envelope, number_of_dimensions,
+                               coded_aperiodicity, fft_size, frame_period, fs, y_lengths, y_stride, y, nbit, f0_scale,
+                               spectral_ratio);
 }
 
 extern "C" int world_b200_synthesis_coded_batch(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts,
@@ -561,4 +774,44 @@ extern "C" int world_b200_synthesis_coded_batch_pcm16(WorldB200 *h, const double
                                                       int y_stride, short *y) {
   return synthesis_coded_batch(h, f0, f0_lengths, n_utts, f0_stride, coded_spectral_envelope, number_of_dimensions,
                                coded_aperiodicity, fft_size, frame_period, fs, y_lengths, y_stride, y, 16);
+}
+
+extern "C" int world_b200_modify_batch(WorldB200 *h, double *f0, const int *f0_lengths, int n_utts, int f0_stride,
+                                       double *spectrogram, int fft_size, int fs, const double *f0_scale,
+                                       const double *spectral_ratio) {
+  if (!h || n_utts < 0 || f0_stride <= 0) return WORLD_B200_EINVAL;
+  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
+  Ctx *ctx = reinterpret_cast<Ctx *>(h);
+  if ((f0_scale && !f0) || (spectral_ratio && !spectrogram)) {
+    ctx->last_error = "modify: f0_scale needs f0 rows and spectral_ratio needs spectrogram rows";
+    return WORLD_B200_EINVAL;
+  }
+  std::vector<int> lens(n_utts > 0 ? n_utts : 1);
+  int max_f = 0;
+  for (int u = 0; u < n_utts; ++u) {
+    lens[u] = f0_lengths ? f0_lengths[u] : f0_stride;
+    if (lens[u] < 0 || lens[u] > f0_stride) {
+      char msg[128];
+      snprintf(msg, sizeof msg, "modify: f0_lengths[%d] = %d is outside its padded row of %d frames", u, lens[u],
+               f0_stride);
+      ctx->last_error = msg;
+      return WORLD_B200_EINVAL;
+    }
+    max_f = imax(max_f, lens[u]);
+  }
+  ModifyPlan plan;
+  int rc = modify_plan(ctx, n_utts, fft_size, fs, f0_scale, spectral_ratio, &plan);
+  if (rc || max_f == 0 || (!f0_scale && !spectral_ratio)) return rc;
+  ArenaPlan a;
+  const size_t o_len = a.add((size_t)n_utts * 4), o_mod = a.add(plan.device_bytes(n_utts));
+  unsigned char *blk = arena_block(ctx, a.total);
+  if (!blk) return WORLD_B200_ENOMEM;
+  ModifyDevice d;
+  rc = dev_memcpy_h2d(ctx, blk + o_len, lens.data(), (size_t)n_utts * 4);
+  if (!rc) rc = modify_upload(ctx, plan, 0, n_utts, blk + o_mod, &d);
+  if (rc) return rc;
+  const int *f_len = (const int *)(blk + o_len);
+  if (f0_scale) modify_f0_launch(ctx, d, f_len, n_utts, f0_stride, max_f, f0, f0);
+  if (spectral_ratio) modify_stretch_launch(ctx, d, fft_size / 2 + 1, f_len, n_utts, f0_stride, max_f, spectrogram);
+  return dev_check(ctx, "modify");
 }
