@@ -474,6 +474,50 @@ int world_b200_analyze_coded_batch_allgather_dio_options(WorldB200 *ctx, const v
                                                          double *coded_spectral_envelope_full,
                                                          double *coded_aperiodicity_full);
 
+/* ---- voice transformation, PCM in and PCM out: the reference demo's loop (test/test.cpp: Harvest or DIO + StoneMask,
+ * CheapTrick, D4C, ParameterModification, Synthesis) over a batch in one call, with one pitch, formant and tempo
+ * factor per utterance ----------------------------------------------------------------------------------------------
+ * y_length of world_b200_transform_*: the demo's formula (test.cpp:418-419) with the synthesis frame period
+ *   fp = frame_period * time_scale (one product, rounded once):
+ *   (int)((world_b200_frames(fs, x_length, frame_period) - 1) * fp / 1000.0 * fs) + 1
+ * 0 when fp is not finite and > 0, or the length does not fit an int. */
+int world_b200_transform_samples(int fs, int x_length, double frame_period, double time_scale);
+/* x: n_utts rows of x_stride samples of `nbit` bits (DEVICE), as for world_b200_analyze_coded_batch (0 = doubles;
+ * 8/16/24/32 = little-endian PCM); x_lengths HOST or NULL.  option selects the F0 method and carries its options and
+ * those of CheapTrick and D4C; harvest_options / dio_options are NULL or one option per utterance of that F0 method
+ * (HOST arrays of n_utts), with the rules of world_b200_analyze_batch_options / _dio_options.
+ *   - f0_scale, spectral_ratio, time_scale: HOST arrays of n_utts, or NULL.  f0_scale and spectral_ratio change f0 and
+ *     the spectral envelope as world_b200_modify_batch does (NULL skips that half).  Utterance u is synthesised with
+ *     the frame period frame_period * time_scale[u] ms (NULL: 1.0): above 1 the speech is slower, below 1 faster;
+ *     f0 and the envelopes are the same, only the frames are further apart.
+ *   - y: [n_utts][y_stride] (DEVICE) of float64 for nbit_out 0, or int16 for nbit_out 16 (the pcm16 rule of
+ *     world_b200_synthesis_coded_batch_pcm16); samples past an utterance's y_length are not written.  y_lengths (HOST,
+ *     may be NULL) receives world_b200_transform_samples of each utterance.
+ *   - Output: every row equals, bit for bit, world_b200_analyze_batch (full rows, the same options) ->
+ *     world_b200_modify_batch (absent when f0_scale and spectral_ratio are both NULL) -> world_b200_synthesis_batch with
+ *     frame_period * time_scale[u] and that y_length, for nbit_out 16 followed by the pcm16 rule.
+ *   - The batch runs in utterance slices on the two internal streams of world_b200_analyze_batch; a slice's full rows
+ *     live only from its analysis to its synthesis, so device memory does not grow with the batch.  The synthesis of
+ *     one slice (whose time base is latency bound) runs beside the analysis of the next.  Synthesis reads its pulse
+ *     counts back once per pass, so the host waits inside the call; the caller's stream is ordered after the work.
+ *   - Validation, before any work is queued (WORLD_B200_EINVAL, world_b200_last_error() naming the first bad
+ *     utterance; y is unchanged): what world_b200_analyze_coded_batch, world_b200_modify_batch and
+ *     world_b200_synthesis_batch check, a time_scale that is not finite or not > 0, option->cheaptrick.fft_size outside
+ *     Synthesis's powers of two in [16, 4096], an utterance of fewer than 2 frames or a y_length above y_stride, and an
+ *     nbit_out other than 0 or 16.  n_utts 0 returns 0. */
+int world_b200_transform_batch(WorldB200 *ctx, const void *x, int nbit, int n_utts, int x_stride, const int *x_lengths,
+                               int fs, const WorldB200AnalysisOption *option, const HarvestOption *harvest_options,
+                               const DioOption *dio_options, const double *f0_scale, const double *spectral_ratio,
+                               const double *time_scale, int nbit_out, void *y, int y_stride, int *y_lengths);
+/* The same for HOST x, y and y_lengths: utterance chunks of PCM are uploaded on one stream, transformed as above, and
+ * their output rows downloaded on another, so only PCM crosses PCIe.  Whole rows of y are written: samples past an
+ * utterance's y_length read 0.  Bit for bit equal to world_b200_transform_batch; pinned host buffers let the copies
+ * run under the kernels.  Returns when the results are in y. */
+int world_b200_transform_host(WorldB200 *ctx, const void *x, int nbit, int n_utts, int x_stride, const int *x_lengths,
+                              int fs, const WorldB200AnalysisOption *option, const HarvestOption *harvest_options,
+                              const DioOption *dio_options, const double *f0_scale, const double *spectral_ratio,
+                              const double *time_scale, int nbit_out, void *y, int y_stride, int *y_lengths);
+
 #ifdef __cplusplus
 }
 #endif

@@ -169,6 +169,13 @@ ABI = {
                                                                        C.c_int, C.POINTER(AnalysisOption),
                                                                        C.POINTER(DioOption), C.c_int, _P, _P, C.c_int,
                                                                        _P, _P]),
+    "world_b200_transform_samples": (C.c_int, [C.c_int, C.c_int, C.c_double, C.c_double]),
+    "world_b200_transform_batch": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(AnalysisOption),
+                                             C.POINTER(HarvestOption), C.POINTER(DioOption), _P, _P, _P, C.c_int, _P,
+                                             C.c_int, _IP]),
+    "world_b200_transform_host": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(AnalysisOption),
+                                            C.POINTER(HarvestOption), C.POINTER(DioOption), _P, _P, _P, C.c_int, _P,
+                                            C.c_int, _IP]),
     # host-only file glue (tools/audioio.h, tools/parameterio.h)
     "wavwrite": (None, [_P, C.c_int, C.c_int, C.c_int, C.c_char_p]),
     "GetAudioLength": (C.c_int, [C.c_char_p]),
@@ -900,6 +907,71 @@ class World:
             self._check(self.lib.world_b200_analyze_coded_batch(self._h, _ptr(x), nbit, n, stride, xl, fs,
                                                                 C.byref(option), *outs))
         return time_axis, f0, coded_sp, coded_ap, fl
+
+    # -- voice transformation: analysis, modification and synthesis in one call --------------------------------
+    def transform_samples(self, fs, x_length, frame_period=5.0, time_scale=1.0) -> int:
+        """Output length of one utterance of transform(): the demo's y_length with frame period frame_period * time_scale
+        (world_b200_transform_samples)."""
+        return int(self.lib.world_b200_transform_samples(fs, x_length, frame_period, time_scale))
+
+    def _transform_args(self, x, nbit, fs, option, f0_scale, spectral_ratio, time_scale, x_lengths, harvest_options,
+                        dio_options, dtype):
+        n, stride, frame_period = self._coded_rows(x, nbit, option)
+        lens = [stride] * n if x_lengths is None else [int(v) for v in x_lengths]
+        ts = _factors(time_scale, n, "time_scale")
+        y_lens = [self.transform_samples(fs, v, frame_period, ts[u] if ts is not None else 1.0)
+                  for u, v in enumerate(lens)]
+        xl, _ = _int_array(x_lengths, n)
+        per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
+        nbit_out = 16 if _pcm16(dtype) else 0
+        y_stride = max(y_lens + [1])
+        args = [nbit, n, stride, xl, fs, C.byref(option), per_utt, per_dio, _factors(f0_scale, n, "f0_scale"),
+                _factors(spectral_ratio, n, "spectral_ratio"), ts, nbit_out]
+        return n, y_stride, nbit_out, args
+
+    def transform(self, x, nbit, fs, option: AnalysisOption, f0_scale=None, spectral_ratio=None, time_scale=None,
+                  x_lengths=None, harvest_options=None, dio_options=None, dtype=None):
+        """The reference demo's loop on DEVICE arrays in one call (world_b200_transform_batch): analysis with option's F0
+        method, CheapTrick and D4C, f0 scaled by f0_scale and the envelope stretched by spectral_ratio (as modify()),
+        and Synthesis with the frame period scaled by time_scale (above 1: slower).  Each factor may be None, one number,
+        or one value per utterance.  x as for analyze_coded_batch (float64 rows for nbit 0, else PCM rows).  Returns
+        (y, y_lengths): y [n, max y_length] float64, or int16 for dtype int16 (wavwrite's quantisation), on x's device,
+        with samples past an utterance's length left 0; y_lengths from transform_samples.  Every row equals
+        analyze_batch -> modify -> synthesis of the same utterance bit for bit."""
+        n, y_stride, nbit_out, args = self._transform_args(x, nbit, fs, option, f0_scale, spectral_ratio, time_scale,
+                                                           x_lengths, harvest_options, dio_options, dtype)
+        if self.xp == "torch":
+            y = self.torch.zeros((n, y_stride), dtype=self.torch.int16 if nbit_out else self.torch.float64,
+                                 device=x.device)
+        else:
+            import numpy as np
+            y = np.zeros((n, y_stride), dtype=np.int16 if nbit_out else np.float64)
+        yl = (C.c_int * max(n, 1))()
+        self._use_current_stream()
+        self._check(self.lib.world_b200_transform_batch(self._h, _ptr(x), *args, _ptr(y), y_stride, yl))
+        return y, list(yl)[:n]
+
+    def transform_host(self, x, nbit, fs, option: AnalysisOption, f0_scale=None, spectral_ratio=None, time_scale=None,
+                       x_lengths=None, harvest_options=None, dio_options=None, dtype=None, out=None):
+        """transform() for HOST arrays (numpy or CPU tensors; world_b200_transform_host): PCM chunks are uploaded,
+        transformed and downloaded pipelined, so only PCM crosses PCIe.  Returns (y, y_lengths) with y a host array of
+        whole rows (0 past each length).  out: a contiguous [n, max y_length] host array of the output dtype to write
+        into (a pinned one lets the copies overlap the kernels)."""
+        import numpy as np
+        n, y_stride, nbit_out, args = self._transform_args(x, nbit, fs, option, f0_scale, spectral_ratio, time_scale,
+                                                           x_lengths, harvest_options, dio_options, dtype)
+        want = np.int16 if nbit_out else np.float64
+        if out is None:
+            out = np.zeros((n, y_stride), dtype=want)
+        y = out.numpy() if hasattr(out, "numpy") else out
+        if y.shape != (n, y_stride) or y.dtype != want or not y.flags.c_contiguous:
+            raise ValueError(f"out: a contiguous [{n}, {y_stride}] {np.dtype(want).name} host array")
+        xh = x.numpy() if hasattr(x, "numpy") else x
+        if not xh.flags.c_contiguous:
+            raise ValueError("x: a contiguous host array")
+        yl = (C.c_int * max(n, 1))()
+        self._check(self.lib.world_b200_transform_host(self._h, _ptr(xh), *args, _ptr(y), y_stride, yl))
+        return out, list(yl)[:n]
 
     def analyze_coded_batch_allgather(self, x, nbit, fs, option: AnalysisOption, number_of_dimensions, time_axis_full,
                                       f0_full, coded_sp_full, coded_ap_full, x_lengths=None, harvest_options=None,

@@ -8,6 +8,8 @@
 #include <stdlib.h>
 #include <vector>
 #include <string>
+#include <algorithm>
+#include <cmath>
 
 struct WorldB200 {
   wb::Ctx c;
@@ -669,6 +671,59 @@ int world_b200_harvest_batch_options(WorldB200 *h, const double *x, int n, int x
   return harvest_batch_impl(h, x, n, x_stride, x_lengths, fs, harvest_options, true, time_axis, f0, f0_stride);
 }
 
+// The two lanes of a chain cut into slices (sibling contexts on their own non-blocking streams, created on first use),
+// ordered after the work already on the context's stream.  lanes[l] receives lane l with half the scratch budget, or
+// the context itself for both when the chain is one slice (and always on the host emulation, which has one stream).
+static int open_lanes(WorldB200 *h, int n_slices, WorldB200 *lanes[2]) {
+  lanes[0] = lanes[1] = h;
+#ifndef WB_EMU
+  if (n_slices > 1) {
+    for (int l = 0; l < 2; ++l) {
+      if (!h->lane[l]) {
+        int rc = world_b200_create(h->c.device, &h->lane[l]);
+        if (rc) { h->c.last_error = "analyze_batch: cannot create a lane context"; return rc; }
+        cudaStream_t st;
+        cudaEvent_t ev;
+        // equal (lowest) priority for both lanes: giving one lane the highest priority was measured slower;
+        // only the communication stream outranks them (wb_multi.cu)
+        if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess ||
+            cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) {
+          h->c.last_error = "analyze_batch: cannot create a lane stream";
+          return WORLD_B200_ECUDA;
+        }
+        h->lane_stream[l] = st; h->ev_join[l] = ev;
+        h->lane[l]->c.stream = st;
+      }
+      h->lane[l]->c.scratch_budget = h->c.scratch_budget / 2;
+      lanes[l] = h->lane[l];
+    }
+    if (!h->ev_fork) {
+      cudaEvent_t ev;
+      if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) return WORLD_B200_ECUDA;
+      h->ev_fork = ev;
+    }
+    cudaEventRecord((cudaEvent_t)h->ev_fork, h->c.stream);
+    for (int l = 0; l < 2; ++l) cudaStreamWaitEvent((cudaStream_t)h->lane_stream[l], (cudaEvent_t)h->ev_fork, 0);
+  }
+#else
+  (void)n_slices;
+#endif
+  return 0;
+}
+
+// The context's stream waits for both lanes of open_lanes.
+static void join_lanes(WorldB200 *h, WorldB200 *const lanes[2]) {
+#ifndef WB_EMU
+  if (lanes[0] != h)
+    for (int l = 0; l < 2; ++l) {
+      cudaEventRecord((cudaEvent_t)h->ev_join[l], (cudaStream_t)h->lane_stream[l]);
+      cudaStreamWaitEvent(h->c.stream, (cudaEvent_t)h->ev_join[l], 0);
+    }
+#else
+  (void)h; (void)lanes;
+#endif
+}
+
 // The whole chain on device arrays, cut into utterance slices that alternate between two lanes (sibling contexts
 // on their own non-blocking streams).  Per slice the stages run in order on the lane's stream; the two lanes run
 // concurrently, so the latency-bound per-utterance kernels of one slice (contour tracking, candidate clean-up, the
@@ -744,38 +799,9 @@ static int analyze_batch_impl(WorldB200 *h, const void *x, int nbit, int n, int 
     for (int s = 0; s < n_slices; ++s) total += wgt[s];
     for (int s = 0; s < n_slices; ++s) { run += wgt[s]; bounds[s + 1] = (int)((long long)n * run / total); }
   }
-  WorldB200 *lanes[2] = {h, h};
-#ifndef WB_EMU
-  if (n_slices > 1) {
-    for (int l = 0; l < 2; ++l) {
-      if (!h->lane[l]) {
-        int rc = world_b200_create(h->c.device, &h->lane[l]);
-        if (rc) { h->c.last_error = "analyze_batch: cannot create a lane context"; return rc; }
-        cudaStream_t st;
-        cudaEvent_t ev;
-        // equal (lowest) priority for both lanes: giving one lane the highest priority was measured slower;
-        // only the communication stream outranks them (wb_multi.cu)
-        if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess ||
-            cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) {
-          h->c.last_error = "analyze_batch: cannot create a lane stream";
-          return WORLD_B200_ECUDA;
-        }
-        h->lane_stream[l] = st; h->ev_join[l] = ev;
-        h->lane[l]->c.stream = st;
-      }
-      h->lane[l]->c.scratch_budget = h->c.scratch_budget / 2;
-      lanes[l] = h->lane[l];
-    }
-    if (!h->ev_fork) {
-      cudaEvent_t ev;
-      if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) return WORLD_B200_ECUDA;
-      h->ev_fork = ev;
-    }
-    cudaEventRecord((cudaEvent_t)h->ev_fork, h->c.stream);
-    for (int l = 0; l < 2; ++l) cudaStreamWaitEvent((cudaStream_t)h->lane_stream[l], (cudaEvent_t)h->ev_fork, 0);
-  }
-#endif
-  int rc = 0;
+  WorldB200 *lanes[2];
+  int rc = open_lanes(h, n_slices, lanes);
+  if (rc) return rc;
   // nbit != 0: each lane converts its slice into a float64 buffer, which the slice's three stages then read.  A lane
   // runs its slices in stream order, so one buffer per lane, sized for its largest slice, serves all of them.  It comes
   // from the lane's pool, not its arena (the stage drivers reset the arena when they return), and its bytes come out
@@ -869,12 +895,8 @@ static int analyze_batch_impl(WorldB200 *h, const void *x, int nbit, int n, int 
     const int g = push ? comm_p2p_finish(h->comm, h->c.stream, &err) : comm_join(h->comm, h->c.stream, &err);
     if (g && !rc) { h->c.last_error = err; rc = WORLD_B200_ECUDA; }
   }
-  if (lanes[0] != h)
-    for (int l = 0; l < 2; ++l) {   // join even after an error: the caller's stream must not run ahead of the lanes
-      cudaEventRecord((cudaEvent_t)h->ev_join[l], (cudaStream_t)h->lane_stream[l]);
-      cudaStreamWaitEvent(h->c.stream, (cudaEvent_t)h->ev_join[l], 0);
-    }
 #endif
+  join_lanes(h, lanes);   // even after an error: the caller's stream must not run ahead of the lanes
   // back to the pool while the lanes may still read them: a pooled buffer is only handed out again to work that is
   // ordered after this call's (the lane's next slices, or the host pipelines, whose uploads wait for the stream)
   pool_release(&lanes[0]->c, xbuf[0]);
@@ -906,6 +928,200 @@ int world_b200_analyze_batch_dio_options(WorldB200 *h, const double *x, int n, i
   if (!dio_options) return WORLD_B200_EINVAL;
   return analyze_batch_impl(h, x, 0, n, x_stride, x_lengths, fs, opt, nullptr, dio_options, 0, time_axis, f0, f0_stride,
                             spectrogram, aperiodicity, false);
+}
+
+}  // extern "C"
+
+// ---- voice transformation: analysis, modification and synthesis in one call (world_b200_transform_*)
+namespace wb {
+
+// Every check of the call before any work is queued (EINVAL, last_error naming the first bad utterance), and the
+// per-utterance frame counts, output lengths and synthesis frame periods.
+int transform_check(WorldB200 *h, const void *x, int nbit, int n, int x_stride, const int *x_lengths, int fs,
+                    const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
+                    const DioOption *dio_options, const double *f0_scale, const double *spectral_ratio,
+                    const double *time_scale, int nbit_out, const void *y, int y_stride, const char *who,
+                    TransformPlan *tp) {
+  Ctx *c = &h->c;
+  char msg[256];
+  auto fail = [&](const char *what) {
+    c->last_error = std::string(who) + ": " + what;
+    return WORLD_B200_EINVAL;
+  };
+  if (!x || !opt || !y || n < 0 || fs <= 0 || x_stride <= 0 || y_stride <= 0)
+    return fail("x, option and y must be given, with n_utts >= 0, fs > 0 and positive strides");
+  if (nbit != 0 && nbit != 8 && nbit != 16 && nbit != 24 && nbit != 32) return fail("nbit must be 0, 8, 16, 24 or 32");
+  if (nbit_out != 0 && nbit_out != 16) return fail("nbit_out must be 0 (float64) or 16 (int16)");
+  int rc = check_chain_f0_options(c, opt, harvest_options, dio_options, n, fs, who);
+  if (!rc) rc = synthesis_fft(c, opt->cheaptrick.fft_size, &tp->lg);
+  if (rc) return rc;
+  tp->modify = f0_scale || spectral_ratio;
+  if (tp->modify) rc = modify_plan(c, n, opt->cheaptrick.fft_size, fs, f0_scale, spectral_ratio, &tp->mod);
+  if (rc) return rc;
+  const double frame_period = opt->f0_method == WORLD_B200_F0_HARVEST ? opt->harvest.frame_period : opt->dio.frame_period;
+  if (!(frame_period > 0.0)) return fail("the F0 method's frame_period must be > 0");
+  tp->nbit = nbit; tp->nbit_out = nbit_out; tp->x_stride = x_stride; tp->y_stride = y_stride; tp->fs = fs;
+  tp->fft_size = opt->cheaptrick.fft_size; tp->frame_period = frame_period; tp->f0_stride = 1;
+  tp->f_len.resize(n); tp->y_len.resize(n); tp->fp.resize(n);
+  for (int u = 0; u < n; ++u) {
+    const int xl = x_lengths ? x_lengths[u] : x_stride;
+    const double ts = time_scale ? time_scale[u] : 1.0;
+    if (xl < 1 || xl > x_stride) {
+      snprintf(msg, sizeof msg, "x_lengths[%d] = %d is outside its padded row of %d samples", u, xl, x_stride);
+      return fail(msg);
+    }
+    if (!(ts > 0.0) || !isfinite(ts)) {
+      snprintf(msg, sizeof msg, "time_scale[%d] = %.17g is not a finite factor > 0", u, ts);
+      return fail(msg);
+    }
+    tp->f_len[u] = frames_for(fs, xl, frame_period);
+    tp->y_len[u] = world_b200_transform_samples(fs, xl, frame_period, ts);
+    if (tp->f_len[u] < 2) {
+      snprintf(msg, sizeof msg, "utterance %d has %d frame(s); Synthesis needs 2", u, tp->f_len[u]);
+      return fail(msg);
+    }
+    if (tp->y_len[u] < 2 || tp->y_len[u] > y_stride) {
+      snprintf(msg, sizeof msg, "y_length of utterance %d is %d, outside [2, y_stride = %d]", u, tp->y_len[u], y_stride);
+      return fail(msg);
+    }
+    tp->fp[u] = (frame_period * ts) / 1000.0;   // synthesis_batch's frame_period / 1000.0, with the same product
+    tp->f0_stride = imax(tp->f0_stride, tp->f_len[u]);
+  }
+  return 0;
+}
+
+// Utterances [u0, u0 + n) of a checked call: x and y point at utterance u0's rows (DEVICE), x_lengths and the
+// per-utterance options are the call's whole arrays.  The utterances are cut into slices that alternate between the
+// two lanes of open_lanes.  A slice's rows (float64 input, time axis, f0, spectrogram, aperiodicity) live from its
+// analysis to its synthesis in one buffer per lane, taken from the lane's pool and sized for its largest slice; slices
+// are sized so that the buffer takes at most about half the lane's scratch budget, leaving the rest to the stages.
+// Issue order A(0), A(1), S(0), A(2), S(1), ... (A = F0 stage, CheapTrick, D4C and modify; S = synthesis): a lane runs
+// its slices in stream order, so A(s + 1) never overwrites rows S(s - 1) still reads, and while synthesis_run waits
+// for its pulse counts (a host synchronisation of its lane), the other lane has an analysis queued.  One lane (one
+// slice, or the host emulation) runs A(s), S(s) in turn.  The caller's stream waits for both lanes on return.
+int transform_run(WorldB200 *h, const TransformPlan &tp, const void *x, const int *x_lengths,
+                  const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
+                  const DioOption *dio_options, int u0, int n, void *y) {
+  if (n <= 0) return 0;
+  const int f0_stride = tp.f0_stride, x_stride = tp.x_stride, bins = tp.fft_size / 2 + 1, fs = tp.fs;
+  const size_t in_row = (size_t)x_stride * (tp.nbit ? tp.nbit / 8 : 8), out_row = (size_t)tp.y_stride * (tp.nbit_out ? 2 : 8);
+  struct Rows {
+    size_t x, t, f, sp, ap, total;
+    Rows(int m, const TransformPlan &tp, int bins) {
+      ArenaPlan a;
+      x = a.add(tp.nbit ? (size_t)m * tp.x_stride * 8 : 0);
+      t = a.add((size_t)m * tp.f0_stride * 8); f = a.add((size_t)m * tp.f0_stride * 8);
+      sp = a.add((size_t)m * tp.f0_stride * bins * 8); ap = a.add((size_t)m * tp.f0_stride * bins * 8);
+      total = a.total;
+    }
+  };
+  int n_slices = 1;
+  {
+#ifndef WB_EMU
+    const bool two = n > 1;
+#else
+    const bool two = false;
+#endif
+    const double lane_budget = (double)h->c.scratch_budget / (two ? 2.0 : 1.0);
+    const int fit = (int)dmax(1.0, dmin((double)n, lane_budget / 2.0 / (double)Rows(1, tp, bins).total));
+    n_slices = (n + fit - 1) / fit;
+    if (two) n_slices = imin(n, (n_slices + 1) / 2 * 2);   // an even count: both lanes get the same work
+  }
+  std::vector<int> bounds(n_slices + 1);
+  for (int s = 0; s <= n_slices; ++s) bounds[s] = (int)((long long)n * s / n_slices);
+  WorldB200 *lanes[2];
+  int rc = open_lanes(h, n_slices, lanes);
+  if (rc) return rc;
+  const bool one_lane = lanes[0] == lanes[1];
+  const size_t own_budget = h->c.scratch_budget;   // restored on return when the context is its own (only) lane
+  int most[2] = {0, 0};
+  for (int s = 0; s < n_slices; ++s) {
+    const int l = one_lane ? 0 : (s & 1);
+    most[l] = imax(most[l], bounds[s + 1] - bounds[s]);
+  }
+  unsigned char *rows[2] = {nullptr, nullptr};
+  for (int l = 0; l < (one_lane ? 1 : 2) && !rc; ++l) {
+    Ctx *c = &lanes[l]->c;
+    const size_t bytes = Rows(most[l], tp, bins).total;
+    rows[l] = (unsigned char *)pool_acquire(c, bytes);
+    if (!rows[l]) { h->c.last_error = c->last_error; rc = WORLD_B200_ENOMEM; }
+    c->scratch_budget -= bytes < c->scratch_budget / 2 ? bytes : c->scratch_budget / 2;
+  }
+  if (one_lane) rows[1] = rows[0];
+  // slice s: its lane, the global index of its first utterance, its size and where its rows are
+  auto slice = [&](int s, WorldB200 **L, int *g, int *m, double **xs, double **t, double **f, double **sp, double **ap) {
+    const int l = one_lane ? 0 : (s & 1);
+    const Rows r(most[l], tp, bins);
+    *L = lanes[l]; *g = u0 + bounds[s]; *m = bounds[s + 1] - bounds[s];
+    *xs = (double *)(rows[l] + r.x); *t = (double *)(rows[l] + r.t); *f = (double *)(rows[l] + r.f);
+    *sp = (double *)(rows[l] + r.sp); *ap = (double *)(rows[l] + r.ap);
+  };
+  auto analyse = [&](int s) {
+    WorldB200 *L; int g, m; double *xd, *t, *f, *sp, *ap;
+    slice(s, &L, &g, &m, &xd, &t, &f, &sp, &ap);
+    const int *xl = x_lengths ? x_lengths + g : nullptr;
+    const int *fl = tp.f_len.data() + g;
+    const unsigned char *xin = (const unsigned char *)x + (size_t)bounds[s] * in_row;
+    const double *xs = tp.nbit ? xd : (const double *)xin;
+    int e = tp.nbit ? world_b200_pcm_to_double_batch(L, xin, tp.nbit, m, x_stride, xl, xd) : 0;
+    if (!e) e = dev_memset(&L->c, t, 0, (size_t)m * f0_stride * 8);
+    if (!e) e = dev_memset(&L->c, f, 0, (size_t)m * f0_stride * 8);
+    if (!e)
+      e = run_f0_stage(L, xs, m, x_stride, xl, fs, opt, harvest_options ? harvest_options + g : nullptr,
+                       dio_options ? dio_options + g : nullptr, fl, t, f, f0_stride);
+    if (!e) e = world_b200_cheaptrick_batch(L, xs, m, x_stride, xl, fs, t, f, fl, f0_stride, &opt->cheaptrick, sp);
+    if (!e)
+      e = world_b200_d4c_batch(L, xs, m, x_stride, xl, fs, t, f, fl, f0_stride, tp.fft_size, &opt->d4c, ap);
+    if (!e && tp.modify) e = modify_run(&L->c, tp.mod, g, m, fl, f0_stride, f, sp);
+    if (e && L != h) h->c.last_error = L->c.last_error;
+    return e;
+  };
+  auto synthesise = [&](int s) {
+    WorldB200 *L; int g, m; double *xd, *t, *f, *sp, *ap;
+    slice(s, &L, &g, &m, &xd, &t, &f, &sp, &ap);
+    const int e = synthesis_run(&L->c, f, tp.f_len.data() + g, m, f0_stride, sp, ap, nullptr, tp.fft_size, tp.lg,
+                                tp.frame_period, fs, tp.y_len.data() + g, tp.y_stride,
+                                (unsigned char *)y + (size_t)bounds[s] * out_row, tp.nbit_out, nullptr, 0,
+                                tp.fp.data() + g);
+    if (e && L != h) h->c.last_error = L->c.last_error;
+    return e;
+  };
+  const int lag = one_lane ? 0 : 1;
+  for (int k = 0; k < n_slices + lag && !rc; ++k) {
+    if (k < n_slices) rc = analyse(k);
+    if (!rc && k >= lag) rc = synthesise(k - lag);
+  }
+  join_lanes(h, lanes);   // even after an error: the caller's stream must not run ahead of the lanes
+  // back to the pools while the lanes may still read them: only work ordered after this call's gets them again
+  pool_release(&lanes[0]->c, rows[0]);
+  if (rows[1] != rows[0]) pool_release(&lanes[1]->c, rows[1]);
+  h->c.scratch_budget = own_budget;
+  return rc;
+}
+
+}  // namespace wb
+
+extern "C" {
+
+int world_b200_transform_samples(int fs, int x_length, double frame_period, double time_scale) {
+  const double fp = frame_period * time_scale;
+  if (!(fp > 0.0) || !isfinite(fp)) return 0;
+  const double v = (frames_for(fs, x_length, frame_period) - 1) * fp / 1000.0 * fs;
+  return v < 2147483646.0 ? static_cast<int>(v) + 1 : 0;
+}
+
+int world_b200_transform_batch(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride, const int *x_lengths,
+                               int fs, const WorldB200AnalysisOption *option, const HarvestOption *harvest_options,
+                               const DioOption *dio_options, const double *f0_scale, const double *spectral_ratio,
+                               const double *time_scale, int nbit_out, void *y, int y_stride, int *y_lengths) {
+  if (!h) return WORLD_B200_EINVAL;
+  DeviceGuard guard_(&h->c);
+  TransformPlan tp;
+  const int rc = transform_check(h, x, nbit, n_utts, x_stride, x_lengths, fs, option, harvest_options, dio_options,
+                                 f0_scale, spectral_ratio, time_scale, nbit_out, y, y_stride, "transform_batch", &tp);
+  if (rc) return rc;
+  if (y_lengths) std::copy(tp.y_len.begin(), tp.y_len.end(), y_lengths);
+  return transform_run(h, tp, x, x_lengths, option, harvest_options, dio_options, 0, n_utts, y);
 }
 
 // ---- multi-GPU (SURVEY.md 8e): utterances sharded over ranks, outputs reassembled on every rank by NCCL

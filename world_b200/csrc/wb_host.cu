@@ -15,6 +15,8 @@
 #include <memory>
 #include <mutex>
 #include <chrono>
+#include <algorithm>
+#include <string.h>
 
 using namespace wb;
 
@@ -25,6 +27,15 @@ int check_chain_f0_options(Ctx *c, const WorldB200AnalysisOption *opt, const Har
 int run_f0_stage(WorldB200 *h, const double *x, int m, int x_stride, const int *x_lengths, int fs,
                  const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options, const DioOption *dio_options,
                  const int *f0_lengths, double *time_axis, double *f0, int f0_stride);
+// wb_api.cu: the checks and plan of a voice transformation, and its device driver over utterances [u0, u0 + n)
+int transform_check(WorldB200 *h, const void *x, int nbit, int n, int x_stride, const int *x_lengths, int fs,
+                    const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
+                    const DioOption *dio_options, const double *f0_scale, const double *spectral_ratio,
+                    const double *time_scale, int nbit_out, const void *y, int y_stride, const char *who,
+                    TransformPlan *tp);
+int transform_run(WorldB200 *h, const TransformPlan &tp, const void *x, const int *x_lengths,
+                  const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
+                  const DioOption *dio_options, int u0, int n, void *y);
 }  // namespace wb
 
 namespace {
@@ -520,6 +531,116 @@ int synthesis_pipeline(WorldB200 *h, CodedRows *coded, int lg, const double *f0,
   return rc;
 }
 
+// Voice transformation for host arrays: utterance chunks of PCM are uploaded on s_in, transformed by transform_run
+// (which forks from and joins back to the context's stream) and their output rows downloaded on s_out.  Inputs and
+// outputs are double-buffered; events order their reuse.  transform_run synchronises the host with its lanes at each
+// synthesis pass, so the upload of chunk k+1 is enqueued before chunk k is transformed.  Chunks of WB_HOST_CHUNK
+// utterances (default 512), fewer when the four buffers would take more than a sixth of the scratch budget.
+int transform_pipeline(WorldB200 *h, const TransformPlan &tp, const void *x, int n_utts, const int *x_lengths,
+                       const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
+                       const DioOption *dio_options, void *y) {
+  Ctx *ctx = ctx_of(h);
+  const size_t per_in = (size_t)tp.x_stride * (tp.nbit ? tp.nbit / 8 : 8);
+  const size_t per_out = (size_t)tp.y_stride * (tp.nbit_out ? 2 : 8);
+  int chunk = 512;
+  if (const char *e = getenv("WB_HOST_CHUNK")) chunk = atoi(e) > 0 ? atoi(e) : chunk;
+  chunk = imin(chunk, (int)dmax(1.0, (double)(ctx->scratch_budget / 6) / (double)(2 * (per_in + per_out))));
+  chunk = balanced_chunk(n_utts, chunk);
+  const int n_chunks = (n_utts + chunk - 1) / chunk;
+#ifndef WB_EMU
+  cudaStream_t s_compute = ctx->stream, s_in = nullptr, s_out = nullptr;
+  if (cudaStreamCreateWithFlags(&s_in, cudaStreamNonBlocking) != cudaSuccess) {
+    ctx->last_error = "cudaStreamCreate failed";
+    cudaGetLastError();
+    return WORLD_B200_ECUDA;
+  }
+  if (cudaStreamCreateWithFlags(&s_out, cudaStreamNonBlocking) != cudaSuccess) {
+    ctx->last_error = "cudaStreamCreate failed";
+    cudaGetLastError();
+    cudaStreamDestroy(s_in);
+    return WORLD_B200_ECUDA;
+  }
+  cudaEvent_t ev_in[2], ev_cdone[2], ev_out[2], ev_start;
+  bool ev_ok = cudaEventCreateWithFlags(&ev_start, cudaEventDisableTiming) == cudaSuccess;
+  for (int i = 0; i < 2; ++i) {
+    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_in[i], cudaEventDisableTiming) == cudaSuccess;
+    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_cdone[i], cudaEventDisableTiming) == cudaSuccess;
+    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_out[i], cudaEventDisableTiming) == cudaSuccess;
+  }
+  if (!ev_ok) {   // (as in analyze_pipeline: events created so far are released with the process)
+    ctx->last_error = "cudaEventCreate failed";
+    cudaGetLastError();
+    cudaStreamDestroy(s_in);
+    cudaStreamDestroy(s_out);
+    return WORLD_B200_ECUDA;
+  }
+  // the uploads start after the work already on the context's stream: a pooled buffer released by a stream-ordered
+  // call may still be read there
+  cudaEventRecord(ev_start, s_compute);
+  cudaStreamWaitEvent(s_in, ev_start, 0);
+#endif
+  DevBuf din[2], dout[2];
+  int rc = 0;
+  for (int i = 0; i < (n_chunks > 1 ? 2 : 1) && !rc; ++i) {
+    rc = ensure(ctx, &din[i], (size_t)chunk * per_in);
+    if (!rc) rc = ensure(ctx, &dout[i], (size_t)chunk * per_out);
+  }
+  // chunk k's PCM rows into din[k & 1]
+  auto upload = [&](int k) {
+    const int u0 = k * chunk, m = imin(chunk, n_utts - u0);
+    const unsigned char *src = (const unsigned char *)x + (size_t)u0 * per_in;
+#ifndef WB_EMU
+    if (k >= 2) cudaStreamWaitEvent(s_in, ev_cdone[k & 1], 0);   // chunk k-2 has read din[k & 1]
+    cudaMemcpyAsync(din[k & 1].p, src, (size_t)m * per_in, cudaMemcpyHostToDevice, s_in);
+    cudaEventRecord(ev_in[k & 1], s_in);
+#else
+    memcpy(din[k & 1].p, src, (size_t)m * per_in);
+#endif
+  };
+  if (!rc) upload(0);
+  for (int k = 0; k < n_chunks && !rc; ++k) {
+    const int u0 = k * chunk, m = imin(chunk, n_utts - u0), s = k & 1;
+    if (k + 1 < n_chunks) upload(k + 1);
+#ifndef WB_EMU
+    cudaStreamWaitEvent(s_compute, ev_in[s], 0);
+    if (k >= 2) cudaStreamWaitEvent(s_compute, ev_out[s], 0);   // chunk k-2's rows are on the host
+#endif
+    // whole rows are downloaded: samples beyond an utterance's length read as zero on the host
+    bool ragged = false;
+    for (int i = 0; i < m; ++i) ragged = ragged || tp.y_len[u0 + i] != tp.y_stride;
+    if (ragged) rc = dev_memset(ctx, dout[s].p, 0, (size_t)m * per_out);
+    if (!rc) rc = transform_run(h, tp, din[s].p, x_lengths, opt, harvest_options, dio_options, u0, m, dout[s].p);
+    if (rc) break;
+    unsigned char *dst = (unsigned char *)y + (size_t)u0 * per_out;
+#ifndef WB_EMU
+    cudaEventRecord(ev_cdone[s], s_compute);
+    cudaStreamWaitEvent(s_out, ev_cdone[s], 0);
+    cudaMemcpyAsync(dst, dout[s].p, (size_t)m * per_out, cudaMemcpyDeviceToHost, s_out);
+    cudaEventRecord(ev_out[s], s_out);
+#else
+    memcpy(dst, dout[s].p, (size_t)m * per_out);
+#endif
+  }
+#ifndef WB_EMU
+  // copies and memsets above are not checked one by one: a failure is sticky and surfaces here
+  cudaError_t e_sync = cudaStreamSynchronize(s_in);
+  if (e_sync == cudaSuccess) e_sync = cudaStreamSynchronize(s_compute);
+  if (e_sync == cudaSuccess) e_sync = cudaStreamSynchronize(s_out);
+  if (e_sync != cudaSuccess && !rc) { ctx->last_error = std::string("transform pipeline: ") + cudaGetErrorString(e_sync); rc = WORLD_B200_ECUDA; }
+  for (int i = 0; i < 2; ++i) { cudaEventDestroy(ev_in[i]); cudaEventDestroy(ev_cdone[i]); cudaEventDestroy(ev_out[i]); }
+  cudaEventDestroy(ev_start);
+  cudaStreamDestroy(s_in);
+  cudaStreamDestroy(s_out);
+  if (!rc) {
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { ctx->last_error = cudaGetErrorString(e); rc = WORLD_B200_ECUDA; }
+  }
+#endif
+  for (int i = 0; i < 2; ++i) { pool_release(ctx, din[i].p); pool_release(ctx, dout[i].p); }
+  if (!rc) rc = world_b200_synchronize(h);
+  return rc;
+}
+
 // world_b200_synthesis_coded_host and, with f0_scale / spectral_ratio, world_b200_synthesis_coded_host_modified
 int synthesis_coded_host(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts, int f0_stride,
                          const double *coded_spectral_envelope, int number_of_dimensions,
@@ -577,6 +698,23 @@ extern "C" int world_b200_synthesis_coded_host_modified(WorldB200 *h, const doub
   return synthesis_coded_host(h, f0, f0_lengths, n_utts, f0_stride, coded_spectral_envelope, number_of_dimensions,
                               coded_aperiodicity, fft_size, frame_period, fs, y_lengths, y_stride, nbit, y, f0_scale,
                               spectral_ratio);
+}
+
+extern "C" int world_b200_transform_host(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride,
+                                         const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                         const HarvestOption *harvest_options, const DioOption *dio_options,
+                                         const double *f0_scale, const double *spectral_ratio,
+                                         const double *time_scale, int nbit_out, void *y, int y_stride,
+                                         int *y_lengths) {
+  if (!h) return WORLD_B200_EINVAL;
+  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
+  TransformPlan tp;
+  const int rc = transform_check(h, x, nbit, n_utts, x_stride, x_lengths, fs, option, harvest_options, dio_options,
+                                 f0_scale, spectral_ratio, time_scale, nbit_out, y, y_stride, "transform_host", &tp);
+  if (rc) return rc;
+  if (y_lengths) std::copy(tp.y_len.begin(), tp.y_len.end(), y_lengths);
+  if (n_utts == 0) return 0;
+  return transform_pipeline(h, tp, x, n_utts, x_lengths, option, harvest_options, dio_options, y);
 }
 
 extern "C" int world_b200_analyze_host(WorldB200 *h, const double *x, int n_utts, int x_stride,

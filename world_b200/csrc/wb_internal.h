@@ -190,6 +190,11 @@ void modify_f0_launch(Ctx *ctx, const ModifyDevice &d, const int *f_len, int n_u
 void modify_stretch_launch(Ctx *ctx, const ModifyDevice &d, int bins, const int *f_len, int n_utts, int f_stride,
                            int max_f, double *spectrogram);
 
+// Both halves of the plan on the device rows of its utterances [u0, u0 + n_utts) in place (f0 [n][f0_stride],
+// spectrogram [n][f0_stride][plan.bins]; host lengths), frames < f0_lengths[u]: world_b200_modify_batch's launches.
+int modify_run(Ctx *ctx, const ModifyPlan &plan, int u0, int n_utts, const int *f0_lengths, int f0_stride, double *f0,
+               double *spectrogram);
+
 int synthesis_fft(Ctx *ctx, int fft_size, int *lg_out);   // EINVAL unless a power of two in [16, 4096]
 // the decode tables of a coded call; EINVAL for number_of_dimensions, or no aperiodicity rows where fs has bands
 int synthesis_coded_tables(Ctx *ctx, int fs, int fft_size, int number_of_dimensions, bool have_aperiodicity,
@@ -213,10 +218,24 @@ struct SynthesisSizing {
 // budget, each with one read-back of its pulse counts.  coded null: full rows; y: double (nbit 0) or int16 (nbit 16).
 // mod (coded rows only): utterance i of the call is the plan's utterance mod_u0 + i; each pass synthesises from a
 // scaled copy of its f0 rows and stretches its decoded envelope block right after the decode.
+// fp_u (host, n_utts entries, or null): the frame period of each utterance in seconds, used instead of
+// frame_period / 1000.0; each pass uploads its slice.
 int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts, int f0_stride,
                   const double *spectrogram, const double *aperiodicity, const CodedRows *coded, int fft_size, int lg,
                   double frame_period, int fs, const int *y_lengths, int y_stride, void *y, int nbit,
-                  const ModifyPlan *mod = nullptr, int mod_u0 = 0);
+                  const ModifyPlan *mod = nullptr, int mod_u0 = 0, const double *fp_u = nullptr);
+// wb_api.cu: voice transformation (world_b200_transform_*), checked and planned once per call by transform_check;
+// transform_run (device rows) and the host pipeline (wb_host.cu) read it.
+struct TransformPlan {
+  int nbit = 0, nbit_out = 0, x_stride = 0, y_stride = 0, fs = 0, fft_size = 0, lg = 0;
+  int f0_stride = 0;               // the largest frame count of the call
+  double frame_period = 0.0;       // the analysis frame period (ms)
+  std::vector<int> f_len, y_len;   // [n] frames and output samples of each utterance
+  std::vector<double> fp;          // [n] synthesis frame period (s): (frame_period * time_scale[u]) / 1000.0
+  bool modify = false;             // f0_scale or spectral_ratio given
+  ModifyPlan mod;
+};
+
 int cheaptrick_run(Ctx *ctx, const Batch &b, double q1, int fft_size, double *spectrogram,
                    const CodecTables *coded = nullptr, double *coded_out = nullptr);
 int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *aperiodicity,

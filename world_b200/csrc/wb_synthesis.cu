@@ -38,6 +38,7 @@ struct SynParams {
   const double *f0; const int *f_len; int f_stride;
   const double *sp; const double *ap; int fft_size, lg_fft;
   double frame_period;      // seconds
+  const double *fp_u;       // [n] frame period of each utterance (seconds), or null: frame_period for all
   int fs;
   const int *y_len; int y_stride;
   // time base scratch
@@ -60,7 +61,7 @@ WB_KERNEL(256, 2) syn_timebase_kernel(SynParams p) {
   WB_SHARED int cnt[258];
   const int tid = WB_TID, nth = WB_NTH, u = blockIdx.x;
   const int L = p.f_len[u], n = p.y_len[u], fs = p.fs;
-  const double fp = p.frame_period;
+  const double fp = p.fp_u ? p.fp_u[u] : p.frame_period;
   const double lowest_f0 = fs / p.fft_size + 1.0;   // synthesis.cpp:362 (integer division, then + 1.0)
   const double *f0 = p.f0 + (size_t)u * p.f_stride;
   double *phase = p.phase + (size_t)u * p.y_stride;
@@ -201,9 +202,10 @@ WB_KERNEL(128, 3) syn_pulse_kernel(SynParams p) {
   const double *sp = p.sp + (size_t)u * p.f_stride * bins, *ap = p.ap + (size_t)u * p.f_stride * bins;
 
   // GetSpectralEnvelope / GetAperiodicRatio (:140-179)
-  const int fl = imin(L - 1, static_cast<int>(floor(current_time / p.frame_period)));
-  const int ce = imin(L - 1, static_cast<int>(ceil(current_time / p.frame_period)));
-  const double interp = current_time / p.frame_period - fl;
+  const double fp = p.fp_u ? p.fp_u[u] : p.frame_period;
+  const int fl = imin(L - 1, static_cast<int>(floor(current_time / fp)));
+  const int ce = imin(L - 1, static_cast<int>(ceil(current_time / fp)));
+  const double interp = current_time / fp - fl;
   for (int k = tid; k <= half; k += nth) {
     double e, a;
     const double a0 = dmax(0.001, dmin(0.999999999999, ap[fl * bins + k]));
@@ -476,6 +478,25 @@ void modify_stretch_launch(Ctx *ctx, const ModifyDevice &d, int bins, const int 
                  n_utts, f_stride, bins, d.table, d.idx, d.frac);
 }
 
+int modify_run(Ctx *ctx, const ModifyPlan &plan, int u0, int n_utts, const int *f0_lengths, int f0_stride, double *f0,
+               double *spectrogram) {
+  int max_f = 0;
+  for (int u = 0; u < n_utts; ++u) max_f = imax(max_f, f0_lengths[u]);
+  if (max_f == 0 || (plan.scale.empty() && plan.table.empty())) return 0;
+  ArenaPlan a;
+  const size_t o_len = a.add((size_t)n_utts * 4), o_mod = a.add(plan.device_bytes(n_utts));
+  unsigned char *blk = arena_block(ctx, a.total);
+  if (!blk) return WORLD_B200_ENOMEM;
+  ModifyDevice d;
+  int rc = dev_memcpy_h2d(ctx, blk + o_len, f0_lengths, (size_t)n_utts * 4);
+  if (!rc) rc = modify_upload(ctx, plan, u0, n_utts, blk + o_mod, &d);
+  if (rc) return rc;
+  const int *f_len = (const int *)(blk + o_len);
+  if (!plan.scale.empty()) modify_f0_launch(ctx, d, f_len, n_utts, f0_stride, max_f, f0, f0);
+  if (!plan.table.empty()) modify_stretch_launch(ctx, d, plan.bins, f_len, n_utts, f0_stride, max_f, spectrogram);
+  return dev_check(ctx, "modify");
+}
+
 int synthesis_fft(Ctx *ctx, int fft_size, int *lg_out) {
   int lg = 0;
   while ((1 << lg) < fft_size) ++lg;
@@ -549,7 +570,7 @@ int SynthesisSizing::fit(int cap) const { return (int)dmin(65535.0, budget / (do
 int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts, int f0_stride,
                   const double *spectrogram, const double *aperiodicity, const CodedRows *coded, int fft_size, int lg,
                   double frame_period, int fs, const int *y_lengths, int y_stride, void *y, int nbit,
-                  const ModifyPlan *mod, int mod_u0) {
+                  const ModifyPlan *mod, int mod_u0, const double *fp_u) {
   if (n_utts == 0) return 0;
   std::vector<int> lens((size_t)2 * n_utts);
   int rc = synthesis_lengths(ctx, f0_lengths, n_utts, f0_stride, y_lengths, y_stride, lens.data());
@@ -605,6 +626,7 @@ int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts,
     }
     const size_t o_mod = mod ? plan.add(mod->device_bytes(n)) : 0;
     const size_t o_f0m = scale_f0 ? plan.add((size_t)n * f0_stride * 8) : 0;
+    const size_t o_fp = fp_u ? plan.add((size_t)n * 8) : 0;
     unsigned char *blk = arena_block(ctx, plan.total);
     if (!blk) return WORLD_B200_ENOMEM;
     std::vector<int> l2((size_t)2 * n), pl(n, pulse_cap);
@@ -613,6 +635,7 @@ int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts,
     rc = dev_memcpy_h2d(ctx, blk + o_len, l2.data(), l2.size() * 4);
     if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_dcr, dcr.data(), dcr.size() * 8);
     if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_pl, pl.data(), (size_t)n * 4);
+    if (!rc && fp_u) rc = dev_memcpy_h2d(ctx, blk + o_fp, fp_u + u0, (size_t)n * 8);
     if (coded) {
       const CodecTables &s = coded->tsp, &a = coded->tap;
       if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_sidx, s.idx.data(), s.idx.size() * 4);
@@ -632,6 +655,7 @@ int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts,
       p.sp = spectrogram + (size_t)u0 * f0_stride * bins; p.ap = aperiodicity + (size_t)u0 * f0_stride * bins;
     }
     p.fft_size = fft_size; p.lg_fft = lg; p.frame_period = frame_period / 1000.0; p.fs = fs;
+    p.fp_u = fp_u ? (const double *)(blk + o_fp) : nullptr;
     p.y_len = (const int *)(blk + o_len) + n; p.y_stride = y_stride;
     p.phase = (double *)(blk + o_phase); p.vuv = (double *)(blk + o_vuv); p.flag_cnt = nullptr;
     p.pulse_idx = (int *)(blk + o_pidx); p.pulse_shift = (double *)(blk + o_psh); p.n_pulses = (int *)(blk + o_np);
@@ -787,7 +811,6 @@ extern "C" int world_b200_modify_batch(WorldB200 *h, double *f0, const int *f0_l
     return WORLD_B200_EINVAL;
   }
   std::vector<int> lens(n_utts > 0 ? n_utts : 1);
-  int max_f = 0;
   for (int u = 0; u < n_utts; ++u) {
     lens[u] = f0_lengths ? f0_lengths[u] : f0_stride;
     if (lens[u] < 0 || lens[u] > f0_stride) {
@@ -797,21 +820,9 @@ extern "C" int world_b200_modify_batch(WorldB200 *h, double *f0, const int *f0_l
       ctx->last_error = msg;
       return WORLD_B200_EINVAL;
     }
-    max_f = imax(max_f, lens[u]);
   }
   ModifyPlan plan;
   int rc = modify_plan(ctx, n_utts, fft_size, fs, f0_scale, spectral_ratio, &plan);
-  if (rc || max_f == 0 || (!f0_scale && !spectral_ratio)) return rc;
-  ArenaPlan a;
-  const size_t o_len = a.add((size_t)n_utts * 4), o_mod = a.add(plan.device_bytes(n_utts));
-  unsigned char *blk = arena_block(ctx, a.total);
-  if (!blk) return WORLD_B200_ENOMEM;
-  ModifyDevice d;
-  rc = dev_memcpy_h2d(ctx, blk + o_len, lens.data(), (size_t)n_utts * 4);
-  if (!rc) rc = modify_upload(ctx, plan, 0, n_utts, blk + o_mod, &d);
   if (rc) return rc;
-  const int *f_len = (const int *)(blk + o_len);
-  if (f0_scale) modify_f0_launch(ctx, d, f_len, n_utts, f0_stride, max_f, f0, f0);
-  if (spectral_ratio) modify_stretch_launch(ctx, d, fft_size / 2 + 1, f_len, n_utts, f0_stride, max_f, spectrogram);
-  return dev_check(ctx, "modify");
+  return modify_run(ctx, plan, 0, n_utts, lens.data(), f0_stride, f0, spectrogram);
 }
