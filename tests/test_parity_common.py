@@ -444,7 +444,7 @@ def check_host_pipeline_chunking(world, golden, f0_method=0):
         rows[u, :lens[u]] = pcm16[2000 + 97 * u: 2000 + 97 * u + lens[u]]
     xd = rows.astype(np.float64) / 32768.0
     opt = world.analysis_option(fs, f0_method)
-    saved = {k: os.environ.get(k) for k in ("WB_HOST_SUB", "WB_HOST_CHUNK", "WB_HOST_TAPER_MIN", "WB_HOST_TAPER")}
+    saved = {k: os.environ.get(k) for k in ("WB_HOST_SUB", "WB_HOST_CHUNK", "WB_HOST_TAPER_MIN")}
     try:
         for k in saved:
             os.environ.pop(k, None)

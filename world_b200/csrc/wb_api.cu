@@ -671,58 +671,100 @@ int world_b200_harvest_batch_options(WorldB200 *h, const double *x, int n, int x
   return harvest_batch_impl(h, x, n, x_stride, x_lengths, fs, harvest_options, true, time_axis, f0, f0_stride);
 }
 
-// The two lanes of a chain cut into slices (sibling contexts on their own non-blocking streams, created on first use),
-// ordered after the work already on the context's stream.  lanes[l] receives lane l with half the scratch budget, or
-// the context itself for both when the chain is one slice (and always on the host emulation, which has one stream).
-static int open_lanes(WorldB200 *h, int n_slices, WorldB200 *lanes[2]) {
-  lanes[0] = lanes[1] = h;
-#ifndef WB_EMU
-  if (n_slices > 1) {
-    for (int l = 0; l < 2; ++l) {
-      if (!h->lane[l]) {
-        int rc = world_b200_create(h->c.device, &h->lane[l]);
-        if (rc) { h->c.last_error = "analyze_batch: cannot create a lane context"; return rc; }
-        cudaStream_t st;
-        cudaEvent_t ev;
-        // equal (lowest) priority for both lanes: giving one lane the highest priority was measured slower;
-        // only the communication stream outranks them (wb_multi.cu)
-        if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess ||
-            cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) {
-          h->c.last_error = "analyze_batch: cannot create a lane stream";
-          return WORLD_B200_ECUDA;
-        }
-        h->lane_stream[l] = st; h->ev_join[l] = ev;
-        h->lane[l]->c.stream = st;
-      }
-      h->lane[l]->c.scratch_budget = h->c.scratch_budget / 2;
-      lanes[l] = h->lane[l];
-    }
-    if (!h->ev_fork) {
-      cudaEvent_t ev;
-      if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) return WORLD_B200_ECUDA;
-      h->ev_fork = ev;
-    }
-    cudaEventRecord((cudaEvent_t)h->ev_fork, h->c.stream);
-    for (int l = 0; l < 2; ++l) cudaStreamWaitEvent((cudaStream_t)h->lane_stream[l], (cudaEvent_t)h->ev_fork, 0);
-  }
-#else
-  (void)n_slices;
-#endif
-  return 0;
-}
+}  // extern "C"
 
-// The context's stream waits for both lanes of open_lanes.
-static void join_lanes(WorldB200 *h, WorldB200 *const lanes[2]) {
+namespace {
+
+// The two lanes of a chain cut into slices: sibling contexts on their own non-blocking streams (created on first use),
+// ordered after the work already on the context's stream, each with half the context's scratch budget and one pooled
+// buffer sized for the largest of its slices.  Slices alternate between the lanes.  The chain has one lane, the context
+// itself, when it is one slice (and always on the host emulation, which has one stream).  On every return path the
+// destructor makes the context's stream wait for both lanes, gives the buffers back and restores the context's budget.
+class LaneScope {
+ public:
+  explicit LaneScope(WorldB200 *h) : h_(h), own_budget_(h->c.scratch_budget) { lanes_[0] = lanes_[1] = h; }
+  LaneScope(const LaneScope &) = delete;
+  LaneScope &operator=(const LaneScope &) = delete;
+  // bounds: the n_slices + 1 slice boundaries; bytes(m): the buffer of a lane whose largest slice has m utterances
+  // (0: no buffer).  A buffer comes from its lane's pool, not its arena (the stage drivers reset the arena when they
+  // return), and its bytes come out of the lane's scratch budget; the stages keep at least half of that budget (less
+  // would only mean more passes).
+  template <class Bytes>
+  int open(const std::vector<int> &bounds, Bytes bytes) {
+    const int n_slices = (int)bounds.size() - 1;
 #ifndef WB_EMU
-  if (lanes[0] != h)
-    for (int l = 0; l < 2; ++l) {
-      cudaEventRecord((cudaEvent_t)h->ev_join[l], (cudaStream_t)h->lane_stream[l]);
-      cudaStreamWaitEvent(h->c.stream, (cudaEvent_t)h->ev_join[l], 0);
+    if (n_slices > 1) {
+      WorldB200 *two[2];
+      for (int l = 0; l < 2; ++l) {
+        if (!h_->lane[l]) {
+          int rc = world_b200_create(h_->c.device, &h_->lane[l]);
+          if (rc) { h_->c.last_error = "analyze_batch: cannot create a lane context"; return rc; }
+          cudaStream_t st;
+          cudaEvent_t ev;
+          // equal (lowest) priority for both lanes: giving one lane the highest priority was measured slower;
+          // only the communication stream outranks them (wb_multi.cu)
+          if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess ||
+              cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) {
+            h_->c.last_error = "analyze_batch: cannot create a lane stream";
+            return WORLD_B200_ECUDA;
+          }
+          h_->lane_stream[l] = st; h_->ev_join[l] = ev;
+          h_->lane[l]->c.stream = st;
+        }
+        h_->lane[l]->c.scratch_budget = h_->c.scratch_budget / 2;
+        two[l] = h_->lane[l];
+      }
+      if (!h_->ev_fork) {
+        cudaEvent_t ev;
+        if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) return WORLD_B200_ECUDA;
+        h_->ev_fork = ev;
+      }
+      cudaEventRecord((cudaEvent_t)h_->ev_fork, h_->c.stream);
+      for (int l = 0; l < 2; ++l) cudaStreamWaitEvent((cudaStream_t)h_->lane_stream[l], (cudaEvent_t)h_->ev_fork, 0);
+      lanes_[0] = two[0]; lanes_[1] = two[1];
     }
-#else
-  (void)h; (void)lanes;
 #endif
-}
+    for (int s = 0; s < n_slices; ++s) most_[index(s)] = imax(most_[index(s)], bounds[s + 1] - bounds[s]);
+    for (int l = 0; l < (one_lane() ? 1 : 2); ++l) {
+      const size_t b = bytes(most_[l]);
+      if (b == 0) continue;
+      Ctx *c = &lanes_[l]->c;
+      buf_[l] = (unsigned char *)pool_acquire(c, b);
+      if (!buf_[l]) { h_->c.last_error = c->last_error; return WORLD_B200_ENOMEM; }
+      c->scratch_budget -= b < c->scratch_budget / 2 ? b : c->scratch_budget / 2;
+    }
+    return 0;
+  }
+  ~LaneScope() {
+#ifndef WB_EMU
+    if (!one_lane())   // even after an error: the caller's stream must not run ahead of the lanes
+      for (int l = 0; l < 2; ++l) {
+        cudaEventRecord((cudaEvent_t)h_->ev_join[l], (cudaStream_t)h_->lane_stream[l]);
+        cudaStreamWaitEvent(h_->c.stream, (cudaEvent_t)h_->ev_join[l], 0);
+      }
+#endif
+    // back to the pools while the lanes may still read them: a pooled buffer is only handed out again to work that is
+    // ordered after this call's (the lane's next slices, or the host pipelines, whose uploads wait for the stream)
+    for (int l = 0; l < 2; ++l) pool_release(&lanes_[l]->c, buf_[l]);
+    h_->c.scratch_budget = own_budget_;
+  }
+  bool one_lane() const { return lanes_[0] == lanes_[1]; }
+  WorldB200 *lane(int s) const { return lanes_[index(s)]; }          // slice s's lane
+  unsigned char *buffer(int s) const { return buf_[index(s)]; }      // ... its buffer
+  int most(int s) const { return most_[index(s)]; }                  // ... and the largest slice of that lane
+
+ private:
+  int index(int s) const { return one_lane() ? 0 : (s & 1); }
+  WorldB200 *h_;
+  WorldB200 *lanes_[2];
+  unsigned char *buf_[2] = {nullptr, nullptr};
+  int most_[2] = {0, 0};
+  size_t own_budget_;
+};
+
+}  // namespace
+
+extern "C" {
 
 // The whole chain on device arrays, cut into utterance slices that alternate between two lanes (sibling contexts
 // on their own non-blocking streams).  Per slice the stages run in order on the lane's stream; the two lanes run
@@ -799,32 +841,11 @@ static int analyze_batch_impl(WorldB200 *h, const void *x, int nbit, int n, int 
     for (int s = 0; s < n_slices; ++s) total += wgt[s];
     for (int s = 0; s < n_slices; ++s) { run += wgt[s]; bounds[s + 1] = (int)((long long)n * run / total); }
   }
-  WorldB200 *lanes[2];
-  int rc = open_lanes(h, n_slices, lanes);
-  if (rc) return rc;
   // nbit != 0: each lane converts its slice into a float64 buffer, which the slice's three stages then read.  A lane
-  // runs its slices in stream order, so one buffer per lane, sized for its largest slice, serves all of them.  It comes
-  // from the lane's pool, not its arena (the stage drivers reset the arena when they return), and its bytes come out
-  // of the lane's scratch budget; the stages keep at least half of that budget (less would only mean more passes).
-  double *xbuf[2] = {nullptr, nullptr};
-  const size_t own_budget = h->c.scratch_budget;   // restored on return when the context is its own (only) lane
-  if (nbit) {
-    const bool one_lane = lanes[0] == lanes[1];
-    int most[2] = {0, 0};
-    for (int s = 0; s < n_slices; ++s) {
-      const int l = one_lane ? 0 : (s & 1);
-      most[l] = imax(most[l], bounds[s + 1] - bounds[s]);
-    }
-    for (int l = 0; l < 2 && !rc; ++l) {
-      if (most[l] == 0) continue;
-      Ctx *c = &lanes[l]->c;
-      const size_t bytes = (size_t)most[l] * x_stride * sizeof(double);
-      xbuf[l] = (double *)pool_acquire(c, bytes);
-      if (!xbuf[l]) { h->c.last_error = c->last_error; rc = WORLD_B200_ENOMEM; }
-      c->scratch_budget -= bytes < c->scratch_budget / 2 ? bytes : c->scratch_budget / 2;
-    }
-    if (one_lane) xbuf[1] = xbuf[0];
-  }
+  // runs its slices in stream order, so one buffer per lane, sized for its largest slice, serves all of them.
+  LaneScope lanes(h);
+  int rc = lanes.open(bounds, [&](int m) { return nbit ? (size_t)m * x_stride * sizeof(double) : (size_t)0; });
+  if (rc) return rc;
 #ifndef WB_EMU
   // multi-GPU: the full arrays and how a finished slice reaches the other ranks -- pushed into their (IPC-mapped)
   // arrays by the copy engines where that is possible, grouped NCCL broadcasts otherwise (wb_multi.cu).  An array
@@ -836,7 +857,7 @@ static int analyze_batch_impl(WorldB200 *h, const void *x, int nbit, int n, int 
                                 aperiodicity ? (size_t)f0_stride * ap_row : 0};
   const bool exchange = gather && comm_ranks(h->comm) > 1;
   bool push = false;
-  if (!rc && exchange && !getenv("WB_NO_P2P")) {
+  if (exchange && !getenv("WB_NO_P2P")) {
     std::string err;
     const int pr = comm_p2p_prepare(h->comm, 4, fulls, &err);
     if (pr == 2) { h->c.last_error = err; rc = WORLD_B200_ECUDA; }
@@ -847,12 +868,12 @@ static int analyze_batch_impl(WorldB200 *h, const void *x, int nbit, int n, int 
     const int u0 = bounds[s], u1 = bounds[s + 1];
     const int m = u1 - u0;
     if (m <= 0) continue;
-    WorldB200 *L = lanes[s & 1];
+    WorldB200 *L = lanes.lane(s);
     const int *xl = x_lengths ? x_lengths + u0 : nullptr;
-    const double *xs = xbuf[s & 1];
+    const double *xs = (const double *)lanes.buffer(s);
     if (nbit)
       rc = world_b200_pcm_to_double_batch(L, (const unsigned char *)x + (size_t)u0 * x_stride * (nbit / 8), nbit, m,
-                                          x_stride, xl, xbuf[s & 1]);
+                                          x_stride, xl, (double *)lanes.buffer(s));
     else
       xs = (const double *)x + (size_t)u0 * x_stride;
     double *ts = time_axis + (size_t)u0 * f0_stride, *fs_ = f0 + (size_t)u0 * f0_stride;
@@ -875,17 +896,19 @@ static int analyze_batch_impl(WorldB200 *h, const void *x, int nbit, int n, int 
 #ifndef WB_EMU
     if (!rc && exchange) {
       // rows u0..u1 of every rank's block, as soon as this rank's are final (event on the lane's stream)
-      while ((int)h->ev_slice.size() <= s) {
+      while (!rc && (int)h->ev_slice.size() <= s) {
         cudaEvent_t ev;
-        if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) return WORLD_B200_ECUDA;
-        h->ev_slice.push_back(ev);
+        if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) == cudaSuccess) h->ev_slice.push_back(ev);
+        else { h->c.last_error = "cudaEventCreate failed"; rc = WORLD_B200_ECUDA; }
       }
-      cudaEvent_t ev = (cudaEvent_t)h->ev_slice[s];
-      cudaEventRecord(ev, L->c.stream);
-      std::string err;
-      const int g = push ? comm_p2p_push(h->comm, 4, full_elems, (size_t)n, (size_t)u0, (size_t)m, ev, &err)
-                         : comm_gather_rows_multi(h->comm, 4, fulls, full_elems, (size_t)n, (size_t)u0, (size_t)m, ev, &err);
-      if (g) { h->c.last_error = err; rc = WORLD_B200_ECUDA; }
+      if (!rc) {
+        cudaEvent_t ev = (cudaEvent_t)h->ev_slice[s];
+        cudaEventRecord(ev, L->c.stream);
+        std::string err;
+        const int g = push ? comm_p2p_push(h->comm, 4, full_elems, (size_t)n, (size_t)u0, (size_t)m, ev, &err)
+                           : comm_gather_rows_multi(h->comm, 4, fulls, full_elems, (size_t)n, (size_t)u0, (size_t)m, ev, &err);
+        if (g) { h->c.last_error = err; rc = WORLD_B200_ECUDA; }
+      }
     }
 #endif
   }
@@ -896,12 +919,6 @@ static int analyze_batch_impl(WorldB200 *h, const void *x, int nbit, int n, int 
     if (g && !rc) { h->c.last_error = err; rc = WORLD_B200_ECUDA; }
   }
 #endif
-  join_lanes(h, lanes);   // even after an error: the caller's stream must not run ahead of the lanes
-  // back to the pool while the lanes may still read them: a pooled buffer is only handed out again to work that is
-  // ordered after this call's (the lane's next slices, or the host pipelines, whose uploads wait for the stream)
-  pool_release(&lanes[0]->c, xbuf[0]);
-  if (xbuf[1] != xbuf[0]) pool_release(&lanes[1]->c, xbuf[1]);
-  h->c.scratch_budget = own_budget;
   return rc;
 }
 
@@ -992,7 +1009,7 @@ int transform_check(WorldB200 *h, const void *x, int nbit, int n, int x_stride, 
 
 // Utterances [u0, u0 + n) of a checked call: x and y point at utterance u0's rows (DEVICE), x_lengths and the
 // per-utterance options are the call's whole arrays.  The utterances are cut into slices that alternate between the
-// two lanes of open_lanes.  A slice's rows (float64 input, time axis, f0, spectrogram, aperiodicity) live from its
+// two lanes of a LaneScope.  A slice's rows (float64 input, time axis, f0, spectrogram, aperiodicity) live from its
 // analysis to its synthesis in one buffer per lane, taken from the lane's pool and sized for its largest slice; slices
 // are sized so that the buffer takes at most about half the lane's scratch budget, leaving the rest to the stages.
 // Issue order A(0), A(1), S(0), A(2), S(1), ... (A = F0 stage, CheapTrick, D4C and modify; S = synthesis): a lane runs
@@ -1029,32 +1046,16 @@ int transform_run(WorldB200 *h, const TransformPlan &tp, const void *x, const in
   }
   std::vector<int> bounds(n_slices + 1);
   for (int s = 0; s <= n_slices; ++s) bounds[s] = (int)((long long)n * s / n_slices);
-  WorldB200 *lanes[2];
-  int rc = open_lanes(h, n_slices, lanes);
+  LaneScope lanes(h);
+  int rc = lanes.open(bounds, [&](int m) { return Rows(m, tp, bins).total; });
   if (rc) return rc;
-  const bool one_lane = lanes[0] == lanes[1];
-  const size_t own_budget = h->c.scratch_budget;   // restored on return when the context is its own (only) lane
-  int most[2] = {0, 0};
-  for (int s = 0; s < n_slices; ++s) {
-    const int l = one_lane ? 0 : (s & 1);
-    most[l] = imax(most[l], bounds[s + 1] - bounds[s]);
-  }
-  unsigned char *rows[2] = {nullptr, nullptr};
-  for (int l = 0; l < (one_lane ? 1 : 2) && !rc; ++l) {
-    Ctx *c = &lanes[l]->c;
-    const size_t bytes = Rows(most[l], tp, bins).total;
-    rows[l] = (unsigned char *)pool_acquire(c, bytes);
-    if (!rows[l]) { h->c.last_error = c->last_error; rc = WORLD_B200_ENOMEM; }
-    c->scratch_budget -= bytes < c->scratch_budget / 2 ? bytes : c->scratch_budget / 2;
-  }
-  if (one_lane) rows[1] = rows[0];
   // slice s: its lane, the global index of its first utterance, its size and where its rows are
   auto slice = [&](int s, WorldB200 **L, int *g, int *m, double **xs, double **t, double **f, double **sp, double **ap) {
-    const int l = one_lane ? 0 : (s & 1);
-    const Rows r(most[l], tp, bins);
-    *L = lanes[l]; *g = u0 + bounds[s]; *m = bounds[s + 1] - bounds[s];
-    *xs = (double *)(rows[l] + r.x); *t = (double *)(rows[l] + r.t); *f = (double *)(rows[l] + r.f);
-    *sp = (double *)(rows[l] + r.sp); *ap = (double *)(rows[l] + r.ap);
+    const Rows r(lanes.most(s), tp, bins);
+    unsigned char *rows = lanes.buffer(s);
+    *L = lanes.lane(s); *g = u0 + bounds[s]; *m = bounds[s + 1] - bounds[s];
+    *xs = (double *)(rows + r.x); *t = (double *)(rows + r.t); *f = (double *)(rows + r.f);
+    *sp = (double *)(rows + r.sp); *ap = (double *)(rows + r.ap);
   };
   auto analyse = [&](int s) {
     WorldB200 *L; int g, m; double *xd, *t, *f, *sp, *ap;
@@ -1086,16 +1087,11 @@ int transform_run(WorldB200 *h, const TransformPlan &tp, const void *x, const in
     if (e && L != h) h->c.last_error = L->c.last_error;
     return e;
   };
-  const int lag = one_lane ? 0 : 1;
+  const int lag = lanes.one_lane() ? 0 : 1;
   for (int k = 0; k < n_slices + lag && !rc; ++k) {
     if (k < n_slices) rc = analyse(k);
     if (!rc && k >= lag) rc = synthesise(k - lag);
   }
-  join_lanes(h, lanes);   // even after an error: the caller's stream must not run ahead of the lanes
-  // back to the pools while the lanes may still read them: only work ordered after this call's gets them again
-  pool_release(&lanes[0]->c, rows[0]);
-  if (rows[1] != rows[0]) pool_release(&lanes[1]->c, rows[1]);
-  h->c.scratch_budget = own_budget;
   return rc;
 }
 

@@ -40,36 +40,188 @@ int transform_run(WorldB200 *h, const TransformPlan &tp, const void *x, const in
 
 namespace {
 
-struct DevBuf {
-  void *p = nullptr;
-  size_t cap = 0;
-};
-
-int ensure(Ctx *ctx, DevBuf *b, size_t bytes) {   // pooled: kept by the context between calls
-  if (bytes <= b->cap) return 0;
-  pool_release(ctx, b->p);
-  b->p = pool_acquire(ctx, bytes);
-  b->cap = b->p ? bytes : 0;
-  return b->p ? 0 : WORLD_B200_ENOMEM;
-}
-
 Ctx *ctx_of(WorldB200 *h) { return reinterpret_cast<Ctx *>(h); }  // Ctx is the first member
 
-}  // namespace
+// The scaffold of the host pipelines: uploads on s_in, kernels on the context's stream, downloads on s_out, the events
+// that order buffer reuse between the three, the pipeline's pooled device buffers and the WB_HOST_TRACE timeline.  On
+// the host emulation the copies are memcpy and the stream operations do nothing.
+//
+// Ordering rules.  open() makes s_in wait for the work already on the context's stream.  finish() synchronises s_in, the
+// context's stream and s_out, in that order, and only then releases the buffers; the destructor does the same on any
+// return path that did not reach finish(), so no buffer goes back to the pool while a copy may still use it.
+class HostPipe {
+ public:
+  enum Stream { IN, RUN, OUT };
 
-namespace {
+  HostPipe(WorldB200 *h, const char *who)
+      : ctx_(ctx_of(h)), who_(who), trace_(getenv("WB_HOST_TRACE") != nullptr), t0_(std::chrono::steady_clock::now()) {}
+  HostPipe(const HostPipe &) = delete;
+  HostPipe &operator=(const HostPipe &) = delete;
+  ~HostPipe() { close(); }
+
+  // the two streams and n_events events (indices 0 .. n_events - 1); ECUDA with last_error when one cannot be made
+  int open(int n_events) {
+#ifndef WB_EMU
+    if (cudaStreamCreateWithFlags(&s_in_, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaStreamCreateWithFlags(&s_out_, cudaStreamNonBlocking) != cudaSuccess)
+      return fail("cudaStreamCreate failed");
+    for (int i = 0; i <= n_events; ++i) {
+      cudaEvent_t e;
+      if (cudaEventCreateWithFlags(&e, cudaEventDisableTiming) != cudaSuccess) return fail("cudaEventCreate failed");
+      ev_.push_back(e);
+    }
+    mark("start", 0, RUN);
+    // the uploads start after the work already on the context's stream: a pooled buffer released by a stream-ordered
+    // call (the PCM buffer of world_b200_analyze_coded_batch) may still be read there
+    cudaEventRecord(ev_[n_events], ctx_->stream);
+    cudaStreamWaitEvent(s_in_, ev_[n_events], 0);
+#else
+    (void)n_events;
+#endif
+    return 0;
+  }
+
+  // a pooled device buffer of `bytes` (none for 0), released by the scaffold; ENOMEM with last_error when none is left
+  template <class T>
+  int buffer(size_t bytes, T **p) {
+    *p = bytes ? (T *)pool_acquire(ctx_, bytes) : nullptr;
+    if (*p) bufs_.push_back(*p);
+    return *p || !bytes ? 0 : WORLD_B200_ENOMEM;
+  }
+
+  void h2d(void *dst, const void *src, size_t bytes) {
+#ifndef WB_EMU
+    cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s_in_);
+#else
+    memcpy(dst, src, bytes);
+#endif
+  }
+  void d2h(void *dst, const void *src, size_t bytes) {
+#ifndef WB_EMU
+    cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s_out_);
+#else
+    memcpy(dst, src, bytes);
+#endif
+  }
+  void record(int ev, Stream s) {
+#ifndef WB_EMU
+    cudaEventRecord(ev_[ev], stream(s));
+#else
+    (void)ev; (void)s;
+#endif
+  }
+  void wait(Stream s, int ev) {
+#ifndef WB_EMU
+    cudaStreamWaitEvent(stream(s), ev_[ev], 0);
+#else
+    (void)s; (void)ev;
+#endif
+  }
+  // WB_HOST_TRACE=1: timeline of this call on stderr (timing events on the three streams + host clock)
+  void mark(const char *what, int idx, Stream s) {
+#ifndef WB_EMU
+    if (!trace_) return;
+    cudaEvent_t e;
+    cudaEventCreate(&e);
+    cudaEventRecord(e, stream(s));
+    marks_.push_back(Mark{what, idx, ms(), e});
+#else
+    (void)what; (void)idx; (void)s;
+#endif
+  }
+
+  // Waits for the three streams, turns a sticky error into "<who> pipeline: ...", prints the trace (its first line is
+  // "[wb trace] <header>: all work issued at ...") and releases the streams, events and buffers.
+  int finish(int rc, const char *header) {
+    const double issued_ms = ms();
+#ifndef WB_EMU
+    // copies and memsets above are not checked one by one: a failure is sticky and surfaces here
+    cudaError_t e = cudaStreamSynchronize(s_in_);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx_->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s_out_);
+    synced_ = true;
+    if (e != cudaSuccess && !rc) {
+      ctx_->last_error = std::string(who_) + " pipeline: " + cudaGetErrorString(e);
+      rc = WORLD_B200_ECUDA;
+    }
+#endif
+    if (trace_) {
+      fprintf(stderr, "[wb trace] %s: all work issued at %.1f ms, finished at %.1f ms (host clock)\n", header, issued_ms,
+              ms());
+#ifndef WB_EMU
+      for (size_t i = 1; i < marks_.size(); ++i) {
+        float gpu_ms = 0.f;
+        cudaEventElapsedTime(&gpu_ms, marks_[0].ev, marks_[i].ev);
+        fprintf(stderr, "[wb trace] %-9s %3d  issued %8.1f  gpu %8.1f\n", marks_[i].what, marks_[i].idx, marks_[i].host_ms,
+                gpu_ms);
+      }
+#endif
+    }
+    close();
+#ifndef WB_EMU
+    if (!rc) {
+      const cudaError_t last = cudaGetLastError();
+      if (last != cudaSuccess) { ctx_->last_error = cudaGetErrorString(last); rc = WORLD_B200_ECUDA; }
+    }
+#endif
+    return rc;
+  }
+
+ private:
+  double ms() const {
+    return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0_).count();
+  }
+#ifndef WB_EMU
+  struct Mark { const char *what; int idx; double host_ms; cudaEvent_t ev; };
+  cudaStream_t stream(Stream s) const { return s == IN ? s_in_ : s == OUT ? s_out_ : ctx_->stream; }
+  int fail(const char *what) {
+    ctx_->last_error = what;
+    cudaGetLastError();
+    return WORLD_B200_ECUDA;
+  }
+#endif
+  void close() {
+#ifndef WB_EMU
+    if (!synced_) {
+      if (s_in_) cudaStreamSynchronize(s_in_);
+      cudaStreamSynchronize(ctx_->stream);
+      if (s_out_) cudaStreamSynchronize(s_out_);
+      synced_ = true;
+    }
+    for (auto &m : marks_) cudaEventDestroy(m.ev);
+    for (cudaEvent_t e : ev_) cudaEventDestroy(e);
+    if (s_in_) cudaStreamDestroy(s_in_);
+    if (s_out_) cudaStreamDestroy(s_out_);
+    marks_.clear(); ev_.clear(); s_in_ = s_out_ = nullptr;
+#endif
+    for (void *p : bufs_) pool_release(ctx_, p);
+    bufs_.clear();
+  }
+
+  Ctx *ctx_;
+  const char *who_;
+  const bool trace_;
+  const std::chrono::steady_clock::time_point t0_;
+  std::vector<void *> bufs_;
+#ifndef WB_EMU
+  cudaStream_t s_in_ = nullptr, s_out_ = nullptr;
+  std::vector<cudaEvent_t> ev_;   // the pipeline's events, then the start event
+  std::vector<Mark> marks_;
+  bool synced_ = false;
+#endif
+};
 
 // One pipeline for both host entry points.  nbit == 0: x holds doubles; otherwise little-endian PCM that
 // is widened on the device (row f3).  dims == 0: the full spectrogram / aperiodicity rows go back to the
-// host; dims > 0: they stay on the device and only their coded rows (row f2) are downloaded.
+// host; dims > 0: they stay on the device and only their coded rows (row f2), written by the fused frame kernels
+// (world_b200_cheaptrick_coded_batch / world_b200_d4c_coded_batch), are downloaded.
 //
 // Two granularities.  The F0 stage runs on OUTER chunks (default 512 utterances): its per-utterance
 // kernels (contour tracking, smoothing, decimation) are latency bound -- one launch costs the same
-// for 96 or 500 utterances -- so few large launches beat many small ones.  CheapTrick / D4C (/ codec) run
+// for 96 or 500 utterances -- so few large launches beat many small ones.  CheapTrick / D4C run
 // on SUB-chunks (default 128 utterances) whose rows start their trip over PCIe as soon as they exist: the
 // un-overlapped tail is one sub-chunk.  Result buffers form a ring two outer chunks deep, so downloads
-// may lag behind the frame kernels and catch up under the next outer chunk's F0 stage.  Streams: s_in
-// (uploads), the context's stream (all kernels), s_out (downloads); events order buffer reuse.
+// may lag behind the frame kernels and catch up under the next outer chunk's F0 stage.  Streams and events: HostPipe.
 // harvest_options / dio_options: nullptr, or one option per utterance (checked by the caller, at most one of the two);
 // the outer chunks split the array.
 int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride, const int *x_lengths, int fs,
@@ -85,9 +237,6 @@ int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_st
       opt->f0_method == WORLD_B200_F0_HARVEST ? opt->harvest.frame_period : opt->dio.frame_period;
   const bool want_sp = out_sp != nullptr, want_ap = out_ap != nullptr && (!dims || n_ap > 0);
   if (n_utts == 0) return 0;
-  // coded mode: the frame kernels write the coded rows themselves (world_b200_cheaptrick_coded_batch /
-  // world_b200_d4c_coded_batch); WB_CODEC_UNFUSED=1 keeps round 1's full rows + codec kernels for A/B runs
-  const bool unfused = dims && getenv("WB_CODEC_UNFUSED") != nullptr;
 
   int sub = 128, outer = 512;
   if (const char *e = getenv("WB_HOST_SUB")) sub = atoi(e) > 0 ? atoi(e) : sub;
@@ -97,96 +246,36 @@ int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_st
   const size_t third = ctx->scratch_budget / 3;
   const size_t per_outer = (size_t)x_stride * (in_bytes + (nbit ? 8 : 0)) + (size_t)f0_stride * 16;
   const size_t per_sub_out = (size_t)f0_stride * ((want_sp ? sp_row : 0) + (want_ap ? ap_row : 0)) * 8;
-  const size_t per_sub_raw = (size_t)f0_stride * ((want_sp ? bins : 0) + (want_ap ? bins : 0)) * 8;
   outer = imin(outer, (int)dmax((double)sub, (double)(third / 3) / (double)(2 * per_outer)));
   outer = imax(sub, outer / sub * sub);
   outer = imin(outer, (n_utts + sub - 1) / sub * sub);
   const int subs_per_outer = outer / sub;
-  const double ring_budget = (double)third - (double)imin(n_utts, outer) * 2.0 * (double)per_outer -
-                             (unfused ? (double)sub * (double)per_sub_raw : 0.0);
+  const double ring_budget = (double)third - (double)imin(n_utts, outer) * 2.0 * (double)per_outer;
   int ring = 2 * subs_per_outer;
   if (per_sub_out > 0)
     ring = imax(2, imin(ring, (int)dmax(0.0, ring_budget / ((double)sub * (double)per_sub_out))));
   ring = imin(ring, (n_utts + sub - 1) / sub);
   if (ring < 1) ring = 1;
 
-#ifndef WB_EMU
-  cudaStream_t s_compute = ctx->stream, s_in = nullptr, s_out = nullptr;
-  if (cudaStreamCreateWithFlags(&s_in, cudaStreamNonBlocking) != cudaSuccess) {
-    ctx->last_error = "cudaStreamCreate failed";
-    cudaGetLastError();
-    return WORLD_B200_ECUDA;
-  }
-  if (cudaStreamCreateWithFlags(&s_out, cudaStreamNonBlocking) != cudaSuccess) {
-    ctx->last_error = "cudaStreamCreate failed";
-    cudaGetLastError();
-    cudaStreamDestroy(s_in);
-    return WORLD_B200_ECUDA;
-  }
-  cudaEvent_t ev_in[2], ev_cdone[2], ev_f0[2], ev_tf[2], ev_start;
-  bool ev_ok = cudaEventCreateWithFlags(&ev_start, cudaEventDisableTiming) == cudaSuccess;
-  for (int i = 0; i < 2; ++i) {
-    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_in[i], cudaEventDisableTiming) == cudaSuccess;
-    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_cdone[i], cudaEventDisableTiming) == cudaSuccess;
-    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_f0[i], cudaEventDisableTiming) == cudaSuccess;
-    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_tf[i], cudaEventDisableTiming) == cudaSuccess;
-  }
-  std::vector<cudaEvent_t> ev_sub_done(ring), ev_sub_out(ring);
-  for (int i = 0; i < ring; ++i) {
-    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_sub_done[i], cudaEventDisableTiming) == cudaSuccess;
-    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_sub_out[i], cudaEventDisableTiming) == cudaSuccess;
-  }
-  if (!ev_ok) {   // (events created so far are released with the process; this only happens when the driver is out of resources)
-    ctx->last_error = "cudaEventCreate failed";
-    cudaGetLastError();
-    cudaStreamDestroy(s_in);
-    cudaStreamDestroy(s_out);
-    return WORLD_B200_ECUDA;
-  }
-#endif
-  // WB_HOST_TRACE=1: timeline of this call on stderr (timing events on the three streams + host clock)
-  const bool trace = getenv("WB_HOST_TRACE") != nullptr;
-  struct Mark { const char *what; int idx; double host_ms; void *ev; };
-  std::vector<Mark> marks;
-  const auto t_host0 = std::chrono::steady_clock::now();
-  auto mark = [&](const char *what, int idx, void *stream) {
-    if (!trace) return;
-    Mark m{what, idx, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_host0).count(), nullptr};
-#ifndef WB_EMU
-    cudaEvent_t e;
-    cudaEventCreate(&e);
-    cudaEventRecord(e, (cudaStream_t)stream);
-    m.ev = e;
-#else
-    (void)stream;
-#endif
-    marks.push_back(m);
-  };
-#ifndef WB_EMU
-  mark("start", 0, s_compute);
-  // the uploads start after the work already on the context's stream: a pooled buffer released by a stream-ordered
-  // call (the PCM buffer of world_b200_analyze_coded_batch) may still be read there
-  cudaEventRecord(ev_start, s_compute);
-  cudaStreamWaitEvent(s_in, ev_start, 0);
-#endif
-  DevBuf din[2], dx[2], dt[2], df[2];
-  const int raw_slots = dims ? (unfused ? 1 : 0) : ring;   // unfused coded mode: the full rows are consumed on the same stream
-  std::vector<DevBuf> dsp(raw_slots), dap(raw_slots), dcs(dims ? ring : 0), dca(dims ? ring : 0);
-  int rc = 0;
+  // events: two of each per outer buffer set, then a "computed" and a "downloaded" event per result slot
+  enum { EV_IN = 0, EV_CDONE = 2, EV_F0 = 4, EV_TF = 6, EV_SUB_DONE = 8 };
+  const int ev_sub_out = EV_SUB_DONE + ring;
+  HostPipe p(h, "analyze");
+  int rc = p.open(EV_SUB_DONE + 2 * ring);
+  if (rc) return rc;
+  unsigned char *din[2] = {nullptr, nullptr};
+  double *dx[2] = {nullptr, nullptr}, *dt[2] = {nullptr, nullptr}, *df[2] = {nullptr, nullptr};
+  std::vector<double *> dsp(ring, nullptr), dap(ring, nullptr);   // the result ring: full or coded rows
   const int n_outer_bufs = n_utts > outer ? 2 : 1;
   for (int i = 0; i < n_outer_bufs && !rc; ++i) {
-    rc = ensure(ctx, &din[i], (size_t)outer * x_stride * in_bytes);
-    if (!rc && nbit) rc = ensure(ctx, &dx[i], (size_t)outer * x_stride * 8);
-    if (!rc) rc = ensure(ctx, &dt[i], (size_t)outer * f0_stride * 8);
-    if (!rc) rc = ensure(ctx, &df[i], (size_t)outer * f0_stride * 8);
+    rc = p.buffer((size_t)outer * x_stride * in_bytes, &din[i]);
+    if (!rc && nbit) rc = p.buffer((size_t)outer * x_stride * 8, &dx[i]);
+    if (!rc) rc = p.buffer((size_t)outer * f0_stride * 8, &dt[i]);
+    if (!rc) rc = p.buffer((size_t)outer * f0_stride * 8, &df[i]);
   }
-  for (int i = 0; i < raw_slots && !rc; ++i) {
-    if (want_sp) rc = ensure(ctx, &dsp[i], (size_t)sub * f0_stride * bins * 8);
-    if (!rc && want_ap) rc = ensure(ctx, &dap[i], (size_t)sub * f0_stride * bins * 8);
-  }
-  for (int i = 0; i < (dims ? ring : 0) && !rc; ++i) {
-    if (want_sp) rc = ensure(ctx, &dcs[i], (size_t)sub * f0_stride * sp_row * 8);
-    if (!rc && want_ap) rc = ensure(ctx, &dca[i], (size_t)sub * f0_stride * ap_row * 8);
+  for (int i = 0; i < ring && !rc; ++i) {
+    if (want_sp) rc = p.buffer((size_t)sub * f0_stride * sp_row * 8, &dsp[i]);
+    if (!rc && want_ap) rc = p.buffer((size_t)sub * f0_stride * ap_row * 8, &dap[i]);
   }
   std::vector<int> flen(n_utts);
   for (int i = 0; i < n_utts && !rc; ++i) {
@@ -200,157 +289,140 @@ int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_st
     const int *xl = x_lengths ? x_lengths + u0 : nullptr;
     const int *fl = flen.data() + u0;
     const size_t fsz = (size_t)n * f0_stride;
-    const unsigned char *src = (const unsigned char *)x + (size_t)u0 * x_stride * in_bytes;
-#ifndef WB_EMU
-    if (it >= 2) cudaStreamWaitEvent(s_in, ev_cdone[s], 0);   // kernels of outer chunk it-2 read din[s] / dx[s]
-    cudaMemcpyAsync(din[s].p, src, (size_t)n * x_stride * in_bytes, cudaMemcpyHostToDevice, s_in);
-    cudaEventRecord(ev_in[s], s_in);
-    mark("h2d_done", it, s_in);
-    cudaStreamWaitEvent(s_compute, ev_in[s], 0);
-    if (it >= 2) cudaStreamWaitEvent(s_compute, ev_tf[s], 0);  // time_axis / f0 of it-2 are on the host
-    mark("f0_begin", it, s_compute);
-#else
-    memcpy(din[s].p, src, (size_t)n * x_stride * in_bytes);
-#endif
-    if (nbit) rc = world_b200_pcm_to_double_batch(h, din[s].p, nbit, n, x_stride, xl, (double *)dx[s].p);
+    if (it >= 2) p.wait(HostPipe::IN, EV_CDONE + s);   // kernels of outer chunk it-2 read din[s] / dx[s]
+    p.h2d(din[s], (const unsigned char *)x + (size_t)u0 * x_stride * in_bytes, (size_t)n * x_stride * in_bytes);
+    p.record(EV_IN + s, HostPipe::IN);
+    p.mark("h2d_done", it, HostPipe::IN);
+    p.wait(HostPipe::RUN, EV_IN + s);
+    if (it >= 2) p.wait(HostPipe::RUN, EV_TF + s);   // time_axis / f0 of it-2 are on the host
+    p.mark("f0_begin", it, HostPipe::RUN);
+    if (nbit) rc = world_b200_pcm_to_double_batch(h, din[s], nbit, n, x_stride, xl, dx[s]);
     if (rc) break;
-    dev_memset(ctx, dt[s].p, 0, fsz * 8);
-    dev_memset(ctx, df[s].p, 0, fsz * 8);
-    const double *xd = (const double *)(nbit ? dx[s].p : din[s].p);
-    double *td = (double *)dt[s].p, *fd = (double *)df[s].p;
+    dev_memset(ctx, dt[s], 0, fsz * 8);
+    dev_memset(ctx, df[s], 0, fsz * 8);
+    const double *xd = nbit ? dx[s] : (const double *)din[s];
     rc = run_f0_stage(h, xd, n, x_stride, xl, fs, opt, harvest_options ? harvest_options + u0 : nullptr,
-                      dio_options ? dio_options + u0 : nullptr, fl, td, fd, f0_stride);
+                      dio_options ? dio_options + u0 : nullptr, fl, dt[s], df[s], f0_stride);
     if (rc) break;
-#ifndef WB_EMU
-    cudaEventRecord(ev_f0[s], s_compute);
-    mark("f0_end", it, s_compute);
-    cudaStreamWaitEvent(s_out, ev_f0[s], 0);
-    if (time_axis) cudaMemcpyAsync(time_axis + (size_t)u0 * f0_stride, td, fsz * 8, cudaMemcpyDeviceToHost, s_out);
-    if (f0) cudaMemcpyAsync(f0 + (size_t)u0 * f0_stride, fd, fsz * 8, cudaMemcpyDeviceToHost, s_out);
-    cudaEventRecord(ev_tf[s], s_out);
-#else
-    if (time_axis) memcpy(time_axis + (size_t)u0 * f0_stride, td, fsz * 8);
-    if (f0) memcpy(f0 + (size_t)u0 * f0_stride, fd, fsz * 8);
-#endif
+    p.record(EV_F0 + s, HostPipe::RUN);
+    p.mark("f0_end", it, HostPipe::RUN);
+    p.wait(HostPipe::OUT, EV_F0 + s);
+    if (time_axis) p.d2h(time_axis + (size_t)u0 * f0_stride, dt[s], fsz * 8);
+    if (f0) p.d2h(f0 + (size_t)u0 * f0_stride, df[s], fsz * 8);
+    p.record(EV_TF + s, HostPipe::OUT);
     // Sub-chunk size.  A sub-chunk's rows go to the host while the next one is computed, and in the full-row mode a
     // sub-chunk takes ~12 % longer to download than to compute: after the LAST outer chunk the copy engine is the
     // critical path, finishing (first sub-chunk's compute + every download) after the chunk's Harvest -- ~50 ms behind
     // the kernels of a 850 ms step at 1024 x 10 s with sub-chunks of 128.  Quarter-size sub-chunks there start the
-    // downloads earlier and leave a shorter last one (~25 ms behind).  WB_HOST_TAPER=0 disables it.
-    const bool taper = !dims && u0 + outer >= n_utts && !(getenv("WB_HOST_TAPER") && atoi(getenv("WB_HOST_TAPER")) == 0);
+    // downloads earlier and leave a shorter last one (~25 ms behind).
+    const bool taper = !dims && u0 + outer >= n_utts;
     int taper_min = 16;   // (WB_HOST_TAPER_MIN: tests exercise the path with a handful of utterances)
     if (const char *e = getenv("WB_HOST_TAPER_MIN")) taper_min = imax(1, atoi(e));
-    int taper_div = 4;
-    if (const char *e = getenv("WB_HOST_TAPER_DIV")) taper_div = imax(1, atoi(e));
-    const int sub_here = taper ? imax(imin(sub, taper_min), sub / taper_div) : sub;
+    const int sub_here = taper ? imax(imin(sub, taper_min), sub / 4) : sub;
     for (int v0 = 0; v0 < n && !rc && (want_sp || want_ap); v0 += sub_here, ++g) {
       const int m = imin(sub_here, n - v0);
-      const int slot = g % ring, rslot = dims ? 0 : slot;
+      const int slot = g % ring;
       const int *sxl = xl ? xl + v0 : nullptr;
       const int *sfl = fl + v0;
       const size_t ssz = (size_t)m * f0_stride;
-      const double *sx = xd + (size_t)v0 * x_stride, *st = td + (size_t)v0 * f0_stride, *sf = fd + (size_t)v0 * f0_stride;
-#ifndef WB_EMU
-      if (g >= ring) cudaStreamWaitEvent(s_compute, ev_sub_out[slot], 0);   // the slot's previous rows are on the host
-#endif
+      const double *sx = xd + (size_t)v0 * x_stride, *st = dt[s] + (size_t)v0 * f0_stride, *sf = df[s] + (size_t)v0 * f0_stride;
+      if (g >= ring) p.wait(HostPipe::RUN, ev_sub_out + slot);   // the slot's previous rows are on the host
       // whole padded rows are downloaded: frames beyond an utterance's length read as zero on the host
       bool ragged = false;
       for (int i = 0; i < m; ++i) ragged = ragged || sfl[i] != f0_stride;
       if (ragged) {
-        if (!dims && want_sp) dev_memset(ctx, dsp[rslot].p, 0, ssz * bins * 8);
-        if (!dims && want_ap) dev_memset(ctx, dap[rslot].p, 0, ssz * bins * 8);
-        if (dims && want_sp) dev_memset(ctx, dcs[slot].p, 0, ssz * sp_row * 8);
-        if (dims && want_ap) dev_memset(ctx, dca[slot].p, 0, ssz * ap_row * 8);
+        if (want_sp) dev_memset(ctx, dsp[slot], 0, ssz * sp_row * 8);
+        if (want_ap) dev_memset(ctx, dap[slot], 0, ssz * ap_row * 8);
       }
-      if (dims && !unfused) {
+      if (dims) {
         if (want_sp)
           rc = world_b200_cheaptrick_coded_batch(h, sx, m, x_stride, sxl, fs, st, sf, sfl, f0_stride, &opt->cheaptrick,
-                                                 dims, (double *)dcs[slot].p);
+                                                 dims, dsp[slot]);
         if (!rc && want_ap)
           rc = world_b200_d4c_coded_batch(h, sx, m, x_stride, sxl, fs, st, sf, sfl, f0_stride,
-                                          opt->cheaptrick.fft_size, &opt->d4c, (double *)dca[slot].p);
+                                          opt->cheaptrick.fft_size, &opt->d4c, dap[slot]);
       } else {
         if (want_sp)
           rc = world_b200_cheaptrick_batch(h, sx, m, x_stride, sxl, fs, st, sf, sfl, f0_stride, &opt->cheaptrick,
-                                           (double *)dsp[rslot].p);
+                                           dsp[slot]);
         if (!rc && want_ap)
           rc = world_b200_d4c_batch(h, sx, m, x_stride, sxl, fs, st, sf, sfl, f0_stride, opt->cheaptrick.fft_size,
-                                    &opt->d4c, (double *)dap[rslot].p);
-        if (!rc && dims && want_sp)
-          rc = world_b200_code_spectral_envelope_batch(h, (const double *)dsp[0].p, m, sfl, f0_stride, fs,
-                                                       opt->cheaptrick.fft_size, dims, (double *)dcs[slot].p);
-        if (!rc && dims && want_ap)
-          rc = world_b200_code_aperiodicity_batch(h, (const double *)dap[0].p, m, sfl, f0_stride, fs,
-                                                  opt->cheaptrick.fft_size, (double *)dca[slot].p);
+                                    &opt->d4c, dap[slot]);
       }
       if (rc) break;
-      const void *sp_src = dims ? dcs[slot].p : dsp[rslot].p, *ap_src = dims ? dca[slot].p : dap[rslot].p;
       const size_t row0 = (size_t)(u0 + v0) * f0_stride;
-#ifndef WB_EMU
-      cudaEventRecord(ev_sub_done[slot], s_compute);
-      mark("sub_end", g, s_compute);
-      cudaStreamWaitEvent(s_out, ev_sub_done[slot], 0);
-      if (want_sp) cudaMemcpyAsync(out_sp + row0 * sp_row, sp_src, ssz * sp_row * 8, cudaMemcpyDeviceToHost, s_out);
-      if (want_ap) cudaMemcpyAsync(out_ap + row0 * ap_row, ap_src, ssz * ap_row * 8, cudaMemcpyDeviceToHost, s_out);
-      cudaEventRecord(ev_sub_out[slot], s_out);
-      mark("d2h_end", g, s_out);
-#else
-      if (want_sp) memcpy(out_sp + row0 * sp_row, sp_src, ssz * sp_row * 8);
-      if (want_ap) memcpy(out_ap + row0 * ap_row, ap_src, ssz * ap_row * 8);
-#endif
+      p.record(EV_SUB_DONE + slot, HostPipe::RUN);
+      p.mark("sub_end", g, HostPipe::RUN);
+      p.wait(HostPipe::OUT, EV_SUB_DONE + slot);
+      if (want_sp) p.d2h(out_sp + row0 * sp_row, dsp[slot], ssz * sp_row * 8);
+      if (want_ap) p.d2h(out_ap + row0 * ap_row, dap[slot], ssz * ap_row * 8);
+      p.record(ev_sub_out + slot, HostPipe::OUT);
+      p.mark("d2h_end", g, HostPipe::OUT);
     }
-#ifndef WB_EMU
-    cudaEventRecord(ev_cdone[s], s_compute);
-#endif
+    p.record(EV_CDONE + s, HostPipe::RUN);
   }
-#ifndef WB_EMU
-  const double issued_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_host0).count();
-  // copies and memsets above are not checked one by one: a failure is sticky and surfaces here
-  cudaError_t e_sync = cudaStreamSynchronize(s_in);
-  if (e_sync == cudaSuccess) e_sync = cudaStreamSynchronize(s_compute);
-  if (e_sync == cudaSuccess) e_sync = cudaStreamSynchronize(s_out);
-  if (e_sync != cudaSuccess && !rc) { ctx->last_error = std::string("analyze pipeline: ") + cudaGetErrorString(e_sync); rc = WORLD_B200_ECUDA; }
-  if (trace && !marks.empty()) {
-    const double done_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_host0).count();
-    fprintf(stderr, "[wb trace] outer %d sub %d ring %d n %d: all work issued at %.1f ms, finished at %.1f ms (host clock)\n",
-            outer, sub, ring, n_utts, issued_ms, done_ms);
-    for (size_t i = 1; i < marks.size(); ++i) {
-      float gpu_ms = 0.f;
-      cudaEventElapsedTime(&gpu_ms, (cudaEvent_t)marks[0].ev, (cudaEvent_t)marks[i].ev);
-      fprintf(stderr, "[wb trace] %-9s %3d  issued %8.1f  gpu %8.1f\n", marks[i].what, marks[i].idx, marks[i].host_ms, gpu_ms);
-    }
-    for (auto &m : marks) cudaEventDestroy((cudaEvent_t)m.ev);
-  }
-  for (int i = 0; i < 2; ++i) {
-    cudaEventDestroy(ev_in[i]); cudaEventDestroy(ev_cdone[i]); cudaEventDestroy(ev_f0[i]); cudaEventDestroy(ev_tf[i]);
-  }
-  for (int i = 0; i < ring; ++i) { cudaEventDestroy(ev_sub_done[i]); cudaEventDestroy(ev_sub_out[i]); }
-  cudaEventDestroy(ev_start);
-  cudaStreamDestroy(s_in);
-  cudaStreamDestroy(s_out);
-  if (!rc) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { ctx->last_error = cudaGetErrorString(e); rc = WORLD_B200_ECUDA; }
-  }
-#endif
-  for (int i = 0; i < 2; ++i) { pool_release(ctx, din[i].p); pool_release(ctx, dx[i].p); pool_release(ctx, dt[i].p); pool_release(ctx, df[i].p); }
-  for (auto &b : dsp) pool_release(ctx, b.p);
-  for (auto &b : dap) pool_release(ctx, b.p);
-  for (auto &b : dcs) pool_release(ctx, b.p);
-  for (auto &b : dca) pool_release(ctx, b.p);
+  char header[96];
+  snprintf(header, sizeof header, "outer %d sub %d ring %d n %d", outer, sub, ring, n_utts);
+  rc = p.finish(rc, header);
   if (!rc) rc = world_b200_synchronize(h);
   return rc;
 }
 
-}  // namespace
+// The chunk loop of the synthesis and transform pipelines.  Utterance chunks of `chunk` are uploaded on s_in into one
+// of two input buffers of in_bytes, run on the context's stream into one of `ring` output slots (at most one per chunk)
+// and downloaded on s_out as whole rows of out_row bytes: a row past its utterance's y_len reads as zero on the host.
+// upload(p, u0, m, in) enqueues the copies of the chunk of utterances u0 .. u0 + m with p.h2d; run(u0, m, in, out) enqueues
+// its work.  Both runners synchronise the host with the device inside a run (pulse counts), so the upload of chunk
+// k + 1 is enqueued before chunk k runs: it then overlaps chunk k's kernels instead of following the host's wait.
+template <class Upload, class Run>
+int chunk_pipeline(WorldB200 *h, const char *who, int n_utts, int chunk, int ring, size_t in_bytes, size_t out_row,
+                   const int *y_len, int y_stride, int nbit, void *y, Upload upload, Run run) {
+  Ctx *ctx = ctx_of(h);
+  const int n_chunks = (n_utts + chunk - 1) / chunk;
+  ring = imin(ring, n_chunks);
+  enum { EV_IN = 0, EV_CDONE = 2, EV_OUT = 4 };   // two input buffers, then `ring` output slots
+  HostPipe p(h, who);
+  int rc = p.open(EV_OUT + ring);
+  if (rc) return rc;
+  unsigned char *din[2] = {nullptr, nullptr};
+  std::vector<unsigned char *> dout(ring, nullptr);
+  for (int i = 0; i < (n_chunks > 1 ? 2 : 1) && !rc; ++i) rc = p.buffer(in_bytes, &din[i]);
+  for (int i = 0; i < ring && !rc; ++i) rc = p.buffer((size_t)chunk * out_row, &dout[i]);
+  auto upload_chunk = [&](int k) {
+    if (k >= 2) p.wait(HostPipe::IN, EV_CDONE + (k & 1));   // the kernels of chunk k-2 have read din[k & 1]
+    upload(p, k * chunk, imin(chunk, n_utts - k * chunk), din[k & 1]);
+    p.record(EV_IN + (k & 1), HostPipe::IN);
+    p.mark("h2d_done", k, HostPipe::IN);
+  };
+  if (!rc) upload_chunk(0);
+  for (int k = 0; k < n_chunks && !rc; ++k) {
+    const int u0 = k * chunk, m = imin(chunk, n_utts - u0), s = k & 1, slot = k % ring;
+    if (k + 1 < n_chunks) upload_chunk(k + 1);
+    p.wait(HostPipe::RUN, EV_IN + s);
+    if (k >= ring) p.wait(HostPipe::RUN, EV_OUT + slot);   // the slot's previous chunk is on the host
+    p.mark("run_begin", k, HostPipe::RUN);
+    bool ragged = false;
+    for (int i = 0; i < m; ++i) ragged = ragged || y_len[u0 + i] != y_stride;
+    if (ragged) rc = dev_memset(ctx, dout[slot], 0, (size_t)m * out_row);
+    if (!rc) rc = run(u0, m, din[s], dout[slot]);
+    if (rc) break;
+    p.record(EV_CDONE + s, HostPipe::RUN);   // behind chunk k's last kernel
+    p.mark("run_end", k, HostPipe::RUN);
+    p.wait(HostPipe::OUT, EV_CDONE + s);
+    p.d2h((unsigned char *)y + (size_t)u0 * out_row, dout[slot], (size_t)m * out_row);
+    p.record(EV_OUT + slot, HostPipe::OUT);
+    p.mark("d2h_end", k, HostPipe::OUT);
+  }
+  char header[128];
+  snprintf(header, sizeof header, "%s chunk %d chunks %d ring %d n %d nbit %d", who, chunk, n_chunks, ring, n_utts,
+           nbit);
+  rc = p.finish(rc, header);
+  if (!rc) rc = world_b200_synchronize(h);
+  return rc;
+}
 
-namespace {
-
-// Synthesis from coded rows for host arrays: utterance chunks, uploads on s_in, synthesis_run on the context's stream,
-// downloads on s_out.  Inputs (f0 + coded rows) are double-buffered, outputs go through a ring of `ring` chunk slots;
-// events order the reuse of both.  synthesis_run synchronises the context's stream once per pass (its pulse counts),
-// so the upload of chunk k+1 is enqueued before synthesis_run is called for chunk k: it then runs under chunk k's
-// kernels instead of after the host has waited for them.  A chunk is one pass of synthesis_run: a longer chunk would
+// Synthesis from coded rows for host arrays: f0 + coded rows in, synthesis_run on each chunk, waveforms out, through
+// chunk_pipeline with an output ring of three chunks.  A chunk is one pass of synthesis_run: a longer chunk would
 // hold its download until all its passes were done, and a shorter one would pay the pass's fixed cost more often
 // (syn_timebase_kernel's sequential phase sum over each utterance takes about as long for a few utterances as for a
 // pass of hundreds; at 1024 x 10 s, 16 kHz, chunks of 128 utterances made the call slower than the serial path).  Two
@@ -367,174 +439,38 @@ int synthesis_pipeline(WorldB200 *h, CodedRows *coded, int lg, const double *f0,
   int max_y = 0;
   for (int i = 0; i < n_utts; ++i) max_y = imax(max_y, lens[n_utts + i]);
   const SynthesisSizing sz(ctx, coded, fft_size, f0_stride, y_stride, max_y, fs, mod);
-  int ring = 3;
+  const int ring = 3;
   const size_t third = ctx->scratch_budget / 3;
   int chunk = imax(1, sz.fit(sz.nominal_cap));
   chunk = imin(chunk, (int)dmax(1.0, (double)third / (double)(2 * per_in + ring * per_out)));
   chunk = balanced_chunk(n_utts, chunk);
-  const int n_chunks = (n_utts + chunk - 1) / chunk;
-  ring = imin(ring, n_chunks);
   ArenaPlan in_plan;
   const size_t o_f0 = in_plan.add((size_t)chunk * f0_stride * 8);
   const size_t o_sp = in_plan.add((size_t)chunk * f0_stride * dims * 8);
   const size_t o_ap = in_plan.add((size_t)chunk * f0_stride * n_ap * 8);
-
-#ifndef WB_EMU
-  cudaStream_t s_compute = ctx->stream, s_in = nullptr, s_out = nullptr;
-  if (cudaStreamCreateWithFlags(&s_in, cudaStreamNonBlocking) != cudaSuccess) {
-    ctx->last_error = "cudaStreamCreate failed";
-    cudaGetLastError();
-    return WORLD_B200_ECUDA;
-  }
-  if (cudaStreamCreateWithFlags(&s_out, cudaStreamNonBlocking) != cudaSuccess) {
-    ctx->last_error = "cudaStreamCreate failed";
-    cudaGetLastError();
-    cudaStreamDestroy(s_in);
-    return WORLD_B200_ECUDA;
-  }
-  cudaEvent_t ev_in[2], ev_cdone[2], ev_start;
-  std::vector<cudaEvent_t> ev_out(ring);
-  bool ev_ok = cudaEventCreateWithFlags(&ev_start, cudaEventDisableTiming) == cudaSuccess;
-  for (int i = 0; i < 2; ++i) {
-    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_in[i], cudaEventDisableTiming) == cudaSuccess;
-    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_cdone[i], cudaEventDisableTiming) == cudaSuccess;
-  }
-  for (int i = 0; i < ring; ++i)
-    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_out[i], cudaEventDisableTiming) == cudaSuccess;
-  if (!ev_ok) {   // (as in analyze_pipeline: events created so far are released with the process)
-    ctx->last_error = "cudaEventCreate failed";
-    cudaGetLastError();
-    cudaStreamDestroy(s_in);
-    cudaStreamDestroy(s_out);
-    return WORLD_B200_ECUDA;
-  }
-#endif
-  // WB_HOST_TRACE=1: timeline of this call on stderr (timing events on the three streams + host clock)
-  const bool trace = getenv("WB_HOST_TRACE") != nullptr;
-  struct Mark { const char *what; int idx; double host_ms; void *ev; };
-  std::vector<Mark> marks;
-  const auto t_host0 = std::chrono::steady_clock::now();
-  auto mark = [&](const char *what, int idx, void *stream) {
-    if (!trace) return;
-    Mark m{what, idx, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_host0).count(), nullptr};
-#ifndef WB_EMU
-    cudaEvent_t e;
-    cudaEventCreate(&e);
-    cudaEventRecord(e, (cudaStream_t)stream);
-    m.ev = e;
-#else
-    (void)stream;
-#endif
-    marks.push_back(m);
-  };
-#ifndef WB_EMU
-  mark("start", 0, s_compute);
-  // the uploads start after the work already on the context's stream: a pooled buffer released by a stream-ordered
-  // call may still be read there
-  cudaEventRecord(ev_start, s_compute);
-  cudaStreamWaitEvent(s_in, ev_start, 0);
-#endif
-  DevBuf din[2];
-  std::vector<DevBuf> dout(ring);
-  int rc = 0;
-  for (int i = 0; i < (n_chunks > 1 ? 2 : 1) && !rc; ++i) rc = ensure(ctx, &din[i], in_plan.total);
-  for (int i = 0; i < ring && !rc; ++i) rc = ensure(ctx, &dout[i], (size_t)chunk * per_out);
-
-  // chunk k's f0 and coded rows into din[k & 1]
-  auto upload = [&](int k) {
-    const int u0 = k * chunk, m = imin(chunk, n_utts - u0);
+  // chunk k's f0 and coded rows
+  auto upload = [&](HostPipe &p, int u0, int m, unsigned char *d) {
     const size_t frames = (size_t)m * f0_stride, row0 = (size_t)u0 * f0_stride;
-    unsigned char *d = (unsigned char *)din[k & 1].p;
-#ifndef WB_EMU
-    if (k >= 2) cudaStreamWaitEvent(s_in, ev_cdone[k & 1], 0);   // the kernels of chunk k-2 have read din[k & 1]
-    cudaMemcpyAsync(d + o_f0, f0 + row0, frames * 8, cudaMemcpyHostToDevice, s_in);
-    cudaMemcpyAsync(d + o_sp, h_sp + row0 * dims, frames * dims * 8, cudaMemcpyHostToDevice, s_in);
-    if (n_ap) cudaMemcpyAsync(d + o_ap, h_ap + row0 * n_ap, frames * n_ap * 8, cudaMemcpyHostToDevice, s_in);
-    cudaEventRecord(ev_in[k & 1], s_in);
-    mark("h2d_done", k, s_in);
-#else
-    memcpy(d + o_f0, f0 + row0, frames * 8);
-    memcpy(d + o_sp, h_sp + row0 * dims, frames * dims * 8);
-    if (n_ap) memcpy(d + o_ap, h_ap + row0 * n_ap, frames * n_ap * 8);
-#endif
+    p.h2d(d + o_f0, f0 + row0, frames * 8);
+    p.h2d(d + o_sp, h_sp + row0 * dims, frames * dims * 8);
+    if (n_ap) p.h2d(d + o_ap, h_ap + row0 * n_ap, frames * n_ap * 8);
   };
-  if (!rc) upload(0);
-  for (int k = 0; k < n_chunks && !rc; ++k) {
-    const int u0 = k * chunk, m = imin(chunk, n_utts - u0), s = k & 1, slot = k % ring;
-    if (k + 1 < n_chunks) upload(k + 1);
-    unsigned char *d = (unsigned char *)din[s].p;
-#ifndef WB_EMU
-    cudaStreamWaitEvent(s_compute, ev_in[s], 0);
-    if (k >= ring) cudaStreamWaitEvent(s_compute, ev_out[slot], 0);   // the slot's previous chunk is on the host
-    mark("syn_begin", k, s_compute);
-#endif
-    // whole padded rows are downloaded: samples beyond an utterance's length read as zero on the host
-    bool ragged = false;
-    for (int i = 0; i < m; ++i) ragged = ragged || lens[n_utts + u0 + i] != y_stride;
-    if (ragged) rc = dev_memset(ctx, dout[slot].p, 0, (size_t)m * per_out);
+  auto run = [&](int u0, int m, unsigned char *d, unsigned char *out) {
     coded->sp = (const double *)(d + o_sp);
     coded->ap = n_ap ? (const double *)(d + o_ap) : nullptr;
-    if (!rc)
-      rc = synthesis_run(ctx, (const double *)(d + o_f0), f0_lengths ? f0_lengths + u0 : nullptr, m, f0_stride, nullptr,
+    return synthesis_run(ctx, (const double *)(d + o_f0), f0_lengths ? f0_lengths + u0 : nullptr, m, f0_stride, nullptr,
                          nullptr, coded, fft_size, lg, frame_period, fs, y_lengths ? y_lengths + u0 : nullptr, y_stride,
-                         dout[slot].p, nbit, mod, u0);
-    if (rc) break;
-    unsigned char *dst = (unsigned char *)y + (size_t)u0 * per_out;
-#ifndef WB_EMU
-    cudaEventRecord(ev_cdone[s], s_compute);   // behind chunk k's overlap kernel
-    mark("syn_end", k, s_compute);
-    cudaStreamWaitEvent(s_out, ev_cdone[s], 0);
-    cudaMemcpyAsync(dst, dout[slot].p, (size_t)m * per_out, cudaMemcpyDeviceToHost, s_out);
-    cudaEventRecord(ev_out[slot], s_out);
-    mark("d2h_end", k, s_out);
-#else
-    memcpy(dst, dout[slot].p, (size_t)m * per_out);
-#endif
-  }
+                         out, nbit, mod, u0);
+  };
+  const int rc = chunk_pipeline(h, "synthesis", n_utts, chunk, ring, in_plan.total, per_out, lens + n_utts, y_stride,
+                                nbit, y, upload, run);
   coded->sp = h_sp;
   coded->ap = h_ap;
-  const double issued_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_host0).count();
-#ifndef WB_EMU
-  // copies and memsets above are not checked one by one: a failure is sticky and surfaces here
-  cudaError_t e_sync = cudaStreamSynchronize(s_in);
-  if (e_sync == cudaSuccess) e_sync = cudaStreamSynchronize(s_compute);
-  if (e_sync == cudaSuccess) e_sync = cudaStreamSynchronize(s_out);
-  if (e_sync != cudaSuccess && !rc) { ctx->last_error = std::string("synthesis pipeline: ") + cudaGetErrorString(e_sync); rc = WORLD_B200_ECUDA; }
-#endif
-  if (trace) {
-    const double done_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_host0).count();
-    fprintf(stderr, "[wb trace] synthesis chunk %d chunks %d ring %d n %d nbit %d: all work issued at %.1f ms, "
-            "finished at %.1f ms (host clock)\n", chunk, n_chunks, ring, n_utts, nbit, issued_ms, done_ms);
-#ifndef WB_EMU
-    for (size_t i = 1; i < marks.size(); ++i) {
-      float gpu_ms = 0.f;
-      cudaEventElapsedTime(&gpu_ms, (cudaEvent_t)marks[0].ev, (cudaEvent_t)marks[i].ev);
-      fprintf(stderr, "[wb trace] %-9s %3d  issued %8.1f  gpu %8.1f\n", marks[i].what, marks[i].idx, marks[i].host_ms, gpu_ms);
-    }
-    for (auto &m : marks) cudaEventDestroy((cudaEvent_t)m.ev);
-#endif
-  }
-#ifndef WB_EMU
-  for (int i = 0; i < 2; ++i) { cudaEventDestroy(ev_in[i]); cudaEventDestroy(ev_cdone[i]); }
-  for (int i = 0; i < ring; ++i) cudaEventDestroy(ev_out[i]);
-  cudaEventDestroy(ev_start);
-  cudaStreamDestroy(s_in);
-  cudaStreamDestroy(s_out);
-  if (!rc) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { ctx->last_error = cudaGetErrorString(e); rc = WORLD_B200_ECUDA; }
-  }
-#endif
-  for (int i = 0; i < 2; ++i) pool_release(ctx, din[i].p);
-  for (auto &b : dout) pool_release(ctx, b.p);
-  if (!rc) rc = world_b200_synchronize(h);
   return rc;
 }
 
-// Voice transformation for host arrays: utterance chunks of PCM are uploaded on s_in, transformed by transform_run
-// (which forks from and joins back to the context's stream) and their output rows downloaded on s_out.  Inputs and
-// outputs are double-buffered; events order their reuse.  transform_run synchronises the host with its lanes at each
-// synthesis pass, so the upload of chunk k+1 is enqueued before chunk k is transformed.  Chunks of WB_HOST_CHUNK
+// Voice transformation for host arrays: chunks of PCM in, transform_run on each chunk (which forks from and joins back
+// to the context's stream), output rows out, through chunk_pipeline with two output slots.  Chunks of WB_HOST_CHUNK
 // utterances (default 512), fewer when the four buffers would take more than a sixth of the scratch budget.
 int transform_pipeline(WorldB200 *h, const TransformPlan &tp, const void *x, int n_utts, const int *x_lengths,
                        const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
@@ -546,99 +482,15 @@ int transform_pipeline(WorldB200 *h, const TransformPlan &tp, const void *x, int
   if (const char *e = getenv("WB_HOST_CHUNK")) chunk = atoi(e) > 0 ? atoi(e) : chunk;
   chunk = imin(chunk, (int)dmax(1.0, (double)(ctx->scratch_budget / 6) / (double)(2 * (per_in + per_out))));
   chunk = balanced_chunk(n_utts, chunk);
-  const int n_chunks = (n_utts + chunk - 1) / chunk;
-#ifndef WB_EMU
-  cudaStream_t s_compute = ctx->stream, s_in = nullptr, s_out = nullptr;
-  if (cudaStreamCreateWithFlags(&s_in, cudaStreamNonBlocking) != cudaSuccess) {
-    ctx->last_error = "cudaStreamCreate failed";
-    cudaGetLastError();
-    return WORLD_B200_ECUDA;
-  }
-  if (cudaStreamCreateWithFlags(&s_out, cudaStreamNonBlocking) != cudaSuccess) {
-    ctx->last_error = "cudaStreamCreate failed";
-    cudaGetLastError();
-    cudaStreamDestroy(s_in);
-    return WORLD_B200_ECUDA;
-  }
-  cudaEvent_t ev_in[2], ev_cdone[2], ev_out[2], ev_start;
-  bool ev_ok = cudaEventCreateWithFlags(&ev_start, cudaEventDisableTiming) == cudaSuccess;
-  for (int i = 0; i < 2; ++i) {
-    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_in[i], cudaEventDisableTiming) == cudaSuccess;
-    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_cdone[i], cudaEventDisableTiming) == cudaSuccess;
-    ev_ok = ev_ok && cudaEventCreateWithFlags(&ev_out[i], cudaEventDisableTiming) == cudaSuccess;
-  }
-  if (!ev_ok) {   // (as in analyze_pipeline: events created so far are released with the process)
-    ctx->last_error = "cudaEventCreate failed";
-    cudaGetLastError();
-    cudaStreamDestroy(s_in);
-    cudaStreamDestroy(s_out);
-    return WORLD_B200_ECUDA;
-  }
-  // the uploads start after the work already on the context's stream: a pooled buffer released by a stream-ordered
-  // call may still be read there
-  cudaEventRecord(ev_start, s_compute);
-  cudaStreamWaitEvent(s_in, ev_start, 0);
-#endif
-  DevBuf din[2], dout[2];
-  int rc = 0;
-  for (int i = 0; i < (n_chunks > 1 ? 2 : 1) && !rc; ++i) {
-    rc = ensure(ctx, &din[i], (size_t)chunk * per_in);
-    if (!rc) rc = ensure(ctx, &dout[i], (size_t)chunk * per_out);
-  }
-  // chunk k's PCM rows into din[k & 1]
-  auto upload = [&](int k) {
-    const int u0 = k * chunk, m = imin(chunk, n_utts - u0);
-    const unsigned char *src = (const unsigned char *)x + (size_t)u0 * per_in;
-#ifndef WB_EMU
-    if (k >= 2) cudaStreamWaitEvent(s_in, ev_cdone[k & 1], 0);   // chunk k-2 has read din[k & 1]
-    cudaMemcpyAsync(din[k & 1].p, src, (size_t)m * per_in, cudaMemcpyHostToDevice, s_in);
-    cudaEventRecord(ev_in[k & 1], s_in);
-#else
-    memcpy(din[k & 1].p, src, (size_t)m * per_in);
-#endif
+  // chunk k's PCM rows
+  auto upload = [&](HostPipe &p, int u0, int m, unsigned char *d) {
+    p.h2d(d, (const unsigned char *)x + (size_t)u0 * per_in, (size_t)m * per_in);
   };
-  if (!rc) upload(0);
-  for (int k = 0; k < n_chunks && !rc; ++k) {
-    const int u0 = k * chunk, m = imin(chunk, n_utts - u0), s = k & 1;
-    if (k + 1 < n_chunks) upload(k + 1);
-#ifndef WB_EMU
-    cudaStreamWaitEvent(s_compute, ev_in[s], 0);
-    if (k >= 2) cudaStreamWaitEvent(s_compute, ev_out[s], 0);   // chunk k-2's rows are on the host
-#endif
-    // whole rows are downloaded: samples beyond an utterance's length read as zero on the host
-    bool ragged = false;
-    for (int i = 0; i < m; ++i) ragged = ragged || tp.y_len[u0 + i] != tp.y_stride;
-    if (ragged) rc = dev_memset(ctx, dout[s].p, 0, (size_t)m * per_out);
-    if (!rc) rc = transform_run(h, tp, din[s].p, x_lengths, opt, harvest_options, dio_options, u0, m, dout[s].p);
-    if (rc) break;
-    unsigned char *dst = (unsigned char *)y + (size_t)u0 * per_out;
-#ifndef WB_EMU
-    cudaEventRecord(ev_cdone[s], s_compute);
-    cudaStreamWaitEvent(s_out, ev_cdone[s], 0);
-    cudaMemcpyAsync(dst, dout[s].p, (size_t)m * per_out, cudaMemcpyDeviceToHost, s_out);
-    cudaEventRecord(ev_out[s], s_out);
-#else
-    memcpy(dst, dout[s].p, (size_t)m * per_out);
-#endif
-  }
-#ifndef WB_EMU
-  // copies and memsets above are not checked one by one: a failure is sticky and surfaces here
-  cudaError_t e_sync = cudaStreamSynchronize(s_in);
-  if (e_sync == cudaSuccess) e_sync = cudaStreamSynchronize(s_compute);
-  if (e_sync == cudaSuccess) e_sync = cudaStreamSynchronize(s_out);
-  if (e_sync != cudaSuccess && !rc) { ctx->last_error = std::string("transform pipeline: ") + cudaGetErrorString(e_sync); rc = WORLD_B200_ECUDA; }
-  for (int i = 0; i < 2; ++i) { cudaEventDestroy(ev_in[i]); cudaEventDestroy(ev_cdone[i]); cudaEventDestroy(ev_out[i]); }
-  cudaEventDestroy(ev_start);
-  cudaStreamDestroy(s_in);
-  cudaStreamDestroy(s_out);
-  if (!rc) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { ctx->last_error = cudaGetErrorString(e); rc = WORLD_B200_ECUDA; }
-  }
-#endif
-  for (int i = 0; i < 2; ++i) { pool_release(ctx, din[i].p); pool_release(ctx, dout[i].p); }
-  if (!rc) rc = world_b200_synchronize(h);
-  return rc;
+  auto run = [&](int u0, int m, unsigned char *d, unsigned char *out) {
+    return transform_run(h, tp, d, x_lengths, opt, harvest_options, dio_options, u0, m, out);
+  };
+  return chunk_pipeline(h, "transform", n_utts, chunk, 2, (size_t)chunk * per_in, per_out, tp.y_len.data(), tp.y_stride,
+                        tp.nbit_out, y, upload, run);
 }
 
 // world_b200_synthesis_coded_host and, with f0_scale / spectral_ratio, world_b200_synthesis_coded_host_modified
