@@ -285,6 +285,38 @@ int world_b200_d4c_coded_batch(WorldB200 *ctx, const double *x, int n_utts, int 
                                const double *f0, const int *f0_lengths, int f0_stride, int fft_size,
                                const D4COption *option, double *coded_aperiodicity);
 
+/* CheapTrick and D4C with one option per utterance, so each speaker of a batch gets the FFT size of its own F0 floor
+ * (CheapTrick analyses a frame at or below 3 fs / (fft_size - 3) as if it were at 500 Hz).  Derive the sizes as the
+ * reference does: options[u].f0_floor = floor[u]; options[u].fft_size = GetFFTSizeForCheapTrick(fs, &options[u]);
+ * f0_floor itself is not read.  options, fft_sizes: HOST arrays of n_utts; every other array as in the one-option
+ * calls.  Full rows: spectrogram / aperiodicity [n][f0_stride][row_stride] (DEVICE), row_stride >= the largest
+ * fft_sizes[u] / 2 + 1; utterance u writes the first fft_size_u / 2 + 1 values of each of its rows and leaves the rest
+ * of the row untouched.  Coded rows keep the one-option layout (number_of_dimensions, resp.
+ * GetNumberOfAperiodicities(fs), values per frame whatever the size), so a mixed batch lands in one array.
+ * Every row equals, bit for bit, what the one-option call gives that utterance with its own option; with equal
+ * options the call equals the one-option call.  CheapTrick runs one launch sequence per distinct option, D4C one for
+ * the batch.  Checked before any work is queued (EINVAL, world_b200_last_error() naming the first bad utterance,
+ * outputs untouched): CheapTrick fft_size a power of two in [16, 8192], D4C fft_size >= 4, q1 / threshold finite,
+ * row_stride, and number_of_dimensions in [1, fft_size / 4 + 1] for every utterance's size. */
+int world_b200_cheaptrick_batch_options(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
+                                        const int *x_lengths, int fs, const double *time_axis,
+                                        const double *f0, const int *f0_lengths, int f0_stride,
+                                        const CheapTrickOption *options, int row_stride, double *spectrogram);
+int world_b200_d4c_batch_options(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
+                                 const int *x_lengths, int fs, const double *time_axis,
+                                 const double *f0, const int *f0_lengths, int f0_stride, const int *fft_sizes,
+                                 const D4COption *options, int row_stride, double *aperiodicity);
+int world_b200_cheaptrick_coded_batch_options(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
+                                              const int *x_lengths, int fs, const double *time_axis,
+                                              const double *f0, const int *f0_lengths, int f0_stride,
+                                              const CheapTrickOption *options, int number_of_dimensions,
+                                              double *coded_spectral_envelope);
+int world_b200_d4c_coded_batch_options(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
+                                       const int *x_lengths, int fs, const double *time_axis,
+                                       const double *f0, const int *f0_lengths, int f0_stride,
+                                       const int *fft_sizes, const D4COption *options,
+                                       double *coded_aperiodicity);
+
 /* ---- ingest (tools/audioio.cpp:217-252) -- SURVEY.md 8 row f3 --------------------------- */
 /* Host-only: locates the sample data of a mono PCM RIFF/WAVE image held in memory, with the
  * acceptance rules of the reference's wavread (16-byte fmt chunk, format 1, one channel). */
@@ -448,6 +480,28 @@ int world_b200_analyze_coded_batch_dio_options(WorldB200 *ctx, const void *x, in
                                                const DioOption *dio_options, int number_of_dimensions,
                                                double *time_axis, double *f0, int f0_stride,
                                                double *coded_spectral_envelope, double *coded_aperiodicity);
+/* ... with per-utterance spectral options as well: cheaptrick_options and d4c_options are HOST arrays of n_utts (either
+ * may be NULL: option->cheaptrick / option->d4c for every utterance), harvest_options / dio_options as above (at most
+ * one, of the chain's F0 method, or both NULL).  CheapTrick runs at cheaptrick_options[u].fft_size and D4C at the same
+ * size, as in world_b200_cheaptrick_coded_batch_options / world_b200_d4c_coded_batch_options, whose rules are checked
+ * for every utterance before any work is queued (number_of_dimensions against every utterance's size).  Each row equals
+ * what world_b200_analyze_coded_batch gives that utterance with its own options, bit for bit. */
+int world_b200_analyze_coded_batch_spectral_options(WorldB200 *ctx, const void *x, int nbit, int n_utts, int x_stride,
+                                                    const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                                    const HarvestOption *harvest_options, const DioOption *dio_options,
+                                                    const CheapTrickOption *cheaptrick_options,
+                                                    const D4COption *d4c_options, int number_of_dimensions,
+                                                    double *time_axis, double *f0, int f0_stride,
+                                                    double *coded_spectral_envelope, double *coded_aperiodicity);
+/* The same for HOST arrays, on world_b200_analyze_coded_host's pipeline: each row equals
+ * world_b200_analyze_coded_batch_spectral_options's for the same utterance and options, bit for bit. */
+int world_b200_analyze_coded_host_spectral_options(WorldB200 *ctx, const void *x, int nbit, int n_utts, int x_stride,
+                                                   const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                                   const HarvestOption *harvest_options, const DioOption *dio_options,
+                                                   const CheapTrickOption *cheaptrick_options,
+                                                   const D4COption *d4c_options, int number_of_dimensions,
+                                                   double *time_axis, double *f0, int f0_stride,
+                                                   double *coded_spectral_envelope, double *coded_aperiodicity);
 /* world_b200_analyze_coded_batch on this rank's n_utts utterances with the outputs given as the FULL arrays of
  * n_ranks * n_utts utterances, gathered on every rank as world_b200_analyze_batch_allgather gathers the full rows:
  * the exchanged rows are the coded ones (f0_stride * number_of_dimensions and f0_stride * GetNumberOfAperiodicities(fs)

@@ -73,6 +73,17 @@ inline int download_frames(const DeviceArray &d, int n, int f_stride, int bins, 
   return 0;
 }
 
+// rows of `row` doubles on the device; utterance u's frames get widths[u] of them
+inline int download_frames(const DeviceArray &d, int n, int f_stride, int row, const std::vector<int> &widths,
+                           const int *f0_lengths, double **const *out) {
+  std::vector<double> h(static_cast<size_t>(n) * f_stride * row);
+  if (cudaMemcpy(h.data(), d.p, h.size() * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess) return WORLD_B200_ECUDA;
+  for (int u = 0; u < n; ++u)
+    for (int i = 0; i < f0_lengths[u]; ++i)
+      std::memcpy(out[u][i], h.data() + (static_cast<size_t>(u) * f_stride + i) * row, sizeof(double) * widths[u]);
+  return 0;
+}
+
 inline std::vector<int> frame_counts(const int *x_lengths, int n, int fs, double frame_period) {
   std::vector<int> fl(n);
   for (int i = 0; i < n; ++i) fl[i] = world_b200_frames(fs, x_lengths[i], frame_period);
@@ -213,6 +224,57 @@ inline int D4C(const double *const *xs, const int *x_lengths, int n_utts, int fs
   if (!rc) rc = world_b200_d4c_batch(w, dx.p, n_utts, xs_stride, x_lengths, fs, dt.p, df.p, f0_lengths, f_stride, fft_size, option, da.p);
   if (!rc) rc = world_b200_synchronize(w);
   if (!rc) rc = download_frames(da, n_utts, f_stride, bins, f0_lengths, aperiodicities);
+  return rc;
+}
+
+// One CheapTrick option per utterance (options.size() == n_utts), so each speaker gets the fft_size of its own F0
+// floor (world_b200_cheaptrick_batch_options): spectrograms[u][i] -> options[u].fft_size / 2 + 1 doubles.
+inline int CheapTrick(const double *const *xs, const int *x_lengths, int n_utts, int fs,
+                      const double *const *temporal_positions, const double *const *f0s, const int *f0_lengths,
+                      const std::vector<CheapTrickOption> &options, double **const *spectrograms) {
+  using namespace world_b200;
+  if (n_utts < 0 || options.size() != static_cast<size_t>(n_utts)) return WORLD_B200_EINVAL;
+  if (n_utts == 0) return 0;
+  WorldB200 *w = shared_context();
+  if (!w) return WORLD_B200_ECUDA;
+  std::vector<int> bins(n_utts);
+  for (int u = 0; u < n_utts; ++u) bins[u] = options[u].fft_size / 2 + 1;
+  const int xs_stride = max_of(x_lengths, n_utts), f_stride = max_of(f0_lengths, n_utts), row = max_of(bins.data(), n_utts);
+  DeviceArray dx(static_cast<size_t>(n_utts) * xs_stride), dt(static_cast<size_t>(n_utts) * f_stride), df(static_cast<size_t>(n_utts) * f_stride);
+  DeviceArray ds(static_cast<size_t>(n_utts) * f_stride * row);
+  int rc = upload(dx, pack(xs, x_lengths, n_utts, xs_stride));
+  if (!rc) rc = upload(dt, pack(temporal_positions, f0_lengths, n_utts, f_stride));
+  if (!rc) rc = upload(df, pack(f0s, f0_lengths, n_utts, f_stride));
+  if (!rc && !ds.p) rc = WORLD_B200_ENOMEM;
+  if (!rc) rc = world_b200_cheaptrick_batch_options(w, dx.p, n_utts, xs_stride, x_lengths, fs, dt.p, df.p, f0_lengths, f_stride, options.data(), row, ds.p);
+  if (!rc) rc = world_b200_synchronize(w);
+  if (!rc) rc = download_frames(ds, n_utts, f_stride, row, bins, f0_lengths, spectrograms);
+  return rc;
+}
+
+// One D4C fft_size and option per utterance (world_b200_d4c_batch_options): aperiodicities[u][i] -> fft_sizes[u] / 2 + 1
+// doubles.
+inline int D4C(const double *const *xs, const int *x_lengths, int n_utts, int fs,
+               const double *const *temporal_positions, const double *const *f0s, const int *f0_lengths,
+               const std::vector<int> &fft_sizes, const std::vector<D4COption> &options, double **const *aperiodicities) {
+  using namespace world_b200;
+  if (n_utts < 0 || fft_sizes.size() != static_cast<size_t>(n_utts) || options.size() != static_cast<size_t>(n_utts))
+    return WORLD_B200_EINVAL;
+  if (n_utts == 0) return 0;
+  WorldB200 *w = shared_context();
+  if (!w) return WORLD_B200_ECUDA;
+  std::vector<int> bins(n_utts);
+  for (int u = 0; u < n_utts; ++u) bins[u] = fft_sizes[u] / 2 + 1;
+  const int xs_stride = max_of(x_lengths, n_utts), f_stride = max_of(f0_lengths, n_utts), row = max_of(bins.data(), n_utts);
+  DeviceArray dx(static_cast<size_t>(n_utts) * xs_stride), dt(static_cast<size_t>(n_utts) * f_stride), df(static_cast<size_t>(n_utts) * f_stride);
+  DeviceArray da(static_cast<size_t>(n_utts) * f_stride * row);
+  int rc = upload(dx, pack(xs, x_lengths, n_utts, xs_stride));
+  if (!rc) rc = upload(dt, pack(temporal_positions, f0_lengths, n_utts, f_stride));
+  if (!rc) rc = upload(df, pack(f0s, f0_lengths, n_utts, f_stride));
+  if (!rc && !da.p) rc = WORLD_B200_ENOMEM;
+  if (!rc) rc = world_b200_d4c_batch_options(w, dx.p, n_utts, xs_stride, x_lengths, fs, dt.p, df.p, f0_lengths, f_stride, fft_sizes.data(), options.data(), row, da.p);
+  if (!rc) rc = world_b200_synchronize(w);
+  if (!rc) rc = download_frames(da, n_utts, f_stride, row, bins, f0_lengths, aperiodicities);
   return rc;
 }
 

@@ -82,6 +82,14 @@ ABI = {
                                                     C.POINTER(CheapTrickOption), C.c_int, _P]),
     "world_b200_d4c_coded_batch": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, _P, _P, _IP, C.c_int, C.c_int,
                                              C.POINTER(D4COption), _P]),
+    "world_b200_cheaptrick_batch_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, _P, _P, _IP, C.c_int,
+                                                      C.POINTER(CheapTrickOption), C.c_int, _P]),
+    "world_b200_d4c_batch_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, _P, _P, _IP, C.c_int, _IP,
+                                               C.POINTER(D4COption), C.c_int, _P]),
+    "world_b200_cheaptrick_coded_batch_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, _P, _P, _IP,
+                                                            C.c_int, C.POINTER(CheapTrickOption), C.c_int, _P]),
+    "world_b200_d4c_coded_batch_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, _P, _P, _IP, C.c_int,
+                                                     _IP, C.POINTER(D4COption), _P]),
     "world_b200_synthesis_batch": (C.c_int, [_P, _P, _IP, C.c_int, C.c_int, _P, _P, C.c_int, C.c_double, C.c_int, _IP,
                                              C.c_int, _P]),
     "world_b200_synthesis_coded_batch": (C.c_int, [_P, _P, _IP, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, C.c_double,
@@ -159,6 +167,16 @@ ABI = {
     "world_b200_analyze_coded_batch_dio_options": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int,
                                                              C.POINTER(AnalysisOption), C.POINTER(DioOption), C.c_int,
                                                              _P, _P, C.c_int, _P, _P]),
+    "world_b200_analyze_coded_host_spectral_options": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int,
+                                                                 C.POINTER(AnalysisOption), C.POINTER(HarvestOption),
+                                                                 C.POINTER(DioOption), C.POINTER(CheapTrickOption),
+                                                                 C.POINTER(D4COption), C.c_int, _P, _P, C.c_int, _P,
+                                                                 _P]),
+    "world_b200_analyze_coded_batch_spectral_options": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int,
+                                                                  C.POINTER(AnalysisOption), C.POINTER(HarvestOption),
+                                                                  C.POINTER(DioOption), C.POINTER(CheapTrickOption),
+                                                                  C.POINTER(D4COption), C.c_int, _P, _P, C.c_int, _P,
+                                                                  _P]),
     "world_b200_analyze_coded_batch_allgather": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int,
                                                            C.POINTER(AnalysisOption), C.c_int, _P, _P, C.c_int, _P,
                                                            _P]),
@@ -231,6 +249,17 @@ def _ptr(a):
     if hasattr(a, "data_ptr"):
         return a.data_ptr()
     return a.ctypes.data
+
+
+def _option_array(cls, options, n):
+    """A list of n options of ctypes type cls (one per utterance) as a ctypes array."""
+    options = list(options)
+    if len(options) != n:
+        raise ValueError(f"{len(options)} {cls.__name__} entries for {n} utterances")
+    arr = (cls * n)()
+    for i, o in enumerate(options):
+        C.memmove(C.byref(arr[i]), C.byref(o), C.sizeof(cls))
+    return arr
 
 
 def _harvest_options(options, n):
@@ -492,8 +521,22 @@ class World:
 
     def cheaptrick(self, x, fs, time_axis, f0, option: CheapTrickOption | None = None, x_lengths=None,
                    f0_lengths=None, out=None):
-        option = option or self.cheaptrick_option(fs)
+        """option: one CheapTrickOption for the batch, or a list of one per utterance (each speaker's fft_size from
+        its own F0 floor).  With a list the rows are [n, L, max fft_size / 2 + 1] (or out's last dimension): the
+        first fft_size / 2 + 1 values of utterance u's rows are written, the rest are left as they are."""
         n, stride = x.shape
+        if isinstance(option, (list, tuple)):
+            opts = _option_array(CheapTrickOption, option, n)
+            if out is None:
+                out = self._zeros(x, (n, f0.shape[1], max([o.fft_size for o in option] or [0]) // 2 + 1))
+            xl, k1 = _int_array(x_lengths, n)
+            fl, k2 = _int_array(f0_lengths, n)
+            self._use_current_stream()
+            self._check(self.lib.world_b200_cheaptrick_batch_options(
+                self._h, _ptr(x), n, stride, xl, fs, _ptr(time_axis), _ptr(f0), fl, f0.shape[1], opts, out.shape[-1],
+                _ptr(out)))
+            return out
+        option = option or self.cheaptrick_option(fs)
         bins = option.fft_size // 2 + 1
         if out is None:
             out = self._zeros(x, (n, f0.shape[1], bins))
@@ -506,8 +549,21 @@ class World:
 
     def d4c(self, x, fs, time_axis, f0, fft_size, option: D4COption | None = None, x_lengths=None,
             f0_lengths=None, out=None):
-        option = option or self.d4c_option()
+        """fft_size / option: one for the batch, or either as a list of one per utterance; then the rows are
+        [n, L, max fft_size / 2 + 1] (or out's last dimension) and utterance u writes fft_size[u] / 2 + 1 of each."""
         n, stride = x.shape
+        if isinstance(fft_size, (list, tuple)) or isinstance(option, (list, tuple)):
+            sizes, opts = self._d4c_options(fft_size, option, n)
+            if out is None:
+                out = self._zeros(x, (n, f0.shape[1], max(list(sizes) or [0]) // 2 + 1))
+            xl, k1 = _int_array(x_lengths, n)
+            fl, k2 = _int_array(f0_lengths, n)
+            self._use_current_stream()
+            self._check(self.lib.world_b200_d4c_batch_options(
+                self._h, _ptr(x), n, stride, xl, fs, _ptr(time_axis), _ptr(f0), fl, f0.shape[1], sizes, opts,
+                out.shape[-1], _ptr(out)))
+            return out
+        option = option or self.d4c_option()
         bins = fft_size // 2 + 1
         if out is None:
             out = self._zeros(x, (n, f0.shape[1], bins))
@@ -520,13 +576,19 @@ class World:
 
     def cheaptrick_coded(self, x, fs, time_axis, f0, number_of_dimensions, option: CheapTrickOption | None = None,
                          x_lengths=None, f0_lengths=None):
-        """CheapTrick + CodeSpectralEnvelope in one kernel per frame -> [n, L, number_of_dimensions]."""
-        option = option or self.cheaptrick_option(fs)
+        """CheapTrick + CodeSpectralEnvelope in one kernel per frame -> [n, L, number_of_dimensions].  option may be
+        a list of one CheapTrickOption per utterance (each coded at its own fft_size)."""
         n, stride = x.shape
         out = self._zeros(x, (n, f0.shape[1], number_of_dimensions))
         xl, k1 = _int_array(x_lengths, n)
         fl, k2 = _int_array(f0_lengths, n)
         self._use_current_stream()
+        if isinstance(option, (list, tuple)):
+            self._check(self.lib.world_b200_cheaptrick_coded_batch_options(
+                self._h, _ptr(x), n, stride, xl, fs, _ptr(time_axis), _ptr(f0), fl, f0.shape[1],
+                _option_array(CheapTrickOption, option, n), number_of_dimensions, _ptr(out)))
+            return out
+        option = option or self.cheaptrick_option(fs)
         self._check(self.lib.world_b200_cheaptrick_coded_batch(self._h, _ptr(x), n, stride, xl, fs, _ptr(time_axis),
                                                                _ptr(f0), fl, f0.shape[1], C.byref(option),
                                                                number_of_dimensions, _ptr(out)))
@@ -534,16 +596,31 @@ class World:
 
     def d4c_coded(self, x, fs, time_axis, f0, fft_size, option: D4COption | None = None, x_lengths=None,
                   f0_lengths=None):
-        """D4C + CodeAperiodicity in one kernel per frame -> [n, L, GetNumberOfAperiodicities(fs)]."""
-        option = option or self.d4c_option()
+        """D4C + CodeAperiodicity in one kernel per frame -> [n, L, GetNumberOfAperiodicities(fs)].  fft_size and
+        option may be lists of one per utterance."""
         n, stride = x.shape
         out = self._zeros(x, (n, f0.shape[1], max(1, self.number_of_aperiodicities(fs))))
         xl, k1 = _int_array(x_lengths, n)
         fl, k2 = _int_array(f0_lengths, n)
         self._use_current_stream()
+        if isinstance(fft_size, (list, tuple)) or isinstance(option, (list, tuple)):
+            sizes, opts = self._d4c_options(fft_size, option, n)
+            self._check(self.lib.world_b200_d4c_coded_batch_options(
+                self._h, _ptr(x), n, stride, xl, fs, _ptr(time_axis), _ptr(f0), fl, f0.shape[1], sizes, opts,
+                _ptr(out)))
+            return out
+        option = option or self.d4c_option()
         self._check(self.lib.world_b200_d4c_coded_batch(self._h, _ptr(x), n, stride, xl, fs, _ptr(time_axis), _ptr(f0),
                                                         fl, f0.shape[1], fft_size, C.byref(option), _ptr(out)))
         return out
+
+    def _d4c_options(self, fft_size, option, n):
+        """Per-utterance D4C arguments as ctypes arrays: a scalar fft_size or option applies to every utterance."""
+        sizes = list(fft_size) if isinstance(fft_size, (list, tuple)) else [int(fft_size)] * n
+        if len(sizes) != n:
+            raise ValueError(f"{len(sizes)} fft sizes for {n} utterances")
+        opts = option if isinstance(option, (list, tuple)) else [option or self.d4c_option()] * n
+        return (C.c_int * n)(*sizes), _option_array(D4COption, opts, n)
 
     def synthesis(self, f0, spectrogram, aperiodicity, fft_size, frame_period, fs, y_length, f0_lengths=None,
                   y_lengths=None):
@@ -825,10 +902,10 @@ class World:
 
     def analyze_coded_host(self, x_host, nbit, fs, option: AnalysisOption, number_of_dimensions, x_lengths=None,
                            time_axis=None, f0=None, coded_sp=None, coded_ap=None, f0_stride=None, harvest_options=None,
-                           dio_options=None):
+                           dio_options=None, cheaptrick_options=None, d4c_options=None):
         """Whole chain with device-side ingest (nbit 0 = float64 rows, 16 = int16 rows, ...) and codec;
         only the coded rows are downloaded.  harvest_options / dio_options: a list of one option per utterance of
-        the chain's F0 method (not both)."""
+        the chain's F0 method (not both).  cheaptrick_options / d4c_options: as for analyze_coded_batch."""
         import numpy as np
         n = x_host.shape[0]
         item = x_host.element_size() if hasattr(x_host, "element_size") else x_host.itemsize
@@ -849,7 +926,12 @@ class World:
         xl, keep = _int_array(x_lengths, n)
         per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
         outs = (number_of_dimensions, _ptr(time_axis), _ptr(f0), f0_stride, _ptr(coded_sp), _ptr(coded_ap))
-        if per_utt is not None:
+        if cheaptrick_options is not None or d4c_options is not None:
+            ct = None if cheaptrick_options is None else _option_array(CheapTrickOption, cheaptrick_options, n)
+            d4 = None if d4c_options is None else _option_array(D4COption, d4c_options, n)
+            self._check(self.lib.world_b200_analyze_coded_host_spectral_options(
+                self._h, _ptr(x_host), nbit, n, stride, xl, fs, C.byref(option), per_utt, per_dio, ct, d4, *outs))
+        elif per_utt is not None:
             self._check(self.lib.world_b200_analyze_coded_host_options(self._h, _ptr(x_host), nbit, n, stride, xl, fs,
                                                                        C.byref(option), per_utt, *outs))
         elif per_dio is not None:
@@ -874,13 +956,15 @@ class World:
 
     def analyze_coded_batch(self, x, nbit, fs, option: AnalysisOption, number_of_dimensions, x_lengths=None,
                             time_axis=None, f0=None, coded_sp=None, coded_ap=None, harvest_options=None,
-                            dio_options=None):
+                            dio_options=None, cheaptrick_options=None, d4c_options=None):
         """Whole chain on DEVICE arrays with coded rows out: analyze_batch's two internal streams, analyze_coded_host's
         formats.  x: float64 rows (nbit 0) or PCM rows (nbit 16: int16; 8/24/32: uint8 rows of nbit/8 bytes per
         sample); the PCM is converted slice by slice on the device.  Outputs are allocated on x's device when None
         and the work is enqueued on torch's current stream.  Returns (t, f0, coded_sp, coded_ap, frame counts) with
         coded_sp [n, L, number_of_dimensions] and coded_ap [n, L, max(1, GetNumberOfAperiodicities(fs))] (left zero
-        below 12 kHz).  harvest_options / dio_options: a list of one option per utterance of the chain's F0 method."""
+        below 12 kHz).  harvest_options / dio_options: a list of one option per utterance of the chain's F0 method.
+        cheaptrick_options / d4c_options: a list of one CheapTrickOption / D4COption per utterance (D4C runs at each
+        utterance's CheapTrick fft_size)."""
         n, stride, frame_period = self._coded_rows(x, nbit, option)
         lens = [stride] * n if x_lengths is None else [int(v) for v in x_lengths]
         fl = [self.frames(fs, v, frame_period) for v in lens]
@@ -897,7 +981,12 @@ class World:
         per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
         outs = (number_of_dimensions, _ptr(time_axis), _ptr(f0), time_axis.shape[1], _ptr(coded_sp), _ptr(coded_ap))
         self._use_current_stream()
-        if per_utt is not None:
+        if cheaptrick_options is not None or d4c_options is not None:
+            ct = None if cheaptrick_options is None else _option_array(CheapTrickOption, cheaptrick_options, n)
+            d4 = None if d4c_options is None else _option_array(D4COption, d4c_options, n)
+            self._check(self.lib.world_b200_analyze_coded_batch_spectral_options(
+                self._h, _ptr(x), nbit, n, stride, xl, fs, C.byref(option), per_utt, per_dio, ct, d4, *outs))
+        elif per_utt is not None:
             self._check(self.lib.world_b200_analyze_coded_batch_options(self._h, _ptr(x), nbit, n, stride, xl, fs,
                                                                         C.byref(option), per_utt, *outs))
         elif per_dio is not None:

@@ -573,6 +573,206 @@ int world_b200_d4c_coded_batch(WorldB200 *h, const double *x, int n, int x_strid
   return d4c_run(&h->c, b, fft_size, opt->threshold, nullptr, &t, coded_aperiodicity);
 }
 
+// ---- per-utterance CheapTrick / D4C options: every check runs before anything is queued and names the first bad
+// utterance
+static int utterance_fail(Ctx *c, int u, const std::string &what) {
+  c->last_error = what + " (utterance " + std::to_string(u) + ")";
+  return WORLD_B200_EINVAL;
+}
+
+// sizes[u] = options[u].fft_size, checked, and the q1 of each option
+static int check_cheaptrick_options(Ctx *c, const CheapTrickOption *o, int n, std::vector<int> *sizes) {
+  sizes->resize(n);
+  for (int u = 0; u < n; ++u) {
+    const int f = o[u].fft_size;
+    if (f < 16 || f > WB_TW_N || (f & (f - 1)))
+      return utterance_fail(c, u, "CheapTrick options: fft_size must be a power of two in [16, 8192]");
+    if (!std::isfinite(o[u].q1)) return utterance_fail(c, u, "CheapTrick options: q1 must be finite");
+    (*sizes)[u] = f;
+  }
+  return 0;
+}
+
+static int check_d4c_options(Ctx *c, const int *fft_sizes, const D4COption *o, int n) {
+  for (int u = 0; u < n; ++u) {
+    if (fft_sizes[u] < 4) return utterance_fail(c, u, "D4C options: fft_size must be at least 4");
+    if (!std::isfinite(o[u].threshold)) return utterance_fail(c, u, "D4C options: threshold must be finite");
+  }
+  return 0;
+}
+
+static int check_row_stride(Ctx *c, const std::vector<int> &sizes, int row_stride) {
+  for (size_t u = 0; u < sizes.size(); ++u)
+    if (row_stride < sizes[u] / 2 + 1)
+      return utterance_fail(c, (int)u, "row_stride is smaller than fft_size / 2 + 1");
+  return 0;
+}
+
+// index of each utterance's size in `distinct` (first appearance order)
+static std::vector<int> size_index(const std::vector<int> &sizes, std::vector<int> *distinct) {
+  std::vector<int> at(sizes.size());
+  for (size_t u = 0; u < sizes.size(); ++u) {
+    const auto it = std::find(distinct->begin(), distinct->end(), sizes[u]);
+    at[u] = (int)(it - distinct->begin());
+    if (it == distinct->end()) distinct->push_back(sizes[u]);
+  }
+  return at;
+}
+
+// CheapTrick over groups of equal options; coded: number_of_dimensions > 0
+static int cheaptrick_options_impl(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
+                                   const double *time_axis, const double *f0, const int *f0_lengths, int f0_stride,
+                                   const CheapTrickOption *opts, int row_stride, double *spectrogram,
+                                   int number_of_dimensions, double *coded) {
+  Ctx *c = &h->c;
+  std::vector<int> sizes, distinct;
+  int rc = check_cheaptrick_options(c, opts, n, &sizes);
+  if (rc || n == 0) return rc;
+  if (!coded && (rc = check_row_stride(c, sizes, row_stride))) return rc;
+  const std::vector<int> at = size_index(sizes, &distinct);
+  std::vector<CodecTables> tables(coded ? distinct.size() : 0);
+  for (size_t s = 0; s < tables.size(); ++s)
+    if ((rc = codec_sp_tables(c, fs, distinct[s], number_of_dimensions, &tables[s]))) {
+      const int u = (int)(std::find(sizes.begin(), sizes.end(), distinct[s]) - sizes.begin());
+      return utterance_fail(c, u, c->last_error);
+    }
+  // one group per distinct (fft_size, q1), in order of first appearance
+  std::vector<UttGroup> groups;
+  for (int u = 0; u < n; ++u) {
+    int g = 0;
+    while (g < (int)groups.size() && !(sizes[groups[g].uid[0]] == sizes[u] && opts[groups[g].uid[0]].q1 == opts[u].q1))
+      ++g;
+    if (g == (int)groups.size()) groups.emplace_back();
+    const int fl = f0_lengths ? f0_lengths[u] : f0_stride;
+    groups[g].uid.push_back(u);
+    groups[g].f_len.push_back(fl);
+    groups[g].max_f_len = std::max(groups[g].max_f_len, fl);
+  }
+  Batch b;
+  b.x = x; b.n = n; b.x_stride = x_stride; b.fs = fs; b.time_axis = time_axis; b.f0 = f0; b.f_stride = f0_stride;
+  if ((rc = upload_lengths(h, n, x_stride, x_lengths, f0_stride, f0_lengths, &b))) return rc;
+  for (size_t g = 0; g < groups.size() && !rc; ++g) {
+    const int u = groups[g].uid[0];
+    // a batch of one option runs exactly as the one-option call
+    const UttGroup *grp = groups.size() > 1 ? &groups[g] : nullptr;
+    rc = cheaptrick_run(c, b, opts[u].q1, sizes[u], coded ? nullptr : spectrogram, coded ? &tables[at[u]] : nullptr,
+                        coded, grp, row_stride);
+  }
+  return rc;
+}
+
+// D4C with per-utterance options in one launch sequence; coded: CodeAperiodicity rows
+static int d4c_options_impl(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
+                            const double *time_axis, const double *f0, const int *f0_lengths, int f0_stride,
+                            const int *fft_sizes, const D4COption *opts, int row_stride, double *aperiodicity,
+                            bool want_coded, double *coded) {
+  Ctx *c = &h->c;
+  int rc = check_d4c_options(c, fft_sizes, opts, n);
+  if (rc || n == 0) return rc;
+  D4cPerUtt pu;
+  pu.fft_size.assign(fft_sizes, fft_sizes + n);
+  if (!want_coded && (rc = check_row_stride(c, pu.fft_size, row_stride))) return rc;
+  std::vector<int> distinct;
+  if (want_coded) {
+    pu.table = size_index(pu.fft_size, &distinct);
+    pu.tables.resize(distinct.size());
+    for (size_t s = 0; s < distinct.size(); ++s)
+      if ((rc = codec_ap_tables(c, fs, distinct[s], &pu.tables[s]))) {
+        const int u = (int)(std::find(pu.fft_size.begin(), pu.fft_size.end(), distinct[s]) - pu.fft_size.begin());
+        return utterance_fail(c, u, c->last_error);
+      }
+    if (pu.tables[0].dims == 0) return 0;   // nothing to write below 12 kHz, as in world_b200_d4c_coded_batch
+    if (!coded) return WORLD_B200_EINVAL;
+  }
+  pu.threshold.resize(n);
+  for (int u = 0; u < n; ++u) pu.threshold[u] = opts[u].threshold;
+  pu.row_stride = row_stride;
+  Batch b;
+  b.x = x; b.n = n; b.x_stride = x_stride; b.fs = fs; b.time_axis = time_axis; b.f0 = f0; b.f_stride = f0_stride;
+  if ((rc = upload_lengths(h, n, x_stride, x_lengths, f0_stride, f0_lengths, &b))) return rc;
+  return d4c_run(c, b, pu.fft_size[0], pu.threshold[0], want_coded ? nullptr : aperiodicity,
+                 want_coded ? &pu.tables[0] : nullptr, coded, &pu);
+}
+
+}  // extern "C"
+
+namespace wb {
+// The spectral options of a coded chain (world_b200_analyze_coded_*_spectral_options) for every utterance, before any
+// work is queued: each utterance's CheapTrick option and D4C (fft_size = its CheapTrick size, option), the chain's
+// option standing in for an array that is NULL; then the stage calls' rules and the codec tables of every distinct size
+// (number_of_dimensions against each CheapTrick size).
+int chain_spectral_options(Ctx *c, int fs, int dims, const WorldB200AnalysisOption *opt,
+                           const CheapTrickOption *ct_options, const D4COption *d4c_options, int n,
+                           bool spectral_envelope, bool aperiodicity, std::vector<CheapTrickOption> *cts,
+                           std::vector<int> *d4_fft, std::vector<D4COption> *d4s) {
+  cts->assign(n, opt->cheaptrick);
+  d4s->assign(n, opt->d4c);
+  if (ct_options) std::copy(ct_options, ct_options + n, cts->begin());
+  if (d4c_options) std::copy(d4c_options, d4c_options + n, d4s->begin());
+  d4_fft->resize(n);
+  for (int u = 0; u < n; ++u) (*d4_fft)[u] = (*cts)[u].fft_size;
+  std::vector<int> sizes, distinct;
+  int rc = check_cheaptrick_options(c, cts->data(), n, &sizes);
+  if (!rc) rc = check_d4c_options(c, d4_fft->data(), d4s->data(), n);
+  if (rc) return rc;
+  size_index(sizes, &distinct);
+  for (const int fft : distinct) {
+    CodecTables t;
+    rc = spectral_envelope ? codec_sp_tables(c, fs, fft, dims, &t) : 0;
+    if (!rc && aperiodicity) rc = codec_ap_tables(c, fs, fft, &t);
+    if (rc) return utterance_fail(c, (int)(std::find(sizes.begin(), sizes.end(), fft) - sizes.begin()), c->last_error);
+  }
+  return 0;
+}
+}  // namespace wb
+
+extern "C" {
+
+int world_b200_cheaptrick_batch_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
+                                        int fs, const double *time_axis, const double *f0, const int *f0_lengths,
+                                        int f0_stride, const CheapTrickOption *options, int row_stride,
+                                        double *spectrogram) {
+  if (!h || !x || !time_axis || !f0 || !spectrogram || n < 0 || fs <= 0 || (n > 0 && !options))
+    return WORLD_B200_EINVAL;
+  DeviceGuard guard_(&h->c);
+  return cheaptrick_options_impl(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, options,
+                                 row_stride, spectrogram, 0, nullptr);
+}
+
+int world_b200_cheaptrick_coded_batch_options(WorldB200 *h, const double *x, int n, int x_stride,
+                                              const int *x_lengths, int fs, const double *time_axis,
+                                              const double *f0, const int *f0_lengths, int f0_stride,
+                                              const CheapTrickOption *options, int number_of_dimensions,
+                                              double *coded_spectral_envelope) {
+  if (!h || !x || !time_axis || !f0 || !coded_spectral_envelope || n < 0 || fs <= 0 || (n > 0 && !options))
+    return WORLD_B200_EINVAL;
+  DeviceGuard guard_(&h->c);
+  return cheaptrick_options_impl(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, options,
+                                 0, nullptr, number_of_dimensions, coded_spectral_envelope);
+}
+
+int world_b200_d4c_batch_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
+                                 const double *time_axis, const double *f0, const int *f0_lengths, int f0_stride,
+                                 const int *fft_sizes, const D4COption *options, int row_stride,
+                                 double *aperiodicity) {
+  if (!h || !x || !time_axis || !f0 || !aperiodicity || n < 0 || fs <= 0 || (n > 0 && (!fft_sizes || !options)))
+    return WORLD_B200_EINVAL;
+  DeviceGuard guard_(&h->c);
+  return d4c_options_impl(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, fft_sizes, options,
+                          row_stride, aperiodicity, false, nullptr);
+}
+
+int world_b200_d4c_coded_batch_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
+                                       int fs, const double *time_axis, const double *f0, const int *f0_lengths,
+                                       int f0_stride, const int *fft_sizes, const D4COption *options,
+                                       double *coded_aperiodicity) {
+  if (!h || !x || !time_axis || !f0 || n < 0 || fs <= 0 || (n > 0 && (!fft_sizes || !options)))
+    return WORLD_B200_EINVAL;
+  DeviceGuard guard_(&h->c);
+  return d4c_options_impl(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, fft_sizes, options,
+                          0, nullptr, true, coded_aperiodicity);
+}
+
 int world_b200_stonemask_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
                                int fs, const double *time_axis, const double *f0, const int *f0_lengths,
                                int f0_stride, double *refined_f0) {
@@ -779,10 +979,13 @@ extern "C" {
 // nbit: 0 = x holds doubles; 8/16/24/32 = little-endian PCM, converted slice by slice on the lane that analyses it.
 // dims: 0 = spectrogram / aperiodicity receive the fft_size/2+1-bin rows; > 0 = they receive the coded rows
 // (number_of_dimensions / GetNumberOfAperiodicities(fs) values per frame) straight from the fused frame kernels.
+// ct_options / d4c_options (coded rows only): nullptr, or one CheapTrick / D4C option per utterance; D4C then runs at
+// each utterance's CheapTrick fft_size (checked up front by chain_spectral_options).
 static int analyze_batch_impl(WorldB200 *h, const void *x, int nbit, int n, int x_stride, const int *x_lengths, int fs,
                               const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
                               const DioOption *dio_options, int dims, double *time_axis, double *f0, int f0_stride,
-                              double *spectrogram, double *aperiodicity, bool gather) {
+                              double *spectrogram, double *aperiodicity, bool gather,
+                              const CheapTrickOption *ct_options = nullptr, const D4COption *d4c_options = nullptr) {
   if (!h || !x || !opt || !time_axis || !f0 || n < 0 || fs <= 0 || x_stride <= 0 || f0_stride <= 0) return WORLD_B200_EINVAL;
   if ((spectrogram || aperiodicity) && opt->cheaptrick.fft_size < 16) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
@@ -797,13 +1000,25 @@ static int analyze_batch_impl(WorldB200 *h, const void *x, int nbit, int n, int 
   }
   const int bins = opt->cheaptrick.fft_size / 2 + 1;
   const int n_ap = dims ? GetNumberOfAperiodicities(fs) : 0;
-  if (dims) {
+  const bool spectral_options = ct_options || d4c_options;
+  if (dims && !spectral_options) {
     // the codec tables of every slice, built once here so that a bad dimension count or fft_size queues nothing
     CodecTables t;
     int rc = spectrogram ? codec_sp_tables(&h->c, fs, opt->cheaptrick.fft_size, dims, &t) : 0;
     if (!rc && aperiodicity) rc = codec_ap_tables(&h->c, fs, opt->cheaptrick.fft_size, &t);
     if (rc) return rc;
     if (n_ap == 0) aperiodicity = nullptr;   // no bands below 12 kHz: nothing to write, D4C is skipped
+  }
+  // per-utterance spectral options: every utterance's CheapTrick option and D4C (fft_size, option), the per-call
+  // option standing in for an array that is not given
+  std::vector<CheapTrickOption> cts;
+  std::vector<D4COption> d4s;
+  std::vector<int> d4_fft;
+  if (spectral_options) {
+    const int rc = chain_spectral_options(&h->c, fs, dims, opt, ct_options, d4c_options, n, spectrogram != nullptr,
+                                          aperiodicity != nullptr, &cts, &d4_fft, &d4s);
+    if (rc) return rc;
+    if (n_ap == 0) aperiodicity = nullptr;
   }
   const size_t sp_row = dims ? (size_t)dims : (size_t)bins, ap_row = dims ? (size_t)n_ap : (size_t)bins;
   if (n == 0) return 0;
@@ -883,11 +1098,17 @@ static int analyze_batch_impl(WorldB200 *h, const void *x, int nbit, int n, int 
                         dio_options ? dio_options + u0 : nullptr, fls, ts, fs_, f0_stride);
     double *sps = spectrogram ? spectrogram + (size_t)u0 * f0_stride * sp_row : nullptr;
     double *aps = aperiodicity ? aperiodicity + (size_t)u0 * f0_stride * ap_row : nullptr;
-    if (!rc && sps)
+    if (!rc && sps && spectral_options)
+      rc = world_b200_cheaptrick_coded_batch_options(L, xs, m, x_stride, xl, fs, ts, fs_, fls, f0_stride,
+                                                     cts.data() + u0, dims, sps);
+    else if (!rc && sps)
       rc = dims ? world_b200_cheaptrick_coded_batch(L, xs, m, x_stride, xl, fs, ts, fs_, fls, f0_stride, &opt->cheaptrick,
                                                     dims, sps)
                 : world_b200_cheaptrick_batch(L, xs, m, x_stride, xl, fs, ts, fs_, fls, f0_stride, &opt->cheaptrick, sps);
-    if (!rc && aps)
+    if (!rc && aps && spectral_options)
+      rc = world_b200_d4c_coded_batch_options(L, xs, m, x_stride, xl, fs, ts, fs_, fls, f0_stride, d4_fft.data() + u0,
+                                              d4s.data() + u0, aps);
+    else if (!rc && aps)
       rc = dims ? world_b200_d4c_coded_batch(L, xs, m, x_stride, xl, fs, ts, fs_, fls, f0_stride,
                                              opt->cheaptrick.fft_size, &opt->d4c, aps)
                 : world_b200_d4c_batch(L, xs, m, x_stride, xl, fs, ts, fs_, fls, f0_stride, opt->cheaptrick.fft_size,
@@ -1240,6 +1461,23 @@ int world_b200_analyze_coded_batch_dio_options(WorldB200 *h, const void *x, int 
   return analyze_coded_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, nullptr, dio_options,
                                   number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope,
                                   coded_aperiodicity, false);
+}
+
+int world_b200_analyze_coded_batch_spectral_options(WorldB200 *h, const void *x, int nbit, int n, int x_stride,
+                                                    const int *x_lengths, int fs, const WorldB200AnalysisOption *opt,
+                                                    const HarvestOption *harvest_options, const DioOption *dio_options,
+                                                    const CheapTrickOption *cheaptrick_options,
+                                                    const D4COption *d4c_options, int number_of_dimensions,
+                                                    double *time_axis, double *f0, int f0_stride,
+                                                    double *coded_spectral_envelope, double *coded_aperiodicity) {
+  if (!h || !opt || number_of_dimensions < 1) return WORLD_B200_EINVAL;
+  if (!cheaptrick_options && !d4c_options)   // the per-call CheapTrick option: analyze_coded_batch's rules
+    return analyze_coded_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, harvest_options, dio_options,
+                                    number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope,
+                                    coded_aperiodicity, false);
+  return analyze_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, harvest_options, dio_options,
+                            number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope, coded_aperiodicity,
+                            false, cheaptrick_options, d4c_options);
 }
 
 int world_b200_analyze_coded_batch_allgather(WorldB200 *h, const void *x, int nbit, int n, int x_stride,

@@ -22,7 +22,9 @@ struct CtParams {
   int fs, fft_size, lg_fft;
   double q1, f0_floor;
   const unsigned *draws; size_t draw_stride; const unsigned *draw_off;
-  double *out;            // [n][f_stride][fft/2+1]
+  double *out;            // [n][f_stride][out_stride]
+  int out_stride;         // doubles per spectrogram row (fft/2+1 unless the caller pads its rows)
+  const int *uid;         // [n] batch index of the launch's utterance blockIdx.y; null: blockIdx.y itself
   const double2 *tw;
   int *status;
   // coded tail (ct_coded_kernel): mel interpolation + DCT of the log envelope, CodeSpectralEnvelope (codec.cpp:279-295)
@@ -37,13 +39,14 @@ WB_DEV double ct_effective_f0(double f0, double f0_floor) {
 // draws consumed by frame = window samples + spectrum bins (SURVEY.md A1)
 WB_KERNEL_PLAIN ct_count_kernel(const double *__restrict__ f0, const int *__restrict__ f_len,
                                 int f_stride, int n_utts, int fs, int fft_size, double f0_floor,
-                                unsigned *__restrict__ counts) {
+                                const int *__restrict__ uid, unsigned *__restrict__ counts) {
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= (long long)n_utts * f_stride) return;
-  const int u = (int)(g / f_stride), i = (int)(g % f_stride);
+  const int ul = (int)(g / f_stride), i = (int)(g % f_stride);   // f_len and counts follow the launch's order
   unsigned c = 0;
-  if (i < f_len[u]) {
-    const double f = ct_effective_f0(f0[g], f0_floor);
+  if (i < f_len[ul]) {
+    const size_t fidx = uid ? (size_t)uid[ul] * f_stride + i : (size_t)g;
+    const double f = ct_effective_f0(f0[fidx], f0_floor);
     const int h = round_half_away(1.5 * fs / f);
     c = (unsigned)(2 * h + 1) + (unsigned)(fft_size / 2 + 1);
   }
@@ -61,8 +64,9 @@ template <bool kCoded>
 WB_DEV void ct_frame_body(const CtParams &p) {
   WB_DYN_SMEM(double2, smem2);
   const int tid = WB_TID, nth = WB_NTH;
-  const int u = blockIdx.y, i = blockIdx.x;
-  if (i >= p.f_len[u]) return;
+  const int ul = blockIdx.y, i = blockIdx.x;   // f_len, draws and draw offsets follow the launch's order
+  if (i >= p.f_len[ul]) return;
+  const int u = p.uid ? __ldg(p.uid + ul) : ul;
   const int N = p.fft_size, half = N / 2;
   const int slots = WB_FPAD_SLOTS(half);
   double2 *A = smem2, *B = smem2 + slots;
@@ -74,7 +78,7 @@ WB_DEV void ct_frame_body(const CtParams &p) {
   const int fs = p.fs;
   const int x_len = p.x_len[u];
   const double *x = p.x + (size_t)u * p.x_stride;
-  const unsigned *draw = p.draws + (size_t)u * p.draw_stride + p.draw_off[fidx];
+  const unsigned *draw = p.draws + (size_t)ul * p.draw_stride + p.draw_off[(size_t)ul * p.f_stride + i];
 
   const int h = round_half_away(1.5 * fs / f);
   const int nwin = 2 * h + 1;
@@ -180,7 +184,7 @@ WB_DEV void ct_frame_body(const CtParams &p) {
   WB_SYNC();
   double2 *z3 = sfft_forward(o2, z2, lgc, p.tw);
   if (!kCoded) {
-    double *row = p.out + fidx * (size_t)(half + 1);
+    double *row = p.out + fidx * (size_t)p.out_stride;
     rfft_unpack(z3, p.lg_fft, p.tw, [&](int k, double2 c) { row[k] = exp(c.x); });
     return;
   }
@@ -223,8 +227,10 @@ void ct_coded_kernel(CtParams p) { ct_frame_body<true>(p); }
 #endif
 
 int cheaptrick_run(Ctx *ctx, const Batch &b, double q1, int fft_size, double *spectrogram,
-                   const CodecTables *coded, double *coded_out) {
-  if (b.n <= 0 || b.max_f_len <= 0) return 0;
+                   const CodecTables *coded, double *coded_out, const UttGroup *group, int row_stride) {
+  const int n_all = group ? (int)group->uid.size() : b.n;
+  const int max_f_len = group ? group->max_f_len : b.max_f_len;
+  if (n_all <= 0 || max_f_len <= 0) return 0;
   int lg = 0;
   while ((1 << lg) < fft_size) ++lg;
   if ((1 << lg) != fft_size || fft_size < 16 || fft_size > WB_TW_N) {
@@ -235,42 +241,54 @@ int cheaptrick_run(Ctx *ctx, const Batch &b, double q1, int fft_size, double *sp
   const int bins = fft_size / 2 + 1;
   // a frame draws at most (fft_size - 2) + bins numbers (2h+1 <= fft_size - 2 above the floor)
   const size_t max_per_frame = (size_t)fft_size + bins;
-  const size_t draw_stride_full = max_per_frame * (size_t)b.max_f_len;
+  const size_t draw_stride_full = max_per_frame * (size_t)max_f_len;
   // utterances per chunk so that the draw scratch fits the budget
   const size_t per_utt_bytes = draw_stride_full * 4 + (size_t)b.f_stride * 8 + 64;
-  int chunk = balanced_chunk(imin(b.n, 65535), (int)dmin(65535.0, (double)ctx->scratch_budget / (double)per_utt_bytes));
+  int chunk = balanced_chunk(imin(n_all, 65535), (int)dmin(65535.0, (double)ctx->scratch_budget / (double)per_utt_bytes));
   const size_t smem = ct_smem_bytes(fft_size);
 #ifndef WB_EMU
   cudaFuncSetAttribute(ct_frame_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   cudaFuncSetAttribute(ct_coded_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 #endif
   const size_t n_tab = coded ? coded->idx.size() : 0, n_w = coded ? coded->weight.size() : 0;
-  for (int u0 = 0; u0 < b.n; u0 += chunk) {
-    const int n = imin(chunk, b.n - u0);
+  for (int u0 = 0; u0 < n_all; u0 += chunk) {
+    const int n = imin(chunk, n_all - u0);
     ArenaPlan plan;
     const size_t o_counts = plan.add((size_t)n * b.f_stride * 4);
     const size_t o_offs = plan.add((size_t)n * b.f_stride * 4);
     const size_t o_totals = plan.add((size_t)n * 4);
     const size_t o_draws = plan.add((size_t)n * draw_stride_full * 4);
     const size_t o_cidx = plan.add(n_tab * 4 + 4), o_cfrac = plan.add(n_tab * 8 + 8), o_cw = plan.add(n_w * 16 + 16);
+    const size_t o_group = plan.add(group ? (size_t)n * 8 : 0);
     unsigned char *blk = arena_block(ctx, plan.total);
     if (!blk) return 2;
     unsigned *counts = (unsigned *)(blk + o_counts), *offs = (unsigned *)(blk + o_offs);
     unsigned *totals = (unsigned *)(blk + o_totals), *draws = (unsigned *)(blk + o_draws);
-    const double *f0 = b.f0 + (size_t)u0 * b.f_stride;
-    const int *f_len = b.f_len + u0;
+    // a group keeps the batch's base pointers and reaches its utterances through uid; its frame counts are uploaded
+    // in the launch's order, which is the order counts, offsets and draws are laid out in
+    const size_t base = group ? 0 : (size_t)u0;
+    const int *uid = nullptr, *f_len = b.f_len + u0;
+    if (group) {
+      int *gd = (int *)(blk + o_group);
+      int rc = dev_memcpy_h2d(ctx, gd, group->uid.data() + u0, (size_t)n * 4);
+      if (!rc) rc = dev_memcpy_h2d(ctx, gd + n, group->f_len.data() + u0, (size_t)n * 4);
+      if (rc) return rc;
+      uid = gd; f_len = gd + n;
+    }
+    const double *f0 = b.f0 + base * b.f_stride;
     const long long total_slots = (long long)n * b.f_stride;
     WB_LAUNCH_FLAT(ct_count_kernel, dim3((unsigned)((total_slots + 255) / 256)), 256, 0, ctx->stream,
-                   f0, f_len, b.f_stride, n, b.fs, fft_size, f0_floor, counts);
+                   f0, f_len, b.f_stride, n, b.fs, fft_size, f0_floor, uid, counts);
     scan_counts(ctx, counts, f_len, b.f_stride, nullptr, offs, totals, n);
     rng_fill(ctx, totals, draws, draw_stride_full, draw_stride_full, n);
     CtParams p;
-    p.x = b.x + (size_t)u0 * b.x_stride; p.x_len = b.x_len + u0; p.x_stride = b.x_stride;
-    p.time_axis = b.time_axis + (size_t)u0 * b.f_stride; p.f0 = f0; p.f_len = f_len;
+    p.x = b.x + base * b.x_stride; p.x_len = b.x_len + base; p.x_stride = b.x_stride;
+    p.time_axis = b.time_axis + base * b.f_stride; p.f0 = f0; p.f_len = f_len; p.uid = uid;
     p.f_stride = b.f_stride; p.fs = b.fs; p.fft_size = fft_size; p.lg_fft = lg;
     p.q1 = q1; p.f0_floor = f0_floor;
     p.draws = draws; p.draw_stride = draw_stride_full; p.draw_off = offs;
-    p.out = spectrogram ? spectrogram + (size_t)u0 * b.f_stride * bins : nullptr;
+    p.out_stride = row_stride > 0 ? row_stride : bins;
+    p.out = spectrogram ? spectrogram + base * b.f_stride * p.out_stride : nullptr;
     p.tw = ctx->twiddle; p.status = ctx->status_dev;
     p.c_dims = 0; p.c_idx = nullptr; p.c_frac = nullptr; p.c_weight = nullptr; p.c_norm = 1.0; p.c_out = nullptr;
     int ct_threads = 128;
@@ -282,10 +300,10 @@ int cheaptrick_run(Ctx *ctx, const Batch &b, double q1, int fft_size, double *sp
       if (rc) return rc;
       p.c_dims = coded->dims; p.c_idx = (const int *)(blk + o_cidx); p.c_frac = (const double *)(blk + o_cfrac);
       p.c_weight = (const double2 *)(blk + o_cw); p.c_norm = coded->norm;
-      p.c_out = coded_out + (size_t)u0 * b.f_stride * coded->dims;
-      WB_LAUNCH_COOP(ct_coded_kernel, dim3((unsigned)b.max_f_len, (unsigned)n), ct_threads, smem, ctx->stream, p);
+      p.c_out = coded_out + base * b.f_stride * coded->dims;
+      WB_LAUNCH_COOP(ct_coded_kernel, dim3((unsigned)max_f_len, (unsigned)n), ct_threads, smem, ctx->stream, p);
     } else
-    WB_LAUNCH_COOP(ct_frame_kernel, dim3((unsigned)b.max_f_len, (unsigned)n), ct_threads, smem, ctx->stream, p);
+    WB_LAUNCH_COOP(ct_frame_kernel, dim3((unsigned)max_f_len, (unsigned)n), ct_threads, smem, ctx->stream, p);
     int rc = dev_check(ctx, "cheaptrick");
     if (rc) return rc;
   }

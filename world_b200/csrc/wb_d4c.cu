@@ -39,7 +39,15 @@ struct D4cParams {
   // coded output (CodeAperiodicity, codec.cpp:228-238): with c_out set the kernels write the dB value at the c_n
   // band centres instead of the ct_fft_size/2+1 bins
   int c_n; const int *c_idx; const double *c_frac; double *c_out;
+  int out_stride;           // doubles per aperiodicity row
+  // per-utterance options, [n] in the chunk's order (null: ct_fft_size / threshold / c_idx + 0 for every utterance):
+  // output width, threshold and the offset of the utterance's band-centre table in c_idx / c_frac
+  const int *u_fft; const double *u_thr; const int *u_ctab;
 };
+
+WB_DEV int d4c_ct_fft(const D4cParams &p, size_t fidx) {
+  return p.u_fft ? __ldg(p.u_fft + fidx / p.f_stride) : p.ct_fft_size;
+}
 
 WB_KERNEL_PLAIN d4c_count_a_kernel(const double *__restrict__ f0, const int *__restrict__ f_len,
                                    int f_stride, int n_utts, int fs, unsigned *__restrict__ counts) {
@@ -96,8 +104,8 @@ WB_DEV void d4c_fill_frame(const D4cParams &p, size_t fidx) {
     for (int b = WB_TID; b < p.c_n; b += WB_NTH) p.c_out[fidx * (size_t)p.c_n + b] = v;
     return;
   }
-  const int bins = p.ct_fft_size / 2 + 1;
-  double *row = p.out + fidx * (size_t)bins;
+  const int bins = d4c_ct_fft(p, fidx) / 2 + 1;
+  double *row = p.out + fidx * (size_t)p.out_stride;
   for (int k = WB_TID; k < bins; k += WB_NTH) row[k] = 1.0 - kTiny;
 }
 
@@ -122,19 +130,21 @@ WB_DEV double d4c_bin_db(const double *coarse, int n_ap, int fs, int ct_fft_size
 template <bool kFastExp>
 WB_DEV void d4c_write_frame(const D4cParams &p, size_t fidx, const double *coarse) {
   const int tid = WB_TID, nth = WB_NTH;
-  const int bins = p.ct_fft_size / 2 + 1;
+  const int ct_fft = d4c_ct_fft(p, fidx);
+  const int bins = ct_fft / 2 + 1;
   if (p.c_out) {
+    const int tab = p.u_ctab ? __ldg(p.u_ctab + fidx / p.f_stride) : 0;
     for (int b = tid; b < p.c_n; b += nth) {
-      const int k = __ldg(p.c_idx + b);
-      const double y0 = d4c_bin_db(coarse, p.n_ap, p.fs, p.ct_fft_size, k);
-      const double dy = (k + 1 < bins) ? d4c_bin_db(coarse, p.n_ap, p.fs, p.ct_fft_size, k + 1) - y0 : 0.0;
-      p.c_out[fidx * (size_t)p.c_n + b] = y0 + dy * __ldg(p.c_frac + b);
+      const int k = __ldg(p.c_idx + tab + b);
+      const double y0 = d4c_bin_db(coarse, p.n_ap, p.fs, ct_fft, k);
+      const double dy = (k + 1 < bins) ? d4c_bin_db(coarse, p.n_ap, p.fs, ct_fft, k + 1) - y0 : 0.0;
+      p.c_out[fidx * (size_t)p.c_n + b] = y0 + dy * __ldg(p.c_frac + tab + b);
     }
     return;
   }
-  double *row = p.out + fidx * (size_t)bins;
+  double *row = p.out + fidx * (size_t)p.out_stride;
   for (int k = tid; k < bins; k += nth) {
-    const double y = d4c_bin_db(coarse, p.n_ap, p.fs, p.ct_fft_size, k);
+    const double y = d4c_bin_db(coarse, p.n_ap, p.fs, ct_fft, k);
     row[k] = kFastExp ? exp(y * 0.11512925464970228420)   // 10^(y/20) = e^(y ln10 / 20)
                       : pow(10.0, y / 20.0);
   }
@@ -178,7 +188,7 @@ WB_KERNEL(128, 4) d4c_lovetrain_kernel(D4cParams p) {
   });
   block_sum2(s_lo, s_hi, red);
   const double ap0 = s_lo / s_hi;
-  const bool sel = ap0 > p.threshold;  // d4c.cpp:386
+  const bool sel = ap0 > (p.u_thr ? p.u_thr[u] : p.threshold);  // d4c.cpp:386
   if (!sel) d4c_fill_frame(p, fidx);
   if (tid == 0) {
     p.selected[fidx] = sel ? 1 : 0;
@@ -658,7 +668,7 @@ WB_KERNEL_PLAIN d4c_list_all_kernel(D4cParams p, int n_utts) {
 }
 
 int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *aperiodicity,
-            const CodecTables *coded, double *coded_out) {
+            const CodecTables *coded, double *coded_out, const D4cPerUtt *per_utt) {
   if (b.n <= 0 || b.max_f_len <= 0) return 0;
   if (coded && coded->dims == 0) return 0;   // below 12 kHz the coded row is empty (codec.cpp:216-219)
   const int fs = b.fs;
@@ -688,6 +698,18 @@ int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *ap
   p.b1 = static_cast<int>(ceil(4000.0 * p.lt_fft / fs));
   p.b2 = static_cast<int>(ceil(7900.0 * p.lt_fft / fs));
   const int bins = fft_size / 2 + 1;
+  p.out_stride = per_utt ? per_utt->row_stride : bins;
+  // per-utterance band-centre tables: one per distinct fft_size, concatenated
+  std::vector<int> ctab_idx;
+  std::vector<double> ctab_frac;
+  std::vector<int> ctab_off;
+  if (per_utt && coded) {
+    for (const CodecTables &t : per_utt->tables) {
+      ctab_off.push_back((int)ctab_idx.size());
+      ctab_idx.insert(ctab_idx.end(), t.idx.begin(), t.idx.end());
+      ctab_frac.insert(ctab_frac.end(), t.frac.begin(), t.frac.end());
+    }
+  }
 
   // Nuttall window of the band analysis (common.cpp:113-121), host libm like the reference
   double *nuttall_host = new double[p.win_len];
@@ -729,8 +751,9 @@ int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *ap
     const size_t o_sel = plan.add(slots), o_nut = plan.add((size_t)p.win_len * 8);
     const size_t o_slow = plan.add(slots * 4), o_nslow = plan.add(4);
     const size_t o_draws = plan.add((size_t)n * draw_stride_full * 4);
-    const size_t n_tab = coded ? coded->idx.size() : 0;
+    const size_t n_tab = coded ? (per_utt ? ctab_idx.size() : coded->idx.size()) : 0;
     const size_t o_cidx = plan.add(n_tab * 4 + 4), o_cfrac = plan.add(n_tab * 8 + 8);
+    const size_t o_uopt = plan.add(per_utt ? (size_t)n * 16 : 0);
     unsigned char *blk = arena_block(ctx, plan.total);
     if (!blk) { rc = 2; break; }
     unsigned *count_a = (unsigned *)(blk + o_ca), *off_a = (unsigned *)(blk + o_oa);
@@ -747,12 +770,25 @@ int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *ap
     p.f_stride = b.f_stride;
     p.nuttall = nuttall; p.draws = draws; p.draw_stride = draw_stride_full;
     p.off_a = off_a; p.count_b = count_b; p.off_b = off_b; p.selected = selected;
-    p.out = aperiodicity ? aperiodicity + (size_t)u0 * b.f_stride * bins : nullptr;
+    p.out = aperiodicity ? aperiodicity + (size_t)u0 * b.f_stride * p.out_stride : nullptr;
     p.tw = ctx->twiddle; p.status = ctx->status_dev;
     p.tw_body = ctx->twiddle_sized + tw_sized_offset(p.d_lg);
+    if (per_utt) {
+      std::vector<int> ui((size_t)2 * n);
+      for (int k = 0; k < n; ++k) {
+        ui[k] = per_utt->fft_size[u0 + k];
+        ui[n + k] = coded ? ctab_off[per_utt->table[u0 + k]] : 0;
+      }
+      unsigned char *d = blk + o_uopt;   // thresholds first: 8-byte aligned
+      rc = dev_memcpy_h2d(ctx, d, per_utt->threshold.data() + u0, (size_t)n * 8);
+      if (!rc) rc = dev_memcpy_h2d(ctx, d + (size_t)n * 8, ui.data(), (size_t)n * 8);
+      if (rc) break;
+      p.u_thr = (const double *)d; p.u_fft = (const int *)(d + (size_t)n * 8);
+      p.u_ctab = coded ? p.u_fft + n : nullptr;
+    }
     if (coded) {
-      rc = dev_memcpy_h2d(ctx, blk + o_cidx, coded->idx.data(), n_tab * 4);
-      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_cfrac, coded->frac.data(), n_tab * 8);
+      rc = dev_memcpy_h2d(ctx, blk + o_cidx, per_utt ? ctab_idx.data() : coded->idx.data(), n_tab * 4);
+      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_cfrac, per_utt ? ctab_frac.data() : coded->frac.data(), n_tab * 8);
       if (rc) break;
       p.c_n = coded->dims; p.c_idx = (const int *)(blk + o_cidx); p.c_frac = (const double *)(blk + o_cfrac);
       p.c_out = coded_out + (size_t)u0 * b.f_stride * coded->dims;

@@ -27,6 +27,11 @@ int check_chain_f0_options(Ctx *c, const WorldB200AnalysisOption *opt, const Har
 int run_f0_stage(WorldB200 *h, const double *x, int m, int x_stride, const int *x_lengths, int fs,
                  const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options, const DioOption *dio_options,
                  const int *f0_lengths, double *time_axis, double *f0, int f0_stride);
+// wb_api.cu: per-utterance spectral options of a coded chain, expanded to every utterance and checked
+int chain_spectral_options(Ctx *c, int fs, int dims, const WorldB200AnalysisOption *opt,
+                           const CheapTrickOption *ct_options, const D4COption *d4c_options, int n,
+                           bool spectral_envelope, bool aperiodicity, std::vector<CheapTrickOption> *cts,
+                           std::vector<int> *d4_fft, std::vector<D4COption> *d4s);
 // wb_api.cu: the checks and plan of a voice transformation, and its device driver over utterances [u0, u0 + n)
 int transform_check(WorldB200 *h, const void *x, int nbit, int n, int x_stride, const int *x_lengths, int fs,
                     const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
@@ -223,11 +228,13 @@ class HostPipe {
 // un-overlapped tail is one sub-chunk.  Result buffers form a ring two outer chunks deep, so downloads
 // may lag behind the frame kernels and catch up under the next outer chunk's F0 stage.  Streams and events: HostPipe.
 // harvest_options / dio_options: nullptr, or one option per utterance (checked by the caller, at most one of the two);
-// the outer chunks split the array.
+// the outer chunks split the array.  cts / d4_fft / d4s (coded rows only): nullptr, or every utterance's CheapTrick
+// option and D4C fft_size / option (chain_spectral_options).
 int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride, const int *x_lengths, int fs,
                      const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
                      const DioOption *dio_options, int dims, double *time_axis, double *f0, int f0_stride,
-                     double *out_sp, double *out_ap) {
+                     double *out_sp, double *out_ap, const CheapTrickOption *cts = nullptr,
+                     const int *d4_fft = nullptr, const D4COption *d4s = nullptr) {
   Ctx *ctx = ctx_of(h);
   const int bins = opt->cheaptrick.fft_size / 2 + 1;
   const int n_ap = GetNumberOfAperiodicities(fs);
@@ -334,7 +341,15 @@ int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_st
         if (want_sp) dev_memset(ctx, dsp[slot], 0, ssz * sp_row * 8);
         if (want_ap) dev_memset(ctx, dap[slot], 0, ssz * ap_row * 8);
       }
-      if (dims) {
+      if (dims && cts) {
+        const int w = u0 + v0;
+        if (want_sp)
+          rc = world_b200_cheaptrick_coded_batch_options(h, sx, m, x_stride, sxl, fs, st, sf, sfl, f0_stride, cts + w,
+                                                         dims, dsp[slot]);
+        if (!rc && want_ap)
+          rc = world_b200_d4c_coded_batch_options(h, sx, m, x_stride, sxl, fs, st, sf, sfl, f0_stride, d4_fft + w,
+                                                  d4s + w, dap[slot]);
+      } else if (dims) {
         if (want_sp)
           rc = world_b200_cheaptrick_coded_batch(h, sx, m, x_stride, sxl, fs, st, sf, sfl, f0_stride, &opt->cheaptrick,
                                                  dims, dsp[slot]);
@@ -627,6 +642,33 @@ static int analyze_coded_host_impl(WorldB200 *h, const void *x, int nbit, int n_
   if (rc) return rc;
   return analyze_pipeline(h, x, nbit, n_utts, x_stride, x_lengths, fs, opt, harvest_options, dio_options,
                           number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope, coded_aperiodicity);
+}
+
+// analyze_coded_host with per-utterance CheapTrick / D4C options (either array may be NULL) and F0 options as above
+extern "C" int world_b200_analyze_coded_host_spectral_options(
+    WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride, const int *x_lengths, int fs,
+    const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options, const DioOption *dio_options,
+    const CheapTrickOption *cheaptrick_options, const D4COption *d4c_options, int number_of_dimensions,
+    double *time_axis, double *f0, int f0_stride, double *coded_spectral_envelope, double *coded_aperiodicity) {
+  if (!cheaptrick_options && !d4c_options)
+    return analyze_coded_host_impl(h, x, nbit, n_utts, x_stride, x_lengths, fs, opt, harvest_options, dio_options,
+                                   number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope,
+                                   coded_aperiodicity);
+  if (!h || !x || !opt || n_utts < 0 || fs <= 0 || x_stride <= 0 || f0_stride <= 0 || number_of_dimensions < 1)
+    return WORLD_B200_EINVAL;
+  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));
+  if (nbit != 0 && nbit != 8 && nbit != 16 && nbit != 24 && nbit != 32) return WORLD_B200_EINVAL;
+  int rc = check_chain_f0_options(ctx_of(h), opt, harvest_options, dio_options, n_utts, fs, "analyze_coded_host");
+  std::vector<CheapTrickOption> cts;
+  std::vector<int> d4_fft;
+  std::vector<D4COption> d4s;
+  if (!rc)
+    rc = chain_spectral_options(ctx_of(h), fs, number_of_dimensions, opt, cheaptrick_options, d4c_options, n_utts,
+                                coded_spectral_envelope != nullptr, coded_aperiodicity != nullptr, &cts, &d4_fft, &d4s);
+  if (rc) return rc;
+  return analyze_pipeline(h, x, nbit, n_utts, x_stride, x_lengths, fs, opt, harvest_options, dio_options,
+                          number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope, coded_aperiodicity,
+                          cts.data(), d4_fft.data(), d4s.data());
 }
 
 extern "C" int world_b200_analyze_coded_host(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride,

@@ -236,10 +236,29 @@ struct TransformPlan {
   ModifyPlan mod;
 };
 
+// The utterances of a batch that share one CheapTrick option (world_b200_cheaptrick_*batch_options): their batch
+// indices, ascending, and their frame counts.  cheaptrick_run runs one launch sequence over them, reaching each row
+// through the batch's own pointers.
+struct UttGroup {
+  std::vector<int> uid, f_len;
+  int max_f_len = 0;
+};
+// row_stride: doubles per spectrogram row (0: fft_size / 2 + 1)
 int cheaptrick_run(Ctx *ctx, const Batch &b, double q1, int fft_size, double *spectrogram,
-                   const CodecTables *coded = nullptr, double *coded_out = nullptr);
+                   const CodecTables *coded = nullptr, double *coded_out = nullptr, const UttGroup *group = nullptr,
+                   int row_stride = 0);
+// Per-utterance D4C options (world_b200_d4c_*batch_options): D4C's own transforms depend on fs alone, so one launch
+// sequence serves the batch; each utterance's threshold, output width (fft_size / 2 + 1 bins) and, for coded rows,
+// band-centre table (codec_ap_tables at its fft_size) come from these host arrays of b.n entries.
+struct D4cPerUtt {
+  std::vector<int> fft_size;
+  std::vector<double> threshold;
+  std::vector<int> table;           // coded: index into tables
+  std::vector<CodecTables> tables;  // coded: one per distinct fft_size
+  int row_stride = 0;               // doubles per aperiodicity row
+};
 int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *aperiodicity,
-            const CodecTables *coded = nullptr, double *coded_out = nullptr);
+            const CodecTables *coded = nullptr, double *coded_out = nullptr, const D4cPerUtt *per_utt = nullptr);
 int stonemask_run(Ctx *ctx, const Batch &b, double *refined_f0);
 struct DioParams { double f0_floor, f0_ceil, channels_in_octave, frame_period, allowed_range; int speed; };
 // per_utt: opts[u] is utterance u's option (f0_floor / f0_ceil / channels_in_octave / allowed_range may differ,
