@@ -1,0 +1,164 @@
+"""Compares two builds of the library call by call: every analysis chain entry point and voice transformation on seeded
+ragged batches, with each call's return code, launch count and outputs required to be identical byte for byte.  Meant
+for a refactor of the chain drivers, with the parent commit's build as A and the change's as B (on the host emulation,
+two tests/emu builds; on a GPU, two libworld_b200.so with --device).
+
+    python tools/compare_chains.py A.so B.so [--device]
+
+Covers 8 and 16 kHz (16 kHz has one aperiodicity band, 8 kHz none), float64 and 16-bit PCM input, Harvest and DIO,
+no options, per-utterance F0 options, per-utterance CheapTrick / D4C options with two FFT sizes, NULL spectrogram /
+aperiodicity, transform with all three factors, and the host pipelines with small chunks (WB_HOST_CHUNK / WB_HOST_SUB).
+Prints the number of calls compared; exits 1 on the first difference."""
+import argparse
+import ctypes as C
+import os
+import sys
+
+import numpy as np
+
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
+from world_b200.api import F0_DIO_STONEMASK, F0_HARVEST, DioOption, HarvestOption, World, _ptr  # noqa: E402
+
+DIMS = 20
+
+
+def batch(fs, seed, n=5, seconds=0.3):
+    rng = np.random.default_rng(seed)
+    stride = int(fs * seconds)
+    lens = [int(stride * f) for f in rng.uniform(0.6, 1.0, n)]
+    lens[0] = stride
+    t = np.arange(stride) / fs
+    x = np.zeros((n, stride))
+    for u, m in enumerate(lens):
+        x[u, :m] = 0.4 * np.sin(2 * np.pi * rng.uniform(110, 260) * t[:m]) + 0.02 * rng.standard_normal(m)
+    pcm = np.clip(np.round(x * 32768), -32768, 32767).astype(np.int16)
+    return x, pcm, lens
+
+
+def f0_options(method, n):
+    if method == F0_HARVEST:
+        out = [HarvestOption() for _ in range(n)]
+        for u, o in enumerate(out):
+            o.f0_floor, o.f0_ceil, o.frame_period = 60.0 + 10 * u, 500.0 + 50 * u, 5.0
+        return out
+    out = [DioOption() for _ in range(n)]
+    for u, o in enumerate(out):
+        o.f0_floor, o.f0_ceil, o.channels_in_octave, o.allowed_range = 60.0 + 10 * u, 500.0 + 50 * u, 2.0, 0.1
+        o.frame_period, o.speed = 5.0, 1
+    return out
+
+
+def calls(w, device):
+    """(name, thunk) pairs; a thunk returns the outputs of one call on World w."""
+    def arr(a):
+        if not device:
+            return a
+        import torch
+        return torch.from_numpy(np.ascontiguousarray(a)).cuda()
+
+    out = []
+    for fs in (8000, 16000):
+        x, pcm, lens = batch(fs, fs)
+        n = len(lens)
+        for method in (F0_HARVEST, F0_DIO_STONEMASK):
+            ao = w.analysis_option(fs, method)
+            tag = f"fs {fs} {'harvest' if method == F0_HARVEST else 'dio'}"
+            small = ao.cheaptrick.fft_size
+            cts, d4s = [w.cheaptrick_option(fs) for _ in range(n)], [w.d4c_option() for _ in range(n)]
+            for u in range(0, n, 2):
+                cts[u].fft_size = 2 * small
+            for u, d in enumerate(d4s):
+                d.threshold = 0.8 + 0.02 * u
+            per_f0 = f0_options(method, n)
+            f0_kw = [{}, {"harvest_options" if method == F0_HARVEST else "dio_options": per_f0}]
+            for kw in f0_kw:
+                name = f"{tag} {'per-utt F0' if kw else 'no options'}"
+                out.append((f"analyze_batch {name}", lambda kw=kw, ao=ao, x=x, lens=lens, fs=fs:
+                            w.analyze_batch(arr(x), fs, ao, x_lengths=lens, **kw)[:4]))
+                out.append((f"analyze_host {name}", lambda kw=kw, ao=ao, x=x, lens=lens, fs=fs:
+                            w.analyze_host(x, fs, ao, x_lengths=lens, **kw)[:4]))
+                for nbit, xin in ((0, x), (16, pcm)):
+                    out.append((f"analyze_coded_batch nbit {nbit} {name}",
+                                lambda kw=kw, ao=ao, xin=xin, nbit=nbit, lens=lens, fs=fs:
+                                w.analyze_coded_batch(arr(xin), nbit, fs, ao, DIMS, x_lengths=lens, **kw)[:4]))
+                    out.append((f"analyze_coded_host nbit {nbit} {name}",
+                                lambda kw=kw, ao=ao, xin=xin, nbit=nbit, lens=lens, fs=fs:
+                                w.analyze_coded_host(xin, nbit, fs, ao, DIMS, x_lengths=lens, **kw)[:4]))
+                    spec = dict(kw, cheaptrick_options=cts, d4c_options=d4s)
+                    out.append((f"analyze_coded_batch nbit {nbit} {name} spectral options",
+                                lambda spec=spec, ao=ao, xin=xin, nbit=nbit, lens=lens, fs=fs:
+                                w.analyze_coded_batch(arr(xin), nbit, fs, ao, DIMS, x_lengths=lens, **spec)[:4]))
+                    out.append((f"analyze_coded_host nbit {nbit} {name} spectral options",
+                                lambda spec=spec, ao=ao, xin=xin, nbit=nbit, lens=lens, fs=fs:
+                                w.analyze_coded_host(xin, nbit, fs, ao, DIMS, x_lengths=lens, **spec)[:4]))
+                    ts = [1.0 + 0.1 * u for u in range(n)]
+                    factors = dict(kw, f0_scale=[1.2] * n, spectral_ratio=[0.9 + 0.05 * u for u in range(n)],
+                                   time_scale=ts)
+                    out.append((f"transform nbit {nbit} {name}", lambda f=factors, ao=ao, xin=xin, nbit=nbit,
+                                lens=lens, fs=fs: w.transform(arr(xin), nbit, fs, ao, x_lengths=lens, dtype="int16",
+                                                              **f)))
+                    out.append((f"transform_host nbit {nbit} {name}", lambda f=factors, ao=ao, xin=xin, nbit=nbit,
+                                lens=lens, fs=fs: w.transform_host(xin, nbit, fs, ao, x_lengths=lens, **f)))
+            # NULL spectrogram / aperiodicity: that stage is skipped
+            L = max(w.frames(fs, m) for m in lens)
+            for entry, host in (("analyze_coded_host", True), ("analyze_coded_batch", False)):
+                for which in ("sp", "ap"):
+                    def null_call(entry=entry, host=host, which=which, ao=ao, fs=fs, x=x, lens=lens, L=L):
+                        mk = (lambda a: a) if host else arr
+                        t, f0 = mk(np.zeros((n, L))), mk(np.zeros((n, L)))
+                        sp = None if which == "sp" else mk(np.zeros((n, L, DIMS)))
+                        ap = None if which == "ap" else mk(np.zeros((n, L, max(1, w.number_of_aperiodicities(fs)))))
+                        xin = x if host else arr(x)
+                        w._chain(entry, (_ptr(xin), 0, n, x.shape[1], (C.c_int * n)(*lens), fs, C.byref(ao)), n,
+                                 None, None, (DIMS, _ptr(t), _ptr(f0), L, _ptr(sp), _ptr(ap)), device=not host)
+                        return [a for a in (t, f0, sp, ap) if a is not None]
+                    out.append((f"{entry} NULL {which} {tag}", null_call))
+    return out
+
+
+def to_np(a):
+    if a is None:
+        return np.zeros(0)
+    if hasattr(a, "cpu"):
+        return a.cpu().numpy()
+    return np.asarray(a)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("lib_a")
+    ap.add_argument("lib_b")
+    ap.add_argument("--device", action="store_true", help="CUDA builds, device arrays as torch tensors")
+    args = ap.parse_args()
+    mod = None if args.device else "numpy"
+    worlds = [World(lib_path=p, array_module=mod or "torch") for p in (args.lib_a, args.lib_b)]
+    compared = 0
+    for chunks in ((None, None), ("2", "1")):
+        for k, v in zip(("WB_HOST_CHUNK", "WB_HOST_SUB"), chunks):
+            if v is None:
+                os.environ.pop(k, None)
+            else:
+                os.environ[k] = v
+        lists = [calls(w, args.device) for w in worlds]
+        for (name, fa), (_, fb) in zip(*lists):
+            res = []
+            for w, fn in zip(worlds, (fa, fb)):
+                before = w.launch_count()
+                try:
+                    outs, err = fn(), None
+                except Exception as e:   # both builds must fail the same way
+                    outs, err = (), str(e)
+                w.synchronize()
+                res.append((err, w.launch_count() - before, [to_np(o).tobytes() for o in outs]))
+            if res[0] != res[1]:
+                print(f"DIFFERENT: {name} (chunks {chunks}): errors {res[0][0]!r} / {res[1][0]!r}, launches "
+                      f"{res[0][1]} / {res[1][1]}, outputs equal: {res[0][2] == res[1][2]}")
+                sys.exit(1)
+            if res[0][0]:
+                print(f"note: both builds raised for {name}: {res[0][0]}")
+            compared += 1
+    print(f"{compared} calls compared, all identical (return codes, launch counts, output bytes)")
+
+
+if __name__ == "__main__":
+    main()

@@ -301,6 +301,11 @@ def _chain_options(harvest_options, dio_options, n):
     return _harvest_options(harvest_options, n), _dio_options(dio_options, n)
 
 
+def _frame_period(option):
+    """The frame period of an AnalysisOption's F0 method."""
+    return option.dio.frame_period if option.f0_method == F0_DIO_STONEMASK else option.harvest.frame_period
+
+
 def _pcm16(dtype):
     """True for an int16 dtype (torch.int16, numpy.int16 or "int16"), False for None / float64."""
     name = str(getattr(dtype, "__name__", dtype)).replace("torch.", "")
@@ -364,6 +369,27 @@ class World:
     def _check(self, rc):
         if rc != 0:
             raise WorldError(f"world_b200 error {rc}: {self.lib.world_b200_last_error(self._h).decode()}")
+
+    def _chain(self, family, head, n, harvest_options, dio_options, outs, cheaptrick_options=None, d4c_options=None,
+               device=False):
+        """Calls the analysis chain world_b200_<family> whose variant fits the per-utterance option lists given
+        (_options: Harvest, _dio_options: DIO, _spectral_options: CheapTrick / D4C, with either F0 list).  head: the
+        arguments between the handle and the option arrays; outs: those after them.  device: the chain is enqueued on
+        torch's current stream."""
+        per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
+        if cheaptrick_options is not None or d4c_options is not None:
+            ct = None if cheaptrick_options is None else _option_array(CheapTrickOption, cheaptrick_options, n)
+            d4 = None if d4c_options is None else _option_array(D4COption, d4c_options, n)
+            suffix, arrays = "_spectral_options", (per_utt, per_dio, ct, d4)
+        elif per_utt is not None:
+            suffix, arrays = "_options", (per_utt,)
+        elif per_dio is not None:
+            suffix, arrays = "_dio_options", (per_dio,)
+        else:
+            suffix, arrays = "", ()
+        if device:
+            self._use_current_stream()
+        self._check(getattr(self.lib, f"world_b200_{family}{suffix}")(self._h, *head, *arrays, *outs))
 
     def _use_current_stream(self):
         if self.xp == "torch":
@@ -733,7 +759,7 @@ class World:
         harvest_options: a list of one HarvestOption per utterance (Harvest with a per-utterance F0 range);
         dio_options: a list of one DioOption per utterance (DIO + StoneMask with a per-utterance F0 range)."""
         n, stride = x.shape
-        frame_period = option.dio.frame_period if option.f0_method == F0_DIO_STONEMASK else option.harvest.frame_period
+        frame_period = _frame_period(option)
         f_stride, fl = self._f0_stride(fs, x, x_lengths, frame_period)
         bins = option.cheaptrick.fft_size // 2 + 1
         if time_axis is None:
@@ -745,22 +771,8 @@ class World:
         if aperiodicity is None:
             aperiodicity = self._zeros(x, (n, f_stride, bins))
         xl, keep = _int_array(x_lengths, n)
-        per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
-        self._use_current_stream()
-        if per_utt is not None:
-            self._check(self.lib.world_b200_analyze_batch_options(self._h, _ptr(x), n, stride, xl, fs, C.byref(option),
-                                                                  per_utt, _ptr(time_axis), _ptr(f0),
-                                                                  time_axis.shape[1], _ptr(spectrogram),
-                                                                  _ptr(aperiodicity)))
-        elif per_dio is not None:
-            self._check(self.lib.world_b200_analyze_batch_dio_options(self._h, _ptr(x), n, stride, xl, fs,
-                                                                      C.byref(option), per_dio, _ptr(time_axis),
-                                                                      _ptr(f0), time_axis.shape[1], _ptr(spectrogram),
-                                                                      _ptr(aperiodicity)))
-        else:
-            self._check(self.lib.world_b200_analyze_batch(self._h, _ptr(x), n, stride, xl, fs, C.byref(option),
-                                                          _ptr(time_axis), _ptr(f0), time_axis.shape[1],
-                                                          _ptr(spectrogram), _ptr(aperiodicity)))
+        self._chain("analyze_batch", (_ptr(x), n, stride, xl, fs, C.byref(option)), n, harvest_options, dio_options,
+                    (_ptr(time_axis), _ptr(f0), time_axis.shape[1], _ptr(spectrogram), _ptr(aperiodicity)), device=True)
         return time_axis, f0, spectrogram, aperiodicity, fl
 
     # -- multi-GPU: one World per GPU / process; the NCCL id travels by the caller's own means -------------------
@@ -793,20 +805,11 @@ class World:
         harvest_options / dio_options: a list of one option per utterance of THIS rank's shard."""
         n, stride = x.shape
         xl, keep = _int_array(x_lengths, n)
-        per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
         outs = (_ptr(time_axis_full), _ptr(f0_full), time_axis_full.shape[1],
                 _ptr(spectrogram_full) if spectrogram_full is not None else None,
                 _ptr(aperiodicity_full) if aperiodicity_full is not None else None)
-        self._use_current_stream()
-        if per_utt is not None:
-            self._check(self.lib.world_b200_analyze_batch_allgather_options(
-                self._h, _ptr(x), n, stride, xl, fs, C.byref(option), per_utt, *outs))
-        elif per_dio is not None:
-            self._check(self.lib.world_b200_analyze_batch_allgather_dio_options(
-                self._h, _ptr(x), n, stride, xl, fs, C.byref(option), per_dio, *outs))
-        else:
-            self._check(self.lib.world_b200_analyze_batch_allgather(
-                self._h, _ptr(x), n, stride, xl, fs, C.byref(option), *outs))
+        self._chain("analyze_batch_allgather", (_ptr(x), n, stride, xl, fs, C.byref(option)), n, harvest_options,
+                    dio_options, outs, device=True)
 
     def analyze_host(self, x_host, fs, option: AnalysisOption, x_lengths=None, time_axis=None, f0=None,
                      spectrogram=None, aperiodicity=None, f0_stride=None, harvest_options=None, dio_options=None):
@@ -815,7 +818,7 @@ class World:
         one option per utterance of the chain's F0 method."""
         import numpy as np
         n, stride = x_host.shape
-        frame_period = option.dio.frame_period if option.f0_method == F0_DIO_STONEMASK else option.harvest.frame_period
+        frame_period = _frame_period(option)
         lens = [stride] * n if x_lengths is None else [int(v) for v in x_lengths]
         fl = [self.frames(fs, v, frame_period) for v in lens]
         f0_stride = f0_stride or max(fl)
@@ -829,20 +832,8 @@ class World:
         if aperiodicity is None:
             aperiodicity = np.zeros((n, f0_stride, bins))
         xl, keep = _int_array(x_lengths, n)
-        per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
-        if per_utt is not None:
-            self._check(self.lib.world_b200_analyze_host_options(self._h, _ptr(x_host), n, stride, xl, fs,
-                                                                 C.byref(option), per_utt, _ptr(time_axis), _ptr(f0),
-                                                                 f0_stride, _ptr(spectrogram), _ptr(aperiodicity)))
-        elif per_dio is not None:
-            self._check(self.lib.world_b200_analyze_host_dio_options(self._h, _ptr(x_host), n, stride, xl, fs,
-                                                                     C.byref(option), per_dio, _ptr(time_axis),
-                                                                     _ptr(f0), f0_stride, _ptr(spectrogram),
-                                                                     _ptr(aperiodicity)))
-        else:
-            self._check(self.lib.world_b200_analyze_host(self._h, _ptr(x_host), n, stride, xl, fs, C.byref(option),
-                                                         _ptr(time_axis), _ptr(f0), f0_stride, _ptr(spectrogram),
-                                                         _ptr(aperiodicity)))
+        self._chain("analyze_host", (_ptr(x_host), n, stride, xl, fs, C.byref(option)), n, harvest_options,
+                    dio_options, (_ptr(time_axis), _ptr(f0), f0_stride, _ptr(spectrogram), _ptr(aperiodicity)))
         return time_axis, f0, spectrogram, aperiodicity, fl
 
     # -- codec (codec.h) and ingest ----------------------------------------------------------
@@ -910,7 +901,7 @@ class World:
         n = x_host.shape[0]
         item = x_host.element_size() if hasattr(x_host, "element_size") else x_host.itemsize
         stride = x_host.shape[1] * item // (nbit // 8 if nbit else 8)
-        frame_period = option.dio.frame_period if option.f0_method == F0_DIO_STONEMASK else option.harvest.frame_period
+        frame_period = _frame_period(option)
         lens = [stride] * n if x_lengths is None else [int(v) for v in x_lengths]
         fl = [self.frames(fs, v, frame_period) for v in lens]
         f0_stride = f0_stride or max(fl)
@@ -924,22 +915,9 @@ class World:
         if coded_ap is None:
             coded_ap = np.zeros((n, f0_stride, max(1, n_ap)))
         xl, keep = _int_array(x_lengths, n)
-        per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
-        outs = (number_of_dimensions, _ptr(time_axis), _ptr(f0), f0_stride, _ptr(coded_sp), _ptr(coded_ap))
-        if cheaptrick_options is not None or d4c_options is not None:
-            ct = None if cheaptrick_options is None else _option_array(CheapTrickOption, cheaptrick_options, n)
-            d4 = None if d4c_options is None else _option_array(D4COption, d4c_options, n)
-            self._check(self.lib.world_b200_analyze_coded_host_spectral_options(
-                self._h, _ptr(x_host), nbit, n, stride, xl, fs, C.byref(option), per_utt, per_dio, ct, d4, *outs))
-        elif per_utt is not None:
-            self._check(self.lib.world_b200_analyze_coded_host_options(self._h, _ptr(x_host), nbit, n, stride, xl, fs,
-                                                                       C.byref(option), per_utt, *outs))
-        elif per_dio is not None:
-            self._check(self.lib.world_b200_analyze_coded_host_dio_options(self._h, _ptr(x_host), nbit, n, stride, xl,
-                                                                           fs, C.byref(option), per_dio, *outs))
-        else:
-            self._check(self.lib.world_b200_analyze_coded_host(self._h, _ptr(x_host), nbit, n, stride, xl, fs,
-                                                               C.byref(option), *outs))
+        self._chain("analyze_coded_host", (_ptr(x_host), nbit, n, stride, xl, fs, C.byref(option)), n, harvest_options,
+                    dio_options, (number_of_dimensions, _ptr(time_axis), _ptr(f0), f0_stride, _ptr(coded_sp),
+                                  _ptr(coded_ap)), cheaptrick_options=cheaptrick_options, d4c_options=d4c_options)
         return time_axis, f0, coded_sp, coded_ap, fl
 
     def _coded_rows(self, x, nbit, option):
@@ -951,7 +929,7 @@ class World:
         width = nbit // 8 if nbit else 8
         if (x.shape[1] * item) % width:
             raise ValueError(f"rows of {x.shape[1] * item} bytes do not hold whole {width}-byte samples")
-        frame_period = option.dio.frame_period if option.f0_method == F0_DIO_STONEMASK else option.harvest.frame_period
+        frame_period = _frame_period(option)
         return x.shape[0], x.shape[1] * item // width, frame_period
 
     def analyze_coded_batch(self, x, nbit, fs, option: AnalysisOption, number_of_dimensions, x_lengths=None,
@@ -978,23 +956,10 @@ class World:
         if coded_ap is None:
             coded_ap = self._zeros(x, (n, f_stride, max(1, self.number_of_aperiodicities(fs))))
         xl, keep = _int_array(x_lengths, n)
-        per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
-        outs = (number_of_dimensions, _ptr(time_axis), _ptr(f0), time_axis.shape[1], _ptr(coded_sp), _ptr(coded_ap))
-        self._use_current_stream()
-        if cheaptrick_options is not None or d4c_options is not None:
-            ct = None if cheaptrick_options is None else _option_array(CheapTrickOption, cheaptrick_options, n)
-            d4 = None if d4c_options is None else _option_array(D4COption, d4c_options, n)
-            self._check(self.lib.world_b200_analyze_coded_batch_spectral_options(
-                self._h, _ptr(x), nbit, n, stride, xl, fs, C.byref(option), per_utt, per_dio, ct, d4, *outs))
-        elif per_utt is not None:
-            self._check(self.lib.world_b200_analyze_coded_batch_options(self._h, _ptr(x), nbit, n, stride, xl, fs,
-                                                                        C.byref(option), per_utt, *outs))
-        elif per_dio is not None:
-            self._check(self.lib.world_b200_analyze_coded_batch_dio_options(self._h, _ptr(x), nbit, n, stride, xl, fs,
-                                                                            C.byref(option), per_dio, *outs))
-        else:
-            self._check(self.lib.world_b200_analyze_coded_batch(self._h, _ptr(x), nbit, n, stride, xl, fs,
-                                                                C.byref(option), *outs))
+        self._chain("analyze_coded_batch", (_ptr(x), nbit, n, stride, xl, fs, C.byref(option)), n, harvest_options,
+                    dio_options, (number_of_dimensions, _ptr(time_axis), _ptr(f0), time_axis.shape[1], _ptr(coded_sp),
+                                  _ptr(coded_ap)), cheaptrick_options=cheaptrick_options, d4c_options=d4c_options,
+                    device=True)
         return time_axis, f0, coded_sp, coded_ap, fl
 
     # -- voice transformation: analysis, modification and synthesis in one call --------------------------------
@@ -1070,16 +1035,7 @@ class World:
         D4C.  harvest_options / dio_options: a list of one option per utterance of THIS rank's shard."""
         n, stride, _ = self._coded_rows(x, nbit, option)
         xl, keep = _int_array(x_lengths, n)
-        per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
-        outs = (number_of_dimensions, _ptr(time_axis_full), _ptr(f0_full), time_axis_full.shape[1],
-                _ptr(coded_sp_full), _ptr(coded_ap_full))
-        self._use_current_stream()
-        if per_utt is not None:
-            self._check(self.lib.world_b200_analyze_coded_batch_allgather_options(
-                self._h, _ptr(x), nbit, n, stride, xl, fs, C.byref(option), per_utt, *outs))
-        elif per_dio is not None:
-            self._check(self.lib.world_b200_analyze_coded_batch_allgather_dio_options(
-                self._h, _ptr(x), nbit, n, stride, xl, fs, C.byref(option), per_dio, *outs))
-        else:
-            self._check(self.lib.world_b200_analyze_coded_batch_allgather(
-                self._h, _ptr(x), nbit, n, stride, xl, fs, C.byref(option), *outs))
+        self._chain("analyze_coded_batch_allgather", (_ptr(x), nbit, n, stride, xl, fs, C.byref(option)), n,
+                    harvest_options, dio_options, (number_of_dimensions, _ptr(time_axis_full), _ptr(f0_full),
+                                                   time_axis_full.shape[1], _ptr(coded_sp_full), _ptr(coded_ap_full)),
+                    device=True)

@@ -1,8 +1,7 @@
 // wb_api.cu -- context, scratch arena and the extern "C" ABI declared in include/world_b200.h,
 // plus the legacy single-utterance entry points of include/world/*.h implemented as n_utts = 1
 // batches (reference boundary: src/world/{dio,harvest,stonemask,cheaptrick,d4c}.h).
-#include "wb_internal.h"
-#include "../../include/world_b200.h"
+#include "wb_chain.h"
 #include <stdio.h>
 #include <string.h>
 #include <stdlib.h>
@@ -10,20 +9,6 @@
 #include <string>
 #include <algorithm>
 #include <cmath>
-
-struct WorldB200 {
-  wb::Ctx c;
-  int *lens_dev = nullptr;
-  size_t lens_cap = 0;
-  // world_b200_analyze_batch: two sibling contexts ("lanes"), each with its own stream, scratch arena and staging
-  // ring, created on first use; fork / join events order them against this context's stream
-  WorldB200 *lane[2] = {nullptr, nullptr};
-  void *lane_stream[2] = {nullptr, nullptr};   // cudaStream_t
-  void *ev_fork = nullptr, *ev_join[2] = {nullptr, nullptr};   // cudaEvent_t
-  // multi-GPU (wb_multi.cu): NCCL communicator + one event per utterance slice of analyze_batch_allgather
-  wb::Comm *comm = nullptr;
-  std::vector<void *> ev_slice;
-};
 
 namespace wb {
 
@@ -262,9 +247,11 @@ int ctx_init_tables(Ctx *ctx) {
 using namespace wb;
 
 // ------------------------------------------------------------------------------------------
-static int upload_lengths(WorldB200 *h, int n, int x_stride, const int *x_lengths, int f_stride,
-                          const int *f_lengths, Batch *b) {
+// The Batch of a stage entry point: its rows, and its lengths checked and uploaded (NULL lengths: full rows).
+static int load_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
+                      const double *time_axis, const double *f0, const int *f_lengths, int f_stride, Batch *b) {
   Ctx *ctx = &h->c;
+  b->x = x; b->n = n; b->x_stride = x_stride; b->fs = fs; b->time_axis = time_axis; b->f0 = f0; b->f_stride = f_stride;
   if ((size_t)2 * n > h->lens_cap) {
     dev_sync(ctx);
     dev_free(h->lens_dev);
@@ -332,47 +319,6 @@ int check_dio_options(Ctx *c, const DioOption *opts, int n, double frame_period,
     p[u] = {opts[u].f0_floor, opts[u].f0_ceil, opts[u].channels_in_octave, opts[u].frame_period, opts[u].allowed_range,
             opts[u].speed};
   return dio_check_options(c, fs, p.data(), n);
-}
-
-// Per-utterance F0 options of a chain (harvest_options or dio_options, at most one): they must belong to the chain's
-// f0_method and pass check_*_options for the whole batch before a slice or chunk is queued.  `who` prefixes the error.
-int check_chain_f0_options(Ctx *c, const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
-                           const DioOption *dio_options, int n, int fs, const char *who) {
-  if (harvest_options && dio_options) {
-    c->last_error = std::string(who) + ": per-utterance options of both F0 methods";
-    return WORLD_B200_EINVAL;
-  }
-  if (harvest_options) {
-    if (opt->f0_method != WORLD_B200_F0_HARVEST) {
-      c->last_error = std::string(who) + ": per-utterance Harvest options need f0_method == WORLD_B200_F0_HARVEST";
-      return WORLD_B200_EINVAL;
-    }
-    return check_harvest_options(c, harvest_options, n, opt->harvest.frame_period, fs);
-  }
-  if (dio_options) {
-    if (opt->f0_method != WORLD_B200_F0_DIO_STONEMASK) {
-      c->last_error = std::string(who) + ": per-utterance DIO options need f0_method == WORLD_B200_F0_DIO_STONEMASK";
-      return WORLD_B200_EINVAL;
-    }
-    return check_dio_options(c, dio_options, n, opt->dio.frame_period, opt->dio.speed, fs);
-  }
-  return 0;
-}
-
-// The F0 stage of a chain on m utterances: Harvest, or DIO + StoneMask.  harvest_options / dio_options: nullptr (the
-// chain's own option) or the options of these m utterances, checked by check_chain_f0_options.
-int run_f0_stage(WorldB200 *h, const double *x, int m, int x_stride, const int *x_lengths, int fs,
-                 const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options, const DioOption *dio_options,
-                 const int *f0_lengths, double *time_axis, double *f0, int f0_stride) {
-  if (opt->f0_method == WORLD_B200_F0_HARVEST)
-    return harvest_options
-               ? world_b200_harvest_batch_options(h, x, m, x_stride, x_lengths, fs, harvest_options, time_axis, f0, f0_stride)
-               : world_b200_harvest_batch(h, x, m, x_stride, x_lengths, fs, &opt->harvest, time_axis, f0, f0_stride);
-  int rc = dio_options
-               ? world_b200_dio_batch_options(h, x, m, x_stride, x_lengths, fs, dio_options, time_axis, f0, f0_stride)
-               : world_b200_dio_batch(h, x, m, x_stride, x_lengths, fs, &opt->dio, time_axis, f0, f0_stride);
-  if (!rc) rc = world_b200_stonemask_batch(h, x, m, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, f0);
-  return rc;
 }
 
 }  // namespace wb
@@ -522,8 +468,7 @@ int world_b200_cheaptrick_batch(WorldB200 *h, const double *x, int n, int x_stri
   if (!h || !x || !time_axis || !f0 || !opt || !spectrogram || n < 0 || fs <= 0) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
   Batch b;
-  b.x = x; b.n = n; b.x_stride = x_stride; b.fs = fs; b.time_axis = time_axis; b.f0 = f0; b.f_stride = f0_stride;
-  int rc = upload_lengths(h, n, x_stride, x_lengths, f0_stride, f0_lengths, &b);
+  int rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, &b);
   if (rc) return rc;
   return cheaptrick_run(&h->c, b, opt->q1, opt->fft_size, spectrogram);
 }
@@ -534,8 +479,7 @@ int world_b200_d4c_batch(WorldB200 *h, const double *x, int n, int x_stride, con
   if (!h || !x || !time_axis || !f0 || !opt || !aperiodicity || n < 0 || fs <= 0) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
   Batch b;
-  b.x = x; b.n = n; b.x_stride = x_stride; b.fs = fs; b.time_axis = time_axis; b.f0 = f0; b.f_stride = f0_stride;
-  int rc = upload_lengths(h, n, x_stride, x_lengths, f0_stride, f0_lengths, &b);
+  int rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, &b);
   if (rc) return rc;
   return d4c_run(&h->c, b, fft_size, opt->threshold, aperiodicity);
 }
@@ -550,8 +494,7 @@ int world_b200_cheaptrick_coded_batch(WorldB200 *h, const double *x, int n, int 
   int rc = codec_sp_tables(&h->c, fs, opt->fft_size, number_of_dimensions, &t);
   if (rc) return rc;
   Batch b;
-  b.x = x; b.n = n; b.x_stride = x_stride; b.fs = fs; b.time_axis = time_axis; b.f0 = f0; b.f_stride = f0_stride;
-  rc = upload_lengths(h, n, x_stride, x_lengths, f0_stride, f0_lengths, &b);
+  rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, &b);
   if (rc) return rc;
   return cheaptrick_run(&h->c, b, opt->q1, opt->fft_size, nullptr, &t, coded_spectral_envelope);
 }
@@ -567,8 +510,7 @@ int world_b200_d4c_coded_batch(WorldB200 *h, const double *x, int n, int x_strid
   if (t.dims == 0) return 0;        // nothing to write below 12 kHz, like the reference's empty loops
   if (!coded_aperiodicity) return WORLD_B200_EINVAL;
   Batch b;
-  b.x = x; b.n = n; b.x_stride = x_stride; b.fs = fs; b.time_axis = time_axis; b.f0 = f0; b.f_stride = f0_stride;
-  rc = upload_lengths(h, n, x_stride, x_lengths, f0_stride, f0_lengths, &b);
+  rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, &b);
   if (rc) return rc;
   return d4c_run(&h->c, b, fft_size, opt->threshold, nullptr, &t, coded_aperiodicity);
 }
@@ -649,8 +591,7 @@ static int cheaptrick_options_impl(WorldB200 *h, const double *x, int n, int x_s
     groups[g].max_f_len = std::max(groups[g].max_f_len, fl);
   }
   Batch b;
-  b.x = x; b.n = n; b.x_stride = x_stride; b.fs = fs; b.time_axis = time_axis; b.f0 = f0; b.f_stride = f0_stride;
-  if ((rc = upload_lengths(h, n, x_stride, x_lengths, f0_stride, f0_lengths, &b))) return rc;
+  if ((rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, &b))) return rc;
   for (size_t g = 0; g < groups.size() && !rc; ++g) {
     const int u = groups[g].uid[0];
     // a batch of one option runs exactly as the one-option call
@@ -688,8 +629,7 @@ static int d4c_options_impl(WorldB200 *h, const double *x, int n, int x_stride, 
   for (int u = 0; u < n; ++u) pu.threshold[u] = opts[u].threshold;
   pu.row_stride = row_stride;
   Batch b;
-  b.x = x; b.n = n; b.x_stride = x_stride; b.fs = fs; b.time_axis = time_axis; b.f0 = f0; b.f_stride = f0_stride;
-  if ((rc = upload_lengths(h, n, x_stride, x_lengths, f0_stride, f0_lengths, &b))) return rc;
+  if ((rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, &b))) return rc;
   return d4c_run(c, b, pu.fft_size[0], pu.threshold[0], want_coded ? nullptr : aperiodicity,
                  want_coded ? &pu.tables[0] : nullptr, coded, &pu);
 }
@@ -697,32 +637,130 @@ static int d4c_options_impl(WorldB200 *h, const double *x, int n, int x_stride, 
 }  // extern "C"
 
 namespace wb {
-// The spectral options of a coded chain (world_b200_analyze_coded_*_spectral_options) for every utterance, before any
-// work is queued: each utterance's CheapTrick option and D4C (fft_size = its CheapTrick size, option), the chain's
-// option standing in for an array that is NULL; then the stage calls' rules and the codec tables of every distinct size
-// (number_of_dimensions against each CheapTrick size).
-int chain_spectral_options(Ctx *c, int fs, int dims, const WorldB200AnalysisOption *opt,
-                           const CheapTrickOption *ct_options, const D4COption *d4c_options, int n,
-                           bool spectral_envelope, bool aperiodicity, std::vector<CheapTrickOption> *cts,
-                           std::vector<int> *d4_fft, std::vector<D4COption> *d4s) {
-  cts->assign(n, opt->cheaptrick);
-  d4s->assign(n, opt->d4c);
-  if (ct_options) std::copy(ct_options, ct_options + n, cts->begin());
-  if (d4c_options) std::copy(d4c_options, d4c_options + n, d4s->begin());
-  d4_fft->resize(n);
-  for (int u = 0; u < n; ++u) (*d4_fft)[u] = (*cts)[u].fft_size;
-  std::vector<int> sizes, distinct;
-  int rc = check_cheaptrick_options(c, cts->data(), n, &sizes);
-  if (!rc) rc = check_d4c_options(c, d4_fft->data(), d4s->data(), n);
+// chain_plan without the caller's prefix on last_error
+static int chain_checks(Ctx *c, const ChainRequest &r, ChainPlan *p) {
+  auto fail = [c](const std::string &what) {
+    c->last_error = what;
+    return WORLD_B200_EINVAL;
+  };
+  const WorldB200AnalysisOption *opt = r.opt;
+  if (!r.x || !opt || r.n < 0 || r.fs <= 0 || r.x_stride <= 0 || r.f0_stride < 0)
+    return fail("x and option must be given, with n_utts >= 0, fs > 0 and positive strides");
+  if (r.nbit != 0 && r.nbit != 8 && r.nbit != 16 && r.nbit != 24 && r.nbit != 32)
+    return fail("nbit must be 0, 8, 16, 24 or 32");
+  const int n = r.n, fft_size = opt->cheaptrick.fft_size;
+  const bool spectral_options = r.cheaptrick_options || r.d4c_options;
+  if ((r.spectrogram || r.aperiodicity) && fft_size < 16) return fail("CheapTrick: fft_size must be at least 16");
+  // with per-utterance spectral options each utterance's size bounds number_of_dimensions (its codec tables, below)
+  if (r.coded && (r.dims < 1 || (!spectral_options && r.dims > fft_size / 4 + 1)))
+    return fail("number_of_dimensions must be in [1, fft_size/4 + 1]");
+
+  // per-utterance F0 options: of the chain's F0 method, one frame_period (and, for DIO, one speed) for the batch, and
+  // every utterance's range against the on-chip limits
+  const bool harvest = opt->f0_method == WORLD_B200_F0_HARVEST;
+  if (r.harvest_options && r.dio_options) return fail("per-utterance options of both F0 methods");
+  if (r.harvest_options && !harvest)
+    return fail("per-utterance Harvest options need f0_method == WORLD_B200_F0_HARVEST");
+  if (r.dio_options && opt->f0_method != WORLD_B200_F0_DIO_STONEMASK)
+    return fail("per-utterance DIO options need f0_method == WORLD_B200_F0_DIO_STONEMASK");
+  int rc = r.harvest_options ? check_harvest_options(c, r.harvest_options, n, opt->harvest.frame_period, r.fs)
+           : r.dio_options   ? check_dio_options(c, r.dio_options, n, opt->dio.frame_period, opt->dio.speed, r.fs)
+                             : 0;
   if (rc) return rc;
-  size_index(sizes, &distinct);
-  for (const int fft : distinct) {
+  p->frame_period = harvest ? opt->harvest.frame_period : opt->dio.frame_period;
+  if (!(p->frame_period > 0.0)) return fail("the F0 method's frame_period must be > 0");
+
+  const int n_ap = r.coded ? GetNumberOfAperiodicities(r.fs) : 0;
+  p->sp_row = r.coded ? (size_t)r.dims : (size_t)(fft_size / 2 + 1);
+  p->ap_row = r.coded ? (size_t)n_ap : (size_t)(fft_size / 2 + 1);
+  p->want_sp = r.spectrogram != nullptr;
+  p->want_ap = r.aperiodicity != nullptr && (!r.coded || n_ap > 0);   // no bands below 12 kHz: D4C is skipped
+  if (spectral_options) {
+    // each utterance's CheapTrick option and D4C (fft_size = its CheapTrick size, option), the per-call option standing
+    // in for an array that is NULL; the stage calls' rules, then the codec tables of every distinct size
+    p->cts.assign(n, opt->cheaptrick);
+    p->d4s.assign(n, opt->d4c);
+    if (r.cheaptrick_options) std::copy(r.cheaptrick_options, r.cheaptrick_options + n, p->cts.begin());
+    if (r.d4c_options) std::copy(r.d4c_options, r.d4c_options + n, p->d4s.begin());
+    p->d4_fft.resize(n);
+    for (int u = 0; u < n; ++u) p->d4_fft[u] = p->cts[u].fft_size;
+    std::vector<int> sizes, distinct;
+    rc = check_cheaptrick_options(c, p->cts.data(), n, &sizes);
+    if (!rc) rc = check_d4c_options(c, p->d4_fft.data(), p->d4s.data(), n);
+    if (rc) return rc;
+    size_index(sizes, &distinct);
+    for (const int fft : distinct) {
+      CodecTables t;
+      rc = r.spectrogram ? codec_sp_tables(c, r.fs, fft, r.dims, &t) : 0;
+      if (!rc && r.aperiodicity) rc = codec_ap_tables(c, r.fs, fft, &t);
+      if (rc) return utterance_fail(c, (int)(std::find(sizes.begin(), sizes.end(), fft) - sizes.begin()), c->last_error);
+    }
+  } else if (r.coded) {
+    // the codec tables of every slice or chunk, built once here so that a bad dimension count or fft_size queues nothing
     CodecTables t;
-    rc = spectral_envelope ? codec_sp_tables(c, fs, fft, dims, &t) : 0;
-    if (!rc && aperiodicity) rc = codec_ap_tables(c, fs, fft, &t);
-    if (rc) return utterance_fail(c, (int)(std::find(sizes.begin(), sizes.end(), fft) - sizes.begin()), c->last_error);
+    rc = r.spectrogram ? codec_sp_tables(c, r.fs, fft_size, r.dims, &t) : 0;
+    if (!rc && r.aperiodicity) rc = codec_ap_tables(c, r.fs, fft_size, &t);
+    if (rc) return rc;
   }
+
+  p->f_len.resize(n);
+  int most = 1;
+  for (int u = 0; u < n; ++u) {
+    const int xl = r.x_lengths ? r.x_lengths[u] : r.x_stride;
+    if (xl < 1 || xl > r.x_stride)
+      return fail("x_lengths[" + std::to_string(u) + "] = " + std::to_string(xl) + " is outside its padded row of " +
+                  std::to_string(r.x_stride) + " samples");
+    p->f_len[u] = frames_for(r.fs, xl, p->frame_period);
+    if (r.f0_stride && p->f_len[u] > r.f0_stride)
+      return utterance_fail(c, u, "f0_stride smaller than the frame count of an utterance");
+    most = imax(most, p->f_len[u]);
+  }
+  p->f0_stride = r.f0_stride ? r.f0_stride : most;
   return 0;
+}
+
+int chain_plan(Ctx *c, const ChainRequest &r, const char *who, ChainPlan *p) {
+  const int rc = chain_checks(c, r, p);
+  if (rc) c->last_error = std::string(who) + ": " + c->last_error;
+  return rc;
+}
+
+int chain_f0(WorldB200 *h, const ChainRequest &r, const ChainPlan &p, int u0, int m, const double *x, double *time_axis,
+             double *f0) {
+  const WorldB200AnalysisOption *opt = r.opt;
+  const int *xl = r.x_lengths ? r.x_lengths + u0 : nullptr;
+  if (opt->f0_method == WORLD_B200_F0_HARVEST)
+    return r.harvest_options ? world_b200_harvest_batch_options(h, x, m, r.x_stride, xl, r.fs, r.harvest_options + u0,
+                                                                time_axis, f0, p.f0_stride)
+                             : world_b200_harvest_batch(h, x, m, r.x_stride, xl, r.fs, &opt->harvest, time_axis, f0,
+                                                        p.f0_stride);
+  int rc = r.dio_options
+               ? world_b200_dio_batch_options(h, x, m, r.x_stride, xl, r.fs, r.dio_options + u0, time_axis, f0, p.f0_stride)
+               : world_b200_dio_batch(h, x, m, r.x_stride, xl, r.fs, &opt->dio, time_axis, f0, p.f0_stride);
+  if (!rc)
+    rc = world_b200_stonemask_batch(h, x, m, r.x_stride, xl, r.fs, time_axis, f0, p.f_len.data() + u0, p.f0_stride, f0);
+  return rc;
+}
+
+int chain_spectral(WorldB200 *h, const ChainRequest &r, const ChainPlan &p, int u0, int m, const double *x,
+                   const double *time_axis, const double *f0, double *sp, double *ap) {
+  const WorldB200AnalysisOption *opt = r.opt;
+  const int *xl = r.x_lengths ? r.x_lengths + u0 : nullptr, *fl = p.f_len.data() + u0;
+  const int xs = r.x_stride, fs = r.fs, fst = p.f0_stride, fft_size = opt->cheaptrick.fft_size;
+  const double *t = time_axis;
+  const bool per_utt = !p.cts.empty();
+  int rc = 0;
+  if (sp)
+    rc = per_utt ? world_b200_cheaptrick_coded_batch_options(h, x, m, xs, xl, fs, t, f0, fl, fst, p.cts.data() + u0,
+                                                             r.dims, sp)
+         : r.coded ? world_b200_cheaptrick_coded_batch(h, x, m, xs, xl, fs, t, f0, fl, fst, &opt->cheaptrick, r.dims, sp)
+                   : world_b200_cheaptrick_batch(h, x, m, xs, xl, fs, t, f0, fl, fst, &opt->cheaptrick, sp);
+  if (!rc && ap)
+    rc = per_utt ? world_b200_d4c_coded_batch_options(h, x, m, xs, xl, fs, t, f0, fl, fst, p.d4_fft.data() + u0,
+                                                      p.d4s.data() + u0, ap)
+         : r.coded ? world_b200_d4c_coded_batch(h, x, m, xs, xl, fs, t, f0, fl, fst, fft_size, &opt->d4c, ap)
+                   : world_b200_d4c_batch(h, x, m, xs, xl, fs, t, f0, fl, fst, fft_size, &opt->d4c, ap);
+  return rc;
 }
 }  // namespace wb
 
@@ -779,8 +817,7 @@ int world_b200_stonemask_batch(WorldB200 *h, const double *x, int n, int x_strid
   if (!h || !x || !time_axis || !f0 || !refined_f0 || n < 0 || fs <= 0) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
   Batch b;
-  b.x = x; b.n = n; b.x_stride = x_stride; b.fs = fs; b.time_axis = time_axis; b.f0 = f0; b.f_stride = f0_stride;
-  int rc = upload_lengths(h, n, x_stride, x_lengths, f0_stride, f0_lengths, &b);
+  int rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, &b);
   if (rc) return rc;
   return stonemask_run(&h->c, b, refined_f0);
 }
@@ -813,8 +850,7 @@ static int dio_batch_impl(WorldB200 *h, const double *x, int n, int x_stride, co
   int rc = f0_lengths_from_x(n, x_stride, x_lengths, fs, opt->frame_period, f0_stride, &fl, &h->c.last_error);
   if (rc) return rc;
   Batch b;
-  b.x = x; b.n = n; b.x_stride = x_stride; b.fs = fs; b.time_axis = time_axis; b.f0 = f0; b.f_stride = f0_stride;
-  rc = upload_lengths(h, n, x_stride, x_lengths, f0_stride, fl.data(), &b);
+  rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, fl.data(), f0_stride, &b);
   if (rc) return rc;
   b.x_len_host = x_lengths;
   std::vector<DioParams> p(per_utt ? (n > 0 ? n : 1) : 1);
@@ -848,8 +884,7 @@ static int harvest_batch_impl(WorldB200 *h, const double *x, int n, int x_stride
   int rc = f0_lengths_from_x(n, x_stride, x_lengths, fs, opt->frame_period, f0_stride, &fl, &h->c.last_error);
   if (rc) return rc;
   Batch b;
-  b.x = x; b.n = n; b.x_stride = x_stride; b.fs = fs; b.time_axis = time_axis; b.f0 = f0; b.f_stride = f0_stride;
-  rc = upload_lengths(h, n, x_stride, x_lengths, f0_stride, fl.data(), &b);
+  rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, fl.data(), f0_stride, &b);
   if (rc) return rc;
   std::vector<int> l1(n > 0 ? n : 1);
   for (int i = 0; i < n; ++i) l1[i] = frames_for(fs, x_lengths ? x_lengths[i] : x_stride, 1.0);
@@ -974,63 +1009,23 @@ extern "C" {
 // gather = false: time_axis / f0 / spectrogram / aperiodicity hold this call's n utterances.
 // gather = true (multi-GPU): they are the FULL arrays of n_ranks * n utterances; this rank computes into block `rank`
 // and every finished slice is broadcast to the other ranks on the communication stream while the next one is computed.
-// harvest_options / dio_options: nullptr, or one option per utterance of the chain's F0 method (at most one of the two;
-// check_chain_f0_options); the slices split the array with the utterances.
-// nbit: 0 = x holds doubles; 8/16/24/32 = little-endian PCM, converted slice by slice on the lane that analyses it.
-// dims: 0 = spectrogram / aperiodicity receive the fft_size/2+1-bin rows; > 0 = they receive the coded rows
-// (number_of_dimensions / GetNumberOfAperiodicities(fs) values per frame) straight from the fused frame kernels.
-// ct_options / d4c_options (coded rows only): nullptr, or one CheapTrick / D4C option per utterance; D4C then runs at
-// each utterance's CheapTrick fft_size (checked up front by chain_spectral_options).
-static int analyze_batch_impl(WorldB200 *h, const void *x, int nbit, int n, int x_stride, const int *x_lengths, int fs,
-                              const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
-                              const DioOption *dio_options, int dims, double *time_axis, double *f0, int f0_stride,
-                              double *spectrogram, double *aperiodicity, bool gather,
-                              const CheapTrickOption *ct_options = nullptr, const D4COption *d4c_options = nullptr) {
-  if (!h || !x || !opt || !time_axis || !f0 || n < 0 || fs <= 0 || x_stride <= 0 || f0_stride <= 0) return WORLD_B200_EINVAL;
-  if ((spectrogram || aperiodicity) && opt->cheaptrick.fft_size < 16) return WORLD_B200_EINVAL;
+// PCM input (nbit != 0) is converted slice by slice on the lane that analyses it; the per-utterance option arrays are
+// split with the utterances.
+static int analyze_chain(WorldB200 *h, const ChainRequest &r, bool gather) {
+  if (!h) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
-  const char *who = dims ? "analyze_coded_batch" : "analyze_batch";
-  if (nbit != 0 && nbit != 8 && nbit != 16 && nbit != 24 && nbit != 32) {
-    h->c.last_error = std::string(who) + ": nbit must be 0, 8, 16, 24 or 32";
+  const char *who = r.coded ? "analyze_coded_batch" : "analyze_batch";
+  if (!r.time_axis || !r.f0 || r.f0_stride <= 0) {
+    h->c.last_error = std::string(who) + ": time_axis and f0 must be given, with f0_stride > 0";
     return WORLD_B200_EINVAL;
   }
-  {
-    const int rc = check_chain_f0_options(&h->c, opt, harvest_options, dio_options, n, fs, who);
-    if (rc) return rc;
-  }
-  const int bins = opt->cheaptrick.fft_size / 2 + 1;
-  const int n_ap = dims ? GetNumberOfAperiodicities(fs) : 0;
-  const bool spectral_options = ct_options || d4c_options;
-  if (dims && !spectral_options) {
-    // the codec tables of every slice, built once here so that a bad dimension count or fft_size queues nothing
-    CodecTables t;
-    int rc = spectrogram ? codec_sp_tables(&h->c, fs, opt->cheaptrick.fft_size, dims, &t) : 0;
-    if (!rc && aperiodicity) rc = codec_ap_tables(&h->c, fs, opt->cheaptrick.fft_size, &t);
-    if (rc) return rc;
-    if (n_ap == 0) aperiodicity = nullptr;   // no bands below 12 kHz: nothing to write, D4C is skipped
-  }
-  // per-utterance spectral options: every utterance's CheapTrick option and D4C (fft_size, option), the per-call
-  // option standing in for an array that is not given
-  std::vector<CheapTrickOption> cts;
-  std::vector<D4COption> d4s;
-  std::vector<int> d4_fft;
-  if (spectral_options) {
-    const int rc = chain_spectral_options(&h->c, fs, dims, opt, ct_options, d4c_options, n, spectrogram != nullptr,
-                                          aperiodicity != nullptr, &cts, &d4_fft, &d4s);
-    if (rc) return rc;
-    if (n_ap == 0) aperiodicity = nullptr;
-  }
-  const size_t sp_row = dims ? (size_t)dims : (size_t)bins, ap_row = dims ? (size_t)n_ap : (size_t)bins;
-  if (n == 0) return 0;
-  const double frame_period = opt->f0_method == WORLD_B200_F0_HARVEST ? opt->harvest.frame_period : opt->dio.frame_period;
-  // every utterance's length and frame count up front: a bad one queues no slice
-  std::vector<int> fl(n);
-  for (int i = 0; i < n; ++i) {
-    const int xl = x_lengths ? x_lengths[i] : x_stride;
-    if (xl < 1 || xl > x_stride) { h->c.last_error = "utterance length outside its padded row"; return WORLD_B200_EINVAL; }
-    fl[i] = frames_for(fs, xl, frame_period);
-    if (fl[i] > f0_stride) { h->c.last_error = "f0_stride smaller than the frame count of an utterance"; return WORLD_B200_EINVAL; }
-  }
+  ChainPlan p;
+  int rc = chain_plan(&h->c, r, who, &p);
+  if (rc || r.n == 0) return rc;
+  const int n = r.n, nbit = r.nbit, x_stride = r.x_stride, f0_stride = p.f0_stride;
+  const size_t sp_row = p.sp_row, ap_row = p.ap_row;
+  double *time_axis = r.time_axis, *f0 = r.f0;
+  double *spectrogram = p.want_sp ? r.spectrogram : nullptr, *aperiodicity = p.want_ap ? r.aperiodicity : nullptr;
   size_t my_block = 0;
   if (gather) {
     if (!h->comm) { h->c.last_error = std::string(who) + "_allgather: no communicator (world_b200_comm_init)"; return WORLD_B200_EINVAL; }
@@ -1059,7 +1054,7 @@ static int analyze_batch_impl(WorldB200 *h, const void *x, int nbit, int n, int 
   // nbit != 0: each lane converts its slice into a float64 buffer, which the slice's three stages then read.  A lane
   // runs its slices in stream order, so one buffer per lane, sized for its largest slice, serves all of them.
   LaneScope lanes(h);
-  int rc = lanes.open(bounds, [&](int m) { return nbit ? (size_t)m * x_stride * sizeof(double) : (size_t)0; });
+  rc = lanes.open(bounds, [&](int m) { return nbit ? (size_t)m * x_stride * sizeof(double) : (size_t)0; });
   if (rc) return rc;
 #ifndef WB_EMU
   // multi-GPU: the full arrays and how a finished slice reaches the other ranks -- pushed into their (IPC-mapped)
@@ -1084,35 +1079,17 @@ static int analyze_batch_impl(WorldB200 *h, const void *x, int nbit, int n, int 
     const int m = u1 - u0;
     if (m <= 0) continue;
     WorldB200 *L = lanes.lane(s);
-    const int *xl = x_lengths ? x_lengths + u0 : nullptr;
     const double *xs = (const double *)lanes.buffer(s);
     if (nbit)
-      rc = world_b200_pcm_to_double_batch(L, (const unsigned char *)x + (size_t)u0 * x_stride * (nbit / 8), nbit, m,
-                                          x_stride, xl, (double *)lanes.buffer(s));
+      rc = world_b200_pcm_to_double_batch(L, (const unsigned char *)r.x + (size_t)u0 * x_stride * (nbit / 8), nbit, m,
+                                          x_stride, r.x_lengths ? r.x_lengths + u0 : nullptr, (double *)lanes.buffer(s));
     else
-      xs = (const double *)x + (size_t)u0 * x_stride;
+      xs = (const double *)r.x + (size_t)u0 * x_stride;
     double *ts = time_axis + (size_t)u0 * f0_stride, *fs_ = f0 + (size_t)u0 * f0_stride;
-    const int *fls = fl.data() + u0;
+    if (!rc) rc = chain_f0(L, r, p, u0, m, xs, ts, fs_);
     if (!rc)
-      rc = run_f0_stage(L, xs, m, x_stride, xl, fs, opt, harvest_options ? harvest_options + u0 : nullptr,
-                        dio_options ? dio_options + u0 : nullptr, fls, ts, fs_, f0_stride);
-    double *sps = spectrogram ? spectrogram + (size_t)u0 * f0_stride * sp_row : nullptr;
-    double *aps = aperiodicity ? aperiodicity + (size_t)u0 * f0_stride * ap_row : nullptr;
-    if (!rc && sps && spectral_options)
-      rc = world_b200_cheaptrick_coded_batch_options(L, xs, m, x_stride, xl, fs, ts, fs_, fls, f0_stride,
-                                                     cts.data() + u0, dims, sps);
-    else if (!rc && sps)
-      rc = dims ? world_b200_cheaptrick_coded_batch(L, xs, m, x_stride, xl, fs, ts, fs_, fls, f0_stride, &opt->cheaptrick,
-                                                    dims, sps)
-                : world_b200_cheaptrick_batch(L, xs, m, x_stride, xl, fs, ts, fs_, fls, f0_stride, &opt->cheaptrick, sps);
-    if (!rc && aps && spectral_options)
-      rc = world_b200_d4c_coded_batch_options(L, xs, m, x_stride, xl, fs, ts, fs_, fls, f0_stride, d4_fft.data() + u0,
-                                              d4s.data() + u0, aps);
-    else if (!rc && aps)
-      rc = dims ? world_b200_d4c_coded_batch(L, xs, m, x_stride, xl, fs, ts, fs_, fls, f0_stride,
-                                             opt->cheaptrick.fft_size, &opt->d4c, aps)
-                : world_b200_d4c_batch(L, xs, m, x_stride, xl, fs, ts, fs_, fls, f0_stride, opt->cheaptrick.fft_size,
-                                       &opt->d4c, aps);
+      rc = chain_spectral(L, r, p, u0, m, xs, ts, fs_, spectrogram ? spectrogram + (size_t)u0 * f0_stride * sp_row : nullptr,
+                          aperiodicity ? aperiodicity + (size_t)u0 * f0_stride * ap_row : nullptr);
     if (rc && L != h) h->c.last_error = L->c.last_error;
 #ifndef WB_EMU
     if (!rc && exchange) {
@@ -1146,8 +1123,8 @@ static int analyze_batch_impl(WorldB200 *h, const void *x, int nbit, int n, int 
 int world_b200_analyze_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
                              const WorldB200AnalysisOption *opt, double *time_axis, double *f0, int f0_stride,
                              double *spectrogram, double *aperiodicity) {
-  return analyze_batch_impl(h, x, 0, n, x_stride, x_lengths, fs, opt, nullptr, nullptr, 0, time_axis, f0, f0_stride,
-                            spectrogram, aperiodicity, false);
+  return analyze_chain(h, ChainRequest(x, 0, n, x_stride, x_lengths, fs, opt, time_axis, f0, f0_stride, spectrogram,
+                                       aperiodicity), false);
 }
 
 int world_b200_analyze_batch_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
@@ -1155,8 +1132,9 @@ int world_b200_analyze_batch_options(WorldB200 *h, const double *x, int n, int x
                                      double *time_axis, double *f0, int f0_stride, double *spectrogram,
                                      double *aperiodicity) {
   if (!harvest_options) return WORLD_B200_EINVAL;
-  return analyze_batch_impl(h, x, 0, n, x_stride, x_lengths, fs, opt, harvest_options, nullptr, 0, time_axis, f0, f0_stride,
-                            spectrogram, aperiodicity, false);
+  ChainRequest r(x, 0, n, x_stride, x_lengths, fs, opt, time_axis, f0, f0_stride, spectrogram, aperiodicity);
+  r.harvest_options = harvest_options;
+  return analyze_chain(h, r, false);
 }
 
 int world_b200_analyze_batch_dio_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
@@ -1164,8 +1142,9 @@ int world_b200_analyze_batch_dio_options(WorldB200 *h, const double *x, int n, i
                                          double *time_axis, double *f0, int f0_stride, double *spectrogram,
                                          double *aperiodicity) {
   if (!dio_options) return WORLD_B200_EINVAL;
-  return analyze_batch_impl(h, x, 0, n, x_stride, x_lengths, fs, opt, nullptr, dio_options, 0, time_axis, f0, f0_stride,
-                            spectrogram, aperiodicity, false);
+  ChainRequest r(x, 0, n, x_stride, x_lengths, fs, opt, time_axis, f0, f0_stride, spectrogram, aperiodicity);
+  r.dio_options = dio_options;
+  return analyze_chain(h, r, false);
 }
 
 }  // extern "C"
@@ -1173,11 +1152,9 @@ int world_b200_analyze_batch_dio_options(WorldB200 *h, const double *x, int n, i
 // ---- voice transformation: analysis, modification and synthesis in one call (world_b200_transform_*)
 namespace wb {
 
-// Every check of the call before any work is queued (EINVAL, last_error naming the first bad utterance), and the
-// per-utterance frame counts, output lengths and synthesis frame periods.
-int transform_check(WorldB200 *h, const void *x, int nbit, int n, int x_stride, const int *x_lengths, int fs,
-                    const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
-                    const DioOption *dio_options, const double *f0_scale, const double *spectral_ratio,
+// Every check of the call before any work is queued (EINVAL, last_error naming the first bad utterance): the analysis
+// plan, then the output lengths and synthesis frame periods.
+int transform_check(WorldB200 *h, const ChainRequest &r, const double *f0_scale, const double *spectral_ratio,
                     const double *time_scale, int nbit_out, const void *y, int y_stride, const char *who,
                     TransformPlan *tp) {
   Ctx *c = &h->c;
@@ -1186,49 +1163,39 @@ int transform_check(WorldB200 *h, const void *x, int nbit, int n, int x_stride, 
     c->last_error = std::string(who) + ": " + what;
     return WORLD_B200_EINVAL;
   };
-  if (!x || !opt || !y || n < 0 || fs <= 0 || x_stride <= 0 || y_stride <= 0)
-    return fail("x, option and y must be given, with n_utts >= 0, fs > 0 and positive strides");
-  if (nbit != 0 && nbit != 8 && nbit != 16 && nbit != 24 && nbit != 32) return fail("nbit must be 0, 8, 16, 24 or 32");
+  if (!y || y_stride <= 0) return fail("y must be given, with y_stride > 0");
   if (nbit_out != 0 && nbit_out != 16) return fail("nbit_out must be 0 (float64) or 16 (int16)");
-  int rc = check_chain_f0_options(c, opt, harvest_options, dio_options, n, fs, who);
-  if (!rc) rc = synthesis_fft(c, opt->cheaptrick.fft_size, &tp->lg);
+  const ChainPlan &p = tp->chain;
+  int rc = chain_plan(c, r, who, &tp->chain);
+  if (!rc) rc = synthesis_fft(c, r.opt->cheaptrick.fft_size, &tp->lg);
   if (rc) return rc;
   tp->modify = f0_scale || spectral_ratio;
-  if (tp->modify) rc = modify_plan(c, n, opt->cheaptrick.fft_size, fs, f0_scale, spectral_ratio, &tp->mod);
+  if (tp->modify) rc = modify_plan(c, r.n, r.opt->cheaptrick.fft_size, r.fs, f0_scale, spectral_ratio, &tp->mod);
   if (rc) return rc;
-  const double frame_period = opt->f0_method == WORLD_B200_F0_HARVEST ? opt->harvest.frame_period : opt->dio.frame_period;
-  if (!(frame_period > 0.0)) return fail("the F0 method's frame_period must be > 0");
-  tp->nbit = nbit; tp->nbit_out = nbit_out; tp->x_stride = x_stride; tp->y_stride = y_stride; tp->fs = fs;
-  tp->fft_size = opt->cheaptrick.fft_size; tp->frame_period = frame_period; tp->f0_stride = 1;
-  tp->f_len.resize(n); tp->y_len.resize(n); tp->fp.resize(n);
-  for (int u = 0; u < n; ++u) {
-    const int xl = x_lengths ? x_lengths[u] : x_stride;
+  tp->nbit_out = nbit_out; tp->y_stride = y_stride;
+  tp->y_len.resize(r.n); tp->fp.resize(r.n);
+  for (int u = 0; u < r.n; ++u) {
+    const int xl = r.x_lengths ? r.x_lengths[u] : r.x_stride;
     const double ts = time_scale ? time_scale[u] : 1.0;
-    if (xl < 1 || xl > x_stride) {
-      snprintf(msg, sizeof msg, "x_lengths[%d] = %d is outside its padded row of %d samples", u, xl, x_stride);
-      return fail(msg);
-    }
     if (!(ts > 0.0) || !isfinite(ts)) {
       snprintf(msg, sizeof msg, "time_scale[%d] = %.17g is not a finite factor > 0", u, ts);
       return fail(msg);
     }
-    tp->f_len[u] = frames_for(fs, xl, frame_period);
-    tp->y_len[u] = world_b200_transform_samples(fs, xl, frame_period, ts);
-    if (tp->f_len[u] < 2) {
-      snprintf(msg, sizeof msg, "utterance %d has %d frame(s); Synthesis needs 2", u, tp->f_len[u]);
+    tp->y_len[u] = world_b200_transform_samples(r.fs, xl, p.frame_period, ts);
+    if (p.f_len[u] < 2) {
+      snprintf(msg, sizeof msg, "utterance %d has %d frame(s); Synthesis needs 2", u, p.f_len[u]);
       return fail(msg);
     }
     if (tp->y_len[u] < 2 || tp->y_len[u] > y_stride) {
       snprintf(msg, sizeof msg, "y_length of utterance %d is %d, outside [2, y_stride = %d]", u, tp->y_len[u], y_stride);
       return fail(msg);
     }
-    tp->fp[u] = (frame_period * ts) / 1000.0;   // synthesis_batch's frame_period / 1000.0, with the same product
-    tp->f0_stride = imax(tp->f0_stride, tp->f_len[u]);
+    tp->fp[u] = (p.frame_period * ts) / 1000.0;   // synthesis_batch's frame_period / 1000.0, with the same product
   }
   return 0;
 }
 
-// Utterances [u0, u0 + n) of a checked call: x and y point at utterance u0's rows (DEVICE), x_lengths and the
+// Utterances [u0, u0 + n) of a checked call: x and y point at utterance u0's rows (DEVICE); the request's x_lengths and
 // per-utterance options are the call's whole arrays.  The utterances are cut into slices that alternate between the
 // two lanes of a LaneScope.  A slice's rows (float64 input, time axis, f0, spectrogram, aperiodicity) live from its
 // analysis to its synthesis in one buffer per lane, taken from the lane's pool and sized for its largest slice; slices
@@ -1237,22 +1204,22 @@ int transform_check(WorldB200 *h, const void *x, int nbit, int n, int x_stride, 
 // its slices in stream order, so A(s + 1) never overwrites rows S(s - 1) still reads, and while synthesis_run waits
 // for its pulse counts (a host synchronisation of its lane), the other lane has an analysis queued.  One lane (one
 // slice, or the host emulation) runs A(s), S(s) in turn.  The caller's stream waits for both lanes on return.
-int transform_run(WorldB200 *h, const TransformPlan &tp, const void *x, const int *x_lengths,
-                  const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
-                  const DioOption *dio_options, int u0, int n, void *y) {
+int transform_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, const void *x, int u0, int n, void *y) {
   if (n <= 0) return 0;
-  const int f0_stride = tp.f0_stride, x_stride = tp.x_stride, bins = tp.fft_size / 2 + 1, fs = tp.fs;
-  const size_t in_row = (size_t)x_stride * (tp.nbit ? tp.nbit / 8 : 8), out_row = (size_t)tp.y_stride * (tp.nbit_out ? 2 : 8);
+  const ChainPlan &p = tp.chain;
+  const int f0_stride = p.f0_stride, x_stride = r.x_stride, fft_size = r.opt->cheaptrick.fft_size, nbit = r.nbit;
+  const size_t in_row = (size_t)x_stride * (nbit ? nbit / 8 : 8), out_row = (size_t)tp.y_stride * (tp.nbit_out ? 2 : 8);
   struct Rows {
     size_t x, t, f, sp, ap, total;
-    Rows(int m, const TransformPlan &tp, int bins) {
+    Rows(int m, int nbit, int x_stride, int f0_stride, int bins) {
       ArenaPlan a;
-      x = a.add(tp.nbit ? (size_t)m * tp.x_stride * 8 : 0);
-      t = a.add((size_t)m * tp.f0_stride * 8); f = a.add((size_t)m * tp.f0_stride * 8);
-      sp = a.add((size_t)m * tp.f0_stride * bins * 8); ap = a.add((size_t)m * tp.f0_stride * bins * 8);
+      x = a.add(nbit ? (size_t)m * x_stride * 8 : 0);
+      t = a.add((size_t)m * f0_stride * 8); f = a.add((size_t)m * f0_stride * 8);
+      sp = a.add((size_t)m * f0_stride * bins * 8); ap = a.add((size_t)m * f0_stride * bins * 8);
       total = a.total;
     }
   };
+  auto rows_of = [&](int m) { return Rows(m, nbit, x_stride, f0_stride, fft_size / 2 + 1); };
   int n_slices = 1;
   {
 #ifndef WB_EMU
@@ -1261,48 +1228,43 @@ int transform_run(WorldB200 *h, const TransformPlan &tp, const void *x, const in
     const bool two = false;
 #endif
     const double lane_budget = (double)h->c.scratch_budget / (two ? 2.0 : 1.0);
-    const int fit = (int)dmax(1.0, dmin((double)n, lane_budget / 2.0 / (double)Rows(1, tp, bins).total));
+    const int fit = (int)dmax(1.0, dmin((double)n, lane_budget / 2.0 / (double)rows_of(1).total));
     n_slices = (n + fit - 1) / fit;
     if (two) n_slices = imin(n, (n_slices + 1) / 2 * 2);   // an even count: both lanes get the same work
   }
   std::vector<int> bounds(n_slices + 1);
   for (int s = 0; s <= n_slices; ++s) bounds[s] = (int)((long long)n * s / n_slices);
   LaneScope lanes(h);
-  int rc = lanes.open(bounds, [&](int m) { return Rows(m, tp, bins).total; });
+  int rc = lanes.open(bounds, [&](int m) { return rows_of(m).total; });
   if (rc) return rc;
   // slice s: its lane, the global index of its first utterance, its size and where its rows are
   auto slice = [&](int s, WorldB200 **L, int *g, int *m, double **xs, double **t, double **f, double **sp, double **ap) {
-    const Rows r(lanes.most(s), tp, bins);
+    const Rows at = rows_of(lanes.most(s));
     unsigned char *rows = lanes.buffer(s);
     *L = lanes.lane(s); *g = u0 + bounds[s]; *m = bounds[s + 1] - bounds[s];
-    *xs = (double *)(rows + r.x); *t = (double *)(rows + r.t); *f = (double *)(rows + r.f);
-    *sp = (double *)(rows + r.sp); *ap = (double *)(rows + r.ap);
+    *xs = (double *)(rows + at.x); *t = (double *)(rows + at.t); *f = (double *)(rows + at.f);
+    *sp = (double *)(rows + at.sp); *ap = (double *)(rows + at.ap);
   };
   auto analyse = [&](int s) {
     WorldB200 *L; int g, m; double *xd, *t, *f, *sp, *ap;
     slice(s, &L, &g, &m, &xd, &t, &f, &sp, &ap);
-    const int *xl = x_lengths ? x_lengths + g : nullptr;
-    const int *fl = tp.f_len.data() + g;
     const unsigned char *xin = (const unsigned char *)x + (size_t)bounds[s] * in_row;
-    const double *xs = tp.nbit ? xd : (const double *)xin;
-    int e = tp.nbit ? world_b200_pcm_to_double_batch(L, xin, tp.nbit, m, x_stride, xl, xd) : 0;
+    const double *xs = nbit ? xd : (const double *)xin;
+    int e = nbit ? world_b200_pcm_to_double_batch(L, xin, nbit, m, x_stride, r.x_lengths ? r.x_lengths + g : nullptr, xd)
+                 : 0;
     if (!e) e = dev_memset(&L->c, t, 0, (size_t)m * f0_stride * 8);
     if (!e) e = dev_memset(&L->c, f, 0, (size_t)m * f0_stride * 8);
-    if (!e)
-      e = run_f0_stage(L, xs, m, x_stride, xl, fs, opt, harvest_options ? harvest_options + g : nullptr,
-                       dio_options ? dio_options + g : nullptr, fl, t, f, f0_stride);
-    if (!e) e = world_b200_cheaptrick_batch(L, xs, m, x_stride, xl, fs, t, f, fl, f0_stride, &opt->cheaptrick, sp);
-    if (!e)
-      e = world_b200_d4c_batch(L, xs, m, x_stride, xl, fs, t, f, fl, f0_stride, tp.fft_size, &opt->d4c, ap);
-    if (!e && tp.modify) e = modify_run(&L->c, tp.mod, g, m, fl, f0_stride, f, sp);
+    if (!e) e = chain_f0(L, r, p, g, m, xs, t, f);
+    if (!e) e = chain_spectral(L, r, p, g, m, xs, t, f, sp, ap);
+    if (!e && tp.modify) e = modify_run(&L->c, tp.mod, g, m, p.f_len.data() + g, f0_stride, f, sp);
     if (e && L != h) h->c.last_error = L->c.last_error;
     return e;
   };
   auto synthesise = [&](int s) {
     WorldB200 *L; int g, m; double *xd, *t, *f, *sp, *ap;
     slice(s, &L, &g, &m, &xd, &t, &f, &sp, &ap);
-    const int e = synthesis_run(&L->c, f, tp.f_len.data() + g, m, f0_stride, sp, ap, nullptr, tp.fft_size, tp.lg,
-                                tp.frame_period, fs, tp.y_len.data() + g, tp.y_stride,
+    const int e = synthesis_run(&L->c, f, p.f_len.data() + g, m, f0_stride, sp, ap, nullptr, fft_size, tp.lg,
+                                p.frame_period, r.fs, tp.y_len.data() + g, tp.y_stride,
                                 (unsigned char *)y + (size_t)bounds[s] * out_row, tp.nbit_out, nullptr, 0,
                                 tp.fp.data() + g);
     if (e && L != h) h->c.last_error = L->c.last_error;
@@ -1333,12 +1295,13 @@ int world_b200_transform_batch(WorldB200 *h, const void *x, int nbit, int n_utts
                                const double *time_scale, int nbit_out, void *y, int y_stride, int *y_lengths) {
   if (!h) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
+  ChainRequest r(x, nbit, n_utts, x_stride, x_lengths, fs, option, nullptr, nullptr, 0, nullptr, nullptr);
+  r.harvest_options = harvest_options; r.dio_options = dio_options;
   TransformPlan tp;
-  const int rc = transform_check(h, x, nbit, n_utts, x_stride, x_lengths, fs, option, harvest_options, dio_options,
-                                 f0_scale, spectral_ratio, time_scale, nbit_out, y, y_stride, "transform_batch", &tp);
+  const int rc = transform_check(h, r, f0_scale, spectral_ratio, time_scale, nbit_out, y, y_stride, "transform_batch", &tp);
   if (rc) return rc;
   if (y_lengths) std::copy(tp.y_len.begin(), tp.y_len.end(), y_lengths);
-  return transform_run(h, tp, x, x_lengths, option, harvest_options, dio_options, 0, n_utts, y);
+  return transform_run(h, r, tp, x, 0, n_utts, y);
 }
 
 // ---- multi-GPU (SURVEY.md 8e): utterances sharded over ranks, outputs reassembled on every rank by NCCL
@@ -1392,8 +1355,8 @@ int world_b200_allgather_rows(WorldB200 *h, double *full, unsigned long long row
 int world_b200_analyze_batch_allgather(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
                                        const WorldB200AnalysisOption *opt, double *time_axis_full, double *f0_full,
                                        int f0_stride, double *spectrogram_full, double *aperiodicity_full) {
-  return analyze_batch_impl(h, x, 0, n, x_stride, x_lengths, fs, opt, nullptr, nullptr, 0, time_axis_full, f0_full, f0_stride,
-                            spectrogram_full, aperiodicity_full, true);
+  return analyze_chain(h, ChainRequest(x, 0, n, x_stride, x_lengths, fs, opt, time_axis_full, f0_full, f0_stride,
+                                       spectrogram_full, aperiodicity_full), true);
 }
 
 int world_b200_analyze_batch_allgather_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
@@ -1402,8 +1365,10 @@ int world_b200_analyze_batch_allgather_options(WorldB200 *h, const double *x, in
                                                double *f0_full, int f0_stride, double *spectrogram_full,
                                                double *aperiodicity_full) {
   if (!harvest_options) return WORLD_B200_EINVAL;
-  return analyze_batch_impl(h, x, 0, n, x_stride, x_lengths, fs, opt, harvest_options, nullptr, 0, time_axis_full, f0_full,
-                            f0_stride, spectrogram_full, aperiodicity_full, true);
+  ChainRequest r(x, 0, n, x_stride, x_lengths, fs, opt, time_axis_full, f0_full, f0_stride, spectrogram_full,
+                 aperiodicity_full);
+  r.harvest_options = harvest_options;
+  return analyze_chain(h, r, true);
 }
 
 int world_b200_analyze_batch_allgather_dio_options(WorldB200 *h, const double *x, int n, int x_stride,
@@ -1412,33 +1377,19 @@ int world_b200_analyze_batch_allgather_dio_options(WorldB200 *h, const double *x
                                                    double *f0_full, int f0_stride, double *spectrogram_full,
                                                    double *aperiodicity_full) {
   if (!dio_options) return WORLD_B200_EINVAL;
-  return analyze_batch_impl(h, x, 0, n, x_stride, x_lengths, fs, opt, nullptr, dio_options, 0, time_axis_full, f0_full,
-                            f0_stride, spectrogram_full, aperiodicity_full, true);
+  ChainRequest r(x, 0, n, x_stride, x_lengths, fs, opt, time_axis_full, f0_full, f0_stride, spectrogram_full,
+                 aperiodicity_full);
+  r.dio_options = dio_options;
+  return analyze_chain(h, r, true);
 }
 
-// The device chain with coded rows out (and PCM or doubles in): the checks of analyze_coded_host, then the slices of
-// analyze_batch_impl with the fused coded frame kernels.
-static int analyze_coded_batch_impl(WorldB200 *h, const void *x, int nbit, int n, int x_stride, const int *x_lengths,
-                                    int fs, const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
-                                    const DioOption *dio_options, int number_of_dimensions, double *time_axis,
-                                    double *f0, int f0_stride, double *coded_spectral_envelope,
-                                    double *coded_aperiodicity, bool gather) {
-  if (!h || !opt) return WORLD_B200_EINVAL;
-  if (number_of_dimensions < 1 || number_of_dimensions > opt->cheaptrick.fft_size / 4 + 1) {
-    h->c.last_error = "analyze_coded_batch: number_of_dimensions must be in [1, fft_size/4 + 1]";
-    return WORLD_B200_EINVAL;
-  }
-  return analyze_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, harvest_options, dio_options,
-                            number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope, coded_aperiodicity,
-                            gather);
-}
-
+// The device chain with coded rows out (and PCM or doubles in): analyze_chain with the fused coded frame kernels.
 int world_b200_analyze_coded_batch(WorldB200 *h, const void *x, int nbit, int n, int x_stride, const int *x_lengths,
                                    int fs, const WorldB200AnalysisOption *opt, int number_of_dimensions,
                                    double *time_axis, double *f0, int f0_stride, double *coded_spectral_envelope,
                                    double *coded_aperiodicity) {
-  return analyze_coded_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, nullptr, nullptr, number_of_dimensions,
-                                  time_axis, f0, f0_stride, coded_spectral_envelope, coded_aperiodicity, false);
+  return analyze_chain(h, coded_request(x, nbit, n, x_stride, x_lengths, fs, opt, number_of_dimensions, time_axis, f0,
+                                        f0_stride, coded_spectral_envelope, coded_aperiodicity), false);
 }
 
 int world_b200_analyze_coded_batch_options(WorldB200 *h, const void *x, int nbit, int n, int x_stride,
@@ -1447,9 +1398,10 @@ int world_b200_analyze_coded_batch_options(WorldB200 *h, const void *x, int nbit
                                            double *time_axis, double *f0, int f0_stride,
                                            double *coded_spectral_envelope, double *coded_aperiodicity) {
   if (!harvest_options) return WORLD_B200_EINVAL;
-  return analyze_coded_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, harvest_options, nullptr,
-                                  number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope,
-                                  coded_aperiodicity, false);
+  ChainRequest r = coded_request(x, nbit, n, x_stride, x_lengths, fs, opt, number_of_dimensions, time_axis, f0,
+                                 f0_stride, coded_spectral_envelope, coded_aperiodicity);
+  r.harvest_options = harvest_options;
+  return analyze_chain(h, r, false);
 }
 
 int world_b200_analyze_coded_batch_dio_options(WorldB200 *h, const void *x, int nbit, int n, int x_stride,
@@ -1458,9 +1410,10 @@ int world_b200_analyze_coded_batch_dio_options(WorldB200 *h, const void *x, int 
                                                double *time_axis, double *f0, int f0_stride,
                                                double *coded_spectral_envelope, double *coded_aperiodicity) {
   if (!dio_options) return WORLD_B200_EINVAL;
-  return analyze_coded_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, nullptr, dio_options,
-                                  number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope,
-                                  coded_aperiodicity, false);
+  ChainRequest r = coded_request(x, nbit, n, x_stride, x_lengths, fs, opt, number_of_dimensions, time_axis, f0,
+                                 f0_stride, coded_spectral_envelope, coded_aperiodicity);
+  r.dio_options = dio_options;
+  return analyze_chain(h, r, false);
 }
 
 int world_b200_analyze_coded_batch_spectral_options(WorldB200 *h, const void *x, int nbit, int n, int x_stride,
@@ -1470,14 +1423,11 @@ int world_b200_analyze_coded_batch_spectral_options(WorldB200 *h, const void *x,
                                                     const D4COption *d4c_options, int number_of_dimensions,
                                                     double *time_axis, double *f0, int f0_stride,
                                                     double *coded_spectral_envelope, double *coded_aperiodicity) {
-  if (!h || !opt || number_of_dimensions < 1) return WORLD_B200_EINVAL;
-  if (!cheaptrick_options && !d4c_options)   // the per-call CheapTrick option: analyze_coded_batch's rules
-    return analyze_coded_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, harvest_options, dio_options,
-                                    number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope,
-                                    coded_aperiodicity, false);
-  return analyze_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, harvest_options, dio_options,
-                            number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope, coded_aperiodicity,
-                            false, cheaptrick_options, d4c_options);
+  ChainRequest r = coded_request(x, nbit, n, x_stride, x_lengths, fs, opt, number_of_dimensions, time_axis, f0,
+                                 f0_stride, coded_spectral_envelope, coded_aperiodicity);
+  r.harvest_options = harvest_options; r.dio_options = dio_options;
+  r.cheaptrick_options = cheaptrick_options; r.d4c_options = d4c_options;
+  return analyze_chain(h, r, false);
 }
 
 int world_b200_analyze_coded_batch_allgather(WorldB200 *h, const void *x, int nbit, int n, int x_stride,
@@ -1485,9 +1435,8 @@ int world_b200_analyze_coded_batch_allgather(WorldB200 *h, const void *x, int nb
                                              int number_of_dimensions, double *time_axis_full, double *f0_full,
                                              int f0_stride, double *coded_spectral_envelope_full,
                                              double *coded_aperiodicity_full) {
-  return analyze_coded_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, nullptr, nullptr, number_of_dimensions,
-                                  time_axis_full, f0_full, f0_stride, coded_spectral_envelope_full,
-                                  coded_aperiodicity_full, true);
+  return analyze_chain(h, coded_request(x, nbit, n, x_stride, x_lengths, fs, opt, number_of_dimensions, time_axis_full,
+                                        f0_full, f0_stride, coded_spectral_envelope_full, coded_aperiodicity_full), true);
 }
 
 int world_b200_analyze_coded_batch_allgather_options(WorldB200 *h, const void *x, int nbit, int n, int x_stride,
@@ -1497,9 +1446,10 @@ int world_b200_analyze_coded_batch_allgather_options(WorldB200 *h, const void *x
                                                      double *coded_spectral_envelope_full,
                                                      double *coded_aperiodicity_full) {
   if (!harvest_options) return WORLD_B200_EINVAL;
-  return analyze_coded_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, harvest_options, nullptr,
-                                  number_of_dimensions, time_axis_full, f0_full, f0_stride,
-                                  coded_spectral_envelope_full, coded_aperiodicity_full, true);
+  ChainRequest r = coded_request(x, nbit, n, x_stride, x_lengths, fs, opt, number_of_dimensions, time_axis_full,
+                                 f0_full, f0_stride, coded_spectral_envelope_full, coded_aperiodicity_full);
+  r.harvest_options = harvest_options;
+  return analyze_chain(h, r, true);
 }
 
 int world_b200_analyze_coded_batch_allgather_dio_options(WorldB200 *h, const void *x, int nbit, int n, int x_stride,
@@ -1510,9 +1460,10 @@ int world_b200_analyze_coded_batch_allgather_dio_options(WorldB200 *h, const voi
                                                          double *coded_spectral_envelope_full,
                                                          double *coded_aperiodicity_full) {
   if (!dio_options) return WORLD_B200_EINVAL;
-  return analyze_coded_batch_impl(h, x, nbit, n, x_stride, x_lengths, fs, opt, nullptr, dio_options,
-                                  number_of_dimensions, time_axis_full, f0_full, f0_stride,
-                                  coded_spectral_envelope_full, coded_aperiodicity_full, true);
+  ChainRequest r = coded_request(x, nbit, n, x_stride, x_lengths, fs, opt, number_of_dimensions, time_axis_full,
+                                 f0_full, f0_stride, coded_spectral_envelope_full, coded_aperiodicity_full);
+  r.dio_options = dio_options;
+  return analyze_chain(h, r, true);
 }
 
 // Per-kernel timing: enable, run, then fetch a JSON object {"kernel": {"launches": n, "ms": t}, ...}

@@ -1,0 +1,104 @@
+// wb_chain.h -- the context behind the C ABI's handle, and the analysis chain that the device drivers (wb_api.cu) and the
+// host pipelines (wb_host.cu) share: one checked plan per call, one stage sequence per slice or chunk.
+#pragma once
+#include "wb_internal.h"
+#include "../../include/world_b200.h"
+
+struct WorldB200 {
+  wb::Ctx c;
+  int *lens_dev = nullptr;
+  size_t lens_cap = 0;
+  // world_b200_analyze_batch: two sibling contexts ("lanes"), each with its own stream, scratch arena and staging
+  // ring, created on first use; fork / join events order them against this context's stream
+  WorldB200 *lane[2] = {nullptr, nullptr};
+  void *lane_stream[2] = {nullptr, nullptr};   // cudaStream_t
+  void *ev_fork = nullptr, *ev_join[2] = {nullptr, nullptr};   // cudaEvent_t
+  // multi-GPU (wb_multi.cu): NCCL communicator + one event per utterance slice of analyze_batch_allgather
+  wb::Comm *comm = nullptr;
+  std::vector<void *> ev_slice;
+};
+
+namespace wb {
+
+// What an analysis entry point receives.  x: n rows of x_stride samples, doubles (nbit 0) or little-endian PCM.  The
+// per-utterance option arrays may be NULL (the AnalysisOption's own option for every utterance); at most one of the two
+// F0 arrays, and the spectral arrays only with coded rows.  coded: spectrogram / aperiodicity receive dims /
+// GetNumberOfAperiodicities(fs) coded values per frame instead of fft_size / 2 + 1 bins.  A NULL spectrogram or
+// aperiodicity skips its stage.  f0_stride 0: a call with no analysis outputs (transform), whose rows are as long as its
+// longest utterance's frame count.
+struct ChainRequest {
+  ChainRequest(const void *x, int nbit, int n, int x_stride, const int *x_lengths, int fs,
+               const WorldB200AnalysisOption *opt, double *time_axis, double *f0, int f0_stride, double *spectrogram,
+               double *aperiodicity)
+      : x(x), nbit(nbit), n(n), x_stride(x_stride), x_lengths(x_lengths), fs(fs), opt(opt), time_axis(time_axis),
+        f0(f0), f0_stride(f0_stride), spectrogram(spectrogram), aperiodicity(aperiodicity) {}
+  const void *x;
+  int nbit, n, x_stride;
+  const int *x_lengths;
+  int fs;
+  const WorldB200AnalysisOption *opt;
+  double *time_axis, *f0;
+  int f0_stride;
+  double *spectrogram, *aperiodicity;
+  bool coded = false;
+  int dims = 0;
+  const HarvestOption *harvest_options = nullptr;
+  const DioOption *dio_options = nullptr;
+  const CheapTrickOption *cheaptrick_options = nullptr;
+  const D4COption *d4c_options = nullptr;
+};
+
+// The request of a coded-row entry point: number_of_dimensions coded values per spectral frame.
+inline ChainRequest coded_request(const void *x, int nbit, int n, int x_stride, const int *x_lengths, int fs,
+                                  const WorldB200AnalysisOption *opt, int number_of_dimensions, double *time_axis,
+                                  double *f0, int f0_stride, double *coded_spectral_envelope,
+                                  double *coded_aperiodicity) {
+  ChainRequest r(x, nbit, n, x_stride, x_lengths, fs, opt, time_axis, f0, f0_stride, coded_spectral_envelope,
+                 coded_aperiodicity);
+  r.coded = true;
+  r.dims = number_of_dimensions;
+  return r;
+}
+
+struct ChainPlan {
+  double frame_period = 0.0;            // ms, of the chain's F0 method
+  std::vector<int> f_len;               // [n] frames of each utterance
+  int f0_stride = 0;                    // the request's, or (f0_stride 0) the largest frame count
+  size_t sp_row = 0, ap_row = 0;        // doubles per frame of the spectrogram / aperiodicity rows
+  bool want_sp = false, want_ap = false;   // CheapTrick / D4C run (coded rows below 12 kHz have no bands: no D4C)
+  // with per-utterance spectral options (empty otherwise): each utterance's CheapTrick option, and D4C's fft_size (the
+  // utterance's CheapTrick size) and option
+  std::vector<CheapTrickOption> cts;
+  std::vector<int> d4_fft;
+  std::vector<D4COption> d4s;
+};
+
+// Every check of an analysis chain, before anything is queued: EINVAL with last_error "<who>: ...", naming the first
+// bad utterance where there is one.  Fills the plan that chain_f0 / chain_spectral and the drivers read.
+int chain_plan(Ctx *c, const ChainRequest &r, const char *who, ChainPlan *p);
+// The chain's stages for utterances [u0, u0 + m) of a planned request, enqueued on h (a lane, or the pipeline's
+// context): x, time_axis, f0, sp and ap are device rows that start at utterance u0.  chain_f0: Harvest, or DIO +
+// StoneMask.  chain_spectral: CheapTrick into sp, then D4C into ap; a NULL sp or ap skips that stage.
+int chain_f0(WorldB200 *h, const ChainRequest &r, const ChainPlan &p, int u0, int m, const double *x, double *time_axis,
+             double *f0);
+int chain_spectral(WorldB200 *h, const ChainRequest &r, const ChainPlan &p, int u0, int m, const double *x,
+                   const double *time_axis, const double *f0, double *sp, double *ap);
+
+// Voice transformation (world_b200_transform_*): the analysis plan of the request (full rows, no spectral options, no
+// analysis outputs) and what synthesis adds to it.  transform_check makes it once per call; transform_run (device rows)
+// and the host pipeline (wb_host.cu) read it.
+struct TransformPlan {
+  ChainPlan chain;
+  int nbit_out = 0, y_stride = 0, lg = 0;
+  std::vector<int> y_len;          // [n] output samples of each utterance
+  std::vector<double> fp;          // [n] synthesis frame period (s): (frame_period * time_scale[u]) / 1000.0
+  bool modify = false;             // f0_scale or spectral_ratio given
+  ModifyPlan mod;
+};
+int transform_check(WorldB200 *h, const ChainRequest &r, const double *f0_scale, const double *spectral_ratio,
+                    const double *time_scale, int nbit_out, const void *y, int y_stride, const char *who,
+                    TransformPlan *tp);
+// Utterances [u0, u0 + n) of a checked call: x and y point at utterance u0's rows (device).
+int transform_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, const void *x, int u0, int n, void *y);
+
+}  // namespace wb

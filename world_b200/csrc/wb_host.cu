@@ -7,8 +7,7 @@
 //     src/world/*.h) as n_utts = 1 batches on a lazily created process-wide context, so existing
 //     callers relink unchanged.  They keep the reference's `void` signature; failures are
 //     reported on stderr and leave the outputs zero-filled.
-#include "wb_internal.h"
-#include "../../include/world_b200.h"
+#include "wb_chain.h"
 #include <stdio.h>
 #include <stdlib.h>
 #include <vector>
@@ -20,32 +19,7 @@
 
 using namespace wb;
 
-namespace wb {
-// wb_api.cu: checks of per-utterance F0 options for a chain, and the chain's F0 stage
-int check_chain_f0_options(Ctx *c, const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
-                           const DioOption *dio_options, int n, int fs, const char *who);
-int run_f0_stage(WorldB200 *h, const double *x, int m, int x_stride, const int *x_lengths, int fs,
-                 const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options, const DioOption *dio_options,
-                 const int *f0_lengths, double *time_axis, double *f0, int f0_stride);
-// wb_api.cu: per-utterance spectral options of a coded chain, expanded to every utterance and checked
-int chain_spectral_options(Ctx *c, int fs, int dims, const WorldB200AnalysisOption *opt,
-                           const CheapTrickOption *ct_options, const D4COption *d4c_options, int n,
-                           bool spectral_envelope, bool aperiodicity, std::vector<CheapTrickOption> *cts,
-                           std::vector<int> *d4_fft, std::vector<D4COption> *d4s);
-// wb_api.cu: the checks and plan of a voice transformation, and its device driver over utterances [u0, u0 + n)
-int transform_check(WorldB200 *h, const void *x, int nbit, int n, int x_stride, const int *x_lengths, int fs,
-                    const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
-                    const DioOption *dio_options, const double *f0_scale, const double *spectral_ratio,
-                    const double *time_scale, int nbit_out, const void *y, int y_stride, const char *who,
-                    TransformPlan *tp);
-int transform_run(WorldB200 *h, const TransformPlan &tp, const void *x, const int *x_lengths,
-                  const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
-                  const DioOption *dio_options, int u0, int n, void *y);
-}  // namespace wb
-
 namespace {
-
-Ctx *ctx_of(WorldB200 *h) { return reinterpret_cast<Ctx *>(h); }  // Ctx is the first member
 
 // The scaffold of the host pipelines: uploads on s_in, kernels on the context's stream, downloads on s_out, the events
 // that order buffer reuse between the three, the pipeline's pooled device buffers and the WB_HOST_TRACE timeline.  On
@@ -59,7 +33,7 @@ class HostPipe {
   enum Stream { IN, RUN, OUT };
 
   HostPipe(WorldB200 *h, const char *who)
-      : ctx_(ctx_of(h)), who_(who), trace_(getenv("WB_HOST_TRACE") != nullptr), t0_(std::chrono::steady_clock::now()) {}
+      : ctx_(&h->c), who_(who), trace_(getenv("WB_HOST_TRACE") != nullptr), t0_(std::chrono::steady_clock::now()) {}
   HostPipe(const HostPipe &) = delete;
   HostPipe &operator=(const HostPipe &) = delete;
   ~HostPipe() { close(); }
@@ -227,23 +201,25 @@ class HostPipe {
 // on SUB-chunks (default 128 utterances) whose rows start their trip over PCIe as soon as they exist: the
 // un-overlapped tail is one sub-chunk.  Result buffers form a ring two outer chunks deep, so downloads
 // may lag behind the frame kernels and catch up under the next outer chunk's F0 stage.  Streams and events: HostPipe.
-// harvest_options / dio_options: nullptr, or one option per utterance (checked by the caller, at most one of the two);
-// the outer chunks split the array.  cts / d4_fft / d4s (coded rows only): nullptr, or every utterance's CheapTrick
-// option and D4C fft_size / option (chain_spectral_options).
-int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride, const int *x_lengths, int fs,
-                     const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
-                     const DioOption *dio_options, int dims, double *time_axis, double *f0, int f0_stride,
-                     double *out_sp, double *out_ap, const CheapTrickOption *cts = nullptr,
-                     const int *d4_fft = nullptr, const D4COption *d4s = nullptr) {
-  Ctx *ctx = ctx_of(h);
-  const int bins = opt->cheaptrick.fft_size / 2 + 1;
-  const int n_ap = GetNumberOfAperiodicities(fs);
+// The whole request is checked (chain_plan) before the first upload; the per-utterance option arrays are split with the
+// outer chunks.  time_axis and f0 may be NULL: they are computed on the device and not downloaded.
+int analyze_pipeline(WorldB200 *h, const ChainRequest &r) {
+  if (!h) return WORLD_B200_EINVAL;
+  DeviceGuard guard_(&h->c);
+  Ctx *ctx = &h->c;
+  const char *who = r.coded ? "analyze_coded_host" : "analyze_host";
+  if (r.f0_stride <= 0) {
+    ctx->last_error = std::string(who) + ": f0_stride must be > 0";
+    return WORLD_B200_EINVAL;
+  }
+  ChainPlan plan;
+  int rc = chain_plan(ctx, r, who, &plan);
+  if (rc || r.n == 0) return rc;
+  const int n_utts = r.n, nbit = r.nbit, x_stride = r.x_stride, f0_stride = r.f0_stride;
   const size_t in_bytes = nbit ? (size_t)(nbit / 8) : 8;
-  const size_t sp_row = dims ? (size_t)dims : (size_t)bins, ap_row = dims ? (size_t)n_ap : (size_t)bins;
-  const double frame_period =
-      opt->f0_method == WORLD_B200_F0_HARVEST ? opt->harvest.frame_period : opt->dio.frame_period;
-  const bool want_sp = out_sp != nullptr, want_ap = out_ap != nullptr && (!dims || n_ap > 0);
-  if (n_utts == 0) return 0;
+  const size_t sp_row = plan.sp_row, ap_row = plan.ap_row;
+  const bool want_sp = plan.want_sp, want_ap = plan.want_ap;
+  double *time_axis = r.time_axis, *f0 = r.f0, *out_sp = r.spectrogram, *out_ap = r.aperiodicity;
 
   int sub = 128, outer = 512;
   if (const char *e = getenv("WB_HOST_SUB")) sub = atoi(e) > 0 ? atoi(e) : sub;
@@ -268,7 +244,7 @@ int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_st
   enum { EV_IN = 0, EV_CDONE = 2, EV_F0 = 4, EV_TF = 6, EV_SUB_DONE = 8 };
   const int ev_sub_out = EV_SUB_DONE + ring;
   HostPipe p(h, "analyze");
-  int rc = p.open(EV_SUB_DONE + 2 * ring);
+  rc = p.open(EV_SUB_DONE + 2 * ring);
   if (rc) return rc;
   unsigned char *din[2] = {nullptr, nullptr};
   double *dx[2] = {nullptr, nullptr}, *dt[2] = {nullptr, nullptr}, *df[2] = {nullptr, nullptr};
@@ -284,32 +260,26 @@ int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_st
     if (want_sp) rc = p.buffer((size_t)sub * f0_stride * sp_row * 8, &dsp[i]);
     if (!rc && want_ap) rc = p.buffer((size_t)sub * f0_stride * ap_row * 8, &dap[i]);
   }
-  std::vector<int> flen(n_utts);
-  for (int i = 0; i < n_utts && !rc; ++i) {
-    flen[i] = world_b200_frames(fs, x_lengths ? x_lengths[i] : x_stride, frame_period);
-    if (flen[i] > f0_stride) { ctx->last_error = "f0_stride too small"; rc = WORLD_B200_EINVAL; }
-  }
   int it = 0, g = 0;   // outer chunk counter, global sub-chunk counter
   for (int u0 = 0; u0 < n_utts && !rc; u0 += outer, ++it) {
     const int n = imin(outer, n_utts - u0);
     const int s = it & 1;
-    const int *xl = x_lengths ? x_lengths + u0 : nullptr;
-    const int *fl = flen.data() + u0;
+    const int *fl = plan.f_len.data() + u0;
     const size_t fsz = (size_t)n * f0_stride;
     if (it >= 2) p.wait(HostPipe::IN, EV_CDONE + s);   // kernels of outer chunk it-2 read din[s] / dx[s]
-    p.h2d(din[s], (const unsigned char *)x + (size_t)u0 * x_stride * in_bytes, (size_t)n * x_stride * in_bytes);
+    p.h2d(din[s], (const unsigned char *)r.x + (size_t)u0 * x_stride * in_bytes, (size_t)n * x_stride * in_bytes);
     p.record(EV_IN + s, HostPipe::IN);
     p.mark("h2d_done", it, HostPipe::IN);
     p.wait(HostPipe::RUN, EV_IN + s);
     if (it >= 2) p.wait(HostPipe::RUN, EV_TF + s);   // time_axis / f0 of it-2 are on the host
     p.mark("f0_begin", it, HostPipe::RUN);
-    if (nbit) rc = world_b200_pcm_to_double_batch(h, din[s], nbit, n, x_stride, xl, dx[s]);
+    if (nbit)
+      rc = world_b200_pcm_to_double_batch(h, din[s], nbit, n, x_stride, r.x_lengths ? r.x_lengths + u0 : nullptr, dx[s]);
     if (rc) break;
     dev_memset(ctx, dt[s], 0, fsz * 8);
     dev_memset(ctx, df[s], 0, fsz * 8);
     const double *xd = nbit ? dx[s] : (const double *)din[s];
-    rc = run_f0_stage(h, xd, n, x_stride, xl, fs, opt, harvest_options ? harvest_options + u0 : nullptr,
-                      dio_options ? dio_options + u0 : nullptr, fl, dt[s], df[s], f0_stride);
+    rc = chain_f0(h, r, plan, u0, n, xd, dt[s], df[s]);
     if (rc) break;
     p.record(EV_F0 + s, HostPipe::RUN);
     p.mark("f0_end", it, HostPipe::RUN);
@@ -322,14 +292,13 @@ int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_st
     // critical path, finishing (first sub-chunk's compute + every download) after the chunk's Harvest -- ~50 ms behind
     // the kernels of a 850 ms step at 1024 x 10 s with sub-chunks of 128.  Quarter-size sub-chunks there start the
     // downloads earlier and leave a shorter last one (~25 ms behind).
-    const bool taper = !dims && u0 + outer >= n_utts;
+    const bool taper = !r.coded && u0 + outer >= n_utts;
     int taper_min = 16;   // (WB_HOST_TAPER_MIN: tests exercise the path with a handful of utterances)
     if (const char *e = getenv("WB_HOST_TAPER_MIN")) taper_min = imax(1, atoi(e));
     const int sub_here = taper ? imax(imin(sub, taper_min), sub / 4) : sub;
     for (int v0 = 0; v0 < n && !rc && (want_sp || want_ap); v0 += sub_here, ++g) {
       const int m = imin(sub_here, n - v0);
       const int slot = g % ring;
-      const int *sxl = xl ? xl + v0 : nullptr;
       const int *sfl = fl + v0;
       const size_t ssz = (size_t)m * f0_stride;
       const double *sx = xd + (size_t)v0 * x_stride, *st = dt[s] + (size_t)v0 * f0_stride, *sf = df[s] + (size_t)v0 * f0_stride;
@@ -341,29 +310,8 @@ int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_st
         if (want_sp) dev_memset(ctx, dsp[slot], 0, ssz * sp_row * 8);
         if (want_ap) dev_memset(ctx, dap[slot], 0, ssz * ap_row * 8);
       }
-      if (dims && cts) {
-        const int w = u0 + v0;
-        if (want_sp)
-          rc = world_b200_cheaptrick_coded_batch_options(h, sx, m, x_stride, sxl, fs, st, sf, sfl, f0_stride, cts + w,
-                                                         dims, dsp[slot]);
-        if (!rc && want_ap)
-          rc = world_b200_d4c_coded_batch_options(h, sx, m, x_stride, sxl, fs, st, sf, sfl, f0_stride, d4_fft + w,
-                                                  d4s + w, dap[slot]);
-      } else if (dims) {
-        if (want_sp)
-          rc = world_b200_cheaptrick_coded_batch(h, sx, m, x_stride, sxl, fs, st, sf, sfl, f0_stride, &opt->cheaptrick,
-                                                 dims, dsp[slot]);
-        if (!rc && want_ap)
-          rc = world_b200_d4c_coded_batch(h, sx, m, x_stride, sxl, fs, st, sf, sfl, f0_stride,
-                                          opt->cheaptrick.fft_size, &opt->d4c, dap[slot]);
-      } else {
-        if (want_sp)
-          rc = world_b200_cheaptrick_batch(h, sx, m, x_stride, sxl, fs, st, sf, sfl, f0_stride, &opt->cheaptrick,
-                                           dsp[slot]);
-        if (!rc && want_ap)
-          rc = world_b200_d4c_batch(h, sx, m, x_stride, sxl, fs, st, sf, sfl, f0_stride, opt->cheaptrick.fft_size,
-                                    &opt->d4c, dap[slot]);
-      }
+      rc = chain_spectral(h, r, plan, u0 + v0, m, sx, st, sf, want_sp ? dsp[slot] : nullptr,
+                          want_ap ? dap[slot] : nullptr);
       if (rc) break;
       const size_t row0 = (size_t)(u0 + v0) * f0_stride;
       p.record(EV_SUB_DONE + slot, HostPipe::RUN);
@@ -392,7 +340,7 @@ int analyze_pipeline(WorldB200 *h, const void *x, int nbit, int n_utts, int x_st
 template <class Upload, class Run>
 int chunk_pipeline(WorldB200 *h, const char *who, int n_utts, int chunk, int ring, size_t in_bytes, size_t out_row,
                    const int *y_len, int y_stride, int nbit, void *y, Upload upload, Run run) {
-  Ctx *ctx = ctx_of(h);
+  Ctx *ctx = &h->c;
   const int n_chunks = (n_utts + chunk - 1) / chunk;
   ring = imin(ring, n_chunks);
   enum { EV_IN = 0, EV_CDONE = 2, EV_OUT = 4 };   // two input buffers, then `ring` output slots
@@ -446,7 +394,7 @@ int chunk_pipeline(WorldB200 *h, const char *who, int n_utts, int chunk, int rin
 int synthesis_pipeline(WorldB200 *h, CodedRows *coded, int lg, const double *f0, const int *f0_lengths, int n_utts,
                        int f0_stride, int fft_size, double frame_period, int fs, const int *y_lengths, int y_stride,
                        const int *lens, int nbit, void *y, const ModifyPlan *mod) {
-  Ctx *ctx = ctx_of(h);
+  Ctx *ctx = &h->c;
   const int dims = coded->tsp.dims, n_ap = coded->tap.dims;
   const double *h_sp = coded->sp, *h_ap = coded->ap;
   const size_t out_bytes = nbit ? 2 : 8;
@@ -487,11 +435,10 @@ int synthesis_pipeline(WorldB200 *h, CodedRows *coded, int lg, const double *f0,
 // Voice transformation for host arrays: chunks of PCM in, transform_run on each chunk (which forks from and joins back
 // to the context's stream), output rows out, through chunk_pipeline with two output slots.  Chunks of WB_HOST_CHUNK
 // utterances (default 512), fewer when the four buffers would take more than a sixth of the scratch budget.
-int transform_pipeline(WorldB200 *h, const TransformPlan &tp, const void *x, int n_utts, const int *x_lengths,
-                       const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
-                       const DioOption *dio_options, void *y) {
-  Ctx *ctx = ctx_of(h);
-  const size_t per_in = (size_t)tp.x_stride * (tp.nbit ? tp.nbit / 8 : 8);
+int transform_pipeline(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, void *y) {
+  Ctx *ctx = &h->c;
+  const int n_utts = r.n;
+  const size_t per_in = (size_t)r.x_stride * (r.nbit ? r.nbit / 8 : 8);
   const size_t per_out = (size_t)tp.y_stride * (tp.nbit_out ? 2 : 8);
   int chunk = 512;
   if (const char *e = getenv("WB_HOST_CHUNK")) chunk = atoi(e) > 0 ? atoi(e) : chunk;
@@ -499,10 +446,10 @@ int transform_pipeline(WorldB200 *h, const TransformPlan &tp, const void *x, int
   chunk = balanced_chunk(n_utts, chunk);
   // chunk k's PCM rows
   auto upload = [&](HostPipe &p, int u0, int m, unsigned char *d) {
-    p.h2d(d, (const unsigned char *)x + (size_t)u0 * per_in, (size_t)m * per_in);
+    p.h2d(d, (const unsigned char *)r.x + (size_t)u0 * per_in, (size_t)m * per_in);
   };
   auto run = [&](int u0, int m, unsigned char *d, unsigned char *out) {
-    return transform_run(h, tp, d, x_lengths, opt, harvest_options, dio_options, u0, m, out);
+    return transform_run(h, r, tp, d, u0, m, out);
   };
   return chunk_pipeline(h, "transform", n_utts, chunk, 2, (size_t)chunk * per_in, per_out, tp.y_len.data(), tp.y_stride,
                         tp.nbit_out, y, upload, run);
@@ -516,8 +463,8 @@ int synthesis_coded_host(WorldB200 *h, const double *f0, const int *f0_lengths, 
                          const double *spectral_ratio) {
   if (!h || !f0 || !coded_spectral_envelope || !y || n_utts < 0 || fs <= 0 || frame_period <= 0)
     return WORLD_B200_EINVAL;
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  Ctx *ctx = ctx_of(h);
+  DeviceGuard guard_(&h->c);
+  Ctx *ctx = &h->c;
   if (nbit != 0 && nbit != 16) {
     ctx->last_error = "synthesis_coded_host: nbit must be 0 (double) or 16 (int16)";
     return WORLD_B200_EINVAL;
@@ -574,37 +521,23 @@ extern "C" int world_b200_transform_host(WorldB200 *h, const void *x, int nbit, 
                                          const double *time_scale, int nbit_out, void *y, int y_stride,
                                          int *y_lengths) {
   if (!h) return WORLD_B200_EINVAL;
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
+  DeviceGuard guard_(&h->c);
+  ChainRequest r(x, nbit, n_utts, x_stride, x_lengths, fs, option, nullptr, nullptr, 0, nullptr, nullptr);
+  r.harvest_options = harvest_options; r.dio_options = dio_options;
   TransformPlan tp;
-  const int rc = transform_check(h, x, nbit, n_utts, x_stride, x_lengths, fs, option, harvest_options, dio_options,
-                                 f0_scale, spectral_ratio, time_scale, nbit_out, y, y_stride, "transform_host", &tp);
+  const int rc = transform_check(h, r, f0_scale, spectral_ratio, time_scale, nbit_out, y, y_stride, "transform_host", &tp);
   if (rc) return rc;
   if (y_lengths) std::copy(tp.y_len.begin(), tp.y_len.end(), y_lengths);
   if (n_utts == 0) return 0;
-  return transform_pipeline(h, tp, x, n_utts, x_lengths, option, harvest_options, dio_options, y);
+  return transform_pipeline(h, r, tp, y);
 }
 
 extern "C" int world_b200_analyze_host(WorldB200 *h, const double *x, int n_utts, int x_stride,
                                        const int *x_lengths, int fs, const WorldB200AnalysisOption *opt,
                                        double *time_axis, double *f0, int f0_stride, double *spectrogram,
                                        double *aperiodicity) {
-  if (!h || !x || !opt || n_utts < 0 || fs <= 0 || x_stride <= 0 || f0_stride <= 0) return WORLD_B200_EINVAL;
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  return analyze_pipeline(h, x, 0, n_utts, x_stride, x_lengths, fs, opt, nullptr, nullptr, 0, time_axis, f0, f0_stride,
-                          spectrogram, aperiodicity);
-}
-
-// analyze_host with per-utterance options of one F0 method (harvest_options or dio_options)
-static int analyze_host_per_utt(WorldB200 *h, const double *x, int n_utts, int x_stride, const int *x_lengths, int fs,
-                                const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
-                                const DioOption *dio_options, double *time_axis, double *f0, int f0_stride,
-                                double *spectrogram, double *aperiodicity) {
-  if (!h || !x || !opt || n_utts < 0 || fs <= 0 || x_stride <= 0 || f0_stride <= 0) return WORLD_B200_EINVAL;
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  const int rc = check_chain_f0_options(ctx_of(h), opt, harvest_options, dio_options, n_utts, fs, "analyze_host");
-  if (rc) return rc;
-  return analyze_pipeline(h, x, 0, n_utts, x_stride, x_lengths, fs, opt, harvest_options, dio_options, 0, time_axis, f0,
-                          f0_stride, spectrogram, aperiodicity);
+  return analyze_pipeline(h, ChainRequest(x, 0, n_utts, x_stride, x_lengths, fs, opt, time_axis, f0, f0_stride,
+                                          spectrogram, aperiodicity));
 }
 
 extern "C" int world_b200_analyze_host_options(WorldB200 *h, const double *x, int n_utts, int x_stride,
@@ -612,8 +545,9 @@ extern "C" int world_b200_analyze_host_options(WorldB200 *h, const double *x, in
                                                const HarvestOption *harvest_options, double *time_axis, double *f0,
                                                int f0_stride, double *spectrogram, double *aperiodicity) {
   if (!harvest_options) return WORLD_B200_EINVAL;
-  return analyze_host_per_utt(h, x, n_utts, x_stride, x_lengths, fs, opt, harvest_options, nullptr, time_axis, f0,
-                              f0_stride, spectrogram, aperiodicity);
+  ChainRequest r(x, 0, n_utts, x_stride, x_lengths, fs, opt, time_axis, f0, f0_stride, spectrogram, aperiodicity);
+  r.harvest_options = harvest_options;
+  return analyze_pipeline(h, r);
 }
 
 extern "C" int world_b200_analyze_host_dio_options(WorldB200 *h, const double *x, int n_utts, int x_stride,
@@ -621,27 +555,9 @@ extern "C" int world_b200_analyze_host_dio_options(WorldB200 *h, const double *x
                                                    const DioOption *dio_options, double *time_axis, double *f0,
                                                    int f0_stride, double *spectrogram, double *aperiodicity) {
   if (!dio_options) return WORLD_B200_EINVAL;
-  return analyze_host_per_utt(h, x, n_utts, x_stride, x_lengths, fs, opt, nullptr, dio_options, time_axis, f0,
-                              f0_stride, spectrogram, aperiodicity);
-}
-
-// analyze_coded_host with per-utterance options of one F0 method, or none (both nullptr)
-static int analyze_coded_host_impl(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride, const int *x_lengths,
-                                   int fs, const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
-                                   const DioOption *dio_options, int number_of_dimensions, double *time_axis,
-                                   double *f0, int f0_stride, double *coded_spectral_envelope,
-                                   double *coded_aperiodicity) {
-  if (!h || !x || !opt || n_utts < 0 || fs <= 0 || x_stride <= 0 || f0_stride <= 0) return WORLD_B200_EINVAL;
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  if (nbit != 0 && nbit != 8 && nbit != 16 && nbit != 24 && nbit != 32) return WORLD_B200_EINVAL;
-  if (number_of_dimensions < 1 || number_of_dimensions > opt->cheaptrick.fft_size / 4 + 1) {
-    ctx_of(h)->last_error = "analyze_coded_host: number_of_dimensions must be in [1, fft_size/4 + 1]";
-    return WORLD_B200_EINVAL;
-  }
-  const int rc = check_chain_f0_options(ctx_of(h), opt, harvest_options, dio_options, n_utts, fs, "analyze_coded_host");
-  if (rc) return rc;
-  return analyze_pipeline(h, x, nbit, n_utts, x_stride, x_lengths, fs, opt, harvest_options, dio_options,
-                          number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope, coded_aperiodicity);
+  ChainRequest r(x, 0, n_utts, x_stride, x_lengths, fs, opt, time_axis, f0, f0_stride, spectrogram, aperiodicity);
+  r.dio_options = dio_options;
+  return analyze_pipeline(h, r);
 }
 
 // analyze_coded_host with per-utterance CheapTrick / D4C options (either array may be NULL) and F0 options as above
@@ -650,34 +566,19 @@ extern "C" int world_b200_analyze_coded_host_spectral_options(
     const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options, const DioOption *dio_options,
     const CheapTrickOption *cheaptrick_options, const D4COption *d4c_options, int number_of_dimensions,
     double *time_axis, double *f0, int f0_stride, double *coded_spectral_envelope, double *coded_aperiodicity) {
-  if (!cheaptrick_options && !d4c_options)
-    return analyze_coded_host_impl(h, x, nbit, n_utts, x_stride, x_lengths, fs, opt, harvest_options, dio_options,
-                                   number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope,
-                                   coded_aperiodicity);
-  if (!h || !x || !opt || n_utts < 0 || fs <= 0 || x_stride <= 0 || f0_stride <= 0 || number_of_dimensions < 1)
-    return WORLD_B200_EINVAL;
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));
-  if (nbit != 0 && nbit != 8 && nbit != 16 && nbit != 24 && nbit != 32) return WORLD_B200_EINVAL;
-  int rc = check_chain_f0_options(ctx_of(h), opt, harvest_options, dio_options, n_utts, fs, "analyze_coded_host");
-  std::vector<CheapTrickOption> cts;
-  std::vector<int> d4_fft;
-  std::vector<D4COption> d4s;
-  if (!rc)
-    rc = chain_spectral_options(ctx_of(h), fs, number_of_dimensions, opt, cheaptrick_options, d4c_options, n_utts,
-                                coded_spectral_envelope != nullptr, coded_aperiodicity != nullptr, &cts, &d4_fft, &d4s);
-  if (rc) return rc;
-  return analyze_pipeline(h, x, nbit, n_utts, x_stride, x_lengths, fs, opt, harvest_options, dio_options,
-                          number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope, coded_aperiodicity,
-                          cts.data(), d4_fft.data(), d4s.data());
+  ChainRequest r = coded_request(x, nbit, n_utts, x_stride, x_lengths, fs, opt, number_of_dimensions, time_axis, f0,
+                                 f0_stride, coded_spectral_envelope, coded_aperiodicity);
+  r.harvest_options = harvest_options; r.dio_options = dio_options;
+  r.cheaptrick_options = cheaptrick_options; r.d4c_options = d4c_options;
+  return analyze_pipeline(h, r);
 }
 
 extern "C" int world_b200_analyze_coded_host(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride,
                                              const int *x_lengths, int fs, const WorldB200AnalysisOption *opt,
                                              int number_of_dimensions, double *time_axis, double *f0, int f0_stride,
                                              double *coded_spectral_envelope, double *coded_aperiodicity) {
-  return analyze_coded_host_impl(h, x, nbit, n_utts, x_stride, x_lengths, fs, opt, nullptr, nullptr,
-                                 number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope,
-                                 coded_aperiodicity);
+  return analyze_pipeline(h, coded_request(x, nbit, n_utts, x_stride, x_lengths, fs, opt, number_of_dimensions,
+                                           time_axis, f0, f0_stride, coded_spectral_envelope, coded_aperiodicity));
 }
 
 extern "C" int world_b200_analyze_coded_host_options(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride,
@@ -686,9 +587,10 @@ extern "C" int world_b200_analyze_coded_host_options(WorldB200 *h, const void *x
                                                      double *time_axis, double *f0, int f0_stride,
                                                      double *coded_spectral_envelope, double *coded_aperiodicity) {
   if (!harvest_options) return WORLD_B200_EINVAL;
-  return analyze_coded_host_impl(h, x, nbit, n_utts, x_stride, x_lengths, fs, opt, harvest_options, nullptr,
-                                 number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope,
-                                 coded_aperiodicity);
+  ChainRequest r = coded_request(x, nbit, n_utts, x_stride, x_lengths, fs, opt, number_of_dimensions, time_axis, f0,
+                                 f0_stride, coded_spectral_envelope, coded_aperiodicity);
+  r.harvest_options = harvest_options;
+  return analyze_pipeline(h, r);
 }
 
 extern "C" int world_b200_analyze_coded_host_dio_options(WorldB200 *h, const void *x, int nbit, int n_utts,
@@ -698,9 +600,10 @@ extern "C" int world_b200_analyze_coded_host_dio_options(WorldB200 *h, const voi
                                                          double *time_axis, double *f0, int f0_stride,
                                                          double *coded_spectral_envelope, double *coded_aperiodicity) {
   if (!dio_options) return WORLD_B200_EINVAL;
-  return analyze_coded_host_impl(h, x, nbit, n_utts, x_stride, x_lengths, fs, opt, nullptr, dio_options,
-                                 number_of_dimensions, time_axis, f0, f0_stride, coded_spectral_envelope,
-                                 coded_aperiodicity);
+  ChainRequest r = coded_request(x, nbit, n_utts, x_stride, x_lengths, fs, opt, number_of_dimensions, time_axis, f0,
+                                 f0_stride, coded_spectral_envelope, coded_aperiodicity);
+  r.dio_options = dio_options;
+  return analyze_pipeline(h, r);
 }
 
 // ------------------------------------------------------------------ legacy single-utterance API
@@ -742,7 +645,7 @@ struct Legacy1 {
   std::unique_ptr<DeviceGuard> guard;   // the legacy context's device is current while this object lives
   Legacy1(const double *xh, int x_length, const double *th, const double *fh, int f0_length) {
     h = legacy_ctx();
-    ctx = h ? ctx_of(h) : nullptr;
+    ctx = h ? &h->c : nullptr;
     if (!h) { rc = WORLD_B200_ECUDA; return; }
     guard.reset(new DeviceGuard(ctx));
     x = (double *)dev_malloc(ctx, (size_t)x_length * 8);
@@ -841,8 +744,8 @@ void Synthesis(const double *f0, int f0_length, const double *const *spectrogram
   std::lock_guard<std::mutex> lock(g_legacy_mutex);
   WorldB200 *h = legacy_ctx();
   if (!h) { fill(y, (size_t)imax(0, y_length), 0.0); report(h, "Synthesis", WORLD_B200_ECUDA); return; }
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  Ctx *ctx = ctx_of(h);
+  DeviceGuard guard_(&h->c);
+  Ctx *ctx = &h->c;
   const int bins = fft_size / 2 + 1;
   std::vector<double> flat((size_t)f0_length * bins);
   double *d_f0 = (double *)dev_malloc(ctx, (size_t)f0_length * 8);
@@ -872,8 +775,8 @@ static void codec_rows(const char *name, const double *const *in_rows, int f0_le
   WorldB200 *h = legacy_ctx();
   if (f0_length <= 0 || out_w <= 0) return;
   if (!h) { fill_rows(out_rows, f0_length, out_w, 0.0); report(h, name, WORLD_B200_ECUDA); return; }
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  Ctx *ctx = ctx_of(h);
+  DeviceGuard guard_(&h->c);
+  Ctx *ctx = &h->c;
   std::vector<double> flat_in((size_t)f0_length * imax(1, in_w)), flat_out((size_t)f0_length * out_w);
   for (int i = 0; i < f0_length && in_w > 0; ++i) memcpy(flat_in.data() + (size_t)i * in_w, in_rows[i], (size_t)in_w * 8);
   double *d_in = (double *)dev_malloc(ctx, flat_in.size() * 8), *d_out = (double *)dev_malloc(ctx, flat_out.size() * 8);

@@ -224,17 +224,6 @@ int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts,
                   const double *spectrogram, const double *aperiodicity, const CodedRows *coded, int fft_size, int lg,
                   double frame_period, int fs, const int *y_lengths, int y_stride, void *y, int nbit,
                   const ModifyPlan *mod = nullptr, int mod_u0 = 0, const double *fp_u = nullptr);
-// wb_api.cu: voice transformation (world_b200_transform_*), checked and planned once per call by transform_check;
-// transform_run (device rows) and the host pipeline (wb_host.cu) read it.
-struct TransformPlan {
-  int nbit = 0, nbit_out = 0, x_stride = 0, y_stride = 0, fs = 0, fft_size = 0, lg = 0;
-  int f0_stride = 0;               // the largest frame count of the call
-  double frame_period = 0.0;       // the analysis frame period (ms)
-  std::vector<int> f_len, y_len;   // [n] frames and output samples of each utterance
-  std::vector<double> fp;          // [n] synthesis frame period (s): (frame_period * time_scale[u]) / 1000.0
-  bool modify = false;             // f0_scale or spectral_ratio given
-  ModifyPlan mod;
-};
 
 // The utterances of a batch that share one CheapTrick option (world_b200_cheaptrick_*batch_options): their batch
 // indices, ascending, and their frame counts.  cheaptrick_run runs one launch sequence over them, reaching each row
