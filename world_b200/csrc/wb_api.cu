@@ -2,6 +2,7 @@
 // plus the legacy single-utterance entry points of include/world/*.h implemented as n_utts = 1
 // batches (reference boundary: src/world/{dio,harvest,stonemask,cheaptrick,d4c}.h).
 #include "wb_chain.h"
+#include "wb_f0common.cuh"
 #include <stdio.h>
 #include <string.h>
 #include <stdlib.h>
@@ -9,6 +10,7 @@
 #include <string>
 #include <algorithm>
 #include <cmath>
+#include <type_traits>
 
 namespace wb {
 
@@ -286,42 +288,6 @@ static int load_batch(WorldB200 *h, const double *x, int n, int x_stride, const 
 static int frames_for(int fs, int x_length, double frame_period) {
   return static_cast<int>(1000.0 * x_length / fs / frame_period) + 1;
 }
-
-namespace wb {
-
-// Per-utterance options: one frame_period for the whole batch; with ranges (fs > 0) also every utterance's F0 range
-// against the on-chip limits, up front, so that a chain cut into slices or chunks names the batch's first bad utterance.
-int check_harvest_options(Ctx *c, const HarvestOption *opts, int n, double frame_period, int fs) {
-  for (int u = 0; u < n; ++u)
-    if (!(opts[u].frame_period == frame_period)) {
-      c->last_error = "harvest options: frame_period differs from the batch's (utterance " + std::to_string(u) + ")";
-      return WORLD_B200_EINVAL;
-    }
-  if (fs <= 0 || n <= 0) return 0;
-  std::vector<HarvestParams> p(n);
-  for (int u = 0; u < n; ++u) p[u] = {opts[u].f0_floor, opts[u].f0_ceil, opts[u].frame_period};
-  return harvest_check_options(c, fs, p.data(), n);
-}
-
-// The same for DIO: one frame_period and one speed for the whole batch (they fix the decimation ratio, the low-cut
-// filter and the frame grid); with fs > 0 also every utterance's band list against the on-chip limits.
-int check_dio_options(Ctx *c, const DioOption *opts, int n, double frame_period, int speed, int fs) {
-  for (int u = 0; u < n; ++u) {
-    const char *what = !(opts[u].frame_period == frame_period) ? "frame_period" : (opts[u].speed != speed ? "speed" : nullptr);
-    if (what) {
-      c->last_error = std::string("dio options: ") + what + " differs from the batch's (utterance " + std::to_string(u) + ")";
-      return WORLD_B200_EINVAL;
-    }
-  }
-  if (fs <= 0 || n <= 0) return 0;
-  std::vector<DioParams> p(n);
-  for (int u = 0; u < n; ++u)
-    p[u] = {opts[u].f0_floor, opts[u].f0_ceil, opts[u].channels_in_octave, opts[u].frame_period, opts[u].allowed_range,
-            opts[u].speed};
-  return dio_check_options(c, fs, p.data(), n);
-}
-
-}  // namespace wb
 
 extern "C" {
 
@@ -663,8 +629,9 @@ static int chain_checks(Ctx *c, const ChainRequest &r, ChainPlan *p) {
     return fail("per-utterance Harvest options need f0_method == WORLD_B200_F0_HARVEST");
   if (r.dio_options && opt->f0_method != WORLD_B200_F0_DIO_STONEMASK)
     return fail("per-utterance DIO options need f0_method == WORLD_B200_F0_DIO_STONEMASK");
-  int rc = r.harvest_options ? check_harvest_options(c, r.harvest_options, n, opt->harvest.frame_period, r.fs)
-           : r.dio_options   ? check_dio_options(c, r.dio_options, n, opt->dio.frame_period, opt->dio.speed, r.fs)
+  RangeGroups groups;
+  int rc = r.harvest_options ? harvest_plan(c, r.fs, r.harvest_options, n, true, opt->harvest.frame_period, &groups)
+           : r.dio_options   ? dio_plan(c, r.fs, r.dio_options, n, true, opt->dio.frame_period, opt->dio.speed, &groups)
                              : 0;
   if (rc) return rc;
   p->frame_period = harvest ? opt->harvest.frame_period : opt->dio.frame_period;
@@ -822,6 +789,8 @@ int world_b200_stonemask_batch(WorldB200 *h, const double *x, int n, int x_strid
   return stonemask_run(&h->c, b, refined_f0);
 }
 
+}  // extern "C"
+
 static int f0_lengths_from_x(int n, int x_stride, const int *x_lengths, int fs, double frame_period,
                              int f0_stride, std::vector<int> *out, std::string *err) {
   out->resize(n);
@@ -836,74 +805,57 @@ static int f0_lengths_from_x(int n, int x_stride, const int *x_lengths, int fs, 
   return 0;
 }
 
-// opt: one option for every utterance, or (per_utt) an array of n
-static int dio_batch_impl(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
-                          const DioOption *opt, bool per_utt, double *time_axis, double *f0, int f0_stride) {
+// The F0 stage calls: opt is one option for every utterance, or (per_utt) an array of n.  The options are checked and
+// grouped before the lengths are uploaded: a bad option queues nothing on the device.
+template <class Option>
+static int f0_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs, const Option *opt,
+                    bool per_utt, double *time_axis, double *f0, int f0_stride) {
   if (!h || !x || !time_axis || !f0 || !opt || n < 0 || fs <= 0) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
-  if (per_utt && n > 0) {
-    // every band list too, before the lengths are uploaded: a bad option queues nothing on the device
-    const int rc = check_dio_options(&h->c, opt, n, opt[0].frame_period, opt[0].speed, fs);
-    if (rc) return rc;
-  }
+  constexpr bool harvest = std::is_same<Option, HarvestOption>::value;
+  RangeGroups groups;
+  int rc;
+  if constexpr (harvest) rc = harvest_plan(&h->c, fs, opt, n, per_utt, opt->frame_period, &groups);
+  else rc = dio_plan(&h->c, fs, opt, n, per_utt, opt->frame_period, opt->speed, &groups);
+  if (rc) return rc;
   std::vector<int> fl;
-  int rc = f0_lengths_from_x(n, x_stride, x_lengths, fs, opt->frame_period, f0_stride, &fl, &h->c.last_error);
+  rc = f0_lengths_from_x(n, x_stride, x_lengths, fs, opt->frame_period, f0_stride, &fl, &h->c.last_error);
   if (rc) return rc;
   Batch b;
   rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, fl.data(), f0_stride, &b);
   if (rc) return rc;
   b.x_len_host = x_lengths;
-  std::vector<DioParams> p(per_utt ? (n > 0 ? n : 1) : 1);
-  for (size_t u = 0; u < p.size(); ++u)
-    p[u] = {opt[u].f0_floor, opt[u].f0_ceil, opt[u].channels_in_octave, opt[u].frame_period, opt[u].allowed_range,
-            opt[u].speed};
-  return dio_run(&h->c, b, p.data(), per_utt, time_axis, f0);
+  if constexpr (harvest) {
+    std::vector<int> l1(n > 0 ? n : 1);
+    for (int i = 0; i < n; ++i) l1[i] = frames_for(fs, x_lengths ? x_lengths[i] : x_stride, 1.0);
+    b.l1_host = l1.data();
+    return harvest_run(&h->c, b, opt->frame_period, groups, time_axis, f0);
+  } else {
+    return dio_run(&h->c, b, opt, per_utt, groups, time_axis, f0);
+  }
 }
+
+extern "C" {
 
 int world_b200_dio_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
                          const DioOption *opt, double *time_axis, double *f0, int f0_stride) {
-  return dio_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, false, time_axis, f0, f0_stride);
+  return f0_batch(h, x, n, x_stride, x_lengths, fs, opt, false, time_axis, f0, f0_stride);
 }
 
 int world_b200_dio_batch_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
                                  const DioOption *dio_options, double *time_axis, double *f0, int f0_stride) {
-  return dio_batch_impl(h, x, n, x_stride, x_lengths, fs, dio_options, true, time_axis, f0, f0_stride);
-}
-
-// opt: one option for every utterance, or (per_utt) an array of n
-static int harvest_batch_impl(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
-                              const HarvestOption *opt, bool per_utt, double *time_axis, double *f0, int f0_stride) {
-  if (!h || !x || !time_axis || !f0 || !opt || n < 0 || fs <= 0) return WORLD_B200_EINVAL;
-  DeviceGuard guard_(&h->c);
-  if (per_utt && n > 0) {
-    // every range too, before the lengths are uploaded: a bad option queues nothing on the device
-    const int rc = check_harvest_options(&h->c, opt, n, opt[0].frame_period, fs);
-    if (rc) return rc;
-  }
-  std::vector<int> fl;
-  int rc = f0_lengths_from_x(n, x_stride, x_lengths, fs, opt->frame_period, f0_stride, &fl, &h->c.last_error);
-  if (rc) return rc;
-  Batch b;
-  rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, fl.data(), f0_stride, &b);
-  if (rc) return rc;
-  std::vector<int> l1(n > 0 ? n : 1);
-  for (int i = 0; i < n; ++i) l1[i] = frames_for(fs, x_lengths ? x_lengths[i] : x_stride, 1.0);
-  b.l1_host = l1.data();
-  b.x_len_host = x_lengths;
-  std::vector<HarvestParams> p(per_utt ? (n > 0 ? n : 1) : 1);
-  for (size_t u = 0; u < p.size(); ++u) p[u] = {opt[u].f0_floor, opt[u].f0_ceil, opt[u].frame_period};
-  return harvest_run(&h->c, b, p.data(), per_utt, time_axis, f0);
+  return f0_batch(h, x, n, x_stride, x_lengths, fs, dio_options, true, time_axis, f0, f0_stride);
 }
 
 int world_b200_harvest_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
                              int fs, const HarvestOption *opt, double *time_axis, double *f0, int f0_stride) {
-  return harvest_batch_impl(h, x, n, x_stride, x_lengths, fs, opt, false, time_axis, f0, f0_stride);
+  return f0_batch(h, x, n, x_stride, x_lengths, fs, opt, false, time_axis, f0, f0_stride);
 }
 
 int world_b200_harvest_batch_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
                                      const HarvestOption *harvest_options, double *time_axis, double *f0,
                                      int f0_stride) {
-  return harvest_batch_impl(h, x, n, x_stride, x_lengths, fs, harvest_options, true, time_axis, f0, f0_stride);
+  return f0_batch(h, x, n, x_stride, x_lengths, fs, harvest_options, true, time_axis, f0, f0_stride);
 }
 
 }  // extern "C"

@@ -7,46 +7,20 @@
 //   K-DIOc  dio_contour_kernel   best candidate + FixStep1..4                     (dio.cpp:112-289)
 // Host side computes every size and filter tap with the reference's own double-precision
 // expressions (and the host libm), so frame counts, band lists and taps are bit-identical.
-// One option per utterance (world_b200_dio_batch_options): the batch's distinct band lists are range groups whose
-// tables are concatenated; the sweep runs on a flat grid over the utterances' own bands and the contour takes each
-// utterance's band count, floor and allowed_range.  speed and frame_period are shared by the batch.
+// One option per utterance (world_b200_dio_batch_options): dio_plan groups the batch's distinct (f0_floor, f0_ceil,
+// channels_in_octave) triples into range groups with the band plan of wb_f0common.cuh; the sweep runs on a flat grid
+// over the utterances' own bands and the contour takes each utterance's band count, floor and allowed_range.  speed
+// and frame_period are shared by the batch.
 #include "wb_internal.h"
 #include "wb_f0common.cuh"
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 #include <array>
-#include <map>
 #include <string>
 #include <vector>
 
 namespace wb {
-
-// Event-list capacity per band and train: crossings of a signal band-limited around/below
-// `boundary` cannot be denser than ~boundary per second for long; 2.5x margin, hard bound
-// ylen/2+2 (a negative-going crossing needs two samples).  The lists are history rings: more events
-// than this wrap around; only a look-back beyond the last `cap` events raises status bit 4.
-static void plan_edge_caps(const std::vector<double> &boundary, double afs, int max_ylen,
-                           std::vector<int> *cap, std::vector<long long> *off, size_t *stride) {
-  const int nb = (int)boundary.size();
-  cap->resize(nb); off->resize(nb);
-  long long run = 0;
-  long long floor_cap = 2048;
-  if (const char *e = getenv("WB_EDGE_CAP_MIN")) floor_cap = atoll(e) > 0 ? atoll(e) : floor_cap;   // test hook: force wraps
-  for (int i = 0; i < nb; ++i) {
-    const long long hard = (long long)max_ylen / 2 + 2;
-    long long soft = (long long)(2.5 * boundary[i] * max_ylen / afs) + 64;
-    if (soft < floor_cap) soft = floor_cap;   // a tile can append up to 1025 events per train; the rings look back 256
-    // DIO keeps every event: with the mirroring ripple in, digital silence makes the difference trains fire
-    // every sample while the crossing trains may stay silent, so frames cannot be finalised until the silence
-    // ends and the look-back is as long as the silence (few bands, so the full lists are affordable)
-    soft = hard;
-    (*cap)[i] = (int)(soft < hard ? soft : hard);
-    (*off)[i] = run;
-    run += 4LL * (*cap)[i];
-  }
-  *stride = (size_t)run;
-}
 
 struct DioPrepParams {
   const double *x; const int *x_len; int x_stride;
@@ -174,20 +148,10 @@ WB_KERNEL(256, 2) dio_contour_kernel(DioContourParams p) {
   for (int i = tid; i < L; i += nth) f0[i] = s3[i];
 }
 
-// The band list of one F0 range (f0_floor, f0_ceil, channels_in_octave): channel boundaries (dio.cpp:582-588), per
-// band Nuttall low-pass of 4 ha taps (GetFilteredSignal, dio.cpp:296-337) and the event-list plan.  A batch with several
-// ranges concatenates the lists of its distinct ranges (range groups); each list is what a call with that range alone
-// builds.
-struct DioRange {
-  double f0_floor = 0.0, f0_ceil = 0.0;
-  int nb = 0, max_taps = 0;
-  std::vector<double> boundary, taps;      // taps: reversed, 8 zeros after each band
-  std::vector<int> tap_off, ntaps, shift;  // tap_off: into this range's taps
-  std::vector<int> ecap; std::vector<long long> eoff; size_t edge_stride = 0;
-};
-
-// nullptr, or why the on-chip kernels cannot serve this range
-static const char *dio_plan_range(const DioParams &o, double afs, int max_ylen, DioRange *r) {
+// The band list of one F0 range (f0_floor, f0_ceil, channels_in_octave): channel boundaries (dio.cpp:582-588) and per
+// band Nuttall low-pass of 4 ha taps (GetFilteredSignal, dio.cpp:296-337).  nullptr, or why the on-chip kernels cannot
+// serve this range.
+static const char *dio_band_list(const DioOption &o, double afs, BandList *r) {
   r->f0_floor = o.f0_floor; r->f0_ceil = o.f0_ceil;
   const int nb = 1 + static_cast<int>(log(o.f0_ceil / o.f0_floor) / kLog2 * o.channels_in_octave);
   if (nb < 1 || nb > 4096) return "Dio: bad band count";
@@ -219,43 +183,26 @@ static const char *dio_plan_range(const DioParams &o, double afs, int max_ylen, 
   }
   if (sweep_smem_bytes(r->max_taps) > 200 * 1024)
     return "Dio: filters too long for shared memory (lower fs / raise f0_floor / use speed > 1)";
-  plan_edge_caps(r->boundary, afs, max_ylen, &r->ecap, &r->eoff, &r->edge_stride);
   return nullptr;
-}
-
-// Range groups of a batch: the distinct (f0_floor, f0_ceil, channels_in_octave) triples in order of first appearance
-// (keyed by bit pattern), each planned and checked against the on-chip limits when it first appears -- so an error
-// names the first offending utterance.  ugrp[u] = the group of utterance u.  allowed_range is not part of the key: only
-// the contour uses it, per utterance.
-static int dio_make_groups(Ctx *ctx, const DioParams *opts, bool per_utt, int n, double afs, int max_ylen,
-                           std::vector<DioRange> *groups, std::vector<int> *ugrp) {
-  std::map<std::array<unsigned long long, 3>, int> seen;
-  ugrp->resize(n);
-  for (int u = 0; u < n; ++u) {
-    const DioParams &o = opts[per_utt ? u : 0];
-    std::array<unsigned long long, 3> key;
-    memcpy(&key[0], &o.f0_floor, 8); memcpy(&key[1], &o.f0_ceil, 8); memcpy(&key[2], &o.channels_in_octave, 8);
-    auto it = seen.find(key);
-    if (it == seen.end()) {
-      groups->emplace_back();
-      if (const char *why = dio_plan_range(o, afs, max_ylen, &groups->back())) {
-        ctx->last_error = why;
-        if (per_utt) ctx->last_error += " (utterance " + std::to_string(u) + ")";
-        return 3;
-      }
-      it = seen.emplace(key, (int)groups->size() - 1).first;
-    }
-    (*ugrp)[u] = it->second;
-  }
-  return 0;
 }
 
 static int dio_ratio(int speed) { return imax(imin(speed, 12), 1); }
 
-int dio_check_options(Ctx *ctx, int fs, const DioParams *opts, int n) {
-  std::vector<DioRange> groups;
-  std::vector<int> ugrp;
-  return dio_make_groups(ctx, opts, true, n, static_cast<double>(fs) / dio_ratio(opts[0].speed), 1, &groups, &ugrp);
+// allowed_range is not part of the group key: only the contour uses it, per utterance
+int dio_plan(Ctx *ctx, int fs, const DioOption *opts, int n, bool per_utt, double frame_period, int speed,
+             RangeGroups *g) {
+  for (int u = 0; per_utt && u < n; ++u) {
+    const char *what = !(opts[u].frame_period == frame_period) ? "frame_period" : (opts[u].speed != speed ? "speed" : nullptr);
+    if (what) {
+      ctx->last_error = std::string("dio options: ") + what + " differs from the batch's (utterance " + std::to_string(u) + ")";
+      return 3;
+    }
+  }
+  const double afs = static_cast<double>(fs) / dio_ratio(speed);
+  return group_ranges(
+      ctx, n, per_utt,
+      [&](int i) { return std::array<double, 3>{opts[i].f0_floor, opts[i].f0_ceil, opts[i].channels_in_octave}; },
+      [&](int i, BandList *r) { return dio_band_list(opts[i], afs, r); }, g);
 }
 
 // WB_LOAD_DIO_CAND=<prefix> (test hook, README): before dio_contour_kernel each chunk's candidate and score rows are
@@ -288,39 +235,18 @@ static int dio_load_cand(Ctx *ctx, const char *prefix, int chunk, int n, int nb,
   return rc;
 }
 
-int dio_run(Ctx *ctx, const Batch &b, const DioParams *opts, bool per_utt, double *time_axis_out, double *f0_out) {
+int dio_run(Ctx *ctx, const Batch &b, const DioOption *opts, bool per_utt, const RangeGroups &groups,
+            double *time_axis_out, double *f0_out) {
   if (b.n <= 0) return 0;
   const int fs = b.fs;
-  // speed and frame_period: equal for every utterance (checked by the ABI layer)
+  // speed and frame_period: equal for every utterance (dio_plan)
   const double frame_period = opts[0].frame_period;
   const int ratio = dio_ratio(opts[0].speed);
   const double afs = static_cast<double>(fs) / ratio;
   const int max_ylen = 1 + b.max_x_len / ratio;
-  std::vector<DioRange> groups;
-  std::vector<int> ugrp;
-  const int rc0 = dio_make_groups(ctx, opts, per_utt, b.n, afs, max_ylen, &groups, &ugrp);
-  if (rc0) return rc0;
-  // the band tables of every group one after the other; scratch strides follow the batch maxima
-  const int n_groups = (int)groups.size();
-  std::vector<double> taps, boundary, grp_floor(n_groups), grp_ceil(n_groups);
-  std::vector<int> tap_off, ntaps, shift, ecap, grp_band0(n_groups), grp_nb(n_groups);
-  std::vector<long long> eoff;
-  int nb = 0, max_taps = 0;   // batch maxima
-  size_t edge_stride = 0;
-  for (int g = 0; g < n_groups; ++g) {
-    const DioRange &r = groups[g];
-    grp_band0[g] = (int)boundary.size(); grp_nb[g] = r.nb; grp_floor[g] = r.f0_floor; grp_ceil[g] = r.f0_ceil;
-    for (int i = 0; i < r.nb; ++i) tap_off.push_back((int)taps.size() + r.tap_off[i]);
-    taps.insert(taps.end(), r.taps.begin(), r.taps.end());
-    boundary.insert(boundary.end(), r.boundary.begin(), r.boundary.end());
-    ntaps.insert(ntaps.end(), r.ntaps.begin(), r.ntaps.end());
-    shift.insert(shift.end(), r.shift.begin(), r.shift.end());
-    ecap.insert(ecap.end(), r.ecap.begin(), r.ecap.end());
-    eoff.insert(eoff.end(), r.eoff.begin(), r.eoff.end());
-    nb = imax(nb, r.nb); max_taps = imax(max_taps, r.max_taps);
-    if (r.edge_stride > edge_stride) edge_stride = r.edge_stride;
-  }
-  const int n_tab = (int)boundary.size();   // rows of the band tables
+  const BandTables tab(groups, afs, max_ylen, true);
+  const int nb = tab.nb, max_taps = tab.max_taps;
+  const size_t edge_stride = tab.edge_stride;
   // allowed_range per utterance only where it differs (it is not part of the group key)
   bool mixed_allowed = false;
   for (int u = 1; per_utt && u < b.n; ++u) mixed_allowed = mixed_allowed || !(opts[u].allowed_range == opts[0].allowed_range);
@@ -357,15 +283,11 @@ int dio_run(Ctx *ctx, const Batch &b, const DioParams *opts, bool per_utt, doubl
     const size_t o_y = plan.add((size_t)n * y_stride * 8), o_ylc = plan.add((size_t)n * y_stride * 8);
     const size_t o_ylen = plan.add((size_t)n * 4), o_nyq = plan.add((size_t)n * 32), o_nfft = plan.add((size_t)n * 4);
     const size_t o_edges = plan.add((size_t)n * edge_stride * 8);
-    const size_t o_ecap = plan.add(n_tab * 4), o_eoff = plan.add(n_tab * 8);
     const size_t o_cand = plan.add((size_t)n * nb * fstr * 8), o_score = plan.add((size_t)n * nb * fstr * 8);
     const size_t o_work = plan.add((size_t)n * 4 * fstr * 8), o_sec = plan.add((size_t)n * 2 * fstr * 4);
     const size_t o_tmp = plan.add((size_t)n * tmp_stride * 8);
-    const size_t o_lc = plan.add(lc_rev.size() * 8 + 64), o_taps = plan.add(taps.size() * 8);
-    const size_t o_toff = plan.add(n_tab * 4), o_nt = plan.add(n_tab * 4), o_sh = plan.add(n_tab * 4), o_bd = plan.add(n_tab * 8);
-    const size_t o_ugrp = plan.add((size_t)n * 4), o_gb0 = plan.add(n_groups * 4), o_gnb = plan.add(n_groups * 4);
-    const size_t o_gfl = plan.add(n_groups * 8), o_gce = plan.add(n_groups * 8);
-    const size_t o_bband = plan.add((size_t)(n + 1) * 4), o_allow = plan.add((size_t)n * 8);
+    const size_t o_lc = plan.add(lc_rev.size() * 8 + 64), o_tab = plan.add(tab.chunk_bytes(n));
+    const size_t o_allow = plan.add((size_t)n * 8);
     unsigned char *blk = arena_block(ctx, plan.total);
     if (!blk) return 2;
     double *y = (double *)(blk + o_y), *ylc = (double *)(blk + o_ylc);
@@ -373,25 +295,9 @@ int dio_run(Ctx *ctx, const Batch &b, const DioParams *opts, bool per_utt, doubl
     int rc = dev_memset(ctx, y, 0, (size_t)n * y_stride * 8);
     if (!rc) rc = dev_memset(ctx, ylc, 0, (size_t)n * y_stride * 8);
     if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_lc, lc_rev.data(), lc_rev.size() * 8);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_taps, taps.data(), taps.size() * 8);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_toff, tap_off.data(), n_tab * 4);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_nt, ntaps.data(), n_tab * 4);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_sh, shift.data(), n_tab * 4);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_bd, boundary.data(), n_tab * 8);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_ecap, ecap.data(), n_tab * 4);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_eoff, eoff.data(), n_tab * 8);
-    // range groups of this chunk's utterances and the first block of each in the flat band grid
-    std::vector<int> bband(n + 1, 0);
+    SweepParams sp;
+    if (!rc) rc = tab.upload(ctx, blk + o_tab, u0, n, &sp);
     std::vector<double> allow;
-    if (n_groups > 1) {
-      for (int i = 0; i < n; ++i) bband[i + 1] = bband[i] + grp_nb[ugrp[u0 + i]];
-      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_ugrp, ugrp.data() + u0, (size_t)n * 4);
-      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_gb0, grp_band0.data(), n_groups * 4);
-      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_gnb, grp_nb.data(), n_groups * 4);
-      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_gfl, grp_floor.data(), n_groups * 8);
-      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_gce, grp_ceil.data(), n_groups * 8);
-      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_bband, bband.data(), (size_t)(n + 1) * 4);
-    }
     if (mixed_allowed) {
       allow.resize(n);
       for (int i = 0; i < n; ++i) allow[i] = opts[u0 + i].allowed_range;
@@ -425,7 +331,7 @@ int dio_run(Ctx *ctx, const Batch &b, const DioParams *opts, bool per_utt, doubl
     for (int i = 0; i < n; ++i) {
       const int xl = b.x_len_host ? b.x_len_host[u0 + i] : b.x_stride;
       const int yl = 1 + xl / ratio;
-      const double b0 = groups[ugrp[u0 + i]].boundary[0];
+      const double b0 = groups.lists[groups.ugrp[u0 + i]].boundary[0];
       const int sample = yl + c * 2 + 1 + 4 * static_cast<int>(1.0 + afs / b0 / 2.0);
       nfft[i] = static_cast<int>(pow(2.0, static_cast<int>(log(static_cast<double>(sample)) / kLog2) + 1.0));
     }
@@ -436,29 +342,17 @@ int dio_run(Ctx *ctx, const Batch &b, const DioParams *opts, bool per_utt, doubl
     np_.nfft = (const int *)(blk + o_nfft); np_.nyq = (double *)(blk + o_nyq);
     launch_nyquist_bins(ctx, np_, (unsigned)n);
 
-    SweepParams sp;
-    sp.sig = ylc; sp.sig_stride = y_stride; sp.sig_origin = padl + c; sp.y_len = ylen; sp.n_bands = nb;
-    sp.taps_rev = (const double *)(blk + o_taps); sp.tap_off = (const int *)(blk + o_toff);
-    sp.ntaps = (const int *)(blk + o_nt); sp.shift = (const int *)(blk + o_sh);
-    sp.boundary = (const double *)(blk + o_bd); sp.afs = afs;
-    sp.edges = (double *)(blk + o_edges); sp.edge_stride = edge_stride;
-    sp.edge_cap = (const int *)(blk + o_ecap); sp.edge_off = (const long long *)(blk + o_eoff);
-    sp.n_frames = b.f_len + u0; sp.frame_stride = fstr; sp.frame_period = frame_period;
-    sp.mode = 0; sp.f0_floor = groups[0].f0_floor; sp.f0_ceil = groups[0].f0_ceil;
-    if (n_groups > 1) {   // one group: bands 0 .. nb - 1 of the tables and the (band, utterance) grid, as without groups
-      sp.ugrp = (const int *)(blk + o_ugrp); sp.grp_band0 = (const int *)(blk + o_gb0); sp.grp_nb = (const int *)(blk + o_gnb);
-      sp.grp_floor = (const double *)(blk + o_gfl); sp.grp_ceil = (const double *)(blk + o_gce);
-      sp.blk0_band = (const int *)(blk + o_bband); sp.n_blk_band = bband[n]; sp.n_utts = n;
-    }
+    sp.sig = ylc; sp.sig_stride = y_stride; sp.sig_origin = padl + c; sp.y_len = ylen; sp.afs = afs;
+    sp.edges = (double *)(blk + o_edges);
+    sp.n_frames = b.f_len + u0; sp.frame_stride = fstr; sp.frame_period = frame_period; sp.mode = 0;
     sp.nyq = (const double *)(blk + o_nyq); sp.ripple = getenv("WB_NO_RIPPLE") ? 0 : 1;   // A/B switch for experiments
-    sp.cand = (double *)(blk + o_cand); sp.score = (double *)(blk + o_score);
-    sp.max_taps = max_taps; sp.status = ctx->status_dev;
+    sp.cand = (double *)(blk + o_cand); sp.score = (double *)(blk + o_score); sp.status = ctx->status_dev;
     launch_band_sweep(ctx, sp, (unsigned)n);
     if (load_cand && (rc = dio_load_cand(ctx, load_cand, u0 / chunk, n, nb, fstr, sp.cand, sp.score))) return rc;
 
     DioContourParams cp;
     cp.cand = sp.cand; cp.score = sp.score; cp.n_bands = nb; cp.frame_stride = fstr; cp.f_len = b.f_len + u0;
-    cp.frame_period = frame_period; cp.f0_floor = groups[0].f0_floor; cp.allowed_range = opts[0].allowed_range;
+    cp.frame_period = frame_period; cp.f0_floor = groups.lists[0].f0_floor; cp.allowed_range = opts[0].allowed_range;
     cp.ugrp = sp.ugrp; cp.grp_nb = sp.grp_nb; cp.grp_floor = sp.grp_floor;
     cp.allowed = mixed_allowed ? (const double *)(blk + o_allow) : nullptr;
     cp.work = (double *)(blk + o_work); cp.sections = (int *)(blk + o_sec);

@@ -3,6 +3,9 @@
 #include "wb_f0common.cuh"
 #include "wb_mma.cuh"
 #include <stdlib.h>
+#include <string.h>
+#include <map>
+#include <string>
 
 namespace wb {
 
@@ -1167,6 +1170,131 @@ void launch_band_sweep_split(Ctx *ctx, const SweepParams &p_in, unsigned n_utts)
   WB_LAUNCH_COOP(band_interp_kernel, sweep_grid(p, n_utts), 256, 0, ctx->stream, p);
   // bands whose edge lists overflowed (usually none): the streaming kernel with its history rings, over the list
   WB_LAUNCH_COOP(band_sweep_list_kernel, dim3((unsigned)(3 * ctx->sm_count)), WB_SWEEP_THREADS, smem_sw, ctx->stream, p);
+}
+
+// ------------------------------------------------------------------------------ band plan (host)
+int group_ranges(Ctx *ctx, int n, bool per_utt, const std::function<std::array<double, 3>(int)> &key,
+                 const std::function<const char *(int, BandList *)> &build, RangeGroups *g) {
+  std::map<std::array<unsigned long long, 3>, int> seen;
+  g->lists.clear();
+  g->ugrp.resize(n);
+  for (int u = 0; u < n; ++u) {
+    const int i = per_utt ? u : 0;
+    const std::array<double, 3> k = key(i);
+    std::array<unsigned long long, 3> bits;
+    memcpy(bits.data(), k.data(), sizeof(bits));
+    auto it = seen.find(bits);
+    if (it == seen.end()) {
+      g->lists.emplace_back();
+      if (const char *why = build(i, &g->lists.back())) {
+        ctx->last_error = why;
+        if (per_utt) ctx->last_error += " (utterance " + std::to_string(u) + ")";
+        return 3;
+      }
+      it = seen.emplace(bits, (int)g->lists.size() - 1).first;
+    }
+    g->ugrp[u] = it->second;
+  }
+  return 0;
+}
+
+// Event-list capacity per band and train: crossings of a signal band-limited around/below
+// `boundary` cannot be denser than ~boundary per second for long; 2.5x margin, hard bound
+// ylen/2+2 (a negative-going crossing needs two samples).  The lists are history rings: more events
+// than this wrap around; only a look-back beyond the last `cap` events raises status bit 4.
+static void plan_edge_caps(const std::vector<double> &boundary, double afs, int max_ylen, bool full,
+                           std::vector<int> *cap, std::vector<long long> *off, size_t *stride) {
+  const int nb = (int)boundary.size();
+  cap->resize(nb); off->resize(nb);
+  long long run = 0;
+  long long floor_cap = 2048;
+  if (const char *e = getenv("WB_EDGE_CAP_MIN")) floor_cap = atoll(e) > 0 ? atoll(e) : floor_cap;   // test hook: force wraps
+  for (int i = 0; i < nb; ++i) {
+    const long long hard = (long long)max_ylen / 2 + 2;
+    long long soft = (long long)(2.5 * boundary[i] * max_ylen / afs) + 64;
+    if (soft < floor_cap) soft = floor_cap;   // a tile can append up to 1025 events per train; the rings look back 256
+    // full (DIO, and Harvest on non-decimated input: the mirroring ripple is in): in digital silence the difference
+    // trains fire every sample while the crossing trains stay silent, so frames cannot be finalised until the silence
+    // ends and the look-back is as long as the silence -- keep every event (DIO has few bands, so the full lists are
+    // affordable)
+    if (full) soft = hard;
+    (*cap)[i] = (int)(soft < hard ? soft : hard);
+    (*off)[i] = run;
+    run += 4LL * (*cap)[i];
+  }
+  *stride = (size_t)run;
+}
+
+BandTables::BandTables(const RangeGroups &g, double afs, int max_ylen, bool full) : ugrp(g.ugrp) {
+  for (const BandList &r : g.lists) {
+    grp_band0.push_back((int)boundary.size()); grp_nb.push_back(r.nb);
+    grp_floor.push_back(r.f0_floor); grp_ceil.push_back(r.f0_ceil);
+    for (int i = 0; i < r.nb; ++i) tap_off.push_back((int)taps.size() + r.tap_off[i]);
+    taps.insert(taps.end(), r.taps.begin(), r.taps.end());
+    boundary.insert(boundary.end(), r.boundary.begin(), r.boundary.end());
+    ntaps.insert(ntaps.end(), r.ntaps.begin(), r.ntaps.end());
+    shift.insert(shift.end(), r.shift.begin(), r.shift.end());
+    std::vector<int> cap;
+    std::vector<long long> off;
+    size_t stride;
+    plan_edge_caps(r.boundary, afs, max_ylen, full, &cap, &off, &stride);
+    ecap.insert(ecap.end(), cap.begin(), cap.end());
+    eoff.insert(eoff.end(), off.begin(), off.end());
+    nb = imax(nb, r.nb); max_taps = imax(max_taps, r.max_taps);
+    if (stride > edge_stride) edge_stride = stride;
+  }
+}
+
+// the chunk's copy in layout order: band tables, group tables, then the chunk's ugrp and the two prefix sums
+enum { P_TAPS, P_TAP_OFF, P_NTAPS, P_SHIFT, P_BOUNDARY, P_ECAP, P_EOFF, P_BAND0, P_NB, P_FLOOR, P_CEIL, P_UGRP, P_BBAND,
+       P_BPAIR };
+std::vector<BandTables::Part> BandTables::chunk_parts(int u0, int n, const int *bband, const int *bpair) const {
+  const size_t nt = boundary.size(), ng = grp_nb.size();
+  return {{taps.data(), taps.size() * 8}, {tap_off.data(), nt * 4}, {ntaps.data(), nt * 4}, {shift.data(), nt * 4},
+          {boundary.data(), nt * 8}, {ecap.data(), nt * 4}, {eoff.data(), nt * 8},
+          {grp_band0.data(), ng * 4}, {grp_nb.data(), ng * 4}, {grp_floor.data(), ng * 8}, {grp_ceil.data(), ng * 8},
+          {ugrp.data() + u0, (size_t)n * 4}, {bband, (size_t)(n + 1) * 4}, {bpair, (size_t)(n + 1) * 4}};
+}
+
+size_t BandTables::chunk_bytes(int n) const {
+  ArenaPlan plan;
+  for (const Part &p : chunk_parts(0, n, nullptr, nullptr)) plan.add(p.bytes);
+  return plan.total;
+}
+
+int BandTables::upload(Ctx *ctx, unsigned char *blk, int u0, int n, SweepParams *sp, GroupTables *gt) const {
+  // the first block of each utterance in the flat band / band-pair grids
+  std::vector<int> bband(n + 1, 0), bpair(n + 1, 0);
+  for (int i = 0; i < n; ++i) {
+    const int nbu = grp_nb[ugrp[u0 + i]];
+    bband[i + 1] = bband[i] + nbu;
+    bpair[i + 1] = bpair[i] + (nbu + 1) / 2;
+  }
+  // one copy of the whole block, each table at its 256-byte aligned place
+  const std::vector<Part> parts = chunk_parts(u0, n, bband.data(), bpair.data());
+  ArenaPlan plan;
+  std::vector<size_t> off;
+  for (const Part &p : parts) off.push_back(plan.add(p.bytes));
+  std::vector<unsigned char> host(plan.total);
+  for (size_t i = 0; i < parts.size(); ++i) memcpy(host.data() + off[i], parts[i].src, parts[i].bytes);
+  const int rc = dev_memcpy_h2d(ctx, blk, host.data(), host.size());
+  if (rc) return rc;
+  auto at = [&](int i) { return blk + off[i]; };
+  sp->taps_rev = (const double *)at(P_TAPS); sp->tap_off = (const int *)at(P_TAP_OFF);
+  sp->ntaps = (const int *)at(P_NTAPS); sp->shift = (const int *)at(P_SHIFT); sp->boundary = (const double *)at(P_BOUNDARY);
+  sp->edge_cap = (const int *)at(P_ECAP); sp->edge_off = (const long long *)at(P_EOFF);
+  sp->n_bands = nb; sp->max_taps = max_taps; sp->edge_stride = edge_stride;
+  sp->f0_floor = grp_floor[0]; sp->f0_ceil = grp_ceil[0];
+  const GroupTables g = {(const int *)at(P_UGRP), (const int *)at(P_NB), (const double *)at(P_FLOOR),
+                         (const double *)at(P_CEIL)};
+  if (gt) *gt = g;
+  if (grp_nb.size() > 1) {
+    sp->ugrp = g.ugrp; sp->grp_band0 = (const int *)at(P_BAND0); sp->grp_nb = g.grp_nb;
+    sp->grp_floor = g.grp_floor; sp->grp_ceil = g.grp_ceil;
+    sp->blk0_band = (const int *)at(P_BBAND); sp->blk0_pair = (const int *)at(P_BPAIR);
+    sp->n_blk_band = bband[n]; sp->n_blk_pair = bpair[n]; sp->n_utts = n;
+  }
+  return 0;
 }
 
 }  // namespace wb

@@ -18,6 +18,9 @@
 #pragma once
 #include "wb_platform.cuh"
 #include "wb_block.cuh"
+#include <array>
+#include <functional>
+#include <vector>
 
 namespace wb {
 
@@ -191,5 +194,51 @@ struct NyquistParams {
   double *nyq;                                       // out [n][4]: Re Ys[N/2-1], Im Ys[N/2-1], Ys[N/2], N
 };
 void launch_nyquist_bins(Ctx *ctx, const NyquistParams &p, unsigned n_utts);
+
+// ------------------------------------------------------------------------------ band plan (host)
+// One F0 range per utterance (Harvest and DIO): the batch's distinct ranges are range groups, in order of first
+// appearance.  Their band lists are concatenated into one set of tables, and each utterance reaches its bands through
+// its group index (SweepParams::ugrp).  Each list is what a call with that range alone builds.
+struct BandList {
+  double f0_floor = 0.0, f0_ceil = 0.0;
+  int nb = 0, max_taps = 0;
+  std::vector<double> boundary, taps;      // taps: reversed, 8 zeros after each band
+  std::vector<int> tap_off, ntaps, shift;  // tap_off: into this list's taps
+};
+struct RangeGroups {
+  std::vector<BandList> lists;   // one per group
+  std::vector<int> ugrp;         // [n] the group of each utterance
+};
+// Groups n utterances by key(i), the doubles that fix option i's band list, compared by bit pattern (per_utt: option u
+// is utterance u's, else option 0 serves every utterance).  build(i, list) makes the list when its key first appears and
+// returns nullptr, or why the on-chip kernels cannot serve it: then 3 (EINVAL) with that reason in last_error and, per
+// utterance, " (utterance u)" after it.  So an error names the first bad utterance.
+int group_ranges(Ctx *ctx, int n, bool per_utt, const std::function<std::array<double, 3>(int)> &key,
+                 const std::function<const char *(int, BandList *)> &build, RangeGroups *g);
+
+// a chunk's device copy of the group tables (BandTables::upload), set with one group too
+struct GroupTables { const int *ugrp, *grp_nb; const double *grp_floor, *grp_ceil; };
+
+// The band tables of a batch: every group's list one after the other, with its event lists planned for the batch's
+// longest decimated utterance (max_ylen; full: keep every event), and the group tables.  Scratch strides follow the
+// batch maxima.
+struct BandTables {
+  BandTables(const RangeGroups &g, double afs, int max_ylen, bool full);
+  std::vector<int> ugrp;
+  std::vector<double> taps, boundary, grp_floor, grp_ceil;
+  std::vector<int> tap_off, ntaps, shift, ecap, grp_band0, grp_nb;
+  std::vector<long long> eoff;
+  int nb = 0, max_taps = 0;   // batch maxima
+  size_t edge_stride = 0;
+  // A chunk of n utterances: the bytes of its copy in the chunk's block, then the copy itself at blk, enqueued on
+  // ctx->stream: the tables, and utterances [u0, u0 + n)'s group indices and the prefix sums of their bands and band
+  // pairs.  upload fills sp's table and group fields.  With one group sp.ugrp stays null and the sweep runs on the
+  // (band, utterance) grid.
+  size_t chunk_bytes(int n) const;
+  int upload(Ctx *ctx, unsigned char *blk, int u0, int n, SweepParams *sp, GroupTables *gt = nullptr) const;
+ private:
+  struct Part { const void *src; size_t bytes; };
+  std::vector<Part> chunk_parts(int u0, int n, const int *bband, const int *bpair) const;
+};
 
 }  // namespace wb

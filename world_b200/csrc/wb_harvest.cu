@@ -18,36 +18,11 @@
 #include <stdlib.h>
 #include <stdio.h>
 #include <string.h>
-#include <map>
+#include <array>
 #include <string>
 #include <vector>
 
 namespace wb {
-
-// Event-list capacity per band and train: crossings of a signal band-limited around/below
-// `boundary` cannot be denser than ~boundary per second for long; 2.5x margin, hard bound
-// ylen/2+2 (a negative-going crossing needs two samples).  The lists are history rings: more events
-// than this wrap around; only a look-back beyond the last `cap` events raises status bit 4.
-static void plan_edge_caps(const std::vector<double> &boundary, double afs, int max_ylen, bool full,
-                           std::vector<int> *cap, std::vector<long long> *off, size_t *stride) {
-  const int nb = (int)boundary.size();
-  cap->resize(nb); off->resize(nb);
-  long long run = 0;
-  long long floor_cap = 2048;
-  if (const char *e = getenv("WB_EDGE_CAP_MIN")) floor_cap = atoll(e) > 0 ? atoll(e) : floor_cap;   // test hook: force wraps
-  for (int i = 0; i < nb; ++i) {
-    const long long hard = (long long)max_ylen / 2 + 2;
-    long long soft = (long long)(2.5 * boundary[i] * max_ylen / afs) + 64;
-    if (soft < floor_cap) soft = floor_cap;   // a tile can append up to 1025 events per train; the rings look back 256
-    // non-decimated input (ripple path): in digital silence the difference trains fire every sample while the
-    // crossing trains are silent, so frames cannot be finalised until the silence ends -- keep every event
-    if (full) soft = hard;
-    (*cap)[i] = (int)(soft < hard ? soft : hard);
-    (*off)[i] = run;
-    run += 4LL * (*cap)[i];
-  }
-  *stride = (size_t)run;
-}
 
 #define WB_HV_BASE 32        // >= round(channels / 10): base candidates kept per frame
 #define WB_HV_WARPS 4
@@ -956,26 +931,19 @@ WB_KERNEL(128, 4) harvest_smooth_kernel(HvSmoothParams p) {
   }
 }
 
-// The band list of one F0 range: channel boundaries, band-pass filters (Nuttall(2 Lh + 1) * cos, GetFilteredSignal,
-// harvest.cpp:99-110) and the event-list plan.  A batch with several ranges concatenates the lists of its distinct
-// ranges (range groups); each list is what a call with that range alone builds.
-struct HvRange {
-  double f0_floor = 0.0, f0_ceil = 0.0;
-  int nb = 0, max_cand = 0, max_taps = 0, nwin_max = 0;
-  std::vector<double> boundary, taps;      // taps: reversed, 8 zeros after each band
-  std::vector<int> tap_off, ntaps, shift;  // tap_off: into this range's taps
-  std::vector<int> ecap; std::vector<long long> eoff; size_t edge_stride = 0;
-};
+// Candidates kept per frame and the refinement window (samples) of the largest h, for a range's channel count and floor
+static int hv_max_cand(int nb) { return round_half_away(nb / 10.0) * 7; }
+static int hv_nwin(double afs, double f0_floor) { return 2 * static_cast<int>(1.5 * afs / f0_floor + 1.0) + 1 + 2; }
 
-// nullptr, or why the on-chip kernels cannot serve this range
-static const char *hv_plan_range(double f0_floor, double f0_ceil, double afs, int max_ylen, bool full, HvRange *r) {
+// The band list of one F0 range: channel boundaries and band-pass filters (Nuttall(2 Lh + 1) * cos, GetFilteredSignal,
+// harvest.cpp:99-110).  nullptr, or why the on-chip kernels cannot serve this range.
+static const char *hv_band_list(double f0_floor, double f0_ceil, double afs, BandList *r) {
   r->f0_floor = f0_floor; r->f0_ceil = f0_ceil;
   const double adj_floor = f0_floor * 0.9, adj_ceil = f0_ceil * 1.1;
   const int nb = 1 + static_cast<int>(log(adj_ceil / adj_floor) / kLog2 * 40);
   if (nb < 3 || nb > 1024) return "Harvest: bad channel count";
   r->nb = nb;
-  r->max_cand = round_half_away(nb / 10.0) * 7;
-  if (r->max_cand / 7 > WB_HV_BASE) return "Harvest: f0 range too wide (more than 325 channels)";
+  if (hv_max_cand(nb) / 7 > WB_HV_BASE) return "Harvest: f0 range too wide (more than 325 channels)";
   r->boundary.resize(nb);
   for (int i = 0; i < nb; ++i) r->boundary[i] = adj_floor * pow(2.0, (i + 1) / 40.0);
   r->tap_off.resize(nb); r->ntaps.resize(nb); r->shift.resize(nb);
@@ -995,41 +963,13 @@ static const char *hv_plan_range(double f0_floor, double f0_ceil, double afs, in
     if (len > r->max_taps) r->max_taps = len;
   }
   const size_t smem_sweep = sweep_smem_bytes(r->max_taps);
-  const int h_max = static_cast<int>(1.5 * afs / f0_floor + 1.0);
-  r->nwin_max = 2 * h_max + 1 + 2;
+  const int nwin = hv_nwin(afs, f0_floor);
   int lgw = 0;
-  while ((2 << lgw) <= r->nwin_max) ++lgw;
-  const size_t smem_refine = (size_t)WB_HV_WARPS * 3 * r->nwin_max * 8;
+  while ((2 << lgw) <= nwin) ++lgw;
+  const size_t smem_refine = (size_t)WB_HV_WARPS * 3 * nwin * 8;
   if (smem_sweep > 200 * 1024 || smem_refine > 200 * 1024 || (1 << (lgw + 2)) > WB_TW_N)
     return "Harvest: f0_floor too low for the on-chip filters";
-  plan_edge_caps(r->boundary, afs, max_ylen, full, &r->ecap, &r->eoff, &r->edge_stride);
   return nullptr;
-}
-
-// Range groups of a batch: the distinct (f0_floor, f0_ceil) pairs in order of first appearance (keyed by bit pattern),
-// each planned and checked against the on-chip limits when it first appears -- so an error names the first offending
-// utterance.  ugrp[u] = the group of utterance u.
-static int hv_make_groups(Ctx *ctx, const HarvestParams *opts, bool per_utt, int n, double afs, int max_ylen, bool full,
-                          std::vector<HvRange> *groups, std::vector<int> *ugrp) {
-  std::map<std::pair<unsigned long long, unsigned long long>, int> seen;
-  ugrp->resize(n);
-  for (int u = 0; u < n; ++u) {
-    const HarvestParams &o = opts[per_utt ? u : 0];
-    std::pair<unsigned long long, unsigned long long> key;
-    memcpy(&key.first, &o.f0_floor, 8); memcpy(&key.second, &o.f0_ceil, 8);
-    auto it = seen.find(key);
-    if (it == seen.end()) {
-      groups->emplace_back();
-      if (const char *why = hv_plan_range(o.f0_floor, o.f0_ceil, afs, max_ylen, full, &groups->back())) {
-        ctx->last_error = why;
-        if (per_utt) ctx->last_error += " (utterance " + std::to_string(u) + ")";
-        return 3;
-      }
-      it = seen.emplace(key, (int)groups->size() - 1).first;
-    }
-    (*ugrp)[u] = it->second;
-  }
-  return 0;
 }
 
 static int hv_ratio(int fs) { return imax(imin(round_half_away(fs / 8000.0), 12), 1); }   // harvest.cpp:1226, :1158
@@ -1052,9 +992,9 @@ enum { HV_DUMP_DECIMATED, HV_DUMP_RAW, HV_DUMP_BASE, HV_DUMP_REFINED, HV_DUMP_CL
 struct HvDumpPart { const void *dev; size_t bytes; };
 
 static int hv_dump(Ctx *ctx, const char *prefix, int stage, int chunk, int u0, int n, int ratio, double afs, int nb,
-                   int l1_stride, int max_cand, const std::vector<int> &ugrp, const std::vector<HvRange> &groups,
-                   const int *ylen_dev, const int *l1_dev, const int *nc_dev, std::vector<HvDumpPart> parts,
-                   const double *y_rows = nullptr, size_t y_stride = 0) {
+                   int l1_stride, int max_cand, const BandTables &t, const int *ylen_dev, const int *l1_dev,
+                   const int *nc_dev, std::vector<HvDumpPart> parts, const double *y_rows = nullptr,
+                   size_t y_stride = 0) {
   std::vector<int> ylen(n), l1(n), nc(n);
   int rc = dev_sync(ctx);
   if (!rc) rc = dev_memcpy_d2h(ctx, ylen.data(), ylen_dev, (size_t)n * 4);
@@ -1075,13 +1015,15 @@ static int hv_dump(Ctx *ctx, const char *prefix, int stage, int chunk, int u0, i
   const std::string path = std::string(prefix) + "." + std::to_string(chunk);
   FILE *f = fopen(path.c_str(), "wb");
   if (!f) { ctx->last_error = "Harvest: cannot write " + path; return 3; }
-  const long long head[10] = {1, stage, chunk, u0, n, ratio, nb, l1_stride, max_cand, (long long)groups.size()};
+  const long long head[10] = {1, stage, chunk, u0, n, ratio, nb, l1_stride, max_cand, (long long)t.grp_nb.size()};
   fwrite("WBHVDUMP", 1, 8, f);
   fwrite(head, 8, 10, f);
   fwrite(&afs, 8, 1, f);
-  fwrite(ugrp.data() + u0, 4, n, f);
+  fwrite(t.ugrp.data() + u0, 4, n, f);
   fwrite(ylen.data(), 4, n, f); fwrite(l1.data(), 4, n, f); fwrite(nc.data(), 4, n, f);
-  for (const HvRange &r : groups) { fwrite(&r.nb, 4, 1, f); fwrite(&r.f0_floor, 8, 1, f); fwrite(&r.f0_ceil, 8, 1, f); }
+  for (size_t g = 0; g < t.grp_nb.size(); ++g) {
+    fwrite(&t.grp_nb[g], 4, 1, f); fwrite(&t.grp_floor[g], 8, 1, f); fwrite(&t.grp_ceil[g], 8, 1, f);
+  }
   for (const auto &h : host) fwrite(h.data(), 1, h.size(), f);
   fclose(f);
   return 0;
@@ -1125,49 +1067,36 @@ static int hv_load_refined(Ctx *ctx, const char *prefix, int chunk, int n, int l
   return rc;
 }
 
-int harvest_check_options(Ctx *ctx, int fs, const HarvestParams *opts, int n) {
-  std::vector<HvRange> groups;
-  std::vector<int> ugrp;
-  const int ratio = hv_ratio(fs);
-  return hv_make_groups(ctx, opts, true, n, static_cast<double>(fs) / ratio, 1, ratio == 1, &groups, &ugrp);
+int harvest_plan(Ctx *ctx, int fs, const HarvestOption *opts, int n, bool per_utt, double frame_period,
+                 RangeGroups *g) {
+  for (int u = 0; per_utt && u < n; ++u)
+    if (!(opts[u].frame_period == frame_period)) {
+      ctx->last_error = "harvest options: frame_period differs from the batch's (utterance " + std::to_string(u) + ")";
+      return 3;
+    }
+  const double afs = static_cast<double>(fs) / hv_ratio(fs);
+  return group_ranges(
+      ctx, n, per_utt, [&](int i) { return std::array<double, 3>{opts[i].f0_floor, opts[i].f0_ceil, 0.0}; },
+      [&](int i, BandList *r) { return hv_band_list(opts[i].f0_floor, opts[i].f0_ceil, afs, r); }, g);
 }
 
-int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_utt, double *time_axis_out,
+int harvest_run(Ctx *ctx, const Batch &b, double frame_period, const RangeGroups &groups, double *time_axis_out,
                 double *f0_out) {
   if (b.n <= 0) return 0;
   const int fs = b.fs;
   const int ratio = hv_ratio(fs);
   const double afs = static_cast<double>(fs) / ratio;
-  const double frame_period = opts[0].frame_period;   // equal for every utterance (checked by the ABI layer)
   // sizes on the 1 ms grid (b.l1_host: per-utterance frame counts at 1 ms, from the ABI layer)
   const int max_ylen = static_cast<int>(ceil(static_cast<double>(b.max_x_len) / ratio));
   const int l1_stride = static_cast<int>(1000.0 * b.max_x_len / fs / 1.0) + 1;
-  std::vector<HvRange> groups;
-  std::vector<int> ugrp;
-  const int rc0 = hv_make_groups(ctx, opts, per_utt, b.n, afs, max_ylen, ratio == 1, &groups, &ugrp);
-  if (rc0) return rc0;
-  // the band tables of every group one after the other; scratch strides follow the batch maxima
-  const int n_groups = (int)groups.size();
-  std::vector<double> taps, boundary, grp_floor(n_groups), grp_ceil(n_groups);
-  std::vector<int> tap_off, ntaps, shift, ecap, grp_band0(n_groups), grp_nb(n_groups);
-  std::vector<long long> eoff;
-  int nb = 0, max_cand = 0, max_taps = 0, nwin_max = 0;   // batch maxima
-  size_t edge_stride = 0;
-  for (int g = 0; g < n_groups; ++g) {
-    const HvRange &r = groups[g];
-    grp_band0[g] = (int)boundary.size(); grp_nb[g] = r.nb; grp_floor[g] = r.f0_floor; grp_ceil[g] = r.f0_ceil;
-    for (int i = 0; i < r.nb; ++i) tap_off.push_back((int)taps.size() + r.tap_off[i]);
-    taps.insert(taps.end(), r.taps.begin(), r.taps.end());
-    boundary.insert(boundary.end(), r.boundary.begin(), r.boundary.end());
-    ntaps.insert(ntaps.end(), r.ntaps.begin(), r.ntaps.end());
-    shift.insert(shift.end(), r.shift.begin(), r.shift.end());
-    ecap.insert(ecap.end(), r.ecap.begin(), r.ecap.end());
-    eoff.insert(eoff.end(), r.eoff.begin(), r.eoff.end());
-    nb = imax(nb, r.nb); max_cand = imax(max_cand, r.max_cand); max_taps = imax(max_taps, r.max_taps);
-    nwin_max = imax(nwin_max, r.nwin_max);
-    if (r.edge_stride > edge_stride) edge_stride = r.edge_stride;
+  const BandTables tab(groups, afs, max_ylen, ratio == 1);
+  const int nb = tab.nb, max_taps = tab.max_taps;
+  const size_t edge_stride = tab.edge_stride;
+  int max_cand = 0, nwin_max = 0;   // batch maxima
+  for (const BandList &r : groups.lists) {
+    max_cand = imax(max_cand, hv_max_cand(r.nb));
+    nwin_max = imax(nwin_max, hv_nwin(afs, r.f0_floor));
   }
-  const int n_tab = (int)boundary.size();   // rows of the band tables
   const size_t smem_refine = (size_t)WB_HV_WARPS * 3 * nwin_max * 8;
   const int T = WB_SWEEP_T;
   const int padl = max_taps + 16;
@@ -1201,7 +1130,6 @@ int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_ut
     const size_t o_l1 = plan.add((size_t)n * 4), o_nc = plan.add((size_t)n * 4);
     const size_t o_nyq = plan.add((size_t)n * 32), o_nfft = plan.add((size_t)n * 4);
     const size_t o_edges = plan.add((size_t)n * edge_stride * 8);
-    const size_t o_ecap = plan.add(n_tab * 4), o_eoff = plan.add(n_tab * 8);
     const size_t o_evc = plan.add((size_t)n * nb * 16), o_redo = plan.add((size_t)n * nb * 4), o_nredo = plan.add(4);
     const size_t o_raw = plan.add((size_t)n * nb * l1_stride * 8);
     const size_t o_base = plan.add((size_t)n * l1_stride * WB_HV_BASE * 8), o_bcnt = plan.add((size_t)n * l1_stride * 4);
@@ -1214,48 +1142,23 @@ int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_ut
     const size_t o_stmp = plan.add((size_t)n * sec_slots * seg_cap * 8);
     const size_t o_basic = plan.add((size_t)n * l1_stride * 8);
     const size_t o_tmp = plan.add((size_t)n * tmp_stride * 8);
-    const size_t o_taps = plan.add(taps.size() * 8);
-    const size_t o_toff = plan.add(n_tab * 4), o_nt = plan.add(n_tab * 4), o_sh = plan.add(n_tab * 4), o_bd = plan.add(n_tab * 8);
-    const size_t o_ugrp = plan.add((size_t)n * 4), o_gb0 = plan.add(n_groups * 4), o_gnb = plan.add(n_groups * 4);
-    const size_t o_gfl = plan.add(n_groups * 8), o_gce = plan.add(n_groups * 8);
-    const size_t o_bband = plan.add((size_t)(n + 1) * 4), o_bpair = plan.add((size_t)(n + 1) * 4);
+    const size_t o_tab = plan.add(tab.chunk_bytes(n));
     unsigned char *blk = arena_block(ctx, plan.total);
     if (!blk) return 2;
     double *y = (double *)(blk + o_y);
     int *ylen = (int *)(blk + o_ylen), *l1 = (int *)(blk + o_l1), *nc = (int *)(blk + o_nc);
     auto dump_stage = [&](int stage, std::vector<HvDumpPart> parts, const double *y_rows = nullptr) {
-      return hv_dump(ctx, dump[stage], stage, u0 / chunk, u0, n, ratio, afs, nb, l1_stride, max_cand, ugrp, groups,
-                     ylen, l1, nc, parts, y_rows, y_stride);
+      return hv_dump(ctx, dump[stage], stage, u0 / chunk, u0, n, ratio, afs, nb, l1_stride, max_cand, tab, ylen, l1, nc,
+                     parts, y_rows, y_stride);
     };
     int rc = dev_memset(ctx, y, 0, (size_t)n * y_stride * 8);
     if (!rc) rc = dev_memset(ctx, nc, 0, (size_t)n * 4);
     if (!rc) rc = dev_memcpy_h2d(ctx, l1, b.l1_host + u0, (size_t)n * 4);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_taps, taps.data(), taps.size() * 8);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_toff, tap_off.data(), n_tab * 4);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_nt, ntaps.data(), n_tab * 4);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_sh, shift.data(), n_tab * 4);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_bd, boundary.data(), n_tab * 8);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_ecap, ecap.data(), n_tab * 4);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_eoff, eoff.data(), n_tab * 8);
-    // range groups of this chunk's utterances and the first block of each in the flat band / band-pair grids
-    std::vector<int> bband(n + 1), bpair(n + 1);
-    bband[0] = bpair[0] = 0;
-    for (int i = 0; i < n; ++i) {
-      const int nbu = grp_nb[ugrp[u0 + i]];
-      bband[i + 1] = bband[i] + nbu;
-      bpair[i + 1] = bpair[i] + (nbu + 1) / 2;
-    }
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_ugrp, ugrp.data() + u0, (size_t)n * 4);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_gb0, grp_band0.data(), n_groups * 4);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_gnb, grp_nb.data(), n_groups * 4);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_gfl, grp_floor.data(), n_groups * 8);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_gce, grp_ceil.data(), n_groups * 8);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_bband, bband.data(), (size_t)(n + 1) * 4);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_bpair, bpair.data(), (size_t)(n + 1) * 4);
+    SweepParams sp;
+    GroupTables gt;
+    if (!rc) rc = tab.upload(ctx, blk + o_tab, u0, n, &sp, &gt);
     if (rc) return rc;
-    HvGroups gr;
-    gr.ugrp = (const int *)(blk + o_ugrp); gr.grp_nb = (const int *)(blk + o_gnb);
-    gr.grp_floor = (const double *)(blk + o_gfl); gr.grp_ceil = (const double *)(blk + o_gce);
+    const HvGroups gr = {gt.ugrp, gt.grp_nb, gt.grp_floor, gt.grp_ceil};
 
     HvPrepParams pp;
     pp.x = b.x + (size_t)u0 * b.x_stride; pp.x_len = b.x_len + u0; pp.x_stride = b.x_stride; pp.ratio = ratio;
@@ -1270,21 +1173,9 @@ int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_ut
     WB_LAUNCH_COOP(harvest_prep_kernel, dim3((unsigned)n), 256, 0, ctx->stream, pp);
     if (dump[HV_DUMP_DECIMATED] && (rc = dump_stage(HV_DUMP_DECIMATED, {}, y + padl))) return rc;
 
-    SweepParams sp;
-    sp.sig = y; sp.sig_stride = y_stride; sp.sig_origin = padl; sp.y_len = ylen; sp.n_bands = nb;
-    sp.taps_rev = (const double *)(blk + o_taps); sp.tap_off = (const int *)(blk + o_toff);
-    sp.ntaps = (const int *)(blk + o_nt); sp.shift = (const int *)(blk + o_sh);
-    sp.boundary = (const double *)(blk + o_bd); sp.afs = afs;
-    sp.edges = (double *)(blk + o_edges); sp.edge_stride = edge_stride;
-    sp.edge_cap = (const int *)(blk + o_ecap); sp.edge_off = (const long long *)(blk + o_eoff);
-    sp.n_frames = l1; sp.frame_stride = l1_stride; sp.frame_period = 1.0;
-    sp.mode = 1; sp.f0_floor = groups[0].f0_floor; sp.f0_ceil = groups[0].f0_ceil;
-    if (n_groups > 1) {   // one group: bands 0 .. nb - 1 of the tables and the (band, utterance) grid, as without groups
-      sp.ugrp = gr.ugrp; sp.grp_band0 = (const int *)(blk + o_gb0); sp.grp_nb = gr.grp_nb;
-      sp.grp_floor = gr.grp_floor; sp.grp_ceil = gr.grp_ceil;
-      sp.blk0_band = (const int *)(blk + o_bband); sp.blk0_pair = (const int *)(blk + o_bpair);
-      sp.n_blk_band = bband[n]; sp.n_blk_pair = bpair[n]; sp.n_utts = n;
-    }
+    sp.sig = y; sp.sig_stride = y_stride; sp.sig_origin = padl; sp.y_len = ylen; sp.afs = afs;
+    sp.edges = (double *)(blk + o_edges);
+    sp.n_frames = l1; sp.frame_stride = l1_stride; sp.frame_period = 1.0; sp.mode = 1;
     sp.nyq = nullptr; sp.ripple = 0;
     if (ratio == 1 && !getenv("WB_NO_RIPPLE")) {
       // Input not decimated (fs below 12 kHz): exact zeros in the waveform reach the band filters, and there the
@@ -1294,7 +1185,7 @@ int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_ut
       for (int i = 0; i < n; ++i) {
         const int xl = b.x_len_host ? b.x_len_host[u0 + i] : b.x_stride;
         const int yl = static_cast<int>(ceil(static_cast<double>(xl) / ratio));
-        const int sample = yl + 5 + 2 * static_cast<int>(2.0 * afs / groups[ugrp[u0 + i]].boundary[0]);
+        const int sample = yl + 5 + 2 * static_cast<int>(2.0 * afs / groups.lists[groups.ugrp[u0 + i]].boundary[0]);
         nfft[i] = static_cast<int>(pow(2.0, static_cast<int>(log(static_cast<double>(sample)) / kLog2) + 1.0));
       }
       rc = dev_memcpy_h2d(ctx, blk + o_nfft, nfft.data(), (size_t)n * 4);
@@ -1305,8 +1196,7 @@ int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_ut
       launch_nyquist_bins(ctx, np_, (unsigned)n);
       sp.nyq = (const double *)(blk + o_nyq); sp.ripple = 1;
     }
-    sp.cand = (double *)(blk + o_raw); sp.score = nullptr;
-    sp.max_taps = max_taps; sp.status = ctx->status_dev;
+    sp.cand = (double *)(blk + o_raw); sp.score = nullptr; sp.status = ctx->status_dev;
     sp.ev_count = (int *)(blk + o_evc); sp.redo_list = (int *)(blk + o_redo); sp.redo_count = (int *)(blk + o_nredo);
     if (!sp.ripple && !getenv("WB_SWEEP_STREAMING") && fe_smem_bytes(max_taps) <= 200 * 1024) {
       // decimated input (every rate from 12 kHz up): FIR + events, then interpolation (wb_f0common.cu)

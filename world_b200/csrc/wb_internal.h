@@ -3,6 +3,8 @@
 #include "wb_platform.cuh"
 #include "wb_block.cuh"
 #include "wb_fft.cuh"
+#include "../../include/world/dio.h"
+#include "../../include/world/harvest.h"
 #include <string>
 #include <vector>
 
@@ -249,16 +251,19 @@ struct D4cPerUtt {
 int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *aperiodicity,
             const CodecTables *coded = nullptr, double *coded_out = nullptr, const D4cPerUtt *per_utt = nullptr);
 int stonemask_run(Ctx *ctx, const Batch &b, double *refined_f0);
-struct DioParams { double f0_floor, f0_ceil, channels_in_octave, frame_period, allowed_range; int speed; };
-// per_utt: opts[u] is utterance u's option (f0_floor / f0_ceil / channels_in_octave / allowed_range may differ,
-// frame_period and speed may not); else opts[0] for all
-int dio_run(Ctx *ctx, const Batch &b, const DioParams *opts, bool per_utt, double *time_axis_out, double *f0_out);
-// the range checks of dio_run for n per-utterance options; 3 (EINVAL) + last_error naming the first bad utterance
-int dio_check_options(Ctx *ctx, int fs, const DioParams *opts, int n);
-struct HarvestParams { double f0_floor, f0_ceil, frame_period; };
-// per_utt: opts[u] is utterance u's option (f0_floor / f0_ceil may differ, frame_period may not); else opts[0] for all
-int harvest_run(Ctx *ctx, const Batch &b, const HarvestParams *opts, bool per_utt, double *time_axis_out, double *f0_out);
-// the range checks of harvest_run for n per-utterance options; 3 (EINVAL) + last_error naming the first bad utterance
-int harvest_check_options(Ctx *ctx, int fs, const HarvestParams *opts, int n);
+// The F0 estimators (wb_harvest.cu, wb_dio.cu) take the public options.  Per utterance (per_utt: opts[u] is utterance
+// u's, else opts[0] serves all), the F0 range may differ, frame_period (DIO: and speed) may not.  *_plan checks that
+// frame_period (and speed) against the batch's, then groups the utterances by range and builds each group's band list
+// (wb_f0common.cuh): 3 (EINVAL) + last_error naming the first bad utterance.  It queues nothing, so a call runs it
+// before its lengths are uploaded, and *_run takes its groups.
+struct RangeGroups;
+int harvest_plan(Ctx *ctx, int fs, const HarvestOption *opts, int n, bool per_utt, double frame_period,
+                 RangeGroups *groups);
+int harvest_run(Ctx *ctx, const Batch &b, double frame_period, const RangeGroups &groups, double *time_axis_out,
+                double *f0_out);
+int dio_plan(Ctx *ctx, int fs, const DioOption *opts, int n, bool per_utt, double frame_period, int speed,
+             RangeGroups *groups);
+int dio_run(Ctx *ctx, const Batch &b, const DioOption *opts, bool per_utt, const RangeGroups &groups,
+            double *time_axis_out, double *f0_out);
 
 }  // namespace wb
