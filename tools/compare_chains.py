@@ -1,14 +1,18 @@
-"""Compares two builds of the library call by call: every analysis chain entry point and voice transformation on seeded
-ragged batches, with each call's return code, launch count and outputs required to be identical byte for byte.  Meant
-for a refactor of the chain drivers, with the parent commit's build as A and the change's as B (on the host emulation,
-two tests/emu builds; on a GPU, two libworld_b200.so with --device).
+"""Compares two builds of the library call by call: every analysis chain entry point, voice transformation, every
+synthesis entry point and modify on seeded ragged batches, with each call's return code, launch count and outputs
+required to be identical byte for byte.  Meant for a refactor of the chain or synthesis drivers, with the parent
+commit's build as A and the change's as B (on the host emulation, two tests/emu builds; on a GPU, two libworld_b200.so
+with --device).
 
     python tools/compare_chains.py A.so B.so [--device]
 
-Covers 8 and 16 kHz (16 kHz has one aperiodicity band, 8 kHz none), float64 and 16-bit PCM input, Harvest and DIO,
-no options, per-utterance F0 options, per-utterance CheapTrick / D4C options with two FFT sizes, NULL spectrogram /
-aperiodicity, transform with all three factors, and the host pipelines with small chunks (WB_HOST_CHUNK / WB_HOST_SUB).
-Prints the number of calls compared; exits 1 on the first difference."""
+Analysis covers 8 and 16 kHz (16 kHz has one aperiodicity band, 8 kHz none), float64 and 16-bit PCM input, Harvest
+and DIO, no options, per-utterance F0 options, per-utterance CheapTrick / D4C options with two FFT sizes, NULL
+spectrogram / aperiodicity, transform with all three factors, and the host pipelines with small chunks (WB_HOST_CHUNK /
+WB_HOST_SUB).  Synthesis covers the same two rates: full rows, coded rows to float64 and int16 on device and host
+arrays, with and without f0_scale / spectral_ratio, and modify, on rows made by numpy (one full-length utterance's f0
+is above 1.2 kHz, so its pass is laid out again), at the default scratch budget and at the smallest one (several
+passes and host chunks).  Prints the number of calls compared; exits 1 on the first difference."""
 import argparse
 import ctypes as C
 import os
@@ -124,6 +128,100 @@ def to_np(a):
     return np.asarray(a)
 
 
+def synthesis_rows(fs, seed, n=5, fft=1024, seconds=1.5, fp=5.0):
+    """f0, full rows and coded rows of n ragged utterances, all from numpy.  Utterance 1 is at 1.5 kHz and as long as
+    the longest row: its 2,250 pulses exceed the 1,864 the pulse arrays are first sized for, so its pass is laid out
+    again."""
+    rng = np.random.default_rng(seed)
+    Y, L, bins, n_ap = int(fs * seconds), int(seconds * 1000 / fp) + 1, fft // 2 + 1, 1 if fs == 16000 else 0
+    ylens = [Y, Y] + [int(Y * f) for f in rng.uniform(0.6, 1.0, n - 2)]
+    flens = [min(L, int(y / fs * 1000 / fp) + 2) for y in ylens]
+    k = np.arange(bins) / bins
+    f0, sp, ap = np.zeros((n, L)), np.ones((n, L, bins)), np.ones((n, L, bins))
+    csp, cap = np.zeros((n, L, DIMS)), np.zeros((n, L, max(n_ap, 1)))
+    for u, m in enumerate(flens):
+        f0[u, :m] = np.where(rng.uniform(size=m) < 0.85, rng.uniform(90.0, 300.0), 0.0)
+        sp[u, :m] = np.exp(-6.0 * k[None, :] + 0.3 * rng.normal(size=(m, 1))) * 1e-3
+        ap[u, :m] = np.clip(k[None, :] ** 2 + 0.05 * rng.uniform(size=(m, bins)), 1e-3, 1 - 1e-12)
+        csp[u, :m, 0] = -7.0 + 0.3 * rng.normal(size=m)
+        csp[u, :m, 1:] = 0.3 * rng.normal(size=(m, DIMS - 1)) / np.arange(2, DIMS + 1)
+        cap[u, :m] = -rng.uniform(1.0, 30.0, size=(m, cap.shape[2]))
+    f0[1, :flens[1]] = 1500.0
+    return f0, sp, ap, csp, (cap if n_ap else None), fft, fp, Y, flens, ylens
+
+
+def synthesis_calls_at(w, arr, fs):
+    """(name, thunk) pairs of the synthesis entry points and modify at one rate.  The thunks run after the whole list
+    is built, so they read only this call's locals (and their own default arguments)."""
+    f0, sp, ap, csp, cap, fft, fp, Y, fl, yl = synthesis_rows(fs, fs + 1)
+    n, L = len(fl), f0.shape[1]
+    factors = dict(f0_scale=[1.1 + 0.05 * u for u in range(n)], spectral_ratio=[0.9 + 0.05 * u for u in range(n)])
+    out = [(f"synthesis fs {fs}", lambda: [w.synthesis(arr(f0), arr(sp), arr(ap), fft, fp, fs, Y, f0_lengths=fl,
+                                                       y_lengths=yl)])]
+    for dtype in ("float64", "int16"):
+        for kw in ({}, factors):
+            tag = f"fs {fs} {dtype}{' factors' if kw else ''}"
+            out.append((f"synthesis_coded {tag}", lambda dtype=dtype, kw=kw: [w.synthesis_coded(
+                arr(f0), arr(csp), arr(cap), fft, fp, fs, Y, f0_lengths=fl, y_lengths=yl, dtype=dtype, **kw)]))
+            out.append((f"synthesis_coded_host {tag}", lambda dtype=dtype, kw=kw: [w.synthesis_coded_host(
+                f0, csp, cap, fft, fp, fs, Y, f0_lengths=fl, y_lengths=yl, nbit=16 if dtype == "int16" else 0,
+                **kw)]))
+
+    # the plain entry points without factors, called directly
+    def plain(entry, nbit, host):
+        y = np.zeros((n, Y), dtype=np.int16 if nbit else np.float64)
+        y = y if host else arr(y)
+        src = (f0, csp, cap) if host else (arr(f0), arr(csp), arr(cap))
+        head = (w._h, _ptr(src[0]), (C.c_int * n)(*fl), n, L, _ptr(src[1]), DIMS, _ptr(src[2]), fft, fp, fs,
+                (C.c_int * n)(*yl), Y)
+        rc = getattr(w.lib, entry)(*head, *((nbit,) if host else ()), _ptr(y))
+        return [np.array([rc]), y]
+    out.append((f"world_b200_synthesis_coded_batch fs {fs}", lambda: plain("world_b200_synthesis_coded_batch", 0,
+                                                                             False)))
+    out.append((f"world_b200_synthesis_coded_batch_pcm16 fs {fs}",
+                lambda: plain("world_b200_synthesis_coded_batch_pcm16", 16, False)))
+    for nbit in (0, 16):
+        out.append((f"world_b200_synthesis_coded_host nbit {nbit} fs {fs}",
+                    lambda nbit=nbit: plain("world_b200_synthesis_coded_host", nbit, True)))
+    out.append((f"modify fs {fs}", lambda: list(w.modify(arr(f0.copy()), arr(sp.copy()), fs, fft, f0_lengths=fl,
+                                                          **factors))))
+    return out
+
+
+def synthesis_calls(w, device):
+    """(name, thunk) pairs of the synthesis entry points and modify at 8 and 16 kHz."""
+    def arr(a):
+        if not device or a is None:
+            return a
+        import torch
+        return torch.from_numpy(np.ascontiguousarray(a)).cuda()
+
+    return synthesis_calls_at(w, arr, 8000) + synthesis_calls_at(w, arr, 16000)
+
+
+def compare(worlds, lists, label):
+    """Runs each pair of calls on the two builds; exits 1 on the first difference.  Returns the number compared."""
+    compared = 0
+    for (name, fa), (_, fb) in zip(*lists):
+        res = []
+        for w, fn in zip(worlds, (fa, fb)):
+            before = w.launch_count()
+            try:
+                outs, err = fn(), None
+            except Exception as e:   # both builds must fail the same way
+                outs, err = (), str(e)
+            w.synchronize()
+            res.append((err, w.launch_count() - before, [to_np(o).tobytes() for o in outs]))
+        if res[0] != res[1]:
+            print(f"DIFFERENT: {name} ({label}): errors {res[0][0]!r} / {res[1][0]!r}, launches "
+                  f"{res[0][1]} / {res[1][1]}, outputs equal: {res[0][2] == res[1][2]}")
+            sys.exit(1)
+        if res[0][0]:
+            print(f"note: both builds raised for {name}: {res[0][0]}")
+        compared += 1
+    return compared
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("lib_a")
@@ -131,7 +229,8 @@ def main():
     ap.add_argument("--device", action="store_true", help="CUDA builds, device arrays as torch tensors")
     args = ap.parse_args()
     mod = None if args.device else "numpy"
-    worlds = [World(lib_path=p, array_module=mod or "torch") for p in (args.lib_a, args.lib_b)]
+    libs = (args.lib_a, args.lib_b)
+    worlds = [World(lib_path=p, array_module=mod or "torch") for p in libs]
     compared = 0
     for chunks in ((None, None), ("2", "1")):
         for k, v in zip(("WB_HOST_CHUNK", "WB_HOST_SUB"), chunks):
@@ -139,24 +238,15 @@ def main():
                 os.environ.pop(k, None)
             else:
                 os.environ[k] = v
-        lists = [calls(w, args.device) for w in worlds]
-        for (name, fa), (_, fb) in zip(*lists):
-            res = []
-            for w, fn in zip(worlds, (fa, fb)):
-                before = w.launch_count()
-                try:
-                    outs, err = fn(), None
-                except Exception as e:   # both builds must fail the same way
-                    outs, err = (), str(e)
-                w.synchronize()
-                res.append((err, w.launch_count() - before, [to_np(o).tobytes() for o in outs]))
-            if res[0] != res[1]:
-                print(f"DIFFERENT: {name} (chunks {chunks}): errors {res[0][0]!r} / {res[1][0]!r}, launches "
-                      f"{res[0][1]} / {res[1][1]}, outputs equal: {res[0][2] == res[1][2]}")
-                sys.exit(1)
-            if res[0][0]:
-                print(f"note: both builds raised for {name}: {res[0][0]}")
-            compared += 1
+        compared += compare(worlds, [calls(w, args.device) for w in worlds], f"chunks {chunks}")
+    for k in ("WB_HOST_CHUNK", "WB_HOST_SUB"):
+        os.environ.pop(k, None)
+    # synthesis at the default scratch budget, then at the smallest one (64 MB: several passes and host chunks)
+    small = [World(lib_path=p, array_module=mod or "torch") for p in libs]
+    for w in small:
+        w.set_scratch_budget(64 << 20)
+    for ws, label in ((worlds, "default budget"), (small, "64 MB budget")):
+        compared += compare(ws, [synthesis_calls(w, args.device) for w in ws], label)
     print(f"{compared} calls compared, all identical (return codes, launch counts, output bytes)")
 
 

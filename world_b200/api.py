@@ -683,17 +683,11 @@ class World:
         fl, k1 = _int_array(f0_lengths, n)
         yl, k2 = _int_array(y_lengths, n)
         self._use_current_stream()
-        if f0_scale is not None or spectral_ratio is not None:
-            self._check(self.lib.world_b200_synthesis_coded_batch_modified(
-                self._h, _ptr(f0), fl, n, f0.shape[1], _ptr(coded_spectral_envelope),
-                int(coded_spectral_envelope.shape[-1]), _ptr(coded_aperiodicity), fft_size, frame_period, fs, yl,
-                y_length, _factors(f0_scale, n, "f0_scale"), _factors(spectral_ratio, n, "spectral_ratio"),
-                16 if pcm16 else 0, _ptr(y)))
-            return y
-        fn = self.lib.world_b200_synthesis_coded_batch_pcm16 if pcm16 else self.lib.world_b200_synthesis_coded_batch
-        self._check(fn(self._h, _ptr(f0), fl, n, f0.shape[1], _ptr(coded_spectral_envelope),
-                       int(coded_spectral_envelope.shape[-1]), _ptr(coded_aperiodicity), fft_size, frame_period, fs,
-                       yl, y_length, _ptr(y)))
+        self._check(self.lib.world_b200_synthesis_coded_batch_modified(
+            self._h, _ptr(f0), fl, n, f0.shape[1], _ptr(coded_spectral_envelope),
+            int(coded_spectral_envelope.shape[-1]), _ptr(coded_aperiodicity), fft_size, frame_period, fs, yl,
+            y_length, _factors(f0_scale, n, "f0_scale"), _factors(spectral_ratio, n, "spectral_ratio"),
+            16 if pcm16 else 0, _ptr(y)))
         return y
 
     def modify(self, f0, spectrogram, fs, fft_size, f0_scale=None, spectral_ratio=None, f0_lengths=None):
@@ -737,15 +731,10 @@ class World:
             raise ValueError(f"out: a contiguous [{n}, {y_length}] {'int16' if nbit == 16 else 'float64'} host array")
         fl, k1 = _int_array(f0_lengths, n)
         yl, k2 = _int_array(y_lengths, n)
-        if f0_scale is not None or spectral_ratio is not None:
-            self._check(self.lib.world_b200_synthesis_coded_host_modified(
-                self._h, _ptr(f0), fl, n, f0.shape[1], _ptr(coded_sp), int(coded_sp.shape[-1]), _ptr(coded_ap),
-                fft_size, frame_period, fs, yl, y_length, _factors(f0_scale, n, "f0_scale"),
-                _factors(spectral_ratio, n, "spectral_ratio"), nbit, _ptr(y)))
-            return y
-        self._check(self.lib.world_b200_synthesis_coded_host(self._h, _ptr(f0), fl, n, f0.shape[1], _ptr(coded_sp),
-                                                             int(coded_sp.shape[-1]), _ptr(coded_ap), fft_size,
-                                                             frame_period, fs, yl, y_length, nbit, _ptr(y)))
+        self._check(self.lib.world_b200_synthesis_coded_host_modified(
+            self._h, _ptr(f0), fl, n, f0.shape[1], _ptr(coded_sp), int(coded_sp.shape[-1]), _ptr(coded_ap),
+            fft_size, frame_period, fs, yl, y_length, _factors(f0_scale, n, "f0_scale"),
+            _factors(spectral_ratio, n, "spectral_ratio"), nbit, _ptr(y)))
         return y
 
     def analysis_option(self, fs, f0_method=F0_HARVEST) -> AnalysisOption:

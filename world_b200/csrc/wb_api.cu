@@ -1104,13 +1104,11 @@ int world_b200_analyze_batch_dio_options(WorldB200 *h, const double *x, int n, i
 // ---- voice transformation: analysis, modification and synthesis in one call (world_b200_transform_*)
 namespace wb {
 
-// Every check of the call before any work is queued (EINVAL, last_error naming the first bad utterance): the analysis
-// plan, then the output lengths and synthesis frame periods.
+// Every check of the call before any work is queued (EINVAL, last_error naming the first bad utterance): y, nbit_out,
+// the analysis plan and time_scale here, then the synthesis plan of the analysis rows.
 int transform_check(WorldB200 *h, const ChainRequest &r, const double *f0_scale, const double *spectral_ratio,
-                    const double *time_scale, int nbit_out, const void *y, int y_stride, const char *who,
-                    TransformPlan *tp) {
+                    const double *time_scale, int nbit_out, void *y, int y_stride, const char *who, TransformPlan *tp) {
   Ctx *c = &h->c;
-  char msg[256];
   auto fail = [&](const char *what) {
     c->last_error = std::string(who) + ": " + what;
     return WORLD_B200_EINVAL;
@@ -1118,33 +1116,24 @@ int transform_check(WorldB200 *h, const ChainRequest &r, const double *f0_scale,
   if (!y || y_stride <= 0) return fail("y must be given, with y_stride > 0");
   if (nbit_out != 0 && nbit_out != 16) return fail("nbit_out must be 0 (float64) or 16 (int16)");
   const ChainPlan &p = tp->chain;
-  int rc = chain_plan(c, r, who, &tp->chain);
-  if (!rc) rc = synthesis_fft(c, r.opt->cheaptrick.fft_size, &tp->lg);
+  const int rc = chain_plan(c, r, who, &tp->chain);
   if (rc) return rc;
-  tp->modify = f0_scale || spectral_ratio;
-  if (tp->modify) rc = modify_plan(c, r.n, r.opt->cheaptrick.fft_size, r.fs, f0_scale, spectral_ratio, &tp->mod);
-  if (rc) return rc;
-  tp->nbit_out = nbit_out; tp->y_stride = y_stride;
-  tp->y_len.resize(r.n); tp->fp.resize(r.n);
+  std::vector<int> y_len(r.n);
+  std::vector<double> fp(r.n);
   for (int u = 0; u < r.n; ++u) {
-    const int xl = r.x_lengths ? r.x_lengths[u] : r.x_stride;
     const double ts = time_scale ? time_scale[u] : 1.0;
     if (!(ts > 0.0) || !isfinite(ts)) {
+      char msg[256];
       snprintf(msg, sizeof msg, "time_scale[%d] = %.17g is not a finite factor > 0", u, ts);
       return fail(msg);
     }
-    tp->y_len[u] = world_b200_transform_samples(r.fs, xl, p.frame_period, ts);
-    if (p.f_len[u] < 2) {
-      snprintf(msg, sizeof msg, "utterance %d has %d frame(s); Synthesis needs 2", u, p.f_len[u]);
-      return fail(msg);
-    }
-    if (tp->y_len[u] < 2 || tp->y_len[u] > y_stride) {
-      snprintf(msg, sizeof msg, "y_length of utterance %d is %d, outside [2, y_stride = %d]", u, tp->y_len[u], y_stride);
-      return fail(msg);
-    }
-    tp->fp[u] = (p.frame_period * ts) / 1000.0;   // synthesis_batch's frame_period / 1000.0, with the same product
+    y_len[u] = world_b200_transform_samples(r.fs, r.x_lengths ? r.x_lengths[u] : r.x_stride, p.frame_period, ts);
+    fp[u] = (p.frame_period * ts) / 1000.0;   // synthesis_batch's frame_period / 1000.0, with the same product
   }
-  return 0;
+  SynthesisRequest s{nullptr, p.f_len.data(), r.n, p.f0_stride, nullptr, nullptr, r.opt->cheaptrick.fft_size,
+                     p.frame_period, r.fs, y_len.data(), y_stride, y, nbit_out};
+  s.f0_scale = f0_scale; s.spectral_ratio = spectral_ratio; s.transform = true; s.fp = fp.data();
+  return synthesis_plan(c, s, who, &tp->syn);
 }
 
 // Utterances [u0, u0 + n) of a checked call: x and y point at utterance u0's rows (DEVICE); the request's x_lengths and
@@ -1160,7 +1149,8 @@ int transform_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, 
   if (n <= 0) return 0;
   const ChainPlan &p = tp.chain;
   const int f0_stride = p.f0_stride, x_stride = r.x_stride, fft_size = r.opt->cheaptrick.fft_size, nbit = r.nbit;
-  const size_t in_row = (size_t)x_stride * (nbit ? nbit / 8 : 8), out_row = (size_t)tp.y_stride * (tp.nbit_out ? 2 : 8);
+  const size_t in_row = (size_t)x_stride * (nbit ? nbit / 8 : 8);
+  const size_t out_row = (size_t)tp.syn.y_stride * (tp.syn.nbit ? 2 : 8);
   struct Rows {
     size_t x, t, f, sp, ap, total;
     Rows(int m, int nbit, int x_stride, int f0_stride, int bins) {
@@ -1208,17 +1198,14 @@ int transform_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, 
     if (!e) e = dev_memset(&L->c, f, 0, (size_t)m * f0_stride * 8);
     if (!e) e = chain_f0(L, r, p, g, m, xs, t, f);
     if (!e) e = chain_spectral(L, r, p, g, m, xs, t, f, sp, ap);
-    if (!e && tp.modify) e = modify_run(&L->c, tp.mod, g, m, p.f_len.data() + g, f0_stride, f, sp);
+    if (!e && tp.syn.modify) e = modify_run(&L->c, tp.syn.mod, g, m, p.f_len.data() + g, f0_stride, f, sp);
     if (e && L != h) h->c.last_error = L->c.last_error;
     return e;
   };
   auto synthesise = [&](int s) {
     WorldB200 *L; int g, m; double *xd, *t, *f, *sp, *ap;
     slice(s, &L, &g, &m, &xd, &t, &f, &sp, &ap);
-    const int e = synthesis_run(&L->c, f, p.f_len.data() + g, m, f0_stride, sp, ap, nullptr, fft_size, tp.lg,
-                                p.frame_period, r.fs, tp.y_len.data() + g, tp.y_stride,
-                                (unsigned char *)y + (size_t)bounds[s] * out_row, tp.nbit_out, nullptr, 0,
-                                tp.fp.data() + g);
+    const int e = synthesis_run(&L->c, tp.syn, g, m, {f, sp, ap, (unsigned char *)y + (size_t)bounds[s] * out_row});
     if (e && L != h) h->c.last_error = L->c.last_error;
     return e;
   };
@@ -1252,7 +1239,7 @@ int world_b200_transform_batch(WorldB200 *h, const void *x, int nbit, int n_utts
   TransformPlan tp;
   const int rc = transform_check(h, r, f0_scale, spectral_ratio, time_scale, nbit_out, y, y_stride, "transform_batch", &tp);
   if (rc) return rc;
-  if (y_lengths) std::copy(tp.y_len.begin(), tp.y_len.end(), y_lengths);
+  if (y_lengths) std::copy(tp.syn.y_len.begin(), tp.syn.y_len.end(), y_lengths);
   return transform_run(h, r, tp, x, 0, n_utts, y);
 }
 

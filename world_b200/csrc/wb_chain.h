@@ -85,19 +85,15 @@ int chain_spectral(WorldB200 *h, const ChainRequest &r, const ChainPlan &p, int 
                    const double *time_axis, const double *f0, double *sp, double *ap);
 
 // Voice transformation (world_b200_transform_*): the analysis plan of the request (full rows, no spectral options, no
-// analysis outputs) and what synthesis adds to it.  transform_check makes it once per call; transform_run (device rows)
-// and the host pipeline (wb_host.cu) read it.
+// analysis outputs) and the synthesis plan of its analysis rows: lengths, the factors (which modify_run applies right
+// after the analysis) and each utterance's frame period, (frame_period * time_scale[u]) / 1000.0 s.  transform_check
+// makes it once per call; transform_run (device rows) and the host pipeline (wb_host.cu) read it.
 struct TransformPlan {
   ChainPlan chain;
-  int nbit_out = 0, y_stride = 0, lg = 0;
-  std::vector<int> y_len;          // [n] output samples of each utterance
-  std::vector<double> fp;          // [n] synthesis frame period (s): (frame_period * time_scale[u]) / 1000.0
-  bool modify = false;             // f0_scale or spectral_ratio given
-  ModifyPlan mod;
+  SynthesisPlan syn;
 };
 int transform_check(WorldB200 *h, const ChainRequest &r, const double *f0_scale, const double *spectral_ratio,
-                    const double *time_scale, int nbit_out, const void *y, int y_stride, const char *who,
-                    TransformPlan *tp);
+                    const double *time_scale, int nbit_out, void *y, int y_stride, const char *who, TransformPlan *tp);
 // Utterances [u0, u0 + n) of a checked call: x and y point at utterance u0's rows (device).
 int transform_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, const void *x, int u0, int n, void *y);
 

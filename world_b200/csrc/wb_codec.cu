@@ -15,7 +15,7 @@
 //   pcm_kernel        sample -> thread: little-endian signed PCM -> sample / 2^(nbit-1)
 // Host side: every axis, index table and DCT weight is computed with the reference's own double
 // expressions and the host libm, so the interpolation indices are the reference's.
-#include "wb_internal.h"
+#include "wb_chain.h"
 #include "../../include/world_b200.h"
 #include <math.h>
 #include <string.h>
@@ -359,8 +359,8 @@ int world_b200_code_spectral_envelope_batch(WorldB200 *h, const double *spectrog
                                             const int *f0_lengths, int f0_stride, int fs, int fft_size,
                                             int number_of_dimensions, double *coded) {
   if (!h || !spectrogram || !coded || n_utts < 0 || fs <= 0 || f0_stride <= 0) return WORLD_B200_EINVAL;
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  Ctx *ctx = reinterpret_cast<Ctx *>(h);
+  DeviceGuard guard_(&h->c);
+  Ctx *ctx = &h->c;
   Tables t;
   int rc = codec_sp_tables(ctx, fs, fft_size, number_of_dimensions, &t);
   if (rc) return rc;
@@ -377,8 +377,8 @@ int world_b200_decode_spectral_envelope_batch(WorldB200 *h, const double *coded,
                                               const int *f0_lengths, int f0_stride, int fs, int fft_size,
                                               int number_of_dimensions, double *spectrogram) {
   if (!h || !spectrogram || !coded || n_utts < 0 || fs <= 0 || f0_stride <= 0) return WORLD_B200_EINVAL;
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  Ctx *ctx = reinterpret_cast<Ctx *>(h);
+  DeviceGuard guard_(&h->c);
+  Ctx *ctx = &h->c;
   Tables t;
   const int rc = codec_decode_sp_tables(ctx, fs, fft_size, number_of_dimensions, &t);
   if (rc) return rc;
@@ -389,8 +389,8 @@ int world_b200_decode_spectral_envelope_batch(WorldB200 *h, const double *coded,
 int world_b200_code_aperiodicity_batch(WorldB200 *h, const double *aperiodicity, int n_utts,
                                        const int *f0_lengths, int f0_stride, int fs, int fft_size, double *coded) {
   if (!h || !aperiodicity || n_utts < 0 || fs <= 0 || f0_stride <= 0 || fft_size < 2) return WORLD_B200_EINVAL;
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  Ctx *ctx = reinterpret_cast<Ctx *>(h);
+  DeviceGuard guard_(&h->c);
+  Ctx *ctx = &h->c;
   const int n_ap = GetNumberOfAperiodicities(fs);
   if (n_ap <= 0) return 0;          // nothing to write below 12 kHz, like the reference's empty loops
   if (!coded) return WORLD_B200_EINVAL;
@@ -406,8 +406,8 @@ int world_b200_code_aperiodicity_batch(WorldB200 *h, const double *aperiodicity,
 int world_b200_decode_aperiodicity_batch(WorldB200 *h, const double *coded, int n_utts, const int *f0_lengths,
                                          int f0_stride, int fs, int fft_size, double *aperiodicity) {
   if (!h || !aperiodicity || n_utts < 0 || fs <= 0 || f0_stride <= 0 || fft_size < 2) return WORLD_B200_EINVAL;
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  Ctx *ctx = reinterpret_cast<Ctx *>(h);
+  DeviceGuard guard_(&h->c);
+  Ctx *ctx = &h->c;
   const int n_ap = GetNumberOfAperiodicities(fs);
   if (n_ap < 0 || (n_ap > 0 && !coded)) return WORLD_B200_EINVAL;
   Tables t;
@@ -440,8 +440,8 @@ int world_b200_wav_parse(const unsigned char *b, unsigned long long size, int *f
 int world_b200_pcm_to_double_batch(WorldB200 *h, const void *pcm, int nbit, int n_utts, int x_stride,
                                    const int *x_lengths, double *x) {
   if (!h || !pcm || !x || n_utts < 0 || x_stride <= 0) return WORLD_B200_EINVAL;
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  Ctx *ctx = reinterpret_cast<Ctx *>(h);
+  DeviceGuard guard_(&h->c);
+  Ctx *ctx = &h->c;
   if (nbit != 8 && nbit != 16 && nbit != 24 && nbit != 32) { ctx->last_error = "pcm: nbit must be 8, 16, 24 or 32"; return WORLD_B200_EINVAL; }
   if (n_utts == 0) return 0;
   std::vector<int> lens(n_utts);

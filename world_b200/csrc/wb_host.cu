@@ -389,19 +389,15 @@ int chunk_pipeline(WorldB200 *h, const char *who, int n_utts, int chunk, int rin
 // hold its download until all its passes were done, and a shorter one would pay the pass's fixed cost more often
 // (syn_timebase_kernel's sequential phase sum over each utterance takes about as long for a few utterances as for a
 // pass of hundreds; at 1024 x 10 s, 16 kHz, chunks of 128 utterances made the call slower than the serial path).  Two
-// input sets and the output ring stay within a third of the scratch budget.  `lens` holds the checked lengths
-// (synthesis_lengths).
-int synthesis_pipeline(WorldB200 *h, CodedRows *coded, int lg, const double *f0, const int *f0_lengths, int n_utts,
-                       int f0_stride, int fft_size, double frame_period, int fs, const int *y_lengths, int y_stride,
-                       const int *lens, int nbit, void *y, const ModifyPlan *mod) {
+// input sets and the output ring stay within a third of the scratch budget.  `host`: the call's host rows.
+int synthesis_pipeline(WorldB200 *h, const SynthesisPlan &plan, const SynthesisRows &host) {
   Ctx *ctx = &h->c;
-  const int dims = coded->tsp.dims, n_ap = coded->tap.dims;
-  const double *h_sp = coded->sp, *h_ap = coded->ap;
-  const size_t out_bytes = nbit ? 2 : 8;
-  const size_t per_in = (size_t)f0_stride * (1 + dims + n_ap) * 8, per_out = (size_t)y_stride * out_bytes;
+  const int n_utts = plan.n, f0_stride = plan.f0_stride, dims = plan.tsp.dims, n_ap = plan.tap.dims;
+  const size_t out_bytes = plan.nbit ? 2 : 8;
+  const size_t per_in = (size_t)f0_stride * (1 + dims + n_ap) * 8, per_out = (size_t)plan.y_stride * out_bytes;
   int max_y = 0;
-  for (int i = 0; i < n_utts; ++i) max_y = imax(max_y, lens[n_utts + i]);
-  const SynthesisSizing sz(ctx, coded, fft_size, f0_stride, y_stride, max_y, fs, mod);
+  for (const int v : plan.y_len) max_y = imax(max_y, v);
+  const SynthesisSizing sz(ctx, plan, max_y);
   const int ring = 3;
   const size_t third = ctx->scratch_budget / 3;
   int chunk = imax(1, sz.fit(sz.nominal_cap));
@@ -414,22 +410,16 @@ int synthesis_pipeline(WorldB200 *h, CodedRows *coded, int lg, const double *f0,
   // chunk k's f0 and coded rows
   auto upload = [&](HostPipe &p, int u0, int m, unsigned char *d) {
     const size_t frames = (size_t)m * f0_stride, row0 = (size_t)u0 * f0_stride;
-    p.h2d(d + o_f0, f0 + row0, frames * 8);
-    p.h2d(d + o_sp, h_sp + row0 * dims, frames * dims * 8);
-    if (n_ap) p.h2d(d + o_ap, h_ap + row0 * n_ap, frames * n_ap * 8);
+    p.h2d(d + o_f0, host.f0 + row0, frames * 8);
+    p.h2d(d + o_sp, host.sp + row0 * dims, frames * dims * 8);
+    if (n_ap) p.h2d(d + o_ap, host.ap + row0 * n_ap, frames * n_ap * 8);
   };
   auto run = [&](int u0, int m, unsigned char *d, unsigned char *out) {
-    coded->sp = (const double *)(d + o_sp);
-    coded->ap = n_ap ? (const double *)(d + o_ap) : nullptr;
-    return synthesis_run(ctx, (const double *)(d + o_f0), f0_lengths ? f0_lengths + u0 : nullptr, m, f0_stride, nullptr,
-                         nullptr, coded, fft_size, lg, frame_period, fs, y_lengths ? y_lengths + u0 : nullptr, y_stride,
-                         out, nbit, mod, u0);
+    return synthesis_run(ctx, plan, u0, m, {(const double *)(d + o_f0), (const double *)(d + o_sp),
+                                            (const double *)(d + o_ap), out});
   };
-  const int rc = chunk_pipeline(h, "synthesis", n_utts, chunk, ring, in_plan.total, per_out, lens + n_utts, y_stride,
-                                nbit, y, upload, run);
-  coded->sp = h_sp;
-  coded->ap = h_ap;
-  return rc;
+  return chunk_pipeline(h, "synthesis", n_utts, chunk, ring, in_plan.total, per_out, plan.y_len.data(), plan.y_stride,
+                        plan.nbit, host.y, upload, run);
 }
 
 // Voice transformation for host arrays: chunks of PCM in, transform_run on each chunk (which forks from and joins back
@@ -439,7 +429,7 @@ int transform_pipeline(WorldB200 *h, const ChainRequest &r, const TransformPlan 
   Ctx *ctx = &h->c;
   const int n_utts = r.n;
   const size_t per_in = (size_t)r.x_stride * (r.nbit ? r.nbit / 8 : 8);
-  const size_t per_out = (size_t)tp.y_stride * (tp.nbit_out ? 2 : 8);
+  const size_t per_out = (size_t)tp.syn.y_stride * (tp.syn.nbit ? 2 : 8);
   int chunk = 512;
   if (const char *e = getenv("WB_HOST_CHUNK")) chunk = atoi(e) > 0 ? atoi(e) : chunk;
   chunk = imin(chunk, (int)dmax(1.0, (double)(ctx->scratch_budget / 6) / (double)(2 * (per_in + per_out))));
@@ -451,43 +441,26 @@ int transform_pipeline(WorldB200 *h, const ChainRequest &r, const TransformPlan 
   auto run = [&](int u0, int m, unsigned char *d, unsigned char *out) {
     return transform_run(h, r, tp, d, u0, m, out);
   };
-  return chunk_pipeline(h, "transform", n_utts, chunk, 2, (size_t)chunk * per_in, per_out, tp.y_len.data(), tp.y_stride,
-                        tp.nbit_out, y, upload, run);
+  return chunk_pipeline(h, "transform", n_utts, chunk, 2, (size_t)chunk * per_in, per_out, tp.syn.y_len.data(),
+                        tp.syn.y_stride, tp.syn.nbit, y, upload, run);
 }
 
-// world_b200_synthesis_coded_host and, with f0_scale / spectral_ratio, world_b200_synthesis_coded_host_modified
+// world_b200_synthesis_coded_host and, with f0_scale / spectral_ratio, world_b200_synthesis_coded_host_modified: every
+// check runs before the first chunk is queued
 int synthesis_coded_host(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts, int f0_stride,
                          const double *coded_spectral_envelope, int number_of_dimensions,
                          const double *coded_aperiodicity, int fft_size, double frame_period, int fs,
                          const int *y_lengths, int y_stride, int nbit, void *y, const double *f0_scale,
                          const double *spectral_ratio) {
-  if (!h || !f0 || !coded_spectral_envelope || !y || n_utts < 0 || fs <= 0 || frame_period <= 0)
-    return WORLD_B200_EINVAL;
+  if (!h) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
-  Ctx *ctx = &h->c;
-  if (nbit != 0 && nbit != 16) {
-    ctx->last_error = "synthesis_coded_host: nbit must be 0 (double) or 16 (int16)";
-    return WORLD_B200_EINVAL;
-  }
-  int lg = 0;
-  int rc = synthesis_fft(ctx, fft_size, &lg);
-  if (rc) return rc;
-  CodedRows coded;
-  rc = synthesis_coded_tables(ctx, fs, fft_size, number_of_dimensions, coded_aperiodicity != nullptr, &coded);
-  if (rc) return rc;
-  ModifyPlan mod;
-  const bool modified = f0_scale || spectral_ratio;
-  if (modified) rc = modify_plan(ctx, n_utts, fft_size, fs, f0_scale, spectral_ratio, &mod);
-  if (rc) return rc;
-  if (n_utts == 0) return 0;
-  // every length is checked before the first chunk is queued
-  std::vector<int> lens((size_t)2 * n_utts);
-  rc = synthesis_lengths(ctx, f0_lengths, n_utts, f0_stride, y_lengths, y_stride, lens.data());
-  if (rc) return rc;
-  coded.sp = coded_spectral_envelope;
-  coded.ap = coded.tap.dims > 0 ? coded_aperiodicity : nullptr;
-  return synthesis_pipeline(h, &coded, lg, f0, f0_lengths, n_utts, f0_stride, fft_size, frame_period, fs, y_lengths,
-                            y_stride, lens.data(), nbit, y, modified ? &mod : nullptr);
+  SynthesisRequest r{f0, f0_lengths, n_utts, f0_stride, coded_spectral_envelope, coded_aperiodicity, fft_size,
+                     frame_period, fs, y_lengths, y_stride, y, nbit};
+  r.coded = true; r.dims = number_of_dimensions; r.f0_scale = f0_scale; r.spectral_ratio = spectral_ratio;
+  SynthesisPlan plan;
+  const int rc = synthesis_plan(&h->c, r, "Synthesis", &plan);
+  if (rc || n_utts == 0) return rc;
+  return synthesis_pipeline(h, plan, {r.f0, r.sp, r.ap, r.y});
 }
 
 }  // namespace
@@ -527,7 +500,7 @@ extern "C" int world_b200_transform_host(WorldB200 *h, const void *x, int nbit, 
   TransformPlan tp;
   const int rc = transform_check(h, r, f0_scale, spectral_ratio, time_scale, nbit_out, y, y_stride, "transform_host", &tp);
   if (rc) return rc;
-  if (y_lengths) std::copy(tp.y_len.begin(), tp.y_len.end(), y_lengths);
+  if (y_lengths) std::copy(tp.syn.y_len.begin(), tp.syn.y_len.end(), y_lengths);
   if (n_utts == 0) return 0;
   return transform_pipeline(h, r, tp, y);
 }

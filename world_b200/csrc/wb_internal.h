@@ -162,11 +162,6 @@ struct CodecDeviceTables { const int *idx; const double *frac; const double2 *we
 void codec_decode_launch(Ctx *ctx, bool spectral_envelope, const CodecTables &t, const CodecDeviceTables &d,
                          int fft_size, const int *f_len, int n_utts, int f_stride, int max_f, const double *in,
                          double *out);
-// wb_synthesis.cu: the Synthesis driver, shared by the device entry points and the host pipeline (wb_host.cu)
-struct CodedRows {            // Synthesis from coded rows: the decode tables, made once per call
-  const double *sp, *ap;      // [n][f0_stride][tsp.dims], [n][f0_stride][tap.dims] (ap null when tap.dims == 0)
-  CodecTables tsp, tap;
-};
 // wb_synthesis.cu: F0 scaling and spectral stretch (the reference demo's ParameterModification, test.cpp:221-258).
 // The interp1 segment and weight of each output bin depend only on (ratio, fft_size, fs), so they are planned on the
 // host once per distinct ratio; the tail rule (bins >= c copy bin c-1 when ratio < 1) is folded into the table.
@@ -179,9 +174,9 @@ struct ModifyPlan {
   size_t device_bytes(int n) const;   // arena bytes of one pass of n utterances: tables, factors, table indices
 };
 // Checks every factor (finite, > 0; a ratio below 1 must keep c = (int)(fft_size / 2.0 * ratio) >= 1) and builds the
-// plan; EINVAL with last_error naming the first bad utterance.  Either array may be null.
-int modify_plan(Ctx *ctx, int n_utts, int fft_size, int fs, const double *f0_scale, const double *spectral_ratio,
-                ModifyPlan *plan);
+// plan; EINVAL with last_error "<who>: ..." naming the first bad utterance.  Either array may be null.
+int modify_plan(Ctx *ctx, const char *who, int n_utts, int fft_size, int fs, const double *f0_scale,
+                const double *spectral_ratio, ModifyPlan *plan);
 // Plan entries [u0, u0 + n) in device memory (layout of device_bytes); the copies are enqueued on ctx->stream.
 struct ModifyDevice { const double *scale; const int *table; const int *idx; const double *frac; };
 int modify_upload(Ctx *ctx, const ModifyPlan &plan, int u0, int n, unsigned char *blk, ModifyDevice *d);
@@ -197,35 +192,75 @@ void modify_stretch_launch(Ctx *ctx, const ModifyDevice &d, int bins, const int 
 int modify_run(Ctx *ctx, const ModifyPlan &plan, int u0, int n_utts, const int *f0_lengths, int f0_stride, double *f0,
                double *spectrogram);
 
-int synthesis_fft(Ctx *ctx, int fft_size, int *lg_out);   // EINVAL unless a power of two in [16, 4096]
-// the decode tables of a coded call; EINVAL for number_of_dimensions, or no aperiodicity rows where fs has bands
-int synthesis_coded_tables(Ctx *ctx, int fs, int fft_size, int number_of_dimensions, bool have_aperiodicity,
-                           CodedRows *coded);
-// lens[0, n) = f0 lengths, lens[n, 2n) = y lengths (NULL: full rows); EINVAL when one is < 2 or beyond its row
-int synthesis_lengths(Ctx *ctx, const int *f0_lengths, int n_utts, int f0_stride, const int *y_lengths, int y_stride,
-                      int *lens);
-// Per-utterance scratch of synthesis_run for a batch whose longest y_length is max_y; fit(nominal_cap) utterances
-// make one pass when no utterance has more than 1,200 pulses per second.
+// out[u] = lengths[u] (NULL: stride) for u < n; EINVAL "<who>: <rows>_lengths[u] = v is outside [least, <rows>_stride =
+// stride] (utterance u)" for the first one outside
+int row_lengths(Ctx *ctx, const char *who, const char *rows, const int *lengths, int n, int stride, int least,
+                std::vector<int> *out);
+
+// wb_synthesis.cu: the Synthesis driver, shared by the device entry points, the host pipeline (wb_host.cu) and voice
+// transformation (wb_api.cu): one checked plan per call, then synthesis_run over the rows of each chunk or slice.
+// What a synthesis call receives: f0 [n][f0_stride], the envelope rows sp / ap (spectrogram / aperiodicity
+// [n][f0_stride][bins], or with `coded` [n][f0_stride][dims] / [GetNumberOfAperiodicities(fs)] coded rows) and y
+// [n][y_stride] (doubles for nbit 0, int16 for nbit 16).  NULL lengths: full rows.  NULL factors: no modification.
+struct SynthesisRequest {   // brace-initialised in field order up to nbit
+  const double *f0;
+  const int *f0_lengths;
+  int n, f0_stride;
+  const double *sp, *ap;
+  int fft_size;
+  double frame_period;   // ms
+  int fs;
+  const int *y_lengths;
+  int y_stride;
+  void *y;
+  int nbit;
+  bool coded = false;
+  int dims = 0;          // coded: number_of_dimensions
+  const double *f0_scale = nullptr, *spectral_ratio = nullptr;
+  // transform: f0 / sp / ap are the call's own analysis rows, not given here, and fp [n] holds each utterance's frame
+  // period (s)
+  bool transform = false;
+  const double *fp = nullptr;
+};
+// Everything synthesis_run reads besides the rows, made once per call and const afterwards.
+struct SynthesisPlan {
+  int n = 0, f0_stride = 0, y_stride = 0, fft_size = 0, lg = 0, fs = 0, nbit = 0;
+  double frame_period = 0.0;        // ms
+  std::vector<int> f_len, y_len;    // [n]
+  bool coded = false;
+  CodecTables tsp, tap;             // coded: the decode tables (tap.dims == 0 below 12 kHz: no aperiodicity rows)
+  // f0_scale or spectral_ratio given.  synthesis_run applies it to coded rows, as it decodes them; full rows are their
+  // producer's to modify (transform runs modify_run on its analysis rows).
+  bool modify = false;
+  ModifyPlan mod;
+  std::vector<double> fp;           // [n] frame period (s) of each utterance, or empty: frame_period / 1000.0 for all
+  std::vector<double> dc_remover;   // [fft_size] GetDCRemover (synthesis.cpp:319-333)
+};
+// Every check of a synthesis call before anything is queued, in this order: the pointers, n, fs and frame_period;
+// nbit; fft_size (a power of two in [16, 4096]); the coded decode tables; the factors (modify_plan); each utterance's
+// f0 and y lengths (2 .. stride).  EINVAL with last_error "<who>: ...", naming the first bad utterance where there is
+// one.
+int synthesis_plan(Ctx *ctx, const SynthesisRequest &r, const char *who, SynthesisPlan *p);
+// Per-utterance scratch of synthesis_run for rows whose longest y_length is max_y; fit(nominal_cap) utterances make one
+// pass when no utterance has more than 1,200 pulses per second.
 struct SynthesisSizing {
-  // mod: the scaled f0 copy (f0_stride * 8 bytes per utterance) and the stretch tables are counted too
-  SynthesisSizing(const Ctx *ctx, const CodedRows *coded, int fft_size, int f0_stride, int y_stride, int max_y, int fs,
-                  const ModifyPlan *mod = nullptr);
+  SynthesisSizing(const Ctx *ctx, const SynthesisPlan &p, int max_y);
   size_t per_utt(int cap) const;
   int fit(int cap) const;
   int fft_size, y_stride, nominal_cap;
   size_t decoded_per_utt, draw_stride;
   double budget;
 };
-// Enqueues Synthesis of n_utts utterances (device rows; host lengths) on ctx->stream, in passes that fit the scratch
-// budget, each with one read-back of its pulse counts.  coded null: full rows; y: double (nbit 0) or int16 (nbit 16).
-// mod (coded rows only): utterance i of the call is the plan's utterance mod_u0 + i; each pass synthesises from a
-// scaled copy of its f0 rows and stretches its decoded envelope block right after the decode.
-// fp_u (host, n_utts entries, or null): the frame period of each utterance in seconds, used instead of
-// frame_period / 1000.0; each pass uploads its slice.
-int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts, int f0_stride,
-                  const double *spectrogram, const double *aperiodicity, const CodedRows *coded, int fft_size, int lg,
-                  double frame_period, int fs, const int *y_lengths, int y_stride, void *y, int nbit,
-                  const ModifyPlan *mod = nullptr, int mod_u0 = 0, const double *fp_u = nullptr);
+// The rows of utterances [u0, u0 + m) of a planned call: device pointers at utterance u0, laid out as the request's
+// (sp / ap: full or coded rows, as the plan says; coded ap is not read below 12 kHz, where there are no bands).
+struct SynthesisRows {
+  const double *f0, *sp, *ap;
+  void *y;
+};
+// Enqueues Synthesis of the plan's utterances [u0, u0 + m) on ctx->stream, in passes that fit the scratch budget, each
+// with one read-back of its pulse counts.  With coded rows and factors, each pass synthesises from a scaled copy of its
+// f0 rows and stretches its decoded envelope block right after the decode.
+int synthesis_run(Ctx *ctx, const SynthesisPlan &p, int u0, int m, const SynthesisRows &rows);
 
 // The utterances of a batch that share one CheapTrick option (world_b200_cheaptrick_*batch_options): their batch
 // indices, ascending, and their frame counts.  cheaptrick_run runs one launch sequence over them, reaching each row

@@ -15,9 +15,8 @@
 //   modify_stretch_kernel, modify_f0_kernel
 // FFT conventions (SURVEY.md App. A0): c2c FORWARD of a == FFT(conj a); c2r of X == Re FFT(conj X~)
 // with X~ the Hermitian extension -- both are forward transforms of wb_fft.cuh.
-#include "wb_internal.h"
+#include "wb_chain.h"
 #include "wb_spectral.cuh"
-#include "../../include/world_b200.h"
 #include "../../include/world/matlabfunctions.h"
 #include <map>
 #include <stdio.h>
@@ -380,9 +379,9 @@ struct ModifyLayout {
   }
 };
 
-int modify_fail(Ctx *ctx, const char *what, int u, double v, const char *why) {
+int modify_fail(Ctx *ctx, const char *who, const char *what, int u, double v, const char *why) {
   char msg[256];
-  snprintf(msg, sizeof msg, "modify: %s[%d] = %.17g %s", what, u, v, why);
+  snprintf(msg, sizeof msg, "%s: %s[%d] = %.17g %s", who, what, u, v, why);
   ctx->last_error = msg;
   return WORLD_B200_EINVAL;
 }
@@ -390,31 +389,31 @@ int modify_fail(Ctx *ctx, const char *what, int u, double v, const char *why) {
 
 size_t ModifyPlan::device_bytes(int n) const { return ModifyLayout(*this, n).total; }
 
-int modify_plan(Ctx *ctx, int n_utts, int fft_size, int fs, const double *f0_scale, const double *spectral_ratio,
-                ModifyPlan *plan) {
+int modify_plan(Ctx *ctx, const char *who, int n_utts, int fft_size, int fs, const double *f0_scale,
+                const double *spectral_ratio, ModifyPlan *plan) {
   *plan = ModifyPlan();
   if (f0_scale) {
     for (int u = 0; u < n_utts; ++u) {
       const double v = f0_scale[u];
-      if (!(v > 0.0) || !isfinite(v)) return modify_fail(ctx, "f0_scale", u, v, "is not a finite factor > 0");
+      if (!(v > 0.0) || !isfinite(v)) return modify_fail(ctx, who, "f0_scale", u, v, "is not a finite factor > 0");
     }
     plan->scale.assign(f0_scale, f0_scale + n_utts);
   }
   if (!spectral_ratio) return 0;
   if (fft_size < 16 || fft_size > 4096 || (fft_size & (fft_size - 1))) {
-    ctx->last_error = "modify: fft_size must be a power of two in [16, 4096]";
+    ctx->last_error = std::string(who) + ": fft_size must be a power of two in [16, 4096]";
     return WORLD_B200_EINVAL;
   }
   if (fs <= 0) {
-    ctx->last_error = "modify: fs must be > 0";
+    ctx->last_error = std::string(who) + ": fs must be > 0";
     return WORLD_B200_EINVAL;
   }
   for (int u = 0; u < n_utts; ++u) {
     const double r = spectral_ratio[u];
     // histc needs an ascending axis; below 1 the tail copies bin c - 1, which must exist (c == 0 reads sp[-1])
-    if (!(r > 0.0) || !isfinite(r)) return modify_fail(ctx, "spectral_ratio", u, r, "is not a finite ratio > 0");
+    if (!(r > 0.0) || !isfinite(r)) return modify_fail(ctx, who, "spectral_ratio", u, r, "is not a finite ratio > 0");
     if (r < 1.0 && static_cast<int>(fft_size / 2.0 * r) < 1)
-      return modify_fail(ctx, "spectral_ratio", u, r, "leaves no bin below (int)(fft_size / 2.0 * ratio)");
+      return modify_fail(ctx, who, "spectral_ratio", u, r, "leaves no bin below (int)(fft_size / 2.0 * ratio)");
   }
   const int half = fft_size / 2, bins = half + 1;
   plan->bins = bins;
@@ -497,67 +496,92 @@ int modify_run(Ctx *ctx, const ModifyPlan &plan, int u0, int n_utts, const int *
   return dev_check(ctx, "modify");
 }
 
-int synthesis_fft(Ctx *ctx, int fft_size, int *lg_out) {
-  int lg = 0;
-  while ((1 << lg) < fft_size) ++lg;
-  if ((1 << lg) != fft_size || fft_size < 16 || fft_size > WB_TW_N / 2) {
-    ctx->last_error = "Synthesis: fft_size must be a power of two in [16, 4096]";
-    return WORLD_B200_EINVAL;
-  }
-  *lg_out = lg;
-  return 0;
-}
-
-int synthesis_coded_tables(Ctx *ctx, int fs, int fft_size, int number_of_dimensions, bool have_aperiodicity,
-                           CodedRows *coded) {
-  const int rc = codec_decode_sp_tables(ctx, fs, fft_size, number_of_dimensions, &coded->tsp);
-  if (rc) return rc;
-  codec_decode_ap_tables(fs, fft_size, &coded->tap);
-  if (coded->tap.dims > 0 && !have_aperiodicity) {
-    ctx->last_error = "Synthesis: coded_aperiodicity is NULL, but fs has GetNumberOfAperiodicities(fs) > 0 bands";
-    return WORLD_B200_EINVAL;
-  }
-  return 0;
-}
-
-int synthesis_lengths(Ctx *ctx, const int *f0_lengths, int n_utts, int f0_stride, const int *y_lengths, int y_stride,
-                      int *lens) {
-  for (int i = 0; i < n_utts; ++i) {
-    lens[i] = f0_lengths ? f0_lengths[i] : f0_stride;
-    lens[n_utts + i] = y_lengths ? y_lengths[i] : y_stride;
-    if (lens[i] < 2 || lens[i] > f0_stride || lens[n_utts + i] < 2 || lens[n_utts + i] > y_stride) {
-      ctx->last_error = "Synthesis: lengths outside the padded rows (need f0_length >= 2, y_length >= 2)";
+int row_lengths(Ctx *ctx, const char *who, const char *rows, const int *lengths, int n, int stride, int least,
+                std::vector<int> *out) {
+  out->resize(n);
+  for (int u = 0; u < n; ++u) {
+    const int v = (*out)[u] = lengths ? lengths[u] : stride;
+    if (v < least || v > stride) {
+      char msg[256];
+      snprintf(msg, sizeof msg, "%s: %s_lengths[%d] = %d is outside [%d, %s_stride = %d] (utterance %d)", who, rows,
+               u, v, least, rows, stride, u);
+      ctx->last_error = msg;
       return WORLD_B200_EINVAL;
     }
   }
   return 0;
 }
 
-SynthesisSizing::SynthesisSizing(const Ctx *ctx, const CodedRows *coded, int fft_size, int f0_stride, int y_stride,
-                                 int max_y, int fs, const ModifyPlan *mod)
-    : fft_size(fft_size), y_stride(y_stride) {
+int synthesis_plan(Ctx *ctx, const SynthesisRequest &r, const char *who, SynthesisPlan *p) {
+  auto fail = [&](const std::string &what) {
+    ctx->last_error = std::string(who) + ": " + what;
+    return WORLD_B200_EINVAL;
+  };
+  if (!r.y || (!r.transform && (!r.f0 || !r.sp || (!r.coded && !r.ap))))
+    return fail(r.coded ? "f0, coded_spectral_envelope and y must be given"
+                        : "f0, spectrogram, aperiodicity and y must be given");
+  if (r.n < 0) return fail("n_utts must be >= 0");
+  if (r.fs <= 0) return fail("fs must be > 0");
+  if (r.frame_period <= 0) return fail("frame_period must be > 0");
+  if (r.nbit != 0 && r.nbit != 16) return fail("nbit must be 0 (double) or 16 (int16)");
+  const int fft_size = r.fft_size;
+  if (fft_size < 16 || fft_size > WB_TW_N / 2 || (fft_size & (fft_size - 1)))
+    return fail("fft_size must be a power of two in [16, 4096]");
+  p->n = r.n; p->f0_stride = r.f0_stride; p->y_stride = r.y_stride; p->fft_size = fft_size; p->fs = r.fs;
+  p->nbit = r.nbit; p->frame_period = r.frame_period;
+  while ((1 << p->lg) < fft_size) ++p->lg;
+  p->coded = r.coded;
+  int rc = 0;
+  if (r.coded) {
+    if (codec_decode_sp_tables(ctx, r.fs, fft_size, r.dims, &p->tsp)) return fail(ctx->last_error);
+    codec_decode_ap_tables(r.fs, fft_size, &p->tap);
+    if (p->tap.dims > 0 && !r.ap)
+      return fail("coded_aperiodicity is NULL, but fs has GetNumberOfAperiodicities(fs) > 0 bands");
+  }
+  p->modify = r.f0_scale || r.spectral_ratio;
+  if (p->modify) rc = modify_plan(ctx, who, r.n, fft_size, r.fs, r.f0_scale, r.spectral_ratio, &p->mod);
+  if (!rc) rc = row_lengths(ctx, who, "f0", r.f0_lengths, r.n, r.f0_stride, 2, &p->f_len);
+  if (!rc) rc = row_lengths(ctx, who, "y", r.y_lengths, r.n, r.y_stride, 2, &p->y_len);
+  if (rc) return rc;
+  if (r.transform) p->fp.assign(r.fp, r.fp + r.n);
+  // DC remover (GetDCRemover, synthesis.cpp:319-333), host libm like the reference
+  std::vector<double> &dcr = p->dc_remover;
+  dcr.resize(fft_size);
+  double dc = 0.0;
+  for (int i = 0; i < fft_size / 2; ++i) {
+    dcr[i] = 0.5 - 0.5 * cos(2.0 * kPi * (i + 1.0) / (1.0 + fft_size));
+    dcr[fft_size - i - 1] = dcr[i];
+    dc += dcr[i] * 2.0;
+  }
+  for (int i = 0; i < fft_size / 2; ++i) { dcr[i] /= dc; dcr[fft_size - i - 1] = dcr[i]; }
+  return 0;
+}
+
+SynthesisSizing::SynthesisSizing(const Ctx *ctx, const SynthesisPlan &p, int max_y)
+    : fft_size(p.fft_size), y_stride(p.y_stride) {
   const size_t bins = (size_t)fft_size / 2 + 1;
   // The coded call holds one chunk's decoded envelope and aperiodicity (16 B per bin and frame) and the decode tables.
   size_t tables = 0;
-  if (coded) {
+  if (p.coded) {
     ArenaPlan tp;
-    tp.add(coded->tsp.idx.size() * 4); tp.add(coded->tsp.frac.size() * 8); tp.add(coded->tsp.weight.size() * 16);
-    tp.add(coded->tap.idx.size() * 4); tp.add(coded->tap.frac.size() * 8);
+    tp.add(p.tsp.idx.size() * 4); tp.add(p.tsp.frac.size() * 8); tp.add(p.tsp.weight.size() * 16);
+    tp.add(p.tap.idx.size() * 4); tp.add(p.tap.frac.size() * 8);
     tables = tp.total;
   }
-  decoded_per_utt = coded ? (size_t)f0_stride * bins * 16 : 0;
+  decoded_per_utt = p.coded ? (size_t)p.f0_stride * bins * 16 : 0;
   // A modified call also holds the stretch tables, and per utterance its factor, table index and scaled f0 row (the
   // 256-byte alignment of the two small arrays is in the 4096 below).
-  if (mod) {
-    tables += mod->device_bytes(0);
-    decoded_per_utt += (size_t)f0_stride * 8 + 12;
+  if (p.coded && p.modify) {
+    tables += p.mod.device_bytes(0);
+    decoded_per_utt += (size_t)p.f0_stride * 8 + 12;
   }
   budget = (double)ctx->scratch_budget - (double)tables;
   // Pulse arrays and responses are sized for 1200 pulses per second (f0 <= 1.2 kHz; the +64 covers the ends).
-  nominal_cap = (int)((double)max_y / fs * 1200.0) + 64;
+  nominal_cap = (int)((double)max_y / p.fs * 1200.0) + 64;
   draw_stride = (size_t)max_y + 8;
 }
 
+// PassLayout's bytes per utterance, with the 256-byte alignment of its small arrays rounded up to 4096
 size_t SynthesisSizing::per_utt(int cap) const {
   return (size_t)y_stride * 16 + (size_t)cap * (4 + 8 + 8) + (size_t)cap * fft_size * 8 + draw_stride * 4 + 4096 +
          decoded_per_utt;
@@ -565,112 +589,111 @@ size_t SynthesisSizing::per_utt(int cap) const {
 
 int SynthesisSizing::fit(int cap) const { return (int)dmin(65535.0, budget / (double)per_utt(cap)); }
 
-// The chunk driver of both entry points: full rows (spectrogram / aperiodicity) or, with `coded`, rows decoded per
-// chunk into the chunk's block.  nbit 0 writes the waveform (double), nbit 16 its 16-bit PCM (short).
-int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts, int f0_stride,
-                  const double *spectrogram, const double *aperiodicity, const CodedRows *coded, int fft_size, int lg,
-                  double frame_period, int fs, const int *y_lengths, int y_stride, void *y, int nbit,
-                  const ModifyPlan *mod, int mod_u0, const double *fp_u) {
-  if (n_utts == 0) return 0;
-  std::vector<int> lens((size_t)2 * n_utts);
-  int rc = synthesis_lengths(ctx, f0_lengths, n_utts, f0_stride, y_lengths, y_stride, lens.data());
-  if (rc) return rc;
-  int max_y = 0;
-  for (int i = 0; i < n_utts; ++i) max_y = imax(max_y, lens[n_utts + i]);
-  // DC remover (GetDCRemover, synthesis.cpp:319-333), host libm like the reference
-  std::vector<double> dcr(fft_size);
-  {
-    double dc = 0.0;
-    for (int i = 0; i < fft_size / 2; ++i) {
-      dcr[i] = 0.5 - 0.5 * cos(2.0 * kPi * (i + 1.0) / (1.0 + fft_size));
-      dcr[fft_size - i - 1] = dcr[i];
-      dc += dcr[i] * 2.0;
+namespace {
+// The scratch block of one pass of n utterances with room for cap pulses each
+struct PassLayout {
+  size_t len, phase, vuv, pidx, psh, np, cnt, dcnt, doff, dtot, pl, draws, resp, dcr;
+  size_t dsp = 0, dap = 0, sidx = 0, sfrac = 0, sw = 0, aidx = 0, afrac = 0;   // coded
+  size_t mod = 0, f0m = 0, fp = 0, total;
+  PassLayout(const SynthesisPlan &p, int n, int cap, size_t draw_stride) {
+    const size_t N = n, frames = N * p.f0_stride, bins = (size_t)p.fft_size / 2 + 1;
+    ArenaPlan a;
+    len = a.add(2 * N * 4);                                          // f0 lengths, then y lengths
+    phase = a.add(N * p.y_stride * 8); vuv = a.add(N * p.y_stride * 8);
+    pidx = a.add(N * cap * 4); psh = a.add(N * cap * 8);
+    np = a.add(N * 4); cnt = a.add(N * 4);
+    dcnt = a.add(N * cap * 4); doff = a.add(N * cap * 4);
+    dtot = a.add(N * 4); pl = a.add(N * 4);
+    draws = a.add(N * draw_stride * 4);
+    resp = a.add(N * cap * p.fft_size * 8);
+    dcr = a.add((size_t)p.fft_size * 8);
+    if (p.coded) {
+      dsp = a.add(frames * bins * 8); dap = a.add(frames * bins * 8);
+      sidx = a.add(p.tsp.idx.size() * 4); sfrac = a.add(p.tsp.frac.size() * 8); sw = a.add(p.tsp.weight.size() * 16);
+      aidx = a.add(p.tap.idx.size() * 4); afrac = a.add(p.tap.frac.size() * 8);
+      if (p.modify) {
+        mod = a.add(p.mod.device_bytes(n));
+        if (!p.mod.scale.empty()) f0m = a.add(frames * 8);
+      }
     }
-    for (int i = 0; i < fft_size / 2; ++i) { dcr[i] /= dc; dcr[fft_size - i - 1] = dcr[i]; }
+    if (!p.fp.empty()) fp = a.add(N * 8);
+    total = a.total;
   }
-  const int half = fft_size / 2;
+};
+}  // namespace
+
+// nbit 0 writes the waveform (double), nbit 16 its 16-bit PCM (short).
+int synthesis_run(Ctx *ctx, const SynthesisPlan &plan, int u0, int m, const SynthesisRows &rows) {
+  if (m == 0) return 0;
+  const int *f_len = plan.f_len.data() + u0, *y_len = plan.y_len.data() + u0;
+  const int fft_size = plan.fft_size, half = fft_size / 2, f0_stride = plan.f0_stride, y_stride = plan.y_stride;
   const size_t bins = (size_t)half + 1;
+  int max_y = 0;
+  for (int i = 0; i < m; ++i) max_y = imax(max_y, y_len[i]);
   // The caller's f0 may be anything up to fs/2 (a pitch-shifted contour), so syn_timebase_kernel also counts the
   // pulses it could not store; a chunk where that count exceeds the cap is laid out again with room for its largest
   // count, in as many passes as the scratch budget needs.  The common case pays one read-back of n counts per chunk.
-  const SynthesisSizing sz(ctx, coded, fft_size, f0_stride, y_stride, max_y, fs, mod);
+  const SynthesisSizing sz(ctx, plan, max_y);
+  const ModifyPlan *mod = plan.coded && plan.modify ? &plan.mod : nullptr;
   const bool scale_f0 = mod && !mod->scale.empty(), stretch = mod && !mod->table.empty();
   const int nominal_cap = sz.nominal_cap;
   const size_t draw_stride = sz.draw_stride;
   auto fit = [&](int cap) { return sz.fit(cap); };
-  const int chunk = balanced_chunk(imin(n_utts, 65535), fit(nominal_cap));
+  const int chunk = balanced_chunk(imin(m, 65535), fit(nominal_cap));
   const size_t smem = (size_t)(2 * fft_size + 2 * (half + 2) + (fft_size + 2) + 2 * (half + 1) + fft_size + WB_RED_DOUBLES) * 8;
 #ifndef WB_EMU
   cudaFuncSetAttribute(syn_pulse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 #endif
   std::vector<int> counts;
-  int u0 = 0, n = imin(chunk, n_utts), pulse_cap = nominal_cap;
+  int v0 = 0, n = imin(chunk, m), pulse_cap = nominal_cap;   // this pass: utterances [u0 + v0, u0 + v0 + n)
   bool relaid = false;
-  while (u0 < n_utts) {
-    ArenaPlan plan;
-    const size_t o_len = plan.add((size_t)2 * n * 4);
-    const size_t o_phase = plan.add((size_t)n * y_stride * 8), o_vuv = plan.add((size_t)n * y_stride * 8);
-    const size_t o_pidx = plan.add((size_t)n * pulse_cap * 4), o_psh = plan.add((size_t)n * pulse_cap * 8);
-    const size_t o_np = plan.add((size_t)n * 4), o_cnt = plan.add((size_t)n * 4);
-    const size_t o_dc = plan.add((size_t)n * pulse_cap * 4), o_do = plan.add((size_t)n * pulse_cap * 4);
-    const size_t o_dt = plan.add((size_t)n * 4), o_pl = plan.add((size_t)n * 4);
-    const size_t o_draws = plan.add((size_t)n * draw_stride * 4);
-    const size_t o_resp = plan.add((size_t)n * pulse_cap * fft_size * 8);
-    const size_t o_dcr = plan.add((size_t)fft_size * 8);
-    size_t o_dsp = 0, o_dap = 0, o_sidx = 0, o_sfrac = 0, o_sw = 0, o_aidx = 0, o_afrac = 0;
-    if (coded) {
-      o_dsp = plan.add((size_t)n * f0_stride * bins * 8); o_dap = plan.add((size_t)n * f0_stride * bins * 8);
-      o_sidx = plan.add(coded->tsp.idx.size() * 4); o_sfrac = plan.add(coded->tsp.frac.size() * 8);
-      o_sw = plan.add(coded->tsp.weight.size() * 16);
-      o_aidx = plan.add(coded->tap.idx.size() * 4); o_afrac = plan.add(coded->tap.frac.size() * 8);
-    }
-    const size_t o_mod = mod ? plan.add(mod->device_bytes(n)) : 0;
-    const size_t o_f0m = scale_f0 ? plan.add((size_t)n * f0_stride * 8) : 0;
-    const size_t o_fp = fp_u ? plan.add((size_t)n * 8) : 0;
-    unsigned char *blk = arena_block(ctx, plan.total);
+  while (v0 < m) {
+    const PassLayout l(plan, n, pulse_cap, draw_stride);
+    unsigned char *blk = arena_block(ctx, l.total);
     if (!blk) return WORLD_B200_ENOMEM;
     std::vector<int> l2((size_t)2 * n), pl(n, pulse_cap);
     int max_f = 0;
-    for (int i = 0; i < n; ++i) { l2[i] = lens[u0 + i]; l2[n + i] = lens[n_utts + u0 + i]; max_f = imax(max_f, l2[i]); }
-    rc = dev_memcpy_h2d(ctx, blk + o_len, l2.data(), l2.size() * 4);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_dcr, dcr.data(), dcr.size() * 8);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_pl, pl.data(), (size_t)n * 4);
-    if (!rc && fp_u) rc = dev_memcpy_h2d(ctx, blk + o_fp, fp_u + u0, (size_t)n * 8);
-    if (coded) {
-      const CodecTables &s = coded->tsp, &a = coded->tap;
-      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_sidx, s.idx.data(), s.idx.size() * 4);
-      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_sfrac, s.frac.data(), s.frac.size() * 8);
-      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_sw, s.weight.data(), s.weight.size() * 16);
-      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_aidx, a.idx.data(), a.idx.size() * 4);
-      if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_afrac, a.frac.data(), a.frac.size() * 8);
+    for (int i = 0; i < n; ++i) { l2[i] = f_len[v0 + i]; l2[n + i] = y_len[v0 + i]; max_f = imax(max_f, l2[i]); }
+    int rc = dev_memcpy_h2d(ctx, blk + l.len, l2.data(), l2.size() * 4);
+    if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.dcr, plan.dc_remover.data(), (size_t)fft_size * 8);
+    if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.pl, pl.data(), (size_t)n * 4);
+    if (!rc && !plan.fp.empty()) rc = dev_memcpy_h2d(ctx, blk + l.fp, plan.fp.data() + u0 + v0, (size_t)n * 8);
+    if (plan.coded) {
+      const CodecTables &s = plan.tsp, &a = plan.tap;
+      if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.sidx, s.idx.data(), s.idx.size() * 4);
+      if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.sfrac, s.frac.data(), s.frac.size() * 8);
+      if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.sw, s.weight.data(), s.weight.size() * 16);
+      if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.aidx, a.idx.data(), a.idx.size() * 4);
+      if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.afrac, a.frac.data(), a.frac.size() * 8);
     }
     ModifyDevice md = {};
-    if (mod && !rc) rc = modify_upload(ctx, *mod, mod_u0 + u0, n, blk + o_mod, &md);
+    if (mod && !rc) rc = modify_upload(ctx, *mod, u0 + v0, n, blk + l.mod, &md);
     if (rc) return rc;
     SynParams p;
-    p.f0 = f0 + (size_t)u0 * f0_stride; p.f_len = (const int *)(blk + o_len); p.f_stride = f0_stride;
-    if (coded) {
-      p.sp = (const double *)(blk + o_dsp); p.ap = (const double *)(blk + o_dap);
+    p.f0 = rows.f0 + (size_t)v0 * f0_stride; p.f_len = (const int *)(blk + l.len); p.f_stride = f0_stride;
+    if (plan.coded) {
+      p.sp = (const double *)(blk + l.dsp); p.ap = (const double *)(blk + l.dap);
     } else {
-      p.sp = spectrogram + (size_t)u0 * f0_stride * bins; p.ap = aperiodicity + (size_t)u0 * f0_stride * bins;
+      p.sp = rows.sp + (size_t)v0 * f0_stride * bins; p.ap = rows.ap + (size_t)v0 * f0_stride * bins;
     }
-    p.fft_size = fft_size; p.lg_fft = lg; p.frame_period = frame_period / 1000.0; p.fs = fs;
-    p.fp_u = fp_u ? (const double *)(blk + o_fp) : nullptr;
-    p.y_len = (const int *)(blk + o_len) + n; p.y_stride = y_stride;
-    p.phase = (double *)(blk + o_phase); p.vuv = (double *)(blk + o_vuv); p.flag_cnt = nullptr;
-    p.pulse_idx = (int *)(blk + o_pidx); p.pulse_shift = (double *)(blk + o_psh); p.n_pulses = (int *)(blk + o_np);
-    p.pulse_cap = pulse_cap; p.pulse_count = (int *)(blk + o_cnt);
-    p.draw_cnt = (unsigned *)(blk + o_dc); p.draw_off = (unsigned *)(blk + o_do); p.draw_tot = (unsigned *)(blk + o_dt);
-    p.draws = (const unsigned *)(blk + o_draws); p.draw_stride = draw_stride;
-    p.resp = (double *)(blk + o_resp); p.dc_remover = (const double *)(blk + o_dcr);
-    p.y = nbit ? nullptr : (double *)y + (size_t)u0 * y_stride;
-    p.y16 = nbit ? (short *)y + (size_t)u0 * y_stride : nullptr;
+    p.fft_size = fft_size; p.lg_fft = plan.lg; p.frame_period = plan.frame_period / 1000.0; p.fs = plan.fs;
+    p.fp_u = plan.fp.empty() ? nullptr : (const double *)(blk + l.fp);
+    p.y_len = (const int *)(blk + l.len) + n; p.y_stride = y_stride;
+    p.phase = (double *)(blk + l.phase); p.vuv = (double *)(blk + l.vuv); p.flag_cnt = nullptr;
+    p.pulse_idx = (int *)(blk + l.pidx); p.pulse_shift = (double *)(blk + l.psh); p.n_pulses = (int *)(blk + l.np);
+    p.pulse_cap = pulse_cap; p.pulse_count = (int *)(blk + l.cnt);
+    p.draw_cnt = (unsigned *)(blk + l.dcnt); p.draw_off = (unsigned *)(blk + l.doff);
+    p.draw_tot = (unsigned *)(blk + l.dtot);
+    p.draws = (const unsigned *)(blk + l.draws); p.draw_stride = draw_stride;
+    p.resp = (double *)(blk + l.resp); p.dc_remover = (const double *)(blk + l.dcr);
+    p.y = plan.nbit ? nullptr : (double *)rows.y + (size_t)v0 * y_stride;
+    p.y16 = plan.nbit ? (short *)rows.y + (size_t)v0 * y_stride : nullptr;
     p.tw = ctx->twiddle;
     // a pass laid out from the counts reports a pulse beyond its arrays as a scratch overflow (status bit 4)
     p.status = relaid ? ctx->status_dev : nullptr;
     if (scale_f0) {
       // the time base, the pulse count (and the relaid pass it may call for) and the pulses all see the scaled contour
-      double *f0m = (double *)(blk + o_f0m);
+      double *f0m = (double *)(blk + l.f0m);
       modify_f0_launch(ctx, md, p.f_len, n, f0_stride, max_f, p.f0, f0m);
       p.f0 = f0m;
     }
@@ -690,30 +713,30 @@ int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts,
         continue;
       }
     }
-    if (coded) {
+    if (plan.coded) {
       // DecodeSpectralEnvelope / DecodeAperiodicity of this pass's utterances, frames [0, f0_length)
-      const CodecDeviceTables ts = {(const int *)(blk + o_sidx), (const double *)(blk + o_sfrac),
-                                    (const double2 *)(blk + o_sw)};
-      const CodecDeviceTables ta = {(const int *)(blk + o_aidx), (const double *)(blk + o_afrac), nullptr};
-      double *dsp = (double *)(blk + o_dsp), *dap = (double *)(blk + o_dap);
-      codec_decode_launch(ctx, true, coded->tsp, ts, fft_size, p.f_len, n, f0_stride, max_f,
-                          coded->sp + (size_t)u0 * f0_stride * coded->tsp.dims, dsp);
+      const CodecDeviceTables ts = {(const int *)(blk + l.sidx), (const double *)(blk + l.sfrac),
+                                    (const double2 *)(blk + l.sw)};
+      const CodecDeviceTables ta = {(const int *)(blk + l.aidx), (const double *)(blk + l.afrac), nullptr};
+      double *dsp = (double *)(blk + l.dsp), *dap = (double *)(blk + l.dap);
+      codec_decode_launch(ctx, true, plan.tsp, ts, fft_size, p.f_len, n, f0_stride, max_f,
+                          rows.sp + (size_t)v0 * f0_stride * plan.tsp.dims, dsp);
       if (stretch) modify_stretch_launch(ctx, md, (int)bins, p.f_len, n, f0_stride, max_f, dsp);
       // below 12 kHz there are no bands: the kernel reads no coded value (its input pointer only has to be valid)
-      codec_decode_launch(ctx, false, coded->tap, ta, fft_size, p.f_len, n, f0_stride, max_f,
-                          coded->ap ? coded->ap + (size_t)u0 * f0_stride * coded->tap.dims : dap, dap);
+      codec_decode_launch(ctx, false, plan.tap, ta, fft_size, p.f_len, n, f0_stride, max_f,
+                          plan.tap.dims > 0 ? rows.ap + (size_t)v0 * f0_stride * plan.tap.dims : dap, dap);
     }
-    scan_counts(ctx, p.draw_cnt, (const int *)(blk + o_pl), pulse_cap, nullptr, p.draw_off, p.draw_tot, n);
-    rng_fill(ctx, p.draw_tot, (unsigned *)(blk + o_draws), draw_stride, draw_stride, n);
+    scan_counts(ctx, p.draw_cnt, (const int *)(blk + l.pl), pulse_cap, nullptr, p.draw_off, p.draw_tot, n);
+    rng_fill(ctx, p.draw_tot, (unsigned *)(blk + l.draws), draw_stride, draw_stride, n);
     WB_LAUNCH_COOP(syn_pulse_kernel, dim3((unsigned)pulse_cap, (unsigned)n), 128, smem, ctx->stream, p);
-    if (nbit)
+    if (plan.nbit)
       WB_LAUNCH_FLAT(syn_overlap_kernel<short>, dim3((unsigned)((max_y + 255) / 256), (unsigned)n), 256, 0, ctx->stream, p);
     else
       WB_LAUNCH_FLAT(syn_overlap_kernel<double>, dim3((unsigned)((max_y + 255) / 256), (unsigned)n), 256, 0, ctx->stream, p);
     rc = dev_check(ctx, "synthesis");
     if (rc) return rc;
-    u0 += n;
-    n = imin(chunk, n_utts - u0);
+    v0 += n;
+    n = imin(chunk, m - v0);
     pulse_cap = nominal_cap;
     relaid = false;
   }
@@ -724,46 +747,32 @@ int synthesis_run(Ctx *ctx, const double *f0, const int *f0_lengths, int n_utts,
 
 using namespace wb;
 
-extern "C" int world_b200_synthesis_batch(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts,
-                                          int f0_stride, const double *spectrogram, const double *aperiodicity,
-                                          int fft_size, double frame_period, int fs, const int *y_lengths,
-                                          int y_stride, double *y) {
-  if (!h || !f0 || !spectrogram || !aperiodicity || !y || n_utts < 0 || fs <= 0 || frame_period <= 0)
-    return WORLD_B200_EINVAL;
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  Ctx *ctx = reinterpret_cast<Ctx *>(h);
-  int lg = 0;
-  const int rc = synthesis_fft(ctx, fft_size, &lg);
-  if (rc) return rc;
-  return synthesis_run(ctx, f0, f0_lengths, n_utts, f0_stride, spectrogram, aperiodicity, nullptr, fft_size, lg,
-                       frame_period, fs, y_lengths, y_stride, y, 0);
+// world_b200_synthesis_batch and the three world_b200_synthesis_coded_batch*: one plan, one run over the whole batch
+static int synthesis_batch(WorldB200 *h, const SynthesisRequest &r) {
+  if (!h) return WORLD_B200_EINVAL;
+  DeviceGuard guard_(&h->c);
+  SynthesisPlan plan;
+  const int rc = synthesis_plan(&h->c, r, "Synthesis", &plan);
+  return rc ? rc : synthesis_run(&h->c, plan, 0, r.n, {r.f0, r.sp, r.ap, r.y});
 }
 
-// world_b200_synthesis_coded_batch (nbit 0, y double), world_b200_synthesis_coded_batch_pcm16 (nbit 16, y short) and,
-// with f0_scale / spectral_ratio, world_b200_synthesis_coded_batch_modified
 static int synthesis_coded_batch(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts, int f0_stride,
                                  const double *coded_spectral_envelope, int number_of_dimensions,
                                  const double *coded_aperiodicity, int fft_size, double frame_period, int fs,
                                  const int *y_lengths, int y_stride, void *y, int nbit,
                                  const double *f0_scale = nullptr, const double *spectral_ratio = nullptr) {
-  if (!h || !f0 || !coded_spectral_envelope || !y || n_utts < 0 || fs <= 0 || frame_period <= 0)
-    return WORLD_B200_EINVAL;
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  Ctx *ctx = reinterpret_cast<Ctx *>(h);
-  int lg = 0;
-  int rc = synthesis_fft(ctx, fft_size, &lg);
-  if (rc) return rc;
-  CodedRows coded;
-  rc = synthesis_coded_tables(ctx, fs, fft_size, number_of_dimensions, coded_aperiodicity != nullptr, &coded);
-  if (rc) return rc;
-  ModifyPlan mod;
-  const bool modified = f0_scale || spectral_ratio;
-  if (modified) rc = modify_plan(ctx, n_utts, fft_size, fs, f0_scale, spectral_ratio, &mod);
-  if (rc) return rc;
-  coded.sp = coded_spectral_envelope;
-  coded.ap = coded.tap.dims > 0 ? coded_aperiodicity : nullptr;
-  return synthesis_run(ctx, f0, f0_lengths, n_utts, f0_stride, nullptr, nullptr, &coded, fft_size, lg, frame_period,
-                       fs, y_lengths, y_stride, y, nbit, modified ? &mod : nullptr);
+  SynthesisRequest r{f0, f0_lengths, n_utts, f0_stride, coded_spectral_envelope, coded_aperiodicity, fft_size,
+                     frame_period, fs, y_lengths, y_stride, y, nbit};
+  r.coded = true; r.dims = number_of_dimensions; r.f0_scale = f0_scale; r.spectral_ratio = spectral_ratio;
+  return synthesis_batch(h, r);
+}
+
+extern "C" int world_b200_synthesis_batch(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts,
+                                          int f0_stride, const double *spectrogram, const double *aperiodicity,
+                                          int fft_size, double frame_period, int fs, const int *y_lengths,
+                                          int y_stride, double *y) {
+  return synthesis_batch(h, {f0, f0_lengths, n_utts, f0_stride, spectrogram, aperiodicity, fft_size, frame_period, fs,
+                             y_lengths, y_stride, y, 0});
 }
 
 extern "C" int world_b200_synthesis_coded_batch_modified(WorldB200 *h, const double *f0, const int *f0_lengths,
@@ -773,10 +782,6 @@ extern "C" int world_b200_synthesis_coded_batch_modified(WorldB200 *h, const dou
                                                          int fft_size, double frame_period, int fs,
                                                          const int *y_lengths, int y_stride, const double *f0_scale,
                                                          const double *spectral_ratio, int nbit, void *y) {
-  if (h && nbit != 0 && nbit != 16) {
-    reinterpret_cast<Ctx *>(h)->last_error = "synthesis_coded_batch_modified: nbit must be 0 (double) or 16 (int16)";
-    return WORLD_B200_EINVAL;
-  }
   return synthesis_coded_batch(h, f0, f0_lengths, n_utts, f0_stride, coded_spectral_envelope, number_of_dimensions,
                                coded_aperiodicity, fft_size, frame_period, fs, y_lengths, y_stride, y, nbit, f0_scale,
                                spectral_ratio);
@@ -803,26 +808,21 @@ extern "C" int world_b200_synthesis_coded_batch_pcm16(WorldB200 *h, const double
 extern "C" int world_b200_modify_batch(WorldB200 *h, double *f0, const int *f0_lengths, int n_utts, int f0_stride,
                                        double *spectrogram, int fft_size, int fs, const double *f0_scale,
                                        const double *spectral_ratio) {
-  if (!h || n_utts < 0 || f0_stride <= 0) return WORLD_B200_EINVAL;
-  DeviceGuard guard_(reinterpret_cast<const Ctx *>(h));  // Ctx is the first member of WorldB200
-  Ctx *ctx = reinterpret_cast<Ctx *>(h);
+  if (!h) return WORLD_B200_EINVAL;
+  DeviceGuard guard_(&h->c);
+  Ctx *ctx = &h->c;
+  if (n_utts < 0 || f0_stride <= 0) {
+    ctx->last_error = "modify: n_utts must be >= 0 and f0_stride > 0";
+    return WORLD_B200_EINVAL;
+  }
   if ((f0_scale && !f0) || (spectral_ratio && !spectrogram)) {
     ctx->last_error = "modify: f0_scale needs f0 rows and spectral_ratio needs spectrogram rows";
     return WORLD_B200_EINVAL;
   }
-  std::vector<int> lens(n_utts > 0 ? n_utts : 1);
-  for (int u = 0; u < n_utts; ++u) {
-    lens[u] = f0_lengths ? f0_lengths[u] : f0_stride;
-    if (lens[u] < 0 || lens[u] > f0_stride) {
-      char msg[128];
-      snprintf(msg, sizeof msg, "modify: f0_lengths[%d] = %d is outside its padded row of %d frames", u, lens[u],
-               f0_stride);
-      ctx->last_error = msg;
-      return WORLD_B200_EINVAL;
-    }
-  }
+  // a length of 0 is allowed here: the utterance's rows are left alone
+  std::vector<int> lens;
   ModifyPlan plan;
-  int rc = modify_plan(ctx, n_utts, fft_size, fs, f0_scale, spectral_ratio, &plan);
-  if (rc) return rc;
-  return modify_run(ctx, plan, 0, n_utts, lens.data(), f0_stride, f0, spectrogram);
+  int rc = row_lengths(ctx, "modify", "f0", f0_lengths, n_utts, f0_stride, 0, &lens);
+  if (!rc) rc = modify_plan(ctx, "modify", n_utts, fft_size, fs, f0_scale, spectral_ratio, &plan);
+  return rc ? rc : modify_run(ctx, plan, 0, n_utts, lens.data(), f0_stride, f0, spectrogram);
 }
