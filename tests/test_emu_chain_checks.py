@@ -61,11 +61,11 @@ class Chain:
         self.outs = [np.full(s, -7.0) for s in shapes]
 
     def call(self, method=F0_DIO_STONEMASK, nbit=0, lens=LENS, f0_stride=None, ho=None, do=None, dims=DIMS, ct=None,
-             opt=None):
+             opt=None, fs=FS):
         n = len(LENS)
-        ao = opt or self.world.analysis_option(FS, method)
+        ao = opt or self.world.analysis_option(fs, method)
         head = (self.world._h, _ptr(self.x)) + ((nbit,) if self.coded or self.transform else ()) + (
-            n, STRIDE, (C.c_int * n)(*lens), FS, C.byref(ao))
+            n, STRIDE, (C.c_int * n)(*lens), fs, C.byref(ao))
         if self.transform:
             return getattr(self.lib, f"world_b200_{self.entry}")(*head, ho, do, None, None, None, 0,
                                                                  _ptr(self.outs[0]), self.Y, None)
@@ -74,7 +74,7 @@ class Chain:
         if self.coded:
             outs = (dims,) + outs
         if self.spectral:
-            cts = [self.world.cheaptrick_option(FS) for _ in LENS]
+            cts = [self.world.cheaptrick_option(fs) for _ in LENS]
             if ct is not None:
                 cts[-1].fft_size = ct
             ct_arr = (CheapTrickOption * n)(*cts)
@@ -106,6 +106,9 @@ def _cases(ch):
         ("Harvest options on a DIO chain", lambda: ch.call(ho=hopts), "f0_method"),
         ("frame_period differs", lambda: ch.call(method=F0_HARVEST, ho=bad_fp), "utterance 3)"),
         ("F0 range below zero", lambda: ch.call(method=F0_HARVEST, ho=bad_range), "utterance 3)"),
+        # the stages' sampling-rate limits: StoneMask's window at 96 kHz, D4C's transforms at 192 kHz
+        ("DIO chain at 96 kHz", lambda: ch.call(fs=96000), "StoneMask: sampling rate"),
+        ("Harvest chain at 192 kHz", lambda: ch.call(method=F0_HARVEST, fs=192000), "D4C: sampling rate"),
     ]
     if ch.coded or ch.transform:
         cases.append(("nbit 12", lambda: ch.call(nbit=12), "nbit"))

@@ -1,18 +1,20 @@
 """Compares two builds of the library call by call: every analysis chain entry point, voice transformation, every
-synthesis entry point and modify on seeded ragged batches, with each call's return code, launch count and outputs
-required to be identical byte for byte.  Meant for a refactor of the chain or synthesis drivers, with the parent
-commit's build as A and the change's as B (on the host emulation, two tests/emu builds; on a GPU, two libworld_b200.so
-with --device).
+CheapTrick / D4C / StoneMask stage entry point, every synthesis entry point and modify on seeded ragged batches, with
+each call's return code, launch count and outputs required to be identical byte for byte.  Meant for a refactor of the
+chain, stage or synthesis drivers, with the parent commit's build as A and the change's as B (on the host emulation,
+two tests/emu builds; on a GPU, two libworld_b200.so with --device).
 
     python tools/compare_chains.py A.so B.so [--device]
 
 Analysis covers 8 and 16 kHz (16 kHz has one aperiodicity band, 8 kHz none), float64 and 16-bit PCM input, Harvest
 and DIO, no options, per-utterance F0 options, per-utterance CheapTrick / D4C options with two FFT sizes, NULL
 spectrogram / aperiodicity, transform with all three factors, and the host pipelines with small chunks (WB_HOST_CHUNK /
-WB_HOST_SUB).  Synthesis covers the same two rates: full rows, coded rows to float64 and int16 on device and host
-arrays, with and without f0_scale / spectral_ratio, and modify, on rows made by numpy (one full-length utterance's f0
-is above 1.2 kHz, so its pass is laid out again), at the default scratch budget and at the smallest one (several
-passes and host chunks).  Prints the number of calls compared; exits 1 on the first difference."""
+WB_HOST_SUB).  The stage calls cover 8, 16 and 44.1 kHz: one option, the same option for every utterance as lists, and
+mixed options, into full and coded rows, and full rows wider than the largest size's bins.  Synthesis covers 8 and
+16 kHz: full rows, coded rows to float64 and int16 on device and host arrays, with and without f0_scale /
+spectral_ratio, and modify, on rows made by numpy (one full-length utterance's f0 is above 1.2 kHz, so its pass is laid
+out again).  The stage calls and synthesis run at the default scratch budget and at the smallest one (several passes
+and host chunks).  Prints the number of calls compared; exits 1 on the first difference."""
 import argparse
 import ctypes as C
 import os
@@ -188,6 +190,55 @@ def synthesis_calls_at(w, arr, fs):
     return out
 
 
+def stage_calls_at(w, arr, fs):
+    """(name, thunk) pairs of the nine CheapTrick, D4C and StoneMask stage entry points at one rate, on numpy rows: one
+    option and mixed options (two FFT sizes, q1 / threshold per utterance), full and coded rows, and full rows wider
+    than the largest size's bins (row_stride)."""
+    x, _, lens = batch(fs, fs + 2)
+    n, L = len(lens), w.frames(fs, x.shape[1])
+    rng = np.random.default_rng(fs + 3)
+    fl = [w.frames(fs, m) for m in lens]
+    t = np.tile(np.arange(L) * 0.005, (n, 1))
+    f0 = np.where(rng.uniform(size=(n, L)) < 0.8, rng.uniform(80.0, 300.0, size=(n, L)), 0.0)
+    xd, td, fd = arr(x), arr(t), arr(f0)
+    kw = dict(x_lengths=lens, f0_lengths=fl)
+    ct = w.cheaptrick_option(fs)
+    cts = [w.cheaptrick_option(fs) for _ in range(n)]
+    for u, o in enumerate(cts):
+        o.fft_size, o.q1 = ct.fft_size * (2 if u % 2 else 1), -0.15 + 0.02 * u
+    d4s = [w.d4c_option() for _ in range(n)]
+    for u, d in enumerate(d4s):
+        d.threshold = 0.8 + 0.02 * u
+    sizes = [o.fft_size for o in cts]
+    wide = (n, L, max(sizes) // 2 + 8)
+    out = [(f"stonemask fs {fs}", lambda: [w.stonemask(xd, fs, td, fd, **kw)])]
+    for tag, opt, size, d4 in (("one option", ct, ct.fft_size, None), ("one option as lists", [ct] * n,
+                                                                         [ct.fft_size] * n, [w.d4c_option()] * n),
+                               ("mixed options", cts, sizes, d4s)):
+        name = f"fs {fs} {tag}"
+        out.append((f"cheaptrick {name}", lambda opt=opt: [w.cheaptrick(xd, fs, td, fd, opt, **kw)]))
+        out.append((f"d4c {name}", lambda size=size, d4=d4: [w.d4c(xd, fs, td, fd, size, d4, **kw)]))
+        out.append((f"cheaptrick_coded {name}", lambda opt=opt: [w.cheaptrick_coded(xd, fs, td, fd, DIMS, opt, **kw)]))
+        out.append((f"d4c_coded {name}", lambda size=size, d4=d4: [w.d4c_coded(xd, fs, td, fd, size, d4, **kw)]))
+        if isinstance(opt, list):
+            out.append((f"cheaptrick row_stride {name}", lambda opt=opt: [
+                w.cheaptrick(xd, fs, td, fd, opt, out=arr(np.full(wide, -1.0)), **kw)]))
+            out.append((f"d4c row_stride {name}", lambda size=size, d4=d4: [
+                w.d4c(xd, fs, td, fd, size, d4, out=arr(np.full(wide, -1.0)), **kw)]))
+    return out
+
+
+def stage_calls(w, device):
+    """(name, thunk) pairs of the stage entry points at 8, 16 and 44.1 kHz."""
+    def arr(a):
+        if not device:
+            return a
+        import torch
+        return torch.from_numpy(np.ascontiguousarray(a)).cuda()
+
+    return [c for fs in (8000, 16000, 44100) for c in stage_calls_at(w, arr, fs)]
+
+
 def synthesis_calls(w, device):
     """(name, thunk) pairs of the synthesis entry points and modify at 8 and 16 kHz."""
     def arr(a):
@@ -241,11 +292,13 @@ def main():
         compared += compare(worlds, [calls(w, args.device) for w in worlds], f"chunks {chunks}")
     for k in ("WB_HOST_CHUNK", "WB_HOST_SUB"):
         os.environ.pop(k, None)
-    # synthesis at the default scratch budget, then at the smallest one (64 MB: several passes and host chunks)
+    # the stage calls and synthesis at the default scratch budget, then at the smallest one (64 MB: several passes and
+    # host chunks)
     small = [World(lib_path=p, array_module=mod or "torch") for p in libs]
     for w in small:
         w.set_scratch_budget(64 << 20)
     for ws, label in ((worlds, "default budget"), (small, "64 MB budget")):
+        compared += compare(ws, [stage_calls(w, args.device) for w in ws], label)
         compared += compare(ws, [synthesis_calls(w, args.device) for w in ws], label)
     print(f"{compared} calls compared, all identical (return codes, launch counts, output bytes)")
 

@@ -536,109 +536,74 @@ class World:
         return t, f0, fl
 
     def stonemask(self, x, fs, time_axis, f0, x_lengths=None, f0_lengths=None):
-        n, stride = x.shape
         out = self._zeros(x, tuple(f0.shape))
-        xl, k1 = _int_array(x_lengths, n)
-        fl, k2 = _int_array(f0_lengths, n)
-        self._use_current_stream()
-        self._check(self.lib.world_b200_stonemask_batch(self._h, _ptr(x), n, stride, xl, fs, _ptr(time_axis),
-                                                        _ptr(f0), fl, f0.shape[1], _ptr(out)))
-        return out
+        return self._stage("stonemask_batch", x, fs, time_axis, f0, x_lengths, f0_lengths, (), out)
 
     def cheaptrick(self, x, fs, time_axis, f0, option: CheapTrickOption | None = None, x_lengths=None,
                    f0_lengths=None, out=None):
         """option: one CheapTrickOption for the batch, or a list of one per utterance (each speaker's fft_size from
         its own F0 floor).  With a list the rows are [n, L, max fft_size / 2 + 1] (or out's last dimension): the
         first fft_size / 2 + 1 values of utterance u's rows are written, the rest are left as they are."""
-        n, stride = x.shape
-        if isinstance(option, (list, tuple)):
-            opts = _option_array(CheapTrickOption, option, n)
-            if out is None:
-                out = self._zeros(x, (n, f0.shape[1], max([o.fft_size for o in option] or [0]) // 2 + 1))
-            xl, k1 = _int_array(x_lengths, n)
-            fl, k2 = _int_array(f0_lengths, n)
-            self._use_current_stream()
-            self._check(self.lib.world_b200_cheaptrick_batch_options(
-                self._h, _ptr(x), n, stride, xl, fs, _ptr(time_axis), _ptr(f0), fl, f0.shape[1], opts, out.shape[-1],
-                _ptr(out)))
-            return out
-        option = option or self.cheaptrick_option(fs)
-        bins = option.fft_size // 2 + 1
         if out is None:
-            out = self._zeros(x, (n, f0.shape[1], bins))
-        xl, k1 = _int_array(x_lengths, n)
-        fl, k2 = _int_array(f0_lengths, n)
-        self._use_current_stream()
-        self._check(self.lib.world_b200_cheaptrick_batch(self._h, _ptr(x), n, stride, xl, fs, _ptr(time_axis),
-                                                         _ptr(f0), fl, f0.shape[1], C.byref(option), _ptr(out)))
-        return out
+            sizes = ([o.fft_size for o in option] if isinstance(option, (list, tuple))
+                     else [(option or self.cheaptrick_option(fs)).fft_size])
+            out = self._zeros(x, (x.shape[0], f0.shape[1], max(sizes or [0]) // 2 + 1))
+        return self._cheaptrick(False, x, fs, time_axis, f0, option, x_lengths, f0_lengths, out.shape[-1], out)
 
     def d4c(self, x, fs, time_axis, f0, fft_size, option: D4COption | None = None, x_lengths=None,
             f0_lengths=None, out=None):
         """fft_size / option: one for the batch, or either as a list of one per utterance; then the rows are
         [n, L, max fft_size / 2 + 1] (or out's last dimension) and utterance u writes fft_size[u] / 2 + 1 of each."""
-        n, stride = x.shape
-        if isinstance(fft_size, (list, tuple)) or isinstance(option, (list, tuple)):
-            sizes, opts = self._d4c_options(fft_size, option, n)
-            if out is None:
-                out = self._zeros(x, (n, f0.shape[1], max(list(sizes) or [0]) // 2 + 1))
-            xl, k1 = _int_array(x_lengths, n)
-            fl, k2 = _int_array(f0_lengths, n)
-            self._use_current_stream()
-            self._check(self.lib.world_b200_d4c_batch_options(
-                self._h, _ptr(x), n, stride, xl, fs, _ptr(time_axis), _ptr(f0), fl, f0.shape[1], sizes, opts,
-                out.shape[-1], _ptr(out)))
-            return out
-        option = option or self.d4c_option()
-        bins = fft_size // 2 + 1
         if out is None:
-            out = self._zeros(x, (n, f0.shape[1], bins))
-        xl, k1 = _int_array(x_lengths, n)
-        fl, k2 = _int_array(f0_lengths, n)
-        self._use_current_stream()
-        self._check(self.lib.world_b200_d4c_batch(self._h, _ptr(x), n, stride, xl, fs, _ptr(time_axis), _ptr(f0),
-                                                  fl, f0.shape[1], fft_size, C.byref(option), _ptr(out)))
-        return out
+            sizes = list(fft_size) if isinstance(fft_size, (list, tuple)) else [int(fft_size)] * x.shape[0]
+            out = self._zeros(x, (x.shape[0], f0.shape[1], max(sizes or [0]) // 2 + 1))
+        return self._d4c(False, x, fs, time_axis, f0, fft_size, option, x_lengths, f0_lengths, out)
 
     def cheaptrick_coded(self, x, fs, time_axis, f0, number_of_dimensions, option: CheapTrickOption | None = None,
                          x_lengths=None, f0_lengths=None):
         """CheapTrick + CodeSpectralEnvelope in one kernel per frame -> [n, L, number_of_dimensions].  option may be
         a list of one CheapTrickOption per utterance (each coded at its own fft_size)."""
-        n, stride = x.shape
-        out = self._zeros(x, (n, f0.shape[1], number_of_dimensions))
-        xl, k1 = _int_array(x_lengths, n)
-        fl, k2 = _int_array(f0_lengths, n)
-        self._use_current_stream()
-        if isinstance(option, (list, tuple)):
-            self._check(self.lib.world_b200_cheaptrick_coded_batch_options(
-                self._h, _ptr(x), n, stride, xl, fs, _ptr(time_axis), _ptr(f0), fl, f0.shape[1],
-                _option_array(CheapTrickOption, option, n), number_of_dimensions, _ptr(out)))
-            return out
-        option = option or self.cheaptrick_option(fs)
-        self._check(self.lib.world_b200_cheaptrick_coded_batch(self._h, _ptr(x), n, stride, xl, fs, _ptr(time_axis),
-                                                               _ptr(f0), fl, f0.shape[1], C.byref(option),
-                                                               number_of_dimensions, _ptr(out)))
-        return out
+        out = self._zeros(x, (x.shape[0], f0.shape[1], number_of_dimensions))
+        return self._cheaptrick(True, x, fs, time_axis, f0, option, x_lengths, f0_lengths, number_of_dimensions, out)
 
     def d4c_coded(self, x, fs, time_axis, f0, fft_size, option: D4COption | None = None, x_lengths=None,
                   f0_lengths=None):
         """D4C + CodeAperiodicity in one kernel per frame -> [n, L, GetNumberOfAperiodicities(fs)].  fft_size and
         option may be lists of one per utterance."""
+        out = self._zeros(x, (x.shape[0], f0.shape[1], max(1, self.number_of_aperiodicities(fs))))
+        return self._d4c(True, x, fs, time_axis, f0, fft_size, option, x_lengths, f0_lengths, out)
+
+    def _stage(self, entry, x, fs, time_axis, f0, x_lengths, f0_lengths, options, out):
+        """Calls the stage entry point world_b200_<entry> on the rows x / time_axis / f0 with options (the arguments
+        between f0_stride and the output) into out, enqueued on the current stream; returns out."""
         n, stride = x.shape
-        out = self._zeros(x, (n, f0.shape[1], max(1, self.number_of_aperiodicities(fs))))
         xl, k1 = _int_array(x_lengths, n)
         fl, k2 = _int_array(f0_lengths, n)
         self._use_current_stream()
-        if isinstance(fft_size, (list, tuple)) or isinstance(option, (list, tuple)):
-            sizes, opts = self._d4c_options(fft_size, option, n)
-            self._check(self.lib.world_b200_d4c_coded_batch_options(
-                self._h, _ptr(x), n, stride, xl, fs, _ptr(time_axis), _ptr(f0), fl, f0.shape[1], sizes, opts,
-                _ptr(out)))
-            return out
-        option = option or self.d4c_option()
-        self._check(self.lib.world_b200_d4c_coded_batch(self._h, _ptr(x), n, stride, xl, fs, _ptr(time_axis), _ptr(f0),
-                                                        fl, f0.shape[1], fft_size, C.byref(option), _ptr(out)))
+        self._check(getattr(self.lib, f"world_b200_{entry}")(self._h, _ptr(x), n, stride, xl, fs, _ptr(time_axis),
+                                                             _ptr(f0), fl, f0.shape[1], *options, _ptr(out)))
         return out
+
+    def _cheaptrick(self, coded, x, fs, time_axis, f0, option, x_lengths, f0_lengths, width, out):
+        """CheapTrick into full or coded rows.  option: one CheapTrickOption (None: the default at fs) or a list of one
+        per utterance.  width: number_of_dimensions (coded), or the row_stride of a list's full rows."""
+        if isinstance(option, (list, tuple)):
+            suffix, options = "_options", (_option_array(CheapTrickOption, option, x.shape[0]), width)
+        else:
+            suffix, options = "", (C.byref(option or self.cheaptrick_option(fs)),) + ((width,) if coded else ())
+        entry = f"cheaptrick{'_coded' if coded else ''}_batch{suffix}"
+        return self._stage(entry, x, fs, time_axis, f0, x_lengths, f0_lengths, options, out)
+
+    def _d4c(self, coded, x, fs, time_axis, f0, fft_size, option, x_lengths, f0_lengths, out):
+        """D4C into full or coded rows; fft_size / option: one for the batch, or either as a list of one per
+        utterance (full rows then take out's last dimension as their row_stride)."""
+        if isinstance(fft_size, (list, tuple)) or isinstance(option, (list, tuple)):
+            sizes, opts = self._d4c_options(fft_size, option, x.shape[0])
+            suffix, options = "_options", (sizes, opts) + (() if coded else (out.shape[-1],))
+        else:
+            suffix, options = "", (fft_size, C.byref(option or self.d4c_option()))
+        entry = f"d4c{'_coded' if coded else ''}_batch{suffix}"
+        return self._stage(entry, x, fs, time_axis, f0, x_lengths, f0_lengths, options, out)
 
     def _d4c_options(self, fft_size, option, n):
         """Per-utterance D4C arguments as ctypes arrays: a scalar fft_size or option applies to every utterance."""

@@ -249,9 +249,9 @@ int ctx_init_tables(Ctx *ctx) {
 using namespace wb;
 
 // ------------------------------------------------------------------------------------------
-// The Batch of a stage entry point: its rows, and its lengths checked and uploaded (NULL lengths: full rows).
-static int load_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
-                      const double *time_axis, const double *f0, const int *f_lengths, int f_stride, Batch *b) {
+// The Batch of n utterances' rows, with their lengths x_len / f_len [n] (checked by the caller) uploaded.
+static int load_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_len, int fs,
+                      const double *time_axis, const double *f0, const int *f_len, int f_stride, Batch *b) {
   Ctx *ctx = &h->c;
   b->x = x; b->n = n; b->x_stride = x_stride; b->fs = fs; b->time_axis = time_axis; b->f0 = f0; b->f_stride = f_stride;
   if ((size_t)2 * n > h->lens_cap) {
@@ -264,15 +264,9 @@ static int load_batch(WorldB200 *h, const double *x, int n, int x_stride, const 
   std::vector<int> tmp((size_t)2 * n);
   int mx = 0, mf = 0;
   for (int i = 0; i < n; ++i) {
-    const int xl = x_lengths ? x_lengths[i] : x_stride;
-    const int fl = f_lengths ? f_lengths[i] : f_stride;
-    if (xl < 1 || xl > x_stride || fl < 0 || fl > f_stride) {
-      ctx->last_error = "utterance length outside its padded row";
-      return WORLD_B200_EINVAL;
-    }
-    tmp[i] = xl; tmp[n + i] = fl;
-    if (xl > mx) mx = xl;
-    if (fl > mf) mf = fl;
+    tmp[i] = x_len[i]; tmp[n + i] = f_len[i];
+    mx = imax(mx, x_len[i]);
+    mf = imax(mf, f_len[i]);
   }
   // the previous call's kernels may still read lens_dev: same stream, so ordering is preserved
   int rc = dev_memcpy_h2d(ctx, h->lens_dev, tmp.data(), tmp.size() * sizeof(int));
@@ -428,176 +422,169 @@ const char *world_b200_last_error(const WorldB200 *h) { return h ? h->c.last_err
 
 unsigned long long world_b200_launch_count(const WorldB200 *) { return wb::g_launches; }
 
+}  // extern "C"
+
+// ---- the CheapTrick, D4C and StoneMask stage calls: one plan, then load_batch and the stage's run
+// EINVAL with last_error "<stage>: <what>", and " (utterance u)" for u >= 0
+static const char *stage_name(StageKind stage) {
+  return stage == STAGE_CHEAPTRICK ? "CheapTrick" : stage == STAGE_D4C ? "D4C" : "StoneMask";
+}
+static int stage_fail(Ctx *c, StageKind stage, const std::string &what, int u = -1) {
+  c->last_error = std::string(stage_name(stage)) + ": " + what;
+  if (u >= 0) c->last_error += " (utterance " + std::to_string(u) + ")";
+  return WORLD_B200_EINVAL;
+}
+
+namespace wb {
+int stage_plan(Ctx *c, const StageRequest &r, StagePlan *p) {
+  const int n = r.n;
+  auto fail = [&](const std::string &what, int u = -1) { return stage_fail(c, r.stage, what, u); };
+  if (n < 0 || r.fs <= 0) return fail("n_utts must be >= 0 and fs > 0");
+  if (r.stage == STAGE_STONEMASK && !stonemask_fits(r.fs))
+    return fail("sampling rate too high for the twiddle table (fs <= 48000 supported)");
+  if (r.stage == STAGE_D4C && !d4c_fits(r.fs)) return fail("sampling rate too high for the on-chip FFT (fft > 8192)");
+  p->coded = r.coded;
+  if (r.stage != STAGE_STONEMASK) {
+    // one option for every utterance, or one each (then named in the messages)
+    const bool ct = r.stage == STAGE_CHEAPTRICK;
+    if ((ct ? !r.ct : !r.fft_size || !r.d4c) && (n > 0 || !r.per_utt)) return fail("the option must be given");
+    p->fft_size.resize(n);
+    p->q.resize(n);
+    for (int u = 0; u < n; ++u) {
+      const int k = r.per_utt ? u : 0;
+      p->fft_size[u] = ct ? r.ct[k].fft_size : r.fft_size[k];
+      p->q[u] = ct ? r.ct[k].q1 : r.d4c[k].threshold;
+    }
+    for (int u = 0; u < n; ++u) {
+      const int f = p->fft_size[u], named = r.per_utt ? u : -1;
+      if (ct && (f < 16 || f > WB_TW_N || (f & (f - 1))))
+        return fail("fft_size must be a power of two in [16, 8192]", named);
+      if (!ct && f < 4) return fail("fft_size must be at least 4", named);
+      if (!std::isfinite(p->q[u])) return fail(ct ? "q1 must be finite" : "threshold must be finite", named);
+    }
+    p->row = r.row_stride || r.per_utt || n == 0 ? r.row_stride : p->fft_size[0] / 2 + 1;
+    for (int u = 0; u < n && !r.coded; ++u)
+      if (p->row < p->fft_size[u] / 2 + 1)
+        return fail("row_stride is smaller than fft_size / 2 + 1", r.per_utt ? u : -1);
+    p->table.assign(r.coded ? n : 0, -1);
+    std::vector<int> first;   // coded: the first utterance of each table
+    for (int u = 0; u < n && r.coded; ++u) {
+      for (int t = 0; t < (int)first.size() && p->table[u] < 0; ++t)
+        if (p->fft_size[first[t]] == p->fft_size[u]) p->table[u] = t;
+      if (p->table[u] >= 0) continue;
+      p->table[u] = (int)first.size();
+      first.push_back(u);
+      p->tables.emplace_back();
+      const int rc = ct ? codec_sp_tables(c, r.fs, p->fft_size[u], r.dims, &p->tables.back())
+                        : codec_ap_tables(c, r.fs, p->fft_size[u], &p->tables.back());
+      if (rc) return fail(c->last_error, r.per_utt ? u : -1);
+    }
+    p->nothing = r.coded && !ct && GetNumberOfAperiodicities(r.fs) == 0;
+  }
+  const char *who = stage_name(r.stage);
+  int rc = row_lengths(c, who, "x", r.x_lengths, n, r.x_stride, 1, &p->x_len);
+  if (!rc) rc = row_lengths(c, who, "f0", r.f0_lengths, n, r.f0_stride, 0, &p->f_len);
+  return rc;
+}
+}  // namespace wb
+
+// A stage entry point: x / time_axis / f0 / out are its device rows.
+static int stage_batch(WorldB200 *h, const StageRequest &r, const double *x, const double *time_axis, const double *f0,
+                       double *out) {
+  if (!h) return WORLD_B200_EINVAL;
+  DeviceGuard guard_(&h->c);
+  Ctx *c = &h->c;
+  if (!x || !time_axis || !f0) return stage_fail(c, r.stage, "x, time_axis and f0 must be given");
+  StagePlan p;
+  int rc = stage_plan(c, r, &p);
+  if (rc || p.nothing) return rc;   // nothing to write below 12 kHz, like the reference's empty loops
+  if (!out) return stage_fail(c, r.stage, "the output rows must be given");
+  if (r.n == 0) return 0;
+  Batch b;
+  rc = load_batch(h, x, r.n, r.x_stride, p.x_len.data(), r.fs, time_axis, f0, p.f_len.data(), r.f0_stride, &b);
+  if (rc) return rc;
+  return r.stage == STAGE_CHEAPTRICK ? cheaptrick_run(c, p, b, 0, out)
+         : r.stage == STAGE_D4C     ? d4c_run(c, p, b, 0, out)
+                                    : stonemask_run(c, b, out);
+}
+
+extern "C" {
+
 int world_b200_cheaptrick_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
                                 int fs, const double *time_axis, const double *f0, const int *f0_lengths,
                                 int f0_stride, const CheapTrickOption *opt, double *spectrogram) {
-  if (!h || !x || !time_axis || !f0 || !opt || !spectrogram || n < 0 || fs <= 0) return WORLD_B200_EINVAL;
-  DeviceGuard guard_(&h->c);
-  Batch b;
-  int rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, &b);
-  if (rc) return rc;
-  return cheaptrick_run(&h->c, b, opt->q1, opt->fft_size, spectrogram);
+  StageRequest r{STAGE_CHEAPTRICK, n, x_stride, x_lengths, fs, f0_lengths, f0_stride};
+  r.ct = opt;
+  return stage_batch(h, r, x, time_axis, f0, spectrogram);
 }
 
 int world_b200_d4c_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
                          const double *time_axis, const double *f0, const int *f0_lengths, int f0_stride,
                          int fft_size, const D4COption *opt, double *aperiodicity) {
-  if (!h || !x || !time_axis || !f0 || !opt || !aperiodicity || n < 0 || fs <= 0) return WORLD_B200_EINVAL;
-  DeviceGuard guard_(&h->c);
-  Batch b;
-  int rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, &b);
-  if (rc) return rc;
-  return d4c_run(&h->c, b, fft_size, opt->threshold, aperiodicity);
+  StageRequest r{STAGE_D4C, n, x_stride, x_lengths, fs, f0_lengths, f0_stride};
+  r.fft_size = &fft_size; r.d4c = opt;
+  return stage_batch(h, r, x, time_axis, f0, aperiodicity);
 }
 
 int world_b200_cheaptrick_coded_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
                                       int fs, const double *time_axis, const double *f0, const int *f0_lengths,
                                       int f0_stride, const CheapTrickOption *opt, int number_of_dimensions,
                                       double *coded_spectral_envelope) {
-  if (!h || !x || !time_axis || !f0 || !opt || !coded_spectral_envelope || n < 0 || fs <= 0) return WORLD_B200_EINVAL;
-  DeviceGuard guard_(&h->c);
-  CodecTables t;
-  int rc = codec_sp_tables(&h->c, fs, opt->fft_size, number_of_dimensions, &t);
-  if (rc) return rc;
-  Batch b;
-  rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, &b);
-  if (rc) return rc;
-  return cheaptrick_run(&h->c, b, opt->q1, opt->fft_size, nullptr, &t, coded_spectral_envelope);
+  StageRequest r{STAGE_CHEAPTRICK, n, x_stride, x_lengths, fs, f0_lengths, f0_stride};
+  r.ct = opt; r.coded = true; r.dims = number_of_dimensions;
+  return stage_batch(h, r, x, time_axis, f0, coded_spectral_envelope);
 }
 
 int world_b200_d4c_coded_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
                                const double *time_axis, const double *f0, const int *f0_lengths, int f0_stride,
                                int fft_size, const D4COption *opt, double *coded_aperiodicity) {
-  if (!h || !x || !time_axis || !f0 || !opt || n < 0 || fs <= 0 || fft_size < 2) return WORLD_B200_EINVAL;
-  DeviceGuard guard_(&h->c);
-  CodecTables t;
-  int rc = codec_ap_tables(&h->c, fs, fft_size, &t);
-  if (rc) return rc;
-  if (t.dims == 0) return 0;        // nothing to write below 12 kHz, like the reference's empty loops
-  if (!coded_aperiodicity) return WORLD_B200_EINVAL;
-  Batch b;
-  rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, &b);
-  if (rc) return rc;
-  return d4c_run(&h->c, b, fft_size, opt->threshold, nullptr, &t, coded_aperiodicity);
+  StageRequest r{STAGE_D4C, n, x_stride, x_lengths, fs, f0_lengths, f0_stride};
+  r.fft_size = &fft_size; r.d4c = opt; r.coded = true;
+  return stage_batch(h, r, x, time_axis, f0, coded_aperiodicity);
 }
 
-// ---- per-utterance CheapTrick / D4C options: every check runs before anything is queued and names the first bad
-// utterance
-static int utterance_fail(Ctx *c, int u, const std::string &what) {
-  c->last_error = what + " (utterance " + std::to_string(u) + ")";
-  return WORLD_B200_EINVAL;
+int world_b200_cheaptrick_batch_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
+                                        int fs, const double *time_axis, const double *f0, const int *f0_lengths,
+                                        int f0_stride, const CheapTrickOption *options, int row_stride,
+                                        double *spectrogram) {
+  StageRequest r{STAGE_CHEAPTRICK, n, x_stride, x_lengths, fs, f0_lengths, f0_stride};
+  r.per_utt = true; r.ct = options; r.row_stride = row_stride;
+  return stage_batch(h, r, x, time_axis, f0, spectrogram);
 }
 
-// sizes[u] = options[u].fft_size, checked, and the q1 of each option
-static int check_cheaptrick_options(Ctx *c, const CheapTrickOption *o, int n, std::vector<int> *sizes) {
-  sizes->resize(n);
-  for (int u = 0; u < n; ++u) {
-    const int f = o[u].fft_size;
-    if (f < 16 || f > WB_TW_N || (f & (f - 1)))
-      return utterance_fail(c, u, "CheapTrick options: fft_size must be a power of two in [16, 8192]");
-    if (!std::isfinite(o[u].q1)) return utterance_fail(c, u, "CheapTrick options: q1 must be finite");
-    (*sizes)[u] = f;
-  }
-  return 0;
+int world_b200_cheaptrick_coded_batch_options(WorldB200 *h, const double *x, int n, int x_stride,
+                                              const int *x_lengths, int fs, const double *time_axis,
+                                              const double *f0, const int *f0_lengths, int f0_stride,
+                                              const CheapTrickOption *options, int number_of_dimensions,
+                                              double *coded_spectral_envelope) {
+  StageRequest r{STAGE_CHEAPTRICK, n, x_stride, x_lengths, fs, f0_lengths, f0_stride};
+  r.per_utt = true; r.ct = options; r.coded = true; r.dims = number_of_dimensions;
+  return stage_batch(h, r, x, time_axis, f0, coded_spectral_envelope);
 }
 
-static int check_d4c_options(Ctx *c, const int *fft_sizes, const D4COption *o, int n) {
-  for (int u = 0; u < n; ++u) {
-    if (fft_sizes[u] < 4) return utterance_fail(c, u, "D4C options: fft_size must be at least 4");
-    if (!std::isfinite(o[u].threshold)) return utterance_fail(c, u, "D4C options: threshold must be finite");
-  }
-  return 0;
+int world_b200_d4c_batch_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
+                                 const double *time_axis, const double *f0, const int *f0_lengths, int f0_stride,
+                                 const int *fft_sizes, const D4COption *options, int row_stride,
+                                 double *aperiodicity) {
+  StageRequest r{STAGE_D4C, n, x_stride, x_lengths, fs, f0_lengths, f0_stride};
+  r.per_utt = true; r.fft_size = fft_sizes; r.d4c = options; r.row_stride = row_stride;
+  return stage_batch(h, r, x, time_axis, f0, aperiodicity);
 }
 
-static int check_row_stride(Ctx *c, const std::vector<int> &sizes, int row_stride) {
-  for (size_t u = 0; u < sizes.size(); ++u)
-    if (row_stride < sizes[u] / 2 + 1)
-      return utterance_fail(c, (int)u, "row_stride is smaller than fft_size / 2 + 1");
-  return 0;
+int world_b200_d4c_coded_batch_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
+                                       int fs, const double *time_axis, const double *f0, const int *f0_lengths,
+                                       int f0_stride, const int *fft_sizes, const D4COption *options,
+                                       double *coded_aperiodicity) {
+  StageRequest r{STAGE_D4C, n, x_stride, x_lengths, fs, f0_lengths, f0_stride};
+  r.per_utt = true; r.fft_size = fft_sizes; r.d4c = options; r.coded = true;
+  return stage_batch(h, r, x, time_axis, f0, coded_aperiodicity);
 }
 
-// index of each utterance's size in `distinct` (first appearance order)
-static std::vector<int> size_index(const std::vector<int> &sizes, std::vector<int> *distinct) {
-  std::vector<int> at(sizes.size());
-  for (size_t u = 0; u < sizes.size(); ++u) {
-    const auto it = std::find(distinct->begin(), distinct->end(), sizes[u]);
-    at[u] = (int)(it - distinct->begin());
-    if (it == distinct->end()) distinct->push_back(sizes[u]);
-  }
-  return at;
-}
-
-// CheapTrick over groups of equal options; coded: number_of_dimensions > 0
-static int cheaptrick_options_impl(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
-                                   const double *time_axis, const double *f0, const int *f0_lengths, int f0_stride,
-                                   const CheapTrickOption *opts, int row_stride, double *spectrogram,
-                                   int number_of_dimensions, double *coded) {
-  Ctx *c = &h->c;
-  std::vector<int> sizes, distinct;
-  int rc = check_cheaptrick_options(c, opts, n, &sizes);
-  if (rc || n == 0) return rc;
-  if (!coded && (rc = check_row_stride(c, sizes, row_stride))) return rc;
-  const std::vector<int> at = size_index(sizes, &distinct);
-  std::vector<CodecTables> tables(coded ? distinct.size() : 0);
-  for (size_t s = 0; s < tables.size(); ++s)
-    if ((rc = codec_sp_tables(c, fs, distinct[s], number_of_dimensions, &tables[s]))) {
-      const int u = (int)(std::find(sizes.begin(), sizes.end(), distinct[s]) - sizes.begin());
-      return utterance_fail(c, u, c->last_error);
-    }
-  // one group per distinct (fft_size, q1), in order of first appearance
-  std::vector<UttGroup> groups;
-  for (int u = 0; u < n; ++u) {
-    int g = 0;
-    while (g < (int)groups.size() && !(sizes[groups[g].uid[0]] == sizes[u] && opts[groups[g].uid[0]].q1 == opts[u].q1))
-      ++g;
-    if (g == (int)groups.size()) groups.emplace_back();
-    const int fl = f0_lengths ? f0_lengths[u] : f0_stride;
-    groups[g].uid.push_back(u);
-    groups[g].f_len.push_back(fl);
-    groups[g].max_f_len = std::max(groups[g].max_f_len, fl);
-  }
-  Batch b;
-  if ((rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, &b))) return rc;
-  for (size_t g = 0; g < groups.size() && !rc; ++g) {
-    const int u = groups[g].uid[0];
-    // a batch of one option runs exactly as the one-option call
-    const UttGroup *grp = groups.size() > 1 ? &groups[g] : nullptr;
-    rc = cheaptrick_run(c, b, opts[u].q1, sizes[u], coded ? nullptr : spectrogram, coded ? &tables[at[u]] : nullptr,
-                        coded, grp, row_stride);
-  }
-  return rc;
-}
-
-// D4C with per-utterance options in one launch sequence; coded: CodeAperiodicity rows
-static int d4c_options_impl(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
-                            const double *time_axis, const double *f0, const int *f0_lengths, int f0_stride,
-                            const int *fft_sizes, const D4COption *opts, int row_stride, double *aperiodicity,
-                            bool want_coded, double *coded) {
-  Ctx *c = &h->c;
-  int rc = check_d4c_options(c, fft_sizes, opts, n);
-  if (rc || n == 0) return rc;
-  D4cPerUtt pu;
-  pu.fft_size.assign(fft_sizes, fft_sizes + n);
-  if (!want_coded && (rc = check_row_stride(c, pu.fft_size, row_stride))) return rc;
-  std::vector<int> distinct;
-  if (want_coded) {
-    pu.table = size_index(pu.fft_size, &distinct);
-    pu.tables.resize(distinct.size());
-    for (size_t s = 0; s < distinct.size(); ++s)
-      if ((rc = codec_ap_tables(c, fs, distinct[s], &pu.tables[s]))) {
-        const int u = (int)(std::find(pu.fft_size.begin(), pu.fft_size.end(), distinct[s]) - pu.fft_size.begin());
-        return utterance_fail(c, u, c->last_error);
-      }
-    if (pu.tables[0].dims == 0) return 0;   // nothing to write below 12 kHz, as in world_b200_d4c_coded_batch
-    if (!coded) return WORLD_B200_EINVAL;
-  }
-  pu.threshold.resize(n);
-  for (int u = 0; u < n; ++u) pu.threshold[u] = opts[u].threshold;
-  pu.row_stride = row_stride;
-  Batch b;
-  if ((rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, &b))) return rc;
-  return d4c_run(c, b, pu.fft_size[0], pu.threshold[0], want_coded ? nullptr : aperiodicity,
-                 want_coded ? &pu.tables[0] : nullptr, coded, &pu);
+int world_b200_stonemask_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
+                               int fs, const double *time_axis, const double *f0, const int *f0_lengths,
+                               int f0_stride, double *refined_f0) {
+  return stage_batch(h, {STAGE_STONEMASK, n, x_stride, x_lengths, fs, f0_lengths, f0_stride}, x, time_axis, f0,
+                     refined_f0);
 }
 
 }  // extern "C"
@@ -637,39 +624,6 @@ static int chain_checks(Ctx *c, const ChainRequest &r, ChainPlan *p) {
   p->frame_period = harvest ? opt->harvest.frame_period : opt->dio.frame_period;
   if (!(p->frame_period > 0.0)) return fail("the F0 method's frame_period must be > 0");
 
-  const int n_ap = r.coded ? GetNumberOfAperiodicities(r.fs) : 0;
-  p->sp_row = r.coded ? (size_t)r.dims : (size_t)(fft_size / 2 + 1);
-  p->ap_row = r.coded ? (size_t)n_ap : (size_t)(fft_size / 2 + 1);
-  p->want_sp = r.spectrogram != nullptr;
-  p->want_ap = r.aperiodicity != nullptr && (!r.coded || n_ap > 0);   // no bands below 12 kHz: D4C is skipped
-  if (spectral_options) {
-    // each utterance's CheapTrick option and D4C (fft_size = its CheapTrick size, option), the per-call option standing
-    // in for an array that is NULL; the stage calls' rules, then the codec tables of every distinct size
-    p->cts.assign(n, opt->cheaptrick);
-    p->d4s.assign(n, opt->d4c);
-    if (r.cheaptrick_options) std::copy(r.cheaptrick_options, r.cheaptrick_options + n, p->cts.begin());
-    if (r.d4c_options) std::copy(r.d4c_options, r.d4c_options + n, p->d4s.begin());
-    p->d4_fft.resize(n);
-    for (int u = 0; u < n; ++u) p->d4_fft[u] = p->cts[u].fft_size;
-    std::vector<int> sizes, distinct;
-    rc = check_cheaptrick_options(c, p->cts.data(), n, &sizes);
-    if (!rc) rc = check_d4c_options(c, p->d4_fft.data(), p->d4s.data(), n);
-    if (rc) return rc;
-    size_index(sizes, &distinct);
-    for (const int fft : distinct) {
-      CodecTables t;
-      rc = r.spectrogram ? codec_sp_tables(c, r.fs, fft, r.dims, &t) : 0;
-      if (!rc && r.aperiodicity) rc = codec_ap_tables(c, r.fs, fft, &t);
-      if (rc) return utterance_fail(c, (int)(std::find(sizes.begin(), sizes.end(), fft) - sizes.begin()), c->last_error);
-    }
-  } else if (r.coded) {
-    // the codec tables of every slice or chunk, built once here so that a bad dimension count or fft_size queues nothing
-    CodecTables t;
-    rc = r.spectrogram ? codec_sp_tables(c, r.fs, fft_size, r.dims, &t) : 0;
-    if (!rc && r.aperiodicity) rc = codec_ap_tables(c, r.fs, fft_size, &t);
-    if (rc) return rc;
-  }
-
   p->f_len.resize(n);
   int most = 1;
   for (int u = 0; u < n; ++u) {
@@ -679,10 +633,39 @@ static int chain_checks(Ctx *c, const ChainRequest &r, ChainPlan *p) {
                   std::to_string(r.x_stride) + " samples");
     p->f_len[u] = frames_for(r.fs, xl, p->frame_period);
     if (r.f0_stride && p->f_len[u] > r.f0_stride)
-      return utterance_fail(c, u, "f0_stride smaller than the frame count of an utterance");
+      return fail("f0_stride smaller than the frame count of an utterance (utterance " + std::to_string(u) + ")");
     most = imax(most, p->f_len[u]);
   }
   p->f0_stride = r.f0_stride ? r.f0_stride : most;
+
+  // The stage plans: CheapTrick when a spectrogram is asked for, D4C when an aperiodicity is (a transform, f0_stride 0,
+  // needs both), StoneMask's sampling-rate limit for DIO.  Each utterance's CheapTrick option, and D4C's fft_size (its
+  // CheapTrick size) and option, with the per-call option standing in for a NULL per-utterance array.
+  const bool transform = r.f0_stride == 0;
+  StageRequest s{STAGE_CHEAPTRICK, n, r.x_stride, r.x_lengths, r.fs, p->f_len.data(), p->f0_stride};
+  s.ct = &opt->cheaptrick; s.fft_size = &opt->cheaptrick.fft_size; s.d4c = &opt->d4c;
+  s.coded = r.coded; s.dims = r.dims;
+  std::vector<CheapTrickOption> cts;
+  std::vector<D4COption> d4s;
+  std::vector<int> d4_fft;
+  if (spectral_options) {
+    cts.assign(n, opt->cheaptrick);
+    d4s.assign(n, opt->d4c);
+    if (r.cheaptrick_options) std::copy(r.cheaptrick_options, r.cheaptrick_options + n, cts.begin());
+    if (r.d4c_options) std::copy(r.d4c_options, r.d4c_options + n, d4s.begin());
+    for (const CheapTrickOption &o : cts) d4_fft.push_back(o.fft_size);
+    s.per_utt = true; s.ct = cts.data(); s.fft_size = d4_fft.data(); s.d4c = d4s.data();
+  }
+  if ((r.spectrogram || transform) && (rc = stage_plan(c, s, &p->ct))) return rc;
+  s.stage = STAGE_D4C;
+  if ((r.aperiodicity || transform) && (rc = stage_plan(c, s, &p->d4))) return rc;
+  s.stage = STAGE_STONEMASK;
+  StagePlan stonemask;
+  if (!harvest && (rc = stage_plan(c, s, &stonemask))) return rc;
+  p->sp_row = r.coded ? (size_t)r.dims : (size_t)(fft_size / 2 + 1);
+  p->ap_row = r.coded ? (size_t)GetNumberOfAperiodicities(r.fs) : (size_t)(fft_size / 2 + 1);
+  p->want_sp = r.spectrogram != nullptr;
+  p->want_ap = r.aperiodicity != nullptr && !p->d4.nothing;   // no bands below 12 kHz: D4C is skipped
   return 0;
 }
 
@@ -711,85 +694,16 @@ int chain_f0(WorldB200 *h, const ChainRequest &r, const ChainPlan &p, int u0, in
 
 int chain_spectral(WorldB200 *h, const ChainRequest &r, const ChainPlan &p, int u0, int m, const double *x,
                    const double *time_axis, const double *f0, double *sp, double *ap) {
-  const WorldB200AnalysisOption *opt = r.opt;
-  const int *xl = r.x_lengths ? r.x_lengths + u0 : nullptr, *fl = p.f_len.data() + u0;
-  const int xs = r.x_stride, fs = r.fs, fst = p.f0_stride, fft_size = opt->cheaptrick.fft_size;
-  const double *t = time_axis;
-  const bool per_utt = !p.cts.empty();
-  int rc = 0;
-  if (sp)
-    rc = per_utt ? world_b200_cheaptrick_coded_batch_options(h, x, m, xs, xl, fs, t, f0, fl, fst, p.cts.data() + u0,
-                                                             r.dims, sp)
-         : r.coded ? world_b200_cheaptrick_coded_batch(h, x, m, xs, xl, fs, t, f0, fl, fst, &opt->cheaptrick, r.dims, sp)
-                   : world_b200_cheaptrick_batch(h, x, m, xs, xl, fs, t, f0, fl, fst, &opt->cheaptrick, sp);
-  if (!rc && ap)
-    rc = per_utt ? world_b200_d4c_coded_batch_options(h, x, m, xs, xl, fs, t, f0, fl, fst, p.d4_fft.data() + u0,
-                                                      p.d4s.data() + u0, ap)
-         : r.coded ? world_b200_d4c_coded_batch(h, x, m, xs, xl, fs, t, f0, fl, fst, fft_size, &opt->d4c, ap)
-                   : world_b200_d4c_batch(h, x, m, xs, xl, fs, t, f0, fl, fst, fft_size, &opt->d4c, ap);
+  if (!sp && !ap) return 0;
+  const StagePlan &lens = sp ? p.ct : p.d4;   // both plans hold the chain's lengths
+  Batch b;
+  int rc = load_batch(h, x, m, r.x_stride, lens.x_len.data() + u0, r.fs, time_axis, f0, lens.f_len.data() + u0,
+                      p.f0_stride, &b);
+  if (!rc && sp) rc = cheaptrick_run(&h->c, p.ct, b, u0, sp);
+  if (!rc && ap) rc = d4c_run(&h->c, p.d4, b, u0, ap);
   return rc;
 }
 }  // namespace wb
-
-extern "C" {
-
-int world_b200_cheaptrick_batch_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
-                                        int fs, const double *time_axis, const double *f0, const int *f0_lengths,
-                                        int f0_stride, const CheapTrickOption *options, int row_stride,
-                                        double *spectrogram) {
-  if (!h || !x || !time_axis || !f0 || !spectrogram || n < 0 || fs <= 0 || (n > 0 && !options))
-    return WORLD_B200_EINVAL;
-  DeviceGuard guard_(&h->c);
-  return cheaptrick_options_impl(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, options,
-                                 row_stride, spectrogram, 0, nullptr);
-}
-
-int world_b200_cheaptrick_coded_batch_options(WorldB200 *h, const double *x, int n, int x_stride,
-                                              const int *x_lengths, int fs, const double *time_axis,
-                                              const double *f0, const int *f0_lengths, int f0_stride,
-                                              const CheapTrickOption *options, int number_of_dimensions,
-                                              double *coded_spectral_envelope) {
-  if (!h || !x || !time_axis || !f0 || !coded_spectral_envelope || n < 0 || fs <= 0 || (n > 0 && !options))
-    return WORLD_B200_EINVAL;
-  DeviceGuard guard_(&h->c);
-  return cheaptrick_options_impl(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, options,
-                                 0, nullptr, number_of_dimensions, coded_spectral_envelope);
-}
-
-int world_b200_d4c_batch_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
-                                 const double *time_axis, const double *f0, const int *f0_lengths, int f0_stride,
-                                 const int *fft_sizes, const D4COption *options, int row_stride,
-                                 double *aperiodicity) {
-  if (!h || !x || !time_axis || !f0 || !aperiodicity || n < 0 || fs <= 0 || (n > 0 && (!fft_sizes || !options)))
-    return WORLD_B200_EINVAL;
-  DeviceGuard guard_(&h->c);
-  return d4c_options_impl(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, fft_sizes, options,
-                          row_stride, aperiodicity, false, nullptr);
-}
-
-int world_b200_d4c_coded_batch_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
-                                       int fs, const double *time_axis, const double *f0, const int *f0_lengths,
-                                       int f0_stride, const int *fft_sizes, const D4COption *options,
-                                       double *coded_aperiodicity) {
-  if (!h || !x || !time_axis || !f0 || n < 0 || fs <= 0 || (n > 0 && (!fft_sizes || !options)))
-    return WORLD_B200_EINVAL;
-  DeviceGuard guard_(&h->c);
-  return d4c_options_impl(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, fft_sizes, options,
-                          0, nullptr, true, coded_aperiodicity);
-}
-
-int world_b200_stonemask_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
-                               int fs, const double *time_axis, const double *f0, const int *f0_lengths,
-                               int f0_stride, double *refined_f0) {
-  if (!h || !x || !time_axis || !f0 || !refined_f0 || n < 0 || fs <= 0) return WORLD_B200_EINVAL;
-  DeviceGuard guard_(&h->c);
-  Batch b;
-  int rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, f0_lengths, f0_stride, &b);
-  if (rc) return rc;
-  return stonemask_run(&h->c, b, refined_f0);
-}
-
-}  // extern "C"
 
 static int f0_lengths_from_x(int n, int x_stride, const int *x_lengths, int fs, double frame_period,
                              int f0_stride, std::vector<int> *out, std::string *err) {
@@ -818,11 +732,12 @@ static int f0_batch(WorldB200 *h, const double *x, int n, int x_stride, const in
   if constexpr (harvest) rc = harvest_plan(&h->c, fs, opt, n, per_utt, opt->frame_period, &groups);
   else rc = dio_plan(&h->c, fs, opt, n, per_utt, opt->frame_period, opt->speed, &groups);
   if (rc) return rc;
-  std::vector<int> fl;
-  rc = f0_lengths_from_x(n, x_stride, x_lengths, fs, opt->frame_period, f0_stride, &fl, &h->c.last_error);
+  std::vector<int> xl, fl;
+  rc = row_lengths(&h->c, harvest ? "Harvest" : "DIO", "x", x_lengths, n, x_stride, 1, &xl);
+  if (!rc) rc = f0_lengths_from_x(n, x_stride, x_lengths, fs, opt->frame_period, f0_stride, &fl, &h->c.last_error);
   if (rc) return rc;
   Batch b;
-  rc = load_batch(h, x, n, x_stride, x_lengths, fs, time_axis, f0, fl.data(), f0_stride, &b);
+  rc = load_batch(h, x, n, x_stride, xl.data(), fs, time_axis, f0, fl.data(), f0_stride, &b);
   if (rc) return rc;
   b.x_len_host = x_lengths;
   if constexpr (harvest) {

@@ -66,19 +66,17 @@ struct ChainPlan {
   int f0_stride = 0;                    // the request's, or (f0_stride 0) the largest frame count
   size_t sp_row = 0, ap_row = 0;        // doubles per frame of the spectrogram / aperiodicity rows
   bool want_sp = false, want_ap = false;   // CheapTrick / D4C run (coded rows below 12 kHz have no bands: no D4C)
-  // with per-utterance spectral options (empty otherwise): each utterance's CheapTrick option, and D4C's fft_size (the
-  // utterance's CheapTrick size) and option
-  std::vector<CheapTrickOption> cts;
-  std::vector<int> d4_fft;
-  std::vector<D4COption> d4s;
+  StagePlan ct, d4;                        // the stage plans of CheapTrick / D4C, where they run (transform: both)
 };
 
-// Every check of an analysis chain, before anything is queued: EINVAL with last_error "<who>: ...", naming the first
-// bad utterance where there is one.  Fills the plan that chain_f0 / chain_spectral and the drivers read.
+// Every check of an analysis chain, before anything is queued (the stage plans' included: a chain whose StoneMask or
+// D4C cannot run at its fs is rejected here): EINVAL with last_error "<who>: ...", naming the first bad utterance
+// where there is one.  Fills the plan that chain_f0 / chain_spectral and the drivers read.
 int chain_plan(Ctx *c, const ChainRequest &r, const char *who, ChainPlan *p);
 // The chain's stages for utterances [u0, u0 + m) of a planned request, enqueued on h (a lane, or the pipeline's
 // context): x, time_axis, f0, sp and ap are device rows that start at utterance u0.  chain_f0: Harvest, or DIO +
-// StoneMask.  chain_spectral: CheapTrick into sp, then D4C into ap; a NULL sp or ap skips that stage.
+// StoneMask (the F0 stage calls).  chain_spectral: one Batch of the rows for both drivers, CheapTrick into sp, then D4C
+// into ap; a NULL sp or ap skips that stage.
 int chain_f0(WorldB200 *h, const ChainRequest &r, const ChainPlan &p, int u0, int m, const double *x, double *time_axis,
              double *f0);
 int chain_spectral(WorldB200 *h, const ChainRequest &r, const ChainPlan &p, int u0, int m, const double *x,

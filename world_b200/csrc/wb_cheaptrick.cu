@@ -226,17 +226,24 @@ void ct_frame_kernel(CtParams p) { ct_frame_body<false>(p); }
 void ct_coded_kernel(CtParams p) { ct_frame_body<true>(p); }
 #endif
 
-int cheaptrick_run(Ctx *ctx, const Batch &b, double q1, int fft_size, double *spectrogram,
-                   const CodecTables *coded, double *coded_out, const UttGroup *group, int row_stride) {
+namespace {
+// The utterances of a batch that share one CheapTrick option: their indices in the batch, ascending, and their frame
+// counts.  ct_launch runs one launch sequence over them, reaching each row through the batch's own pointers.
+struct UttGroup {
+  std::vector<int> uid, f_len;
+  int max_f_len = 0;
+};
+}  // namespace
+
+// One launch sequence of one option (fft_size checked by stage_plan); row_stride: doubles per spectrogram row
+// (0: fft_size / 2 + 1)
+static int ct_launch(Ctx *ctx, const Batch &b, double q1, int fft_size, double *spectrogram, const CodecTables *coded,
+                     double *coded_out, const UttGroup *group, int row_stride) {
   const int n_all = group ? (int)group->uid.size() : b.n;
   const int max_f_len = group ? group->max_f_len : b.max_f_len;
   if (n_all <= 0 || max_f_len <= 0) return 0;
   int lg = 0;
   while ((1 << lg) < fft_size) ++lg;
-  if ((1 << lg) != fft_size || fft_size < 16 || fft_size > WB_TW_N) {
-    ctx->last_error = "CheapTrick: fft_size must be a power of two in [16, 8192]";
-    return 3;
-  }
   const double f0_floor = 3.0 * b.fs / (fft_size - 3.0);  // GetF0FloorForCheapTrick, :196-198
   const int bins = fft_size / 2 + 1;
   // a frame draws at most (fft_size - 2) + bins numbers (2h+1 <= fft_size - 2 above the floor)
@@ -308,6 +315,33 @@ int cheaptrick_run(Ctx *ctx, const Batch &b, double q1, int fft_size, double *sp
     if (rc) return rc;
   }
   return 0;
+}
+
+int cheaptrick_run(Ctx *ctx, const StagePlan &stage, const Batch &b, int u0, double *out) {
+  // one group per distinct (fft_size, q1), in order of first appearance
+  std::vector<UttGroup> groups;
+  for (int k = 0; k < b.n; ++k) {
+    const int u = u0 + k;
+    size_t g = 0;
+    while (g < groups.size() && !(stage.fft_size[u0 + groups[g].uid[0]] == stage.fft_size[u] &&
+                                  stage.q[u0 + groups[g].uid[0]] == stage.q[u]))
+      ++g;
+    if (g == groups.size()) groups.emplace_back();
+    groups[g].uid.push_back(k);
+    groups[g].f_len.push_back(stage.f_len[u]);
+    groups[g].max_f_len = imax(groups[g].max_f_len, stage.f_len[u]);
+  }
+  int rc = 0;
+  for (size_t g = 0; g < groups.size() && !rc; ++g) {
+    const int u = u0 + groups[g].uid[0];
+    // a batch of one option runs exactly as the one-option call
+    const UttGroup *grp = groups.size() > 1 ? &groups[g] : nullptr;
+    const double q1 = stage.q[u];
+    const int fft_size = stage.fft_size[u];
+    rc = stage.coded ? ct_launch(ctx, b, q1, fft_size, nullptr, &stage.tables[stage.table[u]], out, grp, 0)
+                     : ct_launch(ctx, b, q1, fft_size, out, nullptr, nullptr, grp, stage.row);
+  }
+  return rc;
 }
 
 }  // namespace wb

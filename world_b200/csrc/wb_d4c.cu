@@ -667,29 +667,30 @@ WB_KERNEL_PLAIN d4c_list_all_kernel(D4cParams p, int n_utts) {
   p.slow_list[at] = (int)g;
 }
 
-int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *aperiodicity,
-            const CodecTables *coded, double *coded_out, const D4cPerUtt *per_utt) {
-  if (b.n <= 0 || b.max_f_len <= 0) return 0;
-  if (coded && coded->dims == 0) return 0;   // below 12 kHz the coded row is empty (codec.cpp:216-219)
+// sizes with the reference's expressions (host libm), d4c.cpp:350-365 and :262-272
+static int d4c_d_fft(int fs) { return static_cast<int>(pow(2.0, 1.0 + static_cast<int>(log(4.0 * fs / 47.0 + 1) / kLog2))); }
+static int d4c_lt_fft(int fs) { return static_cast<int>(pow(2.0, 1.0 + static_cast<int>(log(3.0 * fs / 40.0 + 1) / kLog2))); }
+
+bool d4c_fits(int fs) { return d4c_d_fft(fs) <= WB_TW_N && d4c_lt_fft(fs) <= WB_TW_N; }
+
+int d4c_run(Ctx *ctx, const StagePlan &stage, const Batch &b, int u0, double *out) {
+  if (b.n <= 0 || b.max_f_len <= 0 || stage.nothing) return 0;   // below 12 kHz the coded row is empty (codec.cpp:216-219)
   const int fs = b.fs;
+  // one option for the whole batch: scalars; otherwise each utterance's threshold, output width (fft_size / 2 + 1 bins)
+  // and, for coded rows, band-centre table come from device arrays (D4C's own transforms depend on fs alone)
+  bool per_utt = false;
+  for (int k = 1; k < b.n; ++k)
+    per_utt = per_utt || stage.fft_size[u0 + k] != stage.fft_size[u0] || stage.q[u0 + k] != stage.q[u0];
+  const CodecTables *coded = stage.coded ? &stage.tables[stage.table[u0]] : nullptr;
   D4cParams p;
   memset(&p, 0, sizeof(p));
   p.fs = fs;
-  p.ct_fft_size = fft_size;
-  p.threshold = threshold;
-  // sizes with the reference's expressions (host libm), d4c.cpp:350-365 and :262-272
-  p.d_fft = static_cast<int>(pow(2.0, 1.0 + static_cast<int>(log(4.0 * fs / 47.0 + 1) / kLog2)));
-  p.lt_fft = static_cast<int>(pow(2.0, 1.0 + static_cast<int>(log(3.0 * fs / 40.0 + 1) / kLog2)));
+  p.ct_fft_size = stage.fft_size[u0];
+  p.threshold = stage.q[u0];
+  p.d_fft = d4c_d_fft(fs);
+  p.lt_fft = d4c_lt_fft(fs);
   for (p.d_lg = 0; (1 << p.d_lg) < p.d_fft; ++p.d_lg) {}
   for (p.lt_lg = 0; (1 << p.lt_lg) < p.lt_fft; ++p.lt_lg) {}
-  if (fft_size < 4) {
-    ctx->last_error = "D4C: fft_size must be at least 4";
-    return 3;
-  }
-  if (p.d_fft > WB_TW_N || p.lt_fft > WB_TW_N) {
-    ctx->last_error = "D4C: sampling rate too high for the on-chip FFT (fft > 8192)";
-    return 3;
-  }
   p.n_ap = static_cast<int>(dmin(15000.0, fs / 2.0 - 3000.0) / 3000.0);
   if (p.n_ap < 0) p.n_ap = 0;
   p.win_len = static_cast<int>(3000.0 * p.d_fft / fs) * 2 + 1;
@@ -697,17 +698,18 @@ int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *ap
   p.b0 = static_cast<int>(ceil(100.0 * p.lt_fft / fs));
   p.b1 = static_cast<int>(ceil(4000.0 * p.lt_fft / fs));
   p.b2 = static_cast<int>(ceil(7900.0 * p.lt_fft / fs));
-  const int bins = fft_size / 2 + 1;
-  p.out_stride = per_utt ? per_utt->row_stride : bins;
-  // per-utterance band-centre tables: one per distinct fft_size, concatenated
+  p.out_stride = stage.row;
+  // per-utterance band-centre tables: one per distinct fft_size of the batch, concatenated in order of first appearance
   std::vector<int> ctab_idx;
   std::vector<double> ctab_frac;
-  std::vector<int> ctab_off;
+  std::vector<int> ctab_off(stage.tables.size(), -1);
   if (per_utt && coded) {
-    for (const CodecTables &t : per_utt->tables) {
-      ctab_off.push_back((int)ctab_idx.size());
-      ctab_idx.insert(ctab_idx.end(), t.idx.begin(), t.idx.end());
-      ctab_frac.insert(ctab_frac.end(), t.frac.begin(), t.frac.end());
+    for (int k = 0; k < b.n; ++k) {
+      const int t = stage.table[u0 + k];
+      if (ctab_off[t] >= 0) continue;
+      ctab_off[t] = (int)ctab_idx.size();
+      ctab_idx.insert(ctab_idx.end(), stage.tables[t].idx.begin(), stage.tables[t].idx.end());
+      ctab_frac.insert(ctab_frac.end(), stage.tables[t].frac.begin(), stage.tables[t].frac.end());
     }
   }
 
@@ -741,8 +743,8 @@ int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *ap
   cudaFuncSetAttribute(d4c_body_slow_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_slow);
 #endif
   int rc = 0;
-  for (int u0 = 0; u0 < b.n && rc == 0; u0 += chunk) {
-    const int n = imin(chunk, b.n - u0);
+  for (int c0 = 0; c0 < b.n && rc == 0; c0 += chunk) {
+    const int n = imin(chunk, b.n - c0);
     const size_t slots = (size_t)n * b.f_stride;
     ArenaPlan plan;
     const size_t o_ca = plan.add(slots * 4), o_oa = plan.add(slots * 4);
@@ -763,24 +765,24 @@ int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *ap
     double *nuttall = (double *)(blk + o_nut);
     unsigned *draws = (unsigned *)(blk + o_draws);
     dev_memcpy_h2d(ctx, nuttall, nuttall_host, (size_t)p.win_len * 8);
-    const double *f0 = b.f0 + (size_t)u0 * b.f_stride;
-    const int *f_len = b.f_len + u0;
-    p.x = b.x + (size_t)u0 * b.x_stride; p.x_len = b.x_len + u0; p.x_stride = b.x_stride;
-    p.time_axis = b.time_axis + (size_t)u0 * b.f_stride; p.f0 = f0; p.f_len = f_len;
+    const double *f0 = b.f0 + (size_t)c0 * b.f_stride;
+    const int *f_len = b.f_len + c0;
+    p.x = b.x + (size_t)c0 * b.x_stride; p.x_len = b.x_len + c0; p.x_stride = b.x_stride;
+    p.time_axis = b.time_axis + (size_t)c0 * b.f_stride; p.f0 = f0; p.f_len = f_len;
     p.f_stride = b.f_stride;
     p.nuttall = nuttall; p.draws = draws; p.draw_stride = draw_stride_full;
     p.off_a = off_a; p.count_b = count_b; p.off_b = off_b; p.selected = selected;
-    p.out = aperiodicity ? aperiodicity + (size_t)u0 * b.f_stride * p.out_stride : nullptr;
+    p.out = coded ? nullptr : out + (size_t)c0 * b.f_stride * p.out_stride;
     p.tw = ctx->twiddle; p.status = ctx->status_dev;
     p.tw_body = ctx->twiddle_sized + tw_sized_offset(p.d_lg);
     if (per_utt) {
       std::vector<int> ui((size_t)2 * n);
       for (int k = 0; k < n; ++k) {
-        ui[k] = per_utt->fft_size[u0 + k];
-        ui[n + k] = coded ? ctab_off[per_utt->table[u0 + k]] : 0;
+        ui[k] = stage.fft_size[u0 + c0 + k];
+        ui[n + k] = coded ? ctab_off[stage.table[u0 + c0 + k]] : 0;
       }
       unsigned char *d = blk + o_uopt;   // thresholds first: 8-byte aligned
-      rc = dev_memcpy_h2d(ctx, d, per_utt->threshold.data() + u0, (size_t)n * 8);
+      rc = dev_memcpy_h2d(ctx, d, stage.q.data() + u0 + c0, (size_t)n * 8);
       if (!rc) rc = dev_memcpy_h2d(ctx, d + (size_t)n * 8, ui.data(), (size_t)n * 8);
       if (rc) break;
       p.u_thr = (const double *)d; p.u_fft = (const int *)(d + (size_t)n * 8);
@@ -791,7 +793,7 @@ int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *ap
       if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_cfrac, per_utt ? ctab_frac.data() : coded->frac.data(), n_tab * 8);
       if (rc) break;
       p.c_n = coded->dims; p.c_idx = (const int *)(blk + o_cidx); p.c_frac = (const double *)(blk + o_cfrac);
-      p.c_out = coded_out + (size_t)u0 * b.f_stride * coded->dims;
+      p.c_out = out + (size_t)c0 * b.f_stride * coded->dims;
     }
     p.slow_list = (int *)(blk + o_slow); p.slow_count = (int *)(blk + o_nslow);
     dev_memset(ctx, p.slow_count, 0, 4);

@@ -5,6 +5,8 @@
 #include "wb_fft.cuh"
 #include "../../include/world/dio.h"
 #include "../../include/world/harvest.h"
+#include "../../include/world/cheaptrick.h"
+#include "../../include/world/d4c.h"
 #include <string>
 #include <vector>
 
@@ -262,30 +264,54 @@ struct SynthesisRows {
 // f0 rows and stretches its decoded envelope block right after the decode.
 int synthesis_run(Ctx *ctx, const SynthesisPlan &p, int u0, int m, const SynthesisRows &rows);
 
-// The utterances of a batch that share one CheapTrick option (world_b200_cheaptrick_*batch_options): their batch
-// indices, ascending, and their frame counts.  cheaptrick_run runs one launch sequence over them, reaching each row
-// through the batch's own pointers.
-struct UttGroup {
-  std::vector<int> uid, f_len;
-  int max_f_len = 0;
+// The CheapTrick, D4C and StoneMask stages: one checked plan per call (a stage entry point, or an analysis chain), then
+// a run over the rows of each batch, slice or chunk.  What a stage call receives besides its device rows: n utterances
+// of x_stride samples and f0_stride frames (NULL lengths: full rows) at fs, and the stage's option -- one (per_utt
+// false) or one per utterance.  CheapTrick takes ct; D4C takes its fft_size and d4c.  coded: the rows take dims
+// (CheapTrick) or GetNumberOfAperiodicities(fs) (D4C) coded values per frame.  row_stride: doubles per full row, at
+// least every utterance's fft_size / 2 + 1 (0: the one option's fft_size / 2 + 1).
+enum StageKind { STAGE_CHEAPTRICK, STAGE_D4C, STAGE_STONEMASK };
+struct StageRequest {   // brace-initialised in field order up to f0_stride
+  StageKind stage;
+  int n, x_stride;
+  const int *x_lengths;
+  int fs;
+  const int *f0_lengths;
+  int f0_stride;
+  bool per_utt = false;
+  const CheapTrickOption *ct = nullptr;
+  const int *fft_size = nullptr;
+  const D4COption *d4c = nullptr;
+  bool coded = false;
+  int dims = 0;
+  int row_stride = 0;
 };
-// row_stride: doubles per spectrogram row (0: fft_size / 2 + 1)
-int cheaptrick_run(Ctx *ctx, const Batch &b, double q1, int fft_size, double *spectrogram,
-                   const CodecTables *coded = nullptr, double *coded_out = nullptr, const UttGroup *group = nullptr,
-                   int row_stride = 0);
-// Per-utterance D4C options (world_b200_d4c_*batch_options): D4C's own transforms depend on fs alone, so one launch
-// sequence serves the batch; each utterance's threshold, output width (fft_size / 2 + 1 bins) and, for coded rows,
-// band-centre table (codec_ap_tables at its fft_size) come from these host arrays of b.n entries.
-struct D4cPerUtt {
-  std::vector<int> fft_size;
-  std::vector<double> threshold;
-  std::vector<int> table;           // coded: index into tables
-  std::vector<CodecTables> tables;  // coded: one per distinct fft_size
-  int row_stride = 0;               // doubles per aperiodicity row
+// Everything a stage run reads besides the rows, made once per call and const afterwards.
+struct StagePlan {
+  std::vector<int> x_len, f_len;    // [n]
+  std::vector<int> fft_size;        // [n] CheapTrick / D4C
+  std::vector<double> q;            // [n] q1 (CheapTrick) or threshold (D4C)
+  bool coded = false;
+  std::vector<int> table;           // [n] coded: the utterance's entry of tables
+  std::vector<CodecTables> tables;  // coded: one per distinct fft_size, in order of first appearance
+  int row = 0;                      // doubles per full output row
+  bool nothing = false;             // coded D4C below 12 kHz: no bands, nothing to write (a NULL output is allowed)
 };
-int d4c_run(Ctx *ctx, const Batch &b, int fft_size, double threshold, double *aperiodicity,
-            const CodecTables *coded = nullptr, double *coded_out = nullptr, const D4cPerUtt *per_utt = nullptr);
+// Every check of a stage call before anything is queued, in this order: n and fs; the stage's sampling-rate limits
+// (StoneMask: fs <= 48 kHz; D4C: its transforms within the on-chip FFT); each option (CheapTrick: fft_size a power of
+// two in [16, 8192], q1 finite; D4C: fft_size >= 4, threshold finite); row_stride; the codec tables of each distinct
+// fft_size; each utterance's x and f0 lengths (1 .. x_stride, 0 .. f0_stride).  EINVAL with last_error "<stage>: ...",
+// naming the first bad utterance where there is one.
+int stage_plan(Ctx *ctx, const StageRequest &r, StagePlan *p);
+// The stage over batch b, whose rows are the plan's utterances [u0, u0 + b.n) (its lengths uploaded from the plan's).
+// CheapTrick runs one launch sequence per distinct (fft_size, q1) among them, in order of first appearance; D4C one
+// launch sequence, with per-utterance device arrays when their options differ.  out: full or coded rows, as planned.
+int cheaptrick_run(Ctx *ctx, const StagePlan &plan, const Batch &b, int u0, double *out);
+int d4c_run(Ctx *ctx, const StagePlan &plan, const Batch &b, int u0, double *out);
 int stonemask_run(Ctx *ctx, const Batch &b, double *refined_f0);
+// the stages' sampling-rate limits (stage_plan): D4C's transforms and StoneMask's largest window fit the on-chip FFT
+bool d4c_fits(int fs);
+bool stonemask_fits(int fs);
 // The F0 estimators (wb_harvest.cu, wb_dio.cu) take the public options.  Per utterance (per_utt: opts[u] is utterance
 // u's, else opts[0] serves all), the F0 range may differ, frame_period (DIO: and speed) may not.  *_plan checks that
 // frame_period (and speed) against the batch's, then groups the utterances by range and builds each group's band list

@@ -117,16 +117,18 @@ WB_KERNEL(64, 8) stonemask_kernel(SmParams p) {
   if (tid == 0) p.out[fidx] = mean_f0;
 }
 
+// the longest window (f0 at 40 Hz) of the kernel's transforms
+static int sm_nwin_max(int fs) { return 2 * static_cast<int>(1.5 * fs / 40.0 + 1.0) + 1; }
+
+bool stonemask_fits(int fs) {
+  int lg = 0;
+  while ((2 << lg) <= sm_nwin_max(fs)) ++lg;
+  return (1 << (lg + 2)) <= WB_TW_N;
+}
+
 int stonemask_run(Ctx *ctx, const Batch &b, double *refined_f0) {
   if (b.n <= 0 || b.max_f_len <= 0) return 0;
-  const int h_max = static_cast<int>(1.5 * b.fs / 40.0 + 1.0);
-  const int nwin_max = 2 * h_max + 1;
-  int lg = 0;
-  while ((2 << lg) <= nwin_max) ++lg;
-  if ((1 << (lg + 2)) > WB_TW_N) {
-    ctx->last_error = "StoneMask: sampling rate too high for the twiddle table (fs <= 48000 supported)";
-    return 3;
-  }
+  const int nwin_max = sm_nwin_max(b.fs);
   const size_t smem = (size_t)(2 * nwin_max + WB_REDN_DOUBLES) * sizeof(double);
 #ifndef WB_EMU
   cudaFuncSetAttribute(stonemask_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
