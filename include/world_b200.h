@@ -254,6 +254,47 @@ int world_b200_synthesis_coded_host_modified(WorldB200 *ctx, const double *f0, c
                                              int y_stride, const double *f0_scale, const double *spectral_ratio,
                                              int nbit, void *y);
 
+/* ---- Synthesis with one fft_size per utterance: the way back from world_b200_cheaptrick_batch_options /
+ * world_b200_d4c_batch_options (full rows) and world_b200_analyze_coded_*_spectral_options (coded rows).
+ * fft_sizes is a HOST array of n_utts: utterance u is synthesised at fft_sizes[u], a power of two in [16, 4096] -- the
+ * size that sets its lowest_f0 = fs / fft_size + 1, its DC remover, its response length and its decode tables, as the
+ * reference demo's Synthesis call with CheapTrick's fft_size.  The sizes may come in any order.
+ *   - Output: every row equals, bit for bit, the one-size call of the same family (world_b200_synthesis_batch,
+ *     world_b200_synthesis_coded_batch_modified, world_b200_synthesis_coded_host_modified, world_b200_modify_batch) on
+ *     that utterance alone at fft_sizes[u].  A call whose sizes are all equal is that call.
+ *   - Validation, before any work is queued (WORLD_B200_EINVAL, world_b200_last_error() naming the first bad
+ *     utterance): fft_sizes non-NULL and each a power of two in [16, 4096]; full rows: row_stride >= fft_sizes[u]/2 + 1
+ *     for every u; coded rows: number_of_dimensions in [1, fft_sizes[u]/2] for every u; then the checks of the one-size
+ *     call.  Stream behaviour as that call's. */
+/* spectrogram / aperiodicity [n][f0_stride][row_stride] (DEVICE), of which utterance u reads fft_sizes[u]/2 + 1 values
+ * per frame: the layout the *_batch_options stages write.  Otherwise world_b200_synthesis_batch. */
+int world_b200_synthesis_batch_options(WorldB200 *ctx, const double *f0, const int *f0_lengths, int n_utts,
+                                       int f0_stride, const double *spectrogram, const double *aperiodicity,
+                                       int row_stride, const int *fft_sizes, double frame_period, int fs,
+                                       const int *y_lengths, int y_stride, double *y);
+/* Coded rows as world_b200_synthesis_coded_batch_modified (f0_scale / spectral_ratio may be NULL; nbit 0: float64 y,
+ * 16: int16 y), each utterance decoded and synthesised at its own size.  The pulse responses of a pass are computed in
+ * one launch per distinct size; the decoded rows of a pass are laid out at the largest size's bins. */
+int world_b200_synthesis_coded_batch_options(WorldB200 *ctx, const double *f0, const int *f0_lengths, int n_utts,
+                                             int f0_stride, const double *coded_spectral_envelope,
+                                             int number_of_dimensions, const double *coded_aperiodicity,
+                                             const int *fft_sizes, double frame_period, int fs, const int *y_lengths,
+                                             int y_stride, const double *f0_scale, const double *spectral_ratio,
+                                             int nbit, void *y);
+/* The same for HOST arrays through the pipeline of world_b200_synthesis_coded_host. */
+int world_b200_synthesis_coded_host_options(WorldB200 *ctx, const double *f0, const int *f0_lengths, int n_utts,
+                                            int f0_stride, const double *coded_spectral_envelope,
+                                            int number_of_dimensions, const double *coded_aperiodicity,
+                                            const int *fft_sizes, double frame_period, int fs, const int *y_lengths,
+                                            int y_stride, const double *f0_scale, const double *spectral_ratio,
+                                            int nbit, void *y);
+/* world_b200_modify_batch on spectrogram rows [n][f0_stride][row_stride] (DEVICE): utterance u's envelope is the first
+ * fft_sizes[u]/2 + 1 values of each row, stretched with its own size (the stretch tables are planned once per distinct
+ * (ratio, fft_size)).  fft_sizes and row_stride are read only with spectral_ratio. */
+int world_b200_modify_batch_options(WorldB200 *ctx, double *f0, const int *f0_lengths, int n_utts, int f0_stride,
+                                    double *spectrogram, int row_stride, const int *fft_sizes, int fs,
+                                    const double *f0_scale, const double *spectral_ratio);
+
 /* ---- codec over a batch (codec.h:20-92) -- SURVEY.md 8 row f2; all DEVICE pointers ------ */
 /* aperiodicity [n][f0_stride][fft_size/2+1] -> coded [n][f0_stride][GetNumberOfAperiodicities(fs)]. */
 int world_b200_code_aperiodicity_batch(WorldB200 *ctx, const double *aperiodicity, int n_utts,
@@ -571,6 +612,27 @@ int world_b200_transform_host(WorldB200 *ctx, const void *x, int nbit, int n_utt
                               int fs, const WorldB200AnalysisOption *option, const HarvestOption *harvest_options,
                               const DioOption *dio_options, const double *f0_scale, const double *spectral_ratio,
                               const double *time_scale, int nbit_out, void *y, int y_stride, int *y_lengths);
+/* world_b200_transform_batch / world_b200_transform_host with per-utterance spectral options: cheaptrick_options and
+ * d4c_options are HOST arrays of n_utts (either may be NULL: option->cheaptrick / option->d4c for every utterance).
+ * Utterance u is analysed by CheapTrick with cheaptrick_options[u] and by D4C at the same fft_size, then modified and
+ * synthesised at that size.  Every row equals, bit for bit, world_b200_cheaptrick_batch_options /
+ * world_b200_d4c_batch_options (after the F0 stage of world_b200_analyze_batch) -> world_b200_modify_batch_options ->
+ * world_b200_synthesis_batch_options with frame_period * time_scale[u].  Validation adds the rules of the stage calls
+ * with options, and each utterance's fft_size within Synthesis's powers of two in [16, 4096]. */
+int world_b200_transform_batch_spectral_options(WorldB200 *ctx, const void *x, int nbit, int n_utts, int x_stride,
+                                                const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                                const HarvestOption *harvest_options, const DioOption *dio_options,
+                                                const CheapTrickOption *cheaptrick_options,
+                                                const D4COption *d4c_options, const double *f0_scale,
+                                                const double *spectral_ratio, const double *time_scale, int nbit_out,
+                                                void *y, int y_stride, int *y_lengths);
+int world_b200_transform_host_spectral_options(WorldB200 *ctx, const void *x, int nbit, int n_utts, int x_stride,
+                                               const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                               const HarvestOption *harvest_options, const DioOption *dio_options,
+                                               const CheapTrickOption *cheaptrick_options,
+                                               const D4COption *d4c_options, const double *f0_scale,
+                                               const double *spectral_ratio, const double *time_scale, int nbit_out,
+                                               void *y, int y_stride, int *y_lengths);
 
 #ifdef __cplusplus
 }

@@ -303,4 +303,35 @@ inline int Synthesis(const double *const *f0s, const int *f0_lengths, int n_utts
   return rc;
 }
 
+// One fft_size per utterance (fft_sizes.size() == n_utts; world_b200_synthesis_batch_options): spectrograms[u][i] and
+// aperiodicities[u][i] hold fft_sizes[u] / 2 + 1 doubles, as the CheapTrick / D4C overloads with options write them;
+// ys[u] -> y_lengths[u] doubles.
+inline int Synthesis(const double *const *f0s, const int *f0_lengths, int n_utts, const double *const *const *spectrograms,
+                     const double *const *const *aperiodicities, const std::vector<int> &fft_sizes,
+                     double frame_period, int fs, const int *y_lengths, double *const *ys) {
+  using namespace world_b200;
+  if (n_utts < 0 || fft_sizes.size() != static_cast<size_t>(n_utts)) return WORLD_B200_EINVAL;
+  if (n_utts == 0) return 0;
+  WorldB200 *w = shared_context();
+  if (!w) return WORLD_B200_ECUDA;
+  std::vector<int> bins(n_utts);
+  for (int u = 0; u < n_utts; ++u) bins[u] = fft_sizes[u] / 2 + 1;
+  const int f_stride = max_of(f0_lengths, n_utts), y_stride = max_of(y_lengths, n_utts), row = max_of(bins.data(), n_utts);
+  std::vector<double> hs(static_cast<size_t>(n_utts) * f_stride * row, 1.0), ha(hs.size(), 1.0);
+  for (int u = 0; u < n_utts; ++u)
+    for (int i = 0; i < f0_lengths[u] && bins[u] > 0; ++i) {
+      std::memcpy(hs.data() + (static_cast<size_t>(u) * f_stride + i) * row, spectrograms[u][i], sizeof(double) * bins[u]);
+      std::memcpy(ha.data() + (static_cast<size_t>(u) * f_stride + i) * row, aperiodicities[u][i], sizeof(double) * bins[u]);
+    }
+  DeviceArray df(static_cast<size_t>(n_utts) * f_stride), ds(hs.size()), da(ha.size()), dy(static_cast<size_t>(n_utts) * y_stride);
+  int rc = upload(df, pack(f0s, f0_lengths, n_utts, f_stride));
+  if (!rc) rc = upload(ds, hs);
+  if (!rc) rc = upload(da, ha);
+  if (!rc && !dy.p) rc = WORLD_B200_ENOMEM;
+  if (!rc) rc = world_b200_synthesis_batch_options(w, df.p, f0_lengths, n_utts, f_stride, ds.p, da.p, row, fft_sizes.data(), frame_period, fs, y_lengths, y_stride, dy.p);
+  if (!rc) rc = world_b200_synchronize(w);
+  if (!rc) rc = download_rows(dy, n_utts, y_stride, y_lengths, ys);
+  return rc;
+}
+
 #endif  // WORLD_B200_HPP_

@@ -103,6 +103,13 @@ ABI = {
                                                             C.c_double, C.c_int, _IP, C.c_int, _P, _P, C.c_int, _P]),
     "world_b200_synthesis_coded_host_modified": (C.c_int, [_P, _P, _IP, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int,
                                                            C.c_double, C.c_int, _IP, C.c_int, _P, _P, C.c_int, _P]),
+    "world_b200_synthesis_batch_options": (C.c_int, [_P, _P, _IP, C.c_int, C.c_int, _P, _P, C.c_int, _IP, C.c_double,
+                                                     C.c_int, _IP, C.c_int, _P]),
+    "world_b200_synthesis_coded_batch_options": (C.c_int, [_P, _P, _IP, C.c_int, C.c_int, _P, C.c_int, _P, _IP,
+                                                           C.c_double, C.c_int, _IP, C.c_int, _P, _P, C.c_int, _P]),
+    "world_b200_synthesis_coded_host_options": (C.c_int, [_P, _P, _IP, C.c_int, C.c_int, _P, C.c_int, _P, _IP,
+                                                          C.c_double, C.c_int, _IP, C.c_int, _P, _P, C.c_int, _P]),
+    "world_b200_modify_batch_options": (C.c_int, [_P, _P, _IP, C.c_int, C.c_int, _P, C.c_int, _IP, C.c_int, _P, _P]),
     "world_b200_default_analysis_option": (None, [C.c_int, C.c_int, C.POINTER(AnalysisOption)]),
     "world_b200_analyze_host": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(AnalysisOption),
                                           _P, _P, C.c_int, _P, _P]),
@@ -194,6 +201,16 @@ ABI = {
     "world_b200_transform_host": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(AnalysisOption),
                                             C.POINTER(HarvestOption), C.POINTER(DioOption), _P, _P, _P, C.c_int, _P,
                                             C.c_int, _IP]),
+    "world_b200_transform_batch_spectral_options": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int,
+                                                              C.POINTER(AnalysisOption), C.POINTER(HarvestOption),
+                                                              C.POINTER(DioOption), C.POINTER(CheapTrickOption),
+                                                              C.POINTER(D4COption), _P, _P, _P, C.c_int, _P, C.c_int,
+                                                              _IP]),
+    "world_b200_transform_host_spectral_options": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int,
+                                                             C.POINTER(AnalysisOption), C.POINTER(HarvestOption),
+                                                             C.POINTER(DioOption), C.POINTER(CheapTrickOption),
+                                                             C.POINTER(D4COption), _P, _P, _P, C.c_int, _P, C.c_int,
+                                                             _IP]),
     # host-only file glue (tools/audioio.h, tools/parameterio.h)
     "wavwrite": (None, [_P, C.c_int, C.c_int, C.c_int, C.c_char_p]),
     "GetAudioLength": (C.c_int, [C.c_char_p]),
@@ -335,6 +352,16 @@ def _int_array(v, n):
         return None, None
     arr = (C.c_int * n)(*[int(t) for t in v])
     return arr, arr
+
+
+def _fft_sizes(fft_size, n):
+    """A sequence of n sizes (one per utterance) as a ctypes int array; None for a single size."""
+    if not isinstance(fft_size, (list, tuple)) and getattr(fft_size, "ndim", 0) == 0:
+        return None
+    sizes = fft_size.tolist() if hasattr(fft_size, "tolist") else list(fft_size)
+    if len(sizes) != n:
+        raise ValueError(f"{len(sizes)} fft sizes for {n} utterances")
+    return (C.c_int * max(n, 1))(*[int(v) for v in sizes])
 
 
 class World:
@@ -615,12 +642,21 @@ class World:
 
     def synthesis(self, f0, spectrogram, aperiodicity, fft_size, frame_period, fs, y_length, f0_lengths=None,
                   y_lengths=None):
-        """Batched Synthesis(): f0 [n, L], spectrogram / aperiodicity [n, L, bins] -> y [n, y_length]."""
+        """Batched Synthesis(): f0 [n, L], spectrogram / aperiodicity [n, L, bins] -> y [n, y_length].  fft_size may
+        be a sequence of one size per utterance (world_b200_synthesis_batch_options): the rows are then
+        [n, L, row_stride], as cheaptrick / d4c with per-utterance options write them, and utterance u reads the first
+        fft_size[u] / 2 + 1 values of each."""
         n = f0.shape[0]
         y = self._zeros(f0, (n, y_length))
         fl, k1 = _int_array(f0_lengths, n)
         yl, k2 = _int_array(y_lengths, n)
+        sizes = _fft_sizes(fft_size, n)
         self._use_current_stream()
+        if sizes is not None:
+            self._check(self.lib.world_b200_synthesis_batch_options(
+                self._h, _ptr(f0), fl, n, f0.shape[1], _ptr(spectrogram), _ptr(aperiodicity),
+                int(spectrogram.shape[-1]), sizes, frame_period, fs, yl, y_length, _ptr(y)))
+            return y
         self._check(self.lib.world_b200_synthesis_batch(self._h, _ptr(f0), fl, n, f0.shape[1], _ptr(spectrogram),
                                                         _ptr(aperiodicity), fft_size, frame_period, fs, yl, y_length,
                                                         _ptr(y)))
@@ -635,7 +671,9 @@ class World:
         int16 for its 16-bit PCM, quantised as wavwrite does by the overlap-add kernel itself.
         f0_scale / spectral_ratio (one factor, or one per utterance): synthesise the voice changed as modify() changes
         it, without touching the inputs (world_b200_synthesis_coded_batch_modified); the output equals decode +
-        modify + synthesis bit for bit."""
+        modify + synthesis bit for bit.
+        fft_size may be a sequence of one size per utterance (world_b200_synthesis_coded_batch_options): each utterance
+        is decoded and synthesised at its own size."""
         pcm16 = _pcm16(dtype)
         n = f0.shape[0]
         if pcm16 and self.xp == "torch":
@@ -647,23 +685,35 @@ class World:
             y = self._zeros(f0, (n, y_length))
         fl, k1 = _int_array(f0_lengths, n)
         yl, k2 = _int_array(y_lengths, n)
+        sizes = _fft_sizes(fft_size, n)
         self._use_current_stream()
-        self._check(self.lib.world_b200_synthesis_coded_batch_modified(
+        entry = (self.lib.world_b200_synthesis_coded_batch_modified if sizes is None
+                 else self.lib.world_b200_synthesis_coded_batch_options)
+        self._check(entry(
             self._h, _ptr(f0), fl, n, f0.shape[1], _ptr(coded_spectral_envelope),
-            int(coded_spectral_envelope.shape[-1]), _ptr(coded_aperiodicity), fft_size, frame_period, fs, yl,
-            y_length, _factors(f0_scale, n, "f0_scale"), _factors(spectral_ratio, n, "spectral_ratio"),
-            16 if pcm16 else 0, _ptr(y)))
+            int(coded_spectral_envelope.shape[-1]), _ptr(coded_aperiodicity), fft_size if sizes is None else sizes,
+            frame_period, fs, yl, y_length, _factors(f0_scale, n, "f0_scale"),
+            _factors(spectral_ratio, n, "spectral_ratio"), 16 if pcm16 else 0, _ptr(y)))
         return y
 
     def modify(self, f0, spectrogram, fs, fft_size, f0_scale=None, spectral_ratio=None, f0_lengths=None):
         """F0 scaling and formant shift in place (world_b200_modify_batch, the reference demo's ParameterModification):
         f0 [n, L] *= f0_scale, and each envelope row [n, L, fft_size/2+1] is stretched along frequency by
         spectral_ratio.  Either factor may be one number for every utterance, a sequence of one per utterance, or None
-        to leave that array alone (it may then be None too).  Returns (f0, spectrogram)."""
+        to leave that array alone (it may then be None too).  fft_size may be a sequence of one size per utterance
+        (world_b200_modify_batch_options): the rows are then [n, L, row_stride] and utterance u's envelope is the first
+        fft_size[u] / 2 + 1 values of each.  Returns (f0, spectrogram)."""
         rows = f0 if f0 is not None else spectrogram
         n, L = int(rows.shape[0]), int(rows.shape[1])
         fl, k1 = _int_array(f0_lengths, n)
+        sizes = _fft_sizes(fft_size, n)
         self._use_current_stream()
+        if sizes is not None:
+            row = int(spectrogram.shape[-1]) if spectrogram is not None else 0
+            self._check(self.lib.world_b200_modify_batch_options(
+                self._h, _ptr(f0), fl, n, L, _ptr(spectrogram), row, sizes, fs, _factors(f0_scale, n, "f0_scale"),
+                _factors(spectral_ratio, n, "spectral_ratio")))
+            return f0, spectrogram
         self._check(self.lib.world_b200_modify_batch(self._h, _ptr(f0), fl, n, L, _ptr(spectrogram), fft_size, fs,
                                                      _factors(f0_scale, n, "f0_scale"),
                                                      _factors(spectral_ratio, n, "spectral_ratio")))
@@ -676,7 +726,8 @@ class World:
         int16 for nbit 16 or float64 for nbit 0, whole rows (samples beyond an utterance's y_length are 0).  out: a
         host array of that shape and dtype to write into (a pinned one lets the downloads overlap the kernels).
         coded_ap may be None below 12 kHz (no bands).  f0_scale / spectral_ratio as in synthesis_coded
-        (world_b200_synthesis_coded_host_modified)."""
+        (world_b200_synthesis_coded_host_modified).  fft_size may be a sequence of one size per utterance
+        (world_b200_synthesis_coded_host_options)."""
         import numpy as np
 
         def host(a):
@@ -696,9 +747,12 @@ class World:
             raise ValueError(f"out: a contiguous [{n}, {y_length}] {'int16' if nbit == 16 else 'float64'} host array")
         fl, k1 = _int_array(f0_lengths, n)
         yl, k2 = _int_array(y_lengths, n)
-        self._check(self.lib.world_b200_synthesis_coded_host_modified(
+        sizes = _fft_sizes(fft_size, n)
+        entry = (self.lib.world_b200_synthesis_coded_host_modified if sizes is None
+                 else self.lib.world_b200_synthesis_coded_host_options)
+        self._check(entry(
             self._h, _ptr(f0), fl, n, f0.shape[1], _ptr(coded_sp), int(coded_sp.shape[-1]), _ptr(coded_ap),
-            fft_size, frame_period, fs, yl, y_length, _factors(f0_scale, n, "f0_scale"),
+            fft_size if sizes is None else sizes, frame_period, fs, yl, y_length, _factors(f0_scale, n, "f0_scale"),
             _factors(spectral_ratio, n, "spectral_ratio"), nbit, _ptr(y)))
         return y
 
@@ -923,7 +977,9 @@ class World:
         return int(self.lib.world_b200_transform_samples(fs, x_length, frame_period, time_scale))
 
     def _transform_args(self, x, nbit, fs, option, f0_scale, spectral_ratio, time_scale, x_lengths, harvest_options,
-                        dio_options, dtype):
+                        dio_options, dtype, cheaptrick_options=None, d4c_options=None):
+        """(n, y_stride, nbit_out, args, suffix): args run from nbit to nbit_out; suffix "_spectral_options" when
+        cheaptrick_options or d4c_options is given (their arrays then follow the F0 option arrays)."""
         n, stride, frame_period = self._coded_rows(x, nbit, option)
         lens = [stride] * n if x_lengths is None else [int(v) for v in x_lengths]
         ts = _factors(time_scale, n, "time_scale")
@@ -933,21 +989,29 @@ class World:
         per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
         nbit_out = 16 if _pcm16(dtype) else 0
         y_stride = max(y_lens + [1])
-        args = [nbit, n, stride, xl, fs, C.byref(option), per_utt, per_dio, _factors(f0_scale, n, "f0_scale"),
-                _factors(spectral_ratio, n, "spectral_ratio"), ts, nbit_out]
-        return n, y_stride, nbit_out, args
+        spectral = []
+        if cheaptrick_options is not None or d4c_options is not None:
+            spectral = [None if cheaptrick_options is None else _option_array(CheapTrickOption, cheaptrick_options, n),
+                        None if d4c_options is None else _option_array(D4COption, d4c_options, n)]
+        args = [nbit, n, stride, xl, fs, C.byref(option), per_utt, per_dio, *spectral,
+                _factors(f0_scale, n, "f0_scale"), _factors(spectral_ratio, n, "spectral_ratio"), ts, nbit_out]
+        return n, y_stride, nbit_out, args, "_spectral_options" if spectral else ""
 
     def transform(self, x, nbit, fs, option: AnalysisOption, f0_scale=None, spectral_ratio=None, time_scale=None,
-                  x_lengths=None, harvest_options=None, dio_options=None, dtype=None):
+                  x_lengths=None, harvest_options=None, dio_options=None, dtype=None, cheaptrick_options=None,
+                  d4c_options=None):
         """The reference demo's loop on DEVICE arrays in one call (world_b200_transform_batch): analysis with option's F0
         method, CheapTrick and D4C, f0 scaled by f0_scale and the envelope stretched by spectral_ratio (as modify()),
         and Synthesis with the frame period scaled by time_scale (above 1: slower).  Each factor may be None, one number,
         or one value per utterance.  x as for analyze_coded_batch (float64 rows for nbit 0, else PCM rows).  Returns
         (y, y_lengths): y [n, max y_length] float64, or int16 for dtype int16 (wavwrite's quantisation), on x's device,
         with samples past an utterance's length left 0; y_lengths from transform_samples.  Every row equals
-        analyze_batch -> modify -> synthesis of the same utterance bit for bit."""
-        n, y_stride, nbit_out, args = self._transform_args(x, nbit, fs, option, f0_scale, spectral_ratio, time_scale,
-                                                           x_lengths, harvest_options, dio_options, dtype)
+        analyze_batch -> modify -> synthesis of the same utterance bit for bit.  cheaptrick_options / d4c_options: a
+        list of one option per utterance (world_b200_transform_batch_spectral_options): utterance u is analysed,
+        modified and synthesised at cheaptrick_options[u].fft_size."""
+        n, y_stride, nbit_out, args, suffix = self._transform_args(x, nbit, fs, option, f0_scale, spectral_ratio,
+                                                                   time_scale, x_lengths, harvest_options, dio_options,
+                                                                   dtype, cheaptrick_options, d4c_options)
         if self.xp == "torch":
             y = self.torch.zeros((n, y_stride), dtype=self.torch.int16 if nbit_out else self.torch.float64,
                                  device=x.device)
@@ -956,18 +1020,21 @@ class World:
             y = np.zeros((n, y_stride), dtype=np.int16 if nbit_out else np.float64)
         yl = (C.c_int * max(n, 1))()
         self._use_current_stream()
-        self._check(self.lib.world_b200_transform_batch(self._h, _ptr(x), *args, _ptr(y), y_stride, yl))
+        self._check(getattr(self.lib, f"world_b200_transform_batch{suffix}")(self._h, _ptr(x), *args, _ptr(y),
+                                                                              y_stride, yl))
         return y, list(yl)[:n]
 
     def transform_host(self, x, nbit, fs, option: AnalysisOption, f0_scale=None, spectral_ratio=None, time_scale=None,
-                       x_lengths=None, harvest_options=None, dio_options=None, dtype=None, out=None):
+                       x_lengths=None, harvest_options=None, dio_options=None, dtype=None, out=None,
+                       cheaptrick_options=None, d4c_options=None):
         """transform() for HOST arrays (numpy or CPU tensors; world_b200_transform_host): PCM chunks are uploaded,
         transformed and downloaded pipelined, so only PCM crosses PCIe.  Returns (y, y_lengths) with y a host array of
         whole rows (0 past each length).  out: a contiguous [n, max y_length] host array of the output dtype to write
-        into (a pinned one lets the copies overlap the kernels)."""
+        into (a pinned one lets the copies overlap the kernels).  cheaptrick_options / d4c_options as in transform()."""
         import numpy as np
-        n, y_stride, nbit_out, args = self._transform_args(x, nbit, fs, option, f0_scale, spectral_ratio, time_scale,
-                                                           x_lengths, harvest_options, dio_options, dtype)
+        n, y_stride, nbit_out, args, suffix = self._transform_args(x, nbit, fs, option, f0_scale, spectral_ratio,
+                                                                   time_scale, x_lengths, harvest_options, dio_options,
+                                                                   dtype, cheaptrick_options, d4c_options)
         want = np.int16 if nbit_out else np.float64
         if out is None:
             out = np.zeros((n, y_stride), dtype=want)
@@ -978,7 +1045,8 @@ class World:
         if not xh.flags.c_contiguous:
             raise ValueError("x: a contiguous host array")
         yl = (C.c_int * max(n, 1))()
-        self._check(self.lib.world_b200_transform_host(self._h, _ptr(xh), *args, _ptr(y), y_stride, yl))
+        self._check(getattr(self.lib, f"world_b200_transform_host{suffix}")(self._h, _ptr(xh), *args, _ptr(y),
+                                                                             y_stride, yl))
         return out, list(yl)[:n]
 
     def analyze_coded_batch_allgather(self, x, nbit, fs, option: AnalysisOption, number_of_dimensions, time_axis_full,

@@ -655,6 +655,8 @@ static int chain_checks(Ctx *c, const ChainRequest &r, ChainPlan *p) {
     if (r.d4c_options) std::copy(r.d4c_options, r.d4c_options + n, d4s.begin());
     for (const CheapTrickOption &o : cts) d4_fft.push_back(o.fft_size);
     s.per_utt = true; s.ct = cts.data(); s.fft_size = d4_fft.data(); s.d4c = d4s.data();
+    // full rows (a transform's): every utterance's row as wide as the largest size's
+    for (const int f : d4_fft) s.row_stride = r.coded ? 0 : imax(s.row_stride, f / 2 + 1);
   }
   if ((r.spectrogram || transform) && (rc = stage_plan(c, s, &p->ct))) return rc;
   s.stage = STAGE_D4C;
@@ -662,8 +664,9 @@ static int chain_checks(Ctx *c, const ChainRequest &r, ChainPlan *p) {
   s.stage = STAGE_STONEMASK;
   StagePlan stonemask;
   if (!harvest && (rc = stage_plan(c, s, &stonemask))) return rc;
-  p->sp_row = r.coded ? (size_t)r.dims : (size_t)(fft_size / 2 + 1);
-  p->ap_row = r.coded ? (size_t)GetNumberOfAperiodicities(r.fs) : (size_t)(fft_size / 2 + 1);
+  const size_t full_row = spectral_options ? (size_t)s.row_stride : (size_t)(fft_size / 2 + 1);
+  p->sp_row = r.coded ? (size_t)r.dims : full_row;
+  p->ap_row = r.coded ? (size_t)GetNumberOfAperiodicities(r.fs) : full_row;
   p->want_sp = r.spectrogram != nullptr;
   p->want_ap = r.aperiodicity != nullptr && !p->d4.nothing;   // no bands below 12 kHz: D4C is skipped
   return 0;
@@ -1048,6 +1051,9 @@ int transform_check(WorldB200 *h, const ChainRequest &r, const double *f0_scale,
   SynthesisRequest s{nullptr, p.f_len.data(), r.n, p.f0_stride, nullptr, nullptr, r.opt->cheaptrick.fft_size,
                      p.frame_period, r.fs, y_len.data(), y_stride, y, nbit_out};
   s.f0_scale = f0_scale; s.spectral_ratio = spectral_ratio; s.transform = true; s.fp = fp.data();
+  if (r.cheaptrick_options || r.d4c_options) {   // each utterance synthesised at its CheapTrick size
+    s.per_utt = true; s.fft_sizes = p.ct.fft_size.data(); s.row_stride = (int)p.sp_row;
+  }
   return synthesis_plan(c, s, who, &tp->syn);
 }
 
@@ -1063,7 +1069,7 @@ int transform_check(WorldB200 *h, const ChainRequest &r, const double *f0_scale,
 int transform_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, const void *x, int u0, int n, void *y) {
   if (n <= 0) return 0;
   const ChainPlan &p = tp.chain;
-  const int f0_stride = p.f0_stride, x_stride = r.x_stride, fft_size = r.opt->cheaptrick.fft_size, nbit = r.nbit;
+  const int f0_stride = p.f0_stride, x_stride = r.x_stride, nbit = r.nbit, row = (int)p.sp_row;
   const size_t in_row = (size_t)x_stride * (nbit ? nbit / 8 : 8);
   const size_t out_row = (size_t)tp.syn.y_stride * (tp.syn.nbit ? 2 : 8);
   struct Rows {
@@ -1076,7 +1082,7 @@ int transform_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, 
       total = a.total;
     }
   };
-  auto rows_of = [&](int m) { return Rows(m, nbit, x_stride, f0_stride, fft_size / 2 + 1); };
+  auto rows_of = [&](int m) { return Rows(m, nbit, x_stride, f0_stride, row); };
   int n_slices = 1;
   {
 #ifndef WB_EMU
@@ -1113,7 +1119,7 @@ int transform_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, 
     if (!e) e = dev_memset(&L->c, f, 0, (size_t)m * f0_stride * 8);
     if (!e) e = chain_f0(L, r, p, g, m, xs, t, f);
     if (!e) e = chain_spectral(L, r, p, g, m, xs, t, f, sp, ap);
-    if (!e && tp.syn.modify) e = modify_run(&L->c, tp.syn.mod, g, m, p.f_len.data() + g, f0_stride, f, sp);
+    if (!e && tp.syn.modify) e = modify_run(&L->c, tp.syn.mod, g, m, p.f_len.data() + g, f0_stride, row, f, sp);
     if (e && L != h) h->c.last_error = L->c.last_error;
     return e;
   };
@@ -1147,10 +1153,23 @@ int world_b200_transform_batch(WorldB200 *h, const void *x, int nbit, int n_utts
                                int fs, const WorldB200AnalysisOption *option, const HarvestOption *harvest_options,
                                const DioOption *dio_options, const double *f0_scale, const double *spectral_ratio,
                                const double *time_scale, int nbit_out, void *y, int y_stride, int *y_lengths) {
+  return world_b200_transform_batch_spectral_options(h, x, nbit, n_utts, x_stride, x_lengths, fs, option,
+                                                     harvest_options, dio_options, nullptr, nullptr, f0_scale,
+                                                     spectral_ratio, time_scale, nbit_out, y, y_stride, y_lengths);
+}
+
+int world_b200_transform_batch_spectral_options(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride,
+                                                const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                                const HarvestOption *harvest_options, const DioOption *dio_options,
+                                                const CheapTrickOption *cheaptrick_options,
+                                                const D4COption *d4c_options, const double *f0_scale,
+                                                const double *spectral_ratio, const double *time_scale, int nbit_out,
+                                                void *y, int y_stride, int *y_lengths) {
   if (!h) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
   ChainRequest r(x, nbit, n_utts, x_stride, x_lengths, fs, option, nullptr, nullptr, 0, nullptr, nullptr);
   r.harvest_options = harvest_options; r.dio_options = dio_options;
+  r.cheaptrick_options = cheaptrick_options; r.d4c_options = d4c_options;
   TransformPlan tp;
   const int rc = transform_check(h, r, f0_scale, spectral_ratio, time_scale, nbit_out, y, y_stride, "transform_batch", &tp);
   if (rc) return rc;

@@ -82,10 +82,11 @@ int chain_f0(WorldB200 *h, const ChainRequest &r, const ChainPlan &p, int u0, in
 int chain_spectral(WorldB200 *h, const ChainRequest &r, const ChainPlan &p, int u0, int m, const double *x,
                    const double *time_axis, const double *f0, double *sp, double *ap);
 
-// Voice transformation (world_b200_transform_*): the analysis plan of the request (full rows, no spectral options, no
-// analysis outputs) and the synthesis plan of its analysis rows: lengths, the factors (which modify_run applies right
-// after the analysis) and each utterance's frame period, (frame_period * time_scale[u]) / 1000.0 s.  transform_check
-// makes it once per call; transform_run (device rows) and the host pipeline (wb_host.cu) read it.
+// Voice transformation (world_b200_transform_*): the analysis plan of the request (full rows, no analysis outputs;
+// with spectral options each row as wide as the largest size's) and the synthesis plan of its analysis rows: lengths,
+// each utterance's CheapTrick size, the factors (which modify_run applies right after the analysis) and each
+// utterance's frame period, (frame_period * time_scale[u]) / 1000.0 s.  transform_check makes it once per call;
+// transform_run (device rows) and the host pipeline (wb_host.cu) read it.
 struct TransformPlan {
   ChainPlan chain;
   SynthesisPlan syn;

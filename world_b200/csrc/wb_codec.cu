@@ -43,6 +43,8 @@ struct CodecParams {
   const double2 *weight;      // DCT / IDCT weights
   double norm;                // sqrt(fft_size / 2)
   const double2 *tw;
+  const int *list;            // decode: the utterance of each blockIdx.y, or NULL: blockIdx.y itself
+  int row;                    // decode: doubles per output frame row (>= bins)
 };
 
 WB_KERNEL(128, 8) code_sp_kernel(CodecParams p) {
@@ -73,7 +75,7 @@ WB_KERNEL(128, 8) code_sp_kernel(CodecParams p) {
 
 WB_KERNEL(128, 8) decode_sp_kernel(CodecParams p) {
   WB_DYN_SMEM(double, smem);
-  const int tid = WB_TID, nth = WB_NTH, u = blockIdx.y, f = blockIdx.x;
+  const int tid = WB_TID, nth = WB_NTH, u = p.list ? p.list[blockIdx.y] : blockIdx.y, f = blockIdx.x;
   if (f >= p.f_len[u]) return;
   const int M = p.max_dim;
   double2 *z = reinterpret_cast<double2 *>(smem);  // M complex
@@ -96,7 +98,7 @@ WB_KERNEL(128, 8) decode_sp_kernel(CodecParams p) {
   WB_SYNC();
   if (tid == 0) { mel[0] = mel[1]; mel[M + 1] = mel[M]; }
   WB_SYNC();
-  double *out = p.out + ((size_t)u * p.f_stride + f) * p.bins;
+  double *out = p.out + ((size_t)u * p.f_stride + f) * p.row;
   for (int j = tid; j < p.bins; j += nth) {                                         // :150-154
     const int k = __ldg(p.idx + j);
     const double v = mel[k] + __ldg(p.frac + j) * (mel[k + 1] - mel[k]);
@@ -117,12 +119,13 @@ WB_KERNEL_PLAIN code_ap_kernel(CodecParams p) {
   }
 }
 
-WB_KERNEL_PLAIN decode_ap_kernel(CodecParams p) {
-  const int u = blockIdx.y, f = blockIdx.x;
+// 128 threads (launch_frames); 16 CTAs per SM is full occupancy, at most 32 registers
+WB_KERNEL(128, 16) decode_ap_kernel(CodecParams p) {
+  const int u = p.list ? p.list[blockIdx.y] : blockIdx.y, f = blockIdx.x;
   if (f >= p.f_len[u]) return;
   const int n_ap = p.dims;
   const double *c = p.in + ((size_t)u * p.f_stride + f) * n_ap;
-  double *out = p.out + ((size_t)u * p.f_stride + f) * p.bins;
+  double *out = p.out + ((size_t)u * p.f_stride + f) * p.row;
   double mean = 0.0;
   for (int b = 0; b < n_ap; ++b) mean += c[b];                                      // CheckVUV :32-40
   mean /= n_ap;
@@ -241,7 +244,7 @@ CodecParams decode_params(int which, const Tables &t, int fft_size, int f_stride
   CodecParams p;
   memset(&p, 0, sizeof(p));
   const int M = fft_size / 2;
-  p.f_stride = f_stride; p.in = in; p.out = out; p.bins = M + 1; p.dims = t.dims;
+  p.f_stride = f_stride; p.in = in; p.out = out; p.bins = M + 1; p.row = M + 1; p.dims = t.dims;
   if (which == 1) { p.max_dim = M; p.lg = t.lg_half; p.norm = t.norm; }
   return p;
 }
@@ -298,12 +301,14 @@ void codec_decode_ap_tables(int fs, int fft_size, CodecTables *t) {
 
 void codec_decode_launch(Ctx *ctx, bool spectral_envelope, const CodecTables &t, const CodecDeviceTables &d,
                          int fft_size, const int *f_len, int n_utts, int f_stride, int max_f, const double *in,
-                         double *out) {
+                         double *out, const int *list, int out_row) {
   if (n_utts == 0 || max_f == 0) return;
   const int which = spectral_envelope ? 1 : 3;
   CodecParams p = decode_params(which, t, fft_size, f_stride, in, out);
   p.idx = d.idx; p.frac = d.frac; p.weight = d.weight;
-  launch_frames(ctx, which, p, f_len, n_utts, max_f, t.dims, fft_size / 2 + 1, decode_smem(which, fft_size));
+  if (out_row) p.row = out_row;
+  p.list = list;   // a list (at most one pass of utterances, < 65536) is one launch over the whole rows
+  launch_frames(ctx, which, p, f_len, n_utts, max_f, t.dims, p.row, decode_smem(which, fft_size));
 }
 
 // GetParametersForCoding (codec.cpp:161-181) + the DCT weights of DCTForCodec (:73-89)

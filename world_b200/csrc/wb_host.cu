@@ -392,7 +392,7 @@ int chunk_pipeline(WorldB200 *h, const char *who, int n_utts, int chunk, int rin
 // input sets and the output ring stay within a third of the scratch budget.  `host`: the call's host rows.
 int synthesis_pipeline(WorldB200 *h, const SynthesisPlan &plan, const SynthesisRows &host) {
   Ctx *ctx = &h->c;
-  const int n_utts = plan.n, f0_stride = plan.f0_stride, dims = plan.tsp.dims, n_ap = plan.tap.dims;
+  const int n_utts = plan.n, f0_stride = plan.f0_stride, dims = plan.dims, n_ap = plan.n_ap;
   const size_t out_bytes = plan.nbit ? 2 : 8;
   const size_t per_in = (size_t)f0_stride * (1 + dims + n_ap) * 8, per_out = (size_t)plan.y_stride * out_bytes;
   int max_y = 0;
@@ -447,16 +447,18 @@ int transform_pipeline(WorldB200 *h, const ChainRequest &r, const TransformPlan 
 
 // world_b200_synthesis_coded_host and, with f0_scale / spectral_ratio, world_b200_synthesis_coded_host_modified: every
 // check runs before the first chunk is queued
+// (fft_sizes NULL: fft_size for every utterance; world_b200_synthesis_coded_host_options passes per_utt)
 int synthesis_coded_host(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts, int f0_stride,
                          const double *coded_spectral_envelope, int number_of_dimensions,
                          const double *coded_aperiodicity, int fft_size, double frame_period, int fs,
                          const int *y_lengths, int y_stride, int nbit, void *y, const double *f0_scale,
-                         const double *spectral_ratio) {
+                         const double *spectral_ratio, bool per_utt = false, const int *fft_sizes = nullptr) {
   if (!h) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
   SynthesisRequest r{f0, f0_lengths, n_utts, f0_stride, coded_spectral_envelope, coded_aperiodicity, fft_size,
                      frame_period, fs, y_lengths, y_stride, y, nbit};
   r.coded = true; r.dims = number_of_dimensions; r.f0_scale = f0_scale; r.spectral_ratio = spectral_ratio;
+  r.per_utt = per_utt; r.fft_sizes = fft_sizes;
   SynthesisPlan plan;
   const int rc = synthesis_plan(&h->c, r, "Synthesis", &plan);
   if (rc || n_utts == 0) return rc;
@@ -487,22 +489,45 @@ extern "C" int world_b200_synthesis_coded_host_modified(WorldB200 *h, const doub
                               spectral_ratio);
 }
 
-extern "C" int world_b200_transform_host(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride,
-                                         const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
-                                         const HarvestOption *harvest_options, const DioOption *dio_options,
-                                         const double *f0_scale, const double *spectral_ratio,
-                                         const double *time_scale, int nbit_out, void *y, int y_stride,
-                                         int *y_lengths) {
+extern "C" int world_b200_synthesis_coded_host_options(WorldB200 *h, const double *f0, const int *f0_lengths,
+                                                       int n_utts, int f0_stride,
+                                                       const double *coded_spectral_envelope,
+                                                       int number_of_dimensions, const double *coded_aperiodicity,
+                                                       const int *fft_sizes, double frame_period, int fs,
+                                                       const int *y_lengths, int y_stride, const double *f0_scale,
+                                                       const double *spectral_ratio, int nbit, void *y) {
+  return synthesis_coded_host(h, f0, f0_lengths, n_utts, f0_stride, coded_spectral_envelope, number_of_dimensions,
+                              coded_aperiodicity, 0, frame_period, fs, y_lengths, y_stride, nbit, y, f0_scale,
+                              spectral_ratio, true, fft_sizes);
+}
+
+extern "C" int world_b200_transform_host_spectral_options(
+    WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride, const int *x_lengths, int fs,
+    const WorldB200AnalysisOption *option, const HarvestOption *harvest_options, const DioOption *dio_options,
+    const CheapTrickOption *cheaptrick_options, const D4COption *d4c_options, const double *f0_scale,
+    const double *spectral_ratio, const double *time_scale, int nbit_out, void *y, int y_stride, int *y_lengths) {
   if (!h) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
   ChainRequest r(x, nbit, n_utts, x_stride, x_lengths, fs, option, nullptr, nullptr, 0, nullptr, nullptr);
   r.harvest_options = harvest_options; r.dio_options = dio_options;
+  r.cheaptrick_options = cheaptrick_options; r.d4c_options = d4c_options;
   TransformPlan tp;
   const int rc = transform_check(h, r, f0_scale, spectral_ratio, time_scale, nbit_out, y, y_stride, "transform_host", &tp);
   if (rc) return rc;
   if (y_lengths) std::copy(tp.syn.y_len.begin(), tp.syn.y_len.end(), y_lengths);
   if (n_utts == 0) return 0;
   return transform_pipeline(h, r, tp, y);
+}
+
+extern "C" int world_b200_transform_host(WorldB200 *h, const void *x, int nbit, int n_utts, int x_stride,
+                                         const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                         const HarvestOption *harvest_options, const DioOption *dio_options,
+                                         const double *f0_scale, const double *spectral_ratio,
+                                         const double *time_scale, int nbit_out, void *y, int y_stride,
+                                         int *y_lengths) {
+  return world_b200_transform_host_spectral_options(h, x, nbit, n_utts, x_stride, x_lengths, fs, option,
+                                                    harvest_options, dio_options, nullptr, nullptr, f0_scale,
+                                                    spectral_ratio, time_scale, nbit_out, y, y_stride, y_lengths);
 }
 
 extern "C" int world_b200_analyze_host(WorldB200 *h, const double *x, int n_utts, int x_stride,

@@ -160,39 +160,46 @@ int codec_ap_tables(Ctx *ctx, int fs, int fft_size, CodecTables *t);   // t->dim
 // tables, lengths (f_len, n_utts entries, largest max_f) and rows already on the device.
 int codec_decode_sp_tables(Ctx *ctx, int fs, int fft_size, int number_of_dimensions, CodecTables *t);
 void codec_decode_ap_tables(int fs, int fft_size, CodecTables *t);    // t->dims = GetNumberOfAperiodicities(fs)
+// list: the n_utts utterances to decode are list[0 .. n_utts) of the rows (NULL: 0 .. n_utts); out_row: doubles per
+// decoded frame row (>= fft_size / 2 + 1).
 struct CodecDeviceTables { const int *idx; const double *frac; const double2 *weight; };
 void codec_decode_launch(Ctx *ctx, bool spectral_envelope, const CodecTables &t, const CodecDeviceTables &d,
                          int fft_size, const int *f_len, int n_utts, int f_stride, int max_f, const double *in,
-                         double *out);
+                         double *out, const int *list = nullptr, int out_row = 0);
 // wb_synthesis.cu: F0 scaling and spectral stretch (the reference demo's ParameterModification, test.cpp:221-258).
 // The interp1 segment and weight of each output bin depend only on (ratio, fft_size, fs), so they are planned on the
-// host once per distinct ratio; the tail rule (bins >= c copy bin c-1 when ratio < 1) is folded into the table.
+// host once per distinct (ratio, fft_size); the tail rule (bins >= c copy bin c-1 when ratio < 1) is folded into the
+// table.
 struct ModifyPlan {
   std::vector<double> scale;   // [n_utts] f0 factor of each utterance; empty: f0 is not scaled
   std::vector<int> table;      // [n_utts] stretch table of each utterance; empty: the envelope is not stretched
-  std::vector<int> idx;        // [n_tables][bins] a = k - 1 of interp1's segment (the kernel reads L[a], L[a + 1])
-  std::vector<double> frac;    // [n_tables][bins] s = (xi - x[a]) / (x[a + 1] - x[a])
-  int n_tables = 0, bins = 0;
+  std::vector<int> idx;        // [sum of tbins] a = k - 1 of interp1's segment (the kernel reads L[a], L[a + 1])
+  std::vector<double> frac;    // [sum of tbins] s = (xi - x[a]) / (x[a + 1] - x[a])
+  std::vector<int> tbins, toff;   // [n_tables] bins of each table (its fft_size / 2 + 1) and its first entry
+  int n_tables = 0, bins = 0;     // bins: the largest table's
   size_t device_bytes(int n) const;   // arena bytes of one pass of n utterances: tables, factors, table indices
 };
 // Checks every factor (finite, > 0; a ratio below 1 must keep c = (int)(fft_size / 2.0 * ratio) >= 1) and builds the
-// plan; EINVAL with last_error "<who>: ..." naming the first bad utterance.  Either array may be null.
+// plan; EINVAL with last_error "<who>: ..." naming the first bad utterance.  Either array may be null.  fft_sizes:
+// utterance u's size (checked by the caller), or NULL: fft_size (checked here) for every utterance.
 int modify_plan(Ctx *ctx, const char *who, int n_utts, int fft_size, int fs, const double *f0_scale,
-                const double *spectral_ratio, ModifyPlan *plan);
+                const double *spectral_ratio, ModifyPlan *plan, const int *fft_sizes = nullptr);
 // Plan entries [u0, u0 + n) in device memory (layout of device_bytes); the copies are enqueued on ctx->stream.
-struct ModifyDevice { const double *scale; const int *table; const int *idx; const double *frac; };
+struct ModifyDevice { const double *scale; const int *table; const int *idx; const double *frac; const int *tbins, *toff; };
 int modify_upload(Ctx *ctx, const ModifyPlan &plan, int u0, int n, unsigned char *blk, ModifyDevice *d);
 // f0_out[u][i] = f0_in[u][i] * scale[u] for i < f_len[u] (f0_out may alias f0_in)
 void modify_f0_launch(Ctx *ctx, const ModifyDevice &d, const int *f_len, int n_utts, int f_stride, int max_f,
                       const double *f0_in, double *f0_out);
-// the envelope rows [n][f_stride][bins] stretched in place, frames < f_len[u]
-void modify_stretch_launch(Ctx *ctx, const ModifyDevice &d, int bins, const int *f_len, int n_utts, int f_stride,
-                           int max_f, double *spectrogram);
+// the envelope rows [n][f_stride][row] stretched in place, frames < f_len[u], the first bins of the utterance's table
+// of each row (max_bins: the plan's largest)
+void modify_stretch_launch(Ctx *ctx, const ModifyDevice &d, int row, int max_bins, const int *f_len, int n_utts,
+                           int f_stride, int max_f, double *spectrogram);
 
 // Both halves of the plan on the device rows of its utterances [u0, u0 + n_utts) in place (f0 [n][f0_stride],
-// spectrogram [n][f0_stride][plan.bins]; host lengths), frames < f0_lengths[u]: world_b200_modify_batch's launches.
-int modify_run(Ctx *ctx, const ModifyPlan &plan, int u0, int n_utts, const int *f0_lengths, int f0_stride, double *f0,
-               double *spectrogram);
+// spectrogram [n][f0_stride][row], row >= plan.bins; host lengths), frames < f0_lengths[u]: world_b200_modify_batch's
+// launches.
+int modify_run(Ctx *ctx, const ModifyPlan &plan, int u0, int n_utts, const int *f0_lengths, int f0_stride, int row,
+               double *f0, double *spectrogram);
 
 // out[u] = lengths[u] (NULL: stride) for u < n; EINVAL "<who>: <rows>_lengths[u] = v is outside [least, <rows>_stride =
 // stride] (utterance u)" for the first one outside
@@ -204,6 +211,8 @@ int row_lengths(Ctx *ctx, const char *who, const char *rows, const int *lengths,
 // What a synthesis call receives: f0 [n][f0_stride], the envelope rows sp / ap (spectrogram / aperiodicity
 // [n][f0_stride][bins], or with `coded` [n][f0_stride][dims] / [GetNumberOfAperiodicities(fs)] coded rows) and y
 // [n][y_stride] (doubles for nbit 0, int16 for nbit 16).  NULL lengths: full rows.  NULL factors: no modification.
+// per_utt: utterance u is synthesised at fft_sizes[u] (fft_size is not read), and full rows hold row_stride doubles
+// per frame, of which utterance u reads fft_sizes[u] / 2 + 1.
 struct SynthesisRequest {   // brace-initialised in field order up to nbit
   const double *f0;
   const int *f0_lengths;
@@ -223,25 +232,36 @@ struct SynthesisRequest {   // brace-initialised in field order up to nbit
   // period (s)
   bool transform = false;
   const double *fp = nullptr;
+  bool per_utt = false;
+  const int *fft_sizes = nullptr;
+  int row_stride = 0;
 };
 // Everything synthesis_run reads besides the rows, made once per call and const afterwards.
+// Sizes: every per-size member has one entry per distinct fft_size of the call, in order of first appearance (one
+// entry for a one-size call).
 struct SynthesisPlan {
-  int n = 0, f0_stride = 0, y_stride = 0, fft_size = 0, lg = 0, fs = 0, nbit = 0;
+  int n = 0, f0_stride = 0, y_stride = 0, fs = 0, nbit = 0;
+  int fft_size = 0;                 // the largest fft_size of the call: responses and decoded rows are laid out by it
+  int row = 0;                      // doubles per full (or decoded) envelope frame row
   double frame_period = 0.0;        // ms
   std::vector<int> f_len, y_len;    // [n]
+  std::vector<int> size;            // [n] index of each utterance's fft_size in sizes
+  std::vector<int> sizes;           // the distinct fft_sizes
   bool coded = false;
-  CodecTables tsp, tap;             // coded: the decode tables (tap.dims == 0 below 12 kHz: no aperiodicity rows)
+  std::vector<CodecTables> tsp, tap;   // per size, coded: the decode tables (tap dims 0 below 12 kHz: no rows)
+  int dims = 0, n_ap = 0;              // coded values per envelope / aperiodicity frame
   // f0_scale or spectral_ratio given.  synthesis_run applies it to coded rows, as it decodes them; full rows are their
   // producer's to modify (transform runs modify_run on its analysis rows).
   bool modify = false;
   ModifyPlan mod;
   std::vector<double> fp;           // [n] frame period (s) of each utterance, or empty: frame_period / 1000.0 for all
-  std::vector<double> dc_remover;   // [fft_size] GetDCRemover (synthesis.cpp:319-333)
+  std::vector<std::vector<double>> dc_remover;   // per size: [fft_size] GetDCRemover (synthesis.cpp:319-333)
 };
 // Every check of a synthesis call before anything is queued, in this order: the pointers, n, fs and frame_period;
-// nbit; fft_size (a power of two in [16, 4096]); the coded decode tables; the factors (modify_plan); each utterance's
-// f0 and y lengths (2 .. stride).  EINVAL with last_error "<who>: ...", naming the first bad utterance where there is
-// one.
+// nbit; fft_size (per_utt: each utterance's, a power of two in [16, 4096]); per_utt full rows: row_stride against each
+// utterance's bins; the coded decode tables (per_utt: number_of_dimensions in [1, fft_sizes[u] / 2]); the factors
+// (modify_plan); each utterance's f0 and y lengths (2 .. stride).  EINVAL with last_error "<who>: ...", naming the
+// first bad utterance where there is one.
 int synthesis_plan(Ctx *ctx, const SynthesisRequest &r, const char *who, SynthesisPlan *p);
 // Per-utterance scratch of synthesis_run for rows whose longest y_length is max_y; fit(nominal_cap) utterances make one
 // pass when no utterance has more than 1,200 pulses per second.
@@ -249,7 +269,7 @@ struct SynthesisSizing {
   SynthesisSizing(const Ctx *ctx, const SynthesisPlan &p, int max_y);
   size_t per_utt(int cap) const;
   int fit(int cap) const;
-  int fft_size, y_stride, nominal_cap;
+  int fft_size, y_stride, nominal_cap;   // fft_size: the plan's largest, the stride of each response
   size_t decoded_per_utt, draw_stride;
   double budget;
 };

@@ -8,7 +8,8 @@
 //                         ordered compaction, randn draw offsets
 //   syn_pulse_kernel      (utterance, pulse) -> 128-thread CTA: envelope / aperiodicity interpolation,
 //                         two GetMinimumPhaseSpectrum (common.cpp:192-226), noise spectrum, two
-//                         inverse transforms, DC removal -> one response of fft_size samples
+//                         inverse transforms, DC removal -> one response of fft_size samples; one launch
+//                         per distinct fft_size of a pass, over the list of its utterances
 //   syn_overlap_kernel    output sample -> thread: sums the responses covering it in pulse order
 //                         (the reference's accumulation order, so the sum is deterministic)
 // and, ahead of it, the voice modification of the reference demo (F0 scaling and formant shift, section below):
@@ -18,6 +19,7 @@
 #include "wb_chain.h"
 #include "wb_spectral.cuh"
 #include "../../include/world/matlabfunctions.h"
+#include <algorithm>
 #include <map>
 #include <stdio.h>
 #include <type_traits>
@@ -36,6 +38,9 @@ namespace wb {
 struct SynParams {
   const double *f0; const int *f_len; int f_stride;
   const double *sp; const double *ap; int fft_size, lg_fft;
+  int row;                  // doubles per sp / ap frame row (>= each utterance's fft_size / 2 + 1)
+  const int *fft_u;         // [n] fft_size of each utterance, or null: fft_size for all
+  const int *list;          // syn_pulse_kernel: the utterance of each blockIdx.y (all of size fft_size), or null
   double frame_period;      // seconds
   const double *fp_u;       // [n] frame period of each utterance (seconds), or null: frame_period for all
   int fs;
@@ -48,7 +53,8 @@ struct SynParams {
   int *pulse_count;         // [n] pulses found, also those beyond pulse_cap (the host sizes the arrays from it)
   unsigned *draw_cnt; unsigned *draw_off; unsigned *draw_tot;
   const unsigned *draws; size_t draw_stride;
-  double *resp;             // [n][pulse_cap][fft_size]
+  double *resp;             // [n][pulse_cap][resp_n]: response i of utterance u at (u * pulse_cap + i) * resp_n
+  int resp_n;               // the largest fft_size of the call
   const double *dc_remover; // [fft_size]
   double *y;
   const double2 *tw;
@@ -61,7 +67,8 @@ WB_KERNEL(256, 2) syn_timebase_kernel(SynParams p) {
   const int tid = WB_TID, nth = WB_NTH, u = blockIdx.x;
   const int L = p.f_len[u], n = p.y_len[u], fs = p.fs;
   const double fp = p.fp_u ? p.fp_u[u] : p.frame_period;
-  const double lowest_f0 = fs / p.fft_size + 1.0;   // synthesis.cpp:362 (integer division, then + 1.0)
+  const int N = p.fft_u ? p.fft_u[u] : p.fft_size;
+  const double lowest_f0 = fs / N + 1.0;   // synthesis.cpp:362 (integer division, then + 1.0)
   const double *f0 = p.f0 + (size_t)u * p.f_stride;
   double *phase = p.phase + (size_t)u * p.y_stride;
   double *vuv = p.vuv + (size_t)u * p.y_stride;
@@ -177,7 +184,7 @@ WB_DEV void syn_c2r(const double2 *spec, double2 *z, int N, int lg, const double
 WB_KERNEL(128, 3) syn_pulse_kernel(SynParams p) {
   WB_DYN_SMEM(double, smem);
   const int tid = WB_TID, nth = WB_NTH;
-  const int u = blockIdx.y, pi = blockIdx.x;
+  const int u = p.list ? p.list[blockIdx.y] : blockIdx.y, pi = blockIdx.x;
   const int np = p.n_pulses[u];
   if (pi >= np) return;
   const int N = p.fft_size, half = N / 2, lg = p.lg_fft, fs = p.fs;
@@ -196,8 +203,8 @@ WB_KERNEL(128, 3) syn_pulse_kernel(SynParams p) {
   const double shift = p.pulse_shift[(size_t)u * p.pulse_cap + pi];
   const double current_vuv = p.vuv[(size_t)u * p.y_stride + idx];
   const double current_time = idx / static_cast<double>(fs);
-  double *resp = p.resp + ((size_t)u * p.pulse_cap + pi) * N;
-  const size_t bins = half + 1;
+  double *resp = p.resp + ((size_t)u * p.pulse_cap + pi) * p.resp_n;
+  const size_t bins = p.row;
   const double *sp = p.sp + (size_t)u * p.f_stride * bins, *ap = p.ap + (size_t)u * p.f_stride * bins;
 
   // GetSpectralEnvelope / GetAperiodicRatio (:140-179)
@@ -303,7 +310,7 @@ WB_KERNEL_PLAIN syn_overlap_kernel(SynParams p) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   const int n = p.y_len[u];
   if (s >= n) return;
-  const int N = p.fft_size, half = N / 2, np = p.n_pulses[u];
+  const int N = p.fft_u ? p.fft_u[u] : p.fft_size, half = N / 2, np = p.n_pulses[u];
   const int *pidx = p.pulse_idx + (size_t)u * p.pulse_cap;
   // pulse i covers samples idx_i - half + 1 .. idx_i + half  ->  idx_i in [s - half, s + half - 1]
   int lo = 0, hi = np;
@@ -311,7 +318,7 @@ WB_KERNEL_PLAIN syn_overlap_kernel(SynParams p) {
   double acc = 0.0;
   for (int i = lo; i < np && pidx[i] <= s + half - 1; ++i) {
     const int j = s - (pidx[i] - half + 1);
-    acc += p.resp[((size_t)u * p.pulse_cap + i) * N + j];
+    acc += p.resp[((size_t)u * p.pulse_cap + i) * p.resp_n + j];
   }
   if constexpr (std::is_same<Out, short>::value) p.y16[(size_t)u * p.y_stride + s] = pcm16_of(acc);
   else p.y[(size_t)u * p.y_stride + s] = acc;
@@ -328,8 +335,9 @@ WB_KERNEL_PLAIN syn_overlap_kernel(SynParams p) {
 //   sp[j] = exp(interp1(x, L, xi)[j])        (histc, then y[k-1] + s * (y[k] - y[k-1]), extrapolating)
 //   ratio < 1: sp[j] = sp[c - 1] for j >= c = (int)(fft_size / 2.0 * ratio)
 // The segment k and the weight s of every bin depend on (ratio, fft_size, fs) only.  They are planned on the host
-// with the reference's expressions and the library's own histc (wb_matlab.cu), one table per distinct ratio, and the
-// tail rule is folded in (entry j := entry c - 1 gives the same value).  The kernel is then one gather per bin:
+// with the reference's expressions and the library's own histc (wb_matlab.cu), one table per distinct (ratio,
+// fft_size), and the tail rule is folded in (entry j := entry c - 1 gives the same value).  The kernel is then one
+// gather per bin:
 //   modify_stretch_kernel  (frame, utterance) -> CTA: the row's logs into shared memory, barrier,
 //                          out[j] = exp(L[a] + s * (L[a + 1] - L[a])), rounded step by step as the reference's
 //                          unfused x86-64 build rounds it
@@ -338,15 +346,18 @@ WB_KERNEL_PLAIN syn_overlap_kernel(SynParams p) {
 #define WB_MODIFY_THREADS 128
 
 // Rows of frames >= f_len[u] (and utterances >= n_utts) are never touched.  The `continue` is uniform over the CTA.
+// Each frame row holds `row` doubles, of which the utterance's table covers the first tbins[t].
 WB_KERNEL(WB_MODIFY_THREADS, 8) modify_stretch_kernel(double *sp, const int *__restrict__ f_len, int n_utts,
-                                                      int f_stride, int bins, const int *__restrict__ table,
+                                                      int f_stride, int row_len, const int *__restrict__ table,
+                                                      const int *__restrict__ tbins, const int *__restrict__ toff,
                                                       const int *__restrict__ idx, const double *__restrict__ frac) {
-  WB_DYN_SMEM(double, logs);   // bins
+  WB_DYN_SMEM(double, logs);   // the largest table's bins
   const int tid = WB_TID, nth = WB_NTH, f = blockIdx.x;
   for (int u = blockIdx.y; u < n_utts; u += gridDim.y) {
     if (f >= f_len[u]) continue;
-    double *row = sp + ((size_t)u * f_stride + f) * bins;
-    const size_t t0 = (size_t)__ldg(&table[u]) * bins;
+    double *row = sp + ((size_t)u * f_stride + f) * row_len;
+    const int t = __ldg(&table[u]), bins = __ldg(&tbins[t]);
+    const size_t t0 = (size_t)__ldg(&toff[t]);
     for (int j = tid; j < bins; j += nth) logs[j] = log(row[j]);
     WB_SYNC();
     for (int j = tid; j < bins; j += nth) {
@@ -369,11 +380,12 @@ WB_KERNEL_PLAIN modify_f0_kernel(const double *f0_in, double *f0_out, const doub
 
 namespace {
 struct ModifyLayout {
-  size_t o_idx, o_frac, o_scale, o_table, total;
+  size_t o_idx, o_frac, o_tbins, o_toff, o_scale, o_table, total;
   ModifyLayout(const ModifyPlan &p, int n) {
     ArenaPlan a;
-    const size_t cells = (size_t)p.n_tables * p.bins;
+    const size_t cells = p.idx.size();
     o_idx = a.add(cells * 4); o_frac = a.add(cells * 8);
+    o_tbins = a.add((size_t)p.n_tables * 4); o_toff = a.add((size_t)p.n_tables * 4);
     o_scale = a.add(p.scale.empty() ? 0 : (size_t)n * 8); o_table = a.add(p.table.empty() ? 0 : (size_t)n * 4);
     total = a.total;
   }
@@ -390,7 +402,7 @@ int modify_fail(Ctx *ctx, const char *who, const char *what, int u, double v, co
 size_t ModifyPlan::device_bytes(int n) const { return ModifyLayout(*this, n).total; }
 
 int modify_plan(Ctx *ctx, const char *who, int n_utts, int fft_size, int fs, const double *f0_scale,
-                const double *spectral_ratio, ModifyPlan *plan) {
+                const double *spectral_ratio, ModifyPlan *plan, const int *fft_sizes) {
   *plan = ModifyPlan();
   if (f0_scale) {
     for (int u = 0; u < n_utts; ++u) {
@@ -400,7 +412,7 @@ int modify_plan(Ctx *ctx, const char *who, int n_utts, int fft_size, int fs, con
     plan->scale.assign(f0_scale, f0_scale + n_utts);
   }
   if (!spectral_ratio) return 0;
-  if (fft_size < 16 || fft_size > 4096 || (fft_size & (fft_size - 1))) {
+  if (!fft_sizes && (fft_size < 16 || fft_size > 4096 || (fft_size & (fft_size - 1)))) {
     ctx->last_error = std::string(who) + ": fft_size must be a power of two in [16, 4096]";
     return WORLD_B200_EINVAL;
   }
@@ -410,40 +422,44 @@ int modify_plan(Ctx *ctx, const char *who, int n_utts, int fft_size, int fs, con
   }
   for (int u = 0; u < n_utts; ++u) {
     const double r = spectral_ratio[u];
+    const int n_fft = fft_sizes ? fft_sizes[u] : fft_size;
     // histc needs an ascending axis; below 1 the tail copies bin c - 1, which must exist (c == 0 reads sp[-1])
     if (!(r > 0.0) || !isfinite(r)) return modify_fail(ctx, who, "spectral_ratio", u, r, "is not a finite ratio > 0");
-    if (r < 1.0 && static_cast<int>(fft_size / 2.0 * r) < 1)
+    if (r < 1.0 && static_cast<int>(n_fft / 2.0 * r) < 1)
       return modify_fail(ctx, who, "spectral_ratio", u, r, "leaves no bin below (int)(fft_size / 2.0 * ratio)");
   }
-  const int half = fft_size / 2, bins = half + 1;
-  plan->bins = bins;
   plan->table.resize(n_utts);
-  std::map<double, int> seen;
-  std::vector<double> x(bins), xi(bins);
-  std::vector<int> k(bins);
+  std::map<std::pair<double, int>, int> seen;
+  std::vector<double> x, xi;
+  std::vector<int> k;
   for (int u = 0; u < n_utts; ++u) {
     const double ratio = spectral_ratio[u];
-    auto it = seen.find(ratio);
+    const int n_fft = fft_sizes ? fft_sizes[u] : fft_size, half = n_fft / 2, bins = half + 1;
+    auto it = seen.find({ratio, n_fft});
     if (it != seen.end()) { plan->table[u] = it->second; continue; }
     const int t = plan->n_tables++;
-    seen[ratio] = t;
+    seen[{ratio, n_fft}] = t;
     plan->table[u] = t;
+    plan->bins = imax(plan->bins, bins);
+    plan->tbins.push_back(bins);
+    plan->toff.push_back((int)plan->idx.size());
+    x.resize(bins); xi.resize(bins); k.resize(bins);
     for (int i = 0; i <= half; ++i) {   // test.cpp:237-240, the same expressions in the same order
-      x[i] = ratio * i / fft_size * fs;
-      xi[i] = static_cast<double>(i) / fft_size * fs;
+      x[i] = ratio * i / n_fft * fs;
+      xi[i] = static_cast<double>(i) / n_fft * fs;
     }
     histc(x.data(), bins, xi.data(), bins, k.data());
-    plan->idx.resize((size_t)plan->n_tables * bins);
-    plan->frac.resize((size_t)plan->n_tables * bins);
-    int *ia = plan->idx.data() + (size_t)t * bins;
-    double *sa = plan->frac.data() + (size_t)t * bins;
+    plan->idx.resize(plan->idx.size() + bins);
+    plan->frac.resize(plan->frac.size() + bins);
+    int *ia = plan->idx.data() + plan->toff[t];
+    double *sa = plan->frac.data() + plan->toff[t];
     for (int j = 0; j < bins; ++j) {   // matlabfunctions.cpp:162-171: h[k-1] = x[k] - x[k-1], s = (xi - x[k-1]) / h
       const int a = k[j] - 1;
       ia[j] = a;
       sa[j] = (xi[j] - x[a]) / (x[a + 1] - x[a]);
     }
     if (ratio < 1.0) {                 // test.cpp:250-254
-      const int c = static_cast<int>(fft_size / 2.0 * ratio);
+      const int c = static_cast<int>(n_fft / 2.0 * ratio);
       for (int j = c; j < bins; ++j) { ia[j] = ia[c - 1]; sa[j] = sa[c - 1]; }
     }
   }
@@ -455,10 +471,13 @@ int modify_upload(Ctx *ctx, const ModifyPlan &plan, int u0, int n, unsigned char
   int rc = 0;
   if (!plan.idx.empty()) rc = dev_memcpy_h2d(ctx, blk + l.o_idx, plan.idx.data(), plan.idx.size() * 4);
   if (!rc && !plan.frac.empty()) rc = dev_memcpy_h2d(ctx, blk + l.o_frac, plan.frac.data(), plan.frac.size() * 8);
+  if (!rc && plan.n_tables) rc = dev_memcpy_h2d(ctx, blk + l.o_tbins, plan.tbins.data(), (size_t)plan.n_tables * 4);
+  if (!rc && plan.n_tables) rc = dev_memcpy_h2d(ctx, blk + l.o_toff, plan.toff.data(), (size_t)plan.n_tables * 4);
   if (!rc && !plan.scale.empty()) rc = dev_memcpy_h2d(ctx, blk + l.o_scale, plan.scale.data() + u0, (size_t)n * 8);
   if (!rc && !plan.table.empty()) rc = dev_memcpy_h2d(ctx, blk + l.o_table, plan.table.data() + u0, (size_t)n * 4);
   d->idx = (const int *)(blk + l.o_idx); d->frac = (const double *)(blk + l.o_frac);
   d->scale = (const double *)(blk + l.o_scale); d->table = (const int *)(blk + l.o_table);
+  d->tbins = (const int *)(blk + l.o_tbins); d->toff = (const int *)(blk + l.o_toff);
   return rc;
 }
 
@@ -469,16 +488,16 @@ void modify_f0_launch(Ctx *ctx, const ModifyDevice &d, const int *f_len, int n_u
   WB_LAUNCH_FLAT(modify_f0_kernel, grid, 256, 0, ctx->stream, f0_in, f0_out, d.scale, f_len, n_utts, f_stride);
 }
 
-void modify_stretch_launch(Ctx *ctx, const ModifyDevice &d, int bins, const int *f_len, int n_utts, int f_stride,
-                           int max_f, double *spectrogram) {
+void modify_stretch_launch(Ctx *ctx, const ModifyDevice &d, int row, int max_bins, const int *f_len, int n_utts,
+                           int f_stride, int max_f, double *spectrogram) {
   if (n_utts <= 0 || max_f <= 0) return;
   const dim3 grid((unsigned)max_f, (unsigned)imin(n_utts, 65535));
-  WB_LAUNCH_COOP(modify_stretch_kernel, grid, WB_MODIFY_THREADS, (size_t)bins * 8, ctx->stream, spectrogram, f_len,
-                 n_utts, f_stride, bins, d.table, d.idx, d.frac);
+  WB_LAUNCH_COOP(modify_stretch_kernel, grid, WB_MODIFY_THREADS, (size_t)max_bins * 8, ctx->stream, spectrogram, f_len,
+                 n_utts, f_stride, row, d.table, d.tbins, d.toff, d.idx, d.frac);
 }
 
-int modify_run(Ctx *ctx, const ModifyPlan &plan, int u0, int n_utts, const int *f0_lengths, int f0_stride, double *f0,
-               double *spectrogram) {
+int modify_run(Ctx *ctx, const ModifyPlan &plan, int u0, int n_utts, const int *f0_lengths, int f0_stride, int row,
+               double *f0, double *spectrogram) {
   int max_f = 0;
   for (int u = 0; u < n_utts; ++u) max_f = imax(max_f, f0_lengths[u]);
   if (max_f == 0 || (plan.scale.empty() && plan.table.empty())) return 0;
@@ -492,7 +511,7 @@ int modify_run(Ctx *ctx, const ModifyPlan &plan, int u0, int n_utts, const int *
   if (rc) return rc;
   const int *f_len = (const int *)(blk + o_len);
   if (!plan.scale.empty()) modify_f0_launch(ctx, d, f_len, n_utts, f0_stride, max_f, f0, f0);
-  if (!plan.table.empty()) modify_stretch_launch(ctx, d, plan.bins, f_len, n_utts, f0_stride, max_f, spectrogram);
+  if (!plan.table.empty()) modify_stretch_launch(ctx, d, row, plan.bins, f_len, n_utts, f0_stride, max_f, spectrogram);
   return dev_check(ctx, "modify");
 }
 
@@ -517,64 +536,108 @@ int synthesis_plan(Ctx *ctx, const SynthesisRequest &r, const char *who, Synthes
     ctx->last_error = std::string(who) + ": " + what;
     return WORLD_B200_EINVAL;
   };
+  auto fail_u = [&](const std::string &what, int u) { return fail(what + " (utterance " + std::to_string(u) + ")"); };
   if (!r.y || (!r.transform && (!r.f0 || !r.sp || (!r.coded && !r.ap))))
     return fail(r.coded ? "f0, coded_spectral_envelope and y must be given"
                         : "f0, spectrogram, aperiodicity and y must be given");
+  if (r.per_utt && !r.fft_sizes) return fail("fft_sizes must be given");
   if (r.n < 0) return fail("n_utts must be >= 0");
   if (r.fs <= 0) return fail("fs must be > 0");
   if (r.frame_period <= 0) return fail("frame_period must be > 0");
   if (r.nbit != 0 && r.nbit != 16) return fail("nbit must be 0 (double) or 16 (int16)");
-  const int fft_size = r.fft_size;
-  if (fft_size < 16 || fft_size > WB_TW_N / 2 || (fft_size & (fft_size - 1)))
-    return fail("fft_size must be a power of two in [16, 4096]");
-  p->n = r.n; p->f0_stride = r.f0_stride; p->y_stride = r.y_stride; p->fft_size = fft_size; p->fs = r.fs;
+  auto bad_size = [](int f) { return f < 16 || f > WB_TW_N / 2 || (f & (f - 1)); };
+  if (!r.per_utt && bad_size(r.fft_size)) return fail("fft_size must be a power of two in [16, 4096]");
+  // each utterance's size, and the distinct sizes in order of first appearance
+  p->size.assign(r.n, 0);
+  if (!r.per_utt) p->sizes.assign(1, r.fft_size);
+  for (int u = 0; u < r.n && r.per_utt; ++u) {
+    const int f = r.fft_sizes[u];
+    if (bad_size(f))
+      return fail_u("fft_sizes[" + std::to_string(u) + "] = " + std::to_string(f) +
+                    " is not a power of two in [16, 4096]", u);
+    const auto it = std::find(p->sizes.begin(), p->sizes.end(), f);
+    p->size[u] = (int)(it - p->sizes.begin());
+    if (it == p->sizes.end()) p->sizes.push_back(f);
+  }
+  p->fft_size = 0;
+  for (const int f : p->sizes) p->fft_size = imax(p->fft_size, f);
+  p->row = p->fft_size / 2 + 1;
+  if (r.per_utt && !r.coded) {
+    p->row = r.row_stride;
+    for (int u = 0; u < r.n; ++u)
+      if (r.row_stride < r.fft_sizes[u] / 2 + 1)
+        return fail_u("row_stride = " + std::to_string(r.row_stride) + " is smaller than fft_sizes[" +
+                      std::to_string(u) + "] / 2 + 1 = " + std::to_string(r.fft_sizes[u] / 2 + 1), u);
+  }
+  p->n = r.n; p->f0_stride = r.f0_stride; p->y_stride = r.y_stride; p->fs = r.fs;
   p->nbit = r.nbit; p->frame_period = r.frame_period;
-  while ((1 << p->lg) < fft_size) ++p->lg;
   p->coded = r.coded;
+  const int n_sizes = (int)p->sizes.size();
   int rc = 0;
   if (r.coded) {
-    if (codec_decode_sp_tables(ctx, r.fs, fft_size, r.dims, &p->tsp)) return fail(ctx->last_error);
-    codec_decode_ap_tables(r.fs, fft_size, &p->tap);
-    if (p->tap.dims > 0 && !r.ap)
-      return fail("coded_aperiodicity is NULL, but fs has GetNumberOfAperiodicities(fs) > 0 bands");
+    p->tsp.resize(n_sizes);
+    p->tap.resize(n_sizes);
+    for (int g = 0; g < n_sizes; ++g) {
+      if (codec_decode_sp_tables(ctx, r.fs, p->sizes[g], r.dims, &p->tsp[g])) {
+        if (!r.per_utt) return fail(ctx->last_error);
+        const int u = (int)(std::find(p->size.begin(), p->size.end(), g) - p->size.begin());
+        return fail_u(ctx->last_error + " (number_of_dimensions = " + std::to_string(r.dims) + ", fft_sizes[" +
+                      std::to_string(u) + "] = " + std::to_string(p->sizes[g]) + ")", u);
+      }
+      codec_decode_ap_tables(r.fs, p->sizes[g], &p->tap[g]);
+    }
+    p->dims = r.dims;
+    p->n_ap = n_sizes ? p->tap[0].dims : 0;
+    if (p->n_ap > 0 && !r.ap) return fail("coded_aperiodicity is NULL, but fs has GetNumberOfAperiodicities(fs) > 0 bands");
   }
   p->modify = r.f0_scale || r.spectral_ratio;
-  if (p->modify) rc = modify_plan(ctx, who, r.n, fft_size, r.fs, r.f0_scale, r.spectral_ratio, &p->mod);
+  if (p->modify)
+    rc = modify_plan(ctx, who, r.n, r.fft_size, r.fs, r.f0_scale, r.spectral_ratio, &p->mod,
+                     r.per_utt ? r.fft_sizes : nullptr);
   if (!rc) rc = row_lengths(ctx, who, "f0", r.f0_lengths, r.n, r.f0_stride, 2, &p->f_len);
   if (!rc) rc = row_lengths(ctx, who, "y", r.y_lengths, r.n, r.y_stride, 2, &p->y_len);
   if (rc) return rc;
   if (r.transform) p->fp.assign(r.fp, r.fp + r.n);
-  // DC remover (GetDCRemover, synthesis.cpp:319-333), host libm like the reference
-  std::vector<double> &dcr = p->dc_remover;
-  dcr.resize(fft_size);
-  double dc = 0.0;
-  for (int i = 0; i < fft_size / 2; ++i) {
-    dcr[i] = 0.5 - 0.5 * cos(2.0 * kPi * (i + 1.0) / (1.0 + fft_size));
-    dcr[fft_size - i - 1] = dcr[i];
-    dc += dcr[i] * 2.0;
+  // DC remover of each size (GetDCRemover, synthesis.cpp:319-333), host libm like the reference
+  p->dc_remover.resize(n_sizes);
+  for (int g = 0; g < n_sizes; ++g) {
+    const int fft_size = p->sizes[g];
+    std::vector<double> &dcr = p->dc_remover[g];
+    dcr.resize(fft_size);
+    double dc = 0.0;
+    for (int i = 0; i < fft_size / 2; ++i) {
+      dcr[i] = 0.5 - 0.5 * cos(2.0 * kPi * (i + 1.0) / (1.0 + fft_size));
+      dcr[fft_size - i - 1] = dcr[i];
+      dc += dcr[i] * 2.0;
+    }
+    for (int i = 0; i < fft_size / 2; ++i) { dcr[i] /= dc; dcr[fft_size - i - 1] = dcr[i]; }
   }
-  for (int i = 0; i < fft_size / 2; ++i) { dcr[i] /= dc; dcr[fft_size - i - 1] = dcr[i]; }
   return 0;
 }
 
 SynthesisSizing::SynthesisSizing(const Ctx *ctx, const SynthesisPlan &p, int max_y)
     : fft_size(p.fft_size), y_stride(p.y_stride) {
-  const size_t bins = (size_t)fft_size / 2 + 1;
-  // The coded call holds one chunk's decoded envelope and aperiodicity (16 B per bin and frame) and the decode tables.
+  // The coded call holds one chunk's decoded envelope and aperiodicity (16 B per row entry and frame) and the decode
+  // tables of every size.
   size_t tables = 0;
   if (p.coded) {
     ArenaPlan tp;
-    tp.add(p.tsp.idx.size() * 4); tp.add(p.tsp.frac.size() * 8); tp.add(p.tsp.weight.size() * 16);
-    tp.add(p.tap.idx.size() * 4); tp.add(p.tap.frac.size() * 8);
+    for (size_t g = 0; g < p.sizes.size(); ++g) {
+      tp.add(p.tsp[g].idx.size() * 4); tp.add(p.tsp[g].frac.size() * 8); tp.add(p.tsp[g].weight.size() * 16);
+      tp.add(p.tap[g].idx.size() * 4); tp.add(p.tap[g].frac.size() * 8);
+    }
     tables = tp.total;
   }
-  decoded_per_utt = p.coded ? (size_t)p.f0_stride * bins * 16 : 0;
+  decoded_per_utt = p.coded ? (size_t)p.f0_stride * p.row * 16 : 0;
   // A modified call also holds the stretch tables, and per utterance its factor, table index and scaled f0 row (the
   // 256-byte alignment of the two small arrays is in the 4096 below).
   if (p.coded && p.modify) {
     tables += p.mod.device_bytes(0);
     decoded_per_utt += (size_t)p.f0_stride * 8 + 12;
   }
+  // A call of several sizes holds the DC removers of the others, and per utterance its size and list entry.
+  for (size_t g = 1; g < p.sizes.size(); ++g) tables += ((size_t)p.sizes[g] * 8 + 255) & ~(size_t)255;
+  if (p.sizes.size() > 1) decoded_per_utt += 8;
   budget = (double)ctx->scratch_budget - (double)tables;
   // Pulse arrays and responses are sized for 1200 pulses per second (f0 <= 1.2 kHz; the +64 covers the ends).
   nominal_cap = (int)((double)max_y / p.fs * 1200.0) + 64;
@@ -590,13 +653,15 @@ size_t SynthesisSizing::per_utt(int cap) const {
 int SynthesisSizing::fit(int cap) const { return (int)dmin(65535.0, budget / (double)per_utt(cap)); }
 
 namespace {
-// The scratch block of one pass of n utterances with room for cap pulses each
+// The scratch block of one pass of n utterances with room for cap pulses each.  Per size g: its DC remover and (coded)
+// its decode tables.
 struct PassLayout {
-  size_t len, phase, vuv, pidx, psh, np, cnt, dcnt, doff, dtot, pl, draws, resp, dcr;
-  size_t dsp = 0, dap = 0, sidx = 0, sfrac = 0, sw = 0, aidx = 0, afrac = 0;   // coded
-  size_t mod = 0, f0m = 0, fp = 0, total;
+  size_t len, phase, vuv, pidx, psh, np, cnt, dcnt, doff, dtot, pl, draws, resp;
+  std::vector<size_t> dcr, sidx, sfrac, sw, aidx, afrac;
+  size_t dsp = 0, dap = 0;   // coded
+  size_t mod = 0, f0m = 0, fp = 0, fft_u = 0, list = 0, total;
   PassLayout(const SynthesisPlan &p, int n, int cap, size_t draw_stride) {
-    const size_t N = n, frames = N * p.f0_stride, bins = (size_t)p.fft_size / 2 + 1;
+    const size_t N = n, frames = N * p.f0_stride, G = p.sizes.size();
     ArenaPlan a;
     len = a.add(2 * N * 4);                                          // f0 lengths, then y lengths
     phase = a.add(N * p.y_stride * 8); vuv = a.add(N * p.y_stride * 8);
@@ -606,33 +671,52 @@ struct PassLayout {
     dtot = a.add(N * 4); pl = a.add(N * 4);
     draws = a.add(N * draw_stride * 4);
     resp = a.add(N * cap * p.fft_size * 8);
-    dcr = a.add((size_t)p.fft_size * 8);
+    for (size_t g = 0; g < G; ++g) dcr.push_back(a.add((size_t)p.sizes[g] * 8));
     if (p.coded) {
-      dsp = a.add(frames * bins * 8); dap = a.add(frames * bins * 8);
-      sidx = a.add(p.tsp.idx.size() * 4); sfrac = a.add(p.tsp.frac.size() * 8); sw = a.add(p.tsp.weight.size() * 16);
-      aidx = a.add(p.tap.idx.size() * 4); afrac = a.add(p.tap.frac.size() * 8);
+      dsp = a.add(frames * p.row * 8); dap = a.add(frames * p.row * 8);
+      for (size_t g = 0; g < G; ++g) {
+        const CodecTables &ts = p.tsp[g], &ta = p.tap[g];
+        sidx.push_back(a.add(ts.idx.size() * 4)); sfrac.push_back(a.add(ts.frac.size() * 8));
+        sw.push_back(a.add(ts.weight.size() * 16));
+        aidx.push_back(a.add(ta.idx.size() * 4)); afrac.push_back(a.add(ta.frac.size() * 8));
+      }
       if (p.modify) {
         mod = a.add(p.mod.device_bytes(n));
         if (!p.mod.scale.empty()) f0m = a.add(frames * 8);
       }
     }
     if (!p.fp.empty()) fp = a.add(N * 8);
+    if (G > 1) { fft_u = a.add(N * 4); list = a.add(N * 4); }
     total = a.total;
   }
 };
+
+int log2_of(int v) {
+  int lg = 0;
+  while ((1 << lg) < v) ++lg;
+  return lg;
+}
+
+// syn_pulse_kernel's dynamic shared memory at one fft_size
+size_t pulse_smem(int fft_size) {
+  const int half = fft_size / 2;
+  return (size_t)(2 * fft_size + 2 * (half + 2) + (fft_size + 2) + 2 * (half + 1) + fft_size + WB_RED_DOUBLES) * 8;
+}
 }  // namespace
 
 // nbit 0 writes the waveform (double), nbit 16 its 16-bit PCM (short).
 int synthesis_run(Ctx *ctx, const SynthesisPlan &plan, int u0, int m, const SynthesisRows &rows) {
   if (m == 0) return 0;
   const int *f_len = plan.f_len.data() + u0, *y_len = plan.y_len.data() + u0;
-  const int fft_size = plan.fft_size, half = fft_size / 2, f0_stride = plan.f0_stride, y_stride = plan.y_stride;
-  const size_t bins = (size_t)half + 1;
+  const int f0_stride = plan.f0_stride, y_stride = plan.y_stride, n_sizes = (int)plan.sizes.size();
+  const size_t row = plan.row;
+  const bool mixed = n_sizes > 1;
   int max_y = 0;
   for (int i = 0; i < m; ++i) max_y = imax(max_y, y_len[i]);
   // The caller's f0 may be anything up to fs/2 (a pitch-shifted contour), so syn_timebase_kernel also counts the
   // pulses it could not store; a chunk where that count exceeds the cap is laid out again with room for its largest
   // count, in as many passes as the scratch budget needs.  The common case pays one read-back of n counts per chunk.
+  // Every response slot holds the call's largest fft_size, so a pass's layout does not depend on which sizes it has.
   const SynthesisSizing sz(ctx, plan, max_y);
   const ModifyPlan *mod = plan.coded && plan.modify ? &plan.mod : nullptr;
   const bool scale_f0 = mod && !mod->scale.empty(), stretch = mod && !mod->table.empty();
@@ -640,9 +724,8 @@ int synthesis_run(Ctx *ctx, const SynthesisPlan &plan, int u0, int m, const Synt
   const size_t draw_stride = sz.draw_stride;
   auto fit = [&](int cap) { return sz.fit(cap); };
   const int chunk = balanced_chunk(imin(m, 65535), fit(nominal_cap));
-  const size_t smem = (size_t)(2 * fft_size + 2 * (half + 2) + (fft_size + 2) + 2 * (half + 1) + fft_size + WB_RED_DOUBLES) * 8;
 #ifndef WB_EMU
-  cudaFuncSetAttribute(syn_pulse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaFuncSetAttribute(syn_pulse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pulse_smem(plan.fft_size));
 #endif
   std::vector<int> counts;
   int v0 = 0, n = imin(chunk, m), pulse_cap = nominal_cap;   // this pass: utterances [u0 + v0, u0 + v0 + n)
@@ -654,17 +737,28 @@ int synthesis_run(Ctx *ctx, const SynthesisPlan &plan, int u0, int m, const Synt
     std::vector<int> l2((size_t)2 * n), pl(n, pulse_cap);
     int max_f = 0;
     for (int i = 0; i < n; ++i) { l2[i] = f_len[v0 + i]; l2[n + i] = y_len[v0 + i]; max_f = imax(max_f, l2[i]); }
+    // the pass's utterances grouped by size: group g is list[first[g] .. first[g + 1])
+    std::vector<int> fft_u(n), list, first(n_sizes + 1, 0);
+    for (int g = 0; g < n_sizes; ++g) {
+      first[g] = (int)list.size();
+      for (int i = 0; i < n; ++i)
+        if (plan.size[u0 + v0 + i] == g) { list.push_back(i); fft_u[i] = plan.sizes[g]; }
+    }
+    first[n_sizes] = n;
     int rc = dev_memcpy_h2d(ctx, blk + l.len, l2.data(), l2.size() * 4);
-    if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.dcr, plan.dc_remover.data(), (size_t)fft_size * 8);
+    for (int g = 0; g < n_sizes && !rc; ++g)
+      rc = dev_memcpy_h2d(ctx, blk + l.dcr[g], plan.dc_remover[g].data(), (size_t)plan.sizes[g] * 8);
     if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.pl, pl.data(), (size_t)n * 4);
     if (!rc && !plan.fp.empty()) rc = dev_memcpy_h2d(ctx, blk + l.fp, plan.fp.data() + u0 + v0, (size_t)n * 8);
-    if (plan.coded) {
-      const CodecTables &s = plan.tsp, &a = plan.tap;
-      if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.sidx, s.idx.data(), s.idx.size() * 4);
-      if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.sfrac, s.frac.data(), s.frac.size() * 8);
-      if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.sw, s.weight.data(), s.weight.size() * 16);
-      if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.aidx, a.idx.data(), a.idx.size() * 4);
-      if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.afrac, a.frac.data(), a.frac.size() * 8);
+    if (!rc && mixed) rc = dev_memcpy_h2d(ctx, blk + l.fft_u, fft_u.data(), (size_t)n * 4);
+    if (!rc && mixed) rc = dev_memcpy_h2d(ctx, blk + l.list, list.data(), (size_t)n * 4);
+    for (int g = 0; g < n_sizes && plan.coded; ++g) {
+      const CodecTables &s = plan.tsp[g], &a = plan.tap[g];
+      if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.sidx[g], s.idx.data(), s.idx.size() * 4);
+      if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.sfrac[g], s.frac.data(), s.frac.size() * 8);
+      if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.sw[g], s.weight.data(), s.weight.size() * 16);
+      if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.aidx[g], a.idx.data(), a.idx.size() * 4);
+      if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.afrac[g], a.frac.data(), a.frac.size() * 8);
     }
     ModifyDevice md = {};
     if (mod && !rc) rc = modify_upload(ctx, *mod, u0 + v0, n, blk + l.mod, &md);
@@ -674,9 +768,11 @@ int synthesis_run(Ctx *ctx, const SynthesisPlan &plan, int u0, int m, const Synt
     if (plan.coded) {
       p.sp = (const double *)(blk + l.dsp); p.ap = (const double *)(blk + l.dap);
     } else {
-      p.sp = rows.sp + (size_t)v0 * f0_stride * bins; p.ap = rows.ap + (size_t)v0 * f0_stride * bins;
+      p.sp = rows.sp + (size_t)v0 * f0_stride * row; p.ap = rows.ap + (size_t)v0 * f0_stride * row;
     }
-    p.fft_size = fft_size; p.lg_fft = plan.lg; p.frame_period = plan.frame_period / 1000.0; p.fs = plan.fs;
+    p.fft_size = plan.fft_size; p.lg_fft = log2_of(plan.fft_size); p.row = (int)row;
+    p.fft_u = mixed ? (const int *)(blk + l.fft_u) : nullptr; p.list = nullptr;
+    p.frame_period = plan.frame_period / 1000.0; p.fs = plan.fs;
     p.fp_u = plan.fp.empty() ? nullptr : (const double *)(blk + l.fp);
     p.y_len = (const int *)(blk + l.len) + n; p.y_stride = y_stride;
     p.phase = (double *)(blk + l.phase); p.vuv = (double *)(blk + l.vuv); p.flag_cnt = nullptr;
@@ -685,7 +781,7 @@ int synthesis_run(Ctx *ctx, const SynthesisPlan &plan, int u0, int m, const Synt
     p.draw_cnt = (unsigned *)(blk + l.dcnt); p.draw_off = (unsigned *)(blk + l.doff);
     p.draw_tot = (unsigned *)(blk + l.dtot);
     p.draws = (const unsigned *)(blk + l.draws); p.draw_stride = draw_stride;
-    p.resp = (double *)(blk + l.resp); p.dc_remover = (const double *)(blk + l.dcr);
+    p.resp = (double *)(blk + l.resp); p.resp_n = plan.fft_size; p.dc_remover = (const double *)(blk + l.dcr[0]);
     p.y = plan.nbit ? nullptr : (double *)rows.y + (size_t)v0 * y_stride;
     p.y16 = plan.nbit ? (short *)rows.y + (size_t)v0 * y_stride : nullptr;
     p.tw = ctx->twiddle;
@@ -713,22 +809,39 @@ int synthesis_run(Ctx *ctx, const SynthesisPlan &plan, int u0, int m, const Synt
         continue;
       }
     }
+    // size group g of this pass: its utterance count, and its list on the device (null: the whole pass)
+    auto group_n = [&](int g) { return first[g + 1] - first[g]; };
+    auto group_list = [&](int g) { return mixed ? (const int *)(blk + l.list) + first[g] : nullptr; };
     if (plan.coded) {
-      // DecodeSpectralEnvelope / DecodeAperiodicity of this pass's utterances, frames [0, f0_length)
-      const CodecDeviceTables ts = {(const int *)(blk + l.sidx), (const double *)(blk + l.sfrac),
-                                    (const double2 *)(blk + l.sw)};
-      const CodecDeviceTables ta = {(const int *)(blk + l.aidx), (const double *)(blk + l.afrac), nullptr};
+      // DecodeSpectralEnvelope / DecodeAperiodicity of this pass's utterances, frames [0, f0_length), each at its size
+      // into rows of the call's largest bins
       double *dsp = (double *)(blk + l.dsp), *dap = (double *)(blk + l.dap);
-      codec_decode_launch(ctx, true, plan.tsp, ts, fft_size, p.f_len, n, f0_stride, max_f,
-                          rows.sp + (size_t)v0 * f0_stride * plan.tsp.dims, dsp);
-      if (stretch) modify_stretch_launch(ctx, md, (int)bins, p.f_len, n, f0_stride, max_f, dsp);
+      for (int g = 0; g < n_sizes; ++g) {
+        const CodecDeviceTables ts = {(const int *)(blk + l.sidx[g]), (const double *)(blk + l.sfrac[g]),
+                                      (const double2 *)(blk + l.sw[g])};
+        codec_decode_launch(ctx, true, plan.tsp[g], ts, plan.sizes[g], p.f_len, group_n(g), f0_stride, max_f,
+                            rows.sp + (size_t)v0 * f0_stride * plan.dims, dsp, group_list(g), (int)row);
+      }
+      if (stretch) modify_stretch_launch(ctx, md, (int)row, mod->bins, p.f_len, n, f0_stride, max_f, dsp);
       // below 12 kHz there are no bands: the kernel reads no coded value (its input pointer only has to be valid)
-      codec_decode_launch(ctx, false, plan.tap, ta, fft_size, p.f_len, n, f0_stride, max_f,
-                          plan.tap.dims > 0 ? rows.ap + (size_t)v0 * f0_stride * plan.tap.dims : dap, dap);
+      for (int g = 0; g < n_sizes; ++g) {
+        const CodecDeviceTables ta = {(const int *)(blk + l.aidx[g]), (const double *)(blk + l.afrac[g]), nullptr};
+        codec_decode_launch(ctx, false, plan.tap[g], ta, plan.sizes[g], p.f_len, group_n(g), f0_stride, max_f,
+                            plan.n_ap > 0 ? rows.ap + (size_t)v0 * f0_stride * plan.n_ap : dap, dap, group_list(g),
+                            (int)row);
+      }
     }
     scan_counts(ctx, p.draw_cnt, (const int *)(blk + l.pl), pulse_cap, nullptr, p.draw_off, p.draw_tot, n);
     rng_fill(ctx, p.draw_tot, (unsigned *)(blk + l.draws), draw_stride, draw_stride, n);
-    WB_LAUNCH_COOP(syn_pulse_kernel, dim3((unsigned)pulse_cap, (unsigned)n), 128, smem, ctx->stream, p);
+    // one launch per size, each with its own shared memory (and so its own occupancy)
+    for (int g = 0; g < n_sizes; ++g) {
+      if (group_n(g) == 0) continue;
+      SynParams q = p;
+      q.fft_size = plan.sizes[g]; q.lg_fft = log2_of(q.fft_size);
+      q.dc_remover = (const double *)(blk + l.dcr[g]); q.list = group_list(g);
+      WB_LAUNCH_COOP(syn_pulse_kernel, dim3((unsigned)pulse_cap, (unsigned)group_n(g)), 128, pulse_smem(q.fft_size),
+                     ctx->stream, q);
+    }
     if (plan.nbit)
       WB_LAUNCH_FLAT(syn_overlap_kernel<short>, dim3((unsigned)((max_y + 255) / 256), (unsigned)n), 256, 0, ctx->stream, p);
     else
@@ -805,24 +918,80 @@ extern "C" int world_b200_synthesis_coded_batch_pcm16(WorldB200 *h, const double
                                coded_aperiodicity, fft_size, frame_period, fs, y_lengths, y_stride, y, 16);
 }
 
-extern "C" int world_b200_modify_batch(WorldB200 *h, double *f0, const int *f0_lengths, int n_utts, int f0_stride,
-                                       double *spectrogram, int fft_size, int fs, const double *f0_scale,
-                                       const double *spectral_ratio) {
+// world_b200_modify_batch (fft_sizes NULL: fft_size for every utterance, rows of fft_size / 2 + 1) and
+// world_b200_modify_batch_options (utterance u at fft_sizes[u], rows of row_stride)
+static int modify_batch(WorldB200 *h, double *f0, const int *f0_lengths, int n_utts, int f0_stride,
+                        double *spectrogram, int row_stride, int fft_size, const int *fft_sizes, bool per_utt, int fs,
+                        const double *f0_scale, const double *spectral_ratio) {
   if (!h) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
   Ctx *ctx = &h->c;
-  if (n_utts < 0 || f0_stride <= 0) {
-    ctx->last_error = "modify: n_utts must be >= 0 and f0_stride > 0";
+  auto fail = [&](const std::string &what) {
+    ctx->last_error = "modify: " + what;
     return WORLD_B200_EINVAL;
-  }
-  if ((f0_scale && !f0) || (spectral_ratio && !spectrogram)) {
-    ctx->last_error = "modify: f0_scale needs f0 rows and spectral_ratio needs spectrogram rows";
-    return WORLD_B200_EINVAL;
+  };
+  if (n_utts < 0 || f0_stride <= 0) return fail("n_utts must be >= 0 and f0_stride > 0");
+  if ((f0_scale && !f0) || (spectral_ratio && !spectrogram))
+    return fail("f0_scale needs f0 rows and spectral_ratio needs spectrogram rows");
+  if (per_utt && spectral_ratio) {
+    if (!fft_sizes) return fail("fft_sizes must be given");
+    if (fs <= 0) return fail("fs must be > 0");
+    for (int u = 0; u < n_utts; ++u) {
+      const int f = fft_sizes[u], why = f < 16 || f > 4096 || (f & (f - 1)) ? 1 : row_stride < f / 2 + 1 ? 2 : 0;
+      if (why == 1)
+        return fail("fft_sizes[" + std::to_string(u) + "] = " + std::to_string(f) +
+                    " is not a power of two in [16, 4096] (utterance " + std::to_string(u) + ")");
+      if (why == 2)
+        return fail("row_stride = " + std::to_string(row_stride) + " is smaller than fft_sizes[" + std::to_string(u) +
+                    "] / 2 + 1 = " + std::to_string(f / 2 + 1) + " (utterance " + std::to_string(u) + ")");
+    }
   }
   // a length of 0 is allowed here: the utterance's rows are left alone
   std::vector<int> lens;
   ModifyPlan plan;
   int rc = row_lengths(ctx, "modify", "f0", f0_lengths, n_utts, f0_stride, 0, &lens);
-  if (!rc) rc = modify_plan(ctx, "modify", n_utts, fft_size, fs, f0_scale, spectral_ratio, &plan);
-  return rc ? rc : modify_run(ctx, plan, 0, n_utts, lens.data(), f0_stride, f0, spectrogram);
+  if (!rc) rc = modify_plan(ctx, "modify", n_utts, fft_size, fs, f0_scale, spectral_ratio, &plan,
+                            per_utt ? fft_sizes : nullptr);
+  return rc ? rc : modify_run(ctx, plan, 0, n_utts, lens.data(), f0_stride, per_utt ? row_stride : plan.bins, f0,
+                              spectrogram);
+}
+
+extern "C" int world_b200_modify_batch(WorldB200 *h, double *f0, const int *f0_lengths, int n_utts, int f0_stride,
+                                       double *spectrogram, int fft_size, int fs, const double *f0_scale,
+                                       const double *spectral_ratio) {
+  return modify_batch(h, f0, f0_lengths, n_utts, f0_stride, spectrogram, 0, fft_size, nullptr, false, fs, f0_scale,
+                      spectral_ratio);
+}
+
+extern "C" int world_b200_modify_batch_options(WorldB200 *h, double *f0, const int *f0_lengths, int n_utts,
+                                               int f0_stride, double *spectrogram, int row_stride,
+                                               const int *fft_sizes, int fs, const double *f0_scale,
+                                               const double *spectral_ratio) {
+  return modify_batch(h, f0, f0_lengths, n_utts, f0_stride, spectrogram, row_stride, 0, fft_sizes, true, fs, f0_scale,
+                      spectral_ratio);
+}
+
+extern "C" int world_b200_synthesis_batch_options(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts,
+                                                  int f0_stride, const double *spectrogram,
+                                                  const double *aperiodicity, int row_stride, const int *fft_sizes,
+                                                  double frame_period, int fs, const int *y_lengths, int y_stride,
+                                                  double *y) {
+  SynthesisRequest r{f0, f0_lengths, n_utts, f0_stride, spectrogram, aperiodicity, 0, frame_period, fs, y_lengths,
+                     y_stride, y, 0};
+  r.per_utt = true; r.fft_sizes = fft_sizes; r.row_stride = row_stride;
+  return synthesis_batch(h, r);
+}
+
+extern "C" int world_b200_synthesis_coded_batch_options(WorldB200 *h, const double *f0, const int *f0_lengths,
+                                                        int n_utts, int f0_stride,
+                                                        const double *coded_spectral_envelope,
+                                                        int number_of_dimensions, const double *coded_aperiodicity,
+                                                        const int *fft_sizes, double frame_period, int fs,
+                                                        const int *y_lengths, int y_stride, const double *f0_scale,
+                                                        const double *spectral_ratio, int nbit, void *y) {
+  SynthesisRequest r{f0, f0_lengths, n_utts, f0_stride, coded_spectral_envelope, coded_aperiodicity, 0, frame_period,
+                     fs, y_lengths, y_stride, y, nbit};
+  r.coded = true; r.dims = number_of_dimensions; r.f0_scale = f0_scale; r.spectral_ratio = spectral_ratio;
+  r.per_utt = true; r.fft_sizes = fft_sizes;
+  return synthesis_batch(h, r);
 }
