@@ -6,7 +6,8 @@ utterance the per-utterance F0 range that tools/bench_f0_ranges.py picks for it 
 call).  Only the Harvest call is timed.  Prints ONE JSON line: ms per call (every timed call and their mean), the
 library's per-kernel CUDA-event times of the timed calls (profile_report, a separate pass so that the per-launch
 events do not slow the timed one) with the band sweep's two kernels, band_fir_events_kernel and band_interp_kernel,
-pulled out, and next to them the two candidate-map kernels that follow, harvest_detect_kernel and harvest_remove_kernel,
+pulled out, next to them the two candidate-map kernels that follow, harvest_detect_kernel and harvest_remove_kernel,
+and the three kernels of the decision tail, harvest_remove_kernel, harvest_contour_kernel and harvest_smooth_kernel,
 and the card's name, power limit and SM clocks read in the same run (read-only nvidia-smi queries).
 Writes nothing unless `--dump DIR` is given: then the time axis and f0 of the last call go to DIR as float64 .npy,
 so that two builds can be compared value for value on the same batch.
@@ -26,6 +27,7 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 SWEEP_KERNELS = ("band_fir_events_kernel", "band_interp_kernel")
 CANDIDATE_KERNELS = ("harvest_detect_kernel", "harvest_remove_kernel")
+TAIL_KERNELS = ("harvest_remove_kernel", "harvest_contour_kernel", "harvest_smooth_kernel")
 
 
 def main():
@@ -91,6 +93,7 @@ def main():
         "ms": [round(v, 3) for v in times],
         "sweep": {k: kernels.get(k, {}).get("ms_per_call") for k in SWEEP_KERNELS},
         "candidates": {k: kernels.get(k, {}).get("ms_per_call") for k in CANDIDATE_KERNELS},
+        "tail": {k: kernels.get(k, {}).get("ms_per_call") for k in TAIL_KERNELS},
         "shape": {"utts": U, "seconds": a.seconds, "fs": fs, "ranges": a.ranges, "frames": U * int(f0.shape[1]),
                   "voiced": int((f0 > 0).sum().item())},
         "kernels": kernels,

@@ -7,7 +7,7 @@
 //   K-HVr  harvest_refine_kernel   instantaneous-frequency refinement, one warp per 1 ms frame,
 //                                  the +-3 frame overlap (:417-429) done as an index map  (:434-631)
 //          harvest_remove_kernel   RemoveUnreliableCandidates                          (:652-688)
-//   K-HVc  harvest_contour_kernel  SearchF0Base + FixStep1..4 (sequential per utterance) (:693-1043)
+//   K-HVc  harvest_contour_kernel  FixStep1..4, one CTA per utterance; ExtendF0 and SearchScore per warp (:693-1043)
 //          harvest_smooth_kernel   zero-lag Butterworth per voiced section + subsample  (:1049-1113, 1246-1251)
 // GetMeanF0's two FFTs per candidate are replaced by a sparse DFT at the <= 6 harmonic bins that
 // FixF0 reads (same linear functional, SURVEY.md A5 step 5).
@@ -674,19 +674,49 @@ WB_DEV int hv_boundaries(const double *f0, int n, int *list, int *cnt) {
   return total;
 }
 
-// SelectBestF0 (harvest.cpp:636-650): last candidate among those with the smallest error <= allowed
-WB_DEV double hv_select_best(double reference, const double *row, int n, double allowed) {
-  double best = 0.0, best_err = allowed;
-  for (int c = 0; c < n; ++c) {
-    const double e = fabs(reference - row[c]) / reference;
-    if (e > best_err) continue;
-    best = row[c];
-    best_err = e;
+// A candidate row as the lanes of a warp hold it: slot lane + q * WB_LANES in r[q].  nc <= WB_HV_BASE, so the
+// 7 * WB_HV_BASE slots of the widest row fit (one lane of the emulation holds the first WB_HV_ROW slots).
+#define WB_HV_ROW (7 * WB_HV_BASE / 32)
+WB_DEV void hv_row_load(double (&r)[WB_HV_ROW], const double *row, int n) {
+  for (int q = 0; q < WB_HV_ROW; ++q) {
+    const int j = WB_LANE + q * WB_LANES;
+    r[q] = j < n ? row[j] : 0.0;
   }
-  return best;
 }
 
-// ExtendF0 (harvest.cpp:791-822) on one section's window `w` (w[j - lo] = contour at frame j)
+// SelectBestF0 (harvest.cpp:636-650), warp-cooperative on the row held in r: the LAST candidate among those with the
+// smallest error <= allowed.  Each lane folds its slots in ascending order by the reference's rule, the warp keeps
+// the smallest error and, among equal errors, the largest slot.  A NaN error makes the reference's fold take every
+// later slot, so its result is then the row's last slot.
+WB_DEV double hv_select_best(double reference, const double (&r)[WB_HV_ROW], const double *row, int n,
+                             double allowed) {
+  double best = 0.0, best_err = allowed;
+  int best_j = -1;
+  bool nan = false;
+  for (int j = WB_LANE, q = 0; j < n; j += WB_LANES, ++q) {
+    const double c = q < WB_HV_ROW ? r[q] : row[j];
+    const double e = fabs(reference - c) / reference;
+    nan |= e != e;
+    if (e > best_err || e != e) continue;
+    best = c;
+    best_err = e;
+    best_j = j;
+  }
+#ifndef WB_EMU
+  for (int o = 16; o; o >>= 1) {
+    const double e2 = __shfl_xor_sync(0xffffffffu, best_err, o);
+    const int j2 = __shfl_xor_sync(0xffffffffu, best_j, o);
+    if (e2 < best_err || (e2 == best_err && j2 > best_j)) { best_err = e2; best_j = j2; }
+  }
+  best = __shfl_sync(0xffffffffu, best, best_j & 31);
+  nan = __any_sync(0xffffffffu, nan);
+#endif
+  if (nan) return row[n - 1];
+  return best_j < 0 ? 0.0 : best;
+}
+
+// ExtendF0 (harvest.cpp:791-822) on one section's window `w` (w[j - lo] = contour at frame j), run by one warp: every
+// lane takes the same steps, lane 0 writes.  The next step's row is loaded before the current one is reduced.
 WB_DEV int hv_extend(double *w, int lo, int hi, int origin, int last_point, int shift, const double *cand,
                      int max_cand, int n_cand, double allowed) {
   const int threshold = 4;
@@ -694,10 +724,14 @@ WB_DEV int hv_extend(double *w, int lo, int hi, int origin, int last_point, int 
   int shifted_origin = origin;
   const int distance = last_point > origin ? last_point - origin : origin - last_point;
   int count = 0;
+  double cur[WB_HV_ROW], next[WB_HV_ROW];
+  hv_row_load(cur, cand + (size_t)(origin + shift) * max_cand, n_cand);
   for (int i = 0; i <= distance; ++i) {
     const int target = origin + shift * i + shift;
-    const double v = hv_select_best(tmp_f0, cand + (size_t)target * max_cand, n_cand, allowed);
-    if (target >= lo && target <= hi) w[target - lo] = v;
+    const double *row = cand + (size_t)target * max_cand;
+    if (i < distance) hv_row_load(next, cand + (size_t)(target + shift) * max_cand, n_cand);
+    const double v = hv_select_best(tmp_f0, cur, row, n_cand, allowed);
+    if (WB_LANE == 0 && target >= lo && target <= hi) w[target - lo] = v;
     if (v == 0.0) {
       ++count;
     } else {
@@ -706,21 +740,47 @@ WB_DEV int hv_extend(double *w, int lo, int hi, int origin, int last_point, int 
       shifted_origin = target;
     }
     if (count == threshold) break;
+    for (int q = 0; q < WB_HV_ROW; ++q) cur[q] = next[q];
   }
   return shifted_origin;
 }
 
-WB_DEV double hv_search_score(double f0, const double *crow, const double *srow, int n) {
-  double score = 0.0;
-  for (int i = 0; i < n; ++i)
-    if (f0 == crow[i] && score < srow[i]) score = srow[i];
-  return score;
+// SearchScore (harvest.cpp:897-908) of two contour values on one frame's row, warp-cooperative: the largest score
+// of a slot holding the value, starting from +0.0 and replacing only on a strict `<` as the reference does.  A
+// lane's result is +0.0 or a score above it, so the warp's maximum is the reference's value bit for bit.
+WB_DEV void hv_search_scores(double f1, double f2, const double *crow, const double *srow, int n, double *t1,
+                             double *t2) {
+  double s1 = 0.0, s2 = 0.0;
+  for (int i = WB_LANE; i < n; i += WB_LANES) {
+    const double c = crow[i];
+    if (c == f1 && s1 < srow[i]) s1 = srow[i];
+    if (c == f2 && s2 < srow[i]) s2 = srow[i];
+  }
+#ifndef WB_EMU
+  for (int o = 16; o; o >>= 1) {
+    const double a = __shfl_xor_sync(0xffffffffu, s1, o), b = __shfl_xor_sync(0xffffffffu, s2, o);
+    if (s1 < a) s1 = a;
+    if (s2 < b) s2 = b;
+  }
+#endif
+  *t1 = s1;
+  *t2 = s2;
 }
 
+// MergeF0Sub's overlap [st2, ed1] is summed in rounds of this many frames.  Two extensions of at most 101 frames
+// make overlaps of up to about 200 frames, so two rounds are common; the loop takes any length.
+#define WB_HV_TERMS 128
 WB_KERNEL(128, 4) harvest_contour_kernel(HvContourParams p) {
   WB_SHARED int cnt[130];
-  WB_SHARED int sh_nch;
+  WB_SHARED int sh_nch, sh_first;
+  WB_SHARED double terms[2][WB_HV_TERMS];  // MergeF0Sub's SearchScore terms of one round of frames
   const int tid = WB_TID, nth = WB_NTH, u = blockIdx.x;
+#ifdef WB_EMU
+  const int warp = 0, nwarps = 1;
+#else
+  const int warp = tid >> 5, nwarps = nth >> 5;
+#endif
+  const int lane = WB_LANE;
   const int L = p.l1[u], nc7 = p.nc[u] * 7, mcand = p.max_cand;
   const double *cand = p.cand + (size_t)u * p.l1_stride * mcand;
   const double *score = p.score + (size_t)u * p.l1_stride * mcand;
@@ -768,16 +828,21 @@ WB_KERNEL(128, 4) harvest_contour_kernel(HvContourParams p) {
   }
   WB_SYNC();
   if (sh_nch < 0) return;
-  // sections are independent until ExtendSub: one thread per section fills its window and runs
+  // sections are independent until ExtendSub: one warp per section fills its window and runs
   // both ExtendF0 calls (Extend, :858-874)
-  for (int s = tid; s < nsec; s += nth) {
+  for (int s = warp; s < nsec; s += nwarps) {
     const int st = bl[2 * s], ed = bl[2 * s + 1], lo = wlo[s], hi = whi[s];
     double *w = mc + off[s];
-    for (int j = lo; j <= hi; ++j) w[j - lo] = (j >= st && j <= ed) ? s2[j] : 0.0;
+    for (int j = lo + lane; j <= hi; j += WB_LANES) w[j - lo] = (j >= st && j <= ed) ? s2[j] : 0.0;
+#ifndef WB_EMU
+    __syncwarp();
+#endif
     const int new_ed = hv_extend(w, lo, hi, ed, imin(L - 2, ed + 100), 1, cand, mcand, nc7, 0.18);
     const int new_st = hv_extend(w, lo, hi, st, imax(1, st - 100), -1, cand, mcand, nc7, 0.18);
-    bl[2 * s + 1] = new_ed;
-    bl[2 * s] = new_st;
+    if (lane == 0) {
+      bl[2 * s + 1] = new_ed;
+      bl[2 * s] = new_st;
+    }
   }
   WB_SYNC();
   if (tid == 0) {
@@ -810,7 +875,6 @@ WB_KERNEL(128, 4) harvest_contour_kernel(HvContourParams p) {
       const double *w = mc + off[0] - lo;
       for (int i = tid; i < L; i += nth) s3[i] = (i < lo || i > hi) ? 0.0 : w[i];
     }
-    WB_SYNC();
     if (tid == 0) {
       for (int i = 0; i < nch; ++i) order[i] = i;
       // MakeSortedOrder exactly as written in the reference (:881-893): the inner loop keeps
@@ -820,35 +884,49 @@ WB_KERNEL(128, 4) harvest_contour_kernel(HvContourParams p) {
           if (bl[order[j] * 2] > bl[order[i] * 2]) { const int t = order[i]; order[i] = order[j]; order[j] = t; }
           else break;
         }
-      for (int i = 1; i < nch; ++i) {
-        const int o = order[i];
-        const int lo = wlo[o], hi = whi[o];
-        const double *w = mc + off[o] - lo;
-#define WB_CH(j) (((j) < lo || (j) > hi) ? 0.0 : w[(j)])
-        if (bl[o * 2] - bl[1] > 0) {
-          for (int j = bl[o * 2]; j <= bl[o * 2 + 1]; ++j) s3[j] = WB_CH(j);
-          bl[0] = bl[o * 2];
-          bl[1] = bl[o * 2 + 1];
-        } else {
-          // MergeF0Sub (:912-935)
-          const int st1 = bl[0], ed1 = bl[1], st2 = bl[o * 2], ed2 = bl[o * 2 + 1];
-          if (st1 <= st2 && ed1 >= ed2) {
-            bl[1] = ed1;
-          } else {
-            double score1 = 0.0, score2 = 0.0;
-            for (int k = st2; k <= ed1; ++k) {
-              score1 += hv_search_score(s3[k], cand + (size_t)k * mcand, score + (size_t)k * mcand, nc7);
-              score2 += hv_search_score(WB_CH(k), cand + (size_t)k * mcand, score + (size_t)k * mcand, nc7);
-            }
-            if (score1 > score2) { for (int k = ed1; k <= ed2; ++k) s3[k] = WB_CH(k); }
-            else { for (int k = st2; k <= ed2; ++k) s3[k] = WB_CH(k); }
-            bl[1] = ed2;
-          }
-        }
-#undef WB_CH
-      }
     }
     WB_SYNC();
+    // The merged contour's boundaries, boundary_list[0] and [1] of the reference, which updates them in place: every
+    // thread keeps them in registers, and channel 0, should order[i] name it, reads them there.
+    int m_st = bl[0], m_ed = bl[1];
+    for (int i = 1; i < nch; ++i) {
+      const int o = order[i];
+      const int lo = wlo[o], hi = whi[o];
+      const double *w = mc + off[o] - lo;
+      const int st2 = o == 0 ? m_st : bl[o * 2], ed2 = o == 0 ? m_ed : bl[o * 2 + 1];
+#define WB_CH(j) (((j) < lo || (j) > hi) ? 0.0 : w[(j)])
+      int from = st2, to = ed2;  // channel o's frames [from, to] go into the merged contour
+      if (st2 - m_ed > 0) {
+        m_st = st2;
+        m_ed = ed2;
+      } else if (m_st <= st2 && m_ed >= ed2) {  // MergeF0Sub (:912-935) from here on
+        to = from - 1;
+      } else {
+        // SearchScore's terms over [st2, ed1], a round of WB_HV_TERMS frames at a time, one warp per frame; thread 0
+        // sums them in ascending k as the reference does
+        double score1 = 0.0, score2 = 0.0;
+        for (int k0 = st2; k0 <= m_ed; k0 += WB_HV_TERMS) {
+          const int nk = imin(WB_HV_TERMS, m_ed - k0 + 1);
+          for (int r = warp; r < nk; r += nwarps) {
+            const int k = k0 + r;
+            double t1, t2;
+            hv_search_scores(s3[k], WB_CH(k), cand + (size_t)k * mcand, score + (size_t)k * mcand, nc7, &t1, &t2);
+            if (lane == 0) { terms[0][r] = t1; terms[1][r] = t2; }
+          }
+          WB_SYNC();
+          if (tid == 0)
+            for (int r = 0; r < nk; ++r) { score1 += terms[0][r]; score2 += terms[1][r]; }
+          WB_SYNC();
+        }
+        if (tid == 0) sh_first = score1 > score2;
+        WB_SYNC();
+        if (sh_first) from = m_ed;
+        m_ed = ed2;
+      }
+      for (int k = from + tid; k <= to; k += nth) s3[k] = WB_CH(k);
+#undef WB_CH
+      WB_SYNC();
+    }
   }
   // FixStep4 (:1000-1022): bridge gaps shorter than 9 frames
   for (int i = tid; i < L; i += nth) s4[i] = s3[i];
