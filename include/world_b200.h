@@ -408,6 +408,25 @@ int world_b200_analyze_batch_dio_options(WorldB200 *ctx, const double *x, int n_
                                          const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
                                          const DioOption *dio_options, double *time_axis, double *f0,
                                          int f0_stride, double *spectrogram, double *aperiodicity);
+/* ... with per-utterance spectral options, so each speaker's full rows come from the FFT size of its own F0 floor:
+ * cheaptrick_options and d4c_options are HOST arrays of n_utts (either may be NULL: option->cheaptrick / option->d4c
+ * for every utterance), harvest_options / dio_options as above (at most one, of the chain's F0 method, or both NULL).
+ * CheapTrick runs at cheaptrick_options[u].fft_size and D4C at the same size.  spectrogram / aperiodicity are
+ * [n_utts][f0_stride][row_stride] (DEVICE), one stride for both, as in world_b200_cheaptrick_batch_options /
+ * world_b200_d4c_batch_options: row_stride >= every utterance's fft_size / 2 + 1 (0: the largest of them).  Utterance
+ * u writes the first fft_size_u / 2 + 1 values of each of its frames; the rest of each row, and every frame past the
+ * utterance's count, are left untouched.  Each row equals, bit for bit, what world_b200_analyze_batch gives that
+ * utterance with its own options; with equal options and row_stride = fft_size / 2 + 1 the call equals
+ * world_b200_analyze_batch.  Checked before any work is queued (EINVAL, world_b200_last_error() naming the first bad
+ * utterance, outputs untouched): the rules of the stage calls with options, those of the *_options / *_dio_options
+ * chains, and row_stride. */
+int world_b200_analyze_batch_spectral_options(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
+                                              const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                              const HarvestOption *harvest_options, const DioOption *dio_options,
+                                              const CheapTrickOption *cheaptrick_options,
+                                              const D4COption *d4c_options, double *time_axis, double *f0,
+                                              int f0_stride, int row_stride, double *spectrogram,
+                                              double *aperiodicity);
 
 /* ---- multi-GPU: one context per GPU (one process or thread each), utterances sharded over ranks --------------
  * There is no exchange inside the analysis; the one collective reassembles the output arrays on every rank
@@ -449,6 +468,20 @@ int world_b200_analyze_batch_allgather_dio_options(WorldB200 *ctx, const double 
                                                    const DioOption *dio_options, double *time_axis_full,
                                                    double *f0_full, int f0_stride, double *spectrogram_full,
                                                    double *aperiodicity_full);
+/* ... with per-utterance spectral options of THIS rank's shard, as world_b200_analyze_batch_spectral_options: the
+ * full arrays are [n_ranks * n_utts][f0_stride][row_stride].  The shards' largest fft_sizes may differ, so the rows
+ * need one stride for all ranks: every rank passes the same n_utts, f0_stride and row_stride, with row_stride >= the
+ * largest fft_size / 2 + 1 of ALL ranks (0 means this rank's largest, which is only safe when every rank's largest
+ * size is the same).  Collective. */
+int world_b200_analyze_batch_allgather_spectral_options(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
+                                                        const int *x_lengths, int fs,
+                                                        const WorldB200AnalysisOption *option,
+                                                        const HarvestOption *harvest_options,
+                                                        const DioOption *dio_options,
+                                                        const CheapTrickOption *cheaptrick_options,
+                                                        const D4COption *d4c_options, double *time_axis_full,
+                                                        double *f0_full, int f0_stride, int row_stride,
+                                                        double *spectrogram_full, double *aperiodicity_full);
 
 /* {Dio+StoneMask | Harvest} -> CheapTrick -> D4C for n_utts host waveforms; outputs are host
  * arrays laid out as described above.  Input upload, compute and result download are pipelined
@@ -468,6 +501,15 @@ int world_b200_analyze_host_dio_options(WorldB200 *ctx, const double *x, int n_u
                                         const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
                                         const DioOption *dio_options, double *time_axis, double *f0,
                                         int f0_stride, double *spectrogram, double *aperiodicity);
+/* ... with per-utterance spectral options and F0 options as world_b200_analyze_batch_spectral_options, its rows
+ * [n_utts][f0_stride][row_stride] in HOST arrays.  Whole padded rows are downloaded: the values past an utterance's
+ * fft_size / 2 + 1, and the frames past its count, come back as zeros.  Every computed value equals the device call's. */
+int world_b200_analyze_host_spectral_options(WorldB200 *ctx, const double *x, int n_utts, int x_stride,
+                                             const int *x_lengths, int fs, const WorldB200AnalysisOption *option,
+                                             const HarvestOption *harvest_options, const DioOption *dio_options,
+                                             const CheapTrickOption *cheaptrick_options, const D4COption *d4c_options,
+                                             double *time_axis, double *f0, int f0_stride, int row_stride,
+                                             double *spectrogram, double *aperiodicity);
 
 /* The same chain with the ingest and the codec fused in on the device: x holds samples of `nbit`
  * bits (0 = doubles as above; 8/16/24/32 = little-endian PCM as in a WAV data chunk), and the
@@ -568,6 +610,15 @@ int world_b200_analyze_coded_batch_allgather_dio_options(WorldB200 *ctx, const v
                                                          double *time_axis_full, double *f0_full, int f0_stride,
                                                          double *coded_spectral_envelope_full,
                                                          double *coded_aperiodicity_full);
+/* ... with per-utterance spectral options of THIS rank's shard, as world_b200_analyze_coded_batch_spectral_options.
+ * Coded rows do not depend on the size, so the shards' sizes may differ freely; every rank passes the same n_utts,
+ * f0_stride and number_of_dimensions, which must fit every utterance's size on every rank.  Collective. */
+int world_b200_analyze_coded_batch_allgather_spectral_options(
+    WorldB200 *ctx, const void *x, int nbit, int n_utts, int x_stride, const int *x_lengths, int fs,
+    const WorldB200AnalysisOption *option, const HarvestOption *harvest_options, const DioOption *dio_options,
+    const CheapTrickOption *cheaptrick_options, const D4COption *d4c_options, int number_of_dimensions,
+    double *time_axis_full, double *f0_full, int f0_stride, double *coded_spectral_envelope_full,
+    double *coded_aperiodicity_full);
 
 /* ---- voice transformation, PCM in and PCM out: the reference demo's loop (test/test.cpp: Harvest or DIO + StoneMask,
  * CheapTrick, D4C, ParameterModification, Synthesis) over a batch in one call, with one pitch, formant and tempo

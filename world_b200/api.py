@@ -132,6 +132,20 @@ ABI = {
     "world_b200_analyze_batch_allgather_dio_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int,
                                                                  C.POINTER(AnalysisOption), C.POINTER(DioOption), _P,
                                                                  _P, C.c_int, _P, _P]),
+    "world_b200_analyze_batch_spectral_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int,
+                                                            C.POINTER(AnalysisOption), C.POINTER(HarvestOption),
+                                                            C.POINTER(DioOption), C.POINTER(CheapTrickOption),
+                                                            C.POINTER(D4COption), _P, _P, C.c_int, C.c_int, _P, _P]),
+    "world_b200_analyze_host_spectral_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int,
+                                                           C.POINTER(AnalysisOption), C.POINTER(HarvestOption),
+                                                           C.POINTER(DioOption), C.POINTER(CheapTrickOption),
+                                                           C.POINTER(D4COption), _P, _P, C.c_int, C.c_int, _P, _P]),
+    "world_b200_analyze_batch_allgather_spectral_options": (C.c_int, [_P, _P, C.c_int, C.c_int, _IP, C.c_int,
+                                                                      C.POINTER(AnalysisOption),
+                                                                      C.POINTER(HarvestOption), C.POINTER(DioOption),
+                                                                      C.POINTER(CheapTrickOption),
+                                                                      C.POINTER(D4COption), _P, _P, C.c_int, C.c_int,
+                                                                      _P, _P]),
     "world_b200_comm_unique_id": (C.c_int, [_P, C.c_int]),
     "world_b200_comm_init": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int]),
     "world_b200_comm_destroy": (C.c_int, [_P]),
@@ -194,6 +208,13 @@ ABI = {
                                                                        C.c_int, C.POINTER(AnalysisOption),
                                                                        C.POINTER(DioOption), C.c_int, _P, _P, C.c_int,
                                                                        _P, _P]),
+    "world_b200_analyze_coded_batch_allgather_spectral_options": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP,
+                                                                            C.c_int, C.POINTER(AnalysisOption),
+                                                                            C.POINTER(HarvestOption),
+                                                                            C.POINTER(DioOption),
+                                                                            C.POINTER(CheapTrickOption),
+                                                                            C.POINTER(D4COption), C.c_int, _P, _P,
+                                                                            C.c_int, _P, _P]),
     "world_b200_transform_samples": (C.c_int, [C.c_int, C.c_int, C.c_double, C.c_double]),
     "world_b200_transform_batch": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _IP, C.c_int, C.POINTER(AnalysisOption),
                                              C.POINTER(HarvestOption), C.POINTER(DioOption), _P, _P, _P, C.c_int, _P,
@@ -318,6 +339,25 @@ def _chain_options(harvest_options, dio_options, n):
     return _harvest_options(harvest_options, n), _dio_options(dio_options, n)
 
 
+def _full_bins(option, cheaptrick_options):
+    """Values per frame of the full rows a chain allocates: the largest fft_size // 2 + 1 of cheaptrick_options, or
+    option's with one CheapTrick option."""
+    sizes = [o.fft_size for o in cheaptrick_options or []] or [option.cheaptrick.fft_size]
+    return max(sizes) // 2 + 1
+
+
+def _row_stride(spectrogram, aperiodicity):
+    """The row_stride of a full-row chain with per-utterance spectral options: the last dimension of its spectrogram
+    and aperiodicity arrays (the same for both; one may be None, not both)."""
+    widths = {int(a.shape[-1]) for a in (spectrogram, aperiodicity) if a is not None}
+    if not widths:
+        raise ValueError("per-utterance spectral options need the spectrogram or aperiodicity array: its last "
+                         "dimension is the row_stride")
+    if len(widths) > 1:
+        raise ValueError(f"spectrogram and aperiodicity share one row_stride, not {sorted(widths)}")
+    return widths.pop()
+
+
 def _frame_period(option):
     """The frame period of an AnalysisOption's F0 method."""
     return option.dio.frame_period if option.f0_method == F0_DIO_STONEMASK else option.harvest.frame_period
@@ -398,16 +438,19 @@ class World:
             raise WorldError(f"world_b200 error {rc}: {self.lib.world_b200_last_error(self._h).decode()}")
 
     def _chain(self, family, head, n, harvest_options, dio_options, outs, cheaptrick_options=None, d4c_options=None,
-               device=False):
+               device=False, rows=None):
         """Calls the analysis chain world_b200_<family> whose variant fits the per-utterance option lists given
         (_options: Harvest, _dio_options: DIO, _spectral_options: CheapTrick / D4C, with either F0 list).  head: the
-        arguments between the handle and the option arrays; outs: those after them.  device: the chain is enqueued on
-        torch's current stream."""
+        arguments between the handle and the option arrays; outs: those after them.  rows: the (spectrogram,
+        aperiodicity) arrays of a full-row chain, whose _spectral_options variant takes their last dimension as the
+        row_stride after f0_stride.  device: the chain is enqueued on torch's current stream."""
         per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
         if cheaptrick_options is not None or d4c_options is not None:
             ct = None if cheaptrick_options is None else _option_array(CheapTrickOption, cheaptrick_options, n)
             d4 = None if d4c_options is None else _option_array(D4COption, d4c_options, n)
             suffix, arrays = "_spectral_options", (per_utt, per_dio, ct, d4)
+            if rows is not None:
+                outs = (*outs[:3], _row_stride(*rows), *outs[3:])
         elif per_utt is not None:
             suffix, arrays = "_options", (per_utt,)
         elif per_dio is not None:
@@ -762,14 +805,19 @@ class World:
         return o
 
     def analyze_batch(self, x, fs, option: AnalysisOption, x_lengths=None, time_axis=None, f0=None,
-                      spectrogram=None, aperiodicity=None, harvest_options=None, dio_options=None):
+                      spectrogram=None, aperiodicity=None, harvest_options=None, dio_options=None,
+                      cheaptrick_options=None, d4c_options=None):
         """Whole chain on DEVICE arrays in one call (two internal streams); returns (t, f0, sp, ap, frame counts).
         harvest_options: a list of one HarvestOption per utterance (Harvest with a per-utterance F0 range);
-        dio_options: a list of one DioOption per utterance (DIO + StoneMask with a per-utterance F0 range)."""
+        dio_options: a list of one DioOption per utterance (DIO + StoneMask with a per-utterance F0 range).
+        cheaptrick_options / d4c_options: a list of one CheapTrickOption / D4COption per utterance
+        (world_b200_analyze_batch_spectral_options; D4C runs at each utterance's CheapTrick fft_size).  The rows are
+        then [n, L, row_stride] with row_stride the last dimension of spectrogram (allocated as max fft_size // 2 + 1
+        when None), and utterance u writes the first fft_size[u] // 2 + 1 values of each of its frames."""
         n, stride = x.shape
         frame_period = _frame_period(option)
         f_stride, fl = self._f0_stride(fs, x, x_lengths, frame_period)
-        bins = option.cheaptrick.fft_size // 2 + 1
+        bins = _full_bins(option, cheaptrick_options)
         if time_axis is None:
             time_axis = self._zeros(x, (n, f_stride))
         if f0 is None:
@@ -780,7 +828,9 @@ class World:
             aperiodicity = self._zeros(x, (n, f_stride, bins))
         xl, keep = _int_array(x_lengths, n)
         self._chain("analyze_batch", (_ptr(x), n, stride, xl, fs, C.byref(option)), n, harvest_options, dio_options,
-                    (_ptr(time_axis), _ptr(f0), time_axis.shape[1], _ptr(spectrogram), _ptr(aperiodicity)), device=True)
+                    (_ptr(time_axis), _ptr(f0), time_axis.shape[1], _ptr(spectrogram), _ptr(aperiodicity)),
+                    cheaptrick_options=cheaptrick_options, d4c_options=d4c_options, device=True,
+                    rows=(spectrogram, aperiodicity))
         return time_axis, f0, spectrogram, aperiodicity, fl
 
     # -- multi-GPU: one World per GPU / process; the NCCL id travels by the caller's own means -------------------
@@ -808,29 +858,37 @@ class World:
         return full
 
     def analyze_batch_allgather(self, x, fs, option: AnalysisOption, time_axis_full, f0_full, spectrogram_full,
-                                aperiodicity_full, x_lengths=None, harvest_options=None, dio_options=None):
+                                aperiodicity_full, x_lengths=None, harvest_options=None, dio_options=None,
+                                cheaptrick_options=None, d4c_options=None):
         """analyze_batch on this rank's shard with every finished slice broadcast into the FULL arrays of all ranks.
-        harvest_options / dio_options: a list of one option per utterance of THIS rank's shard."""
+        harvest_options / dio_options: a list of one option per utterance of THIS rank's shard.
+        cheaptrick_options / d4c_options: the same for the spectral options
+        (world_b200_analyze_batch_allgather_spectral_options).  The shards' largest sizes may differ, so the row_stride
+        is the last dimension of the full arrays, which every rank allocates alike; ValueError when both are None."""
         n, stride = x.shape
         xl, keep = _int_array(x_lengths, n)
         outs = (_ptr(time_axis_full), _ptr(f0_full), time_axis_full.shape[1],
                 _ptr(spectrogram_full) if spectrogram_full is not None else None,
                 _ptr(aperiodicity_full) if aperiodicity_full is not None else None)
         self._chain("analyze_batch_allgather", (_ptr(x), n, stride, xl, fs, C.byref(option)), n, harvest_options,
-                    dio_options, outs, device=True)
+                    dio_options, outs, cheaptrick_options=cheaptrick_options, d4c_options=d4c_options, device=True,
+                    rows=(spectrogram_full, aperiodicity_full))
 
     def analyze_host(self, x_host, fs, option: AnalysisOption, x_lengths=None, time_axis=None, f0=None,
-                     spectrogram=None, aperiodicity=None, f0_stride=None, harvest_options=None, dio_options=None):
+                     spectrogram=None, aperiodicity=None, f0_stride=None, harvest_options=None, dio_options=None,
+                     cheaptrick_options=None, d4c_options=None):
         """Whole chain on HOST arrays (numpy or pinned torch CPU tensors); outputs are written
         into the given host arrays (allocated with numpy when None).  harvest_options / dio_options: a list of
-        one option per utterance of the chain's F0 method."""
+        one option per utterance of the chain's F0 method.  cheaptrick_options / d4c_options: as for analyze_batch
+        (world_b200_analyze_host_spectral_options); whole padded rows come back, 0 past each utterance's
+        fft_size // 2 + 1 values and past its frames."""
         import numpy as np
         n, stride = x_host.shape
         frame_period = _frame_period(option)
         lens = [stride] * n if x_lengths is None else [int(v) for v in x_lengths]
         fl = [self.frames(fs, v, frame_period) for v in lens]
         f0_stride = f0_stride or max(fl)
-        bins = option.cheaptrick.fft_size // 2 + 1
+        bins = _full_bins(option, cheaptrick_options)
         if time_axis is None:
             time_axis = np.zeros((n, f0_stride))
         if f0 is None:
@@ -841,7 +899,8 @@ class World:
             aperiodicity = np.zeros((n, f0_stride, bins))
         xl, keep = _int_array(x_lengths, n)
         self._chain("analyze_host", (_ptr(x_host), n, stride, xl, fs, C.byref(option)), n, harvest_options,
-                    dio_options, (_ptr(time_axis), _ptr(f0), f0_stride, _ptr(spectrogram), _ptr(aperiodicity)))
+                    dio_options, (_ptr(time_axis), _ptr(f0), f0_stride, _ptr(spectrogram), _ptr(aperiodicity)),
+                    cheaptrick_options=cheaptrick_options, d4c_options=d4c_options, rows=(spectrogram, aperiodicity))
         return time_axis, f0, spectrogram, aperiodicity, fl
 
     # -- codec (codec.h) and ingest ----------------------------------------------------------
@@ -1051,13 +1110,14 @@ class World:
 
     def analyze_coded_batch_allgather(self, x, nbit, fs, option: AnalysisOption, number_of_dimensions, time_axis_full,
                                       f0_full, coded_sp_full, coded_ap_full, x_lengths=None, harvest_options=None,
-                                      dio_options=None):
+                                      dio_options=None, cheaptrick_options=None, d4c_options=None):
         """analyze_coded_batch on this rank's shard with every finished slice sent into the FULL arrays of all ranks
         (the coded rows are what crosses between GPUs).  coded_sp_full / coded_ap_full may be None to skip CheapTrick /
-        D4C.  harvest_options / dio_options: a list of one option per utterance of THIS rank's shard."""
+        D4C.  harvest_options / dio_options / cheaptrick_options / d4c_options: a list of one option per utterance of
+        THIS rank's shard (world_b200_analyze_coded_batch_allgather_spectral_options for the spectral ones)."""
         n, stride, _ = self._coded_rows(x, nbit, option)
         xl, keep = _int_array(x_lengths, n)
         self._chain("analyze_coded_batch_allgather", (_ptr(x), nbit, n, stride, xl, fs, C.byref(option)), n,
                     harvest_options, dio_options, (number_of_dimensions, _ptr(time_axis_full), _ptr(f0_full),
                                                    time_axis_full.shape[1], _ptr(coded_sp_full), _ptr(coded_ap_full)),
-                    device=True)
+                    cheaptrick_options=cheaptrick_options, d4c_options=d4c_options, device=True)

@@ -601,6 +601,7 @@ static int chain_checks(Ctx *c, const ChainRequest &r, ChainPlan *p) {
     return fail("x and option must be given, with n_utts >= 0, fs > 0 and positive strides");
   if (r.nbit != 0 && r.nbit != 8 && r.nbit != 16 && r.nbit != 24 && r.nbit != 32)
     return fail("nbit must be 0, 8, 16, 24 or 32");
+  if (r.row_stride < 0) return fail("row_stride must be >= 0");
   const int n = r.n, fft_size = opt->cheaptrick.fft_size;
   const bool spectral_options = r.cheaptrick_options || r.d4c_options;
   if ((r.spectrogram || r.aperiodicity) && fft_size < 16) return fail("CheapTrick: fft_size must be at least 16");
@@ -645,6 +646,7 @@ static int chain_checks(Ctx *c, const ChainRequest &r, ChainPlan *p) {
   StageRequest s{STAGE_CHEAPTRICK, n, r.x_stride, r.x_lengths, r.fs, p->f_len.data(), p->f0_stride};
   s.ct = &opt->cheaptrick; s.fft_size = &opt->cheaptrick.fft_size; s.d4c = &opt->d4c;
   s.coded = r.coded; s.dims = r.dims;
+  s.row_stride = r.coded ? 0 : r.row_stride;   // the stage plans check it against every utterance's size
   std::vector<CheapTrickOption> cts;
   std::vector<D4COption> d4s;
   std::vector<int> d4_fft;
@@ -655,8 +657,9 @@ static int chain_checks(Ctx *c, const ChainRequest &r, ChainPlan *p) {
     if (r.d4c_options) std::copy(r.d4c_options, r.d4c_options + n, d4s.begin());
     for (const CheapTrickOption &o : cts) d4_fft.push_back(o.fft_size);
     s.per_utt = true; s.ct = cts.data(); s.fft_size = d4_fft.data(); s.d4c = d4s.data();
-    // full rows (a transform's): every utterance's row as wide as the largest size's
-    for (const int f : d4_fft) s.row_stride = r.coded ? 0 : imax(s.row_stride, f / 2 + 1);
+    // full rows without a caller's stride (a transform's): every utterance's row as wide as the largest size's
+    if (!r.coded && !r.row_stride)
+      for (const int f : d4_fft) s.row_stride = imax(s.row_stride, f / 2 + 1);
   }
   if ((r.spectrogram || transform) && (rc = stage_plan(c, s, &p->ct))) return rc;
   s.stage = STAGE_D4C;
@@ -664,7 +667,7 @@ static int chain_checks(Ctx *c, const ChainRequest &r, ChainPlan *p) {
   s.stage = STAGE_STONEMASK;
   StagePlan stonemask;
   if (!harvest && (rc = stage_plan(c, s, &stonemask))) return rc;
-  const size_t full_row = spectral_options ? (size_t)s.row_stride : (size_t)(fft_size / 2 + 1);
+  const size_t full_row = s.row_stride ? (size_t)s.row_stride : (size_t)(fft_size / 2 + 1);
   p->sp_row = r.coded ? (size_t)r.dims : full_row;
   p->ap_row = r.coded ? (size_t)GetNumberOfAperiodicities(r.fs) : full_row;
   p->want_sp = r.spectrogram != nullptr;
@@ -1017,6 +1020,18 @@ int world_b200_analyze_batch_dio_options(WorldB200 *h, const double *x, int n, i
   return analyze_chain(h, r, false);
 }
 
+int world_b200_analyze_batch_spectral_options(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths,
+                                              int fs, const WorldB200AnalysisOption *opt,
+                                              const HarvestOption *harvest_options, const DioOption *dio_options,
+                                              const CheapTrickOption *cheaptrick_options, const D4COption *d4c_options,
+                                              double *time_axis, double *f0, int f0_stride, int row_stride,
+                                              double *spectrogram, double *aperiodicity) {
+  ChainRequest r(x, 0, n, x_stride, x_lengths, fs, opt, time_axis, f0, f0_stride, spectrogram, aperiodicity);
+  r.harvest_options = harvest_options; r.dio_options = dio_options;
+  r.cheaptrick_options = cheaptrick_options; r.d4c_options = d4c_options; r.row_stride = row_stride;
+  return analyze_chain(h, r, false);
+}
+
 }  // extern "C"
 
 // ---- voice transformation: analysis, modification and synthesis in one call (world_b200_transform_*)
@@ -1256,6 +1271,18 @@ int world_b200_analyze_batch_allgather_dio_options(WorldB200 *h, const double *x
   return analyze_chain(h, r, true);
 }
 
+int world_b200_analyze_batch_allgather_spectral_options(
+    WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs, const WorldB200AnalysisOption *opt,
+    const HarvestOption *harvest_options, const DioOption *dio_options, const CheapTrickOption *cheaptrick_options,
+    const D4COption *d4c_options, double *time_axis_full, double *f0_full, int f0_stride, int row_stride,
+    double *spectrogram_full, double *aperiodicity_full) {
+  ChainRequest r(x, 0, n, x_stride, x_lengths, fs, opt, time_axis_full, f0_full, f0_stride, spectrogram_full,
+                 aperiodicity_full);
+  r.harvest_options = harvest_options; r.dio_options = dio_options;
+  r.cheaptrick_options = cheaptrick_options; r.d4c_options = d4c_options; r.row_stride = row_stride;
+  return analyze_chain(h, r, true);
+}
+
 // The device chain with coded rows out (and PCM or doubles in): analyze_chain with the fused coded frame kernels.
 int world_b200_analyze_coded_batch(WorldB200 *h, const void *x, int nbit, int n, int x_stride, const int *x_lengths,
                                    int fs, const WorldB200AnalysisOption *opt, int number_of_dimensions,
@@ -1336,6 +1363,19 @@ int world_b200_analyze_coded_batch_allgather_dio_options(WorldB200 *h, const voi
   ChainRequest r = coded_request(x, nbit, n, x_stride, x_lengths, fs, opt, number_of_dimensions, time_axis_full,
                                  f0_full, f0_stride, coded_spectral_envelope_full, coded_aperiodicity_full);
   r.dio_options = dio_options;
+  return analyze_chain(h, r, true);
+}
+
+int world_b200_analyze_coded_batch_allgather_spectral_options(
+    WorldB200 *h, const void *x, int nbit, int n, int x_stride, const int *x_lengths, int fs,
+    const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options, const DioOption *dio_options,
+    const CheapTrickOption *cheaptrick_options, const D4COption *d4c_options, int number_of_dimensions,
+    double *time_axis_full, double *f0_full, int f0_stride, double *coded_spectral_envelope_full,
+    double *coded_aperiodicity_full) {
+  ChainRequest r = coded_request(x, nbit, n, x_stride, x_lengths, fs, opt, number_of_dimensions, time_axis_full,
+                                 f0_full, f0_stride, coded_spectral_envelope_full, coded_aperiodicity_full);
+  r.harvest_options = harvest_options; r.dio_options = dio_options;
+  r.cheaptrick_options = cheaptrick_options; r.d4c_options = d4c_options;
   return analyze_chain(h, r, true);
 }
 

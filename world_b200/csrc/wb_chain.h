@@ -25,7 +25,8 @@ namespace wb {
 // F0 arrays, and the spectral arrays only with coded rows.  coded: spectrogram / aperiodicity receive dims /
 // GetNumberOfAperiodicities(fs) coded values per frame instead of fft_size / 2 + 1 bins.  A NULL spectrogram or
 // aperiodicity skips its stage.  f0_stride 0: a call with no analysis outputs (transform), whose rows are as long as its
-// longest utterance's frame count.
+// longest utterance's frame count.  row_stride: doubles per frame of full rows, at least every utterance's
+// fft_size / 2 + 1; 0 for fft_size / 2 + 1 with one option, or the largest size's with per-utterance options.
 struct ChainRequest {
   ChainRequest(const void *x, int nbit, int n, int x_stride, const int *x_lengths, int fs,
                const WorldB200AnalysisOption *opt, double *time_axis, double *f0, int f0_stride, double *spectrogram,
@@ -46,6 +47,7 @@ struct ChainRequest {
   const DioOption *dio_options = nullptr;
   const CheapTrickOption *cheaptrick_options = nullptr;
   const D4COption *d4c_options = nullptr;
+  int row_stride = 0;
 };
 
 // The request of a coded-row entry point: number_of_dimensions coded values per spectral frame.

@@ -219,6 +219,7 @@ int analyze_pipeline(WorldB200 *h, const ChainRequest &r) {
   const size_t in_bytes = nbit ? (size_t)(nbit / 8) : 8;
   const size_t sp_row = plan.sp_row, ap_row = plan.ap_row;
   const bool want_sp = plan.want_sp, want_ap = plan.want_ap;
+  const StagePlan &sizes = want_sp ? plan.ct : plan.d4;   // each utterance's fft_size (D4C runs at CheapTrick's)
   double *time_axis = r.time_axis, *f0 = r.f0, *out_sp = r.spectrogram, *out_ap = r.aperiodicity;
 
   int sub = 128, outer = 512;
@@ -303,9 +304,11 @@ int analyze_pipeline(WorldB200 *h, const ChainRequest &r) {
       const size_t ssz = (size_t)m * f0_stride;
       const double *sx = xd + (size_t)v0 * x_stride, *st = dt[s] + (size_t)v0 * f0_stride, *sf = df[s] + (size_t)v0 * f0_stride;
       if (g >= ring) p.wait(HostPipe::RUN, ev_sub_out + slot);   // the slot's previous rows are on the host
-      // whole padded rows are downloaded: frames beyond an utterance's length read as zero on the host
+      // whole padded rows are downloaded: frames beyond an utterance's length, and full-row values beyond its
+      // fft_size / 2 + 1 (per-utterance sizes, or a wider row_stride), read as zero on the host
       bool ragged = false;
-      for (int i = 0; i < m; ++i) ragged = ragged || sfl[i] != f0_stride;
+      for (int i = 0; i < m; ++i)
+        ragged = ragged || sfl[i] != f0_stride || (!r.coded && (size_t)(sizes.fft_size[u0 + v0 + i] / 2 + 1) != sp_row);
       if (ragged) {
         if (want_sp) dev_memset(ctx, dsp[slot], 0, ssz * sp_row * 8);
         if (want_ap) dev_memset(ctx, dap[slot], 0, ssz * ap_row * 8);
@@ -555,6 +558,19 @@ extern "C" int world_b200_analyze_host_dio_options(WorldB200 *h, const double *x
   if (!dio_options) return WORLD_B200_EINVAL;
   ChainRequest r(x, 0, n_utts, x_stride, x_lengths, fs, opt, time_axis, f0, f0_stride, spectrogram, aperiodicity);
   r.dio_options = dio_options;
+  return analyze_pipeline(h, r);
+}
+
+// analyze_host with per-utterance CheapTrick / D4C options (either array may be NULL), F0 options as above, and full
+// rows of row_stride doubles per frame
+extern "C" int world_b200_analyze_host_spectral_options(
+    WorldB200 *h, const double *x, int n_utts, int x_stride, const int *x_lengths, int fs,
+    const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options, const DioOption *dio_options,
+    const CheapTrickOption *cheaptrick_options, const D4COption *d4c_options, double *time_axis, double *f0,
+    int f0_stride, int row_stride, double *spectrogram, double *aperiodicity) {
+  ChainRequest r(x, 0, n_utts, x_stride, x_lengths, fs, opt, time_axis, f0, f0_stride, spectrogram, aperiodicity);
+  r.harvest_options = harvest_options; r.dio_options = dio_options;
+  r.cheaptrick_options = cheaptrick_options; r.d4c_options = d4c_options; r.row_stride = row_stride;
   return analyze_pipeline(h, r);
 }
 
