@@ -620,6 +620,52 @@ int world_b200_analyze_coded_batch_allgather_spectral_options(
     double *time_axis_full, double *f0_full, int f0_stride, double *coded_spectral_envelope_full,
     double *coded_aperiodicity_full);
 
+/* ---- packed batches: utterances back to back, no padding ----------------------------------------------------------
+ * x_offsets: a HOST array of n_utts + 1 sample offsets, x_offsets[0] == 0: utterance u is samples
+ * [x_offsets[u], x_offsets[u + 1]) of x (with PCM input, byte offset = sample offset * nbit / 8).  Each utterance is
+ * 1 .. INT_MAX samples long.  Its frames follow on from the previous utterance's:
+ *   f_offsets[0] = 0, f_offsets[u + 1] = f_offsets[u] + world_b200_frames(fs, len_u, frame_period),
+ * frame_period being the chain's F0 method's, and F = f_offsets[n_utts] frames in all.  time_axis and f0 are [F];
+ * full rows are [F][row_stride] (row_stride >= every utterance's fft_size / 2 + 1; 0: the largest); coded rows
+ * [F][number_of_dimensions] and [F][GetNumberOfAperiodicities(fs)]. */
+/* f_offsets (HOST, n_utts + 1) of a packed batch, to size its outputs before the call.  EINVAL for bad offsets. */
+int world_b200_packed_frames(int fs, int n_utts, const long long *x_offsets, double frame_period,
+                             long long *f_offsets);
+/* world_b200_analyze_batch_spectral_options on a packed batch (DEVICE arrays).  Every utterance's time axis, f0 and
+ * rows equal, bit for bit, what the padded call gives it with the same options.  Nothing is written outside frames
+ * [0, F), nor past an utterance's fft_size / 2 + 1 in a full row.  f_offsets (HOST, n_utts + 1, may be NULL) receives
+ * the frame offsets.  Checked before any work is queued: the padded call's rules and the offset rules (EINVAL,
+ * world_b200_last_error() naming the first bad utterance, outputs untouched).  n_utts == 0 writes f_offsets[0] = 0. */
+int world_b200_analyze_packed(WorldB200 *ctx, const double *x, int n_utts, const long long *x_offsets, int fs,
+                              const WorldB200AnalysisOption *option, const HarvestOption *harvest_options,
+                              const DioOption *dio_options, const CheapTrickOption *cheaptrick_options,
+                              const D4COption *d4c_options, double *time_axis, double *f0, int row_stride,
+                              double *spectrogram, double *aperiodicity, long long *f_offsets);
+/* world_b200_analyze_coded_batch_spectral_options on a packed batch of nbit 0/8/16/24/32 samples (DEVICE arrays),
+ * as world_b200_analyze_packed. */
+int world_b200_analyze_coded_packed(WorldB200 *ctx, const void *x, int nbit, int n_utts, const long long *x_offsets,
+                                    int fs, const WorldB200AnalysisOption *option,
+                                    const HarvestOption *harvest_options, const DioOption *dio_options,
+                                    const CheapTrickOption *cheaptrick_options, const D4COption *d4c_options,
+                                    int number_of_dimensions, double *time_axis, double *f0,
+                                    double *coded_spectral_envelope, double *coded_aperiodicity,
+                                    long long *f_offsets);
+/* The same two chains for HOST arrays.  Each chunk of utterances goes up as one contiguous copy of its samples and
+ * comes back as one contiguous copy per output array; no padding crosses PCIe.  Exactly F frames are written, and full
+ * rows read 0 past an utterance's fft_size / 2 + 1.  time_axis and f0 may be NULL (not downloaded). */
+int world_b200_analyze_host_packed(WorldB200 *ctx, const double *x, int n_utts, const long long *x_offsets, int fs,
+                                   const WorldB200AnalysisOption *option, const HarvestOption *harvest_options,
+                                   const DioOption *dio_options, const CheapTrickOption *cheaptrick_options,
+                                   const D4COption *d4c_options, double *time_axis, double *f0, int row_stride,
+                                   double *spectrogram, double *aperiodicity, long long *f_offsets);
+int world_b200_analyze_coded_host_packed(WorldB200 *ctx, const void *x, int nbit, int n_utts,
+                                         const long long *x_offsets, int fs, const WorldB200AnalysisOption *option,
+                                         const HarvestOption *harvest_options, const DioOption *dio_options,
+                                         const CheapTrickOption *cheaptrick_options, const D4COption *d4c_options,
+                                         int number_of_dimensions, double *time_axis, double *f0,
+                                         double *coded_spectral_envelope, double *coded_aperiodicity,
+                                         long long *f_offsets);
+
 /* ---- voice transformation, PCM in and PCM out: the reference demo's loop (test/test.cpp: Harvest or DIO + StoneMask,
  * CheapTrick, D4C, ParameterModification, Synthesis) over a batch in one call, with one pitch, formant and tempo
  * factor per utterance ----------------------------------------------------------------------------------------------

@@ -47,6 +47,7 @@ F0_HARVEST = 1
 
 _P = C.c_void_p
 _IP = C.POINTER(C.c_int)
+_LP = C.POINTER(C.c_longlong)
 
 # every symbol include/world_b200.h and include/world/*.h declare: (restype, argtypes)
 ABI = {
@@ -146,6 +147,24 @@ ABI = {
                                                                       C.POINTER(CheapTrickOption),
                                                                       C.POINTER(D4COption), _P, _P, C.c_int, C.c_int,
                                                                       _P, _P]),
+    # packed batches: x_offsets / f_offsets are n + 1 64-bit offsets
+    "world_b200_packed_frames": (C.c_int, [C.c_int, C.c_int, _LP, C.c_double, _LP]),
+    "world_b200_analyze_packed": (C.c_int, [_P, _P, C.c_int, _LP, C.c_int, C.POINTER(AnalysisOption),
+                                            C.POINTER(HarvestOption), C.POINTER(DioOption),
+                                            C.POINTER(CheapTrickOption), C.POINTER(D4COption), _P, _P, C.c_int, _P,
+                                            _P, _LP]),
+    "world_b200_analyze_host_packed": (C.c_int, [_P, _P, C.c_int, _LP, C.c_int, C.POINTER(AnalysisOption),
+                                                 C.POINTER(HarvestOption), C.POINTER(DioOption),
+                                                 C.POINTER(CheapTrickOption), C.POINTER(D4COption), _P, _P, C.c_int,
+                                                 _P, _P, _LP]),
+    "world_b200_analyze_coded_packed": (C.c_int, [_P, _P, C.c_int, C.c_int, _LP, C.c_int, C.POINTER(AnalysisOption),
+                                                  C.POINTER(HarvestOption), C.POINTER(DioOption),
+                                                  C.POINTER(CheapTrickOption), C.POINTER(D4COption), C.c_int, _P, _P,
+                                                  _P, _P, _LP]),
+    "world_b200_analyze_coded_host_packed": (C.c_int, [_P, _P, C.c_int, C.c_int, _LP, C.c_int,
+                                                       C.POINTER(AnalysisOption), C.POINTER(HarvestOption),
+                                                       C.POINTER(DioOption), C.POINTER(CheapTrickOption),
+                                                       C.POINTER(D4COption), C.c_int, _P, _P, _P, _P, _LP]),
     "world_b200_comm_unique_id": (C.c_int, [_P, C.c_int]),
     "world_b200_comm_init": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int]),
     "world_b200_comm_destroy": (C.c_int, [_P]),
@@ -385,6 +404,16 @@ def _factors(v, n, what):
     if len(v) != n:
         raise ValueError(f"{what}: {len(v)} factors for {n} utterances")
     return (C.c_double * n)(*v)
+
+
+def _offsets(x_offsets):
+    """n + 1 sample offsets (a list, numpy array or CPU tensor) -> (n, ctypes int64 array)."""
+    if hasattr(x_offsets, "tolist"):
+        x_offsets = x_offsets.tolist()
+    v = [int(t) for t in x_offsets]
+    if not v:
+        raise ValueError("x_offsets needs n_utts + 1 entries")
+    return len(v) - 1, (C.c_longlong * len(v))(*v)
 
 
 def _int_array(v, n):
@@ -832,6 +861,94 @@ class World:
                     cheaptrick_options=cheaptrick_options, d4c_options=d4c_options, device=True,
                     rows=(spectrogram, aperiodicity))
         return time_axis, f0, spectrogram, aperiodicity, fl
+
+    # -- packed batches: utterances back to back, utterance u = samples [x_offsets[u], x_offsets[u + 1]) --------
+    def packed_frames(self, fs, x_offsets, frame_period=5.0):
+        """The frame offsets of a packed batch (numpy int64, n + 1): utterance u's frames are rows
+        [f[u], f[u + 1]) of the packed outputs, f[n] = F in all."""
+        import numpy as np
+        n, xo = _offsets(x_offsets)
+        f = (C.c_longlong * (n + 1))()
+        rc = self.lib.world_b200_packed_frames(fs, n, xo, frame_period, f)
+        if rc:
+            raise WorldError(f"world_b200_packed_frames: bad x_offsets or arguments (code {rc})")
+        return np.array(f[:], dtype=np.int64)
+
+    def _packed(self, name, x, head, x_offsets, fs, option, mid, widths, outs, harvest_options, dio_options,
+                cheaptrick_options, d4c_options, device):
+        """Calls world_b200_<name> on a packed batch: head = the arguments before n_utts, mid = those between the
+        option arrays and the output arrays; outs = (time_axis, f0, spectrogram, aperiodicity), each allocated when
+        None with F frames of widths (0: [F]); full rows pass row_stride (widths' row) after f0.  Returns the outputs
+        and the frame offsets."""
+        import numpy as np
+        n, xo = _offsets(x_offsets)
+        per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
+        ct = None if cheaptrick_options is None else _option_array(CheapTrickOption, cheaptrick_options, n)
+        d4 = None if d4c_options is None else _option_array(D4COption, d4c_options, n)
+        outs = list(outs)
+        for i, w in enumerate(widths):
+            if outs[i] is None:
+                F = int(self.packed_frames(fs, x_offsets, _frame_period(option))[-1])
+                shape = (F, w) if w else (F,)
+                outs[i] = self._zeros(x, shape) if device else np.zeros(shape)
+        f = (C.c_longlong * (n + 1))()
+        args = [_ptr(outs[0]), _ptr(outs[1])]
+        if mid is None:   # full rows: the row_stride of the arrays
+            args.append(_row_stride(outs[2], outs[3]))
+        args += [_ptr(outs[2]), _ptr(outs[3]), f]
+        if device:
+            self._use_current_stream()
+        self._check(getattr(self.lib, f"world_b200_{name}")(self._h, _ptr(x), *head, n, xo, fs, C.byref(option),
+                                                             per_utt, per_dio, ct, d4, *([] if mid is None else mid),
+                                                             *args))
+        return (*outs, np.array(f[:], dtype=np.int64))
+
+    def analyze_packed(self, x, x_offsets, fs, option: AnalysisOption, harvest_options=None, dio_options=None,
+                       cheaptrick_options=None, d4c_options=None, row_stride=0, time_axis=None, f0=None,
+                       spectrogram=None, aperiodicity=None):
+        """analyze_batch on a PACKED batch of DEVICE float64 samples (world_b200_analyze_packed): x holds the
+        utterances back to back, utterance u being samples [x_offsets[u], x_offsets[u + 1]) (x_offsets: n + 1
+        offsets, a list, numpy array or CPU tensor).  Returns (time_axis [F], f0 [F], spectrogram [F, W],
+        aperiodicity [F, W], f_offsets [n + 1]): utterance u's frames are rows [f_offsets[u], f_offsets[u + 1]).
+        W = row_stride, or the largest fft_size // 2 + 1 when 0; given arrays set W by their last dimension.  Each
+        utterance's values equal analyze_batch's, bit for bit; the rest of each row is not written."""
+        W = row_stride or (_row_stride(spectrogram, aperiodicity) if spectrogram is not None or aperiodicity is not None
+                           else _full_bins(option, cheaptrick_options))
+        return self._packed("analyze_packed", x, (), x_offsets, fs, option, None, (0, 0, W, W),
+                            (time_axis, f0, spectrogram, aperiodicity), harvest_options, dio_options,
+                            cheaptrick_options, d4c_options, device=True)
+
+    def analyze_host_packed(self, x_host, x_offsets, fs, option: AnalysisOption, harvest_options=None,
+                            dio_options=None, cheaptrick_options=None, d4c_options=None, row_stride=0, time_axis=None,
+                            f0=None, spectrogram=None, aperiodicity=None):
+        """analyze_packed on HOST arrays (world_b200_analyze_host_packed), outputs allocated with numpy when None;
+        full rows read 0 past each utterance's fft_size // 2 + 1."""
+        W = row_stride or (_row_stride(spectrogram, aperiodicity) if spectrogram is not None or aperiodicity is not None
+                           else _full_bins(option, cheaptrick_options))
+        return self._packed("analyze_host_packed", x_host, (), x_offsets, fs, option, None, (0, 0, W, W),
+                            (time_axis, f0, spectrogram, aperiodicity), harvest_options, dio_options,
+                            cheaptrick_options, d4c_options, device=False)
+
+    def analyze_coded_packed(self, x, nbit, x_offsets, fs, option: AnalysisOption, number_of_dimensions,
+                             harvest_options=None, dio_options=None, cheaptrick_options=None, d4c_options=None,
+                             time_axis=None, f0=None, coded_sp=None, coded_ap=None):
+        """analyze_coded_batch on a PACKED batch (world_b200_analyze_coded_packed): x holds float64 samples (nbit 0)
+        or nbit-bit PCM back to back, sample offsets as for analyze_packed.  Returns (time_axis [F], f0 [F],
+        coded_sp [F, number_of_dimensions], coded_ap [F, max(1, GetNumberOfAperiodicities(fs))], f_offsets)."""
+        n_ap = max(1, self.number_of_aperiodicities(fs))
+        return self._packed("analyze_coded_packed", x, (nbit,), x_offsets, fs, option, (number_of_dimensions,),
+                            (0, 0, number_of_dimensions, n_ap), (time_axis, f0, coded_sp, coded_ap), harvest_options,
+                            dio_options, cheaptrick_options, d4c_options, device=True)
+
+    def analyze_coded_host_packed(self, x_host, nbit, x_offsets, fs, option: AnalysisOption, number_of_dimensions,
+                                  harvest_options=None, dio_options=None, cheaptrick_options=None, d4c_options=None,
+                                  time_axis=None, f0=None, coded_sp=None, coded_ap=None):
+        """analyze_coded_packed on HOST arrays (world_b200_analyze_coded_host_packed)."""
+        n_ap = max(1, self.number_of_aperiodicities(fs))
+        return self._packed("analyze_coded_host_packed", x_host, (nbit,), x_offsets, fs, option,
+                            (number_of_dimensions,), (0, 0, number_of_dimensions, n_ap),
+                            (time_axis, f0, coded_sp, coded_ap), harvest_options, dio_options, cheaptrick_options,
+                            d4c_options, device=False)
 
     # -- multi-GPU: one World per GPU / process; the NCCL id travels by the caller's own means -------------------
     def comm_unique_id(self) -> bytes:

@@ -9,6 +9,7 @@
 #include <vector>
 #include <string>
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <type_traits>
 
@@ -589,6 +590,25 @@ int world_b200_stonemask_batch(WorldB200 *h, const double *x, int n, int x_strid
 
 }  // extern "C"
 
+// The packed layout's offsets: x_offsets[0] == 0 and every utterance 1 .. INT_MAX samples long.  Fills x_len [n] and
+// f_off [n + 1] (frames at frame_period ms); "" when the offsets are good, else the first broken rule.
+static std::string packed_layout(int fs, int n, const long long *x_offsets, double frame_period, std::vector<int> *x_len,
+                                 std::vector<long long> *f_off) {
+  if (!x_offsets) return "x_offsets must be given";
+  if (x_offsets[0] != 0) return "x_offsets[0] must be 0";
+  x_len->resize(n);
+  f_off->assign(1, 0);
+  for (int u = 0; u < n; ++u) {
+    const long long len = x_offsets[u + 1] - x_offsets[u];
+    if (len < 1 || len > INT_MAX)
+      return "x_offsets must increase by 1 to INT_MAX samples per utterance, not " + std::to_string(len) +
+             " (utterance " + std::to_string(u) + ")";
+    (*x_len)[u] = (int)len;
+    f_off->push_back(f_off->back() + frames_for(fs, (int)len, frame_period));
+  }
+  return "";
+}
+
 namespace wb {
 // chain_plan without the caller's prefix on last_error
 static int chain_checks(Ctx *c, const ChainRequest &r, ChainPlan *p) {
@@ -597,7 +617,7 @@ static int chain_checks(Ctx *c, const ChainRequest &r, ChainPlan *p) {
     return WORLD_B200_EINVAL;
   };
   const WorldB200AnalysisOption *opt = r.opt;
-  if (!r.x || !opt || r.n < 0 || r.fs <= 0 || r.x_stride <= 0 || r.f0_stride < 0)
+  if (!r.x || !opt || r.n < 0 || r.fs <= 0 || (!r.packed && r.x_stride <= 0) || r.f0_stride < 0)
     return fail("x and option must be given, with n_utts >= 0, fs > 0 and positive strides");
   if (r.nbit != 0 && r.nbit != 8 && r.nbit != 16 && r.nbit != 24 && r.nbit != 32)
     return fail("nbit must be 0, 8, 16, 24 or 32");
@@ -625,13 +645,22 @@ static int chain_checks(Ctx *c, const ChainRequest &r, ChainPlan *p) {
   p->frame_period = harvest ? opt->harvest.frame_period : opt->dio.frame_period;
   if (!(p->frame_period > 0.0)) return fail("the F0 method's frame_period must be > 0");
 
+  // packed: the lengths come from the offsets, and the stage plans see rows as long as the longest utterance
+  int x_stride = r.x_stride;
+  const int *x_lengths = r.x_lengths;
+  if (r.packed) {
+    const std::string bad = packed_layout(r.fs, n, r.x_offsets, p->frame_period, &p->x_len, &p->f_off);
+    if (!bad.empty()) return fail(bad);
+    x_stride = n ? *std::max_element(p->x_len.begin(), p->x_len.end()) : 1;
+    x_lengths = p->x_len.data();
+  }
   p->f_len.resize(n);
   int most = 1;
   for (int u = 0; u < n; ++u) {
-    const int xl = r.x_lengths ? r.x_lengths[u] : r.x_stride;
-    if (xl < 1 || xl > r.x_stride)
+    const int xl = x_lengths ? x_lengths[u] : x_stride;
+    if (xl < 1 || xl > x_stride)
       return fail("x_lengths[" + std::to_string(u) + "] = " + std::to_string(xl) + " is outside its padded row of " +
-                  std::to_string(r.x_stride) + " samples");
+                  std::to_string(x_stride) + " samples");
     p->f_len[u] = frames_for(r.fs, xl, p->frame_period);
     if (r.f0_stride && p->f_len[u] > r.f0_stride)
       return fail("f0_stride smaller than the frame count of an utterance (utterance " + std::to_string(u) + ")");
@@ -642,8 +671,8 @@ static int chain_checks(Ctx *c, const ChainRequest &r, ChainPlan *p) {
   // The stage plans: CheapTrick when a spectrogram is asked for, D4C when an aperiodicity is (a transform, f0_stride 0,
   // needs both), StoneMask's sampling-rate limit for DIO.  Each utterance's CheapTrick option, and D4C's fft_size (its
   // CheapTrick size) and option, with the per-call option standing in for a NULL per-utterance array.
-  const bool transform = r.f0_stride == 0;
-  StageRequest s{STAGE_CHEAPTRICK, n, r.x_stride, r.x_lengths, r.fs, p->f_len.data(), p->f0_stride};
+  const bool transform = !r.packed && r.f0_stride == 0;
+  StageRequest s{STAGE_CHEAPTRICK, n, x_stride, x_lengths, r.fs, p->f_len.data(), p->f0_stride};
   s.ct = &opt->cheaptrick; s.fft_size = &opt->cheaptrick.fft_size; s.d4c = &opt->d4c;
   s.coded = r.coded; s.dims = r.dims;
   s.row_stride = r.coded ? 0 : r.row_stride;   // the stage plans check it against every utterance's size
@@ -682,29 +711,31 @@ int chain_plan(Ctx *c, const ChainRequest &r, const char *who, ChainPlan *p) {
 }
 
 int chain_f0(WorldB200 *h, const ChainRequest &r, const ChainPlan &p, int u0, int m, const double *x, double *time_axis,
-             double *f0) {
+             double *f0, const PackedSlice *ps) {
   const WorldB200AnalysisOption *opt = r.opt;
-  const int *xl = r.x_lengths ? r.x_lengths + u0 : nullptr;
+  const int *xl = ps ? p.x_len.data() + u0 : r.x_lengths ? r.x_lengths + u0 : nullptr;
+  const int x_stride = ps ? ps->x_stride : r.x_stride, f0_stride = ps ? ps->f0_stride : p.f0_stride;
   if (opt->f0_method == WORLD_B200_F0_HARVEST)
-    return r.harvest_options ? world_b200_harvest_batch_options(h, x, m, r.x_stride, xl, r.fs, r.harvest_options + u0,
-                                                                time_axis, f0, p.f0_stride)
-                             : world_b200_harvest_batch(h, x, m, r.x_stride, xl, r.fs, &opt->harvest, time_axis, f0,
-                                                        p.f0_stride);
+    return r.harvest_options ? world_b200_harvest_batch_options(h, x, m, x_stride, xl, r.fs, r.harvest_options + u0,
+                                                                time_axis, f0, f0_stride)
+                             : world_b200_harvest_batch(h, x, m, x_stride, xl, r.fs, &opt->harvest, time_axis, f0,
+                                                        f0_stride);
   int rc = r.dio_options
-               ? world_b200_dio_batch_options(h, x, m, r.x_stride, xl, r.fs, r.dio_options + u0, time_axis, f0, p.f0_stride)
-               : world_b200_dio_batch(h, x, m, r.x_stride, xl, r.fs, &opt->dio, time_axis, f0, p.f0_stride);
+               ? world_b200_dio_batch_options(h, x, m, x_stride, xl, r.fs, r.dio_options + u0, time_axis, f0, f0_stride)
+               : world_b200_dio_batch(h, x, m, x_stride, xl, r.fs, &opt->dio, time_axis, f0, f0_stride);
   if (!rc)
-    rc = world_b200_stonemask_batch(h, x, m, r.x_stride, xl, r.fs, time_axis, f0, p.f_len.data() + u0, p.f0_stride, f0);
+    rc = world_b200_stonemask_batch(h, x, m, x_stride, xl, r.fs, time_axis, f0, p.f_len.data() + u0, f0_stride, f0);
   return rc;
 }
 
 int chain_spectral(WorldB200 *h, const ChainRequest &r, const ChainPlan &p, int u0, int m, const double *x,
-                   const double *time_axis, const double *f0, double *sp, double *ap) {
+                   const double *time_axis, const double *f0, double *sp, double *ap, const PackedSlice *ps) {
   if (!sp && !ap) return 0;
   const StagePlan &lens = sp ? p.ct : p.d4;   // both plans hold the chain's lengths
   Batch b;
-  int rc = load_batch(h, x, m, r.x_stride, lens.x_len.data() + u0, r.fs, time_axis, f0, lens.f_len.data() + u0,
-                      p.f0_stride, &b);
+  int rc = load_batch(h, x, m, ps ? ps->x_stride : r.x_stride, lens.x_len.data() + u0, r.fs, time_axis, f0,
+                      lens.f_len.data() + u0, ps ? ps->f0_stride : p.f0_stride, &b);
+  if (ps) b.f_off = ps->f_off;
   if (!rc && sp) rc = cheaptrick_run(&h->c, p.ct, b, u0, sp);
   if (!rc && ap) rc = d4c_run(&h->c, p.d4, b, u0, ap);
   return rc;
@@ -793,10 +824,10 @@ class LaneScope {
   explicit LaneScope(WorldB200 *h) : h_(h), own_budget_(h->c.scratch_budget) { lanes_[0] = lanes_[1] = h; }
   LaneScope(const LaneScope &) = delete;
   LaneScope &operator=(const LaneScope &) = delete;
-  // bounds: the n_slices + 1 slice boundaries; bytes(m): the buffer of a lane whose largest slice has m utterances
-  // (0: no buffer).  A buffer comes from its lane's pool, not its arena (the stage drivers reset the arena when they
-  // return), and its bytes come out of the lane's scratch budget; the stages keep at least half of that budget (less
-  // would only mean more passes).
+  // bounds: the n_slices + 1 slice boundaries; bytes(s): the buffer slice s needs (0: none), and a lane's buffer is
+  // the largest of its slices'.  A buffer comes from its lane's pool, not its arena (the stage drivers reset the arena
+  // when they return), and its bytes come out of the lane's scratch budget; the stages keep at least half of that
+  // budget (less would only mean more passes).
   template <class Bytes>
   int open(const std::vector<int> &bounds, Bytes bytes) {
     const int n_slices = (int)bounds.size() - 1;
@@ -832,9 +863,13 @@ class LaneScope {
       lanes_[0] = two[0]; lanes_[1] = two[1];
     }
 #endif
-    for (int s = 0; s < n_slices; ++s) most_[index(s)] = imax(most_[index(s)], bounds[s + 1] - bounds[s]);
+    size_t lane_bytes[2] = {0, 0};
+    for (int s = 0; s < n_slices; ++s) {
+      most_[index(s)] = imax(most_[index(s)], bounds[s + 1] - bounds[s]);
+      lane_bytes[index(s)] = std::max(lane_bytes[index(s)], (size_t)bytes(s));
+    }
     for (int l = 0; l < (one_lane() ? 1 : 2); ++l) {
-      const size_t b = bytes(most_[l]);
+      const size_t b = lane_bytes[l];
       if (b == 0) continue;
       Ctx *c = &lanes_[l]->c;
       buf_[l] = (unsigned char *)pool_acquire(c, b);
@@ -927,7 +962,9 @@ static int analyze_chain(WorldB200 *h, const ChainRequest &r, bool gather) {
   // nbit != 0: each lane converts its slice into a float64 buffer, which the slice's three stages then read.  A lane
   // runs its slices in stream order, so one buffer per lane, sized for its largest slice, serves all of them.
   LaneScope lanes(h);
-  rc = lanes.open(bounds, [&](int m) { return nbit ? (size_t)m * x_stride * sizeof(double) : (size_t)0; });
+  rc = lanes.open(bounds, [&](int s) {
+    return nbit ? (size_t)(bounds[s + 1] - bounds[s]) * x_stride * sizeof(double) : (size_t)0;
+  });
   if (rc) return rc;
 #ifndef WB_EMU
   // multi-GPU: the full arrays and how a finished slice reaches the other ranks -- pushed into their (IPC-mapped)
@@ -992,6 +1029,109 @@ static int analyze_chain(WorldB200 *h, const ChainRequest &r, bool gather) {
 #endif
   return rc;
 }
+
+}  // extern "C"
+
+// A packed slice's time axis and f0, from the lane's padded rows (f_stride frames) to the packed rows: utterance u
+// (blockIdx.y) has f_off[u + 1] - f_off[u] frames, written from row f_off[u]
+WB_KERNEL_PLAIN scatter_f0_kernel(const long long *__restrict__ f_off, int f_stride, const double *__restrict__ t,
+                                  const double *__restrict__ f, double *__restrict__ t_out, double *__restrict__ f_out) {
+  const int u = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+  const long long at = f_off[u] + i;
+  if (at >= f_off[u + 1]) return;
+  t_out[at] = t[(size_t)u * f_stride + i];
+  f_out[at] = f[(size_t)u * f_stride + i];
+}
+
+namespace wb {
+
+// Lane slices of the packed utterances [c0, c1): n_slices cuts at equal shares of their samples, so that both lanes get
+// equal work, then halved (at the middle sample) until each slice's padded rows -- bytes(u0, u1) -- fit `cap`, or the
+// slice is one utterance.  Padded rows are as long as a slice's longest utterance: one long utterance among many short
+// ones would otherwise pad them all.
+template <class Bytes>
+static std::vector<int> packed_bounds(const long long *x_offsets, int c0, int c1, int n_slices, size_t cap,
+                                      Bytes bytes) {
+  std::vector<int> bounds{c0};
+  const long long base = x_offsets[c0], total = x_offsets[c1] - base;
+  // the first utterance at or past sample `at` of [u0, u1], kept inside (u0, u1)
+  auto cut = [&](int u0, int u1, long long at) {
+    const int u = (int)(std::lower_bound(x_offsets + u0, x_offsets + u1, at) - x_offsets);
+    return imin(u1 - 1, imax(u0 + 1, u));
+  };
+  std::vector<int> stack;
+  for (int s = 0; s < n_slices; ++s) {
+    const int u1 = s + 1 == n_slices ? c1 : cut(bounds.back(), c1, base + total * (s + 1) / n_slices);
+    if (u1 <= bounds.back()) continue;
+    stack.assign(1, u1);
+    while (!stack.empty()) {   // halve [bounds.back(), stack.back()) until it fits
+      const int u0 = bounds.back(), e = stack.back();
+      if (e - u0 > 1 && bytes(u0, e) > cap) {
+        stack.push_back(cut(u0, e, (x_offsets[u0] + x_offsets[e]) / 2));
+      } else {
+        bounds.push_back(e);
+        stack.pop_back();
+      }
+    }
+  }
+  return bounds;
+}
+
+int packed_run(WorldB200 *h, const ChainRequest &r, const ChainPlan &p, int c0, int c1, const void *x,
+               double *time_axis, double *f0, double *sp, double *ap) {
+  const long long *xo = r.x_offsets;
+  const long long *fo = p.f_off.data();
+  // a slice's lane buffer: its x and f0 offsets, then its padded rows of samples, time axis and f0
+  struct Rows { int x_stride, f0_stride; size_t off, x, t, f, total; };
+  auto rows_of = [&](int u0, int u1) {
+    Rows w{1, 1, 0, 0, 0, 0, 0};
+    for (int u = u0; u < u1; ++u) { w.x_stride = imax(w.x_stride, p.x_len[u]); w.f0_stride = imax(w.f0_stride, p.f_len[u]); }
+    const size_t m = (size_t)(u1 - u0);
+    w.x = 16 * (m + 1);
+    w.t = w.x + m * w.x_stride * 8;
+    w.f = w.t + m * w.f0_stride * 8;
+    w.total = w.f + m * w.f0_stride * 8;
+    return w;
+  };
+  int n_slices = 2;
+  if (const char *e = getenv("WB_LANE_SLICES")) n_slices = atoi(e);
+  n_slices = imax(1, imin(n_slices, c1 - c0));
+  // each lane's buffer comes out of its half of the budget, and the stages keep at least half of that
+  const std::vector<int> bounds = packed_bounds(xo, c0, c1, n_slices, h->c.scratch_budget / 4,
+                                                [&](int u0, int u1) { return rows_of(u0, u1).total; });
+  LaneScope lanes(h);
+  int rc = lanes.open(bounds, [&](int s) { return rows_of(bounds[s], bounds[s + 1]).total; });
+  std::vector<long long> offs;
+  for (size_t s = 0; s + 1 < bounds.size() && !rc; ++s) {
+    const int u0 = bounds[s], m = bounds[s + 1] - u0;
+    WorldB200 *L = lanes.lane((int)s);
+    Ctx *lc = &L->c;
+    const Rows w = rows_of(u0, u0 + m);
+    unsigned char *buf = lanes.buffer((int)s);
+    // offsets relative to x and to the output rows
+    offs.resize(2 * ((size_t)m + 1));
+    for (int k = 0; k <= m; ++k) { offs[k] = xo[u0 + k] - xo[c0]; offs[m + 1 + k] = fo[u0 + k] - fo[c0]; }
+    const long long *x_off = (const long long *)buf, *f_off = x_off + m + 1;
+    double *xs = (double *)(buf + w.x), *ts = (double *)(buf + w.t), *fs_ = (double *)(buf + w.f);
+    rc = dev_memcpy_h2d(lc, buf, offs.data(), offs.size() * 8);
+    if (!rc) rc = gather_samples(lc, x, r.nbit, x_off, m, w.x_stride, w.x_stride, xs);
+    const PackedSlice ps{w.x_stride, w.f0_stride, f_off};
+    if (!rc) rc = chain_f0(L, r, p, u0, m, xs, ts, fs_, &ps);
+    if (!rc) rc = chain_spectral(L, r, p, u0, m, xs, ts, fs_, sp, ap, &ps);
+    for (int k0 = 0; k0 < m && !rc; k0 += 65535) {
+      WB_LAUNCH_FLAT(scatter_f0_kernel, dim3((unsigned)((w.f0_stride + 255) / 256), (unsigned)imin(65535, m - k0)), 256,
+                     0, lc->stream, f_off + k0, w.f0_stride, ts + (size_t)k0 * w.f0_stride,
+                     fs_ + (size_t)k0 * w.f0_stride, time_axis, f0);
+      rc = dev_check(lc, "packed f0");
+    }
+    if (rc && L != h) h->c.last_error = L->c.last_error;
+  }
+  return rc;
+}
+
+}  // namespace wb
+
+extern "C" {
 
 int world_b200_analyze_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_lengths, int fs,
                              const WorldB200AnalysisOption *opt, double *time_axis, double *f0, int f0_stride,
@@ -1113,7 +1253,7 @@ int transform_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, 
   std::vector<int> bounds(n_slices + 1);
   for (int s = 0; s <= n_slices; ++s) bounds[s] = (int)((long long)n * s / n_slices);
   LaneScope lanes(h);
-  int rc = lanes.open(bounds, [&](int m) { return rows_of(m).total; });
+  int rc = lanes.open(bounds, [&](int s) { return rows_of(bounds[s + 1] - bounds[s]).total; });
   if (rc) return rc;
   // slice s: its lane, the global index of its first utterance, its size and where its rows are
   auto slice = [&](int s, WorldB200 **L, int *g, int *m, double **xs, double **t, double **f, double **sp, double **ap) {
@@ -1328,6 +1468,57 @@ int world_b200_analyze_coded_batch_spectral_options(WorldB200 *h, const void *x,
   r.harvest_options = harvest_options; r.dio_options = dio_options;
   r.cheaptrick_options = cheaptrick_options; r.d4c_options = d4c_options;
   return analyze_chain(h, r, false);
+}
+
+// The packed chains on device arrays: one plan, then packed_run over every utterance.  f_offsets (HOST, may be NULL)
+// receives the plan's frame offsets once the request is checked.
+static int analyze_packed_chain(WorldB200 *h, const ChainRequest &r, long long *f_offsets) {
+  if (!h) return WORLD_B200_EINVAL;
+  DeviceGuard guard_(&h->c);
+  const char *who = r.coded ? "analyze_coded_packed" : "analyze_packed";
+  if (r.n > 0 && (!r.time_axis || !r.f0)) {
+    h->c.last_error = std::string(who) + ": time_axis and f0 must be given";
+    return WORLD_B200_EINVAL;
+  }
+  ChainPlan p;
+  int rc = chain_plan(&h->c, r, who, &p);
+  if (rc) return rc;
+  if (f_offsets) std::copy(p.f_off.begin(), p.f_off.end(), f_offsets);
+  if (r.n == 0) return 0;
+  return packed_run(h, r, p, 0, r.n, r.x, r.time_axis, r.f0, p.want_sp ? r.spectrogram : nullptr,
+                    p.want_ap ? r.aperiodicity : nullptr);
+}
+
+int world_b200_packed_frames(int fs, int n, const long long *x_offsets, double frame_period, long long *f_offsets) {
+  if (fs <= 0 || n < 0 || !(frame_period > 0.0) || !f_offsets) return WORLD_B200_EINVAL;
+  std::vector<int> x_len;
+  std::vector<long long> f_off;
+  if (!packed_layout(fs, n, x_offsets, frame_period, &x_len, &f_off).empty()) return WORLD_B200_EINVAL;
+  std::copy(f_off.begin(), f_off.end(), f_offsets);
+  return 0;
+}
+
+int world_b200_analyze_packed(WorldB200 *h, const double *x, int n, const long long *x_offsets, int fs,
+                              const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
+                              const DioOption *dio_options, const CheapTrickOption *cheaptrick_options,
+                              const D4COption *d4c_options, double *time_axis, double *f0, int row_stride,
+                              double *spectrogram, double *aperiodicity, long long *f_offsets) {
+  ChainRequest r = packed_request(x, 0, n, x_offsets, fs, opt, harvest_options, dio_options, cheaptrick_options,
+                                  d4c_options, time_axis, f0, spectrogram, aperiodicity);
+  r.row_stride = row_stride;
+  return analyze_packed_chain(h, r, f_offsets);
+}
+
+int world_b200_analyze_coded_packed(WorldB200 *h, const void *x, int nbit, int n, const long long *x_offsets, int fs,
+                                    const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
+                                    const DioOption *dio_options, const CheapTrickOption *cheaptrick_options,
+                                    const D4COption *d4c_options, int number_of_dimensions, double *time_axis,
+                                    double *f0, double *coded_spectral_envelope, double *coded_aperiodicity,
+                                    long long *f_offsets) {
+  ChainRequest r = packed_request(x, nbit, n, x_offsets, fs, opt, harvest_options, dio_options, cheaptrick_options,
+                                  d4c_options, time_axis, f0, coded_spectral_envelope, coded_aperiodicity);
+  r.coded = true; r.dims = number_of_dimensions;
+  return analyze_packed_chain(h, r, f_offsets);
 }
 
 int world_b200_analyze_coded_batch_allgather(WorldB200 *h, const void *x, int nbit, int n, int x_stride,

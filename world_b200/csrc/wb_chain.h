@@ -48,6 +48,11 @@ struct ChainRequest {
   const CheapTrickOption *cheaptrick_options = nullptr;
   const D4COption *d4c_options = nullptr;
   int row_stride = 0;
+  // packed layout (the *_packed entry points): utterance u is samples [x_offsets[u], x_offsets[u + 1]) of x (HOST,
+  // n + 1 offsets); x_stride, x_lengths and f0_stride are unused, and the outputs are [F] frames, utterance u's from
+  // the plan's f_off[u]
+  bool packed = false;
+  const long long *x_offsets = nullptr;
 };
 
 // The request of a coded-row entry point: number_of_dimensions coded values per spectral frame.
@@ -62,10 +67,25 @@ inline ChainRequest coded_request(const void *x, int nbit, int n, int x_stride, 
   return r;
 }
 
+// The request of a packed entry point, with its per-utterance options.
+inline ChainRequest packed_request(const void *x, int nbit, int n, const long long *x_offsets, int fs,
+                                   const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options,
+                                   const DioOption *dio_options, const CheapTrickOption *cheaptrick_options,
+                                   const D4COption *d4c_options, double *time_axis, double *f0, double *spectrogram,
+                                   double *aperiodicity) {
+  ChainRequest r(x, nbit, n, 0, nullptr, fs, opt, time_axis, f0, 0, spectrogram, aperiodicity);
+  r.packed = true; r.x_offsets = x_offsets;
+  r.harvest_options = harvest_options; r.dio_options = dio_options;
+  r.cheaptrick_options = cheaptrick_options; r.d4c_options = d4c_options;
+  return r;
+}
+
 struct ChainPlan {
   double frame_period = 0.0;            // ms, of the chain's F0 method
   std::vector<int> f_len;               // [n] frames of each utterance
-  int f0_stride = 0;                    // the request's, or (f0_stride 0) the largest frame count
+  int f0_stride = 0;                    // the request's, or (f0_stride 0, packed) the largest frame count
+  std::vector<int> x_len;               // packed: [n] samples of each utterance
+  std::vector<long long> f_off;         // packed: [n + 1] frame offsets, f_off[n] = F
   size_t sp_row = 0, ap_row = 0;        // doubles per frame of the spectrogram / aperiodicity rows
   bool want_sp = false, want_ap = false;   // CheapTrick / D4C run (coded rows below 12 kHz have no bands: no D4C)
   StagePlan ct, d4;                        // the stage plans of CheapTrick / D4C, where they run (transform: both)
@@ -79,10 +99,26 @@ int chain_plan(Ctx *c, const ChainRequest &r, const char *who, ChainPlan *p);
 // context): x, time_axis, f0, sp and ap are device rows that start at utterance u0.  chain_f0: Harvest, or DIO +
 // StoneMask (the F0 stage calls).  chain_spectral: one Batch of the rows for both drivers, CheapTrick into sp, then D4C
 // into ap; a NULL sp or ap skips that stage.
+// A packed request's slice: x, time_axis and f0 are the lane's padded rows of x_stride samples and f0_stride frames;
+// sp / ap are packed rows, utterance u0 + k's frame 0 at row f_off[k] (DEVICE, [m]).
+struct PackedSlice {
+  int x_stride, f0_stride;
+  const long long *f_off;
+};
 int chain_f0(WorldB200 *h, const ChainRequest &r, const ChainPlan &p, int u0, int m, const double *x, double *time_axis,
-             double *f0);
+             double *f0, const PackedSlice *ps = nullptr);
 int chain_spectral(WorldB200 *h, const ChainRequest &r, const ChainPlan &p, int u0, int m, const double *x,
-                   const double *time_axis, const double *f0, double *sp, double *ap);
+                   const double *time_axis, const double *f0, double *sp, double *ap, const PackedSlice *ps = nullptr);
+// The packed chain over utterances [c0, c1) of a planned packed request, in lane slices: x points at sample
+// x_offsets[c0] (DEVICE, doubles or PCM) and the outputs at frame f_off[c0] (DEVICE, NULL sp / ap: not computed).
+// The analysis runs on padded slice rows; only x is read, and only the outputs' frames [f_off[c0], f_off[c1]) written.
+int packed_run(WorldB200 *h, const ChainRequest &r, const ChainPlan &p, int c0, int c1, const void *x,
+               double *time_axis, double *f0, double *sp, double *ap);
+// x_offsets[u] .. x_offsets[u + 1] -> padded rows: out[k][x_stride] (k < m) gets utterance k's samples, converted from
+// nbit-bit PCM by pcm_to_double's rule (nbit 0: copied); x_off is DEVICE [m + 1], relative to x.  Values past an
+// utterance's length are not written.
+int gather_samples(Ctx *ctx, const void *x, int nbit, const long long *x_off, int m, int max_len, int x_stride,
+                   double *out);
 
 // Voice transformation (world_b200_transform_*): the analysis plan of the request (full rows, no analysis outputs;
 // with spectral options each row as wide as the largest size's) and the synthesis plan of its analysis rows: lengths,

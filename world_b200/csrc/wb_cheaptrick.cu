@@ -22,14 +22,15 @@ struct CtParams {
   int fs, fft_size, lg_fft;
   double q1, f0_floor;
   const unsigned *draws; size_t draw_stride; const unsigned *draw_off;
-  double *out;            // [n][f_stride][out_stride]
+  double *out;            // [n][f_stride][out_stride], or (f_off) [F][out_stride]
   int out_stride;         // doubles per spectrogram row (fft/2+1 unless the caller pads its rows)
   const int *uid;         // [n] batch index of the launch's utterance blockIdx.y; null: blockIdx.y itself
+  const long long *f_off; // [n] packed rows: output frame of each utterance's frame 0; null: u * f_stride
   const double2 *tw;
   int *status;
   // coded tail (ct_coded_kernel): mel interpolation + DCT of the log envelope, CodeSpectralEnvelope (codec.cpp:279-295)
   int c_dims; const int *c_idx; const double *c_frac; const double2 *c_weight; double c_norm;
-  double *c_out;          // [n][f_stride][c_dims]
+  double *c_out;          // [n][f_stride][c_dims], or (f_off) [F][c_dims]
 };
 
 WB_DEV double ct_effective_f0(double f0, double f0_floor) {
@@ -73,6 +74,8 @@ WB_DEV void ct_frame_body(const CtParams &p) {
   double *red = reinterpret_cast<double *>(B + slots);   // WB_RED_DOUBLES
 
   const size_t fidx = (size_t)u * p.f_stride + i;
+  // the output row: only the address differs between the padded and the packed layout
+  const size_t oidx = p.f_off ? (size_t)(p.f_off[u] + i) : fidx;
   const double f = ct_effective_f0(p.f0[fidx], p.f0_floor);
   const double t = p.time_axis[fidx];
   const int fs = p.fs;
@@ -184,7 +187,7 @@ WB_DEV void ct_frame_body(const CtParams &p) {
   WB_SYNC();
   double2 *z3 = sfft_forward(o2, z2, lgc, p.tw);
   if (!kCoded) {
-    double *row = p.out + fidx * (size_t)p.out_stride;
+    double *row = p.out + oidx * (size_t)p.out_stride;
     rfft_unpack(z3, p.lg_fft, p.tw, [&](int k, double2 c) { row[k] = exp(c.x); });
     return;
   }
@@ -207,7 +210,7 @@ WB_DEV void ct_frame_body(const CtParams &p) {
   }
   WB_SYNC();
   const double2 *zc = sfft_forward(z3, o3, lgc - 1, p.tw);
-  double *crow = p.c_out + fidx * (size_t)p.c_dims;
+  double *crow = p.c_out + oidx * (size_t)p.c_dims;
   const int dims = p.c_dims;
   const double cn = p.c_norm;
   rfft_unpack(zc, lgc, p.tw, [&](int d, double2 X) {     // :85-88
@@ -295,7 +298,10 @@ static int ct_launch(Ctx *ctx, const Batch &b, double q1, int fft_size, double *
     p.q1 = q1; p.f0_floor = f0_floor;
     p.draws = draws; p.draw_stride = draw_stride_full; p.draw_off = offs;
     p.out_stride = row_stride > 0 ? row_stride : bins;
-    p.out = spectrogram ? spectrogram + base * b.f_stride * p.out_stride : nullptr;
+    // packed rows: the output pointers stay at frame 0 and f_off places each utterance
+    const size_t out_base = b.f_off ? 0 : base * b.f_stride;
+    p.f_off = b.f_off ? b.f_off + base : nullptr;
+    p.out = spectrogram ? spectrogram + out_base * p.out_stride : nullptr;
     p.tw = ctx->twiddle; p.status = ctx->status_dev;
     p.c_dims = 0; p.c_idx = nullptr; p.c_frac = nullptr; p.c_weight = nullptr; p.c_norm = 1.0; p.c_out = nullptr;
     int ct_threads = 128;
@@ -307,7 +313,7 @@ static int ct_launch(Ctx *ctx, const Batch &b, double q1, int fft_size, double *
       if (rc) return rc;
       p.c_dims = coded->dims; p.c_idx = (const int *)(blk + o_cidx); p.c_frac = (const double *)(blk + o_cfrac);
       p.c_weight = (const double2 *)(blk + o_cw); p.c_norm = coded->norm;
-      p.c_out = coded_out + base * b.f_stride * coded->dims;
+      p.c_out = coded_out + out_base * coded->dims;
       WB_LAUNCH_COOP(ct_coded_kernel, dim3((unsigned)max_f_len, (unsigned)n), ct_threads, smem, ctx->stream, p);
     } else
     WB_LAUNCH_COOP(ct_frame_kernel, dim3((unsigned)max_f_len, (unsigned)n), ct_threads, smem, ctx->stream, p);

@@ -142,17 +142,42 @@ WB_KERNEL(128, 16) decode_ap_kernel(CodecParams p) {
 
 struct PcmParams { const unsigned char *pcm; int bytes; const int *x_len; int x_stride; double zero_line; double *x; };
 
+// audioio.cpp:238-249: magnitude of the low bits, minus 2^(nbit-1) when the sign bit is set
+WB_DEV double pcm_sample(const unsigned char *s, int bytes, double zero_line) {
+  unsigned v = 0;
+  for (int j = bytes - 1; j >= 0; --j) v = v * 256u + s[j];
+  const unsigned sign = 1u << (8 * bytes - 1);
+  const double mag = static_cast<double>(v & (sign - 1u));
+  const double bias = (v & sign) ? zero_line : 0.0;
+  return (mag - bias) / zero_line;
+}
+
 WB_KERNEL_PLAIN pcm_kernel(PcmParams p) {
   const int u = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= p.x_len[u]) return;
-  const unsigned char *s = p.pcm + ((size_t)u * p.x_stride + i) * p.bytes;
-  // audioio.cpp:238-249: magnitude of the low bits, minus 2^(nbit-1) when the sign bit is set
-  unsigned v = 0;
-  for (int j = p.bytes - 1; j >= 0; --j) v = v * 256u + s[j];
-  const unsigned sign = 1u << (8 * p.bytes - 1);
-  const double mag = static_cast<double>(v & (sign - 1u));
-  const double bias = (v & sign) ? p.zero_line : 0.0;
-  p.x[(size_t)u * p.x_stride + i] = (mag - bias) / p.zero_line;
+  p.x[(size_t)u * p.x_stride + i] = pcm_sample(p.pcm + ((size_t)u * p.x_stride + i) * p.bytes, p.bytes, p.zero_line);
+}
+
+// packed samples -> padded float64 rows: utterance u (blockIdx.y) is samples [x_off[u], x_off[u + 1]) of src
+WB_KERNEL_PLAIN gather_kernel(const unsigned char *__restrict__ src, int bytes, double zero_line,
+                              const long long *__restrict__ x_off, int x_stride, double *__restrict__ out) {
+  const int u = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+  const long long at = x_off[u] + i;
+  if (at >= x_off[u + 1]) return;
+  double *o = out + (size_t)u * x_stride + i;
+  if (bytes == 0) *o = reinterpret_cast<const double *>(src)[at];
+  else *o = pcm_sample(src + (size_t)at * bytes, bytes, zero_line);
+}
+
+int gather_samples(Ctx *ctx, const void *x, int nbit, const long long *x_off, int m, int max_len, int x_stride,
+                   double *out) {
+  const double zero_line = nbit ? pow(2.0, nbit - 1) : 1.0;
+  for (int u0 = 0; u0 < m; u0 += 65535) {
+    const int n = imin(65535, m - u0);
+    WB_LAUNCH_FLAT(gather_kernel, dim3((unsigned)((max_len + 255) / 256), (unsigned)n), 256, 0, ctx->stream,
+                   (const unsigned char *)x, nbit / 8, zero_line, x_off + u0, x_stride, out + (size_t)u0 * x_stride);
+  }
+  return dev_check(ctx, "gather");
 }
 
 // ---------------------------------------------------------------------------------- host side

@@ -33,6 +33,7 @@ struct D4cParams {
   int *slow_list; int *slow_count;   // frames whose window does not fit the fast body kernel (long windows, f0 near the floor)
   int pw_doubles;                    // doubles of the fast body kernel's power row (d4c_body_pw_doubles)
   double *out;
+  const long long *f_off;   // [n] packed rows: output frame of each utterance's frame 0; null: u * f_stride
   const double2 *tw;
   const double2 *tw_body;   // compact twiddles of size d_fft (tw_sized_offset): the fast body kernel's
   int *status;
@@ -47,6 +48,12 @@ struct D4cParams {
 
 WB_DEV int d4c_ct_fft(const D4cParams &p, size_t fidx) {
   return p.u_fft ? __ldg(p.u_fft + fidx / p.f_stride) : p.ct_fft_size;
+}
+
+// the output frame of frame fidx (= u * f_stride + i of the slice's rows): only the address differs between the padded
+// and the packed layout; f0, the time axis, the draws and slow_list keep the slice's own indices
+WB_DEV size_t d4c_out_frame(const D4cParams &p, size_t fidx) {
+  return p.f_off ? (size_t)p.f_off[fidx / p.f_stride] + fidx % p.f_stride : fidx;
 }
 
 WB_KERNEL_PLAIN d4c_count_a_kernel(const double *__restrict__ f0, const int *__restrict__ f_len,
@@ -99,13 +106,14 @@ WB_DEV int d4c_windowed(const double *__restrict__ x, int x_len, int fs, double 
 // a frame D4C does not analyse (unvoiced, or LoveTrain says noise): 1 - 1e-12 in every bin (d4c.cpp:372-383);
 // coded: 20 log10 of that at every band centre (interp1Q between equal nodes)
 WB_DEV void d4c_fill_frame(const D4cParams &p, size_t fidx) {
+  const size_t oidx = d4c_out_frame(p, fidx);
   if (p.c_out) {
     const double v = 20 * log10(1.0 - kTiny);
-    for (int b = WB_TID; b < p.c_n; b += WB_NTH) p.c_out[fidx * (size_t)p.c_n + b] = v;
+    for (int b = WB_TID; b < p.c_n; b += WB_NTH) p.c_out[oidx * (size_t)p.c_n + b] = v;
     return;
   }
   const int bins = d4c_ct_fft(p, fidx) / 2 + 1;
-  double *row = p.out + fidx * (size_t)p.out_stride;
+  double *row = p.out + oidx * (size_t)p.out_stride;
   for (int k = WB_TID; k < bins; k += WB_NTH) row[k] = 1.0 - kTiny;
 }
 
@@ -132,17 +140,18 @@ WB_DEV void d4c_write_frame(const D4cParams &p, size_t fidx, const double *coars
   const int tid = WB_TID, nth = WB_NTH;
   const int ct_fft = d4c_ct_fft(p, fidx);
   const int bins = ct_fft / 2 + 1;
+  const size_t oidx = d4c_out_frame(p, fidx);
   if (p.c_out) {
     const int tab = p.u_ctab ? __ldg(p.u_ctab + fidx / p.f_stride) : 0;
     for (int b = tid; b < p.c_n; b += nth) {
       const int k = __ldg(p.c_idx + tab + b);
       const double y0 = d4c_bin_db(coarse, p.n_ap, p.fs, ct_fft, k);
       const double dy = (k + 1 < bins) ? d4c_bin_db(coarse, p.n_ap, p.fs, ct_fft, k + 1) - y0 : 0.0;
-      p.c_out[fidx * (size_t)p.c_n + b] = y0 + dy * __ldg(p.c_frac + tab + b);
+      p.c_out[oidx * (size_t)p.c_n + b] = y0 + dy * __ldg(p.c_frac + tab + b);
     }
     return;
   }
-  double *row = p.out + fidx * (size_t)p.out_stride;
+  double *row = p.out + oidx * (size_t)p.out_stride;
   for (int k = tid; k < bins; k += nth) {
     const double y = d4c_bin_db(coarse, p.n_ap, p.fs, ct_fft, k);
     row[k] = kFastExp ? exp(y * 0.11512925464970228420)   // 10^(y/20) = e^(y ln10 / 20)
@@ -772,7 +781,10 @@ int d4c_run(Ctx *ctx, const StagePlan &stage, const Batch &b, int u0, double *ou
     p.f_stride = b.f_stride;
     p.nuttall = nuttall; p.draws = draws; p.draw_stride = draw_stride_full;
     p.off_a = off_a; p.count_b = count_b; p.off_b = off_b; p.selected = selected;
-    p.out = coded ? nullptr : out + (size_t)c0 * b.f_stride * p.out_stride;
+    // packed rows: the output pointers stay at frame 0 and f_off places each utterance
+    const size_t out_base = b.f_off ? 0 : (size_t)c0 * b.f_stride;
+    p.f_off = b.f_off ? b.f_off + c0 : nullptr;
+    p.out = coded ? nullptr : out + out_base * p.out_stride;
     p.tw = ctx->twiddle; p.status = ctx->status_dev;
     p.tw_body = ctx->twiddle_sized + tw_sized_offset(p.d_lg);
     if (per_utt) {
@@ -793,7 +805,7 @@ int d4c_run(Ctx *ctx, const StagePlan &stage, const Batch &b, int u0, double *ou
       if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_cfrac, per_utt ? ctab_frac.data() : coded->frac.data(), n_tab * 8);
       if (rc) break;
       p.c_n = coded->dims; p.c_idx = (const int *)(blk + o_cidx); p.c_frac = (const double *)(blk + o_cfrac);
-      p.c_out = out + (size_t)c0 * b.f_stride * coded->dims;
+      p.c_out = out + out_base * coded->dims;
     }
     p.slow_list = (int *)(blk + o_slow); p.slow_count = (int *)(blk + o_nslow);
     dev_memset(ctx, p.slow_count, 0, 4);

@@ -334,6 +334,95 @@ int analyze_pipeline(WorldB200 *h, const ChainRequest &r) {
   return rc;
 }
 
+// The packed chains for host arrays.  Utterances go in chunks (at most WB_HOST_CHUNK, default 512, and as many as keep
+// one chunk's device rows within a twelfth of the scratch budget: two input buffers and two output sets take a third).
+// A chunk's samples [x_offsets[c0], x_offsets[c1]) go up as one copy on s_in, packed_run analyses them on the context's
+// stream with chunk-relative offsets, and each output array's frames [f_off[c0], f_off[c1]) come back as one copy on
+// s_out, so the upload of the next chunk and the download of the last overlap this chunk's kernels.  Full rows are
+// zeroed first where an utterance is narrower than the row.  time_axis and f0 may be NULL: not downloaded.
+int analyze_packed_pipeline(WorldB200 *h, const ChainRequest &r, long long *f_offsets) {
+  if (!h) return WORLD_B200_EINVAL;
+  DeviceGuard guard_(&h->c);
+  Ctx *ctx = &h->c;
+  ChainPlan plan;
+  int rc = chain_plan(ctx, r, r.coded ? "analyze_coded_host_packed" : "analyze_host_packed", &plan);
+  if (rc) return rc;
+  if (f_offsets) std::copy(plan.f_off.begin(), plan.f_off.end(), f_offsets);
+  const int n_utts = r.n;
+  if (n_utts == 0) return 0;
+  const long long *xo = r.x_offsets, *fo = plan.f_off.data();
+  const size_t in_bytes = r.nbit ? (size_t)(r.nbit / 8) : 8;
+  const bool want_sp = plan.want_sp, want_ap = plan.want_ap;
+  const size_t sp_row = want_sp ? plan.sp_row : 0, ap_row = want_ap ? plan.ap_row : 0;
+  const StagePlan &sizes = want_sp ? plan.ct : plan.d4;   // each utterance's fft_size (D4C runs at CheapTrick's)
+  const size_t per_frame = (2 + sp_row + ap_row) * 8;
+  int outer = 512;
+  if (const char *e = getenv("WB_HOST_CHUNK")) outer = atoi(e) > 0 ? atoi(e) : outer;
+  const size_t cap = ctx->scratch_budget / 12;
+  auto bytes = [&](int c0, int c1) {
+    return (size_t)(xo[c1] - xo[c0]) * in_bytes + (size_t)(fo[c1] - fo[c0]) * per_frame;
+  };
+  std::vector<int> bounds{0};
+  while (bounds.back() < n_utts) {
+    const int c0 = bounds.back();
+    int c1 = c0 + 1;
+    while (c1 < n_utts && c1 - c0 < outer && bytes(c0, c1 + 1) <= cap) ++c1;
+    bounds.push_back(c1);
+  }
+  const int n_chunks = (int)bounds.size() - 1;
+  size_t most_in = 0, most_frames = 0;
+  for (int k = 0; k < n_chunks; ++k) {
+    most_in = std::max(most_in, (size_t)(xo[bounds[k + 1]] - xo[bounds[k]]) * in_bytes);
+    most_frames = std::max(most_frames, (size_t)(fo[bounds[k + 1]] - fo[bounds[k]]));
+  }
+
+  enum { EV_IN = 0, EV_CDONE = 2, EV_OUT = 4 };   // per buffer set: uploaded, computed, downloaded
+  HostPipe p(h, "analyze_packed");
+  rc = p.open(6);
+  if (rc) return rc;
+  unsigned char *din[2] = {nullptr, nullptr};
+  double *dt[2] = {nullptr, nullptr}, *df[2] = {nullptr, nullptr}, *dsp[2] = {nullptr, nullptr},
+         *dap[2] = {nullptr, nullptr};
+  for (int i = 0; i < (n_chunks > 1 ? 2 : 1) && !rc; ++i) {
+    rc = p.buffer(most_in, &din[i]);
+    if (!rc) rc = p.buffer(most_frames * 8, &dt[i]);
+    if (!rc) rc = p.buffer(most_frames * 8, &df[i]);
+    if (!rc) rc = p.buffer(most_frames * sp_row * 8, &dsp[i]);
+    if (!rc) rc = p.buffer(most_frames * ap_row * 8, &dap[i]);
+  }
+  for (int k = 0; k < n_chunks && !rc; ++k) {
+    const int c0 = bounds[k], c1 = bounds[k + 1], s = k & 1;
+    const size_t frames = (size_t)(fo[c1] - fo[c0]);
+    if (k >= 2) p.wait(HostPipe::IN, EV_CDONE + s);   // the kernels of chunk k - 2 have read din[s]
+    p.h2d(din[s], (const unsigned char *)r.x + (size_t)xo[c0] * in_bytes, (size_t)(xo[c1] - xo[c0]) * in_bytes);
+    p.record(EV_IN + s, HostPipe::IN);
+    p.mark("h2d_done", k, HostPipe::IN);
+    p.wait(HostPipe::RUN, EV_IN + s);
+    if (k >= 2) p.wait(HostPipe::RUN, EV_OUT + s);   // the rows of chunk k - 2 are on the host
+    p.mark("run_begin", k, HostPipe::RUN);
+    bool narrow = false;
+    for (int u = c0; u < c1 && !r.coded; ++u) narrow = narrow || (size_t)(sizes.fft_size[u] / 2 + 1) != plan.sp_row;
+    if (narrow && want_sp) rc = dev_memset(ctx, dsp[s], 0, frames * sp_row * 8);
+    if (narrow && want_ap && !rc) rc = dev_memset(ctx, dap[s], 0, frames * ap_row * 8);
+    if (!rc) rc = packed_run(h, r, plan, c0, c1, din[s], dt[s], df[s], dsp[s], dap[s]);
+    if (rc) break;
+    p.record(EV_CDONE + s, HostPipe::RUN);
+    p.mark("run_end", k, HostPipe::RUN);
+    p.wait(HostPipe::OUT, EV_CDONE + s);
+    if (r.time_axis) p.d2h(r.time_axis + fo[c0], dt[s], frames * 8);
+    if (r.f0) p.d2h(r.f0 + fo[c0], df[s], frames * 8);
+    if (want_sp) p.d2h(r.spectrogram + (size_t)fo[c0] * sp_row, dsp[s], frames * sp_row * 8);
+    if (want_ap) p.d2h(r.aperiodicity + (size_t)fo[c0] * ap_row, dap[s], frames * ap_row * 8);
+    p.record(EV_OUT + s, HostPipe::OUT);
+    p.mark("d2h_end", k, HostPipe::OUT);
+  }
+  char header[96];
+  snprintf(header, sizeof header, "chunks %d n %d", n_chunks, n_utts);
+  rc = p.finish(rc, header);
+  if (!rc) rc = world_b200_synchronize(h);
+  return rc;
+}
+
 // The chunk loop of the synthesis and transform pipelines.  Utterance chunks of `chunk` are uploaded on s_in into one
 // of two input buffers of in_bytes, run on the context's stream into one of `ring` output slots (at most one per chunk)
 // and downloaded on s_out as whole rows of out_row bytes: a row past its utterance's y_len reads as zero on the host.
@@ -572,6 +661,29 @@ extern "C" int world_b200_analyze_host_spectral_options(
   r.harvest_options = harvest_options; r.dio_options = dio_options;
   r.cheaptrick_options = cheaptrick_options; r.d4c_options = d4c_options; r.row_stride = row_stride;
   return analyze_pipeline(h, r);
+}
+
+extern "C" int world_b200_analyze_host_packed(WorldB200 *h, const double *x, int n_utts, const long long *x_offsets,
+                                              int fs, const WorldB200AnalysisOption *opt,
+                                              const HarvestOption *harvest_options, const DioOption *dio_options,
+                                              const CheapTrickOption *cheaptrick_options, const D4COption *d4c_options,
+                                              double *time_axis, double *f0, int row_stride, double *spectrogram,
+                                              double *aperiodicity, long long *f_offsets) {
+  ChainRequest r = packed_request(x, 0, n_utts, x_offsets, fs, opt, harvest_options, dio_options, cheaptrick_options,
+                                  d4c_options, time_axis, f0, spectrogram, aperiodicity);
+  r.row_stride = row_stride;
+  return analyze_packed_pipeline(h, r, f_offsets);
+}
+
+extern "C" int world_b200_analyze_coded_host_packed(
+    WorldB200 *h, const void *x, int nbit, int n_utts, const long long *x_offsets, int fs,
+    const WorldB200AnalysisOption *opt, const HarvestOption *harvest_options, const DioOption *dio_options,
+    const CheapTrickOption *cheaptrick_options, const D4COption *d4c_options, int number_of_dimensions,
+    double *time_axis, double *f0, double *coded_spectral_envelope, double *coded_aperiodicity, long long *f_offsets) {
+  ChainRequest r = packed_request(x, nbit, n_utts, x_offsets, fs, opt, harvest_options, dio_options, cheaptrick_options,
+                                  d4c_options, time_axis, f0, coded_spectral_envelope, coded_aperiodicity);
+  r.coded = true; r.dims = number_of_dimensions;
+  return analyze_packed_pipeline(h, r, f_offsets);
 }
 
 // analyze_coded_host with per-utterance CheapTrick / D4C options (either array may be NULL) and F0 options as above

@@ -142,6 +142,9 @@ struct Batch {
   int max_x_len, max_f_len;  // host-known maxima
   const int *l1_host = nullptr;  // [n] host: frames on the 1 ms grid (Harvest only)
   const int *x_len_host = nullptr;  // [n] host copy of x_len, or nullptr = every row is full (DIO only)
+  // CheapTrick / D4C output rows: [n] device frame offsets (packed rows, utterance u's frame i at row f_off[u] + i), or
+  // nullptr = padded rows (u * f_stride + i)
+  const long long *f_off = nullptr;
 };
 
 // stage drivers (each: enqueue on ctx->stream, return 0 / error code)
