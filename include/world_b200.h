@@ -666,6 +666,45 @@ int world_b200_analyze_coded_host_packed(WorldB200 *ctx, const void *x, int nbit
                                          double *coded_spectral_envelope, double *coded_aperiodicity,
                                          long long *f_offsets);
 
+/* The way back on packed rows.  f_offsets and y_offsets are HOST arrays of n_utts + 1 offsets starting at 0:
+ * utterance u is frames [f_offsets[u], f_offsets[u + 1]) of f0 / the rows and samples [y_offsets[u], y_offsets[u + 1])
+ * of y.  f_offsets may be the array world_b200_analyze_*packed returns, and y_offsets = x_offsets gives the output the
+ * input's layout.  fft_sizes (HOST, n_utts) is required, as in the _options calls.  Every address is 64-bit: F,
+ * F * row_stride and Y may exceed 2^31.
+ * Equality: utterance u's samples equal, bit for bit, what the padded call of the same family gives it with the same
+ * fft_sizes, f0_lengths[u] = f_offsets[u + 1] - f_offsets[u] and y_lengths[u] = y_offsets[u + 1] - y_offsets[u]:
+ * world_b200_synthesis_batch_options, world_b200_synthesis_coded_batch_options, world_b200_modify_batch_options.
+ * Checked before any work is queued: the padded call's rules, offsets starting at 0, and for synthesis 2 .. INT_MAX
+ * frames and samples per utterance (modification: 0 .. INT_MAX frames); EINVAL, world_b200_last_error() naming the
+ * first bad utterance, outputs untouched.  n_utts == 0 returns 0. */
+/* Synthesis on packed rows (DEVICE arrays): f0 [F]; spectrogram / aperiodicity [F][row_stride] (0: the largest
+ * fft_sizes[u] / 2 + 1); y [Y] float64, Y = y_offsets[n_utts].  Writes samples [0, Y) of y and nothing else. */
+int world_b200_synthesis_packed(WorldB200 *ctx, const double *f0, int n_utts, const long long *f_offsets,
+                                const double *spectrogram, const double *aperiodicity, int row_stride,
+                                const int *fft_sizes, double frame_period, int fs, const long long *y_offsets,
+                                double *y);
+/* Synthesis from coded rows [F][number_of_dimensions] and [F][GetNumberOfAperiodicities(fs)] (DEVICE arrays).
+ * f0_scale / spectral_ratio (HOST, n_utts) may be NULL.  nbit 0: y is float64; nbit 16: int16, quantised as wavwrite
+ * does.  Writes samples [0, Y) of y and nothing else. */
+int world_b200_synthesis_coded_packed(WorldB200 *ctx, const double *f0, int n_utts, const long long *f_offsets,
+                                      const double *coded_spectral_envelope, int number_of_dimensions,
+                                      const double *coded_aperiodicity, const int *fft_sizes, double frame_period,
+                                      int fs, const long long *y_offsets, const double *f0_scale,
+                                      const double *spectral_ratio, int nbit, void *y);
+/* The same for HOST arrays, pipelined: each chunk's frames go up as one copy per input array and its samples come back
+ * as one copy.  Writes exactly Y samples; its output equals world_b200_synthesis_coded_packed's. */
+int world_b200_synthesis_coded_host_packed(WorldB200 *ctx, const double *f0, int n_utts, const long long *f_offsets,
+                                           const double *coded_spectral_envelope, int number_of_dimensions,
+                                           const double *coded_aperiodicity, const int *fft_sizes,
+                                           double frame_period, int fs, const long long *y_offsets,
+                                           const double *f0_scale, const double *spectral_ratio, int nbit, void *y);
+/* ParameterModification in place on packed rows (DEVICE arrays): f0 [F], spectrogram [F][row_stride] (0: the largest
+ * fft_sizes[u] / 2 + 1; fft_sizes may be NULL when spectral_ratio is).  Writes nothing outside frames [0, F), nor past
+ * an utterance's fft_size / 2 + 1 in a row. */
+int world_b200_modify_packed(WorldB200 *ctx, double *f0, int n_utts, const long long *f_offsets, double *spectrogram,
+                             int row_stride, const int *fft_sizes, int fs, const double *f0_scale,
+                             const double *spectral_ratio);
+
 /* ---- voice transformation, PCM in and PCM out: the reference demo's loop (test/test.cpp: Harvest or DIO + StoneMask,
  * CheapTrick, D4C, ParameterModification, Synthesis) over a batch in one call, with one pitch, formant and tempo
  * factor per utterance ----------------------------------------------------------------------------------------------

@@ -165,6 +165,13 @@ ABI = {
                                                        C.POINTER(AnalysisOption), C.POINTER(HarvestOption),
                                                        C.POINTER(DioOption), C.POINTER(CheapTrickOption),
                                                        C.POINTER(D4COption), C.c_int, _P, _P, _P, _P, _LP]),
+    "world_b200_synthesis_packed": (C.c_int, [_P, _P, C.c_int, _LP, _P, _P, C.c_int, _IP, C.c_double, C.c_int, _LP,
+                                              _P]),
+    "world_b200_synthesis_coded_packed": (C.c_int, [_P, _P, C.c_int, _LP, _P, C.c_int, _P, _IP, C.c_double, C.c_int,
+                                                    _LP, _P, _P, C.c_int, _P]),
+    "world_b200_synthesis_coded_host_packed": (C.c_int, [_P, _P, C.c_int, _LP, _P, C.c_int, _P, _IP, C.c_double,
+                                                         C.c_int, _LP, _P, _P, C.c_int, _P]),
+    "world_b200_modify_packed": (C.c_int, [_P, _P, C.c_int, _LP, _P, C.c_int, _IP, C.c_int, _P, _P]),
     "world_b200_comm_unique_id": (C.c_int, [_P, C.c_int]),
     "world_b200_comm_init": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int]),
     "world_b200_comm_destroy": (C.c_int, [_P]),
@@ -949,6 +956,104 @@ class World:
                             (number_of_dimensions,), (0, 0, number_of_dimensions, n_ap),
                             (time_axis, f0, coded_sp, coded_ap), harvest_options, dio_options, cheaptrick_options,
                             d4c_options, device=False)
+
+    # -- the way back on packed rows: utterance u = frames [f_offsets[u], f_offsets[u + 1]) and samples
+    #    [y_offsets[u], y_offsets[u + 1]) ----------------------------------------------------------------------------
+    def _packed_way_back(self, f_offsets, y_offsets, fft_size):
+        """(n, f_offsets, y_offsets as ctypes int64 arrays, Y, per-utterance fft sizes as a ctypes int array)."""
+        n, fo = _offsets(f_offsets)
+        ny, yo = _offsets(y_offsets)
+        if ny != n:
+            raise ValueError(f"{n + 1} f_offsets but {ny + 1} y_offsets")
+        sizes = _fft_sizes(fft_size, n)
+        if sizes is None:
+            sizes = (C.c_int * max(n, 1))(*([int(fft_size)] * n))
+        return n, fo, yo, int(yo[n]), sizes
+
+    def _packed_y(self, like, Y, pcm16):
+        if self.xp == "torch":
+            dtype = self.torch.int16 if pcm16 else self.torch.float64
+            return self.torch.zeros((Y,), dtype=dtype, device=like.device)
+        import numpy as np
+        return np.zeros((Y,), dtype=np.int16 if pcm16 else np.float64)
+
+    def synthesis_packed(self, f0, spectrogram, aperiodicity, f_offsets, fft_size, frame_period, fs, y_offsets,
+                         y=None):
+        """synthesis on PACKED rows of DEVICE arrays (world_b200_synthesis_packed): f0 [F], spectrogram / aperiodicity
+        [F, W] (W >= every fft_size // 2 + 1, as analyze_packed writes them), utterance u being frames
+        [f_offsets[u], f_offsets[u + 1]).  Returns y [Y] (float64), utterance u being samples
+        [y_offsets[u], y_offsets[u + 1]); offsets as analyze_packed takes them.  fft_size: one int, or one per
+        utterance.  Each utterance's samples equal synthesis()'s with the same sizes, bit for bit."""
+        n, fo, yo, Y, sizes = self._packed_way_back(f_offsets, y_offsets, fft_size)
+        if y is None:
+            y = self._packed_y(f0, Y, False)
+        self._use_current_stream()
+        self._check(self.lib.world_b200_synthesis_packed(
+            self._h, _ptr(f0), n, fo, _ptr(spectrogram), _ptr(aperiodicity), int(spectrogram.shape[-1]), sizes,
+            frame_period, fs, yo, _ptr(y)))
+        return y
+
+    def synthesis_coded_packed(self, f0, coded_spectral_envelope, coded_aperiodicity, f_offsets, fft_size,
+                               frame_period, fs, y_offsets, dtype=None, f0_scale=None, spectral_ratio=None, y=None):
+        """synthesis_coded on PACKED rows of DEVICE arrays (world_b200_synthesis_coded_packed): f0 [F],
+        coded_spectral_envelope [F, number_of_dimensions], coded_aperiodicity [F, GetNumberOfAperiodicities(fs)] (may
+        be None below 12 kHz).  Returns y [Y], float64 or (dtype int16) 16-bit PCM.  f0_scale / spectral_ratio as in
+        synthesis_coded."""
+        pcm16 = _pcm16(dtype)
+        n, fo, yo, Y, sizes = self._packed_way_back(f_offsets, y_offsets, fft_size)
+        if y is None:
+            y = self._packed_y(f0, Y, pcm16)
+        self._use_current_stream()
+        self._check(self.lib.world_b200_synthesis_coded_packed(
+            self._h, _ptr(f0), n, fo, _ptr(coded_spectral_envelope), int(coded_spectral_envelope.shape[-1]),
+            _ptr(coded_aperiodicity), sizes, frame_period, fs, yo, _factors(f0_scale, n, "f0_scale"),
+            _factors(spectral_ratio, n, "spectral_ratio"), 16 if pcm16 else 0, _ptr(y)))
+        return y
+
+    def synthesis_coded_host_packed(self, f0, coded_sp, coded_ap, f_offsets, fft_size, frame_period, fs, y_offsets,
+                                    nbit=16, out=None, f0_scale=None, spectral_ratio=None):
+        """synthesis_coded_packed for HOST arrays (numpy arrays or CPU tensors, float64), pipelined over chunks of
+        utterances (world_b200_synthesis_coded_host_packed).  Returns y [Y] as a numpy array, int16 for nbit 16 or
+        float64 for nbit 0.  out: a contiguous host array of that shape and dtype to write into (pinned, the downloads
+        overlap the kernels)."""
+        import numpy as np
+
+        def host(a):
+            if a is None:
+                return None
+            if hasattr(a, "numpy"):
+                a = a.detach().numpy()
+            return np.ascontiguousarray(a, dtype=np.float64)
+
+        f0, coded_sp, coded_ap = host(f0), host(coded_sp), host(coded_ap)
+        n, fo, yo, Y, sizes = self._packed_way_back(f_offsets, y_offsets, fft_size)
+        dt = np.int16 if nbit == 16 else np.float64
+        if out is None:
+            out = np.empty((Y,), dtype=dt)
+        y = out.numpy() if hasattr(out, "numpy") else out
+        if nbit in (0, 16) and (y.shape != (Y,) or y.dtype != dt or not y.flags.c_contiguous):
+            raise ValueError(f"out: a contiguous [{Y}] {np.dtype(dt).name} host array")
+        self._check(self.lib.world_b200_synthesis_coded_host_packed(
+            self._h, _ptr(f0), n, fo, _ptr(coded_sp), int(coded_sp.shape[-1]), _ptr(coded_ap), sizes, frame_period,
+            fs, yo, _factors(f0_scale, n, "f0_scale"), _factors(spectral_ratio, n, "spectral_ratio"), nbit, _ptr(y)))
+        return y
+
+    def modify_packed(self, f0, spectrogram, f_offsets, fs, fft_size=None, f0_scale=None, spectral_ratio=None):
+        """modify on PACKED rows in place (world_b200_modify_packed): f0 [F], spectrogram [F, W] (W >= every
+        fft_size // 2 + 1), utterance u being frames [f_offsets[u], f_offsets[u + 1]).  fft_size (one int or one per
+        utterance) is needed with spectral_ratio.  Returns (f0, spectrogram)."""
+        n, fo = _offsets(f_offsets)
+        sizes = None
+        if fft_size is not None:
+            sizes = _fft_sizes(fft_size, n)
+            if sizes is None:
+                sizes = (C.c_int * max(n, 1))(*([int(fft_size)] * n))
+        row = int(spectrogram.shape[-1]) if spectrogram is not None else 0
+        self._use_current_stream()
+        self._check(self.lib.world_b200_modify_packed(
+            self._h, _ptr(f0), n, fo, _ptr(spectrogram), row, sizes, fs, _factors(f0_scale, n, "f0_scale"),
+            _factors(spectral_ratio, n, "spectral_ratio")))
+        return f0, spectrogram
 
     # -- multi-GPU: one World per GPU / process; the NCCL id travels by the caller's own means -------------------
     def comm_unique_id(self) -> bytes:

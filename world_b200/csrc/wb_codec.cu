@@ -45,7 +45,23 @@ struct CodecParams {
   const double2 *tw;
   const int *list;            // decode: the utterance of each blockIdx.y, or NULL: blockIdx.y itself
   int row;                    // decode: doubles per output frame row (>= bins)
+  // decode over packed rows (null: padded rows of f_stride): utterance u's frame i is row f_off[u] + i of in and out;
+  // blockIdx.x is a frame of the launch, entry j of list owning frames [cum[j], cum[j + 1])
+  const long long *f_off, *cum;
+  int list_n;
 };
+
+// decode: the utterance, frame and (in and out) row of this CTA
+struct DecodeAt { int u, f; size_t row; };
+WB_DEV DecodeAt decode_at(const CodecParams &p) {
+  if (p.cum) {
+    const int j = packed_find(p.cum, p.list_n, (long long)blockIdx.x);
+    const int u = p.list ? p.list[j] : j, f = (int)(blockIdx.x - p.cum[j]);
+    return {u, f, (size_t)p.f_off[u] + f};
+  }
+  const int u = p.list ? p.list[blockIdx.y] : blockIdx.y, f = blockIdx.x;
+  return {u, f, (size_t)u * p.f_stride + f};
+}
 
 WB_KERNEL(128, 8) code_sp_kernel(CodecParams p) {
   WB_DYN_SMEM(double, smem);
@@ -75,12 +91,13 @@ WB_KERNEL(128, 8) code_sp_kernel(CodecParams p) {
 
 WB_KERNEL(128, 8) decode_sp_kernel(CodecParams p) {
   WB_DYN_SMEM(double, smem);
-  const int tid = WB_TID, nth = WB_NTH, u = p.list ? p.list[blockIdx.y] : blockIdx.y, f = blockIdx.x;
-  if (f >= p.f_len[u]) return;
+  const int tid = WB_TID, nth = WB_NTH;
+  const DecodeAt at = decode_at(p);
+  if (at.f >= p.f_len[at.u]) return;
   const int M = p.max_dim;
   double2 *z = reinterpret_cast<double2 *>(smem);  // M complex
   double *mel = smem + 2 * M;                      // M + 2
-  const double *c = p.in + ((size_t)u * p.f_stride + f) * p.dims;
+  const double *c = p.in + at.row * p.dims;
   for (int d = tid; d < M; d += nth) {                                              // :97-107
     double2 v = make_double2(0.0, 0.0);
     if (d < p.dims) {
@@ -98,7 +115,7 @@ WB_KERNEL(128, 8) decode_sp_kernel(CodecParams p) {
   WB_SYNC();
   if (tid == 0) { mel[0] = mel[1]; mel[M + 1] = mel[M]; }
   WB_SYNC();
-  double *out = p.out + ((size_t)u * p.f_stride + f) * p.row;
+  double *out = p.out + at.row * p.row;
   for (int j = tid; j < p.bins; j += nth) {                                         // :150-154
     const int k = __ldg(p.idx + j);
     const double v = mel[k] + __ldg(p.frac + j) * (mel[k + 1] - mel[k]);
@@ -121,11 +138,11 @@ WB_KERNEL_PLAIN code_ap_kernel(CodecParams p) {
 
 // 128 threads (launch_frames); 16 CTAs per SM is full occupancy, at most 32 registers
 WB_KERNEL(128, 16) decode_ap_kernel(CodecParams p) {
-  const int u = p.list ? p.list[blockIdx.y] : blockIdx.y, f = blockIdx.x;
-  if (f >= p.f_len[u]) return;
+  const DecodeAt at = decode_at(p);
+  if (at.f >= p.f_len[at.u]) return;
   const int n_ap = p.dims;
-  const double *c = p.in + ((size_t)u * p.f_stride + f) * n_ap;
-  double *out = p.out + ((size_t)u * p.f_stride + f) * p.row;
+  const double *c = p.in + at.row * n_ap;
+  double *out = p.out + at.row * p.row;
   double mean = 0.0;
   for (int b = 0; b < n_ap; ++b) mean += c[b];                                      // CheckVUV :32-40
   mean /= n_ap;
@@ -334,6 +351,24 @@ void codec_decode_launch(Ctx *ctx, bool spectral_envelope, const CodecTables &t,
   if (out_row) p.row = out_row;
   p.list = list;   // a list (at most one pass of utterances, < 65536) is one launch over the whole rows
   launch_frames(ctx, which, p, f_len, n_utts, max_f, t.dims, p.row, decode_smem(which, fft_size));
+}
+
+void codec_decode_packed_launch(Ctx *ctx, bool spectral_envelope, const CodecTables &t, const CodecDeviceTables &d,
+                                int fft_size, const int *f_len, const long long *f_off, const int *list,
+                                int list_n, const long long *cum, long long frames, const double *in, double *out,
+                                int out_row) {
+  if (list_n == 0 || frames == 0) return;
+  const int which = spectral_envelope ? 1 : 3;
+  CodecParams p = decode_params(which, t, fft_size, 0, in, out);
+  p.idx = d.idx; p.frac = d.frac; p.weight = d.weight;
+  p.row = out_row; p.list = list; p.f_off = f_off; p.cum = cum; p.list_n = list_n;
+  p.tw = ctx->twiddle; p.f_len = f_len;   // every frame of the grid is within its utterance's f_len
+  const size_t smem = decode_smem(which, fft_size);
+#ifndef WB_EMU
+  if (which == 1) cudaFuncSetAttribute(decode_sp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+#endif
+  if (which == 1) WB_LAUNCH_COOP(decode_sp_kernel, dim3((unsigned)frames), 128, smem, ctx->stream, p);
+  else WB_LAUNCH_FLAT(decode_ap_kernel, dim3((unsigned)frames), 128, 0, ctx->stream, p);
 }
 
 // GetParametersForCoding (codec.cpp:161-181) + the DCT weights of DCTForCodec (:73-89)

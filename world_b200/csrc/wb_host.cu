@@ -423,17 +423,21 @@ int analyze_packed_pipeline(WorldB200 *h, const ChainRequest &r, long long *f_of
   return rc;
 }
 
-// The chunk loop of the synthesis and transform pipelines.  Utterance chunks of `chunk` are uploaded on s_in into one
-// of two input buffers of in_bytes, run on the context's stream into one of `ring` output slots (at most one per chunk)
-// and downloaded on s_out as whole rows of out_row bytes: a row past its utterance's y_len reads as zero on the host.
-// upload(p, u0, m, in) enqueues the copies of the chunk of utterances u0 .. u0 + m with p.h2d; run(u0, m, in, out) enqueues
-// its work.  Both runners synchronise the host with the device inside a run (pulse counts), so the upload of chunk
-// k + 1 is enqueued before chunk k runs: it then overlaps chunk k's kernels instead of following the host's wait.
-template <class Upload, class Run>
-int chunk_pipeline(WorldB200 *h, const char *who, int n_utts, int chunk, int ring, size_t in_bytes, size_t out_row,
-                   const int *y_len, int y_stride, int nbit, void *y, Upload upload, Run run) {
+// The chunk loop of the synthesis and transform pipelines.  Chunk k is utterances [bounds[k], bounds[k + 1]); it is
+// uploaded on s_in into one of two input buffers of in_bytes, run on the context's stream into one of `ring` output
+// slots of out_bytes (at most one per chunk) and downloaded on s_out as one copy: bytes [out_at(c0), out_at(c1)) of y.
+// zero(c0, c1): the chunk's slot is zeroed before its run (whole padded rows, of which a row past its utterance's y_len
+// reads as zero on the host).  upload(p, u0, m, in) enqueues the copies of the chunk of utterances u0 .. u0 + m with
+// p.h2d; run(u0, m, in, out) enqueues its work.  Both runners synchronise the host with the device inside a run (pulse
+// counts), so the upload of chunk k + 1 is enqueued before chunk k runs: it then overlaps chunk k's kernels instead of
+// following the host's wait.
+template <class Upload, class Run, class OutAt, class Zero>
+int chunk_pipeline(WorldB200 *h, const char *who, const std::vector<int> &bounds, int ring, size_t in_bytes,
+                   size_t out_bytes, OutAt out_at, Zero zero, int nbit, void *y, Upload upload, Run run) {
   Ctx *ctx = &h->c;
-  const int n_chunks = (n_utts + chunk - 1) / chunk;
+  const int n_chunks = (int)bounds.size() - 1, n_utts = bounds.back();
+  int chunk = 0;
+  for (int k = 0; k < n_chunks; ++k) chunk = imax(chunk, bounds[k + 1] - bounds[k]);
   ring = imin(ring, n_chunks);
   enum { EV_IN = 0, EV_CDONE = 2, EV_OUT = 4 };   // two input buffers, then `ring` output slots
   HostPipe p(h, who);
@@ -442,29 +446,28 @@ int chunk_pipeline(WorldB200 *h, const char *who, int n_utts, int chunk, int rin
   unsigned char *din[2] = {nullptr, nullptr};
   std::vector<unsigned char *> dout(ring, nullptr);
   for (int i = 0; i < (n_chunks > 1 ? 2 : 1) && !rc; ++i) rc = p.buffer(in_bytes, &din[i]);
-  for (int i = 0; i < ring && !rc; ++i) rc = p.buffer((size_t)chunk * out_row, &dout[i]);
+  for (int i = 0; i < ring && !rc; ++i) rc = p.buffer(out_bytes, &dout[i]);
   auto upload_chunk = [&](int k) {
     if (k >= 2) p.wait(HostPipe::IN, EV_CDONE + (k & 1));   // the kernels of chunk k-2 have read din[k & 1]
-    upload(p, k * chunk, imin(chunk, n_utts - k * chunk), din[k & 1]);
+    upload(p, bounds[k], bounds[k + 1] - bounds[k], din[k & 1]);
     p.record(EV_IN + (k & 1), HostPipe::IN);
     p.mark("h2d_done", k, HostPipe::IN);
   };
   if (!rc) upload_chunk(0);
   for (int k = 0; k < n_chunks && !rc; ++k) {
-    const int u0 = k * chunk, m = imin(chunk, n_utts - u0), s = k & 1, slot = k % ring;
+    const int u0 = bounds[k], m = bounds[k + 1] - u0, s = k & 1, slot = k % ring;
+    const size_t o0 = out_at(u0), o1 = out_at(u0 + m);
     if (k + 1 < n_chunks) upload_chunk(k + 1);
     p.wait(HostPipe::RUN, EV_IN + s);
     if (k >= ring) p.wait(HostPipe::RUN, EV_OUT + slot);   // the slot's previous chunk is on the host
     p.mark("run_begin", k, HostPipe::RUN);
-    bool ragged = false;
-    for (int i = 0; i < m; ++i) ragged = ragged || y_len[u0 + i] != y_stride;
-    if (ragged) rc = dev_memset(ctx, dout[slot], 0, (size_t)m * out_row);
+    if (zero(u0, u0 + m)) rc = dev_memset(ctx, dout[slot], 0, o1 - o0);
     if (!rc) rc = run(u0, m, din[s], dout[slot]);
     if (rc) break;
     p.record(EV_CDONE + s, HostPipe::RUN);   // behind chunk k's last kernel
     p.mark("run_end", k, HostPipe::RUN);
     p.wait(HostPipe::OUT, EV_CDONE + s);
-    p.d2h((unsigned char *)y + (size_t)u0 * out_row, dout[slot], (size_t)m * out_row);
+    p.d2h((unsigned char *)y + o0, dout[slot], o1 - o0);
     p.record(EV_OUT + slot, HostPipe::OUT);
     p.mark("d2h_end", k, HostPipe::OUT);
   }
@@ -474,6 +477,25 @@ int chunk_pipeline(WorldB200 *h, const char *who, int n_utts, int chunk, int rin
   rc = p.finish(rc, header);
   if (!rc) rc = world_b200_synchronize(h);
   return rc;
+}
+
+// chunk_pipeline's chunks of `chunk` utterances (the last one shorter), their outputs whole rows of `row` bytes, and
+// whether a chunk's rows need zeroing: a row past its utterance's y_len
+std::vector<int> even_bounds(int n_utts, int chunk) {
+  std::vector<int> b;
+  for (int u = 0; u < n_utts; u += chunk) b.push_back(u);
+  b.push_back(n_utts);
+  return b;
+}
+auto padded_at(size_t row) {
+  return [row](int u) { return (size_t)u * row; };
+}
+auto ragged_rows(const int *y_len, int y_stride) {
+  return [y_len, y_stride](int c0, int c1) {
+    for (int u = c0; u < c1; ++u)
+      if (y_len[u] != y_stride) return true;
+    return false;
+  };
 }
 
 // Synthesis from coded rows for host arrays: f0 + coded rows in, synthesis_run on each chunk, waveforms out, through
@@ -510,7 +532,60 @@ int synthesis_pipeline(WorldB200 *h, const SynthesisPlan &plan, const SynthesisR
     return synthesis_run(ctx, plan, u0, m, {(const double *)(d + o_f0), (const double *)(d + o_sp),
                                             (const double *)(d + o_ap), out});
   };
-  return chunk_pipeline(h, "synthesis", n_utts, chunk, ring, in_plan.total, per_out, plan.y_len.data(), plan.y_stride,
+  return chunk_pipeline(h, "synthesis", even_bounds(n_utts, chunk), ring, in_plan.total, (size_t)chunk * per_out,
+                        padded_at(per_out), ragged_rows(plan.y_len.data(), plan.y_stride), plan.nbit, host.y, upload,
+                        run);
+}
+
+// The packed form for host arrays: chunk k is utterances [c0, c1) whose frames [f_off[c0], f_off[c1]) of each input array
+// go up as one copy and whose samples [y_off[c0], y_off[c1]) come back as one copy.  A chunk is one packed pass of
+// synthesis_run (at most WB_HOST_CHUNK utterances when that is set), and two input sets and the output ring stay within
+// a third of the scratch budget.
+int synthesis_packed_pipeline(WorldB200 *h, const SynthesisPlan &plan, const SynthesisRows &host) {
+  Ctx *ctx = &h->c;
+  const int n_utts = plan.n, dims = plan.dims, n_ap = plan.n_ap;
+  const long long *fo = plan.f_off.data(), *yo = plan.y_off.data();
+  const size_t out_bytes = plan.nbit ? 2 : 8, per_frame = (size_t)(1 + dims + n_ap) * 8;
+  const SynthesisSizing sz(ctx, plan, plan.y_stride);
+  const int ring = 3;
+  const double third = (double)(ctx->scratch_budget / 3);
+  int most = 65535;
+  if (const char *e = getenv("WB_HOST_CHUNK")) most = atoi(e) > 0 ? imin(most, atoi(e)) : most;
+  std::vector<int> bounds{0};
+  size_t most_frames = 0, most_samples = 0;
+  while (bounds.back() < n_utts) {
+    const int c0 = bounds.back();
+    double pass = (double)sz.packed_pass();
+    int c1 = c0;
+    while (c1 < n_utts && c1 - c0 < most) {
+      const double next = pass + (double)sz.packed_utt(plan.y_len[c1], plan.f_len[c1], sz.cap_of(plan.y_len[c1]));
+      const double io = 2.0 * (double)(fo[c1 + 1] - fo[c0]) * per_frame + ring * (double)(yo[c1 + 1] - yo[c0]) * out_bytes;
+      if (c1 > c0 && (next > sz.budget || io > third)) break;
+      pass = next;
+      ++c1;
+    }
+    bounds.push_back(c1);
+    most_frames = std::max(most_frames, (size_t)(fo[c1] - fo[c0]));
+    most_samples = std::max(most_samples, (size_t)(yo[c1] - yo[c0]));
+  }
+  ArenaPlan in_plan;
+  const size_t o_f0 = in_plan.add(most_frames * 8);
+  const size_t o_sp = in_plan.add(most_frames * dims * 8);
+  const size_t o_ap = in_plan.add(most_frames * n_ap * 8);
+  // the chunk's frames of f0 and of the coded rows, one copy each
+  auto upload = [&](HostPipe &p, int u0, int m, unsigned char *d) {
+    const size_t frames = (size_t)(fo[u0 + m] - fo[u0]), f0 = (size_t)fo[u0];
+    p.h2d(d + o_f0, host.f0 + f0, frames * 8);
+    p.h2d(d + o_sp, host.sp + f0 * dims, frames * dims * 8);
+    if (n_ap) p.h2d(d + o_ap, host.ap + f0 * n_ap, frames * n_ap * 8);
+  };
+  auto run = [&](int u0, int m, unsigned char *d, unsigned char *out) {
+    return synthesis_run(ctx, plan, u0, m, {(const double *)(d + o_f0), (const double *)(d + o_sp),
+                                            (const double *)(d + o_ap), out});
+  };
+  auto out_at = [&](int u) { return (size_t)yo[u] * out_bytes; };
+  auto zero = [](int, int) { return false; };   // every sample of the chunk is written
+  return chunk_pipeline(h, "synthesis_packed", bounds, ring, in_plan.total, most_samples * out_bytes, out_at, zero,
                         plan.nbit, host.y, upload, run);
 }
 
@@ -533,8 +608,9 @@ int transform_pipeline(WorldB200 *h, const ChainRequest &r, const TransformPlan 
   auto run = [&](int u0, int m, unsigned char *d, unsigned char *out) {
     return transform_run(h, r, tp, d, u0, m, out);
   };
-  return chunk_pipeline(h, "transform", n_utts, chunk, 2, (size_t)chunk * per_in, per_out, tp.syn.y_len.data(),
-                        tp.syn.y_stride, tp.syn.nbit, y, upload, run);
+  return chunk_pipeline(h, "transform", even_bounds(n_utts, chunk), 2, (size_t)chunk * per_in, (size_t)chunk * per_out,
+                        padded_at(per_out), ragged_rows(tp.syn.y_len.data(), tp.syn.y_stride), tp.syn.nbit, y, upload,
+                        run);
 }
 
 // world_b200_synthesis_coded_host and, with f0_scale / spectral_ratio, world_b200_synthesis_coded_host_modified: every
@@ -558,6 +634,29 @@ int synthesis_coded_host(WorldB200 *h, const double *f0, const int *f0_lengths, 
 }
 
 }  // namespace
+
+extern "C" int world_b200_synthesis_coded_host_packed(WorldB200 *h, const double *f0, int n_utts,
+                                                      const long long *f_offsets,
+                                                      const double *coded_spectral_envelope, int number_of_dimensions,
+                                                      const double *coded_aperiodicity, const int *fft_sizes,
+                                                      double frame_period, int fs, const long long *y_offsets,
+                                                      const double *f0_scale, const double *spectral_ratio, int nbit,
+                                                      void *y) {
+  if (!h) return WORLD_B200_EINVAL;
+  if (n_utts == 0) return 0;
+  DeviceGuard guard_(&h->c);
+  if (!f_offsets || !y_offsets) {
+    h->c.last_error = "Synthesis: f_offsets and y_offsets must be given";
+    return WORLD_B200_EINVAL;
+  }
+  SynthesisRequest r{f0, nullptr, n_utts, 0, coded_spectral_envelope, coded_aperiodicity, 0, frame_period, fs, nullptr,
+                     0, y, nbit};
+  r.coded = true; r.dims = number_of_dimensions; r.f0_scale = f0_scale; r.spectral_ratio = spectral_ratio;
+  r.per_utt = true; r.fft_sizes = fft_sizes; r.f_offsets = f_offsets; r.y_offsets = y_offsets;
+  SynthesisPlan plan;
+  const int rc = synthesis_plan(&h->c, r, "Synthesis", &plan);
+  return rc ? rc : synthesis_packed_pipeline(h, plan, {r.f0, r.sp, r.ap, r.y});
+}
 
 extern "C" int world_b200_synthesis_coded_host(WorldB200 *h, const double *f0, const int *f0_lengths, int n_utts,
                                                int f0_stride, const double *coded_spectral_envelope,

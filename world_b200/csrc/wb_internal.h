@@ -86,6 +86,17 @@ inline int balanced_chunk(int n, int fit) {
   const int passes = (n + fit - 1) / fit;
   return (n + passes - 1) / passes;
 }
+// The u in [0, n) with off[u] <= x < off[u + 1] for ascending off with off[0] <= x < off[n]: the largest u with
+// off[u] <= x, so that empty entries are passed over.
+WB_HD inline int packed_find(const long long *off, int n, long long x) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (off[mid] <= x) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
 struct ArenaPlan {                                   // lay out 256-byte aligned sub-blocks
   size_t total = 0;
   size_t add(size_t bytes) { const size_t off = total; total += (bytes + 255) & ~(size_t)255; return off; }
@@ -104,11 +115,14 @@ int dev_check(Ctx *ctx, const char *what);      // cudaGetLastError -> last_erro
 
 // wb_rng.cu
 void rng_build_jump_tables(uint32_t *tables);
-// draws [first, totals[u]) of utterance u's stream into out + u * utt_stride (first = 0 in the stages)
+// draws [first, totals[u]) of utterance u's stream into out + u * utt_stride (first = 0 in the stages), or with
+// utt_off (device, [n_utts]) into out + utt_off[u]
 void rng_fill(const Ctx *ctx, const unsigned *totals_dev, unsigned *out, size_t utt_stride,
-              size_t max_draws_per_utt, int n_utts, unsigned first = 0);
+              size_t max_draws_per_utt, int n_utts, unsigned first = 0, const long long *utt_off = nullptr);
+// counts / offsets of utterance u at u * stride, or with utt_off (device, [n_utts]) at utt_off[u]
 void scan_counts(const Ctx *ctx, const unsigned *counts, const int *lens_dev, int stride,
-                 const unsigned *base, unsigned *offsets, unsigned *totals, int n_utts);
+                 const unsigned *base, unsigned *offsets, unsigned *totals, int n_utts,
+                 const long long *utt_off = nullptr);
 
 // wb_multi.cu: NCCL communicator behind the C ABI (bound at run time)
 struct Comm;
@@ -169,6 +183,12 @@ struct CodecDeviceTables { const int *idx; const double *frac; const double2 *we
 void codec_decode_launch(Ctx *ctx, bool spectral_envelope, const CodecTables &t, const CodecDeviceTables &d,
                          int fft_size, const int *f_len, int n_utts, int f_stride, int max_f, const double *in,
                          double *out, const int *list = nullptr, int out_row = 0);
+// The same over packed rows, one CTA per frame: utterance u's frame i is row f_off[u] + i of both in and out (device,
+// [n + 1]; f_len: device, [n]).  The launch decodes `frames` frames: entry j of list (list_n entries; NULL: utterance j)
+// owns frames cum[j] .. cum[j + 1] - 1 of the grid (cum: device, [list_n + 1]).
+void codec_decode_packed_launch(Ctx *ctx, bool spectral_envelope, const CodecTables &t, const CodecDeviceTables &d,
+                                int fft_size, const int *f_len, const long long *f_off, const int *list, int list_n,
+                                const long long *cum, long long frames, const double *in, double *out, int out_row);
 // wb_synthesis.cu: F0 scaling and spectral stretch (the reference demo's ParameterModification, test.cpp:221-258).
 // The interp1 segment and weight of each output bin depend only on (ratio, fft_size, fs), so they are planned on the
 // host once per distinct (ratio, fft_size); the tail rule (bins >= c copy bin c-1 when ratio < 1) is folded into the
@@ -190,19 +210,21 @@ int modify_plan(Ctx *ctx, const char *who, int n_utts, int fft_size, int fs, con
 // Plan entries [u0, u0 + n) in device memory (layout of device_bytes); the copies are enqueued on ctx->stream.
 struct ModifyDevice { const double *scale; const int *table; const int *idx; const double *frac; const int *tbins, *toff; };
 int modify_upload(Ctx *ctx, const ModifyPlan &plan, int u0, int n, unsigned char *blk, ModifyDevice *d);
-// f0_out[u][i] = f0_in[u][i] * scale[u] for i < f_len[u] (f0_out may alias f0_in)
+// f0_out[u][i] = f0_in[u][i] * scale[u] for i < f_len[u] (f0_out may alias f0_in).  f_off (device, [n_utts + 1]):
+// packed rows, utterance u's frame i at f_off[u] + i; NULL: padded rows of f_stride.
 void modify_f0_launch(Ctx *ctx, const ModifyDevice &d, const int *f_len, int n_utts, int f_stride, int max_f,
-                      const double *f0_in, double *f0_out);
+                      const double *f0_in, double *f0_out, const long long *f_off = nullptr);
 // the envelope rows [n][f_stride][row] stretched in place, frames < f_len[u], the first bins of the utterance's table
-// of each row (max_bins: the plan's largest)
+// of each row (max_bins: the plan's largest); f_off as for modify_f0_launch
 void modify_stretch_launch(Ctx *ctx, const ModifyDevice &d, int row, int max_bins, const int *f_len, int n_utts,
-                           int f_stride, int max_f, double *spectrogram);
+                           int f_stride, int max_f, double *spectrogram, const long long *f_off = nullptr);
 
 // Both halves of the plan on the device rows of its utterances [u0, u0 + n_utts) in place (f0 [n][f0_stride],
 // spectrogram [n][f0_stride][row], row >= plan.bins; host lengths), frames < f0_lengths[u]: world_b200_modify_batch's
 // launches.
+// f_offsets (host, [n_utts + 1]): packed rows, utterance u's frame i at row f_offsets[u] + i (f0_stride is not read).
 int modify_run(Ctx *ctx, const ModifyPlan &plan, int u0, int n_utts, const int *f0_lengths, int f0_stride, int row,
-               double *f0, double *spectrogram);
+               double *f0, double *spectrogram, const long long *f_offsets = nullptr);
 
 // out[u] = lengths[u] (NULL: stride) for u < n; EINVAL "<who>: <rows>_lengths[u] = v is outside [least, <rows>_stride =
 // stride] (utterance u)" for the first one outside
@@ -238,6 +260,10 @@ struct SynthesisRequest {   // brace-initialised in field order up to nbit
   bool per_utt = false;
   const int *fft_sizes = nullptr;
   int row_stride = 0;
+  // packed (per_utt): utterance u is frames [f_offsets[u], f_offsets[u + 1]) of f0 / sp / ap and samples
+  // [y_offsets[u], y_offsets[u + 1]) of y (host arrays, n + 1 entries); f0_lengths, y_lengths and the strides are not
+  // read, and row_stride 0 is the largest fft_sizes[u] / 2 + 1
+  const long long *f_offsets = nullptr, *y_offsets = nullptr;
 };
 // Everything synthesis_run reads besides the rows, made once per call and const afterwards.
 // Sizes: every per-size member has one entry per distinct fft_size of the call, in order of first appearance (one
@@ -259,24 +285,35 @@ struct SynthesisPlan {
   ModifyPlan mod;
   std::vector<double> fp;           // [n] frame period (s) of each utterance, or empty: frame_period / 1000.0 for all
   std::vector<std::vector<double>> dc_remover;   // per size: [fft_size] GetDCRemover (synthesis.cpp:319-333)
+  // packed rows: [n + 1] frame and sample offsets (f_len / y_len derived from them); empty: padded rows
+  std::vector<long long> f_off, y_off;
+  bool packed() const { return !f_off.empty(); }
 };
 // Every check of a synthesis call before anything is queued, in this order: the pointers, n, fs and frame_period;
 // nbit; fft_size (per_utt: each utterance's, a power of two in [16, 4096]); per_utt full rows: row_stride against each
 // utterance's bins; the coded decode tables (per_utt: number_of_dimensions in [1, fft_sizes[u] / 2]); the factors
-// (modify_plan); each utterance's f0 and y lengths (2 .. stride).  EINVAL with last_error "<who>: ...", naming the
-// first bad utterance where there is one.
+// (modify_plan); each utterance's f0 and y lengths (2 .. stride; packed: the offsets start at 0 and give each
+// utterance 2 .. INT_MAX frames and samples).  EINVAL with last_error "<who>: ...", naming the first bad utterance where
+// there is one.
 int synthesis_plan(Ctx *ctx, const SynthesisRequest &r, const char *who, SynthesisPlan *p);
 // Per-utterance scratch of synthesis_run for rows whose longest y_length is max_y; fit(nominal_cap) utterances make one
 // pass when no utterance has more than 1,200 pulses per second.
+// A packed pass holds each utterance's own scratch instead: packed_utt(y_len, f_len, cap) bytes for an utterance of
+// y_len samples and f_len frames with room for cap pulses (cap_of(y_len) when it has at most 1,200 per second), plus
+// packed_pass bytes per pass.
 struct SynthesisSizing {
   SynthesisSizing(const Ctx *ctx, const SynthesisPlan &p, int max_y);
   size_t per_utt(int cap) const;
   int fit(int cap) const;
-  int fft_size, y_stride, nominal_cap;   // fft_size: the plan's largest, the stride of each response
-  size_t decoded_per_utt, draw_stride;
+  int cap_of(int y_len) const;
+  size_t packed_utt(int y_len, int f_len, int cap) const;
+  size_t packed_pass() const;
+  int fft_size, y_stride, nominal_cap, fs;   // fft_size: the plan's largest, the stride of each response
+  size_t decoded_per_utt, draw_stride, decoded_per_frame;
   double budget;
 };
-// The rows of utterances [u0, u0 + m) of a planned call: device pointers at utterance u0, laid out as the request's
+// The rows of utterances [u0, u0 + m) of a planned call: device pointers at utterance u0 (packed: at its first frame
+// and first sample), laid out as the request's
 // (sp / ap: full or coded rows, as the plan says; coded ap is not read below 12 kHz, where there are no bands).
 struct SynthesisRows {
   const double *f0, *sp, *ap;

@@ -93,12 +93,14 @@ WB_DEV unsigned rng_draw(uint4 &s) {
 // 32 chunks of WB_RNG_CHUNK draws = 4096 consecutive draws, stored coalesced via a smem tile.
 // Draws [first, totals[u]) of the stream, draw d at out[u * utt_stride + d - first]; the stages
 // pass first = 0, the window hook any first.  Every total is at most WB_RNG_REACH (scan_counts
-// clamps and flags larger ones), so chunk g < 2^WB_RNG_NJ and no draw index wraps.
+// clamps and flags larger ones), so chunk g < 2^WB_RNG_NJ and no draw index wraps.  utt_off: the
+// utterances' draws packed, utterance u's from out + utt_off[u] (null: out + u * utt_stride).
 WB_KERNEL_PLAIN rng_fill_kernel(const uint4 *__restrict__ jump, const unsigned *__restrict__ totals,
-                                unsigned *__restrict__ out, size_t utt_stride, unsigned first) {
+                                unsigned *__restrict__ out, size_t utt_stride, unsigned first,
+                                const long long *__restrict__ utt_off) {
   const int utt = blockIdx.y;
   const unsigned total = totals[utt];
-  unsigned *dst = out + (size_t)utt * utt_stride;
+  unsigned *dst = out + (utt_off ? (size_t)utt_off[utt] : (size_t)utt * utt_stride);
   const unsigned chunk0 = first / WB_RNG_CHUNK;
   // draw d goes to dst[d - first] if d - first < span: one unsigned compare (d < first wraps past span)
   const unsigned span = total > first ? total - first : 0u;
@@ -139,7 +141,7 @@ WB_KERNEL_PLAIN rng_fill_kernel(const uint4 *__restrict__ jump, const unsigned *
 }
 
 void rng_fill(const Ctx *ctx, const unsigned *totals_dev, unsigned *out, size_t utt_stride,
-              size_t max_draws_per_utt, int n_utts, unsigned first) {
+              size_t max_draws_per_utt, int n_utts, unsigned first, const long long *utt_off) {
   if (max_draws_per_utt > WB_RNG_REACH) max_draws_per_utt = WB_RNG_REACH;   // totals never exceed the reach
   if (n_utts <= 0 || max_draws_per_utt <= first) return;
   const size_t chunk0 = first / WB_RNG_CHUNK;
@@ -147,7 +149,7 @@ void rng_fill(const Ctx *ctx, const unsigned *totals_dev, unsigned *out, size_t 
   const unsigned per_block = 32 * WB_RNG_WARPS;
   dim3 grid((unsigned)((chunks + per_block - 1) / per_block), (unsigned)n_utts);
   WB_LAUNCH_FLAT(rng_fill_kernel, grid, per_block, 0, ctx->stream,
-                 reinterpret_cast<const uint4 *>(ctx->rng_jump), totals_dev, out, utt_stride, first);
+                 reinterpret_cast<const uint4 *>(ctx->rng_jump), totals_dev, out, utt_stride, first, utt_off);
 }
 
 // ------------------------------------------------------------------ per-utterance scans
@@ -155,15 +157,17 @@ void rng_fill(const Ctx *ctx, const unsigned *totals_dev, unsigned *out, size_t 
 // offset, used by D4C's second pass which continues the stream after the first pass).  The sums
 // run in 64 bits: a total beyond WB_RNG_REACH sets status bit 8 (world_b200_synchronize reports
 // WORLD_B200_EDOMAIN) and is stored clamped to the reach, so rng_fill never repeats the stream.
+// utt_off: utterance u's counts and offsets start at utt_off[u] (packed; null: at u * stride).
 WB_KERNEL_PLAIN scan_counts_kernel(const unsigned *__restrict__ counts, const int *__restrict__ lens,
                                    int stride, const unsigned *__restrict__ base,
                                    unsigned *__restrict__ offsets, unsigned *__restrict__ totals,
-                                   int *__restrict__ status) {
+                                   int *__restrict__ status, const long long *__restrict__ utt_off) {
   WB_SHARED unsigned long long part[1025];
   const int utt = blockIdx.x, tid = WB_TID, nth = WB_NTH;
   const int len = lens[utt];
-  const unsigned *c = counts + (size_t)utt * stride;
-  unsigned *o = offsets + (size_t)utt * stride;
+  const size_t at = utt_off ? (size_t)utt_off[utt] : (size_t)utt * stride;
+  const unsigned *c = counts + at;
+  unsigned *o = offsets + at;
   const int chunk = (len + nth - 1) / nth;
   const int lo = imin(len, tid * chunk), hi = imin(len, lo + chunk);
   unsigned long long s = 0;
@@ -185,10 +189,11 @@ WB_KERNEL_PLAIN scan_counts_kernel(const unsigned *__restrict__ counts, const in
 }
 
 void scan_counts(const Ctx *ctx, const unsigned *counts, const int *lens_dev, int stride,
-                 const unsigned *base, unsigned *offsets, unsigned *totals, int n_utts) {
+                 const unsigned *base, unsigned *offsets, unsigned *totals, int n_utts,
+                 const long long *utt_off) {
   if (n_utts <= 0) return;
   WB_LAUNCH_COOP(scan_counts_kernel, dim3((unsigned)n_utts), 256, 0, ctx->stream, counts, lens_dev,
-                 stride, base, offsets, totals, ctx->status_dev);
+                 stride, base, offsets, totals, ctx->status_dev, utt_off);
 }
 
 }  // namespace wb

@@ -20,6 +20,7 @@
 #include "wb_spectral.cuh"
 #include "../../include/world/matlabfunctions.h"
 #include <algorithm>
+#include <climits>
 #include <map>
 #include <stdio.h>
 #include <type_traits>
@@ -60,21 +61,39 @@ struct SynParams {
   const double2 *tw;
   int *status;
   short *y16;               // [n][y_stride] 16-bit PCM output (syn_overlap_kernel<short>), else null
+  // A packed pass (null: the padded addressing above).  [n + 1] offsets from the pass's first utterance:
+  const long long *f_off;   // frames: f0, sp and ap rows of utterance u start at frame f_off[u]
+  const long long *s_off;   // samples: phase, vuv and y; utterance u's draws start at s_off[u] + 8u
+  const long long *p_off;   // pulse slots: pulse_idx, pulse_shift, draw counts / offsets and responses (its capacity
+                            // is p_off[u + 1] - p_off[u])
+  const long long *cum;     // syn_pulse_kernel: [list_n + 1] first pulse of each entry of `list`; blockIdx.x is the pulse
+  int list_n;               // of the launch's size group
+  int n_utts;               // utterances of the pass (syn_overlap_kernel's flat grid)
 };
 
+// Where utterance u's entries start: its packed offset, or u rows of `stride` in a padded pass
+WB_HD inline size_t syn_at(const long long *off, int u, size_t stride) { return off ? (size_t)off[u] : (size_t)u * stride; }
+
+// Packed: the pass's utterances are packed (SynParams::f_off, s_off, p_off); the padded instantiation compiles without
+// the offsets, as before they existed.
+template <bool Packed>
 WB_KERNEL(256, 2) syn_timebase_kernel(SynParams p) {
   WB_SHARED int cnt[258];
   const int tid = WB_TID, nth = WB_NTH, u = blockIdx.x;
+  const long long *f_off = Packed ? p.f_off : nullptr, *s_off = Packed ? p.s_off : nullptr;
+  const long long *p_off = Packed ? p.p_off : nullptr;
   const int L = p.f_len[u], n = p.y_len[u], fs = p.fs;
   const double fp = p.fp_u ? p.fp_u[u] : p.frame_period;
   const int N = p.fft_u ? p.fft_u[u] : p.fft_size;
   const double lowest_f0 = fs / N + 1.0;   // synthesis.cpp:362 (integer division, then + 1.0)
-  const double *f0 = p.f0 + (size_t)u * p.f_stride;
-  double *phase = p.phase + (size_t)u * p.y_stride;
-  double *vuv = p.vuv + (size_t)u * p.y_stride;
-  int *pidx = p.pulse_idx + (size_t)u * p.pulse_cap;
-  double *pshift = p.pulse_shift + (size_t)u * p.pulse_cap;
-  unsigned *dcnt = p.draw_cnt + (size_t)u * p.pulse_cap;
+  const double *f0 = p.f0 + syn_at(f_off, u, p.f_stride);
+  double *phase = p.phase + syn_at(s_off, u, p.y_stride);
+  double *vuv = p.vuv + syn_at(s_off, u, p.y_stride);
+  const size_t p0 = syn_at(p_off, u, p.pulse_cap);
+  const int cap = Packed ? (int)(p_off[u + 1] - p_off[u]) : p.pulse_cap;
+  int *pidx = p.pulse_idx + p0;
+  double *pshift = p.pulse_shift + p0;
+  unsigned *dcnt = p.draw_cnt + p0;
   // coarse arrays are f0 thresholded; the extra point L is extrapolated (:238-245).  They are read
   // through a small accessor instead of being materialised.
 #define WB_CF0(i) (f0[(i)] < lowest_f0 ? 0.0 : f0[(i)])
@@ -120,15 +139,15 @@ WB_KERNEL(256, 2) syn_timebase_kernel(SynParams p) {
     int run = 0;
     for (int t = 0; t < nth; ++t) { const int v = cnt[t]; cnt[t] = run; run += v; }
     cnt[nth] = run;
-    p.n_pulses[u] = imin(run, p.pulse_cap);
-    p.pulse_count[u] = run;   // run > pulse_cap: the host lays the chunk out again before anything reads the list
-    if (run > p.pulse_cap) atomicOr_status(p.status, 4);   // status is null unless the counts sized this layout
+    p.n_pulses[u] = imin(run, cap);
+    p.pulse_count[u] = run;   // run > cap: the host lays the chunk out again before anything reads the list
+    if (run > cap) atomicOr_status(p.status, 4);   // status is null unless the counts sized this layout
   }
   WB_SYNC();
   int k = cnt[tid];
   for (int i = lo; i < hi; ++i) {
     if (fabs(phase[i + 1] - phase[i]) > kPi) {
-      if (k < p.pulse_cap) {
+      if (k < cap) {
         pidx[k] = i;
         const double y1 = phase[i] - 2.0 * kPi, y2 = phase[i + 1];
         pshift[k] = (-y1 / (y2 - y1)) / fs;
@@ -138,8 +157,8 @@ WB_KERNEL(256, 2) syn_timebase_kernel(SynParams p) {
   }
   WB_SYNC();
   // noise_size = idx[min(np-1, i+1)] - idx[i] draws per pulse (:372-374, :19-25)
-  const int np = imin(cnt[nth], p.pulse_cap);
-  for (int i = tid; i < p.pulse_cap; i += nth)
+  const int np = imin(cnt[nth], cap);
+  for (int i = tid; i < cap; i += nth)
     dcnt[i] = (i < np) ? (unsigned)(pidx[imin(np - 1, i + 1)] - pidx[i]) : 0u;
 }
 
@@ -181,10 +200,15 @@ WB_DEV void syn_c2r(const double2 *spec, double2 *z, int N, int lg, const double
   cfft_forward(z, lg, tw);
 }
 
+template <bool Packed>
 WB_KERNEL(128, 3) syn_pulse_kernel(SynParams p) {
   WB_DYN_SMEM(double, smem);
   const int tid = WB_TID, nth = WB_NTH;
-  const int u = p.list ? p.list[blockIdx.y] : blockIdx.y, pi = blockIdx.x;
+  const long long *f_off = Packed ? p.f_off : nullptr, *s_off = Packed ? p.s_off : nullptr;
+  const long long *p_off = Packed ? p.p_off : nullptr, *cum = Packed ? p.cum : nullptr;
+  // a packed pass launches one CTA per pulse of the group: entry j of the list owns CTAs [cum[j], cum[j + 1])
+  const int j = Packed ? packed_find(cum, p.list_n, (long long)blockIdx.x) : (int)blockIdx.y;
+  const int u = p.list ? p.list[j] : j, pi = Packed ? (int)(blockIdx.x - cum[j]) : (int)blockIdx.x;
   const int np = p.n_pulses[u];
   if (pi >= np) return;
   const int N = p.fft_size, half = N / 2, lg = p.lg_fft, fs = p.fs;
@@ -197,15 +221,17 @@ WB_KERNEL(128, 3) syn_pulse_kernel(SynParams p) {
   double *red = per + N;                                          // WB_RED_DOUBLES
 
   const int L = p.f_len[u];
-  const int idx = p.pulse_idx[(size_t)u * p.pulse_cap + pi];
-  const int idx_next = p.pulse_idx[(size_t)u * p.pulse_cap + imin(np - 1, pi + 1)];
+  const size_t p0 = syn_at(p_off, u, p.pulse_cap);
+  const int idx = p.pulse_idx[p0 + pi];
+  const int idx_next = p.pulse_idx[p0 + imin(np - 1, pi + 1)];
   const int noise_size = idx_next - idx;
-  const double shift = p.pulse_shift[(size_t)u * p.pulse_cap + pi];
-  const double current_vuv = p.vuv[(size_t)u * p.y_stride + idx];
+  const double shift = p.pulse_shift[p0 + pi];
+  const double current_vuv = p.vuv[syn_at(s_off, u, p.y_stride) + idx];
   const double current_time = idx / static_cast<double>(fs);
-  double *resp = p.resp + ((size_t)u * p.pulse_cap + pi) * p.resp_n;
+  double *resp = p.resp + (p0 + pi) * p.resp_n;
   const size_t bins = p.row;
-  const double *sp = p.sp + (size_t)u * p.f_stride * bins, *ap = p.ap + (size_t)u * p.f_stride * bins;
+  const size_t r0 = syn_at(f_off, u, p.f_stride) * bins;
+  const double *sp = p.sp + r0, *ap = p.ap + r0;
 
   // GetSpectralEnvelope / GetAperiodicRatio (:140-179)
   const double fp = p.fp_u ? p.fp_u[u] : p.frame_period;
@@ -257,7 +283,8 @@ WB_KERNEL(128, 3) syn_pulse_kernel(SynParams p) {
 
   // ---- aperiodic response (:36-69)
   if (noise_size > 0) {
-    const unsigned *draw = p.draws + (size_t)u * p.draw_stride + p.draw_off[(size_t)u * p.pulse_cap + pi];
+    const size_t d0 = Packed ? (size_t)s_off[u] + 8 * (size_t)u : (size_t)u * p.draw_stride;
+    const unsigned *draw = p.draws + d0 + p.draw_off[p0 + pi];
     double s = 0.0;
     for (int i = tid; i < N + 2; i += nth) {
       const double v = (i < noise_size && i < N) ? randn_value(draw[i]) : 0.0;
@@ -304,24 +331,35 @@ WB_HD inline short pcm16_of(double v) {
 }
 
 // Out = double: the waveform (p.y); Out = short: its 16-bit PCM (p.y16), the sum never reaching memory
+// Padded: (sample, utterance) -> thread over a (max_y, n) grid.  Packed: one flat grid over the pass's samples, each
+// thread finding its utterance in s_off.
 template <typename Out>
 WB_KERNEL_PLAIN syn_overlap_kernel(SynParams p) {
-  const int u = blockIdx.y;
-  const int s = blockIdx.x * blockDim.x + threadIdx.x;
-  const int n = p.y_len[u];
-  if (s >= n) return;
+  int u, s;
+  if (p.s_off) {
+    const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= p.s_off[p.n_utts]) return;
+    u = packed_find(p.s_off, p.n_utts, g);
+    s = (int)(g - p.s_off[u]);
+  } else {
+    u = blockIdx.y;
+    s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= p.y_len[u]) return;
+  }
   const int N = p.fft_u ? p.fft_u[u] : p.fft_size, half = N / 2, np = p.n_pulses[u];
-  const int *pidx = p.pulse_idx + (size_t)u * p.pulse_cap;
+  const size_t p0 = syn_at(p.p_off, u, p.pulse_cap);
+  const int *pidx = p.pulse_idx + p0;
   // pulse i covers samples idx_i - half + 1 .. idx_i + half  ->  idx_i in [s - half, s + half - 1]
   int lo = 0, hi = np;
   while (lo < hi) { const int mid = (lo + hi) >> 1; if (pidx[mid] < s - half) lo = mid + 1; else hi = mid; }
   double acc = 0.0;
   for (int i = lo; i < np && pidx[i] <= s + half - 1; ++i) {
     const int j = s - (pidx[i] - half + 1);
-    acc += p.resp[((size_t)u * p.pulse_cap + i) * p.resp_n + j];
+    acc += p.resp[(p0 + i) * p.resp_n + j];
   }
-  if constexpr (std::is_same<Out, short>::value) p.y16[(size_t)u * p.y_stride + s] = pcm16_of(acc);
-  else p.y[(size_t)u * p.y_stride + s] = acc;
+  const size_t at = syn_at(p.s_off, u, p.y_stride) + s;
+  if constexpr (std::is_same<Out, short>::value) p.y16[at] = pcm16_of(acc);
+  else p.y[at] = acc;
 }
 
 // ---- voice modification --------------------------------------------------------------------------------------------
@@ -347,15 +385,17 @@ WB_KERNEL_PLAIN syn_overlap_kernel(SynParams p) {
 
 // Rows of frames >= f_len[u] (and utterances >= n_utts) are never touched.  The `continue` is uniform over the CTA.
 // Each frame row holds `row` doubles, of which the utterance's table covers the first tbins[t].
+// f_off: [n_utts + 1] frame offsets of packed rows (utterance u's frame f at row f_off[u] + f), or null: padded rows.
 WB_KERNEL(WB_MODIFY_THREADS, 8) modify_stretch_kernel(double *sp, const int *__restrict__ f_len, int n_utts,
                                                       int f_stride, int row_len, const int *__restrict__ table,
                                                       const int *__restrict__ tbins, const int *__restrict__ toff,
-                                                      const int *__restrict__ idx, const double *__restrict__ frac) {
+                                                      const int *__restrict__ idx, const double *__restrict__ frac,
+                                                      const long long *__restrict__ f_off) {
   WB_DYN_SMEM(double, logs);   // the largest table's bins
   const int tid = WB_TID, nth = WB_NTH, f = blockIdx.x;
   for (int u = blockIdx.y; u < n_utts; u += gridDim.y) {
     if (f >= f_len[u]) continue;
-    double *row = sp + ((size_t)u * f_stride + f) * row_len;
+    double *row = sp + (syn_at(f_off, u, f_stride) + f) * row_len;
     const int t = __ldg(&table[u]), bins = __ldg(&tbins[t]);
     const size_t t0 = (size_t)__ldg(&toff[t]);
     for (int j = tid; j < bins; j += nth) logs[j] = log(row[j]);
@@ -372,10 +412,14 @@ WB_KERNEL(WB_MODIFY_THREADS, 8) modify_stretch_kernel(double *sp, const int *__r
 }
 
 WB_KERNEL_PLAIN modify_f0_kernel(const double *f0_in, double *f0_out, const double *__restrict__ scale,
-                                 const int *__restrict__ f_len, int n_utts, int f_stride) {
+                                 const int *__restrict__ f_len, int n_utts, int f_stride,
+                                 const long long *__restrict__ f_off) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   for (int u = blockIdx.y; u < n_utts; u += gridDim.y)
-    if (i < f_len[u]) f0_out[(size_t)u * f_stride + i] = __dmul_rn(f0_in[(size_t)u * f_stride + i], scale[u]);
+    if (i < f_len[u]) {
+      const size_t at = syn_at(f_off, u, f_stride) + i;
+      f0_out[at] = __dmul_rn(f0_in[at], scale[u]);
+    }
 }
 
 namespace {
@@ -482,36 +526,40 @@ int modify_upload(Ctx *ctx, const ModifyPlan &plan, int u0, int n, unsigned char
 }
 
 void modify_f0_launch(Ctx *ctx, const ModifyDevice &d, const int *f_len, int n_utts, int f_stride, int max_f,
-                      const double *f0_in, double *f0_out) {
+                      const double *f0_in, double *f0_out, const long long *f_off) {
   if (n_utts <= 0 || max_f <= 0) return;
   const dim3 grid((unsigned)((max_f + 255) / 256), (unsigned)imin(n_utts, 65535));
-  WB_LAUNCH_FLAT(modify_f0_kernel, grid, 256, 0, ctx->stream, f0_in, f0_out, d.scale, f_len, n_utts, f_stride);
+  WB_LAUNCH_FLAT(modify_f0_kernel, grid, 256, 0, ctx->stream, f0_in, f0_out, d.scale, f_len, n_utts, f_stride, f_off);
 }
 
 void modify_stretch_launch(Ctx *ctx, const ModifyDevice &d, int row, int max_bins, const int *f_len, int n_utts,
-                           int f_stride, int max_f, double *spectrogram) {
+                           int f_stride, int max_f, double *spectrogram, const long long *f_off) {
   if (n_utts <= 0 || max_f <= 0) return;
   const dim3 grid((unsigned)max_f, (unsigned)imin(n_utts, 65535));
   WB_LAUNCH_COOP(modify_stretch_kernel, grid, WB_MODIFY_THREADS, (size_t)max_bins * 8, ctx->stream, spectrogram, f_len,
-                 n_utts, f_stride, row, d.table, d.tbins, d.toff, d.idx, d.frac);
+                 n_utts, f_stride, row, d.table, d.tbins, d.toff, d.idx, d.frac, f_off);
 }
 
 int modify_run(Ctx *ctx, const ModifyPlan &plan, int u0, int n_utts, const int *f0_lengths, int f0_stride, int row,
-               double *f0, double *spectrogram) {
+               double *f0, double *spectrogram, const long long *f_offsets) {
   int max_f = 0;
   for (int u = 0; u < n_utts; ++u) max_f = imax(max_f, f0_lengths[u]);
   if (max_f == 0 || (plan.scale.empty() && plan.table.empty())) return 0;
   ArenaPlan a;
   const size_t o_len = a.add((size_t)n_utts * 4), o_mod = a.add(plan.device_bytes(n_utts));
+  const size_t o_off = a.add(f_offsets ? (size_t)(n_utts + 1) * 8 : 0);
   unsigned char *blk = arena_block(ctx, a.total);
   if (!blk) return WORLD_B200_ENOMEM;
   ModifyDevice d;
   int rc = dev_memcpy_h2d(ctx, blk + o_len, f0_lengths, (size_t)n_utts * 4);
   if (!rc) rc = modify_upload(ctx, plan, u0, n_utts, blk + o_mod, &d);
+  if (!rc && f_offsets) rc = dev_memcpy_h2d(ctx, blk + o_off, f_offsets, (size_t)(n_utts + 1) * 8);
   if (rc) return rc;
   const int *f_len = (const int *)(blk + o_len);
-  if (!plan.scale.empty()) modify_f0_launch(ctx, d, f_len, n_utts, f0_stride, max_f, f0, f0);
-  if (!plan.table.empty()) modify_stretch_launch(ctx, d, row, plan.bins, f_len, n_utts, f0_stride, max_f, spectrogram);
+  const long long *f_off = f_offsets ? (const long long *)(blk + o_off) : nullptr;
+  if (!plan.scale.empty()) modify_f0_launch(ctx, d, f_len, n_utts, f0_stride, max_f, f0, f0, f_off);
+  if (!plan.table.empty())
+    modify_stretch_launch(ctx, d, row, plan.bins, f_len, n_utts, f0_stride, max_f, spectrogram, f_off);
   return dev_check(ctx, "modify");
 }
 
@@ -531,6 +579,31 @@ int row_lengths(Ctx *ctx, const char *who, const char *rows, const int *lengths,
   return 0;
 }
 
+// Packed rows: utterance u is entries [off[u], off[u + 1]) of the `rows` arrays; out[u] = its count.  EINVAL "<who>:
+// <rows>_offsets[0] = v is not 0" or "<rows>_offsets gives utterance u v <what>, outside [least, INT_MAX] (utterance
+// u)" for the first one outside.
+int packed_lengths(Ctx *ctx, const char *who, const char *rows, const char *what, const long long *off, int n,
+                   int least, std::vector<int> *out) {
+  char msg[256];
+  if (off[0] != 0) {
+    snprintf(msg, sizeof msg, "%s: %s_offsets[0] = %lld is not 0", who, rows, off[0]);
+    ctx->last_error = msg;
+    return WORLD_B200_EINVAL;
+  }
+  out->resize(n);
+  for (int u = 0; u < n; ++u) {
+    const long long v = off[u + 1] - off[u];
+    if (off[u + 1] < off[u] || v < least || v > INT_MAX) {
+      snprintf(msg, sizeof msg, "%s: %s_offsets gives utterance %d %lld %s, outside [%d, INT_MAX] (utterance %d)", who,
+               rows, u, off[u + 1] < off[u] ? off[u + 1] - off[u] : v, what, least, u);
+      ctx->last_error = msg;
+      return WORLD_B200_EINVAL;
+    }
+    (*out)[u] = (int)v;
+  }
+  return 0;
+}
+
 int synthesis_plan(Ctx *ctx, const SynthesisRequest &r, const char *who, SynthesisPlan *p) {
   auto fail = [&](const std::string &what) {
     ctx->last_error = std::string(who) + ": " + what;
@@ -541,6 +614,8 @@ int synthesis_plan(Ctx *ctx, const SynthesisRequest &r, const char *who, Synthes
     return fail(r.coded ? "f0, coded_spectral_envelope and y must be given"
                         : "f0, spectrogram, aperiodicity and y must be given");
   if (r.per_utt && !r.fft_sizes) return fail("fft_sizes must be given");
+  const bool packed = r.f_offsets || r.y_offsets;
+  if (packed && (!r.f_offsets || !r.y_offsets)) return fail("f_offsets and y_offsets must be given");
   if (r.n < 0) return fail("n_utts must be >= 0");
   if (r.fs <= 0) return fail("fs must be > 0");
   if (r.frame_period <= 0) return fail("frame_period must be > 0");
@@ -563,10 +638,12 @@ int synthesis_plan(Ctx *ctx, const SynthesisRequest &r, const char *who, Synthes
   for (const int f : p->sizes) p->fft_size = imax(p->fft_size, f);
   p->row = p->fft_size / 2 + 1;
   if (r.per_utt && !r.coded) {
-    p->row = r.row_stride;
+    // packed rows of row_stride 0: the largest size's bins, as the packed analysis writes them
+    const int row_stride = packed && r.row_stride == 0 ? p->row : r.row_stride;
+    p->row = row_stride;
     for (int u = 0; u < r.n; ++u)
-      if (r.row_stride < r.fft_sizes[u] / 2 + 1)
-        return fail_u("row_stride = " + std::to_string(r.row_stride) + " is smaller than fft_sizes[" +
+      if (row_stride < r.fft_sizes[u] / 2 + 1)
+        return fail_u("row_stride = " + std::to_string(row_stride) + " is smaller than fft_sizes[" +
                       std::to_string(u) + "] / 2 + 1 = " + std::to_string(r.fft_sizes[u] / 2 + 1), u);
   }
   p->n = r.n; p->f0_stride = r.f0_stride; p->y_stride = r.y_stride; p->fs = r.fs;
@@ -594,9 +671,20 @@ int synthesis_plan(Ctx *ctx, const SynthesisRequest &r, const char *who, Synthes
   if (p->modify)
     rc = modify_plan(ctx, who, r.n, r.fft_size, r.fs, r.f0_scale, r.spectral_ratio, &p->mod,
                      r.per_utt ? r.fft_sizes : nullptr);
-  if (!rc) rc = row_lengths(ctx, who, "f0", r.f0_lengths, r.n, r.f0_stride, 2, &p->f_len);
-  if (!rc) rc = row_lengths(ctx, who, "y", r.y_lengths, r.n, r.y_stride, 2, &p->y_len);
-  if (rc) return rc;
+  if (packed) {
+    if (!rc) rc = packed_lengths(ctx, who, "f", "frames", r.f_offsets, r.n, 2, &p->f_len);
+    if (!rc) rc = packed_lengths(ctx, who, "y", "samples", r.y_offsets, r.n, 2, &p->y_len);
+    if (rc) return rc;
+    p->f_off.assign(r.f_offsets, r.f_offsets + r.n + 1);
+    p->y_off.assign(r.y_offsets, r.y_offsets + r.n + 1);
+    // the strides of a padded batch of these utterances: the sizing of a pass's decode tables and nominal pulse room
+    p->f0_stride = p->y_stride = 0;
+    for (int u = 0; u < r.n; ++u) { p->f0_stride = imax(p->f0_stride, p->f_len[u]); p->y_stride = imax(p->y_stride, p->y_len[u]); }
+  } else {
+    if (!rc) rc = row_lengths(ctx, who, "f0", r.f0_lengths, r.n, r.f0_stride, 2, &p->f_len);
+    if (!rc) rc = row_lengths(ctx, who, "y", r.y_lengths, r.n, r.y_stride, 2, &p->y_len);
+    if (rc) return rc;
+  }
   if (r.transform) p->fp.assign(r.fp, r.fp + r.n);
   // DC remover of each size (GetDCRemover, synthesis.cpp:319-333), host libm like the reference
   p->dc_remover.resize(n_sizes);
@@ -616,7 +704,7 @@ int synthesis_plan(Ctx *ctx, const SynthesisRequest &r, const char *who, Synthes
 }
 
 SynthesisSizing::SynthesisSizing(const Ctx *ctx, const SynthesisPlan &p, int max_y)
-    : fft_size(p.fft_size), y_stride(p.y_stride) {
+    : fft_size(p.fft_size), y_stride(p.y_stride), fs(p.fs) {
   // The coded call holds one chunk's decoded envelope and aperiodicity (16 B per row entry and frame) and the decode
   // tables of every size.
   size_t tables = 0;
@@ -629,11 +717,13 @@ SynthesisSizing::SynthesisSizing(const Ctx *ctx, const SynthesisPlan &p, int max
     tables = tp.total;
   }
   decoded_per_utt = p.coded ? (size_t)p.f0_stride * p.row * 16 : 0;
+  decoded_per_frame = p.coded ? (size_t)p.row * 16 : 0;
   // A modified call also holds the stretch tables, and per utterance its factor, table index and scaled f0 row (the
   // 256-byte alignment of the two small arrays is in the 4096 below).
   if (p.coded && p.modify) {
     tables += p.mod.device_bytes(0);
     decoded_per_utt += (size_t)p.f0_stride * 8 + 12;
+    decoded_per_frame += 8;
   }
   // A call of several sizes holds the DC removers of the others, and per utterance its size and list entry.
   for (size_t g = 1; g < p.sizes.size(); ++g) tables += ((size_t)p.sizes[g] * 8 + 255) & ~(size_t)255;
@@ -652,25 +742,45 @@ size_t SynthesisSizing::per_utt(int cap) const {
 
 int SynthesisSizing::fit(int cap) const { return (int)dmin(65535.0, budget / (double)per_utt(cap)); }
 
+int SynthesisSizing::cap_of(int y_len) const { return (int)((double)y_len / fs * 1200.0) + 64; }
+
+// PassLayout's bytes of one utterance in a packed pass: phase and vuv, its y_len + 8 draws, cap pulse slots (index,
+// shift, draw count and offset) with their responses, its decoded rows, and 128 bytes for its entries of the small
+// arrays (lengths, counts, offsets, factors, size lists)
+size_t SynthesisSizing::packed_utt(int y_len, int f_len, int cap) const {
+  return (size_t)y_len * 16 + ((size_t)y_len + 8) * 4 + (size_t)cap * (4 + 8 + 8 + (size_t)fft_size * 8) +
+         (size_t)f_len * decoded_per_frame + 128;
+}
+
+// the 256-byte alignment of a packed pass's sub-blocks
+size_t SynthesisSizing::packed_pass() const { return (size_t)64 * 256; }
+
 namespace {
 // The scratch block of one pass of n utterances with room for cap pulses each.  Per size g: its DC remover and (coded)
 // its decode tables.
+// A padded pass gives every utterance y_stride samples, cap pulse slots, f0_stride frames and draw_stride draws; a packed
+// pass gives each its own, back to back: the pass's totals are samples, pulses, frames and draws, and it also holds the
+// [n + 1] frame, sample, pulse and draw offsets and the [n + G] per-group prefixes of pulses and frames.
 struct PassLayout {
   size_t len, phase, vuv, pidx, psh, np, cnt, dcnt, doff, dtot, pl, draws, resp;
   std::vector<size_t> dcr, sidx, sfrac, sw, aidx, afrac;
   size_t dsp = 0, dap = 0;   // coded
   size_t mod = 0, f0m = 0, fp = 0, fft_u = 0, list = 0, total;
-  PassLayout(const SynthesisPlan &p, int n, int cap, size_t draw_stride) {
-    const size_t N = n, frames = N * p.f0_stride, G = p.sizes.size();
+  size_t offs = 0, cums = 0;   // packed
+  PassLayout(const SynthesisPlan &p, int n, int cap, size_t draw_stride)
+      : PassLayout(p, n, (size_t)n * p.y_stride, (size_t)n * cap, (size_t)n * p.f0_stride, (size_t)n * draw_stride,
+                   false) {}
+  PassLayout(const SynthesisPlan &p, int n, size_t samples, size_t pulses, size_t frames, size_t n_draws, bool packed) {
+    const size_t N = n, G = p.sizes.size();
     ArenaPlan a;
     len = a.add(2 * N * 4);                                          // f0 lengths, then y lengths
-    phase = a.add(N * p.y_stride * 8); vuv = a.add(N * p.y_stride * 8);
-    pidx = a.add(N * cap * 4); psh = a.add(N * cap * 8);
+    phase = a.add(samples * 8); vuv = a.add(samples * 8);
+    pidx = a.add(pulses * 4); psh = a.add(pulses * 8);
     np = a.add(N * 4); cnt = a.add(N * 4);
-    dcnt = a.add(N * cap * 4); doff = a.add(N * cap * 4);
+    dcnt = a.add(pulses * 4); doff = a.add(pulses * 4);
     dtot = a.add(N * 4); pl = a.add(N * 4);
-    draws = a.add(N * draw_stride * 4);
-    resp = a.add(N * cap * p.fft_size * 8);
+    draws = a.add(n_draws * 4);
+    resp = a.add(pulses * p.fft_size * 8);
     for (size_t g = 0; g < G; ++g) dcr.push_back(a.add((size_t)p.sizes[g] * 8));
     if (p.coded) {
       dsp = a.add(frames * p.row * 8); dap = a.add(frames * p.row * 8);
@@ -687,6 +797,7 @@ struct PassLayout {
     }
     if (!p.fp.empty()) fp = a.add(N * 8);
     if (G > 1) { fft_u = a.add(N * 4); list = a.add(N * 4); }
+    if (packed) { offs = a.add(4 * (N + 1) * 8); cums = a.add(2 * (N + G) * 8); }
     total = a.total;
   }
 };
@@ -710,31 +821,75 @@ int synthesis_run(Ctx *ctx, const SynthesisPlan &plan, int u0, int m, const Synt
   const int *f_len = plan.f_len.data() + u0, *y_len = plan.y_len.data() + u0;
   const int f0_stride = plan.f0_stride, y_stride = plan.y_stride, n_sizes = (int)plan.sizes.size();
   const size_t row = plan.row;
-  const bool mixed = n_sizes > 1;
+  const bool mixed = n_sizes > 1, packed = plan.packed();
+  // packed: the offsets of this run's utterances, and where utterance v's rows and samples start from the run's first
+  const long long *fo = packed ? plan.f_off.data() + u0 : nullptr, *yo = packed ? plan.y_off.data() + u0 : nullptr;
+  auto frame_at = [&](int v) { return packed ? (size_t)(fo[v] - fo[0]) : (size_t)v * f0_stride; };
+  auto sample_at = [&](int v) { return packed ? (size_t)(yo[v] - yo[0]) : (size_t)v * y_stride; };
   int max_y = 0;
   for (int i = 0; i < m; ++i) max_y = imax(max_y, y_len[i]);
   // The caller's f0 may be anything up to fs/2 (a pitch-shifted contour), so syn_timebase_kernel also counts the
   // pulses it could not store; a chunk where that count exceeds the cap is laid out again with room for its largest
   // count, in as many passes as the scratch budget needs.  The common case pays one read-back of n counts per chunk.
   // Every response slot holds the call's largest fft_size, so a pass's layout does not depend on which sizes it has.
+  // A packed pass is a run of consecutive utterances whose own scratch fits the budget, each with room for its own
+  // pulses; an utterance with more pulses than that gets room for exactly its count, and the pass is cut short until it
+  // fits again.
   const SynthesisSizing sz(ctx, plan, max_y);
   const ModifyPlan *mod = plan.coded && plan.modify ? &plan.mod : nullptr;
   const bool scale_f0 = mod && !mod->scale.empty(), stretch = mod && !mod->table.empty();
   const int nominal_cap = sz.nominal_cap;
   const size_t draw_stride = sz.draw_stride;
   auto fit = [&](int cap) { return sz.fit(cap); };
-  const int chunk = balanced_chunk(imin(m, 65535), fit(nominal_cap));
+  const int chunk = packed ? 0 : balanced_chunk(imin(m, 65535), fit(nominal_cap));
+  // packed: caps[i] is the pulse room of the pass's utterance i; the longest prefix of [v0, v0 + k) that fits
+  std::vector<int> caps;
+  auto packed_fit = [&](int v0, int k) {
+    double bytes = (double)sz.packed_pass();
+    int n = 0;
+    while (n < k && n < 65535) {
+      const int v = v0 + n;
+      bytes += (double)sz.packed_utt(y_len[v], f_len[v], caps[n]);
+      if (n > 0 && bytes > sz.budget) break;
+      ++n;
+    }
+    return n;
+  };
+  auto packed_pass = [&](int v0) {
+    caps.resize(m - v0);
+    for (int i = 0; i < m - v0; ++i) caps[i] = sz.cap_of(y_len[v0 + i]);
+    return packed_fit(v0, m - v0);
+  };
 #ifndef WB_EMU
-  cudaFuncSetAttribute(syn_pulse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pulse_smem(plan.fft_size));
+  const int smem = (int)pulse_smem(plan.fft_size);
+  cudaFuncSetAttribute(syn_pulse_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  cudaFuncSetAttribute(syn_pulse_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
 #endif
   std::vector<int> counts;
-  int v0 = 0, n = imin(chunk, m), pulse_cap = nominal_cap;   // this pass: utterances [u0 + v0, u0 + v0 + n)
+  int v0 = 0, n = packed ? packed_pass(0) : imin(chunk, m), pulse_cap = nominal_cap;   // this pass: [u0 + v0, +n)
   bool relaid = false;
   while (v0 < m) {
-    const PassLayout l(plan, n, pulse_cap, draw_stride);
+    // packed: the pass's offsets from its first utterance -- frames, samples, pulse slots, draws
+    std::vector<long long> offs(packed ? 4 * ((size_t)n + 1) : 0);
+    long long *foff = offs.data(), *soff = foff + n + 1, *poff = soff + n + 1, *doff = poff + n + 1;
+    size_t samples = 0, pulses = 0, frames = 0, n_draws = 0, max_draws = draw_stride;
+    if (packed) {
+      max_draws = 0;
+      for (int i = 0; i <= n; ++i) {
+        foff[i] = (long long)(frame_at(v0 + i) - frame_at(v0));
+        soff[i] = (long long)(sample_at(v0 + i) - sample_at(v0));
+        poff[i] = i ? poff[i - 1] + caps[i - 1] : 0;
+        doff[i] = soff[i] + 8LL * i;
+        if (i < n) max_draws = std::max(max_draws, (size_t)y_len[v0 + i] + 8);
+      }
+      samples = soff[n]; pulses = poff[n]; frames = foff[n]; n_draws = doff[n];
+    }
+    const PassLayout l = packed ? PassLayout(plan, n, samples, pulses, frames, n_draws, true)
+                                : PassLayout(plan, n, pulse_cap, draw_stride);
     unsigned char *blk = arena_block(ctx, l.total);
     if (!blk) return WORLD_B200_ENOMEM;
     std::vector<int> l2((size_t)2 * n), pl(n, pulse_cap);
+    if (packed) std::copy(caps.begin(), caps.begin() + n, pl.begin());
     int max_f = 0;
     for (int i = 0; i < n; ++i) { l2[i] = f_len[v0 + i]; l2[n + i] = y_len[v0 + i]; max_f = imax(max_f, l2[i]); }
     // the pass's utterances grouped by size: group g is list[first[g] .. first[g + 1])
@@ -752,6 +907,7 @@ int synthesis_run(Ctx *ctx, const SynthesisPlan &plan, int u0, int m, const Synt
     if (!rc && !plan.fp.empty()) rc = dev_memcpy_h2d(ctx, blk + l.fp, plan.fp.data() + u0 + v0, (size_t)n * 8);
     if (!rc && mixed) rc = dev_memcpy_h2d(ctx, blk + l.fft_u, fft_u.data(), (size_t)n * 4);
     if (!rc && mixed) rc = dev_memcpy_h2d(ctx, blk + l.list, list.data(), (size_t)n * 4);
+    if (!rc && packed) rc = dev_memcpy_h2d(ctx, blk + l.offs, offs.data(), offs.size() * 8);
     for (int g = 0; g < n_sizes && plan.coded; ++g) {
       const CodecTables &s = plan.tsp[g], &a = plan.tap[g];
       if (!rc) rc = dev_memcpy_h2d(ctx, blk + l.sidx[g], s.idx.data(), s.idx.size() * 4);
@@ -763,12 +919,13 @@ int synthesis_run(Ctx *ctx, const SynthesisPlan &plan, int u0, int m, const Synt
     ModifyDevice md = {};
     if (mod && !rc) rc = modify_upload(ctx, *mod, u0 + v0, n, blk + l.mod, &md);
     if (rc) return rc;
-    SynParams p;
-    p.f0 = rows.f0 + (size_t)v0 * f0_stride; p.f_len = (const int *)(blk + l.len); p.f_stride = f0_stride;
+    const long long *d_off = packed ? (const long long *)(blk + l.offs) : nullptr;
+    SynParams p{};
+    p.f0 = rows.f0 + frame_at(v0); p.f_len = (const int *)(blk + l.len); p.f_stride = f0_stride;
     if (plan.coded) {
       p.sp = (const double *)(blk + l.dsp); p.ap = (const double *)(blk + l.dap);
     } else {
-      p.sp = rows.sp + (size_t)v0 * f0_stride * row; p.ap = rows.ap + (size_t)v0 * f0_stride * row;
+      p.sp = rows.sp + frame_at(v0) * row; p.ap = rows.ap + frame_at(v0) * row;
     }
     p.fft_size = plan.fft_size; p.lg_fft = log2_of(plan.fft_size); p.row = (int)row;
     p.fft_u = mixed ? (const int *)(blk + l.fft_u) : nullptr; p.list = nullptr;
@@ -782,29 +939,44 @@ int synthesis_run(Ctx *ctx, const SynthesisPlan &plan, int u0, int m, const Synt
     p.draw_tot = (unsigned *)(blk + l.dtot);
     p.draws = (const unsigned *)(blk + l.draws); p.draw_stride = draw_stride;
     p.resp = (double *)(blk + l.resp); p.resp_n = plan.fft_size; p.dc_remover = (const double *)(blk + l.dcr[0]);
-    p.y = plan.nbit ? nullptr : (double *)rows.y + (size_t)v0 * y_stride;
-    p.y16 = plan.nbit ? (short *)rows.y + (size_t)v0 * y_stride : nullptr;
+    p.y = plan.nbit ? nullptr : (double *)rows.y + sample_at(v0);
+    p.y16 = plan.nbit ? (short *)rows.y + sample_at(v0) : nullptr;
     p.tw = ctx->twiddle;
+    if (packed) {
+      p.f_off = d_off; p.s_off = d_off + (n + 1); p.p_off = d_off + 2 * (n + 1);
+      p.n_utts = n;
+    }
     // a pass laid out from the counts reports a pulse beyond its arrays as a scratch overflow (status bit 4)
     p.status = relaid ? ctx->status_dev : nullptr;
     if (scale_f0) {
       // the time base, the pulse count (and the relaid pass it may call for) and the pulses all see the scaled contour
       double *f0m = (double *)(blk + l.f0m);
-      modify_f0_launch(ctx, md, p.f_len, n, f0_stride, max_f, p.f0, f0m);
+      modify_f0_launch(ctx, md, p.f_len, n, f0_stride, max_f, p.f0, f0m, p.f_off);
       p.f0 = f0m;
     }
-    WB_LAUNCH_COOP(syn_timebase_kernel, dim3((unsigned)n), 256, 0, ctx->stream, p);
+    if (packed)
+      WB_LAUNCH_COOP(syn_timebase_kernel<true>, dim3((unsigned)n), 256, 0, ctx->stream, p);
+    else
+      WB_LAUNCH_COOP(syn_timebase_kernel<false>, dim3((unsigned)n), 256, 0, ctx->stream, p);
     if (!relaid) {
       counts.resize(n);
       rc = dev_memcpy_d2h(ctx, counts.data(), p.pulse_count, (size_t)n * 4);
       if (!rc) rc = dev_sync(ctx);
       if (rc) return rc;
       int most = 0;
-      for (int i = 0; i < n; ++i) most = imax(most, counts[i]);
-      if (most > pulse_cap) {
+      bool over = false;
+      for (int i = 0; i < n; ++i) {
+        most = imax(most, counts[i]);
+        if (packed && counts[i] > caps[i]) { caps[i] = counts[i]; over = true; }
+      }
+      if (packed ? over : most > pulse_cap) {
         // the time base is deterministic: run again over the first n' of these utterances, it finds the same pulses
-        pulse_cap = most;
-        n = imin(n, imax(1, fit(pulse_cap)));
+        if (packed) {
+          n = imax(1, packed_fit(v0, n));
+        } else {
+          pulse_cap = most;
+          n = imin(n, imax(1, fit(pulse_cap)));
+        }
         relaid = true;
         continue;
       }
@@ -812,44 +984,81 @@ int synthesis_run(Ctx *ctx, const SynthesisPlan &plan, int u0, int m, const Synt
     // size group g of this pass: its utterance count, and its list on the device (null: the whole pass)
     auto group_n = [&](int g) { return first[g + 1] - first[g]; };
     auto group_list = [&](int g) { return mixed ? (const int *)(blk + l.list) + first[g] : nullptr; };
+    // packed: per size group, the prefix sums of its utterances' pulses and frames ([group_n + 1] at first[g] + g):
+    // the pulse and decode kernels run one CTA per pulse or frame, not over the padded grid
+    std::vector<long long> cums(packed ? 2 * ((size_t)n + n_sizes) : 0);
+    long long *pcum = cums.data(), *fcum = pcum + (n + n_sizes);
+    for (int g = 0; g < n_sizes && packed; ++g) {
+      long long *pc = pcum + first[g] + g, *fc = fcum + first[g] + g;
+      pc[0] = fc[0] = 0;
+      for (int j = 0; j < group_n(g); ++j) {
+        const int i = list.empty() ? j : list[first[g] + j];
+        pc[j + 1] = pc[j] + imin(counts[i], caps[i]);
+        fc[j + 1] = fc[j] + f_len[v0 + i];
+      }
+    }
+    if (packed) rc = dev_memcpy_h2d(ctx, blk + l.cums, cums.data(), cums.size() * 8);
+    if (rc) return rc;
+    const long long *pcum_d = packed ? (const long long *)(blk + l.cums) : nullptr;
+    const long long *fcum_d = packed ? pcum_d + (n + n_sizes) : nullptr;
     if (plan.coded) {
       // DecodeSpectralEnvelope / DecodeAperiodicity of this pass's utterances, frames [0, f0_length), each at its size
       // into rows of the call's largest bins
       double *dsp = (double *)(blk + l.dsp), *dap = (double *)(blk + l.dap);
+      const double *csp = rows.sp + frame_at(v0) * plan.dims;
+      const double *cap = plan.n_ap > 0 ? rows.ap + frame_at(v0) * plan.n_ap : dap;
       for (int g = 0; g < n_sizes; ++g) {
         const CodecDeviceTables ts = {(const int *)(blk + l.sidx[g]), (const double *)(blk + l.sfrac[g]),
                                       (const double2 *)(blk + l.sw[g])};
-        codec_decode_launch(ctx, true, plan.tsp[g], ts, plan.sizes[g], p.f_len, group_n(g), f0_stride, max_f,
-                            rows.sp + (size_t)v0 * f0_stride * plan.dims, dsp, group_list(g), (int)row);
+        if (packed)
+          codec_decode_packed_launch(ctx, true, plan.tsp[g], ts, plan.sizes[g], p.f_len, p.f_off, group_list(g),
+                                     group_n(g), fcum_d + first[g] + g, fcum[first[g] + g + group_n(g)], csp, dsp,
+                                     (int)row);
+        else
+          codec_decode_launch(ctx, true, plan.tsp[g], ts, plan.sizes[g], p.f_len, group_n(g), f0_stride, max_f, csp,
+                              dsp, group_list(g), (int)row);
       }
-      if (stretch) modify_stretch_launch(ctx, md, (int)row, mod->bins, p.f_len, n, f0_stride, max_f, dsp);
+      if (stretch) modify_stretch_launch(ctx, md, (int)row, mod->bins, p.f_len, n, f0_stride, max_f, dsp, p.f_off);
       // below 12 kHz there are no bands: the kernel reads no coded value (its input pointer only has to be valid)
       for (int g = 0; g < n_sizes; ++g) {
         const CodecDeviceTables ta = {(const int *)(blk + l.aidx[g]), (const double *)(blk + l.afrac[g]), nullptr};
-        codec_decode_launch(ctx, false, plan.tap[g], ta, plan.sizes[g], p.f_len, group_n(g), f0_stride, max_f,
-                            plan.n_ap > 0 ? rows.ap + (size_t)v0 * f0_stride * plan.n_ap : dap, dap, group_list(g),
-                            (int)row);
+        if (packed)
+          codec_decode_packed_launch(ctx, false, plan.tap[g], ta, plan.sizes[g], p.f_len, p.f_off, group_list(g),
+                                     group_n(g), fcum_d + first[g] + g, fcum[first[g] + g + group_n(g)], cap, dap,
+                                     (int)row);
+        else
+          codec_decode_launch(ctx, false, plan.tap[g], ta, plan.sizes[g], p.f_len, group_n(g), f0_stride, max_f, cap,
+                              dap, group_list(g), (int)row);
       }
     }
-    scan_counts(ctx, p.draw_cnt, (const int *)(blk + l.pl), pulse_cap, nullptr, p.draw_off, p.draw_tot, n);
-    rng_fill(ctx, p.draw_tot, (unsigned *)(blk + l.draws), draw_stride, draw_stride, n);
+    scan_counts(ctx, p.draw_cnt, (const int *)(blk + l.pl), pulse_cap, nullptr, p.draw_off, p.draw_tot, n, p.p_off);
+    rng_fill(ctx, p.draw_tot, (unsigned *)(blk + l.draws), draw_stride, max_draws, n, 0,
+             packed ? d_off + 3 * (n + 1) : nullptr);
     // one launch per size, each with its own shared memory (and so its own occupancy)
     for (int g = 0; g < n_sizes; ++g) {
       if (group_n(g) == 0) continue;
       SynParams q = p;
       q.fft_size = plan.sizes[g]; q.lg_fft = log2_of(q.fft_size);
       q.dc_remover = (const double *)(blk + l.dcr[g]); q.list = group_list(g);
-      WB_LAUNCH_COOP(syn_pulse_kernel, dim3((unsigned)pulse_cap, (unsigned)group_n(g)), 128, pulse_smem(q.fft_size),
-                     ctx->stream, q);
+      if (packed) {
+        const long long total = pcum[first[g] + g + group_n(g)];
+        if (total == 0) continue;
+        q.cum = pcum_d + first[g] + g; q.list_n = group_n(g);
+        WB_LAUNCH_COOP(syn_pulse_kernel<true>, dim3((unsigned)total), 128, pulse_smem(q.fft_size), ctx->stream, q);
+      } else {
+        WB_LAUNCH_COOP(syn_pulse_kernel<false>, dim3((unsigned)pulse_cap, (unsigned)group_n(g)), 128,
+                       pulse_smem(q.fft_size), ctx->stream, q);
+      }
     }
+    const dim3 grid = packed ? dim3((unsigned)((samples + 255) / 256)) : dim3((unsigned)((max_y + 255) / 256), (unsigned)n);
     if (plan.nbit)
-      WB_LAUNCH_FLAT(syn_overlap_kernel<short>, dim3((unsigned)((max_y + 255) / 256), (unsigned)n), 256, 0, ctx->stream, p);
+      WB_LAUNCH_FLAT(syn_overlap_kernel<short>, grid, 256, 0, ctx->stream, p);
     else
-      WB_LAUNCH_FLAT(syn_overlap_kernel<double>, dim3((unsigned)((max_y + 255) / 256), (unsigned)n), 256, 0, ctx->stream, p);
+      WB_LAUNCH_FLAT(syn_overlap_kernel<double>, grid, 256, 0, ctx->stream, p);
     rc = dev_check(ctx, "synthesis");
     if (rc) return rc;
     v0 += n;
-    n = imin(chunk, m - v0);
+    n = packed ? (v0 < m ? packed_pass(v0) : 0) : imin(chunk, m - v0);
     pulse_cap = nominal_cap;
     relaid = false;
   }
@@ -920,9 +1129,12 @@ extern "C" int world_b200_synthesis_coded_batch_pcm16(WorldB200 *h, const double
 
 // world_b200_modify_batch (fft_sizes NULL: fft_size for every utterance, rows of fft_size / 2 + 1) and
 // world_b200_modify_batch_options (utterance u at fft_sizes[u], rows of row_stride)
+// world_b200_modify_packed: f_offsets (host, [n_utts + 1]) instead of f0_lengths / f0_stride, row_stride 0 = the largest
+// fft_sizes[u] / 2 + 1
 static int modify_batch(WorldB200 *h, double *f0, const int *f0_lengths, int n_utts, int f0_stride,
                         double *spectrogram, int row_stride, int fft_size, const int *fft_sizes, bool per_utt, int fs,
-                        const double *f0_scale, const double *spectral_ratio) {
+                        const double *f0_scale, const double *spectral_ratio, const long long *f_offsets = nullptr,
+                        bool packed = false) {
   if (!h) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
   Ctx *ctx = &h->c;
@@ -930,12 +1142,20 @@ static int modify_batch(WorldB200 *h, double *f0, const int *f0_lengths, int n_u
     ctx->last_error = "modify: " + what;
     return WORLD_B200_EINVAL;
   };
-  if (n_utts < 0 || f0_stride <= 0) return fail("n_utts must be >= 0 and f0_stride > 0");
+  if (packed) {
+    if (n_utts < 0) return fail("n_utts must be >= 0");
+    if (n_utts == 0) return 0;
+    if (!f_offsets) return fail("f_offsets must be given");
+  } else if (n_utts < 0 || f0_stride <= 0) {
+    return fail("n_utts must be >= 0 and f0_stride > 0");
+  }
   if ((f0_scale && !f0) || (spectral_ratio && !spectrogram))
     return fail("f0_scale needs f0 rows and spectral_ratio needs spectrogram rows");
   if (per_utt && spectral_ratio) {
     if (!fft_sizes) return fail("fft_sizes must be given");
     if (fs <= 0) return fail("fs must be > 0");
+    if (packed && row_stride == 0)
+      for (int u = 0; u < n_utts; ++u) row_stride = imax(row_stride, fft_sizes[u] / 2 + 1);
     for (int u = 0; u < n_utts; ++u) {
       const int f = fft_sizes[u], why = f < 16 || f > 4096 || (f & (f - 1)) ? 1 : row_stride < f / 2 + 1 ? 2 : 0;
       if (why == 1)
@@ -949,11 +1169,12 @@ static int modify_batch(WorldB200 *h, double *f0, const int *f0_lengths, int n_u
   // a length of 0 is allowed here: the utterance's rows are left alone
   std::vector<int> lens;
   ModifyPlan plan;
-  int rc = row_lengths(ctx, "modify", "f0", f0_lengths, n_utts, f0_stride, 0, &lens);
+  int rc = packed ? packed_lengths(ctx, "modify", "f", "frames", f_offsets, n_utts, 0, &lens)
+                  : row_lengths(ctx, "modify", "f0", f0_lengths, n_utts, f0_stride, 0, &lens);
   if (!rc) rc = modify_plan(ctx, "modify", n_utts, fft_size, fs, f0_scale, spectral_ratio, &plan,
                             per_utt ? fft_sizes : nullptr);
   return rc ? rc : modify_run(ctx, plan, 0, n_utts, lens.data(), f0_stride, per_utt ? row_stride : plan.bins, f0,
-                              spectrogram);
+                              spectrogram, packed ? f_offsets : nullptr);
 }
 
 extern "C" int world_b200_modify_batch(WorldB200 *h, double *f0, const int *f0_lengths, int n_utts, int f0_stride,
@@ -994,4 +1215,45 @@ extern "C" int world_b200_synthesis_coded_batch_options(WorldB200 *h, const doub
   r.coded = true; r.dims = number_of_dimensions; r.f0_scale = f0_scale; r.spectral_ratio = spectral_ratio;
   r.per_utt = true; r.fft_sizes = fft_sizes;
   return synthesis_batch(h, r);
+}
+
+// ---- packed rows: utterance u is frames [f_offsets[u], f_offsets[u + 1]) and samples [y_offsets[u], y_offsets[u + 1])
+static int packed_missing(WorldB200 *h) {
+  h->c.last_error = "Synthesis: f_offsets and y_offsets must be given";
+  return WORLD_B200_EINVAL;
+}
+
+extern "C" int world_b200_synthesis_packed(WorldB200 *h, const double *f0, int n_utts, const long long *f_offsets,
+                                           const double *spectrogram, const double *aperiodicity, int row_stride,
+                                           const int *fft_sizes, double frame_period, int fs,
+                                           const long long *y_offsets, double *y) {
+  if (h && n_utts == 0) return 0;
+  if (h && (!f_offsets || !y_offsets)) return packed_missing(h);
+  SynthesisRequest r{f0, nullptr, n_utts, 0, spectrogram, aperiodicity, 0, frame_period, fs, nullptr, 0, y, 0};
+  r.per_utt = true; r.fft_sizes = fft_sizes; r.row_stride = row_stride;
+  r.f_offsets = f_offsets; r.y_offsets = y_offsets;
+  return synthesis_batch(h, r);
+}
+
+extern "C" int world_b200_synthesis_coded_packed(WorldB200 *h, const double *f0, int n_utts,
+                                                 const long long *f_offsets, const double *coded_spectral_envelope,
+                                                 int number_of_dimensions, const double *coded_aperiodicity,
+                                                 const int *fft_sizes, double frame_period, int fs,
+                                                 const long long *y_offsets, const double *f0_scale,
+                                                 const double *spectral_ratio, int nbit, void *y) {
+  if (h && n_utts == 0) return 0;
+  if (h && (!f_offsets || !y_offsets)) return packed_missing(h);
+  SynthesisRequest r{f0, nullptr, n_utts, 0, coded_spectral_envelope, coded_aperiodicity, 0, frame_period, fs, nullptr,
+                     0, y, nbit};
+  r.coded = true; r.dims = number_of_dimensions; r.f0_scale = f0_scale; r.spectral_ratio = spectral_ratio;
+  r.per_utt = true; r.fft_sizes = fft_sizes;
+  r.f_offsets = f_offsets; r.y_offsets = y_offsets;
+  return synthesis_batch(h, r);
+}
+
+extern "C" int world_b200_modify_packed(WorldB200 *h, double *f0, int n_utts, const long long *f_offsets,
+                                        double *spectrogram, int row_stride, const int *fft_sizes, int fs,
+                                        const double *f0_scale, const double *spectral_ratio) {
+  return modify_batch(h, f0, nullptr, n_utts, 0, spectrogram, row_stride, 0, fft_sizes, true, fs, f0_scale,
+                      spectral_ratio, f_offsets, true);
 }
