@@ -769,6 +769,44 @@ int world_b200_transform_host_spectral_options(WorldB200 *ctx, const void *x, in
                                                const D4COption *d4c_options, const double *f0_scale,
                                                const double *spectral_ratio, const double *time_scale, int nbit_out,
                                                void *y, int y_stride, int *y_lengths);
+/* The voice transformation on a packed batch: utterances back to back in, transformed samples back to back out.
+ * x_offsets is a HOST array of n_utts + 1 sample offsets with the rules of the packed analysis calls (above): x
+ * holds nbit 0/8/16/24/32 samples, with byte offset = sample offset * nbit / 8.  Utterance u's output is samples
+ * [y_offsets[u], y_offsets[u + 1]) of y, [Y] float64 (nbit_out 0) or int16 (nbit_out 16, the pcm16 rule), where
+ * Y = y_offsets[n_utts] and
+ *   y_offsets[0] = 0, y_offsets[u + 1] - y_offsets[u] =
+ *     world_b200_transform_samples(fs, x_offsets[u + 1] - x_offsets[u], frame_period, time_scale ? time_scale[u] : 1)
+ * with the F0 method's frame_period.  Every offset is 64-bit: Y may exceed 2^31.
+ * world_b200_transform_packed_samples gives y_offsets (HOST, n_utts + 1) beforehand; EINVAL for bad offsets, a
+ * time_scale that is not finite and > 0, or an utterance whose output length does not fit an int. */
+int world_b200_transform_packed_samples(int fs, int n_utts, const long long *x_offsets, double frame_period,
+                                        const double *time_scale, long long *y_offsets);
+/* On DEVICE x and y.  The option arrays and factors are those of world_b200_transform_batch_spectral_options.
+ *   - Output: utterance u's samples equal, bit for bit, row u of world_b200_transform_batch_spectral_options (or
+ *     world_b200_transform_batch when both spectral option arrays are NULL) on the same utterances padded, with the
+ *     same options and factors.  Samples [0, Y) of y are written and nothing else.  y_offsets (HOST, n_utts + 1, may be
+ *     NULL) receives the sample offsets before any work is queued.
+ *   - The batch runs in slices cut by their own lengths: a slice's rows are as long as its own longest utterance, so
+ *     one long utterance does not shrink every slice.  Synthesis runs in packed passes.
+ *   - Validation, before any work is queued (WORLD_B200_EINVAL, world_b200_last_error() naming the first bad
+ *     utterance; y is unchanged): the padded call's rules (time_scale, at least 2 frames per utterance, Synthesis's FFT
+ *     sizes, nbit_out, y given), the offset rules of the packed analysis calls, and an output length that does not fit
+ *     an int.  n_utts 0 writes y_offsets[0] = 0 and returns 0. */
+int world_b200_transform_packed(WorldB200 *ctx, const void *x, int nbit, int n_utts, const long long *x_offsets,
+                                int fs, const WorldB200AnalysisOption *option, const HarvestOption *harvest_options,
+                                const DioOption *dio_options, const CheapTrickOption *cheaptrick_options,
+                                const D4COption *d4c_options, const double *f0_scale, const double *spectral_ratio,
+                                const double *time_scale, int nbit_out, void *y, long long *y_offsets);
+/* The same for HOST x and y: chunks of consecutive utterances go up as one copy of their samples and come back as one
+ * copy of their output samples; no padding crosses PCIe.  Writes exactly Y samples, equal to
+ * world_b200_transform_packed's; pinned host buffers let the copies run under the kernels.  Returns when the results
+ * are in y. */
+int world_b200_transform_host_packed(WorldB200 *ctx, const void *x, int nbit, int n_utts, const long long *x_offsets,
+                                     int fs, const WorldB200AnalysisOption *option,
+                                     const HarvestOption *harvest_options, const DioOption *dio_options,
+                                     const CheapTrickOption *cheaptrick_options, const D4COption *d4c_options,
+                                     const double *f0_scale, const double *spectral_ratio, const double *time_scale,
+                                     int nbit_out, void *y, long long *y_offsets);
 
 #ifdef __cplusplus
 }

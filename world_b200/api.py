@@ -258,6 +258,15 @@ ABI = {
                                                              C.POINTER(DioOption), C.POINTER(CheapTrickOption),
                                                              C.POINTER(D4COption), _P, _P, _P, C.c_int, _P, C.c_int,
                                                              _IP]),
+    "world_b200_transform_packed_samples": (C.c_int, [C.c_int, C.c_int, _LP, C.c_double, _P, _LP]),
+    "world_b200_transform_packed": (C.c_int, [_P, _P, C.c_int, C.c_int, _LP, C.c_int, C.POINTER(AnalysisOption),
+                                              C.POINTER(HarvestOption), C.POINTER(DioOption),
+                                              C.POINTER(CheapTrickOption), C.POINTER(D4COption), _P, _P, _P, C.c_int,
+                                              _P, _LP]),
+    "world_b200_transform_host_packed": (C.c_int, [_P, _P, C.c_int, C.c_int, _LP, C.c_int, C.POINTER(AnalysisOption),
+                                                   C.POINTER(HarvestOption), C.POINTER(DioOption),
+                                                   C.POINTER(CheapTrickOption), C.POINTER(D4COption), _P, _P, _P,
+                                                   C.c_int, _P, _LP]),
     # host-only file glue (tools/audioio.h, tools/parameterio.h)
     "wavwrite": (None, [_P, C.c_int, C.c_int, C.c_int, C.c_char_p]),
     "GetAudioLength": (C.c_int, [C.c_char_p]),
@@ -1329,6 +1338,81 @@ class World:
         self._check(getattr(self.lib, f"world_b200_transform_host{suffix}")(self._h, _ptr(xh), *args, _ptr(y),
                                                                              y_stride, yl))
         return out, list(yl)[:n]
+
+    # -- the voice transformation on packed batches: utterance u = samples [x_offsets[u], x_offsets[u + 1]) in and
+    #    samples [y_offsets[u], y_offsets[u + 1]) out ------------------------------------------------------------------
+    def transform_packed_samples(self, fs, x_offsets, frame_period=5.0, time_scale=None):
+        """The output offsets of a packed transform (numpy int64, n + 1; world_b200_transform_packed_samples): utterance
+        u's output is samples [y[u], y[u + 1]), of transform_samples(fs, its length, frame_period, time_scale[u])."""
+        import numpy as np
+        n, xo = _offsets(x_offsets)
+        y = (C.c_longlong * (n + 1))()
+        rc = self.lib.world_b200_transform_packed_samples(fs, n, xo, frame_period, _factors(time_scale, n, "time_scale"),
+                                                          y)
+        if rc:
+            raise WorldError(f"world_b200_transform_packed_samples: bad x_offsets, time_scale or arguments (code {rc})")
+        return np.array(y[:], dtype=np.int64)
+
+    def _transform_packed(self, name, x, nbit, x_offsets, fs, option, f0_scale, spectral_ratio, time_scale,
+                          harvest_options, dio_options, cheaptrick_options, d4c_options, dtype, y, host):
+        """Calls world_b200_<name> on a packed batch: (y [Y], y_offsets as numpy int64), y allocated when None (device:
+        on x's device; host: numpy)."""
+        import numpy as np
+        n, xo = _offsets(x_offsets)
+        per_utt, per_dio = _chain_options(harvest_options, dio_options, n)
+        ct = None if cheaptrick_options is None else _option_array(CheapTrickOption, cheaptrick_options, n)
+        d4 = None if d4c_options is None else _option_array(D4COption, d4c_options, n)
+        pcm16 = _pcm16(dtype)
+        try:
+            Y = int(self.transform_packed_samples(fs, x_offsets, _frame_period(option), time_scale)[-1])
+        except WorldError:   # the call below names what is wrong
+            Y = 0
+        if host:
+            want = np.int16 if pcm16 else np.float64
+            if y is None:
+                y = np.empty((Y,), dtype=want)
+            yh = y.numpy() if hasattr(y, "numpy") else y
+            if yh.shape != (Y,) or yh.dtype != want or not yh.flags.c_contiguous:
+                raise ValueError(f"out: a contiguous [{Y}] {np.dtype(want).name} host array")
+            xh = x.numpy() if hasattr(x, "numpy") else x
+            if not xh.flags.c_contiguous:
+                raise ValueError("x: a contiguous host array")
+            xp, yp = _ptr(xh), _ptr(yh)
+        else:
+            if y is None:
+                y = self._packed_y(x, Y, pcm16)
+            xp, yp = _ptr(x), _ptr(y)
+            self._use_current_stream()
+        got = (C.c_longlong * (n + 1))()
+        self._check(getattr(self.lib, f"world_b200_{name}")(
+            self._h, xp, nbit, n, xo, fs, C.byref(option), per_utt, per_dio, ct, d4, _factors(f0_scale, n, "f0_scale"),
+            _factors(spectral_ratio, n, "spectral_ratio"), _factors(time_scale, n, "time_scale"), 16 if pcm16 else 0,
+            yp, got))
+        return y, np.array(got[:], dtype=np.int64)
+
+    def transform_packed(self, x, nbit, x_offsets, fs, option: AnalysisOption, f0_scale=None, spectral_ratio=None,
+                         time_scale=None, harvest_options=None, dio_options=None, cheaptrick_options=None,
+                         d4c_options=None, dtype=None, y=None):
+        """transform() on a PACKED batch of DEVICE samples (world_b200_transform_packed): x holds float64 samples (nbit
+        0) or nbit-bit PCM back to back, utterance u being samples [x_offsets[u], x_offsets[u + 1]) (x_offsets: n + 1
+        offsets, a list, numpy array or CPU tensor).  Returns (y [Y], y_offsets [n + 1]) on x's device: float64, or
+        int16 for dtype int16; utterance u's output is samples [y_offsets[u], y_offsets[u + 1]).  Each utterance's
+        samples equal transform()'s row of the same utterance padded, bit for bit.  Factors and option lists as in
+        transform(); y: a [Y] device array to write into."""
+        return self._transform_packed("transform_packed", x, nbit, x_offsets, fs, option, f0_scale, spectral_ratio,
+                                      time_scale, harvest_options, dio_options, cheaptrick_options, d4c_options, dtype,
+                                      y, host=False)
+
+    def transform_host_packed(self, x, nbit, x_offsets, fs, option: AnalysisOption, f0_scale=None,
+                              spectral_ratio=None, time_scale=None, harvest_options=None, dio_options=None,
+                              cheaptrick_options=None, d4c_options=None, dtype=None, out=None):
+        """transform_packed for HOST arrays (numpy or CPU tensors; world_b200_transform_host_packed): chunks of
+        utterances go up and come back as one copy each.  Returns (y [Y], y_offsets) with y a host array.  out: a
+        contiguous [Y] host array of the output dtype to write into (a pinned one lets the copies overlap the
+        kernels)."""
+        return self._transform_packed("transform_host_packed", x, nbit, x_offsets, fs, option, f0_scale,
+                                      spectral_ratio, time_scale, harvest_options, dio_options, cheaptrick_options,
+                                      d4c_options, dtype, out, host=True)
 
     def analyze_coded_batch_allgather(self, x, nbit, fs, option: AnalysisOption, number_of_dimensions, time_axis_full,
                                       f0_full, coded_sp_full, coded_ap_full, x_lengths=None, harvest_options=None,

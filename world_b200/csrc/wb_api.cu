@@ -668,10 +668,10 @@ static int chain_checks(Ctx *c, const ChainRequest &r, ChainPlan *p) {
   }
   p->f0_stride = r.f0_stride ? r.f0_stride : most;
 
-  // The stage plans: CheapTrick when a spectrogram is asked for, D4C when an aperiodicity is (a transform, f0_stride 0,
-  // needs both), StoneMask's sampling-rate limit for DIO.  Each utterance's CheapTrick option, and D4C's fft_size (its
-  // CheapTrick size) and option, with the per-call option standing in for a NULL per-utterance array.
-  const bool transform = !r.packed && r.f0_stride == 0;
+  // The stage plans: CheapTrick when a spectrogram is asked for, D4C when an aperiodicity is (a transform needs both),
+  // StoneMask's sampling-rate limit for DIO.  Each utterance's CheapTrick option, and D4C's fft_size (its CheapTrick
+  // size) and option, with the per-call option standing in for a NULL per-utterance array.
+  const bool transform = r.transform;
   StageRequest s{STAGE_CHEAPTRICK, n, x_stride, x_lengths, r.fs, p->f_len.data(), p->f0_stride};
   s.ct = &opt->cheaptrick; s.fft_size = &opt->cheaptrick.fft_size; s.d4c = &opt->d4c;
   s.coded = r.coded; s.dims = r.dims;
@@ -1033,13 +1033,13 @@ static int analyze_chain(WorldB200 *h, const ChainRequest &r, bool gather) {
 }  // extern "C"
 
 // A packed slice's time axis and f0, from the lane's padded rows (f_stride frames) to the packed rows: utterance u
-// (blockIdx.y) has f_off[u + 1] - f_off[u] frames, written from row f_off[u]
+// (blockIdx.y) has f_off[u + 1] - f_off[u] frames, written from row f_off[u].  t_out NULL: f0 only (a transform).
 WB_KERNEL_PLAIN scatter_f0_kernel(const long long *__restrict__ f_off, int f_stride, const double *__restrict__ t,
                                   const double *__restrict__ f, double *__restrict__ t_out, double *__restrict__ f_out) {
   const int u = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
   const long long at = f_off[u] + i;
   if (at >= f_off[u + 1]) return;
-  t_out[at] = t[(size_t)u * f_stride + i];
+  if (t_out) t_out[at] = t[(size_t)u * f_stride + i];
   f_out[at] = f[(size_t)u * f_stride + i];
 }
 
@@ -1186,43 +1186,155 @@ int transform_check(WorldB200 *h, const ChainRequest &r, const double *f0_scale,
     c->last_error = std::string(who) + ": " + what;
     return WORLD_B200_EINVAL;
   };
-  if (!y || y_stride <= 0) return fail("y must be given, with y_stride > 0");
+  if (!y || (!r.packed && y_stride <= 0)) return fail(r.packed ? "y must be given" : "y must be given, with y_stride > 0");
   if (nbit_out != 0 && nbit_out != 16) return fail("nbit_out must be 0 (float64) or 16 (int16)");
   const ChainPlan &p = tp->chain;
   const int rc = chain_plan(c, r, who, &tp->chain);
   if (rc) return rc;
   std::vector<int> y_len(r.n);
   std::vector<double> fp(r.n);
+  std::vector<long long> y_off(1, 0);
   for (int u = 0; u < r.n; ++u) {
     const double ts = time_scale ? time_scale[u] : 1.0;
+    char msg[256];
     if (!(ts > 0.0) || !isfinite(ts)) {
-      char msg[256];
       snprintf(msg, sizeof msg, "time_scale[%d] = %.17g is not a finite factor > 0", u, ts);
       return fail(msg);
     }
-    y_len[u] = world_b200_transform_samples(r.fs, r.x_lengths ? r.x_lengths[u] : r.x_stride, p.frame_period, ts);
+    const int x_len = r.packed ? p.x_len[u] : r.x_lengths ? r.x_lengths[u] : r.x_stride;
+    y_len[u] = world_b200_transform_samples(r.fs, x_len, p.frame_period, ts);
     fp[u] = (p.frame_period * ts) / 1000.0;   // synthesis_batch's frame_period / 1000.0, with the same product
+    if (r.packed && y_len[u] == 0) {
+      snprintf(msg, sizeof msg, "the output of utterance %d (%d samples at time_scale %.17g) does not fit an int", u,
+               x_len, ts);
+      return fail(msg);
+    }
+    y_off.push_back(y_off.back() + y_len[u]);
   }
   SynthesisRequest s{nullptr, p.f_len.data(), r.n, p.f0_stride, nullptr, nullptr, r.opt->cheaptrick.fft_size,
                      p.frame_period, r.fs, y_len.data(), y_stride, y, nbit_out};
   s.f0_scale = f0_scale; s.spectral_ratio = spectral_ratio; s.transform = true; s.fp = fp.data();
-  if (r.cheaptrick_options || r.d4c_options) {   // each utterance synthesised at its CheapTrick size
+  if (r.cheaptrick_options || r.d4c_options || r.packed) {   // each utterance synthesised at its CheapTrick size
     s.per_utt = true; s.fft_sizes = p.ct.fft_size.data(); s.row_stride = (int)p.sp_row;
   }
+  if (r.packed) { s.f_offsets = p.f_off.data(); s.y_offsets = y_off.data(); }
   return synthesis_plan(c, s, who, &tp->syn);
 }
 
-// Utterances [u0, u0 + n) of a checked call: x and y point at utterance u0's rows (DEVICE); the request's x_lengths and
-// per-utterance options are the call's whole arrays.  The utterances are cut into slices that alternate between the
-// two lanes of a LaneScope.  A slice's rows (float64 input, time axis, f0, spectrogram, aperiodicity) live from its
-// analysis to its synthesis in one buffer per lane, taken from the lane's pool and sized for its largest slice; slices
-// are sized so that the buffer takes at most about half the lane's scratch budget, leaving the rest to the stages.
-// Issue order A(0), A(1), S(0), A(2), S(1), ... (A = F0 stage, CheapTrick, D4C and modify; S = synthesis): a lane runs
-// its slices in stream order, so A(s + 1) never overwrites rows S(s - 1) still reads, and while synthesis_run waits
-// for its pulse counts (a host synchronisation of its lane), the other lane has an analysis queued.  One lane (one
-// slice, or the host emulation) runs A(s), S(s) in turn.  The caller's stream waits for both lanes on return.
+// The slice loop of both transform drivers.  Slice s is utterances [bounds[s], bounds[s + 1]) and bytes(s) the rows it
+// keeps in its lane's buffer from its analysis to its synthesis; analyse(lanes, s) and synthesise(lanes, s) enqueue its
+// two halves on lanes.lane(s).  Issue order A(0), A(1), S(0), A(2), S(1), ... (A = F0 stage, CheapTrick, D4C and
+// modify; S = synthesis): a lane runs its slices in stream order, so A(s + 1) never overwrites rows S(s - 1) still
+// reads, and while synthesis_run waits for its pulse counts (a host synchronisation of its lane), the other lane has an
+// analysis queued.  One lane (one slice, or the host emulation) runs A(s), S(s) in turn.  The caller's stream waits for
+// both lanes on return.
+template <class Bytes, class Analyse, class Synthesise>
+static int transform_slices(WorldB200 *h, const std::vector<int> &bounds, Bytes bytes, Analyse analyse,
+                            Synthesise synthesise) {
+  const int n_slices = (int)bounds.size() - 1;
+  LaneScope lanes(h);
+  int rc = lanes.open(bounds, bytes);
+  if (rc) return rc;
+  const int lag = lanes.one_lane() ? 0 : 1;
+  for (int k = 0; k < n_slices + lag && !rc; ++k) {
+    if (k < n_slices) rc = analyse(lanes, k);
+    if (!rc && k >= lag) rc = synthesise(lanes, k - lag);
+  }
+  return rc;
+}
+
+// A lane's error as the context's
+static int lane_error(WorldB200 *h, WorldB200 *L, int e) {
+  if (e && L != h) h->c.last_error = L->c.last_error;
+  return e;
+}
+
+// The packed transform over utterances [u0, u0 + n): x at sample x_offsets[u0] and y at sample y_off[u0] (DEVICE).
+// Slices are cut by packed_bounds at equal shares of the samples, halved until a slice's own rows fit half its lane's
+// budget.  A slice's lane buffer holds its offsets, padded rows of samples, time axis and f0 as long as its longest
+// utterance (what the F0 stage reads), then its packed f0, spectrogram and aperiodicity frames (what CheapTrick and D4C
+// write and modification and synthesis read), so one long utterance only lengthens the rows of its own slice.
+static int transform_packed_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, const void *x, int u0,
+                                int n, void *y) {
+  const ChainPlan &p = tp.chain;
+  const long long *xo = r.x_offsets, *fo = p.f_off.data(), *yo = tp.syn.y_off.data();
+  const size_t row = p.sp_row, out_bytes = tp.syn.nbit ? 2 : 8;
+  struct Rows { int x_stride, f0_stride; size_t x, t, f, pf, sp, ap, total; };
+  auto rows_of = [&](int a, int b) {
+    Rows w{1, 1, 0, 0, 0, 0, 0, 0, 0};
+    for (int u = a; u < b; ++u) { w.x_stride = imax(w.x_stride, p.x_len[u]); w.f0_stride = imax(w.f0_stride, p.f_len[u]); }
+    const size_t m = (size_t)(b - a), frames = (size_t)(fo[b] - fo[a]);
+    ArenaPlan l;
+    l.add(16 * (m + 1));
+    w.x = l.add(m * w.x_stride * 8);
+    w.t = l.add(m * w.f0_stride * 8); w.f = l.add(m * w.f0_stride * 8);
+    w.pf = l.add(frames * 8); w.sp = l.add(frames * row * 8); w.ap = l.add(frames * row * 8);
+    w.total = l.total;
+    return w;
+  };
+#ifndef WB_EMU
+  const bool two = n > 1;
+#else
+  const bool two = false;
+#endif
+  const size_t cap = h->c.scratch_budget / (two ? 2 : 1) / 2;
+  size_t own = 0;   // every utterance's rows on their own: the least the slices can take
+  for (int u = u0; u < u0 + n; ++u) own += rows_of(u, u + 1).total;
+  int n_slices = (int)std::min<size_t>((size_t)n, std::max<size_t>(1, (own + cap - 1) / cap));
+  if (two) n_slices = imin(n, (n_slices + 1) / 2 * 2);   // an even count: both lanes get the same work
+  const std::vector<int> bounds = packed_bounds(xo, u0, u0 + n, n_slices, cap,
+                                                [&](int a, int b) { return rows_of(a, b).total; });
+  auto bytes = [&](int s) { return rows_of(bounds[s], bounds[s + 1]).total; };
+  std::vector<long long> offs;
+  auto analyse = [&](const LaneScope &lanes, int s) {
+    const int a = bounds[s], m = bounds[s + 1] - a;
+    WorldB200 *L = lanes.lane(s);
+    Ctx *lc = &L->c;
+    const Rows w = rows_of(a, a + m);
+    unsigned char *buf = lanes.buffer(s);
+    // sample offsets relative to x, frame offsets relative to the slice's first frame
+    offs.resize(2 * ((size_t)m + 1));
+    for (int k = 0; k <= m; ++k) { offs[k] = xo[a + k] - xo[u0]; offs[m + 1 + k] = fo[a + k] - fo[a]; }
+    const long long *x_off = (const long long *)buf, *f_off = x_off + m + 1;
+    double *xs = (double *)(buf + w.x), *ts = (double *)(buf + w.t), *fs_ = (double *)(buf + w.f);
+    double *f0 = (double *)(buf + w.pf), *sp = (double *)(buf + w.sp), *ap = (double *)(buf + w.ap);
+    int e = dev_memcpy_h2d(lc, buf, offs.data(), offs.size() * 8);
+    if (!e) e = gather_samples(lc, x, r.nbit, x_off, m, w.x_stride, w.x_stride, xs);
+    const PackedSlice ps{w.x_stride, w.f0_stride, f_off};
+    if (!e) e = chain_f0(L, r, p, a, m, xs, ts, fs_, &ps);
+    if (!e) e = chain_spectral(L, r, p, a, m, xs, ts, fs_, sp, ap, &ps);
+    for (int k0 = 0; k0 < m && !e; k0 += 65535) {
+      WB_LAUNCH_FLAT(scatter_f0_kernel, dim3((unsigned)((w.f0_stride + 255) / 256), (unsigned)imin(65535, m - k0)), 256,
+                     0, lc->stream, f_off + k0, w.f0_stride, ts + (size_t)k0 * w.f0_stride,
+                     fs_ + (size_t)k0 * w.f0_stride, nullptr, f0);
+      e = dev_check(lc, "transform_packed f0");
+    }
+    if (!e && tp.syn.modify)
+      e = modify_run(lc, tp.syn.mod, a, m, p.f_len.data() + a, 0, (int)row, f0, sp, offs.data() + m + 1);
+    return lane_error(h, L, e);
+  };
+  auto synthesise = [&](const LaneScope &lanes, int s) {
+    const int a = bounds[s], m = bounds[s + 1] - a;
+    WorldB200 *L = lanes.lane(s);
+    const Rows w = rows_of(a, a + m);
+    unsigned char *buf = lanes.buffer(s);
+    const int e = synthesis_run(&L->c, tp.syn, a, m, {(const double *)(buf + w.pf), (const double *)(buf + w.sp),
+                                                      (const double *)(buf + w.ap),
+                                                      (unsigned char *)y + (size_t)(yo[a] - yo[u0]) * out_bytes});
+    return lane_error(h, L, e);
+  };
+  return transform_slices(h, bounds, bytes, analyse, synthesise);
+}
+
+// Utterances [u0, u0 + n) of a checked call: x and y point at utterance u0's rows (DEVICE; packed: its first samples);
+// the request's x_lengths and per-utterance options are the call's whole arrays.  The utterances are cut into slices
+// that alternate between the two lanes of a LaneScope (transform_slices).  A slice's rows (float64 input, time axis, f0,
+// spectrogram, aperiodicity) live from its analysis to its synthesis in one buffer per lane, taken from the lane's pool
+// and sized for its largest slice; slices are sized so that the buffer takes at most about half the lane's scratch
+// budget, leaving the rest to the stages.
 int transform_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, const void *x, int u0, int n, void *y) {
   if (n <= 0) return 0;
+  if (r.packed) return transform_packed_run(h, r, tp, x, u0, n, y);
   const ChainPlan &p = tp.chain;
   const int f0_stride = p.f0_stride, x_stride = r.x_stride, nbit = r.nbit, row = (int)p.sp_row;
   const size_t in_row = (size_t)x_stride * (nbit ? nbit / 8 : 8);
@@ -1252,20 +1364,18 @@ int transform_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, 
   }
   std::vector<int> bounds(n_slices + 1);
   for (int s = 0; s <= n_slices; ++s) bounds[s] = (int)((long long)n * s / n_slices);
-  LaneScope lanes(h);
-  int rc = lanes.open(bounds, [&](int s) { return rows_of(bounds[s + 1] - bounds[s]).total; });
-  if (rc) return rc;
   // slice s: its lane, the global index of its first utterance, its size and where its rows are
-  auto slice = [&](int s, WorldB200 **L, int *g, int *m, double **xs, double **t, double **f, double **sp, double **ap) {
+  auto slice = [&](const LaneScope &lanes, int s, WorldB200 **L, int *g, int *m, double **xs, double **t, double **f,
+                   double **sp, double **ap) {
     const Rows at = rows_of(lanes.most(s));
     unsigned char *rows = lanes.buffer(s);
     *L = lanes.lane(s); *g = u0 + bounds[s]; *m = bounds[s + 1] - bounds[s];
     *xs = (double *)(rows + at.x); *t = (double *)(rows + at.t); *f = (double *)(rows + at.f);
     *sp = (double *)(rows + at.sp); *ap = (double *)(rows + at.ap);
   };
-  auto analyse = [&](int s) {
+  auto analyse = [&](const LaneScope &lanes, int s) {
     WorldB200 *L; int g, m; double *xd, *t, *f, *sp, *ap;
-    slice(s, &L, &g, &m, &xd, &t, &f, &sp, &ap);
+    slice(lanes, s, &L, &g, &m, &xd, &t, &f, &sp, &ap);
     const unsigned char *xin = (const unsigned char *)x + (size_t)bounds[s] * in_row;
     const double *xs = nbit ? xd : (const double *)xin;
     int e = nbit ? world_b200_pcm_to_double_batch(L, xin, nbit, m, x_stride, r.x_lengths ? r.x_lengths + g : nullptr, xd)
@@ -1275,22 +1385,16 @@ int transform_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, 
     if (!e) e = chain_f0(L, r, p, g, m, xs, t, f);
     if (!e) e = chain_spectral(L, r, p, g, m, xs, t, f, sp, ap);
     if (!e && tp.syn.modify) e = modify_run(&L->c, tp.syn.mod, g, m, p.f_len.data() + g, f0_stride, row, f, sp);
-    if (e && L != h) h->c.last_error = L->c.last_error;
-    return e;
+    return lane_error(h, L, e);
   };
-  auto synthesise = [&](int s) {
+  auto synthesise = [&](const LaneScope &lanes, int s) {
     WorldB200 *L; int g, m; double *xd, *t, *f, *sp, *ap;
-    slice(s, &L, &g, &m, &xd, &t, &f, &sp, &ap);
+    slice(lanes, s, &L, &g, &m, &xd, &t, &f, &sp, &ap);
     const int e = synthesis_run(&L->c, tp.syn, g, m, {f, sp, ap, (unsigned char *)y + (size_t)bounds[s] * out_row});
-    if (e && L != h) h->c.last_error = L->c.last_error;
-    return e;
+    return lane_error(h, L, e);
   };
-  const int lag = lanes.one_lane() ? 0 : 1;
-  for (int k = 0; k < n_slices + lag && !rc; ++k) {
-    if (k < n_slices) rc = analyse(k);
-    if (!rc && k >= lag) rc = synthesise(k - lag);
-  }
-  return rc;
+  return transform_slices(h, bounds, [&](int s) { return rows_of(bounds[s + 1] - bounds[s]).total; }, analyse,
+                          synthesise);
 }
 
 }  // namespace wb
@@ -1325,10 +1429,49 @@ int world_b200_transform_batch_spectral_options(WorldB200 *h, const void *x, int
   ChainRequest r(x, nbit, n_utts, x_stride, x_lengths, fs, option, nullptr, nullptr, 0, nullptr, nullptr);
   r.harvest_options = harvest_options; r.dio_options = dio_options;
   r.cheaptrick_options = cheaptrick_options; r.d4c_options = d4c_options;
+  r.transform = true;
   TransformPlan tp;
   const int rc = transform_check(h, r, f0_scale, spectral_ratio, time_scale, nbit_out, y, y_stride, "transform_batch", &tp);
   if (rc) return rc;
   if (y_lengths) std::copy(tp.syn.y_len.begin(), tp.syn.y_len.end(), y_lengths);
+  return transform_run(h, r, tp, x, 0, n_utts, y);
+}
+
+int world_b200_transform_packed_samples(int fs, int n_utts, const long long *x_offsets, double frame_period,
+                                        const double *time_scale, long long *y_offsets) {
+  if (fs <= 0 || n_utts < 0 || !(frame_period > 0.0) || !y_offsets) return WORLD_B200_EINVAL;
+  std::vector<int> x_len;
+  std::vector<long long> f_off;
+  if (!packed_layout(fs, n_utts, x_offsets, frame_period, &x_len, &f_off).empty()) return WORLD_B200_EINVAL;
+  std::vector<long long> y_off(1, 0);
+  for (int u = 0; u < n_utts; ++u) {
+    const double ts = time_scale ? time_scale[u] : 1.0;
+    const int y_len = world_b200_transform_samples(fs, x_len[u], frame_period, ts);
+    if (!(ts > 0.0) || !isfinite(ts) || y_len == 0) return WORLD_B200_EINVAL;
+    y_off.push_back(y_off.back() + y_len);
+  }
+  std::copy(y_off.begin(), y_off.end(), y_offsets);
+  return 0;
+}
+
+int world_b200_transform_packed(WorldB200 *h, const void *x, int nbit, int n_utts, const long long *x_offsets, int fs,
+                                const WorldB200AnalysisOption *option, const HarvestOption *harvest_options,
+                                const DioOption *dio_options, const CheapTrickOption *cheaptrick_options,
+                                const D4COption *d4c_options, const double *f0_scale, const double *spectral_ratio,
+                                const double *time_scale, int nbit_out, void *y, long long *y_offsets) {
+  if (!h) return WORLD_B200_EINVAL;
+  if (n_utts == 0) {   // as the packed synthesis calls: nothing to check against, nothing to queue
+    if (y_offsets) y_offsets[0] = 0;
+    return 0;
+  }
+  DeviceGuard guard_(&h->c);
+  ChainRequest r = packed_request(x, nbit, n_utts, x_offsets, fs, option, harvest_options, dio_options,
+                                  cheaptrick_options, d4c_options, nullptr, nullptr, nullptr, nullptr);
+  r.transform = true;
+  TransformPlan tp;
+  const int rc = transform_check(h, r, f0_scale, spectral_ratio, time_scale, nbit_out, y, 0, "transform_packed", &tp);
+  if (rc) return rc;
+  if (y_offsets) std::copy(tp.syn.y_off.begin(), tp.syn.y_off.end(), y_offsets);
   return transform_run(h, r, tp, x, 0, n_utts, y);
 }
 

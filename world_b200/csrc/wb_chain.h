@@ -24,9 +24,10 @@ namespace wb {
 // per-utterance option arrays may be NULL (the AnalysisOption's own option for every utterance); at most one of the two
 // F0 arrays, and the spectral arrays only with coded rows.  coded: spectrogram / aperiodicity receive dims /
 // GetNumberOfAperiodicities(fs) coded values per frame instead of fft_size / 2 + 1 bins.  A NULL spectrogram or
-// aperiodicity skips its stage.  f0_stride 0: a call with no analysis outputs (transform), whose rows are as long as its
-// longest utterance's frame count.  row_stride: doubles per frame of full rows, at least every utterance's
-// fft_size / 2 + 1; 0 for fft_size / 2 + 1 with one option, or the largest size's with per-utterance options.
+// aperiodicity skips its stage.  f0_stride 0: rows as long as the longest utterance's frame count.  row_stride: doubles
+// per frame of full rows, at least every utterance's fft_size / 2 + 1; 0 for fft_size / 2 + 1 with one option, or the
+// largest size's with per-utterance options.  transform: a voice transformation, which has no analysis outputs and
+// plans both spectral stages.
 struct ChainRequest {
   ChainRequest(const void *x, int nbit, int n, int x_stride, const int *x_lengths, int fs,
                const WorldB200AnalysisOption *opt, double *time_axis, double *f0, int f0_stride, double *spectrogram,
@@ -53,6 +54,7 @@ struct ChainRequest {
   // the plan's f_off[u]
   bool packed = false;
   const long long *x_offsets = nullptr;
+  bool transform = false;
 };
 
 // The request of a coded-row entry point: number_of_dimensions coded values per spectral frame.
@@ -123,15 +125,19 @@ int gather_samples(Ctx *ctx, const void *x, int nbit, const long long *x_off, in
 // Voice transformation (world_b200_transform_*): the analysis plan of the request (full rows, no analysis outputs;
 // with spectral options each row as wide as the largest size's) and the synthesis plan of its analysis rows: lengths,
 // each utterance's CheapTrick size, the factors (which modify_run applies right after the analysis) and each
-// utterance's frame period, (frame_period * time_scale[u]) / 1000.0 s.  transform_check makes it once per call;
-// transform_run (device rows) and the host pipeline (wb_host.cu) read it.
+// utterance's frame period, (frame_period * time_scale[u]) / 1000.0 s.  A packed request (r.packed) gets a packed
+// synthesis plan: the chain's frame offsets, sample offsets from world_b200_transform_samples, every utterance at its
+// CheapTrick size on rows of sp_row doubles.  transform_check makes it once per call; transform_run (device rows) and
+// the host pipelines (wb_host.cu) read it.
 struct TransformPlan {
   ChainPlan chain;
   SynthesisPlan syn;
 };
+// y_stride is not read for a packed request.
 int transform_check(WorldB200 *h, const ChainRequest &r, const double *f0_scale, const double *spectral_ratio,
                     const double *time_scale, int nbit_out, void *y, int y_stride, const char *who, TransformPlan *tp);
-// Utterances [u0, u0 + n) of a checked call: x and y point at utterance u0's rows (device).
+// Utterances [u0, u0 + n) of a checked call: x and y point at utterance u0's rows (device); packed: at its first sample
+// of x and of y.
 int transform_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, const void *x, int u0, int n, void *y);
 
 }  // namespace wb

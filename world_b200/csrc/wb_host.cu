@@ -613,6 +613,43 @@ int transform_pipeline(WorldB200 *h, const ChainRequest &r, const TransformPlan 
                         run);
 }
 
+// The packed form for host arrays: chunks of consecutive utterances (at most WB_HOST_CHUNK, default 512, fewer when two
+// input and two output buffers would take more than a sixth of the scratch budget).  Chunk k's samples
+// [x_offsets[c0], x_offsets[c1]) go up as one copy, transform_run transforms them, and its samples [y_off[c0],
+// y_off[c1]) come back as one copy; every sample of a chunk is written, so nothing is zeroed.
+int transform_packed_pipeline(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, void *y) {
+  Ctx *ctx = &h->c;
+  const int n_utts = r.n;
+  const long long *xo = r.x_offsets, *yo = tp.syn.y_off.data();
+  const size_t in_bytes = r.nbit ? (size_t)(r.nbit / 8) : 8, out_bytes = tp.syn.nbit ? 2 : 8;
+  int most = 512;
+  if (const char *e = getenv("WB_HOST_CHUNK")) most = atoi(e) > 0 ? atoi(e) : most;
+  const size_t cap = ctx->scratch_budget / 6;
+  auto bytes = [&](int c0, int c1) {
+    return 2 * ((size_t)(xo[c1] - xo[c0]) * in_bytes + (size_t)(yo[c1] - yo[c0]) * out_bytes);
+  };
+  std::vector<int> bounds{0};
+  size_t most_in = 0, most_out = 0;
+  while (bounds.back() < n_utts) {
+    const int c0 = bounds.back();
+    int c1 = c0 + 1;
+    while (c1 < n_utts && c1 - c0 < most && bytes(c0, c1 + 1) <= cap) ++c1;
+    bounds.push_back(c1);
+    most_in = std::max(most_in, (size_t)(xo[c1] - xo[c0]) * in_bytes);
+    most_out = std::max(most_out, (size_t)(yo[c1] - yo[c0]) * out_bytes);
+  }
+  // chunk k's samples, one copy
+  auto upload = [&](HostPipe &p, int u0, int m, unsigned char *d) {
+    p.h2d(d, (const unsigned char *)r.x + (size_t)xo[u0] * in_bytes, (size_t)(xo[u0 + m] - xo[u0]) * in_bytes);
+  };
+  auto run = [&](int u0, int m, unsigned char *d, unsigned char *out) {
+    return transform_run(h, r, tp, d, u0, m, out);
+  };
+  auto out_at = [&](int u) { return (size_t)yo[u] * out_bytes; };
+  auto zero = [](int, int) { return false; };
+  return chunk_pipeline(h, "transform_packed", bounds, 2, most_in, most_out, out_at, zero, tp.syn.nbit, y, upload, run);
+}
+
 // world_b200_synthesis_coded_host and, with f0_scale / spectral_ratio, world_b200_synthesis_coded_host_modified: every
 // check runs before the first chunk is queued
 // (fft_sizes NULL: fft_size for every utterance; world_b200_synthesis_coded_host_options passes per_utt)
@@ -702,6 +739,7 @@ extern "C" int world_b200_transform_host_spectral_options(
   ChainRequest r(x, nbit, n_utts, x_stride, x_lengths, fs, option, nullptr, nullptr, 0, nullptr, nullptr);
   r.harvest_options = harvest_options; r.dio_options = dio_options;
   r.cheaptrick_options = cheaptrick_options; r.d4c_options = d4c_options;
+  r.transform = true;
   TransformPlan tp;
   const int rc = transform_check(h, r, f0_scale, spectral_ratio, time_scale, nbit_out, y, y_stride, "transform_host", &tp);
   if (rc) return rc;
@@ -719,6 +757,31 @@ extern "C" int world_b200_transform_host(WorldB200 *h, const void *x, int nbit, 
   return world_b200_transform_host_spectral_options(h, x, nbit, n_utts, x_stride, x_lengths, fs, option,
                                                     harvest_options, dio_options, nullptr, nullptr, f0_scale,
                                                     spectral_ratio, time_scale, nbit_out, y, y_stride, y_lengths);
+}
+
+extern "C" int world_b200_transform_host_packed(WorldB200 *h, const void *x, int nbit, int n_utts,
+                                                const long long *x_offsets, int fs,
+                                                const WorldB200AnalysisOption *option,
+                                                const HarvestOption *harvest_options, const DioOption *dio_options,
+                                                const CheapTrickOption *cheaptrick_options,
+                                                const D4COption *d4c_options, const double *f0_scale,
+                                                const double *spectral_ratio, const double *time_scale, int nbit_out,
+                                                void *y, long long *y_offsets) {
+  if (!h) return WORLD_B200_EINVAL;
+  if (n_utts == 0) {
+    if (y_offsets) y_offsets[0] = 0;
+    return 0;
+  }
+  DeviceGuard guard_(&h->c);
+  ChainRequest r = packed_request(x, nbit, n_utts, x_offsets, fs, option, harvest_options, dio_options,
+                                  cheaptrick_options, d4c_options, nullptr, nullptr, nullptr, nullptr);
+  r.transform = true;
+  TransformPlan tp;
+  const int rc = transform_check(h, r, f0_scale, spectral_ratio, time_scale, nbit_out, y, 0, "transform_host_packed",
+                                 &tp);
+  if (rc) return rc;
+  if (y_offsets) std::copy(tp.syn.y_off.begin(), tp.syn.y_off.end(), y_offsets);
+  return transform_packed_pipeline(h, r, tp, y);
 }
 
 extern "C" int world_b200_analyze_host(WorldB200 *h, const double *x, int n_utts, int x_stride,
