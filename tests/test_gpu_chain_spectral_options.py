@@ -11,10 +11,6 @@ from world_b200.api import WorldError
 pytestmark = pytest.mark.gpu
 
 CASES = [(16000, 12000), (22050, 13230), (48000, 24000)]
-# DIO's own stage call departs from the reference (up to 2 % on the first frames) and from itself in another batch on
-# these 48 kHz voices, which are voiced from their first sample, once its floor is at 50 Hz or below.  The chain only
-# passes DIO's rows on, so the DIO cases with per-utterance F0 floors stop at 22.05 kHz.
-DIO_48K = "DIO's stage call itself differs at 48 kHz with floors of 50 Hz and below on these signals"
 
 
 @pytest.mark.parametrize("fs,n", CASES)
@@ -22,8 +18,6 @@ DIO_48K = "DIO's stage call itself differs at 48 kHz with floors of 50 Hz and be
 @pytest.mark.parametrize("f0_options", [True, False])
 def test_gpu_chain_spectral_options_groups(gpu_world, fs, n, method, f0_options):
     """Ten utterances in two lane slices."""
-    if method == "dio" and fs == 48000 and f0_options:
-        pytest.skip(DIO_48K)
     cs.check_groups(gpu_world, fs, n, 10, method=method, f0_options=f0_options)
 
 
@@ -40,8 +34,6 @@ def test_gpu_chain_spectral_options_identity(gpu_world, fs, n, method):
 @pytest.mark.parametrize("fs,n", CASES)
 @pytest.mark.parametrize("method", ["harvest", "dio"])
 def test_gpu_chain_spectral_options_vs_reference(gpu_world, ref, fs, n, method):
-    if method == "dio" and fs == 48000:
-        pytest.skip(DIO_48K)
     cs.check_vs_ref(gpu_world, ref, fs, n, n_utts=8, method=method)
 
 

@@ -7,17 +7,12 @@ import packed_common as pk
 pytestmark = pytest.mark.gpu
 
 CASES = [(16000, 12000), (22050, 13230), (48000, 24000)]
-# as in test_gpu_chain_spectral_options.py: DIO's own stage call departs from the reference and from itself in another
-# batch at 48 kHz with floors of 50 Hz and below on these signals
-DIO_48K = "DIO's stage call itself differs at 48 kHz with floors of 50 Hz and below on these signals"
 
 
 @pytest.mark.parametrize("fs,n", CASES)
 @pytest.mark.parametrize("method", ["harvest", "dio"])
 @pytest.mark.parametrize("f0_options", [True, False])
 def test_gpu_packed_equals_padded(gpu_world, fs, n, method, f0_options):
-    if method == "dio" and fs == 48000 and f0_options:
-        pytest.skip(DIO_48K)
     pk.check_equal(gpu_world, fs, n, 10, method=method, f0_options=f0_options)
 
 

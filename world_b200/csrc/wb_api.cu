@@ -201,8 +201,21 @@ void pool_release(Ctx *ctx, void *p) {
 // One block of `bytes` device scratch, valid until the next arena_block() call on this
 // context.  Stage drivers lay out their scratch with ArenaPlan and ask for the total; the block
 // only grows (sync + free + cudaMalloc), so steady-state calls allocate nothing.
+// WB_ARENA_POISON=<byte> (test hook, README): the block is filled with that byte (stream ordered) before it is
+// returned, so a stage that reads scratch it did not write this call sees the poison instead of earlier values.  A
+// value that is not one byte (0..255, decimal or 0x hex) fails the call rather than poisoning with something else.
 unsigned char *arena_block(Ctx *ctx, size_t bytes) {
   Arena &a = ctx->arena;
+  int poison = -1;
+  if (const char *e = getenv("WB_ARENA_POISON")) {
+    char *end = nullptr;
+    const long v = strtol(e, &end, 0);
+    if (end == e || *end != '\0' || v < 0 || v > 255) {
+      ctx->last_error = std::string("WB_ARENA_POISON=\"") + e + "\": not a byte value (0..255, decimal or 0x hex)";
+      return nullptr;
+    }
+    poison = (int)v;
+  }
   if (bytes > a.capacity) {
     dev_sync(ctx);
     dev_free(a.base);
@@ -214,6 +227,7 @@ unsigned char *arena_block(Ctx *ctx, size_t bytes) {
     a.capacity = want;
   }
   a.used = bytes;
+  if (poison >= 0 && dev_memset(ctx, a.base, poison, bytes)) return nullptr;
   return a.base;
 }
 

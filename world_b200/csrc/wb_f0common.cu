@@ -417,11 +417,15 @@ WB_DEV void sweep_body(const SweepParams &p, const int b, const int u) {
       }
       ni[q] = n_new;
       tr.ifrom[q] = from;
-      if (n_new < 1) can = false;
+      if (n_new < 2) can = false;
     }
     WB_SYNC();
     // ---- streaming candidates: every frame whose time lies before the last complete interval of
-    // all four trains can be interpolated now.
+    // all four trains can be interpolated now.  Such a frame precedes interval ni - 1 of every train, so interp1's
+    // segment is k = max(1, count) <= ni - 1 whatever the final interval count; k = 1 (frames before a train's
+    // second interval) needs intervals 0 and 1, hence two intervals per train before anything streams.  With one,
+    // train_value would clamp k to 0, and interval -1 (below ifrom) goes to edge_at(q, -1): the element just before
+    // the train's global edge list, i.e. another train's, band's or utterance's edges, or what an earlier call left.
     if (can) {
       double t_safe = loc_at(tr, 0, ni[0] - 1);
       for (int q = 1; q < 4; ++q) t_safe = dmin(t_safe, loc_at(tr, q, ni[q] - 1));
