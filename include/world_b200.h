@@ -62,8 +62,8 @@ int world_b200_set_stream(WorldB200 *ctx, void *cuda_stream);
  * utterance chunks that fit it.  Default: a third of the memory free at creation, clamped to
  * [4, 64] GiB. */
 int world_b200_set_scratch_budget(WorldB200 *ctx, unsigned long long bytes);
-/* Synchronises and releases the device memory the context keeps between calls (scratch arena and the
- * staging buffers of the *_host pipelines); the next call allocates again. */
+/* Synchronises and releases the device memory the context keeps between calls (scratch arena, the randn()
+ * stream table and the staging buffers of the *_host pipelines); the next call allocates again. */
 int world_b200_trim(WorldB200 *ctx);
 int world_b200_synchronize(WorldB200 *ctx);
 const char *world_b200_last_error(const WorldB200 *ctx);

@@ -255,6 +255,7 @@ int ctx_init_tables(Ctx *ctx) {
   if (!rc) rc = dev_memcpy_h2d(ctx, ctx->twiddle_sized, tw_sized.data(), tw_sized.size() * sizeof(double2));
   if (!rc) rc = dev_memcpy_h2d(ctx, ctx->rng_jump, jump.data(), jump.size() * 4);
   if (!rc) rc = dev_memset(ctx, ctx->status_dev, 0, sizeof(int));
+  if (!rc && !rng_table_reserve(ctx, 1)) rc = WORLD_B200_ENOMEM;
   if (!rc) rc = dev_sync(ctx);
   return rc;
 }
@@ -360,6 +361,7 @@ void world_b200_destroy(WorldB200 *h) {
   dev_free(h->c.twiddle);
   dev_free(h->c.twiddle_sized);
   dev_free(h->c.rng_jump);
+  dev_free(h->c.rng_table);
   dev_free(h->c.status_dev);
   dev_free(h->c.arena.base);
   dev_free(h->lens_dev);
@@ -394,6 +396,9 @@ int world_b200_trim(WorldB200 *h) {
   pool_trim(&h->c);
   dev_free(h->c.arena.base);
   h->c.arena = Arena();
+  dev_free(h->c.rng_table);
+  h->c.rng_table = nullptr;
+  h->c.rng_table_len = 0;
   return rc;
 }
 
@@ -1928,12 +1933,7 @@ int world_b200_randn_window(WorldB200 *h, unsigned long long first, unsigned n, 
     return WORLD_B200_EINVAL;
   }
   if (n == 0) return 0;
-  unsigned char *blk = arena_block(ctx, 256);
-  if (!blk) return WORLD_B200_ENOMEM;
-  const unsigned end = (unsigned)(first + n);
-  int rc = dev_memcpy_h2d(ctx, blk, &end, sizeof(unsigned));
-  if (rc) return rc;
-  rng_fill(ctx, reinterpret_cast<unsigned *>(blk), out_dev, 0, end, 1, (unsigned)first);
+  rng_fill(ctx, out_dev, (unsigned)first, (unsigned)(first + n));
   return dev_check(ctx, "randn_window");
 }
 

@@ -21,7 +21,8 @@ struct CtParams {
   const double *time_axis; const double *f0; const int *f_len; int f_stride;
   int fs, fft_size, lg_fft;
   double q1, f0_floor;
-  const unsigned *draws; size_t draw_stride; const unsigned *draw_off;
+  const unsigned *draws;  // the context's stream table: a frame's draws start at its draw_off entry
+  const unsigned *draw_off;
   double *out;            // [n][f_stride][out_stride], or (f_off) [F][out_stride]
   int out_stride;         // doubles per spectrogram row (fft/2+1 unless the caller pads its rows)
   const int *uid;         // [n] batch index of the launch's utterance blockIdx.y; null: blockIdx.y itself
@@ -65,7 +66,7 @@ template <bool kCoded>
 WB_DEV void ct_frame_body(const CtParams &p) {
   WB_DYN_SMEM(double2, smem2);
   const int tid = WB_TID, nth = WB_NTH;
-  const int ul = blockIdx.y, i = blockIdx.x;   // f_len, draws and draw offsets follow the launch's order
+  const int ul = blockIdx.y, i = blockIdx.x;   // f_len and draw offsets follow the launch's order
   if (i >= p.f_len[ul]) return;
   const int u = p.uid ? __ldg(p.uid + ul) : ul;
   const int N = p.fft_size, half = N / 2;
@@ -81,7 +82,7 @@ WB_DEV void ct_frame_body(const CtParams &p) {
   const int fs = p.fs;
   const int x_len = p.x_len[u];
   const double *x = p.x + (size_t)u * p.x_stride;
-  const unsigned *draw = p.draws + (size_t)ul * p.draw_stride + p.draw_off[(size_t)ul * p.f_stride + i];
+  const unsigned *draw = p.draws + p.draw_off[(size_t)ul * p.f_stride + i];
 
   const int h = round_half_away(1.5 * fs / f);
   const int nwin = 2 * h + 1;
@@ -251,9 +252,10 @@ static int ct_launch(Ctx *ctx, const Batch &b, double q1, int fft_size, double *
   const int bins = fft_size / 2 + 1;
   // a frame draws at most (fft_size - 2) + bins numbers (2h+1 <= fft_size - 2 above the floor)
   const size_t max_per_frame = (size_t)fft_size + bins;
-  const size_t draw_stride_full = max_per_frame * (size_t)max_f_len;
-  // utterances per chunk so that the draw scratch fits the budget
-  const size_t per_utt_bytes = draw_stride_full * 4 + (size_t)b.f_stride * 8 + 64;
+  const unsigned *table = rng_table_reserve(ctx, max_per_frame * (size_t)max_f_len);
+  if (!table) return 2;
+  // utterances per chunk so that the draw counts and offsets fit the budget
+  const size_t per_utt_bytes = (size_t)b.f_stride * 8 + 64;
   int chunk = balanced_chunk(imin(n_all, 65535), (int)dmin(65535.0, (double)ctx->scratch_budget / (double)per_utt_bytes));
   const size_t smem = ct_smem_bytes(fft_size);
 #ifndef WB_EMU
@@ -267,15 +269,14 @@ static int ct_launch(Ctx *ctx, const Batch &b, double q1, int fft_size, double *
     const size_t o_counts = plan.add((size_t)n * b.f_stride * 4);
     const size_t o_offs = plan.add((size_t)n * b.f_stride * 4);
     const size_t o_totals = plan.add((size_t)n * 4);
-    const size_t o_draws = plan.add((size_t)n * draw_stride_full * 4);
     const size_t o_cidx = plan.add(n_tab * 4 + 4), o_cfrac = plan.add(n_tab * 8 + 8), o_cw = plan.add(n_w * 16 + 16);
     const size_t o_group = plan.add(group ? (size_t)n * 8 : 0);
     unsigned char *blk = arena_block(ctx, plan.total);
     if (!blk) return 2;
     unsigned *counts = (unsigned *)(blk + o_counts), *offs = (unsigned *)(blk + o_offs);
-    unsigned *totals = (unsigned *)(blk + o_totals), *draws = (unsigned *)(blk + o_draws);
+    unsigned *totals = (unsigned *)(blk + o_totals);
     // a group keeps the batch's base pointers and reaches its utterances through uid; its frame counts are uploaded
-    // in the launch's order, which is the order counts, offsets and draws are laid out in
+    // in the launch's order, which is the order counts and offsets are laid out in
     const size_t base = group ? 0 : (size_t)u0;
     const int *uid = nullptr, *f_len = b.f_len + u0;
     if (group) {
@@ -290,13 +291,12 @@ static int ct_launch(Ctx *ctx, const Batch &b, double q1, int fft_size, double *
     WB_LAUNCH_FLAT(ct_count_kernel, dim3((unsigned)((total_slots + 255) / 256)), 256, 0, ctx->stream,
                    f0, f_len, b.f_stride, n, b.fs, fft_size, f0_floor, uid, counts);
     scan_counts(ctx, counts, f_len, b.f_stride, nullptr, offs, totals, n);
-    rng_fill(ctx, totals, draws, draw_stride_full, draw_stride_full, n);
     CtParams p;
     p.x = b.x + base * b.x_stride; p.x_len = b.x_len + base; p.x_stride = b.x_stride;
     p.time_axis = b.time_axis + base * b.f_stride; p.f0 = f0; p.f_len = f_len; p.uid = uid;
     p.f_stride = b.f_stride; p.fs = b.fs; p.fft_size = fft_size; p.lg_fft = lg;
     p.q1 = q1; p.f0_floor = f0_floor;
-    p.draws = draws; p.draw_stride = draw_stride_full; p.draw_off = offs;
+    p.draws = table; p.draw_off = offs;
     p.out_stride = row_stride > 0 ? row_stride : bins;
     // packed rows: the output pointers stay at frame 0 and f_off places each utterance
     const size_t out_base = b.f_off ? 0 : base * b.f_stride;

@@ -27,7 +27,7 @@ struct D4cParams {
   int d_fft, d_lg, n_ap, win_len, bd;
   double threshold;
   const double *nuttall;    // [win_len]
-  const unsigned *draws; size_t draw_stride;
+  const unsigned *draws;    // the context's stream table: a frame's draws start at its off_a / off_b entry
   const unsigned *off_a; unsigned *count_b; const unsigned *off_b;
   unsigned char *selected;  // [n][f_stride]
   int *slow_list; int *slow_count;   // frames whose window does not fit the fast body kernel (long windows, f0 near the floor)
@@ -179,7 +179,7 @@ WB_KERNEL(128, 4) d4c_lovetrain_kernel(D4cParams p) {
   double *za = reinterpret_cast<double *>(A), *win = reinterpret_cast<double *>(B);
   const double f = dmax(f0, 40.0);
   const double *x = p.x + (size_t)u * p.x_stride;
-  const unsigned *draw = p.draws + (size_t)u * p.draw_stride + p.off_a[fidx];
+  const unsigned *draw = p.draws + p.off_a[fidx];
   const int nwin = d4c_windowed(x, p.x_len[u], p.fs, f, p.time_axis[fidx], 2, 3.0, draw,
                                 [&](int j) { return za + rpad(j); }, [&](int j) { return win + j; }, red);
   for (int j = nwin + tid; j < N; j += nth) za[rpad(j)] = 0.0;
@@ -419,7 +419,7 @@ WB_DEV void d4c_body_frame(const D4cParams &p) {
   }
   const double *x = p.x + (size_t)u * p.x_stride;
   const int x_len = p.x_len[u];
-  const unsigned *draw = p.draws + (size_t)u * p.draw_stride + p.off_b[fidx];
+  const unsigned *draw = p.draws + p.off_b[fidx];
 
   // ---- static centroid = centroid(t - 1/4f) + centroid(t + 1/4f)   (d4c.cpp:90-140)
   for (int pass = 0; pass < 2; ++pass) {
@@ -555,7 +555,7 @@ WB_DEV void d4c_body_slow_frame(const D4cParams &p, int u, int i, double *smem) 
   const double t = p.time_axis[fidx];
   const double *x = p.x + (size_t)u * p.x_stride;
   const int x_len = p.x_len[u];
-  const unsigned *draw = p.draws + (size_t)u * p.draw_stride + p.off_b[fidx];
+  const unsigned *draw = p.draws + p.off_b[fidx];
 
   // ---- static centroid = centroid(t - 1/4f) + centroid(t + 1/4f)   (d4c.cpp:90-140)
   for (int pass = 0; pass < 2; ++pass) {
@@ -722,6 +722,12 @@ int d4c_run(Ctx *ctx, const StagePlan &stage, const Batch &b, int u0, double *ou
     }
   }
 
+  // a frame draws at most max_a numbers in pass A and max_b in pass B
+  const size_t max_a = (size_t)(2 * round_half_away(3.0 * fs / 40.0 / 2.0) + 1);
+  const size_t max_b = 3 * (size_t)(2 * round_half_away(4.0 * fs / 47.0 / 2.0) + 1);
+  const unsigned *table = rng_table_reserve(ctx, (max_a + max_b) * (size_t)b.max_f_len);
+  if (!table) return 2;
+
   // Nuttall window of the band analysis (common.cpp:113-121), host libm like the reference
   double *nuttall_host = new double[p.win_len];
   for (int i = 0; i < p.win_len; ++i) {
@@ -730,10 +736,7 @@ int d4c_run(Ctx *ctx, const StagePlan &stage, const Batch &b, int u0, double *ou
                       0.012604 * cos(6.0 * kPi * tmp);
   }
 
-  const size_t max_a = (size_t)(2 * round_half_away(3.0 * fs / 40.0 / 2.0) + 1);
-  const size_t max_b = 3 * (size_t)(2 * round_half_away(4.0 * fs / 47.0 / 2.0) + 1);
-  const size_t draw_stride_full = (max_a + max_b) * (size_t)b.max_f_len;
-  const size_t per_utt_bytes = draw_stride_full * 4 + (size_t)b.f_stride * 28 + 64;
+  const size_t per_utt_bytes = (size_t)b.f_stride * 28 + 64;
   int chunk = balanced_chunk(imin(b.n, 65535), (int)dmin(65535.0, (double)ctx->scratch_budget / (double)per_utt_bytes));
   // fast body kernel: one radix-8 butterfly per thread in the passes of the d_fft / 2 complex transforms; at d_fft
   // above 4096 its thread count would exceed a CTA, below 512 a warp
@@ -761,7 +764,6 @@ int d4c_run(Ctx *ctx, const StagePlan &stage, const Batch &b, int u0, double *ou
     const size_t o_ta = plan.add((size_t)n * 4), o_tab = plan.add((size_t)n * 4);
     const size_t o_sel = plan.add(slots), o_nut = plan.add((size_t)p.win_len * 8);
     const size_t o_slow = plan.add(slots * 4), o_nslow = plan.add(4);
-    const size_t o_draws = plan.add((size_t)n * draw_stride_full * 4);
     const size_t n_tab = coded ? (per_utt ? ctab_idx.size() : coded->idx.size()) : 0;
     const size_t o_cidx = plan.add(n_tab * 4 + 4), o_cfrac = plan.add(n_tab * 8 + 8);
     const size_t o_uopt = plan.add(per_utt ? (size_t)n * 16 : 0);
@@ -772,14 +774,13 @@ int d4c_run(Ctx *ctx, const StagePlan &stage, const Batch &b, int u0, double *ou
     unsigned *total_a = (unsigned *)(blk + o_ta), *total_ab = (unsigned *)(blk + o_tab);
     unsigned char *selected = blk + o_sel;
     double *nuttall = (double *)(blk + o_nut);
-    unsigned *draws = (unsigned *)(blk + o_draws);
     dev_memcpy_h2d(ctx, nuttall, nuttall_host, (size_t)p.win_len * 8);
     const double *f0 = b.f0 + (size_t)c0 * b.f_stride;
     const int *f_len = b.f_len + c0;
     p.x = b.x + (size_t)c0 * b.x_stride; p.x_len = b.x_len + c0; p.x_stride = b.x_stride;
     p.time_axis = b.time_axis + (size_t)c0 * b.f_stride; p.f0 = f0; p.f_len = f_len;
     p.f_stride = b.f_stride;
-    p.nuttall = nuttall; p.draws = draws; p.draw_stride = draw_stride_full;
+    p.nuttall = nuttall; p.draws = table;
     p.off_a = off_a; p.count_b = count_b; p.off_b = off_b; p.selected = selected;
     // packed rows: the output pointers stay at frame 0 and f_off places each utterance
     const size_t out_base = b.f_off ? 0 : (size_t)c0 * b.f_stride;
@@ -813,12 +814,9 @@ int d4c_run(Ctx *ctx, const StagePlan &stage, const Batch &b, int u0, double *ou
     WB_LAUNCH_FLAT(d4c_count_a_kernel, dim3((unsigned)((slots + 255) / 256)), 256, 0, ctx->stream, f0,
                    f_len, b.f_stride, n, fs, count_a);
     scan_counts(ctx, count_a, f_len, b.f_stride, nullptr, off_a, total_a, n);
-    rng_fill(ctx, total_a, draws, draw_stride_full, max_a * (size_t)b.max_f_len, n);
     WB_LAUNCH_COOP(d4c_lovetrain_kernel, dim3((unsigned)b.max_f_len, (unsigned)n), lt_threads, smem_lt,
                    ctx->stream, p);
     scan_counts(ctx, count_b, f_len, b.f_stride, total_a, off_b, total_ab, n);
-    // regenerates the pass-A prefix as well (identical values) -- simple, and pass A is ~20 % of the stream
-    rng_fill(ctx, total_ab, draws, draw_stride_full, draw_stride_full, n);
     if (all_slow)
       WB_LAUNCH_FLAT(d4c_list_all_kernel, dim3((unsigned)((slots + 255) / 256)), 256, 0, ctx->stream, p, n);
     else

@@ -48,6 +48,10 @@ struct Ctx {
   double2 *twiddle = nullptr;        // [WB_TW_N/2] exp(-j 2 pi k / WB_TW_N)
   double2 *twiddle_sized = nullptr;  // [WB_TW_SIZED_ENTRIES] the same values, one contiguous table per size (wb_fft.cuh)
   uint32_t *rng_jump = nullptr;      // [WB_RNG_NJ][32][16] uint4
+  // Draws [0, rng_table_len) of the randn() stream, the exact uint32 sums (those below WB_RNG_REACH filled): every
+  // CheapTrick, D4C and Synthesis call reads its frames' draws at their stream offsets here (rng_table_reserve)
+  unsigned *rng_table = nullptr;
+  size_t rng_table_len = 0;
   Arena arena;
   Staging staging;
   std::vector<PoolBuf> pool;
@@ -115,10 +119,13 @@ int dev_check(Ctx *ctx, const char *what);      // cudaGetLastError -> last_erro
 
 // wb_rng.cu
 void rng_build_jump_tables(uint32_t *tables);
-// draws [first, totals[u]) of utterance u's stream into out + u * utt_stride (first = 0 in the stages), or with
-// utt_off (device, [n_utts]) into out + utt_off[u]
-void rng_fill(const Ctx *ctx, const unsigned *totals_dev, unsigned *out, size_t utt_stride,
-              size_t max_draws_per_utt, int n_utts, unsigned first = 0, const long long *utt_off = nullptr);
+// draws [first, end) of the stream into out[0, end - first) (end <= WB_RNG_REACH)
+void rng_fill(const Ctx *ctx, unsigned *out, unsigned first, unsigned end);
+// The context's stream table holding at least draws [0, draws) (nullptr + last_error on failure).  The table is context
+// memory like the twiddle and jump tables, outside the scratch budget: it grows (synchronise, free, allocate a little
+// more than asked, fill) and never shrinks except through world_b200_trim().  Draws at and past WB_RNG_REACH are
+// allocated but not generated: a call whose offsets reach them has had scan_counts flag WORLD_B200_EDOMAIN.
+const unsigned *rng_table_reserve(Ctx *ctx, size_t draws);
 // counts / offsets of utterance u at u * stride, or with utt_off (device, [n_utts]) at utt_off[u]
 void scan_counts(const Ctx *ctx, const unsigned *counts, const int *lens_dev, int stride,
                  const unsigned *base, unsigned *offsets, unsigned *totals, int n_utts,
@@ -309,7 +316,7 @@ struct SynthesisSizing {
   size_t packed_utt(int y_len, int f_len, int cap) const;
   size_t packed_pass() const;
   int fft_size, y_stride, nominal_cap, fs;   // fft_size: the plan's largest, the stride of each response
-  size_t decoded_per_utt, draw_stride, decoded_per_frame;
+  size_t decoded_per_utt, max_draws, decoded_per_frame;
   double budget;
 };
 // The rows of utterances [u0, u0 + m) of a planned call: device pointers at utterance u0 (packed: at its first frame

@@ -7,7 +7,8 @@
 //
 // GPU restatement: the draw counts per frame are a pure function of f0 (counted by the
 // stage's own kernel), an exclusive scan gives every frame its offset into the utterance's
-// stream, and the stream itself is materialised by `rng_fill_kernel`: thread g produces draws
+// stream, and the stream itself -- the same for every utterance -- is materialised once per
+// context (rng_table_reserve) by `rng_fill_kernel`: thread g produces draws
 // [128 g, 128 g + 128) after jumping there with popcount(g) GF(2) matrix-vector products
 // (xorshift128 is linear over GF(2); J_k = T^(12*128*2^k) are precomputed on the host as
 // 4-bit lookup tables).  Draws are stored as the exact uint32 sum so consumers evaluate
@@ -89,18 +90,12 @@ WB_DEV unsigned rng_draw(uint4 &s) {
   return acc;
 }
 
-// grid: (ceil(chunks / 32) , n_utts); block: 32*WB_RNG_WARPS threads; each warp produces
-// 32 chunks of WB_RNG_CHUNK draws = 4096 consecutive draws, stored coalesced via a smem tile.
-// Draws [first, totals[u]) of the stream, draw d at out[u * utt_stride + d - first]; the stages
-// pass first = 0, the window hook any first.  Every total is at most WB_RNG_REACH (scan_counts
-// clamps and flags larger ones), so chunk g < 2^WB_RNG_NJ and no draw index wraps.  utt_off: the
-// utterances' draws packed, utterance u's from out + utt_off[u] (null: out + u * utt_stride).
-WB_KERNEL_PLAIN rng_fill_kernel(const uint4 *__restrict__ jump, const unsigned *__restrict__ totals,
-                                unsigned *__restrict__ out, size_t utt_stride, unsigned first,
-                                const long long *__restrict__ utt_off) {
-  const int utt = blockIdx.y;
-  const unsigned total = totals[utt];
-  unsigned *dst = out + (utt_off ? (size_t)utt_off[utt] : (size_t)utt * utt_stride);
+// grid: ceil(chunks / 32 / WB_RNG_WARPS); block: 32*WB_RNG_WARPS threads; each warp produces 32 chunks of
+// WB_RNG_CHUNK draws = 4096 consecutive draws, stored coalesced via a smem tile.  Draws [first, total) of the stream,
+// draw d at dst[d - first]; the context's table takes first = 0, the window hook any first.  total is at most
+// WB_RNG_REACH, so chunk g < 2^WB_RNG_NJ and no draw index wraps.
+WB_KERNEL_PLAIN rng_fill_kernel(const uint4 *__restrict__ jump, unsigned *__restrict__ dst, unsigned first,
+                                unsigned total) {
   const unsigned chunk0 = first / WB_RNG_CHUNK;
   // draw d goes to dst[d - first] if d - first < span: one unsigned compare (d < first wraps past span)
   const unsigned span = total > first ? total - first : 0u;
@@ -140,23 +135,45 @@ WB_KERNEL_PLAIN rng_fill_kernel(const uint4 *__restrict__ jump, const unsigned *
 #endif
 }
 
-void rng_fill(const Ctx *ctx, const unsigned *totals_dev, unsigned *out, size_t utt_stride,
-              size_t max_draws_per_utt, int n_utts, unsigned first, const long long *utt_off) {
-  if (max_draws_per_utt > WB_RNG_REACH) max_draws_per_utt = WB_RNG_REACH;   // totals never exceed the reach
-  if (n_utts <= 0 || max_draws_per_utt <= first) return;
+void rng_fill(const Ctx *ctx, unsigned *out, unsigned first, unsigned end) {
+  if (end <= first) return;
   const size_t chunk0 = first / WB_RNG_CHUNK;
-  const size_t chunks = (max_draws_per_utt + WB_RNG_CHUNK - 1) / WB_RNG_CHUNK - chunk0;
+  const size_t chunks = ((size_t)end + WB_RNG_CHUNK - 1) / WB_RNG_CHUNK - chunk0;
   const unsigned per_block = 32 * WB_RNG_WARPS;
-  dim3 grid((unsigned)((chunks + per_block - 1) / per_block), (unsigned)n_utts);
-  WB_LAUNCH_FLAT(rng_fill_kernel, grid, per_block, 0, ctx->stream,
-                 reinterpret_cast<const uint4 *>(ctx->rng_jump), totals_dev, out, utt_stride, first, utt_off);
+  WB_LAUNCH_FLAT(rng_fill_kernel, dim3((unsigned)((chunks + per_block - 1) / per_block)), per_block, 0, ctx->stream,
+                 reinterpret_cast<const uint4 *>(ctx->rng_jump), out, first, end);
+}
+
+// ------------------------------------------------------------------ the context's stream table
+// Every utterance of every call reads the same stream from draw 0 (the reference reseeds at each call), so one table
+// serves them all; a frame's draws are table + its offset.  The table is sized to the largest per-utterance bound a call
+// asked for, plus an eighth, in steps of 2^20 draws (4 MB): calls of similar shapes do not grow it again.  A context
+// starts with one step (ctx_init_tables), so calls on short utterances never grow it.
+const unsigned *rng_table_reserve(Ctx *ctx, size_t draws) {
+  if (ctx->rng_table && draws <= ctx->rng_table_len) return ctx->rng_table;
+  const size_t step = (size_t)1 << 20;
+  const size_t len = (draws + draws / 8 + step - 1) / step * step;
+  // kernels queued on the stream may still read the old table
+  if (ctx->rng_table) {
+    if (dev_sync(ctx)) return nullptr;
+    dev_free(ctx->rng_table);
+    ctx->rng_table = nullptr;
+    ctx->rng_table_len = 0;
+  }
+  unsigned *t = (unsigned *)dev_malloc(ctx, len * sizeof(unsigned));
+  if (!t) return nullptr;
+  rng_fill(ctx, t, 0, (unsigned)(len < WB_RNG_REACH ? len : WB_RNG_REACH));
+  if (dev_check(ctx, "randn table")) { dev_free(t); return nullptr; }
+  ctx->rng_table = t;
+  ctx->rng_table_len = len;
+  return t;
 }
 
 // ------------------------------------------------------------------ per-utterance scans
 // counts[u][0..len_u) -> exclusive offsets (same layout) + totals[u] (+ base[u] added to every
 // offset, used by D4C's second pass which continues the stream after the first pass).  The sums
 // run in 64 bits: a total beyond WB_RNG_REACH sets status bit 8 (world_b200_synchronize reports
-// WORLD_B200_EDOMAIN) and is stored clamped to the reach, so rng_fill never repeats the stream.
+// WORLD_B200_EDOMAIN) and is stored clamped to the reach.
 // utt_off: utterance u's counts and offsets start at utt_off[u] (packed; null: at u * stride).
 WB_KERNEL_PLAIN scan_counts_kernel(const unsigned *__restrict__ counts, const int *__restrict__ lens,
                                    int stride, const unsigned *__restrict__ base,

@@ -53,7 +53,7 @@ struct SynParams {
   int *pulse_idx; double *pulse_shift; int *n_pulses; int pulse_cap;   // [n][pulse_cap]
   int *pulse_count;         // [n] pulses found, also those beyond pulse_cap (the host sizes the arrays from it)
   unsigned *draw_cnt; unsigned *draw_off; unsigned *draw_tot;
-  const unsigned *draws; size_t draw_stride;
+  const unsigned *draws;    // the context's stream table: a pulse's draws start at its draw_off entry
   double *resp;             // [n][pulse_cap][resp_n]: response i of utterance u at (u * pulse_cap + i) * resp_n
   int resp_n;               // the largest fft_size of the call
   const double *dc_remover; // [fft_size]
@@ -63,7 +63,7 @@ struct SynParams {
   short *y16;               // [n][y_stride] 16-bit PCM output (syn_overlap_kernel<short>), else null
   // A packed pass (null: the padded addressing above).  [n + 1] offsets from the pass's first utterance:
   const long long *f_off;   // frames: f0, sp and ap rows of utterance u start at frame f_off[u]
-  const long long *s_off;   // samples: phase, vuv and y; utterance u's draws start at s_off[u] + 8u
+  const long long *s_off;   // samples: phase, vuv and y
   const long long *p_off;   // pulse slots: pulse_idx, pulse_shift, draw counts / offsets and responses (its capacity
                             // is p_off[u + 1] - p_off[u])
   const long long *cum;     // syn_pulse_kernel: [list_n + 1] first pulse of each entry of `list`; blockIdx.x is the pulse
@@ -283,8 +283,7 @@ WB_KERNEL(128, 3) syn_pulse_kernel(SynParams p) {
 
   // ---- aperiodic response (:36-69)
   if (noise_size > 0) {
-    const size_t d0 = Packed ? (size_t)s_off[u] + 8 * (size_t)u : (size_t)u * p.draw_stride;
-    const unsigned *draw = p.draws + d0 + p.draw_off[p0 + pi];
+    const unsigned *draw = p.draws + p.draw_off[p0 + pi];
     double s = 0.0;
     for (int i = tid; i < N + 2; i += nth) {
       const double v = (i < noise_size && i < N) ? randn_value(draw[i]) : 0.0;
@@ -731,25 +730,24 @@ SynthesisSizing::SynthesisSizing(const Ctx *ctx, const SynthesisPlan &p, int max
   budget = (double)ctx->scratch_budget - (double)tables;
   // Pulse arrays and responses are sized for 1200 pulses per second (f0 <= 1.2 kHz; the +64 covers the ends).
   nominal_cap = (int)((double)max_y / p.fs * 1200.0) + 64;
-  draw_stride = (size_t)max_y + 8;
+  max_draws = (size_t)max_y + 8;
 }
 
 // PassLayout's bytes per utterance, with the 256-byte alignment of its small arrays rounded up to 4096
 size_t SynthesisSizing::per_utt(int cap) const {
-  return (size_t)y_stride * 16 + (size_t)cap * (4 + 8 + 8) + (size_t)cap * fft_size * 8 + draw_stride * 4 + 4096 +
-         decoded_per_utt;
+  return (size_t)y_stride * 16 + (size_t)cap * (4 + 8 + 8) + (size_t)cap * fft_size * 8 + 4096 + decoded_per_utt;
 }
 
 int SynthesisSizing::fit(int cap) const { return (int)dmin(65535.0, budget / (double)per_utt(cap)); }
 
 int SynthesisSizing::cap_of(int y_len) const { return (int)((double)y_len / fs * 1200.0) + 64; }
 
-// PassLayout's bytes of one utterance in a packed pass: phase and vuv, its y_len + 8 draws, cap pulse slots (index,
-// shift, draw count and offset) with their responses, its decoded rows, and 128 bytes for its entries of the small
-// arrays (lengths, counts, offsets, factors, size lists)
+// PassLayout's bytes of one utterance in a packed pass: phase and vuv, cap pulse slots (index, shift, draw count and
+// offset) with their responses, its decoded rows, and 128 bytes for its entries of the small arrays (lengths, counts,
+// offsets, factors, size lists)
 size_t SynthesisSizing::packed_utt(int y_len, int f_len, int cap) const {
-  return (size_t)y_len * 16 + ((size_t)y_len + 8) * 4 + (size_t)cap * (4 + 8 + 8 + (size_t)fft_size * 8) +
-         (size_t)f_len * decoded_per_frame + 128;
+  return (size_t)y_len * 16 + (size_t)cap * (4 + 8 + 8 + (size_t)fft_size * 8) + (size_t)f_len * decoded_per_frame +
+         128;
 }
 
 // the 256-byte alignment of a packed pass's sub-blocks
@@ -758,19 +756,18 @@ size_t SynthesisSizing::packed_pass() const { return (size_t)64 * 256; }
 namespace {
 // The scratch block of one pass of n utterances with room for cap pulses each.  Per size g: its DC remover and (coded)
 // its decode tables.
-// A padded pass gives every utterance y_stride samples, cap pulse slots, f0_stride frames and draw_stride draws; a packed
-// pass gives each its own, back to back: the pass's totals are samples, pulses, frames and draws, and it also holds the
-// [n + 1] frame, sample, pulse and draw offsets and the [n + G] per-group prefixes of pulses and frames.
+// A padded pass gives every utterance y_stride samples, cap pulse slots and f0_stride frames; a packed pass gives each
+// its own, back to back: the pass's totals are samples, pulses and frames, and it also holds the [n + 1] frame, sample
+// and pulse offsets and the [n + G] per-group prefixes of pulses and frames.
 struct PassLayout {
-  size_t len, phase, vuv, pidx, psh, np, cnt, dcnt, doff, dtot, pl, draws, resp;
+  size_t len, phase, vuv, pidx, psh, np, cnt, dcnt, doff, dtot, pl, resp;
   std::vector<size_t> dcr, sidx, sfrac, sw, aidx, afrac;
   size_t dsp = 0, dap = 0;   // coded
   size_t mod = 0, f0m = 0, fp = 0, fft_u = 0, list = 0, total;
   size_t offs = 0, cums = 0;   // packed
-  PassLayout(const SynthesisPlan &p, int n, int cap, size_t draw_stride)
-      : PassLayout(p, n, (size_t)n * p.y_stride, (size_t)n * cap, (size_t)n * p.f0_stride, (size_t)n * draw_stride,
-                   false) {}
-  PassLayout(const SynthesisPlan &p, int n, size_t samples, size_t pulses, size_t frames, size_t n_draws, bool packed) {
+  PassLayout(const SynthesisPlan &p, int n, int cap)
+      : PassLayout(p, n, (size_t)n * p.y_stride, (size_t)n * cap, (size_t)n * p.f0_stride, false) {}
+  PassLayout(const SynthesisPlan &p, int n, size_t samples, size_t pulses, size_t frames, bool packed) {
     const size_t N = n, G = p.sizes.size();
     ArenaPlan a;
     len = a.add(2 * N * 4);                                          // f0 lengths, then y lengths
@@ -779,7 +776,6 @@ struct PassLayout {
     np = a.add(N * 4); cnt = a.add(N * 4);
     dcnt = a.add(pulses * 4); doff = a.add(pulses * 4);
     dtot = a.add(N * 4); pl = a.add(N * 4);
-    draws = a.add(n_draws * 4);
     resp = a.add(pulses * p.fft_size * 8);
     for (size_t g = 0; g < G; ++g) dcr.push_back(a.add((size_t)p.sizes[g] * 8));
     if (p.coded) {
@@ -797,7 +793,7 @@ struct PassLayout {
     }
     if (!p.fp.empty()) fp = a.add(N * 8);
     if (G > 1) { fft_u = a.add(N * 4); list = a.add(N * 4); }
-    if (packed) { offs = a.add(4 * (N + 1) * 8); cums = a.add(2 * (N + G) * 8); }
+    if (packed) { offs = a.add(3 * (N + 1) * 8); cums = a.add(2 * (N + G) * 8); }
     total = a.total;
   }
 };
@@ -836,10 +832,11 @@ int synthesis_run(Ctx *ctx, const SynthesisPlan &plan, int u0, int m, const Synt
   // pulses; an utterance with more pulses than that gets room for exactly its count, and the pass is cut short until it
   // fits again.
   const SynthesisSizing sz(ctx, plan, max_y);
+  const unsigned *table = rng_table_reserve(ctx, sz.max_draws);
+  if (!table) return WORLD_B200_ENOMEM;
   const ModifyPlan *mod = plan.coded && plan.modify ? &plan.mod : nullptr;
   const bool scale_f0 = mod && !mod->scale.empty(), stretch = mod && !mod->table.empty();
   const int nominal_cap = sz.nominal_cap;
-  const size_t draw_stride = sz.draw_stride;
   auto fit = [&](int cap) { return sz.fit(cap); };
   const int chunk = packed ? 0 : balanced_chunk(imin(m, 65535), fit(nominal_cap));
   // packed: caps[i] is the pulse room of the pass's utterance i; the longest prefix of [v0, v0 + k) that fits
@@ -869,23 +866,19 @@ int synthesis_run(Ctx *ctx, const SynthesisPlan &plan, int u0, int m, const Synt
   int v0 = 0, n = packed ? packed_pass(0) : imin(chunk, m), pulse_cap = nominal_cap;   // this pass: [u0 + v0, +n)
   bool relaid = false;
   while (v0 < m) {
-    // packed: the pass's offsets from its first utterance -- frames, samples, pulse slots, draws
-    std::vector<long long> offs(packed ? 4 * ((size_t)n + 1) : 0);
-    long long *foff = offs.data(), *soff = foff + n + 1, *poff = soff + n + 1, *doff = poff + n + 1;
-    size_t samples = 0, pulses = 0, frames = 0, n_draws = 0, max_draws = draw_stride;
+    // packed: the pass's offsets from its first utterance -- frames, samples, pulse slots
+    std::vector<long long> offs(packed ? 3 * ((size_t)n + 1) : 0);
+    long long *foff = offs.data(), *soff = foff + n + 1, *poff = soff + n + 1;
+    size_t samples = 0, pulses = 0, frames = 0;
     if (packed) {
-      max_draws = 0;
       for (int i = 0; i <= n; ++i) {
         foff[i] = (long long)(frame_at(v0 + i) - frame_at(v0));
         soff[i] = (long long)(sample_at(v0 + i) - sample_at(v0));
         poff[i] = i ? poff[i - 1] + caps[i - 1] : 0;
-        doff[i] = soff[i] + 8LL * i;
-        if (i < n) max_draws = std::max(max_draws, (size_t)y_len[v0 + i] + 8);
       }
-      samples = soff[n]; pulses = poff[n]; frames = foff[n]; n_draws = doff[n];
+      samples = soff[n]; pulses = poff[n]; frames = foff[n];
     }
-    const PassLayout l = packed ? PassLayout(plan, n, samples, pulses, frames, n_draws, true)
-                                : PassLayout(plan, n, pulse_cap, draw_stride);
+    const PassLayout l = packed ? PassLayout(plan, n, samples, pulses, frames, true) : PassLayout(plan, n, pulse_cap);
     unsigned char *blk = arena_block(ctx, l.total);
     if (!blk) return WORLD_B200_ENOMEM;
     std::vector<int> l2((size_t)2 * n), pl(n, pulse_cap);
@@ -937,7 +930,7 @@ int synthesis_run(Ctx *ctx, const SynthesisPlan &plan, int u0, int m, const Synt
     p.pulse_cap = pulse_cap; p.pulse_count = (int *)(blk + l.cnt);
     p.draw_cnt = (unsigned *)(blk + l.dcnt); p.draw_off = (unsigned *)(blk + l.doff);
     p.draw_tot = (unsigned *)(blk + l.dtot);
-    p.draws = (const unsigned *)(blk + l.draws); p.draw_stride = draw_stride;
+    p.draws = table;
     p.resp = (double *)(blk + l.resp); p.resp_n = plan.fft_size; p.dc_remover = (const double *)(blk + l.dcr[0]);
     p.y = plan.nbit ? nullptr : (double *)rows.y + sample_at(v0);
     p.y16 = plan.nbit ? (short *)rows.y + sample_at(v0) : nullptr;
@@ -1032,8 +1025,6 @@ int synthesis_run(Ctx *ctx, const SynthesisPlan &plan, int u0, int m, const Synt
       }
     }
     scan_counts(ctx, p.draw_cnt, (const int *)(blk + l.pl), pulse_cap, nullptr, p.draw_off, p.draw_tot, n, p.p_off);
-    rng_fill(ctx, p.draw_tot, (unsigned *)(blk + l.draws), draw_stride, max_draws, n, 0,
-             packed ? d_off + 3 * (n + 1) : nullptr);
     // one launch per size, each with its own shared memory (and so its own occupancy)
     for (int g = 0; g < n_sizes; ++g) {
       if (group_n(g) == 0) continue;
