@@ -705,6 +705,57 @@ int world_b200_modify_packed(WorldB200 *ctx, double *f0, int n_utts, const long 
                              int row_stride, const int *fft_sizes, int fs, const double *f0_scale,
                              const double *spectral_ratio);
 
+/* The stage calls on packed batches (DEVICE arrays), for callers who bring their own F0 or rows.  x_offsets and
+ * f_offsets are HOST arrays of n_utts + 1 offsets, each starting at 0: utterance u is samples
+ * [x_offsets[u], x_offsets[u + 1]) of x (1 .. INT_MAX of them) and frames [f_offsets[u], f_offsets[u + 1]) of time_axis,
+ * f0 and every output (0 .. INT_MAX of them).  f_offsets is the caller's: world_b200_packed_frames or
+ * world_b200_analyze_packed give one, but an F0 at another hop has its own frame counts.  Options and sizes are HOST
+ * arrays of n_utts and are required (a batch of one option repeats it); d4c_options may be NULL (InitializeD4COption).
+ * Full rows are [F][row_stride] (0: the largest fft_size / 2 + 1); coded rows [F][number_of_dimensions] and
+ * [F][GetNumberOfAperiodicities(fs)].  Every address is 64-bit.  The kernels read x, time_axis and f0 where they are:
+ * no padded copy is made.
+ * Equality: utterance u's output equals, bit for bit, what the padded call of the same family gives it with the same
+ * option and f0_lengths[u] = f_offsets[u + 1] - f_offsets[u]: world_b200_stonemask_batch,
+ * world_b200_cheaptrick_batch_options, world_b200_cheaptrick_coded_batch_options, world_b200_d4c_batch_options,
+ * world_b200_d4c_coded_batch_options, and the *_batch codec call at the utterance's fft_size.
+ * Nothing is written outside frames [0, F), nor past an utterance's fft_size / 2 + 1 in a full row.  Checked before any
+ * work is queued: the padded call's rules, offsets that start at 0 and never decrease, and a row_stride wide enough for
+ * every utterance's size; EINVAL, world_b200_last_error() naming the first bad utterance, outputs untouched.  n_utts == 0
+ * returns 0.  F0 alone on a packed batch is world_b200_analyze_packed / world_b200_analyze_coded_packed with NULL rows. */
+/* StoneMask: refined_f0 [F] (may alias f0). */
+int world_b200_stonemask_packed(WorldB200 *ctx, const double *x, int n_utts, const long long *x_offsets, int fs,
+                                const double *time_axis, const double *f0, const long long *f_offsets,
+                                double *refined_f0);
+int world_b200_cheaptrick_packed(WorldB200 *ctx, const double *x, int n_utts, const long long *x_offsets, int fs,
+                                 const double *time_axis, const double *f0, const long long *f_offsets,
+                                 const CheapTrickOption *cheaptrick_options, int row_stride, double *spectrogram);
+int world_b200_cheaptrick_coded_packed(WorldB200 *ctx, const double *x, int n_utts, const long long *x_offsets, int fs,
+                                       const double *time_axis, const double *f0, const long long *f_offsets,
+                                       const CheapTrickOption *cheaptrick_options, int number_of_dimensions,
+                                       double *coded_spectral_envelope);
+/* D4C at each utterance's CheapTrick size fft_sizes[u]. */
+int world_b200_d4c_packed(WorldB200 *ctx, const double *x, int n_utts, const long long *x_offsets, int fs,
+                          const double *time_axis, const double *f0, const long long *f_offsets, const int *fft_sizes,
+                          const D4COption *d4c_options, int row_stride, double *aperiodicity);
+/* Below 12 kHz there are no bands: nothing is written, and coded_aperiodicity may be NULL. */
+int world_b200_d4c_coded_packed(WorldB200 *ctx, const double *x, int n_utts, const long long *x_offsets, int fs,
+                                const double *time_axis, const double *f0, const long long *f_offsets,
+                                const int *fft_sizes, const D4COption *d4c_options, double *coded_aperiodicity);
+/* The codec between full rows [F][row_stride] and coded rows, each utterance at its own fft_sizes[u].  Below 12 kHz the
+ * coded aperiodicity is empty (may be NULL): coding it writes nothing, decoding it writes the unvoiced rows. */
+int world_b200_code_spectral_envelope_packed(WorldB200 *ctx, const double *spectrogram, int n_utts,
+                                             const long long *f_offsets, int row_stride, const int *fft_sizes, int fs,
+                                             int number_of_dimensions, double *coded_spectral_envelope);
+int world_b200_decode_spectral_envelope_packed(WorldB200 *ctx, const double *coded_spectral_envelope, int n_utts,
+                                               const long long *f_offsets, int row_stride, const int *fft_sizes,
+                                               int fs, int number_of_dimensions, double *spectrogram);
+int world_b200_code_aperiodicity_packed(WorldB200 *ctx, const double *aperiodicity, int n_utts,
+                                        const long long *f_offsets, int row_stride, const int *fft_sizes, int fs,
+                                        double *coded_aperiodicity);
+int world_b200_decode_aperiodicity_packed(WorldB200 *ctx, const double *coded_aperiodicity, int n_utts,
+                                          const long long *f_offsets, int row_stride, const int *fft_sizes, int fs,
+                                          double *aperiodicity);
+
 /* ---- voice transformation, PCM in and PCM out: the reference demo's loop (test/test.cpp: Harvest or DIO + StoneMask,
  * CheapTrick, D4C, ParameterModification, Synthesis) over a batch in one call, with one pitch, formant and tempo
  * factor per utterance ----------------------------------------------------------------------------------------------

@@ -267,6 +267,19 @@ ABI = {
                                                    C.POINTER(HarvestOption), C.POINTER(DioOption),
                                                    C.POINTER(CheapTrickOption), C.POINTER(D4COption), _P, _P, _P,
                                                    C.c_int, _P, _LP]),
+    "world_b200_stonemask_packed": (C.c_int, [_P, _P, C.c_int, _LP, C.c_int, _P, _P, _LP, _P]),
+    "world_b200_cheaptrick_packed": (C.c_int, [_P, _P, C.c_int, _LP, C.c_int, _P, _P, _LP, C.POINTER(CheapTrickOption),
+                                               C.c_int, _P]),
+    "world_b200_cheaptrick_coded_packed": (C.c_int, [_P, _P, C.c_int, _LP, C.c_int, _P, _P, _LP,
+                                                     C.POINTER(CheapTrickOption), C.c_int, _P]),
+    "world_b200_d4c_packed": (C.c_int, [_P, _P, C.c_int, _LP, C.c_int, _P, _P, _LP, _IP, C.POINTER(D4COption), C.c_int,
+                                        _P]),
+    "world_b200_d4c_coded_packed": (C.c_int, [_P, _P, C.c_int, _LP, C.c_int, _P, _P, _LP, _IP, C.POINTER(D4COption),
+                                              _P]),
+    "world_b200_code_spectral_envelope_packed": (C.c_int, [_P, _P, C.c_int, _LP, C.c_int, _IP, C.c_int, C.c_int, _P]),
+    "world_b200_decode_spectral_envelope_packed": (C.c_int, [_P, _P, C.c_int, _LP, C.c_int, _IP, C.c_int, C.c_int, _P]),
+    "world_b200_code_aperiodicity_packed": (C.c_int, [_P, _P, C.c_int, _LP, C.c_int, _IP, C.c_int, _P]),
+    "world_b200_decode_aperiodicity_packed": (C.c_int, [_P, _P, C.c_int, _LP, C.c_int, _IP, C.c_int, _P]),
     # host-only file glue (tools/audioio.h, tools/parameterio.h)
     "wavwrite": (None, [_P, C.c_int, C.c_int, C.c_int, C.c_char_p]),
     "GetAudioLength": (C.c_int, [C.c_char_p]),
@@ -1063,6 +1076,135 @@ class World:
             self._h, _ptr(f0), n, fo, _ptr(spectrogram), row, sizes, fs, _factors(f0_scale, n, "f0_scale"),
             _factors(spectral_ratio, n, "spectral_ratio")))
         return f0, spectrogram
+
+    # -- the stage calls on packed batches: utterance u = samples [x_offsets[u], x_offsets[u + 1]) of x and frames
+    #    [f_offsets[u], f_offsets[u + 1]) of time_axis, f0 and the rows ------------------------------------------------
+    def _stage_packed(self, entry, x, x_offsets, fs, time_axis, f0, f_offsets, options, out):
+        """Calls world_b200_<entry> on packed DEVICE arrays with options (the arguments between f_offsets and the
+        output) into out, enqueued on the current stream; returns out."""
+        n, xo = _offsets(x_offsets)
+        nf, fo = _offsets(f_offsets)
+        if nf != n:
+            raise ValueError(f"{n + 1} x_offsets but {nf + 1} f_offsets")
+        self._use_current_stream()
+        self._check(getattr(self.lib, f"world_b200_{entry}")(self._h, _ptr(x), n, xo, fs, _ptr(time_axis), _ptr(f0),
+                                                             fo, *options, _ptr(out)))
+        return out
+
+    def _packed_options(self, cls, option, n, default):
+        """One option (None: default()) for every utterance, or a list of n -> a ctypes array of n."""
+        if option is None or isinstance(option, cls):
+            option = [option or default()] * n
+        return _option_array(cls, option, n)
+
+    def _packed_sizes(self, fft_size, n):
+        sizes = _fft_sizes(fft_size, n)
+        return sizes if sizes is not None else (C.c_int * max(n, 1))(*([int(fft_size)] * n))
+
+    def _packed_rows(self, like, f_offsets, width, out):
+        """out, or zeros [F, width] with F = f_offsets[-1]."""
+        if out is not None:
+            return out
+        n, fo = _offsets(f_offsets)
+        return self._zeros(like, (int(fo[n]), width))
+
+    def stonemask_packed(self, x, x_offsets, fs, time_axis, f0, f_offsets, out=None):
+        """stonemask on a PACKED batch of DEVICE arrays (world_b200_stonemask_packed): x holds the utterances back to
+        back (x_offsets: n + 1 sample offsets), time_axis / f0 their frames back to back (f_offsets: n + 1 frame
+        offsets, the caller's own or analyze_packed's).  Offsets may be a list, numpy array or CPU tensor.  Returns the
+        refined f0 [F] (out, which may be f0 itself).  Each utterance's values equal stonemask()'s bit for bit."""
+        if out is None:
+            out = self._zeros(f0, tuple(f0.shape))
+        return self._stage_packed("stonemask_packed", x, x_offsets, fs, time_axis, f0, f_offsets, (), out)
+
+    def _cheaptrick_packed(self, coded, x, x_offsets, fs, time_axis, f0, f_offsets, option, width, out):
+        n = len(x_offsets) - 1
+        opts = self._packed_options(CheapTrickOption, option, n, lambda: self.cheaptrick_option(fs))
+        if out is None:
+            if not coded:
+                width = width or max([o.fft_size for o in opts] or [0]) // 2 + 1
+            out = self._packed_rows(f0, f_offsets, width, None)
+        elif not coded:
+            width = int(out.shape[-1])
+        entry = "cheaptrick_coded_packed" if coded else "cheaptrick_packed"
+        return self._stage_packed(entry, x, x_offsets, fs, time_axis, f0, f_offsets, (opts, width), out)
+
+    def cheaptrick_packed(self, x, x_offsets, fs, time_axis, f0, f_offsets, option=None, row_stride=0, out=None):
+        """cheaptrick on a PACKED batch (world_b200_cheaptrick_packed), arrays and offsets as stonemask_packed.
+        option: one CheapTrickOption for every utterance (None: the default at fs) or a list of one per utterance.
+        Returns the spectrogram [F, W]: W = out's last dimension, or row_stride, or the largest fft_size // 2 + 1.
+        Utterance u writes the first fft_size[u] // 2 + 1 values of each of its rows, equal to cheaptrick()'s."""
+        return self._cheaptrick_packed(False, x, x_offsets, fs, time_axis, f0, f_offsets, option, row_stride, out)
+
+    def cheaptrick_coded_packed(self, x, x_offsets, fs, time_axis, f0, f_offsets, number_of_dimensions, option=None,
+                                out=None):
+        """cheaptrick_coded on a PACKED batch (world_b200_cheaptrick_coded_packed) -> [F, number_of_dimensions]."""
+        return self._cheaptrick_packed(True, x, x_offsets, fs, time_axis, f0, f_offsets, option,
+                                       number_of_dimensions, out)
+
+    def _d4c_packed(self, coded, x, x_offsets, fs, time_axis, f0, f_offsets, fft_size, option, row_stride, out):
+        n = len(x_offsets) - 1
+        sizes = self._packed_sizes(fft_size, n)
+        opts = None if option is None else self._packed_options(D4COption, option, n, self.d4c_option)
+        if coded:
+            out = self._packed_rows(f0, f_offsets, max(1, self.number_of_aperiodicities(fs)), out)
+            options = (sizes, opts)
+        else:
+            out = self._packed_rows(f0, f_offsets, row_stride or max(list(sizes)[:n] or [0]) // 2 + 1, out)
+            options = (sizes, opts, int(out.shape[-1]))
+        entry = "d4c_coded_packed" if coded else "d4c_packed"
+        return self._stage_packed(entry, x, x_offsets, fs, time_axis, f0, f_offsets, options, out)
+
+    def d4c_packed(self, x, x_offsets, fs, time_axis, f0, f_offsets, fft_size, option=None, row_stride=0, out=None):
+        """d4c on a PACKED batch (world_b200_d4c_packed), arrays and offsets as stonemask_packed.  fft_size: one int
+        or one per utterance (its CheapTrick size); option: one D4COption, a list of one per utterance, or None
+        (InitializeD4COption).  Returns the aperiodicity [F, W], W as in cheaptrick_packed."""
+        return self._d4c_packed(False, x, x_offsets, fs, time_axis, f0, f_offsets, fft_size, option, row_stride, out)
+
+    def d4c_coded_packed(self, x, x_offsets, fs, time_axis, f0, f_offsets, fft_size, option=None, out=None):
+        """d4c_coded on a PACKED batch (world_b200_d4c_coded_packed) -> [F, max(1, GetNumberOfAperiodicities(fs))]
+        (nothing is written below 12 kHz)."""
+        return self._d4c_packed(True, x, x_offsets, fs, time_axis, f0, f_offsets, fft_size, option, 0, out)
+
+    def _codec_packed(self, entry, src, f_offsets, full_rows, fs, fft_size, dims, width, out):
+        """world_b200_<entry> between full rows [F, W] and coded rows [F, dims]; full_rows: the full-row array (the
+        input when coding, the output when decoding), whose last dimension is the row_stride."""
+        n, fo = _offsets(f_offsets)
+        sizes = self._packed_sizes(fft_size, n)
+        if out is None:
+            out = self._packed_rows(src, f_offsets, width, None)
+        row = int((src if full_rows == "in" else out).shape[-1])
+        args = [self._h, _ptr(src), n, fo, row, sizes, fs] + ([] if dims is None else [dims])
+        self._use_current_stream()
+        self._check(getattr(self.lib, f"world_b200_{entry}")(*args, _ptr(out)))
+        return out
+
+    def code_spectral_envelope_packed(self, spectrogram, f_offsets, fs, fft_size, number_of_dimensions, out=None):
+        """code_spectral_envelope on PACKED rows (world_b200_code_spectral_envelope_packed): spectrogram [F, W] (W >=
+        every fft_size // 2 + 1), utterance u being frames [f_offsets[u], f_offsets[u + 1]) at fft_size (one int or
+        one per utterance) -> [F, number_of_dimensions]."""
+        return self._codec_packed("code_spectral_envelope_packed", spectrogram, f_offsets, "in", fs, fft_size,
+                                  number_of_dimensions, number_of_dimensions, out)
+
+    def decode_spectral_envelope_packed(self, coded, f_offsets, fs, fft_size, number_of_dimensions, row_stride=0,
+                                        out=None):
+        """decode_spectral_envelope on PACKED rows -> [F, W] (W: out's last dimension, or row_stride, or the largest
+        fft_size // 2 + 1); utterance u writes the first fft_size[u] // 2 + 1 values of each row."""
+        n = len(f_offsets) - 1
+        W = row_stride or max(list(self._packed_sizes(fft_size, n))[:n] or [0]) // 2 + 1
+        return self._codec_packed("decode_spectral_envelope_packed", coded, f_offsets, "out", fs, fft_size,
+                                  number_of_dimensions, W, out)
+
+    def code_aperiodicity_packed(self, aperiodicity, f_offsets, fs, fft_size, out=None):
+        """code_aperiodicity on PACKED rows -> [F, max(1, GetNumberOfAperiodicities(fs))]."""
+        return self._codec_packed("code_aperiodicity_packed", aperiodicity, f_offsets, "in", fs, fft_size, None,
+                                  max(1, self.number_of_aperiodicities(fs)), out)
+
+    def decode_aperiodicity_packed(self, coded, f_offsets, fs, fft_size, row_stride=0, out=None):
+        """decode_aperiodicity on PACKED rows -> [F, W], W as in decode_spectral_envelope_packed."""
+        n = len(f_offsets) - 1
+        W = row_stride or max(list(self._packed_sizes(fft_size, n))[:n] or [0]) // 2 + 1
+        return self._codec_packed("decode_aperiodicity_packed", coded, f_offsets, "out", fs, fft_size, None, W, out)
 
     # -- multi-GPU: one World per GPU / process; the NCCL id travels by the caller's own means -------------------
     def comm_unique_id(self) -> bytes:

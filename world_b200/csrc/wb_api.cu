@@ -265,19 +265,28 @@ int ctx_init_tables(Ctx *ctx) {
 using namespace wb;
 
 // ------------------------------------------------------------------------------------------
-// The Batch of n utterances' rows, with their lengths x_len / f_len [n] (checked by the caller) uploaded.
+// The Batch of n utterances' rows, with their lengths x_len / f_len [n] (checked by the caller) uploaded.  offs (packed
+// inputs): the host offsets x_off [n] and f_off [n + 1], uploaded after the lengths for b->x_off / b->f_off.
 static int load_batch(WorldB200 *h, const double *x, int n, int x_stride, const int *x_len, int fs,
-                      const double *time_axis, const double *f0, const int *f_len, int f_stride, Batch *b) {
+                      const double *time_axis, const double *f0, const int *f_len, int f_stride, Batch *b,
+                      const std::vector<long long> *offs = nullptr) {
   Ctx *ctx = &h->c;
   b->x = x; b->n = n; b->x_stride = x_stride; b->fs = fs; b->time_axis = time_axis; b->f0 = f0; b->f_stride = f_stride;
-  if ((size_t)2 * n > h->lens_cap) {
+  // the offsets follow the 2n lengths, at an 8-byte boundary
+  const size_t ints = (size_t)2 * n + (offs ? 2 * offs->size() : 0);
+  if (ints > h->lens_cap) {
     dev_sync(ctx);
     dev_free(h->lens_dev);
-    h->lens_cap = (size_t)2 * n + 64;
+    h->lens_cap = ints + 64;
     h->lens_dev = (int *)dev_malloc(ctx, h->lens_cap * sizeof(int));
     if (!h->lens_dev) { h->lens_cap = 0; return WORLD_B200_ENOMEM; }
   }
-  std::vector<int> tmp((size_t)2 * n);
+  std::vector<int> tmp(ints);
+  if (offs) {
+    memcpy(tmp.data() + 2 * n, offs->data(), offs->size() * 8);
+    b->x_off = (const long long *)(h->lens_dev + 2 * n);
+    b->f_off = b->x_off + n;
+  }
   int mx = 0, mf = 0;
   for (int i = 0; i < n; ++i) {
     tmp[i] = x_len[i]; tmp[n + i] = f_len[i];
@@ -444,6 +453,34 @@ unsigned long long world_b200_launch_count(const WorldB200 *) { return wb::g_lau
 
 }  // extern "C"
 
+namespace wb {
+std::string packed_lengths(const char *name, const char *unit, int n, const long long *off, int least,
+                           std::vector<int> *len) {
+  if (!off) return std::string(name) + " must be given";
+  if (off[0] != 0) return std::string(name) + "[0] = " + std::to_string(off[0]) + " is not 0";
+  len->resize(n);
+  for (int u = 0; u < n; ++u) {
+    const long long l = off[u + 1] - off[u];
+    if (l < least || l > INT_MAX)
+      return std::string(name) + " must increase by " + std::to_string(least) + " to INT_MAX " + unit +
+             " per utterance, not " + std::to_string(l) + " (utterance " + std::to_string(u) + ")";
+    (*len)[u] = (int)l;
+  }
+  return "";
+}
+}  // namespace wb
+
+// The packed layout's offsets: x_offsets[0] == 0 and every utterance 1 .. INT_MAX samples long.  Fills x_len [n] and
+// f_off [n + 1] (frames at frame_period ms); "" when the offsets are good, else the first broken rule.
+static std::string packed_layout(int fs, int n, const long long *x_offsets, double frame_period, std::vector<int> *x_len,
+                                 std::vector<long long> *f_off) {
+  const std::string bad = packed_lengths("x_offsets", "samples", n, x_offsets, 1, x_len);
+  if (!bad.empty()) return bad;
+  f_off->assign(1, 0);
+  for (int u = 0; u < n; ++u) f_off->push_back(f_off->back() + frames_for(fs, (*x_len)[u], frame_period));
+  return "";
+}
+
 // ---- the CheapTrick, D4C and StoneMask stage calls: one plan, then load_batch and the stage's run
 // EINVAL with last_error "<stage>: <what>", and " (utterance u)" for u >= 0
 static const char *stage_name(StageKind stage) {
@@ -483,6 +520,7 @@ int stage_plan(Ctx *c, const StageRequest &r, StagePlan *p) {
       if (!std::isfinite(p->q[u])) return fail(ct ? "q1 must be finite" : "threshold must be finite", named);
     }
     p->row = r.row_stride || r.per_utt || n == 0 ? r.row_stride : p->fft_size[0] / 2 + 1;
+    for (int u = 0; u < n && r.x_offsets && !r.row_stride; ++u) p->row = imax(p->row, p->fft_size[u] / 2 + 1);
     for (int u = 0; u < n && !r.coded; ++u)
       if (p->row < p->fft_size[u] / 2 + 1)
         return fail("row_stride is smaller than fft_size / 2 + 1", r.per_utt ? u : -1);
@@ -500,6 +538,14 @@ int stage_plan(Ctx *c, const StageRequest &r, StagePlan *p) {
       if (rc) return fail(c->last_error, r.per_utt ? u : -1);
     }
     p->nothing = r.coded && !ct && GetNumberOfAperiodicities(r.fs) == 0;
+  }
+  if (r.x_offsets || r.f_offsets) {
+    std::string bad = packed_lengths("x_offsets", "samples", n, r.x_offsets, 1, &p->x_len);
+    if (bad.empty()) bad = packed_lengths("f_offsets", "frames", n, r.f_offsets, 0, &p->f_len);
+    if (!bad.empty()) return fail(bad);
+    p->x_off.assign(r.x_offsets, r.x_offsets + n + 1);
+    p->f_off.assign(r.f_offsets, r.f_offsets + n + 1);
+    return 0;
   }
   const char *who = stage_name(r.stage);
   int rc = row_lengths(c, who, "x", r.x_lengths, n, r.x_stride, 1, &p->x_len);
@@ -609,24 +655,115 @@ int world_b200_stonemask_batch(WorldB200 *h, const double *x, int n, int x_strid
 
 }  // extern "C"
 
-// The packed layout's offsets: x_offsets[0] == 0 and every utterance 1 .. INT_MAX samples long.  Fills x_len [n] and
-// f_off [n + 1] (frames at frame_period ms); "" when the offsets are good, else the first broken rule.
-static std::string packed_layout(int fs, int n, const long long *x_offsets, double frame_period, std::vector<int> *x_len,
-                                 std::vector<long long> *f_off) {
-  if (!x_offsets) return "x_offsets must be given";
-  if (x_offsets[0] != 0) return "x_offsets[0] must be 0";
-  x_len->resize(n);
-  f_off->assign(1, 0);
-  for (int u = 0; u < n; ++u) {
-    const long long len = x_offsets[u + 1] - x_offsets[u];
-    if (len < 1 || len > INT_MAX)
-      return "x_offsets must increase by 1 to INT_MAX samples per utterance, not " + std::to_string(len) +
-             " (utterance " + std::to_string(u) + ")";
-    (*x_len)[u] = (int)len;
-    f_off->push_back(f_off->back() + frames_for(fs, (int)len, frame_period));
+// A packed stage call: x [X], time_axis / f0 [F] and out [F][the planned row] read and written where they are.  The
+// utterances run in chunks of consecutive utterances whose per-frame scratch fits the budget (and of at most 65535, the
+// frame kernels' grid), each loaded with offsets relative to its first sample and frame.
+static int stage_packed(WorldB200 *h, StageRequest r, const long long *x_offsets, const long long *f_offsets,
+                        const double *x, const double *time_axis, const double *f0, double *out) {
+  if (!h) return WORLD_B200_EINVAL;
+  DeviceGuard guard_(&h->c);
+  Ctx *c = &h->c;
+  r.per_utt = true; r.x_offsets = x_offsets; r.f_offsets = f_offsets;
+  StagePlan p;
+  int rc = stage_plan(c, r, &p);
+  if (rc) return rc;
+  // empty arrays may be NULL: a batch without utterances or frames reads and writes nothing
+  const bool frames = r.n > 0 && p.f_off[r.n] > 0;
+  if ((r.n > 0 && !x) || (frames && (!time_axis || !f0)))
+    return stage_fail(c, r.stage, "x, time_axis and f0 must be given");
+  if (p.nothing) return 0;   // nothing to write below 12 kHz, like the reference's empty loops
+  if (!out && frames) return stage_fail(c, r.stage, "the output rows must be given");
+  const size_t row = r.stage == STAGE_STONEMASK                     ? 1
+                     : !r.coded                                     ? (size_t)p.row
+                     : r.stage == STAGE_CHEAPTRICK                  ? (size_t)r.dims
+                                                                    : (size_t)GetNumberOfAperiodicities(r.fs);
+  const long long *xo = p.x_off.data(), *fo = p.f_off.data();
+  std::vector<long long> offs;
+  for (int a = 0; a < r.n && !rc;) {
+    int e = a, most_x = 1, most_f = 1;
+    size_t bytes = 0;
+    while (e < r.n && e - a < 65535) {
+      const size_t more = WB_STAGE_UTT_BYTES + (size_t)p.f_len[e] * WB_STAGE_FRAME_BYTES;
+      if (e > a && (WB_STAGE_CHUNK_BYTES + bytes + more > c->scratch_budget || fo[e + 1] - fo[a] > INT_MAX)) break;
+      bytes += more;
+      most_x = imax(most_x, p.x_len[e]);
+      most_f = imax(most_f, p.f_len[e]);
+      ++e;
+    }
+    const int m = e - a;
+    offs.clear();
+    for (int k = 0; k < m; ++k) offs.push_back(xo[a + k] - xo[a]);
+    for (int k = 0; k <= m; ++k) offs.push_back(fo[a + k] - fo[a]);
+    Batch b;
+    rc = load_batch(h, x + xo[a], m, most_x, p.x_len.data() + a, r.fs, time_axis + fo[a], f0 + fo[a],
+                    p.f_len.data() + a, most_f, &b, &offs);
+    if (rc) break;
+    b.f_off_host = offs.data() + m;
+    double *o = out + (size_t)fo[a] * row;
+    rc = r.stage == STAGE_CHEAPTRICK ? cheaptrick_run(c, p, b, a, o)
+         : r.stage == STAGE_D4C     ? d4c_run(c, p, b, a, o)
+                                    : stonemask_run(c, b, o);
+    a = e;
   }
-  return "";
+  return rc;
 }
+
+extern "C" {
+
+int world_b200_stonemask_packed(WorldB200 *h, const double *x, int n, const long long *x_offsets, int fs,
+                                const double *time_axis, const double *f0, const long long *f_offsets,
+                                double *refined_f0) {
+  return stage_packed(h, {STAGE_STONEMASK, n, 0, nullptr, fs, nullptr, 0}, x_offsets, f_offsets, x, time_axis, f0,
+                      refined_f0);
+}
+
+int world_b200_cheaptrick_packed(WorldB200 *h, const double *x, int n, const long long *x_offsets, int fs,
+                                 const double *time_axis, const double *f0, const long long *f_offsets,
+                                 const CheapTrickOption *cheaptrick_options, int row_stride, double *spectrogram) {
+  StageRequest r{STAGE_CHEAPTRICK, n, 0, nullptr, fs, nullptr, 0};
+  r.ct = cheaptrick_options; r.row_stride = row_stride;
+  return stage_packed(h, r, x_offsets, f_offsets, x, time_axis, f0, spectrogram);
+}
+
+int world_b200_cheaptrick_coded_packed(WorldB200 *h, const double *x, int n, const long long *x_offsets, int fs,
+                                       const double *time_axis, const double *f0, const long long *f_offsets,
+                                       const CheapTrickOption *cheaptrick_options, int number_of_dimensions,
+                                       double *coded_spectral_envelope) {
+  StageRequest r{STAGE_CHEAPTRICK, n, 0, nullptr, fs, nullptr, 0};
+  r.ct = cheaptrick_options; r.coded = true; r.dims = number_of_dimensions;
+  return stage_packed(h, r, x_offsets, f_offsets, x, time_axis, f0, coded_spectral_envelope);
+}
+
+// d4c_options NULL: InitializeD4COption for every utterance
+static int d4c_packed(WorldB200 *h, const double *x, int n, const long long *x_offsets, int fs, const double *time_axis,
+                      const double *f0, const long long *f_offsets, const int *fft_sizes, const D4COption *d4c_options,
+                      bool coded, int row_stride, double *out) {
+  StageRequest r{STAGE_D4C, n, 0, nullptr, fs, nullptr, 0};
+  std::vector<D4COption> defaults;
+  if (!d4c_options && n > 0) {
+    defaults.resize(n);
+    for (D4COption &o : defaults) InitializeD4COption(&o);
+    d4c_options = defaults.data();
+  }
+  r.fft_size = fft_sizes; r.d4c = d4c_options; r.coded = coded; r.row_stride = row_stride;
+  return stage_packed(h, r, x_offsets, f_offsets, x, time_axis, f0, out);
+}
+
+int world_b200_d4c_packed(WorldB200 *h, const double *x, int n, const long long *x_offsets, int fs,
+                          const double *time_axis, const double *f0, const long long *f_offsets, const int *fft_sizes,
+                          const D4COption *d4c_options, int row_stride, double *aperiodicity) {
+  return d4c_packed(h, x, n, x_offsets, fs, time_axis, f0, f_offsets, fft_sizes, d4c_options, false, row_stride,
+                    aperiodicity);
+}
+
+int world_b200_d4c_coded_packed(WorldB200 *h, const double *x, int n, const long long *x_offsets, int fs,
+                                const double *time_axis, const double *f0, const long long *f_offsets,
+                                const int *fft_sizes, const D4COption *d4c_options, double *coded_aperiodicity) {
+  return d4c_packed(h, x, n, x_offsets, fs, time_axis, f0, f_offsets, fft_sizes, d4c_options, true, 0,
+                    coded_aperiodicity);
+}
+
+}  // extern "C"
 
 namespace wb {
 // chain_plan without the caller's prefix on last_error

@@ -27,6 +27,11 @@ struct CtParams {
   int out_stride;         // doubles per spectrogram row (fft/2+1 unless the caller pads its rows)
   const int *uid;         // [n] batch index of the launch's utterance blockIdx.y; null: blockIdx.y itself
   const long long *f_off; // [n] packed rows: output frame of each utterance's frame 0; null: u * f_stride
+  // packed inputs: utterance u's samples at x + x_off[u], its frames (time_axis, f0 and output) at f_off[u] + i, and
+  // the launch's utterance ul's draw offsets at cum[ul] + i (cum: [n + 1] frames of the launch's utterances before
+  // it); null: padded inputs
+  const long long *x_off, *cum;
+  int n_launch;           // packed: utterances of the launch (entries of cum)
   const double2 *tw;
   int *status;
   // coded tail (ct_coded_kernel): mel interpolation + DCT of the log envelope, CodeSpectralEnvelope (codec.cpp:279-295)
@@ -55,6 +60,19 @@ WB_KERNEL_PLAIN ct_count_kernel(const double *__restrict__ f0, const int *__rest
   counts[g] = c;
 }
 
+// the same over packed inputs: one thread per frame of the launch's utterances, frame g of utterance ul at cum[ul] + i
+WB_KERNEL_PLAIN ct_count_packed_kernel(const double *__restrict__ f0, const long long *__restrict__ f_off,
+                                       const long long *__restrict__ cum, int n_utts, int fs, int fft_size,
+                                       double f0_floor, const int *__restrict__ uid, unsigned *__restrict__ counts) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= cum[n_utts]) return;
+  const int ul = packed_find(cum, n_utts, g);
+  const int u = uid ? uid[ul] : ul;
+  const double f = ct_effective_f0(f0[f_off[u] + (g - cum[ul])], f0_floor);
+  const int h = round_half_away(1.5 * fs / f);
+  counts[g] = (unsigned)(2 * h + 1) + (unsigned)(fft_size / 2 + 1);
+}
+
 // Shared memory: two padded complex buffers of fft_size/2 slots (the FFT ping-pongs between them, wb_fft.cuh)
 // + the reduction scratch.  Between transforms the buffer that does not hold FFT input serves as the plain
 // double array of the phase (window, power spectrum, smoothing scratch), so nothing else is needed.
@@ -62,27 +80,38 @@ WB_HD inline size_t ct_smem_bytes(int fft_size) {
   return (size_t)2 * WB_FPAD_SLOTS(fft_size / 2) * sizeof(double2) + WB_RED_DOUBLES * sizeof(double);
 }
 
-template <bool kCoded>
+// kPacked: packed inputs (p.x_off, p.cum), a compile-time choice so that the padded kernels keep their own code
+template <bool kCoded, bool kPacked>
 WB_DEV void ct_frame_body(const CtParams &p) {
   WB_DYN_SMEM(double2, smem2);
   const int tid = WB_TID, nth = WB_NTH;
-  const int ul = blockIdx.y, i = blockIdx.x;   // f_len and draw offsets follow the launch's order
-  if (i >= p.f_len[ul]) return;
+  // f_len and draw offsets follow the launch's order.  Packed: the grid runs over the launch's packed frames (none of it
+  // idles on short utterances), blockIdx.x being frame i of launch entry ul, its draw offsets' index
+  int ul, i;
+  if (kPacked) {
+    ul = packed_find(p.cum, p.n_launch, (long long)blockIdx.x);
+    i = (int)((long long)blockIdx.x - p.cum[ul]);
+  } else {
+    ul = blockIdx.y;
+    i = blockIdx.x;
+    if (i >= p.f_len[ul]) return;
+  }
   const int u = p.uid ? __ldg(p.uid + ul) : ul;
   const int N = p.fft_size, half = N / 2;
   const int slots = WB_FPAD_SLOTS(half);
   double2 *A = smem2, *B = smem2 + slots;
   double *red = reinterpret_cast<double *>(B + slots);   // WB_RED_DOUBLES
 
-  const size_t fidx = (size_t)u * p.f_stride + i;
-  // the output row: only the address differs between the padded and the packed layout
+  // only the addresses differ between the padded and the packed layouts: the output row, and with packed inputs the
+  // input frame, the samples and the draw offset
+  const size_t fidx = kPacked ? (size_t)(p.f_off[u] + i) : (size_t)u * p.f_stride + i;
   const size_t oidx = p.f_off ? (size_t)(p.f_off[u] + i) : fidx;
   const double f = ct_effective_f0(p.f0[fidx], p.f0_floor);
   const double t = p.time_axis[fidx];
   const int fs = p.fs;
   const int x_len = p.x_len[u];
-  const double *x = p.x + (size_t)u * p.x_stride;
-  const unsigned *draw = p.draws + p.draw_off[(size_t)ul * p.f_stride + i];
+  const double *x = kPacked ? p.x + p.x_off[u] : p.x + (size_t)u * p.x_stride;
+  const unsigned *draw = p.draws + p.draw_off[kPacked ? (size_t)blockIdx.x : (size_t)ul * p.f_stride + i];
 
   const int h = round_half_away(1.5 * fs / f);
   const int nwin = 2 * h + 1;
@@ -223,11 +252,15 @@ WB_DEV void ct_frame_body(const CtParams &p) {
 }
 
 #ifndef WB_EMU
-__global__ void __launch_bounds__(128, 8) ct_frame_kernel(CtParams p) { ct_frame_body<false>(p); }
-__global__ void __launch_bounds__(128, 8) ct_coded_kernel(CtParams p) { ct_frame_body<true>(p); }
+__global__ void __launch_bounds__(128, 8) ct_frame_kernel(CtParams p) { ct_frame_body<false, false>(p); }
+__global__ void __launch_bounds__(128, 8) ct_coded_kernel(CtParams p) { ct_frame_body<true, false>(p); }
+__global__ void __launch_bounds__(128, 8) ct_frame_packed_kernel(CtParams p) { ct_frame_body<false, true>(p); }
+__global__ void __launch_bounds__(128, 8) ct_coded_packed_kernel(CtParams p) { ct_frame_body<true, true>(p); }
 #else
-void ct_frame_kernel(CtParams p) { ct_frame_body<false>(p); }
-void ct_coded_kernel(CtParams p) { ct_frame_body<true>(p); }
+void ct_frame_kernel(CtParams p) { ct_frame_body<false, false>(p); }
+void ct_coded_kernel(CtParams p) { ct_frame_body<true, false>(p); }
+void ct_frame_packed_kernel(CtParams p) { ct_frame_body<false, true>(p); }
+void ct_coded_packed_kernel(CtParams p) { ct_frame_body<true, true>(p); }
 #endif
 
 namespace {
@@ -254,23 +287,41 @@ static int ct_launch(Ctx *ctx, const Batch &b, double q1, int fft_size, double *
   const size_t max_per_frame = (size_t)fft_size + bins;
   const unsigned *table = rng_table_reserve(ctx, max_per_frame * (size_t)max_f_len);
   if (!table) return 2;
-  // utterances per chunk so that the draw counts and offsets fit the budget
+  // utterances per chunk so that the draw counts and offsets fit the budget (packed inputs: one pass, the packed stage
+  // call cut its chunks by frames)
   const size_t per_utt_bytes = (size_t)b.f_stride * 8 + 64;
-  int chunk = balanced_chunk(imin(n_all, 65535), (int)dmin(65535.0, (double)ctx->scratch_budget / (double)per_utt_bytes));
+  int chunk = b.x_off ? n_all
+                      : balanced_chunk(imin(n_all, 65535), (int)dmin(65535.0, (double)ctx->scratch_budget / (double)per_utt_bytes));
+  // packed inputs: the launch's frames back to back in launch order, cum[k] before utterance k (the group's order)
+  std::vector<long long> cum;
+  if (b.x_off) {
+    cum.assign(1, 0);
+    for (int k = 0; k < n_all; ++k) {
+      const int u = group ? group->uid[k] : k;
+      cum.push_back(cum.back() + (b.f_off_host[u + 1] - b.f_off_host[u]));
+    }
+  }
   const size_t smem = ct_smem_bytes(fft_size);
 #ifndef WB_EMU
   cudaFuncSetAttribute(ct_frame_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   cudaFuncSetAttribute(ct_coded_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (b.x_off) {
+    cudaFuncSetAttribute(ct_frame_packed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(ct_coded_packed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  }
 #endif
   const size_t n_tab = coded ? coded->idx.size() : 0, n_w = coded ? coded->weight.size() : 0;
   for (int u0 = 0; u0 < n_all; u0 += chunk) {
     const int n = imin(chunk, n_all - u0);
     ArenaPlan plan;
-    const size_t o_counts = plan.add((size_t)n * b.f_stride * 4);
-    const size_t o_offs = plan.add((size_t)n * b.f_stride * 4);
+    const size_t slots = b.x_off ? (size_t)cum.back() : (size_t)n * b.f_stride;
+    static_assert(WB_CT_FRAME_BYTES == 2 * sizeof(unsigned), "the per-frame arrays below");
+    const size_t o_counts = plan.add(slots * sizeof(unsigned));
+    const size_t o_offs = plan.add(slots * sizeof(unsigned));
     const size_t o_totals = plan.add((size_t)n * 4);
     const size_t o_cidx = plan.add(n_tab * 4 + 4), o_cfrac = plan.add(n_tab * 8 + 8), o_cw = plan.add(n_w * 16 + 16);
     const size_t o_group = plan.add(group ? (size_t)n * 8 : 0);
+    const size_t o_cum = plan.add(b.x_off ? cum.size() * 8 : 0);
     unsigned char *blk = arena_block(ctx, plan.total);
     if (!blk) return 2;
     unsigned *counts = (unsigned *)(blk + o_counts), *offs = (unsigned *)(blk + o_offs);
@@ -286,14 +337,30 @@ static int ct_launch(Ctx *ctx, const Batch &b, double q1, int fft_size, double *
       if (rc) return rc;
       uid = gd; f_len = gd + n;
     }
+    const long long *cum_dev = nullptr;
+    if (b.x_off) {
+      cum_dev = (const long long *)(blk + o_cum);
+      const int rc = dev_memcpy_h2d(ctx, blk + o_cum, cum.data(), cum.size() * 8);
+      if (rc) return rc;
+    }
     const double *f0 = b.f0 + base * b.f_stride;
-    const long long total_slots = (long long)n * b.f_stride;
-    WB_LAUNCH_FLAT(ct_count_kernel, dim3((unsigned)((total_slots + 255) / 256)), 256, 0, ctx->stream,
-                   f0, f_len, b.f_stride, n, b.fs, fft_size, f0_floor, uid, counts);
-    scan_counts(ctx, counts, f_len, b.f_stride, nullptr, offs, totals, n);
+    const long long total_slots = (long long)slots;
+    if (b.x_off) {
+      if (total_slots)
+        WB_LAUNCH_FLAT(ct_count_packed_kernel, dim3((unsigned)((total_slots + 255) / 256)), 256, 0, ctx->stream,
+                       f0, b.f_off, cum_dev, n, b.fs, fft_size, f0_floor, uid, counts);
+      scan_counts(ctx, counts, f_len, 0, nullptr, offs, totals, n, cum_dev);
+    } else {
+      WB_LAUNCH_FLAT(ct_count_kernel, dim3((unsigned)((total_slots + 255) / 256)), 256, 0, ctx->stream,
+                     f0, f_len, b.f_stride, n, b.fs, fft_size, f0_floor, uid, counts);
+      scan_counts(ctx, counts, f_len, b.f_stride, nullptr, offs, totals, n);
+    }
     CtParams p;
     p.x = b.x + base * b.x_stride; p.x_len = b.x_len + base; p.x_stride = b.x_stride;
     p.time_axis = b.time_axis + base * b.f_stride; p.f0 = f0; p.f_len = f_len; p.uid = uid;
+    p.x_off = b.x_off; p.cum = cum_dev; p.n_launch = n;
+    // padded: one CTA per (frame, utterance) of the rows; packed: one per frame of the launch
+    const dim3 grid = b.x_off ? dim3((unsigned)total_slots) : dim3((unsigned)max_f_len, (unsigned)n);
     p.f_stride = b.f_stride; p.fs = b.fs; p.fft_size = fft_size; p.lg_fft = lg;
     p.q1 = q1; p.f0_floor = f0_floor;
     p.draws = table; p.draw_off = offs;
@@ -314,7 +381,12 @@ static int ct_launch(Ctx *ctx, const Batch &b, double q1, int fft_size, double *
       p.c_dims = coded->dims; p.c_idx = (const int *)(blk + o_cidx); p.c_frac = (const double *)(blk + o_cfrac);
       p.c_weight = (const double2 *)(blk + o_cw); p.c_norm = coded->norm;
       p.c_out = coded_out + out_base * coded->dims;
-      WB_LAUNCH_COOP(ct_coded_kernel, dim3((unsigned)max_f_len, (unsigned)n), ct_threads, smem, ctx->stream, p);
+      if (b.x_off)
+        WB_LAUNCH_COOP(ct_coded_packed_kernel, grid, ct_threads, smem, ctx->stream, p);
+      else
+        WB_LAUNCH_COOP(ct_coded_kernel, dim3((unsigned)max_f_len, (unsigned)n), ct_threads, smem, ctx->stream, p);
+    } else if (b.x_off) {
+      WB_LAUNCH_COOP(ct_frame_packed_kernel, grid, ct_threads, smem, ctx->stream, p);
     } else
     WB_LAUNCH_COOP(ct_frame_kernel, dim3((unsigned)max_f_len, (unsigned)n), ct_threads, smem, ctx->stream, p);
     int rc = dev_check(ctx, "cheaptrick");

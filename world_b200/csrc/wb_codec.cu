@@ -19,6 +19,8 @@
 #include "../../include/world_b200.h"
 #include <math.h>
 #include <string.h>
+#include <algorithm>
+#include <string>
 #include <vector>
 
 namespace wb {
@@ -43,15 +45,15 @@ struct CodecParams {
   const double2 *weight;      // DCT / IDCT weights
   double norm;                // sqrt(fft_size / 2)
   const double2 *tw;
-  const int *list;            // decode: the utterance of each blockIdx.y, or NULL: blockIdx.y itself
-  int row;                    // decode: doubles per output frame row (>= bins)
-  // decode over packed rows (null: padded rows of f_stride): utterance u's frame i is row f_off[u] + i of in and out;
-  // blockIdx.x is a frame of the launch, entry j of list owning frames [cum[j], cum[j + 1])
+  const int *list;            // the utterance of each blockIdx.y, or NULL: blockIdx.y itself
+  int row;                    // doubles per full frame row (>= bins): decode's output, code's input
+  // packed rows (null: padded rows of f_stride): utterance u's frame i is row f_off[u] + i of in and out; a frame of
+  // the launch (blockIdx.x, code_ap_kernel: its thread) is one of entry j of list, which owns frames [cum[j], cum[j + 1])
   const long long *f_off, *cum;
   int list_n;
 };
 
-// decode: the utterance, frame and (in and out) row of this CTA
+// the utterance, frame and (in and out) row of this CTA
 struct DecodeAt { int u, f; size_t row; };
 WB_DEV DecodeAt decode_at(const CodecParams &p) {
   if (p.cum) {
@@ -63,13 +65,17 @@ WB_DEV DecodeAt decode_at(const CodecParams &p) {
   return {u, f, (size_t)u * p.f_stride + f};
 }
 
+// kPacked: packed rows (p.cum), a compile-time choice so that the padded kernel keeps its own code
+template <bool kPacked>
 WB_KERNEL(128, 8) code_sp_kernel(CodecParams p) {
   WB_DYN_SMEM(double, smem);
-  const int tid = WB_TID, nth = WB_NTH, u = blockIdx.y, f = blockIdx.x;
-  if (f >= p.f_len[u]) return;
+  const int tid = WB_TID, nth = WB_NTH;
+  const DecodeAt at = kPacked ? decode_at(p) : DecodeAt{(int)blockIdx.y, (int)blockIdx.x,
+                                                        (size_t)blockIdx.y * p.f_stride + blockIdx.x};
+  if (at.f >= p.f_len[at.u]) return;
   double *lgs = smem;                       // bins (+1 pad)
   double *buf = smem + ((p.bins + 2) & ~1); // max_dim + 2
-  const double *row = p.in + ((size_t)u * p.f_stride + f) * p.bins;
+  const double *row = p.in + at.row * p.row;
   for (int j = tid; j < p.bins; j += nth) lgs[j] = log(row[j]);                     // codec.cpp:288-289
   WB_SYNC();
   const int M = p.max_dim, bias = M / 2;
@@ -82,7 +88,8 @@ WB_KERNEL(128, 8) code_sp_kernel(CodecParams p) {
   WB_SYNC();
   rfft_forward(buf, p.lg, p.tw);
   const double2 *X = reinterpret_cast<const double2 *>(buf);
-  double *out = p.out + ((size_t)u * p.f_stride + f) * p.dims;
+  // packed: the row is looked up again after the transform rather than held across it
+  double *out = p.out + (kPacked ? decode_at(p).row : at.row) * p.dims;
   for (int d = tid; d < p.dims; d += nth) {                                         // :85-88
     const double2 w = __ldg(p.weight + d);
     out[d] = (X[d].x * w.x - X[d].y * w.y) / p.norm;
@@ -124,10 +131,19 @@ WB_KERNEL(128, 8) decode_sp_kernel(CodecParams p) {
 }
 
 WB_KERNEL_PLAIN code_ap_kernel(CodecParams p) {
-  const int u = blockIdx.y, f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= p.f_len[u]) return;
-  const double *row = p.in + ((size_t)u * p.f_stride + f) * p.bins;
-  double *out = p.out + ((size_t)u * p.f_stride + f) * p.dims;
+  size_t r;
+  if (p.cum) {   // packed rows: the thread's frame of the launch
+    const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= p.cum[p.list_n]) return;
+    const int j = packed_find(p.cum, p.list_n, g);
+    r = (size_t)(p.f_off[p.list ? p.list[j] : j] + (g - p.cum[j]));
+  } else {
+    const int u = blockIdx.y, f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= p.f_len[u]) return;
+    r = (size_t)u * p.f_stride + f;
+  }
+  const double *row = p.in + r * p.row;
+  double *out = p.out + r * p.dims;
   for (int b = 0; b < p.dims; ++b) {                                                // :231-236
     const int k = __ldg(p.idx + b);
     const double y0 = 20 * log10(row[k]);
@@ -236,7 +252,7 @@ void launch_frames(Ctx *ctx, int which, CodecParams p, const int *f_len, int n_u
                    size_t out_row, size_t smem) {
   p.tw = ctx->twiddle;
 #ifndef WB_EMU
-  if (which == 0) cudaFuncSetAttribute(code_sp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (which == 0) cudaFuncSetAttribute(code_sp_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (which == 1) cudaFuncSetAttribute(decode_sp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 #endif
   const double *in = p.in;
@@ -246,7 +262,7 @@ void launch_frames(Ctx *ctx, int which, CodecParams p, const int *f_len, int n_u
     p.f_len = f_len + u0;
     p.in = in + (size_t)u0 * p.f_stride * in_row;
     p.out = out + (size_t)u0 * p.f_stride * out_row;
-    if (which == 0) WB_LAUNCH_COOP(code_sp_kernel, dim3((unsigned)max_f, (unsigned)n), 128, smem, ctx->stream, p);
+    if (which == 0) WB_LAUNCH_COOP(code_sp_kernel<false>, dim3((unsigned)max_f, (unsigned)n), 128, smem, ctx->stream, p);
     if (which == 1) WB_LAUNCH_COOP(decode_sp_kernel, dim3((unsigned)max_f, (unsigned)n), 128, smem, ctx->stream, p);
     if (which == 2) WB_LAUNCH_FLAT(code_ap_kernel, dim3((unsigned)((max_f + 127) / 128), (unsigned)n), 128, 0, ctx->stream, p);
     if (which == 3) WB_LAUNCH_FLAT(decode_ap_kernel, dim3((unsigned)max_f, (unsigned)n), 128, 0, ctx->stream, p);
@@ -412,6 +428,114 @@ int codec_ap_tables(Ctx *ctx, int fs, int fft_size, CodecTables *t) {
   return 0;
 }
 
+// The packed codec calls (which: 0 CodeSpectralEnvelope, 1 DecodeSpectralEnvelope, 2 CodeAperiodicity,
+// 3 DecodeAperiodicity): utterance u is frames [f_offsets[u], f_offsets[u + 1]) of its full rows ([F][row_stride], 0:
+// the largest fft_sizes[u] / 2 + 1) and of its coded rows ([F][dims]).  Every check runs first, with the padded call's
+// rules at each utterance's size; then the utterances are grouped by fft_size, in order of first appearance, and each
+// group's frames are one launch in which entry j of the group's list owns frames [cum[j], cum[j + 1]) of the grid.
+static int codec_packed(WorldB200 *h, int which, const double *in, int n, const long long *f_offsets, int row_stride,
+                        const int *fft_sizes, int fs, int dims, double *out) {
+  static const char *const names[4] = {"code_spectral_envelope_packed", "decode_spectral_envelope_packed",
+                                       "code_aperiodicity_packed", "decode_aperiodicity_packed"};
+  if (!h) return WORLD_B200_EINVAL;
+  DeviceGuard guard_(&h->c);
+  Ctx *ctx = &h->c;
+  auto fail = [&](const std::string &what, int u = -1) {
+    ctx->last_error = std::string(names[which]) + ": " + what;
+    if (u >= 0) ctx->last_error += " (utterance " + std::to_string(u) + ")";
+    return WORLD_B200_EINVAL;
+  };
+  const bool sp = which < 2, code = which == 0 || which == 2;
+  if (n < 0 || fs <= 0) return fail("n_utts must be >= 0 and fs > 0");
+  if (!fft_sizes) return fail("fft_sizes must be given");
+  const int n_ap = number_of_aperiodicities(fs);
+  // the coded rows of the aperiodicity are empty below 12 kHz: CodeAperiodicity writes nothing, and its decode reads
+  // nothing (a NULL array is allowed there)
+  const double *coded = code ? out : in;
+  std::vector<int> f_len;
+  const std::string bad = packed_lengths("f_offsets", "frames", n, f_offsets, 0, &f_len);
+  if (!bad.empty()) return fail(bad);
+  // empty arrays may be NULL: a batch without frames reads and writes nothing
+  if (n > 0 && f_offsets[n] > 0 && (!(code ? in : out) || (!coded && (sp || n_ap > 0))))
+    return fail("the input and output rows must be given");
+  std::vector<int> sizes, table(n);   // the distinct sizes, and each utterance's entry
+  std::vector<Tables> tables;
+  int row = row_stride;
+  for (int u = 0; u < n; ++u) {
+    const int f = fft_sizes[u];
+    if (!sp && f < 2) return fail("fft_size must be at least 2", u);
+    if (!row_stride) row = imax(row, f / 2 + 1);
+    table[u] = (int)(std::find(sizes.begin(), sizes.end(), f) - sizes.begin());
+    if (table[u] < (int)sizes.size()) continue;
+    sizes.push_back(f);
+    tables.emplace_back();
+    const int rc = which == 0   ? codec_sp_tables(ctx, fs, f, dims, &tables.back())
+                   : which == 1 ? codec_decode_sp_tables(ctx, fs, f, dims, &tables.back())
+                   : which == 2 ? codec_ap_tables(ctx, fs, f, &tables.back())
+                                : (codec_decode_ap_tables(fs, f, &tables.back()), 0);
+    if (rc) {   // the table builder's message names its codec function already
+      ctx->last_error += " (utterance " + std::to_string(u) + ")";
+      return rc;
+    }
+  }
+  for (int u = 0; u < n; ++u)
+    if (row < fft_sizes[u] / 2 + 1) return fail("row_stride is smaller than fft_size / 2 + 1", u);
+  if (which == 2 && n_ap <= 0) return 0;   // nothing to write below 12 kHz, like the reference's empty loops
+  int rc = 0;
+  for (size_t s = 0; s < sizes.size() && !rc; ++s) {
+    const Tables &t = tables[s];
+    const int fft_size = sizes[s], M = fft_size / 2;
+    std::vector<int> list;
+    std::vector<long long> cum(1, 0);
+    for (int u = 0; u < n; ++u)
+      if (table[u] == (int)s && f_len[u] > 0) { list.push_back(u); cum.push_back(cum.back() + f_len[u]); }
+    const long long frames = cum.back();
+    if (frames == 0) continue;
+    const int m = (int)list.size();
+    ArenaPlan plan;
+    const size_t o_off = plan.add((size_t)(n + 1) * 8), o_cum = plan.add((size_t)(m + 1) * 8);
+    const size_t o_len = plan.add((size_t)n * 4), o_list = plan.add((size_t)m * 4);
+    const size_t o_idx = plan.add(t.idx.size() * 4 + 4), o_frac = plan.add(t.frac.size() * 8 + 8);
+    const size_t o_w = plan.add(t.weight.size() * 16 + 16);
+    unsigned char *blk = arena_block(ctx, plan.total);
+    if (!blk) return WORLD_B200_ENOMEM;
+    rc = dev_memcpy_h2d(ctx, blk + o_off, f_offsets, (size_t)(n + 1) * 8);
+    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_cum, cum.data(), cum.size() * 8);
+    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_len, f_len.data(), (size_t)n * 4);
+    if (!rc) rc = dev_memcpy_h2d(ctx, blk + o_list, list.data(), (size_t)m * 4);
+    if (!rc && !t.idx.empty()) rc = dev_memcpy_h2d(ctx, blk + o_idx, t.idx.data(), t.idx.size() * 4);
+    if (!rc && !t.frac.empty()) rc = dev_memcpy_h2d(ctx, blk + o_frac, t.frac.data(), t.frac.size() * 8);
+    if (!rc && !t.weight.empty()) rc = dev_memcpy_h2d(ctx, blk + o_w, t.weight.data(), t.weight.size() * 16);
+    if (rc) return rc;
+    const long long *f_off = (const long long *)(blk + o_off), *cum_dev = (const long long *)(blk + o_cum);
+    const int *f_len_dev = (const int *)(blk + o_len), *list_dev = (const int *)(blk + o_list);
+    const CodecDeviceTables d{(const int *)(blk + o_idx), (const double *)(blk + o_frac),
+                              (const double2 *)(blk + o_w)};
+    if (!code) {
+      codec_decode_packed_launch(ctx, sp, t, d, fft_size, f_len_dev, f_off, list_dev, m, cum_dev, frames,
+                                 coded ? coded : out, out, row);
+    } else {
+      CodecParams p;
+      memset(&p, 0, sizeof(p));
+      p.in = in; p.out = out; p.bins = M + 1; p.row = row; p.dims = t.dims;
+      p.idx = d.idx; p.frac = d.frac; p.weight = d.weight; p.tw = ctx->twiddle;
+      p.f_len = f_len_dev; p.f_off = f_off; p.list = list_dev; p.cum = cum_dev; p.list_n = m;
+      if (sp) {
+        p.max_dim = M; p.lg = t.lg_half; p.norm = t.norm;
+        const size_t smem = (size_t)(((M + 3) & ~1) + M + 2) * 8;
+#ifndef WB_EMU
+        cudaFuncSetAttribute(code_sp_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+#endif
+        WB_LAUNCH_COOP(code_sp_kernel<true>, dim3((unsigned)frames), 128, smem, ctx->stream, p);
+      } else {
+        WB_LAUNCH_FLAT(code_ap_kernel, dim3((unsigned)((frames + 127) / 128)), 128, 0, ctx->stream, p);
+      }
+    }
+    rc = dev_check(ctx, "codec");
+  }
+  return rc;
+}
+
 }  // namespace wb
 
 using namespace wb;
@@ -419,6 +543,32 @@ using namespace wb;
 extern "C" {
 
 int GetNumberOfAperiodicities(int fs) { return number_of_aperiodicities(fs); }
+
+int world_b200_code_spectral_envelope_packed(WorldB200 *h, const double *spectrogram, int n_utts,
+                                             const long long *f_offsets, int row_stride, const int *fft_sizes, int fs,
+                                             int number_of_dimensions, double *coded_spectral_envelope) {
+  return codec_packed(h, 0, spectrogram, n_utts, f_offsets, row_stride, fft_sizes, fs, number_of_dimensions,
+                      coded_spectral_envelope);
+}
+
+int world_b200_decode_spectral_envelope_packed(WorldB200 *h, const double *coded_spectral_envelope, int n_utts,
+                                               const long long *f_offsets, int row_stride, const int *fft_sizes,
+                                               int fs, int number_of_dimensions, double *spectrogram) {
+  return codec_packed(h, 1, coded_spectral_envelope, n_utts, f_offsets, row_stride, fft_sizes, fs,
+                      number_of_dimensions, spectrogram);
+}
+
+int world_b200_code_aperiodicity_packed(WorldB200 *h, const double *aperiodicity, int n_utts,
+                                        const long long *f_offsets, int row_stride, const int *fft_sizes, int fs,
+                                        double *coded_aperiodicity) {
+  return codec_packed(h, 2, aperiodicity, n_utts, f_offsets, row_stride, fft_sizes, fs, 0, coded_aperiodicity);
+}
+
+int world_b200_decode_aperiodicity_packed(WorldB200 *h, const double *coded_aperiodicity, int n_utts,
+                                          const long long *f_offsets, int row_stride, const int *fft_sizes, int fs,
+                                          double *aperiodicity) {
+  return codec_packed(h, 3, coded_aperiodicity, n_utts, f_offsets, row_stride, fft_sizes, fs, 0, aperiodicity);
+}
 
 int world_b200_code_spectral_envelope_batch(WorldB200 *h, const double *spectrogram, int n_utts,
                                             const int *f0_lengths, int f0_stride, int fs, int fft_size,
@@ -432,8 +582,8 @@ int world_b200_code_spectral_envelope_batch(WorldB200 *h, const double *spectrog
   const int M = fft_size / 2, lg = t.lg_half;
   CodecParams p;
   memset(&p, 0, sizeof(p));
-  p.f_stride = f0_stride; p.in = spectrogram; p.out = coded; p.bins = M + 1; p.dims = number_of_dimensions;
-  p.max_dim = M; p.lg = lg; p.norm = sqrt((double)M);
+  p.f_stride = f0_stride; p.in = spectrogram; p.out = coded; p.bins = M + 1; p.row = M + 1;
+  p.dims = number_of_dimensions; p.max_dim = M; p.lg = lg; p.norm = sqrt((double)M);
   const size_t smem = (size_t)(((M + 3) & ~1) + M + 2) * 8;
   return run_frames(ctx, 0, p, t, f0_lengths, n_utts, M + 1, number_of_dimensions, smem);
 }
@@ -464,7 +614,7 @@ int world_b200_code_aperiodicity_batch(WorldB200 *h, const double *aperiodicity,
   if (rc) return rc;
   CodecParams p;
   memset(&p, 0, sizeof(p));
-  p.f_stride = f0_stride; p.in = aperiodicity; p.out = coded; p.bins = fft_size / 2 + 1; p.dims = n_ap;
+  p.f_stride = f0_stride; p.in = aperiodicity; p.out = coded; p.bins = fft_size / 2 + 1; p.row = p.bins; p.dims = n_ap;
   return run_frames(ctx, 2, p, t, f0_lengths, n_utts, fft_size / 2 + 1, n_ap, 0);
 }
 

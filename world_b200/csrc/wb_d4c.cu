@@ -34,6 +34,11 @@ struct D4cParams {
   int pw_doubles;                    // doubles of the fast body kernel's power row (d4c_body_pw_doubles)
   double *out;
   const long long *f_off;   // [n] packed rows: output frame of each utterance's frame 0; null: u * f_stride
+  // packed inputs: utterance u's samples at x + x_off[u]; its frames at f_off[u] + i ([n_utts + 1]) in the inputs, the
+  // outputs and every per-frame array (draw counts and offsets, selected, slow_list); null: padded inputs
+  const long long *x_off;
+  int n_utts;
+  int *frame_u;             // packed: [frames] the utterance of each frame, written by LoveTrain for the body kernel
   const double2 *tw;
   const double2 *tw_body;   // compact twiddles of size d_fft (tw_sized_offset): the fast body kernel's
   int *status;
@@ -46,14 +51,50 @@ struct D4cParams {
   const int *u_fft; const double *u_thr; const int *u_ctab;
 };
 
-WB_DEV int d4c_ct_fft(const D4cParams &p, size_t fidx) {
-  return p.u_fft ? __ldg(p.u_fft + fidx / p.f_stride) : p.ct_fft_size;
+// kPacked (every kernel below): packed inputs (p.x_off), a compile-time choice so that the padded kernels keep their own
+// code.  fidx: utterance u's frame in the inputs and the per-frame arrays (d4c_frame).
+template <bool kPacked>
+WB_DEV int d4c_ct_fft(const D4cParams &p, int u, size_t fidx) {
+  return p.u_fft ? __ldg(p.u_fft + (kPacked ? (size_t)u : fidx / p.f_stride)) : p.ct_fft_size;
 }
 
-// the output frame of frame fidx (= u * f_stride + i of the slice's rows): only the address differs between the padded
-// and the packed layout; f0, the time axis, the draws and slow_list keep the slice's own indices
+// frame i of utterance u in the inputs and the per-frame arrays: u * f_stride + i of the slice's rows, or with packed
+// inputs its packed frame
+template <bool kPacked>
+WB_DEV size_t d4c_frame(const D4cParams &p, int u, int i) {
+  return kPacked ? (size_t)(p.f_off[u] + i) : (size_t)u * p.f_stride + i;
+}
+
+// the output frame of frame fidx: only the address differs between the padded and the packed layout; f0, the time
+// axis, the draws and slow_list keep the slice's own indices (packed inputs: the output's too)
+template <bool kPacked>
 WB_DEV size_t d4c_out_frame(const D4cParams &p, size_t fidx) {
-  return p.f_off ? (size_t)p.f_off[fidx / p.f_stride] + fidx % p.f_stride : fidx;
+  return !kPacked && p.f_off ? (size_t)p.f_off[fidx / p.f_stride] + fidx % p.f_stride : fidx;
+}
+
+template <bool kPacked>
+WB_DEV const double *d4c_samples(const D4cParams &p, int u) {
+  return kPacked ? p.x + p.x_off[u] : p.x + (size_t)u * p.x_stride;
+}
+
+// The frame kernels' CTA: padded, frame blockIdx.x of utterance blockIdx.y (false past its frames); packed, the chunk's
+// frame blockIdx.x -- the grid runs over the packed frames, so none of it idles on short utterances -- of the utterance
+// found by binary search over f_off.  Its frame index (d4c_frame) is then blockIdx.x itself, which the compiler
+// recomputes rather than keeps live across the frame's transforms.
+template <bool kPacked>
+WB_DEV bool d4c_cta_frame(const D4cParams &p, int &u, int &i) {
+  if (kPacked) {
+    u = packed_find(p.f_off, p.n_utts, (long long)blockIdx.x);
+    i = (int)((long long)blockIdx.x - p.f_off[u]);
+    return true;
+  }
+  u = blockIdx.y;
+  i = blockIdx.x;
+  return i < p.f_len[u];
+}
+template <bool kPacked>
+WB_DEV size_t d4c_cta_fidx(const D4cParams &p) {
+  return kPacked ? (size_t)blockIdx.x : (size_t)blockIdx.y * p.f_stride + blockIdx.x;
 }
 
 WB_KERNEL_PLAIN d4c_count_a_kernel(const double *__restrict__ f0, const int *__restrict__ f_len,
@@ -63,6 +104,19 @@ WB_KERNEL_PLAIN d4c_count_a_kernel(const double *__restrict__ f0, const int *__r
   const int u = (int)(g / f_stride), i = (int)(g % f_stride);
   unsigned c = 0;
   if (i < f_len[u] && f0[g] != 0.0) {
+    const double f = dmax(f0[g], 40.0);
+    c = (unsigned)(2 * round_half_away(3.0 * fs / f / 2.0) + 1);
+  }
+  counts[g] = c;
+}
+
+// the same over the packed frames [0, frames): every one lies inside its utterance
+WB_KERNEL_PLAIN d4c_count_a_packed_kernel(const double *__restrict__ f0, long long frames, int fs,
+                                          unsigned *__restrict__ counts) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= frames) return;
+  unsigned c = 0;
+  if (f0[g] != 0.0) {
     const double f = dmax(f0[g], 40.0);
     c = (unsigned)(2 * round_half_away(3.0 * fs / f / 2.0) + 1);
   }
@@ -105,14 +159,15 @@ WB_DEV int d4c_windowed(const double *__restrict__ x, int x_len, int fs, double 
 
 // a frame D4C does not analyse (unvoiced, or LoveTrain says noise): 1 - 1e-12 in every bin (d4c.cpp:372-383);
 // coded: 20 log10 of that at every band centre (interp1Q between equal nodes)
-WB_DEV void d4c_fill_frame(const D4cParams &p, size_t fidx) {
-  const size_t oidx = d4c_out_frame(p, fidx);
+template <bool kPacked>
+WB_DEV void d4c_fill_frame(const D4cParams &p, int u, size_t fidx) {
+  const size_t oidx = d4c_out_frame<kPacked>(p, fidx);
   if (p.c_out) {
     const double v = 20 * log10(1.0 - kTiny);
     for (int b = WB_TID; b < p.c_n; b += WB_NTH) p.c_out[oidx * (size_t)p.c_n + b] = v;
     return;
   }
-  const int bins = d4c_ct_fft(p, fidx) / 2 + 1;
+  const int bins = d4c_ct_fft<kPacked>(p, u, fidx) / 2 + 1;
   double *row = p.out + oidx * (size_t)p.out_stride;
   for (int k = WB_TID; k < bins; k += WB_NTH) row[k] = 1.0 - kTiny;
 }
@@ -135,14 +190,14 @@ WB_DEV double d4c_bin_db(const double *coarse, int n_ap, int fs, int ct_fft_size
 
 // dB -> amplitude row (d4c.cpp:372-383), or the coded row: the dB values themselves, interp1Q'd onto the band centres
 // (the 10^(y/20) / 20 log10 pair of the unfused path cancels)
-template <bool kFastExp>
-WB_DEV void d4c_write_frame(const D4cParams &p, size_t fidx, const double *coarse) {
+template <bool kFastExp, bool kPacked>
+WB_DEV void d4c_write_frame(const D4cParams &p, int u, size_t fidx, const double *coarse) {
   const int tid = WB_TID, nth = WB_NTH;
-  const int ct_fft = d4c_ct_fft(p, fidx);
+  const int ct_fft = d4c_ct_fft<kPacked>(p, u, fidx);
   const int bins = ct_fft / 2 + 1;
-  const size_t oidx = d4c_out_frame(p, fidx);
+  const size_t oidx = d4c_out_frame<kPacked>(p, fidx);
   if (p.c_out) {
-    const int tab = p.u_ctab ? __ldg(p.u_ctab + fidx / p.f_stride) : 0;
+    const int tab = p.u_ctab ? __ldg(p.u_ctab + (kPacked ? (size_t)u : fidx / p.f_stride)) : 0;
     for (int b = tid; b < p.c_n; b += nth) {
       const int k = __ldg(p.c_idx + tab + b);
       const double y0 = d4c_bin_db(coarse, p.n_ap, p.fs, ct_fft, k);
@@ -160,16 +215,18 @@ WB_DEV void d4c_write_frame(const D4cParams &p, size_t fidx, const double *coars
 }
 
 // ------------------------------------------------------------------ pass A: LoveTrain
+template <bool kPacked>
 WB_KERNEL(128, 4) d4c_lovetrain_kernel(D4cParams p) {
   WB_DYN_SMEM(double2, smem2);
   const int tid = WB_TID, nth = WB_NTH;
-  const int u = blockIdx.y, i = blockIdx.x;
-  if (i >= p.f_len[u]) return;
-  const size_t fidx = (size_t)u * p.f_stride + i;
+  int u, i;
+  if (!d4c_cta_frame<kPacked>(p, u, i)) return;
+  const size_t fidx = d4c_cta_fidx<kPacked>(p);
   const double f0 = p.f0[fidx];
   if (f0 == 0.0) {
-    d4c_fill_frame(p, fidx);
+    d4c_fill_frame<kPacked>(p, u, fidx);
     if (tid == 0) { p.selected[fidx] = 0; p.count_b[fidx] = 0; }
+    if (kPacked && tid == 0) p.frame_u[fidx] = u;
     return;
   }
   const int N = p.lt_fft, half = N / 2;
@@ -178,7 +235,7 @@ WB_KERNEL(128, 4) d4c_lovetrain_kernel(D4cParams p) {
   double *red = reinterpret_cast<double *>(B + slots);
   double *za = reinterpret_cast<double *>(A), *win = reinterpret_cast<double *>(B);
   const double f = dmax(f0, 40.0);
-  const double *x = p.x + (size_t)u * p.x_stride;
+  const double *x = d4c_samples<kPacked>(p, u);
   const unsigned *draw = p.draws + p.off_a[fidx];
   const int nwin = d4c_windowed(x, p.x_len[u], p.fs, f, p.time_axis[fidx], 2, 3.0, draw,
                                 [&](int j) { return za + rpad(j); }, [&](int j) { return win + j; }, red);
@@ -198,7 +255,8 @@ WB_KERNEL(128, 4) d4c_lovetrain_kernel(D4cParams p) {
   block_sum2(s_lo, s_hi, red);
   const double ap0 = s_lo / s_hi;
   const bool sel = ap0 > (p.u_thr ? p.u_thr[u] : p.threshold);  // d4c.cpp:386
-  if (!sel) d4c_fill_frame(p, fidx);
+  if (!sel) d4c_fill_frame<kPacked>(p, u, fidx);
+  if (kPacked && tid == 0) p.frame_u[fidx] = u;
   if (tid == 0) {
     p.selected[fidx] = sel ? 1 : 0;
     unsigned c = 0;
@@ -379,14 +437,17 @@ WB_HD inline int d4c_body_pw_doubles(int d_fft, int fs, int n_ap, int threads) {
 // kLg = log2(d_fft), 9..12: the transforms are sfft_forward_fixed at compile-time size on d_fft / 16 threads, with the
 // compact twiddle table p.tw_body of size d_fft (every twiddle the frame reads: the passes, the real-FFT unpack and the
 // centroid's DIF split)
-template <int kLg>
+template <int kLg, bool kPacked>
 WB_DEV void d4c_body_frame(const D4cParams &p) {
   WB_DYN_SMEM(double2, smem2);
   const int tid = WB_TID, nth = WB_NTH;
-  const int u = blockIdx.y, i = blockIdx.x;
-  if (i >= p.f_len[u]) return;
-  const size_t fidx = (size_t)u * p.f_stride + i;
+  // packed: the grid runs over the packed frames, and the frame's utterance is read from frame_u (LoveTrain's) at each
+  // use, after barriers, so that like the padded kernel's blockIdx-derived indices nothing is held across the transforms
+  const int u = kPacked ? 0 : (int)blockIdx.y, i = blockIdx.x;
+  if (!kPacked && i >= p.f_len[u]) return;
+  const size_t fidx = kPacked ? (size_t)blockIdx.x : d4c_frame<kPacked>(p, u, i);
   if (!p.selected[fidx]) return;
+  auto utt = [&]() { return kPacked ? p.frame_u[blockIdx.x] : u; };
   constexpr int N = 1 << kLg, half = N / 2;
   const int fs = p.fs;
   const double2 *__restrict__ twc = p.tw_body;
@@ -412,18 +473,19 @@ WB_DEV void d4c_body_frame(const D4cParams &p) {
 #else
         const int at = atomicAdd(p.slow_count, 1);
 #endif
-        p.slow_list[at] = (int)(u * p.f_stride + i);
+        p.slow_list[at] = (int)fidx;
       }
       return;
     }
   }
-  const double *x = p.x + (size_t)u * p.x_stride;
-  const int x_len = p.x_len[u];
+  const double *x = d4c_samples<kPacked>(p, u);
+  int x_len = p.x_len[u];
   const unsigned *draw = p.draws + p.off_b[fidx];
 
   // ---- static centroid = centroid(t - 1/4f) + centroid(t + 1/4f)   (d4c.cpp:90-140)
   for (int pass = 0; pass < 2; ++pass) {
     const double pos = pass == 0 ? t - 0.25 / f : t + 0.25 / f;
+    if (kPacked) { x = d4c_samples<kPacked>(p, utt()); x_len = p.x_len[utt()]; }
     const int nwin = d4c_windowed(x, x_len, fs, f, pos, 2, 4.0, draw, [&](int j) { return pw + j; },
                                   [&](int j) { return wv + j; }, red);
     draw += nwin;
@@ -456,6 +518,7 @@ WB_DEV void d4c_body_frame(const D4cParams &p) {
 
   // ---- smoothed power spectrum (d4c.cpp:149-166)
   {
+    if (kPacked) { x = d4c_samples<kPacked>(p, utt()); x_len = p.x_len[utt()]; }
     const int nwin = d4c_windowed(x, x_len, fs, f, t, 1, 4.0, draw, [&](int j) { return pd + rpad(j); },
                                   [&](int j) { return pw + j; }, red);
     for (int j = nwin + tid; j < N; j += nth) pd[rpad(j)] = 0.0;
@@ -516,22 +579,23 @@ WB_DEV void d4c_body_frame(const D4cParams &p) {
   WB_SYNC();
 
   // ---- interp1 onto the CheapTrick frequency grid, dB -> amplitude (d4c.cpp:330-338, 372-383)
-  d4c_write_frame<true>(p, fidx, coarse);
+  d4c_write_frame<true, kPacked>(p, utt(), kPacked ? (size_t)blockIdx.x : fidx, coarse);
 }
 
 // d_fft / 16 threads; the register budget (80) of 768 threads per SM -- six CTAs at 16 kHz, as many as the shared
 // memory holds
-template <int kLg>
-WB_KERNEL(1 << (kLg - 4), 768 >> (kLg - 4)) d4c_body_kernel_lg(D4cParams p) { d4c_body_frame<kLg>(p); }
+template <int kLg, bool kPacked>
+WB_KERNEL(1 << (kLg - 4), 768 >> (kLg - 4)) d4c_body_kernel_lg(D4cParams p) { d4c_body_frame<kLg, kPacked>(p); }
 
 typedef void (*D4cBodyKernel)(D4cParams);
 // nullptr: no fast body kernel at this size (d_fft below 512 or above 4096)
+template <bool kPacked>
 static D4cBodyKernel d4c_body_kernel_for(int d_lg) {
   switch (d_lg) {
-    case 9: return d4c_body_kernel_lg<9>;
-    case 10: return d4c_body_kernel_lg<10>;
-    case 11: return d4c_body_kernel_lg<11>;
-    case 12: return d4c_body_kernel_lg<12>;
+    case 9: return d4c_body_kernel_lg<9, kPacked>;
+    case 10: return d4c_body_kernel_lg<10, kPacked>;
+    case 11: return d4c_body_kernel_lg<11, kPacked>;
+    case 12: return d4c_body_kernel_lg<12, kPacked>;
     default: return nullptr;
   }
 }
@@ -539,9 +603,10 @@ static D4cBodyKernel d4c_body_kernel_for(int d_lg) {
 // ------------------------------------------------------------------ pass B, any window length (round-1 body, in-place DIT FFT)
 // Persistent kernel over slow_list (frames the fast kernel handed over); with d_fft > 4096 (fs above 48.1 kHz: the
 // fast kernel's thread count would exceed a CTA) the driver puts every selected frame on the list instead.
+template <bool kPacked>
 WB_DEV void d4c_body_slow_frame(const D4cParams &p, int u, int i, double *smem) {
   const int tid = WB_TID, nth = WB_NTH;
-  const size_t fidx = (size_t)u * p.f_stride + i;
+  const size_t fidx = d4c_frame<kPacked>(p, u, i);
   const int N = p.d_fft, half = N / 2, fs = p.fs;
   double *zb = smem;                       // 2N (+2): complex FFT buffer / smoothing scratch
   double *cent = zb + 2 * N + 2;           // half + 1
@@ -553,7 +618,7 @@ WB_DEV void d4c_body_slow_frame(const D4cParams &p, int u, int i, double *smem) 
 
   const double f = dmax(47.0, p.f0[fidx]);
   const double t = p.time_axis[fidx];
-  const double *x = p.x + (size_t)u * p.x_stride;
+  const double *x = d4c_samples<kPacked>(p, u);
   const int x_len = p.x_len[u];
   const unsigned *draw = p.draws + p.off_b[fidx];
 
@@ -649,25 +714,36 @@ WB_DEV void d4c_body_slow_frame(const D4cParams &p, int u, int i, double *smem) 
   WB_SYNC();
 
   // ---- interp1 onto the CheapTrick frequency grid, dB -> amplitude (d4c.cpp:330-338, 372-383)
-  d4c_write_frame<false>(p, fidx, coarse);
+  d4c_write_frame<false, kPacked>(p, u, fidx, coarse);
 }
 
+template <bool kPacked>
 WB_KERNEL(256, 2) d4c_body_slow_kernel(D4cParams p) {
   WB_DYN_SMEM(double, smem);
   const int count = *p.slow_count;
   for (int at = blockIdx.x; at < count; at += gridDim.x) {
     const int g = p.slow_list[at];
-    d4c_body_slow_frame(p, g / p.f_stride, g % p.f_stride, smem);
+    if (kPacked) {
+      const int u = packed_find(p.f_off, p.n_utts, g);
+      d4c_body_slow_frame<kPacked>(p, u, (int)(g - p.f_off[u]), smem);
+    } else {
+      d4c_body_slow_frame<kPacked>(p, g / p.f_stride, g % p.f_stride, smem);
+    }
     WB_SYNC();   // the next frame reuses the shared buffers
   }
 }
 
 // no fast body kernel at this d_fft: every selected frame goes through the list
+template <bool kPacked>
 WB_KERNEL_PLAIN d4c_list_all_kernel(D4cParams p, int n_utts) {
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= (long long)n_utts * p.f_stride) return;
-  const int u = (int)(g / p.f_stride), i = (int)(g % p.f_stride);
-  if (i >= p.f_len[u] || !p.selected[g]) return;
+  if (kPacked) {   // packed inputs: g is a packed frame, inside its utterance
+    if (g >= p.f_off[n_utts] || !p.selected[g]) return;
+  } else {
+    if (g >= (long long)n_utts * p.f_stride) return;
+    const int u = (int)(g / p.f_stride), i = (int)(g % p.f_stride);
+    if (i >= p.f_len[u] || !p.selected[g]) return;
+  }
 #ifdef WB_EMU
   const int at = (*p.slow_count)++;
 #else
@@ -736,11 +812,17 @@ int d4c_run(Ctx *ctx, const StagePlan &stage, const Batch &b, int u0, double *ou
                       0.012604 * cos(6.0 * kPi * tmp);
   }
 
+  // packed inputs: one pass, the packed stage call cut its chunks by frames
   const size_t per_utt_bytes = (size_t)b.f_stride * 28 + 64;
-  int chunk = balanced_chunk(imin(b.n, 65535), (int)dmin(65535.0, (double)ctx->scratch_budget / (double)per_utt_bytes));
+  int chunk = b.x_off ? b.n
+                      : balanced_chunk(imin(b.n, 65535), (int)dmin(65535.0, (double)ctx->scratch_budget / (double)per_utt_bytes));
   // fast body kernel: one radix-8 butterfly per thread in the passes of the d_fft / 2 complex transforms; at d_fft
   // above 4096 its thread count would exceed a CTA, below 512 a warp
-  const D4cBodyKernel d4c_body_kernel = d4c_body_kernel_for(p.d_lg);
+  const bool packed = b.x_off != nullptr;
+  const D4cBodyKernel d4c_body_kernel = packed ? d4c_body_kernel_for<true>(p.d_lg) : d4c_body_kernel_for<false>(p.d_lg);
+  // named as the kernels, which the launches' profile entries are
+  const D4cBodyKernel d4c_lovetrain_kernel = packed ? wb::d4c_lovetrain_kernel<true> : wb::d4c_lovetrain_kernel<false>;
+  const D4cBodyKernel d4c_body_slow_kernel = packed ? wb::d4c_body_slow_kernel<true> : wb::d4c_body_slow_kernel<false>;
   const bool all_slow = d4c_body_kernel == nullptr;
   int body_threads = p.d_fft / 16, lt_threads = 128, slow_threads = 128;
   if (const char *e = getenv("WB_LT_THREADS")) lt_threads = atoi(e);
@@ -757,13 +839,16 @@ int d4c_run(Ctx *ctx, const StagePlan &stage, const Batch &b, int u0, double *ou
   int rc = 0;
   for (int c0 = 0; c0 < b.n && rc == 0; c0 += chunk) {
     const int n = imin(chunk, b.n - c0);
-    const size_t slots = (size_t)n * b.f_stride;
+    const size_t slots = b.x_off ? (size_t)b.f_off_host[b.n] : (size_t)n * b.f_stride;
     ArenaPlan plan;
+    // per frame: the four arrays of counts and offsets, selected, slow_list and (packed) frame_u
+    static_assert(WB_D4C_FRAME_BYTES == 4 * sizeof(unsigned) + 1 + 2 * sizeof(int), "the per-frame arrays below");
     const size_t o_ca = plan.add(slots * 4), o_oa = plan.add(slots * 4);
     const size_t o_cb = plan.add(slots * 4), o_ob = plan.add(slots * 4);
     const size_t o_ta = plan.add((size_t)n * 4), o_tab = plan.add((size_t)n * 4);
     const size_t o_sel = plan.add(slots), o_nut = plan.add((size_t)p.win_len * 8);
     const size_t o_slow = plan.add(slots * 4), o_nslow = plan.add(4);
+    const size_t o_fu = plan.add(packed ? slots * 4 : 0);
     const size_t n_tab = coded ? (per_utt ? ctab_idx.size() : coded->idx.size()) : 0;
     const size_t o_cidx = plan.add(n_tab * 4 + 4), o_cfrac = plan.add(n_tab * 8 + 8);
     const size_t o_uopt = plan.add(per_utt ? (size_t)n * 16 : 0);
@@ -780,6 +865,7 @@ int d4c_run(Ctx *ctx, const StagePlan &stage, const Batch &b, int u0, double *ou
     p.x = b.x + (size_t)c0 * b.x_stride; p.x_len = b.x_len + c0; p.x_stride = b.x_stride;
     p.time_axis = b.time_axis + (size_t)c0 * b.f_stride; p.f0 = f0; p.f_len = f_len;
     p.f_stride = b.f_stride;
+    p.x_off = b.x_off; p.n_utts = n;
     p.nuttall = nuttall; p.draws = table;
     p.off_a = off_a; p.count_b = count_b; p.off_b = off_b; p.selected = selected;
     // packed rows: the output pointers stay at frame 0 and f_off places each utterance
@@ -809,18 +895,29 @@ int d4c_run(Ctx *ctx, const StagePlan &stage, const Batch &b, int u0, double *ou
       p.c_out = out + out_base * coded->dims;
     }
     p.slow_list = (int *)(blk + o_slow); p.slow_count = (int *)(blk + o_nslow);
+    p.frame_u = packed ? (int *)(blk + o_fu) : nullptr;
     dev_memset(ctx, p.slow_count, 0, 4);
 
-    WB_LAUNCH_FLAT(d4c_count_a_kernel, dim3((unsigned)((slots + 255) / 256)), 256, 0, ctx->stream, f0,
-                   f_len, b.f_stride, n, fs, count_a);
-    scan_counts(ctx, count_a, f_len, b.f_stride, nullptr, off_a, total_a, n);
-    WB_LAUNCH_COOP(d4c_lovetrain_kernel, dim3((unsigned)b.max_f_len, (unsigned)n), lt_threads, smem_lt,
-                   ctx->stream, p);
-    scan_counts(ctx, count_b, f_len, b.f_stride, total_a, off_b, total_ab, n);
-    if (all_slow)
-      WB_LAUNCH_FLAT(d4c_list_all_kernel, dim3((unsigned)((slots + 255) / 256)), 256, 0, ctx->stream, p, n);
+    if (b.x_off) {
+      if (slots)
+        WB_LAUNCH_FLAT(d4c_count_a_packed_kernel, dim3((unsigned)((slots + 255) / 256)), 256, 0, ctx->stream, f0,
+                       (long long)slots, fs, count_a);
+      scan_counts(ctx, count_a, f_len, 0, nullptr, off_a, total_a, n, b.f_off);
+    } else {
+      WB_LAUNCH_FLAT(d4c_count_a_kernel, dim3((unsigned)((slots + 255) / 256)), 256, 0, ctx->stream, f0,
+                     f_len, b.f_stride, n, fs, count_a);
+      scan_counts(ctx, count_a, f_len, b.f_stride, nullptr, off_a, total_a, n);
+    }
+    // padded: one CTA per (frame, utterance) of the rows; packed: one per packed frame
+    const dim3 frame_grid = packed ? dim3((unsigned)slots) : dim3((unsigned)b.max_f_len, (unsigned)n);
+    WB_LAUNCH_COOP(d4c_lovetrain_kernel, frame_grid, lt_threads, smem_lt, ctx->stream, p);
+    scan_counts(ctx, count_b, f_len, b.x_off ? 0 : b.f_stride, total_a, off_b, total_ab, n, b.x_off ? b.f_off : nullptr);
+    if (all_slow && packed)
+      WB_LAUNCH_FLAT(d4c_list_all_kernel<true>, dim3((unsigned)((slots + 255) / 256)), 256, 0, ctx->stream, p, n);
+    else if (all_slow)
+      WB_LAUNCH_FLAT(d4c_list_all_kernel<false>, dim3((unsigned)((slots + 255) / 256)), 256, 0, ctx->stream, p, n);
     else
-      WB_LAUNCH_COOP(d4c_body_kernel, dim3((unsigned)b.max_f_len, (unsigned)n), body_threads, smem_body,
+      WB_LAUNCH_COOP(d4c_body_kernel, frame_grid, body_threads, smem_body,
                      ctx->stream, p);
     // long windows (f0 near the floor): persistent CTAs over the list the fast kernel filled, usually empty
     WB_LAUNCH_COOP(d4c_body_slow_kernel, dim3((unsigned)(2 * ctx->sm_count)), slow_threads, smem_slow, ctx->stream, p);

@@ -166,6 +166,11 @@ struct Batch {
   // CheapTrick / D4C output rows: [n] device frame offsets (packed rows, utterance u's frame i at row f_off[u] + i), or
   // nullptr = padded rows (u * f_stride + i)
   const long long *f_off = nullptr;
+  // Packed inputs (the packed stage calls): [n] device sample offsets, utterance u's samples at x + x_off[u].  With them
+  // f_off ([n + 1], from 0) also places the input frames -- time_axis / f0 at f_off[u] + i -- and the stages' per-frame
+  // scratch follows the packed frames; f_off_host is its host copy.  nullptr = padded inputs (x_stride / f_stride).
+  const long long *x_off = nullptr;
+  const long long *f_off_host = nullptr;
 };
 
 // stage drivers (each: enqueue on ctx->stream, return 0 / error code)
@@ -352,6 +357,10 @@ struct StageRequest {   // brace-initialised in field order up to f0_stride
   bool coded = false;
   int dims = 0;
   int row_stride = 0;
+  // packed (per_utt): utterance u is samples [x_offsets[u], x_offsets[u + 1]) and frames [f_offsets[u], f_offsets[u + 1])
+  // (host arrays, n + 1 entries); the lengths and strides are not read, and row_stride 0 is the largest
+  // fft_size[u] / 2 + 1
+  const long long *x_offsets = nullptr, *f_offsets = nullptr;
 };
 // Everything a stage run reads besides the rows, made once per call and const afterwards.
 struct StagePlan {
@@ -363,13 +372,29 @@ struct StagePlan {
   std::vector<CodecTables> tables;  // coded: one per distinct fft_size, in order of first appearance
   int row = 0;                      // doubles per full output row
   bool nothing = false;             // coded D4C below 12 kHz: no bands, nothing to write (a NULL output is allowed)
+  std::vector<long long> x_off, f_off;   // packed: the request's offsets [n + 1]; empty: padded rows
 };
 // Every check of a stage call before anything is queued, in this order: n and fs; the stage's sampling-rate limits
 // (StoneMask: fs <= 48 kHz; D4C: its transforms within the on-chip FFT); each option (CheapTrick: fft_size a power of
 // two in [16, 8192], q1 finite; D4C: fft_size >= 4, threshold finite); row_stride; the codec tables of each distinct
-// fft_size; each utterance's x and f0 lengths (1 .. x_stride, 0 .. f0_stride).  EINVAL with last_error "<stage>: ...",
-// naming the first bad utterance where there is one.
+// fft_size; each utterance's x and f0 lengths (1 .. x_stride, 0 .. f0_stride; packed: the offsets start at 0 and give
+// each utterance 1 .. INT_MAX samples and 0 .. INT_MAX frames).  EINVAL with last_error "<stage>: ...", naming the first
+// bad utterance where there is one.
 int stage_plan(Ctx *ctx, const StageRequest &r, StagePlan *p);
+// The rule of packed offsets: off (host, n + 1) starts at 0 and every utterance spans least .. INT_MAX `unit`, filling
+// len [n]; "" when they are good, else the broken rule naming the first bad utterance.
+std::string packed_lengths(const char *name, const char *unit, int n, const long long *off, int least,
+                           std::vector<int> *len);
+// Scratch of the packed stage runs, by which the packed stage calls cut their utterances into chunks of at most the
+// scratch budget: per packed frame, CheapTrick's draw count and offset, and D4C's two counts, two offsets, selected
+// flag, frame-list entry and frame utterance (ct_launch and d4c_run check their layouts against these); per utterance,
+// their per-utterance arrays (totals, group indices, offsets, options); per chunk, the arrays' 256-byte alignment and
+// the codec tables.
+constexpr size_t WB_CT_FRAME_BYTES = 2 * sizeof(unsigned);
+constexpr size_t WB_D4C_FRAME_BYTES = 4 * sizeof(unsigned) + 1 + 2 * sizeof(int);
+constexpr size_t WB_STAGE_FRAME_BYTES = WB_CT_FRAME_BYTES > WB_D4C_FRAME_BYTES ? WB_CT_FRAME_BYTES : WB_D4C_FRAME_BYTES;
+constexpr size_t WB_STAGE_UTT_BYTES = 64;
+constexpr size_t WB_STAGE_CHUNK_BYTES = (size_t)1 << 20;
 // The stage over batch b, whose rows are the plan's utterances [u0, u0 + b.n) (its lengths uploaded from the plan's).
 // CheapTrick runs one launch sequence per distinct (fft_size, q1) among them, in order of first appearance; D4C one
 // launch sequence, with per-utterance device arrays when their options differ.  out: full or coded rows, as planned.

@@ -13,6 +13,8 @@ struct SmParams {
   const double *x; const int *x_len; int x_stride;
   const double *time_axis; const double *f0; const int *f_len; int f_stride;
   int fs; double *out; const double2 *tw;
+  // packed inputs: utterance u's samples at x + x_off[u], its frames (inputs and output) at f_off[u] + i; null: padded
+  const long long *x_off, *f_off;
 };
 
 // exp(-j 2 pi idx / WB_TW_N) for idx in [0, WB_TW_N)
@@ -72,7 +74,7 @@ WB_KERNEL(64, 8) stonemask_kernel(SmParams p) {
   const int tid = WB_TID, nth = WB_NTH;
   const int u = blockIdx.y, i = blockIdx.x;
   if (i >= p.f_len[u]) return;
-  const size_t fidx = (size_t)u * p.f_stride + i;
+  const size_t fidx = p.x_off ? (size_t)(p.f_off[u] + i) : (size_t)u * p.f_stride + i;
   const double f0 = p.f0[fidx];
   const int fs = p.fs;
   if (f0 <= 40.0 || f0 > fs / 12.0) {  // kFloorF0StoneMask, stonemask.cpp:187-188
@@ -87,7 +89,7 @@ WB_KERNEL(64, 8) stonemask_kernel(SmParams p) {
   const int lg_nfft = lg + 2, nfft = 1 << lg_nfft;
   const double T = (2.0 * h + 1.0) / fs;
   double *xw = smem, *xd = smem + nwin, *red = xd + nwin;
-  const double *x = p.x + (size_t)u * p.x_stride;
+  const double *x = p.x_off ? p.x + p.x_off[u] : p.x + (size_t)u * p.x_stride;
   const int x_len = p.x_len[u];
   for (int j = tid; j < nwin; j += nth) {
     // index_raw[j] = round((t + base_time[j]) * fs), base_time[j] = (j - h) / fs  (:24-28, :193-194)
@@ -136,6 +138,11 @@ int stonemask_run(Ctx *ctx, const Batch &b, double *refined_f0) {
   SmParams p;
   p.x = b.x; p.x_len = b.x_len; p.x_stride = b.x_stride; p.time_axis = b.time_axis; p.f0 = b.f0;
   p.f_len = b.f_len; p.f_stride = b.f_stride; p.fs = b.fs; p.out = refined_f0; p.tw = ctx->twiddle;
+  p.x_off = b.x_off; p.f_off = b.f_off;
+  if (b.x_off) {   // packed inputs: the packed stage call's chunks have at most 65535 utterances
+    WB_LAUNCH_COOP(stonemask_kernel, dim3((unsigned)b.max_f_len, (unsigned)b.n), 64, smem, ctx->stream, p);
+    return dev_check(ctx, "stonemask");
+  }
   for (int u0 = 0; u0 < b.n; u0 += 65535) {
     const int n = imin(65535, b.n - u0);
     SmParams q = p;

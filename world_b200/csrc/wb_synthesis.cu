@@ -578,29 +578,14 @@ int row_lengths(Ctx *ctx, const char *who, const char *rows, const int *lengths,
   return 0;
 }
 
-// Packed rows: utterance u is entries [off[u], off[u + 1]) of the `rows` arrays; out[u] = its count.  EINVAL "<who>:
-// <rows>_offsets[0] = v is not 0" or "<rows>_offsets gives utterance u v <what>, outside [least, INT_MAX] (utterance
-// u)" for the first one outside.
+// Packed rows: utterance u is entries [off[u], off[u + 1]) of the `rows` arrays; out[u] = its count.  The rule of
+// packed_lengths (wb_api.cu); EINVAL with last_error "<who>: " and its message for the first utterance that breaks it.
 int packed_lengths(Ctx *ctx, const char *who, const char *rows, const char *what, const long long *off, int n,
                    int least, std::vector<int> *out) {
-  char msg[256];
-  if (off[0] != 0) {
-    snprintf(msg, sizeof msg, "%s: %s_offsets[0] = %lld is not 0", who, rows, off[0]);
-    ctx->last_error = msg;
-    return WORLD_B200_EINVAL;
-  }
-  out->resize(n);
-  for (int u = 0; u < n; ++u) {
-    const long long v = off[u + 1] - off[u];
-    if (off[u + 1] < off[u] || v < least || v > INT_MAX) {
-      snprintf(msg, sizeof msg, "%s: %s_offsets gives utterance %d %lld %s, outside [%d, INT_MAX] (utterance %d)", who,
-               rows, u, off[u + 1] < off[u] ? off[u + 1] - off[u] : v, what, least, u);
-      ctx->last_error = msg;
-      return WORLD_B200_EINVAL;
-    }
-    (*out)[u] = (int)v;
-  }
-  return 0;
+  const std::string bad = packed_lengths((std::string(rows) + "_offsets").c_str(), what, n, off, least, out);
+  if (bad.empty()) return 0;
+  ctx->last_error = std::string(who) + ": " + bad;
+  return WORLD_B200_EINVAL;
 }
 
 int synthesis_plan(Ctx *ctx, const SynthesisRequest &r, const char *who, SynthesisPlan *p) {
