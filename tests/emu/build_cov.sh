@@ -3,7 +3,7 @@
 # say which lines and branches of the kernels a test run reached.  Usage:
 #   sh tests/emu/build_cov.sh /tmp/cov
 #   WB_EMU_LIB=/tmp/cov/libworld_b200_emu_cov.so python -m pytest tests/test_emu_f0_tail.py -q
-#   python tests/emu/cov_report.py /tmp/cov            # the F0 decision kernels; --all-functions FILE... for others
+#   python tests/emu/cov_report.py /tmp/cov            # the F0 decision kernels; FILE:FUNCTION,... for others
 # The counters (*.gcda) accumulate over runs in the output directory: remove them to start a new reading.
 set -e
 OUT=${1:-/tmp/cov}

@@ -3,10 +3,18 @@
 kernels and their device helpers, the source lines that never ran and the branches that were never taken.
 
     python tests/emu/cov_report.py /tmp/cov
+    python tests/emu/cov_report.py /tmp/cov wb_stonemask.cu:stonemask_kernel,sm_fix_f0 wb_spectral.cuh:dc_correction
+
+Without FILE:FUNCTION,... arguments it reports on the F0 decision kernels below.  A header's functions are compiled
+into every object that includes it: their counters are merged by source line (a line ran if it ran in any object) and
+by instantiation and branch (a template instantiation's branch was taken if it was taken in any object).
 
 An instrument for whoever tests or rewrites these kernels, not a gate: lines compiled out of the emulation (#ifndef
 WB_EMU) do not appear at all, and a branch gcov reports may be one the compiler made (a loop's entry test, the two
 halves of a && condition)."""
+import glob
+import gzip
+import json
 import os
 import re
 import subprocess
@@ -36,54 +44,79 @@ def function_spans(path, names):
     return spans
 
 
+def requested(args):
+    """FILE:FUNCTION,... arguments -> {file: [functions]}; none: FUNCTIONS"""
+    if not args:
+        return FUNCTIONS
+    req = {}
+    for a in args:
+        fname, _, names = a.partition(":")
+        if not names:
+            sys.exit(f"{a}: expected FILE:FUNCTION[,FUNCTION...]")
+        req.setdefault(fname, []).extend(names.split(","))
+    return req
+
+
+def counters(out, fname):
+    """The merged counters of source file fname over its own object (a .cu) or every object (a header):
+    ({line: count}, {(line, instantiation, branch index): count}), or None if no object has counters for it"""
+    stems = [fname[:-3]] if fname.endswith(".cu") else sorted(f[:-5] for f in os.listdir(out) if f.endswith(".gcda"))
+    lines, branches, found = {}, {}, False
+    for stem in stems:
+        if not os.path.exists(os.path.join(out, stem + ".gcda")):
+            continue
+        with tempfile.TemporaryDirectory() as tmp:
+            subprocess.check_call(["gcov", "--json-format", "-b", "-c", "-o", out, os.path.join(out, stem + ".o")],
+                                  cwd=tmp, stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
+            data = [json.load(gzip.open(f)) for f in glob.glob(os.path.join(tmp, "*.gcov.json.gz"))]
+        for d in data:
+            for entry in d["files"]:
+                if os.path.basename(entry["file"]) != fname:
+                    continue
+                found = True
+                names = {f["name"]: f["demangled_name"] for f in entry["functions"]}
+                for ln in entry["lines"]:
+                    n = ln["line_number"]
+                    lines[n] = lines.get(n, 0) + ln["count"]
+                    inst = names.get(ln.get("function_name", ""), ln.get("function_name", ""))
+                    for k, b in enumerate(ln["branches"]):
+                        key = (n, inst, k)
+                        branches[key] = branches.get(key, 0) + b["count"]
+    return (lines, branches) if found else None
+
+
 def main():
     out = os.path.abspath(sys.argv[1] if len(sys.argv) > 1 else "/tmp/cov")
     src = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "..", "world_b200", "csrc")
     total_lines = total_branches = 0
-    for fname, names in FUNCTIONS.items():
-        stem = fname[:-3]
-        if not os.path.exists(os.path.join(out, stem + ".gcda")):
+    for fname, names in requested(sys.argv[2:]).items():
+        got = counters(out, fname)
+        if got is None:
             print(f"{fname}: no counters in {out} (run something through WB_EMU_LIB first)")
             continue
-        with tempfile.TemporaryDirectory() as tmp:
-            subprocess.check_call(["gcov", "-b", "-c", "-o", out, os.path.join(out, stem + ".o")], cwd=tmp,
-                                  stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
-            text = open(os.path.join(tmp, fname + ".gcov")).read().split("\n")
+        lines, branches = got
+        text = open(os.path.join(src, fname)).read().split("\n")
         spans = function_spans(os.path.join(src, fname), names)
-        missed_lines, missed_branches, executable = {}, {}, {}
-        cur = None
-        for ln in text:
-            m = re.match(r"\s*([0-9#=\-*]+):\s*(\d+):(.*)", ln)
-            if m:
-                cur = int(m.group(2))
-                count = m.group(1).rstrip("*")
-                for name, (a, b) in spans.items():
-                    if a <= cur <= b and count != "-":
-                        executable[name] = executable.get(name, 0) + 1
-                        if count.startswith("#") or count.startswith("="):
-                            missed_lines.setdefault(name, []).append((cur, m.group(3).strip()))
-                continue
-            m = re.match(r"branch\s+(\d+) (never executed|taken (\d+))", ln)
-            if m and cur is not None and (m.group(2) == "never executed" or m.group(3) == "0"):
-                for name, (a, b) in spans.items():
-                    if a <= cur <= b:
-                        missed_branches.setdefault(name, []).append((cur, int(m.group(1))))
         for name in names:
             if name not in spans:
                 print(f"{fname}: {name} not found")
                 continue
-            ml, mb = missed_lines.get(name, []), missed_branches.get(name, [])
+            a, b = spans[name]
+            executable = sorted(n for n in lines if a <= n <= b)
+            ml = [n for n in executable if lines[n] == 0]
+            mb = {}
+            for (n, inst, k), c in sorted(branches.items()):
+                if a <= n <= b and c == 0:
+                    mb.setdefault((n, inst), []).append(k)
+            n_mb = sum(len(v) for v in mb.values())
             total_lines += len(ml)
-            total_branches += len(mb)
-            print(f"{fname} {name} (lines {spans[name][0]}-{spans[name][1]}): {executable.get(name, 0)} executable "
-                  f"lines, {len(ml)} never ran, {len(mb)} branch outcomes never taken")
-            for n, t in ml:
-                print(f"    line {n} never ran: {t}")
-            by_line = {}
-            for n, b in mb:
-                by_line.setdefault(n, []).append(b)
-            for n in sorted(by_line):
-                print(f"    line {n}: branch {', '.join(map(str, by_line[n]))} never taken")
+            total_branches += n_mb
+            print(f"{fname} {name} (lines {a}-{b}): {len(executable)} executable lines, {len(ml)} never ran, "
+                  f"{n_mb} branch outcomes never taken")
+            for n in ml:
+                print(f"    line {n} never ran: {text[n - 1].strip()}")
+            for (n, inst), ks in sorted(mb.items()):
+                print(f"    line {n}: branch {', '.join(map(str, ks))} never taken" + (f" in {inst}" if inst else ""))
     print(f"total: {total_lines} lines never ran, {total_branches} branch outcomes never taken")
 
 

@@ -52,7 +52,10 @@ WB_DEV void dc_correction(double *spec, double f0, int fs, int fft_size, double 
   const int tid = WB_TID, nth = WB_NTH;
   // f0 is caller supplied: at or above fs/2 (or non-finite) the reference indexes past its arrays.  Here such a
   // value is clamped two bins below the Nyquist bin -- every index stays inside the fft_size/2 + 1 values of
-  // `spec`; the row is meaningless either way, but there is no fault.  No effect on any f0 the reference accepts.
+  // `spec`; the row is meaningless either way, but there is no fault.  The reference stays in bounds up to one bin
+  // below Nyquist, so between two and one bin below it the clamp would move the interpolation's origin -- but no such
+  // row is kept: both callers' linear_smoothing then refuses the frame (status 2), as it does every f0 above 3/8 fs
+  // (CheapTrick) or fs/4 (D4C).
   f0 = dmin(dmax(f0, 0.0), (0.5 - 2.0 / fft_size) * fs);
   const int upper_limit = 2 + static_cast<int>(f0 * fft_size / fs);
   const int n_rep = upper_limit - 1;
@@ -81,9 +84,13 @@ WB_DEV bool linear_smoothing(const double *in, double width, int fs, int fft_siz
                              double *seg, double *red_big) {
   const int tid = WB_TID, nth = WB_NTH;
   const int half = fft_size / 2;
-  const int boundary = static_cast<int>(width * fft_size / fs) + 1;
+  // a caller-supplied f0 makes the width anything, infinite included: it is tested before the conversion to int
+  // (boundary > half exactly when width * fft_size / fs >= half), which would otherwise wrap round into range
+  const double b = width * fft_size / fs;
+  if (!(b < half)) return false;
+  const int boundary = static_cast<int>(b) + 1;
   const int n_ext = half + boundary * 2 + 1;
-  if (boundary > half || n_ext > smoothing_capacity(fft_size)) return false;
+  if (n_ext > smoothing_capacity(fft_size)) return false;
 
   const double inv_n = 1.0 / fft_size;          // exact: fft_size is a power of two
   // mirror-extend and scale:  seg[i] = ext[i] * fs / fft_size   (common.cpp:30-41)
