@@ -705,6 +705,27 @@ int world_b200_modify_packed(WorldB200 *ctx, double *f0, int n_utts, const long 
                              int row_stride, const int *fft_sizes, int fs, const double *f0_scale,
                              const double *spectral_ratio);
 
+/* ---- pitch and formant curves: one f0 factor and one spectral ratio per FRAME ---------------------------------------
+ * Frame i of an utterance is modified exactly as ParameterModification (test.cpp:221-258) modifies a one-frame
+ * spectrogram with shift = f0_curve[i] and ratio = spectral_ratio_curve[i] at the utterance's fft_size.  The curves are
+ * DEVICE arrays laid out as f0: [n_utts][f0_stride] for world_b200_modify_curves, [F] at f_offsets for
+ * world_b200_modify_curves_packed; either may be NULL, which skips that half.  Rows, lengths, sizes and row_stride are
+ * those of world_b200_modify_batch_options / world_b200_modify_packed (fft_sizes may be NULL without a ratio curve).
+ * Constant curves (curve[i] = factor[u] on every frame of utterance u) give world_b200_modify_batch_options /
+ * world_b200_modify_packed's result with those factors, bit for bit.  Writes nothing outside the utterances' frames
+ * (frames [0, F) packed), nor past an utterance's fft_size / 2 + 1 in a row.
+ * Validation, before any modification is queued (WORLD_B200_EINVAL, world_b200_last_error() naming the curve, index,
+ * utterance, frame and value; the rows are unchanged): the rules of the factor calls, and per frame an f0 factor that is
+ * not finite and > 0, or a ratio that is not finite and > 0 or has (int)(fft_size / 2.0 * ratio) < 1.  The curves are
+ * checked where they are, on the device, by one small kernel: these calls synchronise the stream once.  n_utts == 0
+ * returns 0. */
+int world_b200_modify_curves(WorldB200 *ctx, double *f0, const int *f0_lengths, int n_utts, int f0_stride,
+                             double *spectrogram, int row_stride, const int *fft_sizes, int fs, const double *f0_curve,
+                             const double *spectral_ratio_curve);
+int world_b200_modify_curves_packed(WorldB200 *ctx, double *f0, int n_utts, const long long *f_offsets,
+                                    double *spectrogram, int row_stride, const int *fft_sizes, int fs,
+                                    const double *f0_curve, const double *spectral_ratio_curve);
+
 /* The stage calls on packed batches (DEVICE arrays), for callers who bring their own F0 or rows.  x_offsets and
  * f_offsets are HOST arrays of n_utts + 1 offsets, each starting at 0: utterance u is samples
  * [x_offsets[u], x_offsets[u + 1]) of x (1 .. INT_MAX of them) and frames [f_offsets[u], f_offsets[u + 1]) of time_axis,
@@ -858,6 +879,27 @@ int world_b200_transform_host_packed(WorldB200 *ctx, const void *x, int nbit, in
                                      const CheapTrickOption *cheaptrick_options, const D4COption *d4c_options,
                                      const double *f0_scale, const double *spectral_ratio, const double *time_scale,
                                      int nbit_out, void *y, long long *y_offsets);
+/* world_b200_transform_packed / world_b200_transform_host_packed with pitch and formant curves in place of f0_scale and
+ * spectral_ratio (time_scale stays one factor per utterance).  The curves are on the analysis frame grid: [F] frames at
+ * the offsets world_b200_packed_frames(fs, n_utts, x_offsets, frame_period) gives for the F0 method's frame_period;
+ * DEVICE arrays for world_b200_transform_packed_curves, HOST arrays for world_b200_transform_host_packed_curves (each
+ * chunk's curve frames go up as one copy beside its samples).  Either may be NULL.  Every utterance's output equals,
+ * bit for bit, world_b200_analyze_packed -> world_b200_modify_curves_packed -> world_b200_synthesis_packed at
+ * frame_period * time_scale[u]; with constant curves it equals world_b200_transform_packed with those factors.
+ * Validation adds the per-frame rules of world_b200_modify_curves to the packed transform's, before any work is queued;
+ * the device call checks its curves with one kernel and one synchronisation. */
+int world_b200_transform_packed_curves(WorldB200 *ctx, const void *x, int nbit, int n_utts, const long long *x_offsets,
+                                       int fs, const WorldB200AnalysisOption *option,
+                                       const HarvestOption *harvest_options, const DioOption *dio_options,
+                                       const CheapTrickOption *cheaptrick_options, const D4COption *d4c_options,
+                                       const double *f0_curve, const double *spectral_ratio_curve,
+                                       const double *time_scale, int nbit_out, void *y, long long *y_offsets);
+int world_b200_transform_host_packed_curves(WorldB200 *ctx, const void *x, int nbit, int n_utts,
+                                            const long long *x_offsets, int fs, const WorldB200AnalysisOption *option,
+                                            const HarvestOption *harvest_options, const DioOption *dio_options,
+                                            const CheapTrickOption *cheaptrick_options, const D4COption *d4c_options,
+                                            const double *f0_curve, const double *spectral_ratio_curve,
+                                            const double *time_scale, int nbit_out, void *y, long long *y_offsets);
 
 #ifdef __cplusplus
 }

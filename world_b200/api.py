@@ -172,6 +172,8 @@ ABI = {
     "world_b200_synthesis_coded_host_packed": (C.c_int, [_P, _P, C.c_int, _LP, _P, C.c_int, _P, _IP, C.c_double,
                                                          C.c_int, _LP, _P, _P, C.c_int, _P]),
     "world_b200_modify_packed": (C.c_int, [_P, _P, C.c_int, _LP, _P, C.c_int, _IP, C.c_int, _P, _P]),
+    "world_b200_modify_curves": (C.c_int, [_P, _P, _IP, C.c_int, C.c_int, _P, C.c_int, _IP, C.c_int, _P, _P]),
+    "world_b200_modify_curves_packed": (C.c_int, [_P, _P, C.c_int, _LP, _P, C.c_int, _IP, C.c_int, _P, _P]),
     "world_b200_comm_unique_id": (C.c_int, [_P, C.c_int]),
     "world_b200_comm_init": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int]),
     "world_b200_comm_destroy": (C.c_int, [_P]),
@@ -267,6 +269,14 @@ ABI = {
                                                    C.POINTER(HarvestOption), C.POINTER(DioOption),
                                                    C.POINTER(CheapTrickOption), C.POINTER(D4COption), _P, _P, _P,
                                                    C.c_int, _P, _LP]),
+    "world_b200_transform_packed_curves": (C.c_int, [_P, _P, C.c_int, C.c_int, _LP, C.c_int,
+                                                     C.POINTER(AnalysisOption), C.POINTER(HarvestOption),
+                                                     C.POINTER(DioOption), C.POINTER(CheapTrickOption),
+                                                     C.POINTER(D4COption), _P, _P, _P, C.c_int, _P, _LP]),
+    "world_b200_transform_host_packed_curves": (C.c_int, [_P, _P, C.c_int, C.c_int, _LP, C.c_int,
+                                                          C.POINTER(AnalysisOption), C.POINTER(HarvestOption),
+                                                          C.POINTER(DioOption), C.POINTER(CheapTrickOption),
+                                                          C.POINTER(D4COption), _P, _P, _P, C.c_int, _P, _LP]),
     "world_b200_stonemask_packed": (C.c_int, [_P, _P, C.c_int, _LP, C.c_int, _P, _P, _LP, _P]),
     "world_b200_cheaptrick_packed": (C.c_int, [_P, _P, C.c_int, _LP, C.c_int, _P, _P, _LP, C.POINTER(CheapTrickOption),
                                                C.c_int, _P]),
@@ -460,6 +470,22 @@ def _fft_sizes(fft_size, n):
     if len(sizes) != n:
         raise ValueError(f"{len(sizes)} fft sizes for {n} utterances")
     return (C.c_int * max(n, 1))(*[int(v) for v in sizes])
+
+
+def _curve_sizes(fft_size, n):
+    """One size, or a sequence of n sizes -> a ctypes int array of one size per utterance."""
+    sizes = _fft_sizes(fft_size, n)
+    return (C.c_int * max(n, 1))(*([int(fft_size)] * n)) if sizes is None else sizes
+
+
+def _curve(c):
+    """A curve of float64 factors in its array's memory (tensor or numpy array, contiguous) -> its address, or None."""
+    if c is None:
+        return None
+    tensor = hasattr(c, "data_ptr")
+    if str(c.dtype) not in ("float64", "torch.float64") or not (c.is_contiguous() if tensor else c.flags.c_contiguous):
+        raise ValueError("a curve: a contiguous float64 array")
+    return c.data_ptr() if tensor else c.ctypes.data
 
 
 class World:
@@ -1077,6 +1103,36 @@ class World:
             _factors(spectral_ratio, n, "spectral_ratio")))
         return f0, spectrogram
 
+    # -- pitch and formant curves: one f0 factor and one spectral ratio per frame -----------------------------------
+    def modify_curves(self, f0, spectrogram, fs, fft_size, f0_curve=None, spectral_ratio_curve=None, f0_lengths=None):
+        """modify with one factor per FRAME in place (world_b200_modify_curves): f0 [n, L] *= f0_curve [n, L], and
+        frame i of utterance u's envelope [n, L, W] is stretched by spectral_ratio_curve[u, i] at fft_size (one int, or
+        one per utterance; W >= every fft_size // 2 + 1).  The curves are arrays on the rows' device (either may be
+        None, which leaves that half alone).  The call checks every frame of the curves on the device before it
+        modifies anything, and so synchronises the stream once.  Returns (f0, spectrogram)."""
+        rows = f0 if f0 is not None else spectrogram
+        n, L = int(rows.shape[0]), int(rows.shape[1])
+        fl, k1 = _int_array(f0_lengths, n)
+        sizes = _curve_sizes(fft_size, n)
+        row = int(spectrogram.shape[-1]) if spectrogram is not None else 0
+        self._use_current_stream()
+        self._check(self.lib.world_b200_modify_curves(self._h, _ptr(f0), fl, n, L, _ptr(spectrogram), row, sizes, fs,
+                                                      _curve(f0_curve), _curve(spectral_ratio_curve)))
+        return f0, spectrogram
+
+    def modify_curves_packed(self, f0, spectrogram, f_offsets, fs, fft_size=None, f0_curve=None,
+                             spectral_ratio_curve=None):
+        """modify_curves on PACKED rows in place (world_b200_modify_curves_packed): f0 [F], spectrogram [F, W] and the
+        curves [F] on the rows' device, utterance u being frames [f_offsets[u], f_offsets[u + 1]).  fft_size (one int
+        or one per utterance) is needed with spectral_ratio_curve.  Returns (f0, spectrogram)."""
+        n, fo = _offsets(f_offsets)
+        sizes = None if fft_size is None else _curve_sizes(fft_size, n)
+        row = int(spectrogram.shape[-1]) if spectrogram is not None else 0
+        self._use_current_stream()
+        self._check(self.lib.world_b200_modify_curves_packed(self._h, _ptr(f0), n, fo, _ptr(spectrogram), row, sizes,
+                                                             fs, _curve(f0_curve), _curve(spectral_ratio_curve)))
+        return f0, spectrogram
+
     # -- the stage calls on packed batches: utterance u = samples [x_offsets[u], x_offsets[u + 1]) of x and frames
     #    [f_offsets[u], f_offsets[u + 1]) of time_axis, f0 and the rows ------------------------------------------------
     def _stage_packed(self, entry, x, x_offsets, fs, time_axis, f0, f_offsets, options, out):
@@ -1496,7 +1552,7 @@ class World:
         return np.array(y[:], dtype=np.int64)
 
     def _transform_packed(self, name, x, nbit, x_offsets, fs, option, f0_scale, spectral_ratio, time_scale,
-                          harvest_options, dio_options, cheaptrick_options, d4c_options, dtype, y, host):
+                          harvest_options, dio_options, cheaptrick_options, d4c_options, dtype, y, host, curves=None):
         """Calls world_b200_<name> on a packed batch: (y [Y], y_offsets as numpy int64), y allocated when None (device:
         on x's device; host: numpy)."""
         import numpy as np
@@ -1526,10 +1582,13 @@ class World:
             xp, yp = _ptr(x), _ptr(y)
             self._use_current_stream()
         got = (C.c_longlong * (n + 1))()
+        if curves is None:
+            pitch, formant = _factors(f0_scale, n, "f0_scale"), _factors(spectral_ratio, n, "spectral_ratio")
+        else:
+            pitch, formant = curves
         self._check(getattr(self.lib, f"world_b200_{name}")(
-            self._h, xp, nbit, n, xo, fs, C.byref(option), per_utt, per_dio, ct, d4, _factors(f0_scale, n, "f0_scale"),
-            _factors(spectral_ratio, n, "spectral_ratio"), _factors(time_scale, n, "time_scale"), 16 if pcm16 else 0,
-            yp, got))
+            self._h, xp, nbit, n, xo, fs, C.byref(option), per_utt, per_dio, ct, d4, pitch, formant,
+            _factors(time_scale, n, "time_scale"), 16 if pcm16 else 0, yp, got))
         return y, np.array(got[:], dtype=np.int64)
 
     def transform_packed(self, x, nbit, x_offsets, fs, option: AnalysisOption, f0_scale=None, spectral_ratio=None,
@@ -1555,6 +1614,32 @@ class World:
         return self._transform_packed("transform_host_packed", x, nbit, x_offsets, fs, option, f0_scale,
                                       spectral_ratio, time_scale, harvest_options, dio_options, cheaptrick_options,
                                       d4c_options, dtype, out, host=True)
+
+    def transform_packed_curves(self, x, nbit, x_offsets, fs, option: AnalysisOption, f0_curve=None,
+                                spectral_ratio_curve=None, time_scale=None, harvest_options=None, dio_options=None,
+                                cheaptrick_options=None, d4c_options=None, dtype=None, y=None):
+        """transform_packed with pitch and formant curves (world_b200_transform_packed_curves): f0_curve and
+        spectral_ratio_curve are [F] DEVICE arrays of one factor per analysis frame, at the frame offsets
+        packed_frames(fs, x_offsets, frame_period) gives (either may be None); time_scale stays one per utterance.
+        Every utterance's output equals analyze_packed -> modify_curves_packed -> synthesis_packed at
+        frame_period * time_scale[u], bit for bit.  Returns (y [Y], y_offsets) as transform_packed."""
+        return self._transform_packed("transform_packed_curves", x, nbit, x_offsets, fs, option, None, None,
+                                      time_scale, harvest_options, dio_options, cheaptrick_options, d4c_options, dtype,
+                                      y, host=False, curves=(_curve(f0_curve), _curve(spectral_ratio_curve)))
+
+    def transform_host_packed_curves(self, x, nbit, x_offsets, fs, option: AnalysisOption, f0_curve=None,
+                                     spectral_ratio_curve=None, time_scale=None, harvest_options=None,
+                                     dio_options=None, cheaptrick_options=None, d4c_options=None, dtype=None,
+                                     out=None):
+        """transform_packed_curves for HOST arrays (world_b200_transform_host_packed_curves): x, out and the [F]
+        curves are host arrays (numpy or CPU tensors); each chunk's curve frames go up beside its samples.  Returns
+        (y [Y], y_offsets) as transform_host_packed."""
+        import numpy as np
+        keep = [None if c is None else np.ascontiguousarray(c.numpy() if hasattr(c, "numpy") else c,
+                                                            dtype=np.float64) for c in (f0_curve, spectral_ratio_curve)]
+        return self._transform_packed("transform_host_packed_curves", x, nbit, x_offsets, fs, option, None, None,
+                                      time_scale, harvest_options, dio_options, cheaptrick_options, d4c_options, dtype,
+                                      out, host=True, curves=tuple(_ptr(c) for c in keep))
 
     def analyze_coded_batch_allgather(self, x, nbit, fs, option: AnalysisOption, number_of_dimensions, time_axis_full,
                                       f0_full, coded_sp_full, coded_ap_full, x_lengths=None, harvest_options=None,

@@ -1411,7 +1411,7 @@ static int lane_error(WorldB200 *h, WorldB200 *L, int e) {
 // utterance (what the F0 stage reads), then its packed f0, spectrogram and aperiodicity frames (what CheapTrick and D4C
 // write and modification and synthesis read), so one long utterance only lengthens the rows of its own slice.
 static int transform_packed_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, const void *x, int u0,
-                                int n, void *y) {
+                                int n, void *y, const ModifyCurves *cv) {
   const ChainPlan &p = tp.chain;
   const long long *xo = r.x_offsets, *fo = p.f_off.data(), *yo = tp.syn.y_off.data();
   const size_t row = p.sp_row, out_bytes = tp.syn.nbit ? 2 : 8;
@@ -1467,6 +1467,13 @@ static int transform_packed_run(WorldB200 *h, const ChainRequest &r, const Trans
     }
     if (!e && tp.syn.modify)
       e = modify_run(lc, tp.syn.mod, a, m, p.f_len.data() + a, 0, (int)row, f0, sp, offs.data() + m + 1);
+    if (!e && cv) {   // the slice's curve frames, read at fo[a]
+      const long long d = fo[a] - fo[u0];
+      ModifyCurves sc;
+      sc.f0 = cv->f0 ? cv->f0 + d : nullptr; sc.ratio = cv->ratio ? cv->ratio + d : nullptr;
+      e = curves_run(lc, sc, m, p.f_len.data() + a, 0, offs.data() + m + 1, p.ct.fft_size.data() + a, r.fs, (int)row,
+                     f0, sp);
+    }
     return lane_error(h, L, e);
   };
   auto synthesise = [&](const LaneScope &lanes, int s) {
@@ -1488,9 +1495,10 @@ static int transform_packed_run(WorldB200 *h, const ChainRequest &r, const Trans
 // spectrogram, aperiodicity) live from its analysis to its synthesis in one buffer per lane, taken from the lane's pool
 // and sized for its largest slice; slices are sized so that the buffer takes at most about half the lane's scratch
 // budget, leaving the rest to the stages.
-int transform_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, const void *x, int u0, int n, void *y) {
+int transform_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, const void *x, int u0, int n, void *y,
+                  const ModifyCurves *cv) {
   if (n <= 0) return 0;
-  if (r.packed) return transform_packed_run(h, r, tp, x, u0, n, y);
+  if (r.packed) return transform_packed_run(h, r, tp, x, u0, n, y, cv);
   const ChainPlan &p = tp.chain;
   const int f0_stride = p.f0_stride, x_stride = r.x_stride, nbit = r.nbit, row = (int)p.sp_row;
   const size_t in_row = (size_t)x_stride * (nbit ? nbit / 8 : 8);
@@ -1610,11 +1618,16 @@ int world_b200_transform_packed_samples(int fs, int n_utts, const long long *x_o
   return 0;
 }
 
-int world_b200_transform_packed(WorldB200 *h, const void *x, int nbit, int n_utts, const long long *x_offsets, int fs,
-                                const WorldB200AnalysisOption *option, const HarvestOption *harvest_options,
-                                const DioOption *dio_options, const CheapTrickOption *cheaptrick_options,
-                                const D4COption *d4c_options, const double *f0_scale, const double *spectral_ratio,
-                                const double *time_scale, int nbit_out, void *y, long long *y_offsets) {
+}  // extern "C"
+
+// world_b200_transform_packed, and with cv (factors null) world_b200_transform_packed_curves: the curves are checked
+// on the device after every host check, before any work is queued
+static int transform_packed(WorldB200 *h, const void *x, int nbit, int n_utts, const long long *x_offsets, int fs,
+                            const WorldB200AnalysisOption *option, const HarvestOption *harvest_options,
+                            const DioOption *dio_options, const CheapTrickOption *cheaptrick_options,
+                            const D4COption *d4c_options, const double *f0_scale, const double *spectral_ratio,
+                            const double *time_scale, int nbit_out, void *y, long long *y_offsets,
+                            const ModifyCurves *cv) {
   if (!h) return WORLD_B200_EINVAL;
   if (n_utts == 0) {   // as the packed synthesis calls: nothing to check against, nothing to queue
     if (y_offsets) y_offsets[0] = 0;
@@ -1625,10 +1638,36 @@ int world_b200_transform_packed(WorldB200 *h, const void *x, int nbit, int n_utt
                                   cheaptrick_options, d4c_options, nullptr, nullptr, nullptr, nullptr);
   r.transform = true;
   TransformPlan tp;
-  const int rc = transform_check(h, r, f0_scale, spectral_ratio, time_scale, nbit_out, y, 0, "transform_packed", &tp);
+  const char *who = cv ? "transform_packed_curves" : "transform_packed";
+  int rc = transform_check(h, r, f0_scale, spectral_ratio, time_scale, nbit_out, y, 0, who, &tp);
+  const ChainPlan &p = tp.chain;
+  if (!rc && cv) rc = curves_check(&h->c, who, *cv, n_utts, p.f_len.data(), 0, p.f_off.data(), p.ct.fft_size.data());
   if (rc) return rc;
   if (y_offsets) std::copy(tp.syn.y_off.begin(), tp.syn.y_off.end(), y_offsets);
-  return transform_run(h, r, tp, x, 0, n_utts, y);
+  return transform_run(h, r, tp, x, 0, n_utts, y, cv);
+}
+
+extern "C" {
+
+int world_b200_transform_packed(WorldB200 *h, const void *x, int nbit, int n_utts, const long long *x_offsets, int fs,
+                                const WorldB200AnalysisOption *option, const HarvestOption *harvest_options,
+                                const DioOption *dio_options, const CheapTrickOption *cheaptrick_options,
+                                const D4COption *d4c_options, const double *f0_scale, const double *spectral_ratio,
+                                const double *time_scale, int nbit_out, void *y, long long *y_offsets) {
+  return transform_packed(h, x, nbit, n_utts, x_offsets, fs, option, harvest_options, dio_options, cheaptrick_options,
+                          d4c_options, f0_scale, spectral_ratio, time_scale, nbit_out, y, y_offsets, nullptr);
+}
+
+int world_b200_transform_packed_curves(WorldB200 *h, const void *x, int nbit, int n_utts, const long long *x_offsets,
+                                       int fs, const WorldB200AnalysisOption *option,
+                                       const HarvestOption *harvest_options, const DioOption *dio_options,
+                                       const CheapTrickOption *cheaptrick_options, const D4COption *d4c_options,
+                                       const double *f0_curve, const double *spectral_ratio_curve,
+                                       const double *time_scale, int nbit_out, void *y, long long *y_offsets) {
+  ModifyCurves cv;
+  cv.f0 = f0_curve; cv.ratio = spectral_ratio_curve;
+  return transform_packed(h, x, nbit, n_utts, x_offsets, fs, option, harvest_options, dio_options, cheaptrick_options,
+                          d4c_options, nullptr, nullptr, time_scale, nbit_out, y, y_offsets, &cv);
 }
 
 // ---- multi-GPU (SURVEY.md 8e): utterances sharded over ranks, outputs reassembled on every rank by NCCL

@@ -137,7 +137,9 @@ struct TransformPlan {
 int transform_check(WorldB200 *h, const ChainRequest &r, const double *f0_scale, const double *spectral_ratio,
                     const double *time_scale, int nbit_out, void *y, int y_stride, const char *who, TransformPlan *tp);
 // Utterances [u0, u0 + n) of a checked call: x and y point at utterance u0's rows (device); packed: at its first sample
-// of x and of y.
-int transform_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, const void *x, int u0, int n, void *y);
+// of x and of y.  cv (packed only, checked curves): DEVICE curves on the analysis frames, at utterance u0's first frame;
+// each slice's frames are modified by curves_run in place of modify_run.
+int transform_run(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, const void *x, int u0, int n, void *y,
+                  const ModifyCurves *cv = nullptr);
 
 }  // namespace wb

@@ -617,19 +617,24 @@ int transform_pipeline(WorldB200 *h, const ChainRequest &r, const TransformPlan 
 // input and two output buffers would take more than a sixth of the scratch budget).  Chunk k's samples
 // [x_offsets[c0], x_offsets[c1]) go up as one copy, transform_run transforms them, and its samples [y_off[c0],
 // y_off[c1]) come back as one copy; every sample of a chunk is written, so nothing is zeroed.
-int transform_packed_pipeline(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, void *y) {
+// cv: HOST curves on the analysis frames (world_b200_transform_host_packed_curves); each chunk's curve frames
+// [f_off[c0], f_off[c1]) go up as one copy per curve after its samples, in the same input buffer.
+int transform_packed_pipeline(WorldB200 *h, const ChainRequest &r, const TransformPlan &tp, void *y,
+                              const ModifyCurves *cv = nullptr) {
   Ctx *ctx = &h->c;
   const int n_utts = r.n;
-  const long long *xo = r.x_offsets, *yo = tp.syn.y_off.data();
+  const long long *xo = r.x_offsets, *yo = tp.syn.y_off.data(), *fo = tp.chain.f_off.data();
   const size_t in_bytes = r.nbit ? (size_t)(r.nbit / 8) : 8, out_bytes = tp.syn.nbit ? 2 : 8;
+  const size_t curve_bytes = cv ? 8 * ((cv->f0 ? 1 : 0) + (cv->ratio ? 1 : 0)) : 0;   // per frame
   int most = 512;
   if (const char *e = getenv("WB_HOST_CHUNK")) most = atoi(e) > 0 ? atoi(e) : most;
   const size_t cap = ctx->scratch_budget / 6;
   auto bytes = [&](int c0, int c1) {
-    return 2 * ((size_t)(xo[c1] - xo[c0]) * in_bytes + (size_t)(yo[c1] - yo[c0]) * out_bytes);
+    return 2 * ((size_t)(xo[c1] - xo[c0]) * in_bytes + (size_t)(yo[c1] - yo[c0]) * out_bytes +
+                (size_t)(fo[c1] - fo[c0]) * curve_bytes);
   };
   std::vector<int> bounds{0};
-  size_t most_in = 0, most_out = 0;
+  size_t most_in = 0, most_out = 0, most_frames = 0;
   while (bounds.back() < n_utts) {
     const int c0 = bounds.back();
     int c1 = c0 + 1;
@@ -637,17 +642,30 @@ int transform_packed_pipeline(WorldB200 *h, const ChainRequest &r, const Transfo
     bounds.push_back(c1);
     most_in = std::max(most_in, (size_t)(xo[c1] - xo[c0]) * in_bytes);
     most_out = std::max(most_out, (size_t)(yo[c1] - yo[c0]) * out_bytes);
+    most_frames = std::max(most_frames, (size_t)(fo[c1] - fo[c0]));
   }
-  // chunk k's samples, one copy
+  ArenaPlan in_plan;
+  in_plan.add(most_in);
+  const size_t o_f0 = in_plan.add(cv && cv->f0 ? most_frames * 8 : 0);
+  const size_t o_ratio = in_plan.add(cv && cv->ratio ? most_frames * 8 : 0);
+  // chunk k's samples, one copy, and its frames of each curve, one copy each
   auto upload = [&](HostPipe &p, int u0, int m, unsigned char *d) {
     p.h2d(d, (const unsigned char *)r.x + (size_t)xo[u0] * in_bytes, (size_t)(xo[u0 + m] - xo[u0]) * in_bytes);
+    const size_t frames = (size_t)(fo[u0 + m] - fo[u0]);
+    if (cv && cv->f0) p.h2d(d + o_f0, cv->f0 + fo[u0], frames * 8);
+    if (cv && cv->ratio) p.h2d(d + o_ratio, cv->ratio + fo[u0], frames * 8);
   };
   auto run = [&](int u0, int m, unsigned char *d, unsigned char *out) {
-    return transform_run(h, r, tp, d, u0, m, out);
+    if (!cv) return transform_run(h, r, tp, d, u0, m, out);
+    ModifyCurves dc;
+    dc.f0 = cv->f0 ? (const double *)(d + o_f0) : nullptr;
+    dc.ratio = cv->ratio ? (const double *)(d + o_ratio) : nullptr;
+    return transform_run(h, r, tp, d, u0, m, out, &dc);
   };
   auto out_at = [&](int u) { return (size_t)yo[u] * out_bytes; };
   auto zero = [](int, int) { return false; };
-  return chunk_pipeline(h, "transform_packed", bounds, 2, most_in, most_out, out_at, zero, tp.syn.nbit, y, upload, run);
+  return chunk_pipeline(h, "transform_packed", bounds, 2, in_plan.total, most_out, out_at, zero, tp.syn.nbit, y, upload,
+                        run);
 }
 
 // world_b200_synthesis_coded_host and, with f0_scale / spectral_ratio, world_b200_synthesis_coded_host_modified: every
@@ -782,6 +800,36 @@ extern "C" int world_b200_transform_host_packed(WorldB200 *h, const void *x, int
   if (rc) return rc;
   if (y_offsets) std::copy(tp.syn.y_off.begin(), tp.syn.y_off.end(), y_offsets);
   return transform_packed_pipeline(h, r, tp, y);
+}
+
+extern "C" int world_b200_transform_host_packed_curves(WorldB200 *h, const void *x, int nbit, int n_utts,
+                                                       const long long *x_offsets, int fs,
+                                                       const WorldB200AnalysisOption *option,
+                                                       const HarvestOption *harvest_options,
+                                                       const DioOption *dio_options,
+                                                       const CheapTrickOption *cheaptrick_options,
+                                                       const D4COption *d4c_options, const double *f0_curve,
+                                                       const double *spectral_ratio_curve, const double *time_scale,
+                                                       int nbit_out, void *y, long long *y_offsets) {
+  if (!h) return WORLD_B200_EINVAL;
+  if (n_utts == 0) {
+    if (y_offsets) y_offsets[0] = 0;
+    return 0;
+  }
+  DeviceGuard guard_(&h->c);
+  ChainRequest r = packed_request(x, nbit, n_utts, x_offsets, fs, option, harvest_options, dio_options,
+                                  cheaptrick_options, d4c_options, nullptr, nullptr, nullptr, nullptr);
+  r.transform = true;
+  TransformPlan tp;
+  const char *who = "transform_host_packed_curves";
+  ModifyCurves cv;
+  cv.f0 = f0_curve; cv.ratio = spectral_ratio_curve;
+  int rc = transform_check(h, r, nullptr, nullptr, time_scale, nbit_out, y, 0, who, &tp);
+  const ChainPlan &p = tp.chain;
+  if (!rc) rc = curves_check_host(&h->c, who, cv, n_utts, p.f_len.data(), 0, p.f_off.data(), p.ct.fft_size.data());
+  if (rc) return rc;
+  if (y_offsets) std::copy(tp.syn.y_off.begin(), tp.syn.y_off.end(), y_offsets);
+  return transform_packed_pipeline(h, r, tp, y, &cv);
 }
 
 extern "C" int world_b200_analyze_host(WorldB200 *h, const double *x, int n_utts, int x_stride,

@@ -238,6 +238,23 @@ void modify_stretch_launch(Ctx *ctx, const ModifyDevice &d, int row, int max_bin
 int modify_run(Ctx *ctx, const ModifyPlan &plan, int u0, int n_utts, const int *f0_lengths, int f0_stride, int row,
                double *f0, double *spectrogram, const long long *f_offsets = nullptr);
 
+// Pitch and formant curves: one f0 factor and one spectral ratio per frame, laid out as the frames' rows (padded
+// [n][f_stride], or packed [F] at the frame offsets).  Either may be null (that half is not modified).
+struct ModifyCurves { const double *f0 = nullptr, *ratio = nullptr; };
+// modify_plan's rule for every frame < f_len[u] of each curve (ratio: at fft_sizes[u]), on DEVICE curves: one check
+// kernel and one read-back, so ctx->stream is synchronised.  Host lengths, sizes and offsets (f_off [n_utts + 1]: packed
+// rows; null: padded rows of f_stride).  EINVAL with last_error "<who>: f0_curve[i] = v (utterance u, frame f) ..." for
+// the first bad frame of the first bad curve; nothing is modified.
+int curves_check(Ctx *ctx, const char *who, const ModifyCurves &cv, int n_utts, const int *f_len, int f_stride,
+                 const long long *f_off, const int *fft_sizes);
+// The same rule on HOST curves
+int curves_check_host(Ctx *ctx, const char *who, const ModifyCurves &cv, int n_utts, const int *f_len, int f_stride,
+                      const long long *f_off, const int *fft_sizes);
+// Both halves on the device rows in place (checked curves; the layout of curves_check, row doubles per envelope frame):
+// modify_curve_f0_kernel and modify_curve_stretch_kernel, enqueued on ctx->stream.
+int curves_run(Ctx *ctx, const ModifyCurves &cv, int n_utts, const int *f_len, int f_stride, const long long *f_off,
+               const int *fft_sizes, int fs, int row, double *f0, double *spectrogram);
+
 // out[u] = lengths[u] (NULL: stride) for u < n; EINVAL "<who>: <rows>_lengths[u] = v is outside [least, <rows>_stride =
 // stride] (utterance u)" for the first one outside
 int row_lengths(Ctx *ctx, const char *who, const char *rows, const int *lengths, int n, int stride, int least,

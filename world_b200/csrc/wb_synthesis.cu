@@ -13,7 +13,7 @@
 //   syn_overlap_kernel    output sample -> thread: sums the responses covering it in pulse order
 //                         (the reference's accumulation order, so the sum is deterministic)
 // and, ahead of it, the voice modification of the reference demo (F0 scaling and formant shift, section below):
-//   modify_stretch_kernel, modify_f0_kernel
+//   modify_stretch_kernel, modify_f0_kernel, and per frame modify_curve_stretch_kernel, modify_curve_f0_kernel
 // FFT conventions (SURVEY.md App. A0): c2c FORWARD of a == FFT(conj a); c2r of X == Re FFT(conj X~)
 // with X~ the Hermitian extension -- both are forward transforms of wb_fft.cuh.
 #include "wb_chain.h"
@@ -32,6 +32,8 @@
 static inline double __dadd_rn(double a, double b) { return a + b; }
 static inline double __dsub_rn(double a, double b) { return a - b; }
 static inline double __dmul_rn(double a, double b) { return a * b; }
+static inline double __ddiv_rn(double a, double b) { return a / b; }
+static inline void atomicMin(unsigned long long *p, unsigned long long v) { if (v < *p) *p = v; }
 #endif
 
 namespace wb {
@@ -421,6 +423,110 @@ WB_KERNEL_PLAIN modify_f0_kernel(const double *f0_in, double *f0_out, const doub
     }
 }
 
+// ---- pitch and formant curves: one f0 factor and one spectral ratio per frame ----------------------------------------
+// Frame i of an utterance is modified as ParameterModification modifies a one-frame spectrogram with shift =
+// f0_curve[i] and ratio = ratio_curve[i] at the utterance's fft_size.  A (ratio, fft_size) table per frame would be
+// 12 bytes per bin per frame, so the stretch works out each frame's segments and weights on the device instead, with
+// modify_plan's expressions in modify_plan's order (every step rounded on its own: no FMA):
+//   modify_curve_stretch_kernel  frame -> CTA.  Padded rows: the (frame, utterance) grid of modify_stretch_kernel;
+//                                packed rows: one CTA per packed frame, the utterance found by packed_find.  The CTA
+//                                builds x[i] = ratio * i / n_fft * fs and L[i] = log(sp[i]) in shared memory, then per
+//                                bin j (j := c - 1 past the tail c = (int)(n_fft / 2.0 * ratio) when ratio < 1, as
+//                                modify_plan folds it) takes xi = (double)j / n_fft * fs, its histc segment k, s =
+//                                (xi - x[k - 1]) / (x[k] - x[k - 1]) and exp(L[a] + s * (L[a + 1] - L[a])) with the
+//                                three roundings of modify_stretch_kernel.  On constant curves each row equals
+//                                modify_stretch_kernel's bit for bit.
+//   modify_curve_f0_kernel       frame -> thread: f0 * curve, rounded as modify_f0_kernel
+//   modify_curve_check_kernel    frame -> thread: the first frame of each curve that breaks modify_plan's rule
+//                                (atomicMin on its index), read back once by the host before any modification.
+// Segment search: histc (wb_matlab.cu) walks the edges and nodes in step.  For a strictly ascending x (ratio > 0:
+// consecutive nodes differ by ratio * fs / n_fft, far above an ulp) and ascending edges xi, the bin it gives edge xi is
+//   k = min(bins - 1, the first b >= 1 with xi < x[b])
+// (an edge below x[1] stays in bin 1; the walk advances past node b exactly when xi >= x[b]; past the last node every
+// edge is bin bins - 1).  That is a binary search over x in shared memory, about log2(bins) loads per bin.  Where xi
+// equals a node (ratios 0.5, 1.0, 2.0 put edges on nodes), xi < x[b] is false at that node, so the edge goes to the
+// segment that starts there, as in histc.
+
+WB_DEV void curve_stretch_row(double *row, int n_fft, int fs, double ratio, double *x, double *logs) {
+  const int tid = WB_TID, nth = WB_NTH, bins = n_fft / 2 + 1;
+  const double nf = (double)n_fft, fsd = (double)fs;
+  for (int i = tid; i < bins; i += nth) {   // test.cpp:237-240 as modify_plan: ((ratio * i) / n_fft) * fs
+    x[i] = __dmul_rn(__ddiv_rn(__dmul_rn(ratio, (double)i), nf), fsd);
+    logs[i] = log(row[i]);
+  }
+  WB_SYNC();
+  const int c = ratio < 1.0 ? static_cast<int>(n_fft / 2.0 * ratio) : bins;   // test.cpp:250-254
+  for (int j = tid; j < bins; j += nth) {
+    const int e = j < c ? j : c - 1;
+    const double xi = __dmul_rn(__ddiv_rn((double)e, nf), fsd);
+    int lo = 1, hi = bins - 1;   // the first b in [1, bins - 1] with xi < x[b], else bins - 1
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (xi < x[mid]) hi = mid; else lo = mid + 1;
+    }
+    const int a = lo - 1;
+    const double s = __dsub_rn(xi, x[a]) / __dsub_rn(x[a + 1], x[a]);   // matlabfunctions.cpp:162-171
+    const double la = logs[a], lb = logs[a + 1];
+    row[j] = exp(__dadd_rn(la, __dmul_rn(s, __dsub_rn(lb, la))));
+  }
+  WB_SYNC();
+}
+
+// fft_u: [n_utts] each utterance's fft_size; ratio: the curve, indexed like the frames' rows.  f_off null: padded rows,
+// grid (max_f, utterances); else packed rows, frames [0, frames) over a 1-D grid.  Dynamic shared memory: 2 * max_bins
+// doubles.
+WB_KERNEL(WB_MODIFY_THREADS, 8) modify_curve_stretch_kernel(double *sp, const int *__restrict__ f_len, int n_utts,
+                                                            int f_stride, int row_len, const int *__restrict__ fft_u,
+                                                            int fs, const double *__restrict__ ratio,
+                                                            const long long *__restrict__ f_off, long long frames,
+                                                            int max_bins) {
+  WB_DYN_SMEM(double, x);
+  double *logs = x + max_bins;
+  if (f_off) {
+    for (long long g = blockIdx.x; g < frames; g += gridDim.x) {
+      const int u = packed_find(f_off, n_utts, g);
+      curve_stretch_row(sp + (size_t)g * row_len, __ldg(&fft_u[u]), fs, __ldg(&ratio[g]), x, logs);
+    }
+    return;
+  }
+  const int f = blockIdx.x;
+  for (int u = blockIdx.y; u < n_utts; u += gridDim.y) {
+    if (f >= f_len[u]) continue;   // uniform over the CTA
+    const size_t at = (size_t)u * f_stride + f;
+    curve_stretch_row(sp + at * row_len, __ldg(&fft_u[u]), fs, __ldg(&ratio[at]), x, logs);
+  }
+}
+
+WB_KERNEL_PLAIN modify_curve_f0_kernel(double *f0, const double *__restrict__ curve, const int *__restrict__ f_len,
+                                       int n_utts, int f_stride, const long long *__restrict__ f_off) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  for (int u = blockIdx.y; u < n_utts; u += gridDim.y)
+    if (i < f_len[u]) {
+      const size_t at = syn_at(f_off, u, f_stride) + i;
+      f0[at] = __dmul_rn(f0[at], curve[at]);
+    }
+}
+
+// modify_plan's rules for one value (f0: a finite factor > 0; ratio: also c = (int)(n_fft / 2.0 * r) >= 1 below 1)
+WB_HD inline bool curve_f0_bad(double v) { return !(v > 0.0) || !isfinite(v); }
+WB_HD inline bool curve_ratio_bad(double r, int n_fft) {
+  return !(r > 0.0) || !isfinite(r) || (r < 1.0 && static_cast<int>(n_fft / 2.0 * r) < 1);
+}
+
+// first[0] / first[1]: the smallest index of a bad f0 / ratio value (ULLONG_MAX on entry: none)
+WB_KERNEL_PLAIN modify_curve_check_kernel(const double *__restrict__ f0c, const double *__restrict__ ratio,
+                                          const int *__restrict__ f_len, int n_utts, int f_stride,
+                                          const int *__restrict__ fft_u, const long long *__restrict__ f_off,
+                                          unsigned long long *first) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  for (int u = blockIdx.y; u < n_utts; u += gridDim.y)
+    if (i < f_len[u]) {
+      const size_t at = syn_at(f_off, u, f_stride) + i;
+      if (f0c && curve_f0_bad(f0c[at])) atomicMin(&first[0], (unsigned long long)at);
+      if (ratio && curve_ratio_bad(ratio[at], fft_u[u])) atomicMin(&first[1], (unsigned long long)at);
+    }
+}
+
 namespace {
 struct ModifyLayout {
   size_t o_idx, o_frac, o_tbins, o_toff, o_scale, o_table, total;
@@ -560,6 +666,109 @@ int modify_run(Ctx *ctx, const ModifyPlan &plan, int u0, int n_utts, const int *
   if (!plan.table.empty())
     modify_stretch_launch(ctx, d, row, plan.bins, f_len, n_utts, f0_stride, max_f, spectrogram, f_off);
   return dev_check(ctx, "modify");
+}
+
+namespace {
+// The rows' lengths, sizes and (packed) offsets on the device, in one arena block with `extra` bytes after them
+struct CurveRows {
+  const int *f_len, *fft; const long long *f_off; unsigned char *extra;
+  int max_f; long long frames;
+};
+int curve_rows(Ctx *ctx, int n_utts, const int *f_len, int f_stride, const long long *f_off, const int *fft_sizes,
+               size_t extra, CurveRows *d) {
+  d->max_f = 0;
+  for (int u = 0; u < n_utts; ++u) d->max_f = imax(d->max_f, f_len[u]);
+  d->frames = f_off ? f_off[n_utts] : (long long)n_utts * f_stride;
+  ArenaPlan a;
+  const size_t o_len = a.add((size_t)n_utts * 4), o_fft = a.add(fft_sizes ? (size_t)n_utts * 4 : 0);
+  const size_t o_off = a.add(f_off ? (size_t)(n_utts + 1) * 8 : 0), o_extra = a.add(extra);
+  unsigned char *blk = arena_block(ctx, a.total);
+  if (!blk) return WORLD_B200_ENOMEM;
+  int rc = dev_memcpy_h2d(ctx, blk + o_len, f_len, (size_t)n_utts * 4);
+  if (!rc && fft_sizes) rc = dev_memcpy_h2d(ctx, blk + o_fft, fft_sizes, (size_t)n_utts * 4);
+  if (!rc && f_off) rc = dev_memcpy_h2d(ctx, blk + o_off, f_off, (size_t)(n_utts + 1) * 8);
+  d->f_len = (const int *)(blk + o_len);
+  d->fft = fft_sizes ? (const int *)(blk + o_fft) : nullptr;
+  d->f_off = f_off ? (const long long *)(blk + o_off) : nullptr;
+  d->extra = blk + o_extra;
+  return rc;
+}
+
+// EINVAL naming the curve value at index `at` of the rows: its utterance and frame
+int curve_fail(Ctx *ctx, const char *who, bool ratio, long long at, int n_utts, int f_stride, const long long *f_off,
+               double v) {
+  const int u = f_off ? packed_find(f_off, n_utts, at) : (int)(at / f_stride);
+  const long long f = f_off ? at - f_off[u] : at % f_stride;
+  char msg[320];
+  snprintf(msg, sizeof msg, "%s: %s[%lld] = %.17g (utterance %d, frame %lld) %s", who,
+           ratio ? "spectral_ratio_curve" : "f0_curve", at, v, u, f,
+           ratio ? "is not a finite ratio > 0 that leaves a bin below (int)(fft_size / 2.0 * ratio)"
+                 : "is not a finite factor > 0");
+  ctx->last_error = msg;
+  return WORLD_B200_EINVAL;
+}
+}  // namespace
+
+int curves_check(Ctx *ctx, const char *who, const ModifyCurves &cv, int n_utts, const int *f_len, int f_stride,
+                 const long long *f_off, const int *fft_sizes) {
+  if (n_utts <= 0 || (!cv.f0 && !cv.ratio)) return 0;
+  CurveRows d;
+  int rc = curve_rows(ctx, n_utts, f_len, f_stride, f_off, cv.ratio ? fft_sizes : nullptr, 16, &d);
+  if (rc || d.max_f == 0) return rc;
+  unsigned long long *first = (unsigned long long *)d.extra, got[2];
+  rc = dev_memset(ctx, first, 0xff, 16);
+  if (rc) return rc;
+  const dim3 grid((unsigned)((d.max_f + 255) / 256), (unsigned)imin(n_utts, 65535));
+  WB_LAUNCH_FLAT(modify_curve_check_kernel, grid, 256, 0, ctx->stream, cv.f0, cv.ratio, d.f_len, n_utts, f_stride,
+                 d.fft, d.f_off, first);
+  rc = dev_check(ctx, "modify curves check");
+  if (!rc) rc = dev_memcpy_d2h(ctx, got, first, 16);
+  if (!rc) rc = dev_sync(ctx);
+  for (int k = 0; k < 2 && !rc; ++k) {
+    if (got[k] == ~0ull) continue;
+    double v = 0.0;
+    rc = dev_memcpy_d2h(ctx, &v, (k ? cv.ratio : cv.f0) + got[k], 8);
+    if (!rc) rc = dev_sync(ctx);
+    if (!rc) rc = curve_fail(ctx, who, k == 1, (long long)got[k], n_utts, f_stride, f_off, v);
+  }
+  return rc;
+}
+
+int curves_check_host(Ctx *ctx, const char *who, const ModifyCurves &cv, int n_utts, const int *f_len, int f_stride,
+                      const long long *f_off, const int *fft_sizes) {
+  for (int k = 0; k < 2; ++k) {
+    const double *c = k ? cv.ratio : cv.f0;
+    for (int u = 0; u < n_utts && c; ++u)
+      for (int i = 0; i < f_len[u]; ++i) {
+        const long long at = (long long)syn_at(f_off, u, f_stride) + i;
+        if (k ? curve_ratio_bad(c[at], fft_sizes[u]) : curve_f0_bad(c[at]))
+          return curve_fail(ctx, who, k == 1, at, n_utts, f_stride, f_off, c[at]);
+      }
+  }
+  return 0;
+}
+
+int curves_run(Ctx *ctx, const ModifyCurves &cv, int n_utts, const int *f_len, int f_stride, const long long *f_off,
+               const int *fft_sizes, int fs, int row, double *f0, double *spectrogram) {
+  const bool scale = cv.f0 && f0, stretch = cv.ratio && spectrogram;
+  if (n_utts <= 0 || (!scale && !stretch)) return 0;
+  CurveRows d;
+  int rc = curve_rows(ctx, n_utts, f_len, f_stride, f_off, stretch ? fft_sizes : nullptr, 0, &d);
+  if (rc || d.max_f == 0) return rc;
+  if (scale) {
+    const dim3 grid((unsigned)((d.max_f + 255) / 256), (unsigned)imin(n_utts, 65535));
+    WB_LAUNCH_FLAT(modify_curve_f0_kernel, grid, 256, 0, ctx->stream, f0, cv.f0, d.f_len, n_utts, f_stride, d.f_off);
+  }
+  if (stretch) {
+    int max_bins = 0;
+    for (int u = 0; u < n_utts; ++u) max_bins = imax(max_bins, fft_sizes[u] / 2 + 1);
+    const dim3 grid = f_off ? dim3((unsigned)std::min<long long>(d.frames, INT_MAX))
+                            : dim3((unsigned)d.max_f, (unsigned)imin(n_utts, 65535));
+    if (d.frames > 0)
+      WB_LAUNCH_COOP(modify_curve_stretch_kernel, grid, WB_MODIFY_THREADS, (size_t)max_bins * 16, ctx->stream,
+                     spectrogram, d.f_len, n_utts, f_stride, row, d.fft, fs, cv.ratio, d.f_off, d.frames, max_bins);
+  }
+  return dev_check(ctx, "modify curves");
 }
 
 int row_lengths(Ctx *ctx, const char *who, const char *rows, const int *lengths, int n, int stride, int least,
@@ -1107,27 +1316,35 @@ extern "C" int world_b200_synthesis_coded_batch_pcm16(WorldB200 *h, const double
 // world_b200_modify_batch_options (utterance u at fft_sizes[u], rows of row_stride)
 // world_b200_modify_packed: f_offsets (host, [n_utts + 1]) instead of f0_lengths / f0_stride, row_stride 0 = the largest
 // fft_sizes[u] / 2 + 1
+// cv (world_b200_modify_curves / _curves_packed): DEVICE curves in place of the factors (which are then null), checked
+// by curves_check after the host checks
 static int modify_batch(WorldB200 *h, double *f0, const int *f0_lengths, int n_utts, int f0_stride,
                         double *spectrogram, int row_stride, int fft_size, const int *fft_sizes, bool per_utt, int fs,
                         const double *f0_scale, const double *spectral_ratio, const long long *f_offsets = nullptr,
-                        bool packed = false) {
+                        bool packed = false, const ModifyCurves *cv = nullptr) {
   if (!h) return WORLD_B200_EINVAL;
   DeviceGuard guard_(&h->c);
   Ctx *ctx = &h->c;
+  const char *who = cv ? "modify_curves" : "modify";
   auto fail = [&](const std::string &what) {
-    ctx->last_error = "modify: " + what;
+    ctx->last_error = std::string(who) + ": " + what;
     return WORLD_B200_EINVAL;
   };
-  if (packed) {
+  const bool stretch = spectral_ratio || (cv && cv->ratio);
+  if (packed || cv) {
     if (n_utts < 0) return fail("n_utts must be >= 0");
     if (n_utts == 0) return 0;
+  }
+  if (packed) {
     if (!f_offsets) return fail("f_offsets must be given");
   } else if (n_utts < 0 || f0_stride <= 0) {
     return fail("n_utts must be >= 0 and f0_stride > 0");
   }
+  if (cv && ((cv->f0 && !f0) || (cv->ratio && !spectrogram)))
+    return fail("f0_curve needs f0 rows and spectral_ratio_curve needs spectrogram rows");
   if ((f0_scale && !f0) || (spectral_ratio && !spectrogram))
     return fail("f0_scale needs f0 rows and spectral_ratio needs spectrogram rows");
-  if (per_utt && spectral_ratio) {
+  if (per_utt && stretch) {
     if (!fft_sizes) return fail("fft_sizes must be given");
     if (fs <= 0) return fail("fs must be > 0");
     if (packed && row_stride == 0)
@@ -1145,8 +1362,14 @@ static int modify_batch(WorldB200 *h, double *f0, const int *f0_lengths, int n_u
   // a length of 0 is allowed here: the utterance's rows are left alone
   std::vector<int> lens;
   ModifyPlan plan;
-  int rc = packed ? packed_lengths(ctx, "modify", "f", "frames", f_offsets, n_utts, 0, &lens)
-                  : row_lengths(ctx, "modify", "f0", f0_lengths, n_utts, f0_stride, 0, &lens);
+  int rc = packed ? packed_lengths(ctx, who, "f", "frames", f_offsets, n_utts, 0, &lens)
+                  : row_lengths(ctx, who, "f0", f0_lengths, n_utts, f0_stride, 0, &lens);
+  if (cv) {
+    const long long *off = packed ? f_offsets : nullptr;
+    if (!rc) rc = curves_check(ctx, who, *cv, n_utts, lens.data(), f0_stride, off, fft_sizes);
+    return rc ? rc : curves_run(ctx, *cv, n_utts, lens.data(), f0_stride, off, fft_sizes, fs, row_stride, f0,
+                                spectrogram);
+  }
   if (!rc) rc = modify_plan(ctx, "modify", n_utts, fft_size, fs, f0_scale, spectral_ratio, &plan,
                             per_utt ? fft_sizes : nullptr);
   return rc ? rc : modify_run(ctx, plan, 0, n_utts, lens.data(), f0_stride, per_utt ? row_stride : plan.bins, f0,
@@ -1232,4 +1455,22 @@ extern "C" int world_b200_modify_packed(WorldB200 *h, double *f0, int n_utts, co
                                         const double *f0_scale, const double *spectral_ratio) {
   return modify_batch(h, f0, nullptr, n_utts, 0, spectrogram, row_stride, 0, fft_sizes, true, fs, f0_scale,
                       spectral_ratio, f_offsets, true);
+}
+
+extern "C" int world_b200_modify_curves(WorldB200 *h, double *f0, const int *f0_lengths, int n_utts, int f0_stride,
+                                        double *spectrogram, int row_stride, const int *fft_sizes, int fs,
+                                        const double *f0_curve, const double *spectral_ratio_curve) {
+  ModifyCurves cv;
+  cv.f0 = f0_curve; cv.ratio = spectral_ratio_curve;
+  return modify_batch(h, f0, f0_lengths, n_utts, f0_stride, spectrogram, row_stride, 0, fft_sizes, true, fs, nullptr,
+                      nullptr, nullptr, false, &cv);
+}
+
+extern "C" int world_b200_modify_curves_packed(WorldB200 *h, double *f0, int n_utts, const long long *f_offsets,
+                                               double *spectrogram, int row_stride, const int *fft_sizes, int fs,
+                                               const double *f0_curve, const double *spectral_ratio_curve) {
+  ModifyCurves cv;
+  cv.f0 = f0_curve; cv.ratio = spectral_ratio_curve;
+  return modify_batch(h, f0, nullptr, n_utts, 0, spectrogram, row_stride, 0, fft_sizes, true, fs, nullptr, nullptr,
+                      f_offsets, true, &cv);
 }
