@@ -283,40 +283,37 @@ WB_KERNEL(128, 3) syn_pulse_kernel(SynParams p) {
   }
   WB_SYNC();
 
-  // ---- aperiodic response (:36-69)
-  if (noise_size > 0) {
-    const unsigned *draw = p.draws + p.draw_off[p0 + pi];
-    double s = 0.0;
-    for (int i = tid; i < N + 2; i += nth) {
-      const double v = (i < noise_size && i < N) ? randn_value(draw[i]) : 0.0;
-      buf[i] = v;
-      s += v;
-    }
-    const double average = block_sum(s, red) / noise_size;
-    for (int i = tid; i < noise_size && i < N; i += nth) buf[i] -= average;
-    WB_SYNC();
-    rfft_forward(buf, lg, p.tw);
-    const double2 *ns = reinterpret_cast<const double2 *>(buf);
-    for (int k = tid; k <= half; k += nth) mps[k] = ns[k];        // keep the noise spectrum
-    WB_SYNC();
-    for (int k = tid; k <= half; k += nth)
-      buf[k] = (current_vuv != 0.0) ? log(env[k] * apr[k]) / 2.0 : log(env[k]) / 2.0;
-    WB_SYNC();
-    syn_minimum_phase(buf, z, N, lg, p.tw);
-    for (int k = tid; k <= half; k += nth) {
-      const double2 m = z[k], q = mps[k];
-      mps[k] = make_double2(m.x * q.x - m.y * q.y, m.x * q.y + m.y * q.x);
-    }
-    WB_SYNC();
-    syn_c2r(mps, z, N, lg, p.tw);
-    const double sq = sqrt(static_cast<double>(noise_size));
-    for (int i = tid; i < N; i += nth) {
-      const double aper = (i < half) ? z[i + half].x : z[i - half].x;   // fftshift
-      resp[i] = (per[i] * sq + aper) / N;                                // :214-217
-    }
-  } else {
-    // last pulse: noise_size = 0 -> zero noise, sqrt(0) kills the periodic part (:372-374)
-    for (int i = tid; i < N; i += nth) resp[i] = 0.0;
+  // ---- aperiodic response (:36-69).  The last pulse (noise_size 0) runs it too: its noise is all zeros and sqrt(0)
+  // scales the periodic part away, which gives zeros where both responses are finite and NaN where either is not (a
+  // zero envelope's log(0)), as in the reference.
+  const unsigned *draw = p.draws + p.draw_off[p0 + pi];
+  double s = 0.0;
+  for (int i = tid; i < N + 2; i += nth) {
+    const double v = (i < noise_size && i < N) ? randn_value(draw[i]) : 0.0;
+    buf[i] = v;
+    s += v;
+  }
+  const double average = block_sum(s, red) / noise_size;
+  for (int i = tid; i < noise_size && i < N; i += nth) buf[i] -= average;
+  WB_SYNC();
+  rfft_forward(buf, lg, p.tw);
+  const double2 *ns = reinterpret_cast<const double2 *>(buf);
+  for (int k = tid; k <= half; k += nth) mps[k] = ns[k];        // keep the noise spectrum
+  WB_SYNC();
+  for (int k = tid; k <= half; k += nth)
+    buf[k] = (current_vuv != 0.0) ? log(env[k] * apr[k]) / 2.0 : log(env[k]) / 2.0;
+  WB_SYNC();
+  syn_minimum_phase(buf, z, N, lg, p.tw);
+  for (int k = tid; k <= half; k += nth) {
+    const double2 m = z[k], q = mps[k];
+    mps[k] = make_double2(m.x * q.x - m.y * q.y, m.x * q.y + m.y * q.x);
+  }
+  WB_SYNC();
+  syn_c2r(mps, z, N, lg, p.tw);
+  const double sq = sqrt(static_cast<double>(noise_size));
+  for (int i = tid; i < N; i += nth) {
+    const double aper = (i < half) ? z[i + half].x : z[i - half].x;   // fftshift
+    resp[i] = (per[i] * sq + aper) / N;                                // :214-217
   }
 }
 
